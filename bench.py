@@ -1,11 +1,11 @@
 #!/usr/bin/env python
 """bench.py -- PGPE generations/s on synthetic Rastrigin (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--popsize P] [--dim D]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--popsize P] [--dim D] [--dump-outputs DIR]
 
 Workload (config.workload): PGPE (symmetric sampling, ClipUp, centered ranking, stdev_max_change 0.2; the reference's
 defaults), Rastrigin, popsize 1,000,000 x dim 10,000 fp32 -- the configuration BASELINE.json's metric is quoted on; the
-40 GB population fits one B200.  With N > 1 (torchrun, one rank per GPU) the SAME population is row-sharded over the ranks
+40 GB population fits one 80 GB H100.  With N > 1 (torchrun, one rank per GPU) the SAME population is row-sharded over the ranks
 (strong scaling): per generation one all-gather of the fitness vector and one all-reduce of the stacked gradients.
 
 One "step" = one generation through the public API (`searcher.step()`): rank -> weighted gradient reduction -> ClipUp /
@@ -16,6 +16,10 @@ e2e = the same generation driven through `Problem.sample_and_compute_gradients` 
 pinned host memory are copied to the device every step, gradients and mean fitness are copied back; the reference's
 `dist_on_cpu` actor protocol, core.py:2958); roofline = the dominant kernel (fused sample+evaluate) timed live with CUDA
 events; cpu_baseline = the reference's torch-CPU op sequence (oracle/ref_cpu_path.py) on this box's host cores.
+
+--dump-outputs DIR writes what the last timed generation handed to its caller (center, stdev, the population's fitnesses and a
+fixed, seeded sample of its rows) as DIR/<name>.npy, so that two builds can be compared output for output: the workload is
+seeded, so the same arguments give the same inputs on every run.
 """
 
 from __future__ import annotations
@@ -40,7 +44,7 @@ LR_MU, LR_SIGMA, STDEV_INIT, SEED = 0.5, 0.1, 1.0, 0
 
 
 CONFIGS = {  # BASELINE.json configs that are bench workloads (the others are parity-test cases)
-    "metric": dict(popsize=1_000_000, dim=10_000),  # the configuration the metric is quoted on; fits one B200 (40 GB)
+    "metric": dict(popsize=1_000_000, dim=10_000),  # the configuration the metric is quoted on; fits one 80 GB H100 (40 GB)
     "cfg2": dict(popsize=100_000, dim=10_000),      # BASELINE configs[1]
     "cfg5": dict(popsize=1_000_000, dim=100_000),   # BASELINE configs[4]: 400 GB of samples, sharded over 2 / 4 / 8 GPUs
 }
@@ -65,6 +69,7 @@ def parse_args():
     ap.add_argument("--no-other-configs", action="store_true", help="skip the short cfg2 / cfg3 / cfg4 legs of the default N = 1 line")
     ap.add_argument("--no-sharded-parity", action="store_true", help="skip the sharded-vs-unsharded parity leg at N > 1")
     ap.add_argument("--cuda-graph", type=int, default=-1, help="1/0: replay each generation from a CUDA graph. Default: 0 at N = 1 (kernels are timed live inside the timed region), 1 at N > 1 (the fused kernel is then timed stand-alone right after the timed region)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="after the timed steps, write the last generation's outputs as DIR/<name>.npy")
     ap.add_argument("--peer", type=int, default=-1, help="1/0: at N > 1 move fitnesses and gradients between the GPUs from inside the producing kernels (NVLink peer memory, evotorch_b200/peer.py) instead of NCCL all_gather/all_reduce. Default: 1 at N > 1")
     a = ap.parse_args()
     cfg = CONFIGS[a.config]
@@ -91,7 +96,7 @@ def workload_config(args, n_gpus, collectives="nccl"):
         "stdev_learning_rate": LR_SIGMA,
         "stdev_init": STDEV_INIT,
         "parallelism": f"population row-sharded over {n_gpus} GPU(s); {how}" if n_gpus > 1 else "single GPU",
-        "l2": "inputs larger than L2 (population %.1f GB >> 126 MB): no flush needed" % (4.0 * args.popsize * args.dim / 1e9 / n_gpus),
+        "l2": "inputs larger than L2 (population %.1f GB >> 50 MB): no flush needed" % (4.0 * args.popsize * args.dim / 1e9 / n_gpus),
     }
 
 
@@ -251,7 +256,7 @@ def measured_peak_gbs() -> tuple:
         with open(path) as fh:
             return float(json.load(fh)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "fallback (H100 SXM data sheet HBM3 bandwidth)"
 
 
 def run_ours(args):
@@ -335,6 +340,8 @@ def run_ours(args):
     clock_info = clocks.stop(t_begin, t_end) if clocks is not None else None
     mean_eval = float(searcher.status["mean_eval"])
     value = K / (elapsed_ms / 1e3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, searcher, problem, lazy)
 
     # ---- roofline of the dominant kernel (fused sample + evaluate): algorithmic bytes = the population written once
     n_local = N // world
@@ -356,19 +363,10 @@ def run_ours(args):
     fused_ms = timers["sample_eval"][1]
     fused_bytes = 4.0 * n_local * D + 4.0 * n_local
     achieved = fused_bytes / (fused_ms * 1e-3) / 1e9
-    # DRAM traffic of the kernel from the committed ncu --set full capture (profiles/traffic.json), scaled by rows x columns
-    traffic, traffic_note = None, "no capture"
-    try:
-        with open(os.path.join(ROOT, "profiles", "traffic.json")) as fh:
-            cap = json.load(fh)["sample_eval"]
-        if lazy:
-            traffic_note = "lazy population: the kernel stores nothing (fitnesses only); the figure is MODEL bandwidth (bytes a materialising kernel would write)"
-        else:
-            traffic = cap["ratio"] * fused_bytes
-            traffic_note = (f"dram__bytes_read+write = {cap['ratio']:.4f} x algorithmic bytes in {cap['source']} "
-                            f"(captured at popsize {cap['capture']['popsize']}, scaled linearly to this launch)")
-    except Exception:
-        pass
+    # measured DRAM traffic needs a hardware-counter capture, which this benchmark does not take
+    traffic = None
+    traffic_note = ("lazy population: the kernel stores nothing (fitnesses only); the figure is MODEL bandwidth (bytes a materialising kernel would write)"
+                    if lazy else "not measured")
     roofline = {"kernel": "evok::sample_eval_kernel<RASTRIGIN, symmetric, %s, vec4>" % ("no store (lazy)" if lazy else "store"), "bound": "hbm",
                 "achieved": achieved, "peak": peak,
                 "unit": "GB/s", "frac": achieved / peak, "traffic": traffic, "traffic_note": traffic_note, "peak_source": peak_src,
@@ -474,6 +472,38 @@ def run_ours(args):
                                                  with_gpu_eager=True)
     emit(line)
     finish()
+
+
+def dump_outputs(out_dir: str, searcher, problem, lazy: bool, max_bytes: int = 64 << 20):
+    """The arrays a caller of `searcher.step()` receives after the last timed generation, as .npy files (at most `max_bytes` in
+    all): center and stdev; the fitnesses of this process's population -- with several processes, the local shard of the rank
+    that calls this (rank 0) -- (a fixed, seeded sample of 4 M when larger); a fixed, seeded sample of population rows (not with
+    the lazy population, which holds no rows).  `evals_index` / `population_rows` give the sampled row indices: integers, stored
+    as float64 (exact below 2^53)."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    gen = torch.Generator().manual_seed(20240611)
+    arrays = {"center": searcher.status["center"], "stdev": searcher.status["stdev"]}
+    pop = searcher.population
+    if pop is None and getattr(problem, "_grad_batches", None):  # sharded: this rank's shard
+        pop = next(iter(problem._grad_batches.values()))
+    if pop is not None:
+        f = pop.evals.reshape(len(pop), -1)[:, 0]
+        if len(f) > (4 << 20):
+            idx = torch.randperm(len(f), generator=gen)[: 4 << 20].sort().values
+            arrays["evals_index"], f = idx.to(torch.float64), f[idx.to(f.device)]
+        arrays["evals"] = f
+        if not lazy:
+            room = max_bytes - sum(8 * a.numel() for a in arrays.values())
+            n_rows = max(1, min(len(pop), 256, room // (4 * pop.values.shape[1] + 8)))
+            rows = torch.randperm(len(pop), generator=gen)[:n_rows].sort().values
+            arrays["population_rows"] = rows.to(torch.float64)
+            arrays["population_sample"] = pop.values[rows.to(pop.values.device)]
+    for name, a in arrays.items():
+        a = torch.as_tensor(a).detach().cpu()
+        np.save(os.path.join(out_dir, name + ".npy"), a.numpy().astype(np.float64 if a.dtype == torch.float64 else np.float32))
 
 
 def sharded_parity_leg(dev, use_peer: bool) -> dict:
@@ -594,7 +624,7 @@ def other_config_legs(dev, peak_gbs: float) -> dict:
             with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as fh:
                 tf32_peak = float(json.load(fh)["bf16_tflops"]) / 2.0
         except Exception:
-            tf32_peak = 1100.0
+            tf32_peak = 495.0  # H100 SXM data sheet, dense TF32
         out["cfg3_cmaes_1024_x_4096"] = {"generations_per_s": 1e3 / ms, "ms_per_step": ms, "steps": 20, "useful_flop_per_generation": flops,
                                          "useful_tflops": flops / ms / 1e9, "tensor_flop_per_generation_3xtf32": 3 * 2.0 * n * d * d * 2,
                                          "frac_of_tf32_peak_3x": 3 * 2.0 * n * d * d * 2 / ms / 1e9 / tf32_peak, "tf32_peak_tflops": tf32_peak,
@@ -626,7 +656,7 @@ def other_config_legs(dev, peak_gbs: float) -> dict:
         out["cfg4_mlp_376_256_17_x_65536"] = {"ms_per_forward": ms, "gbs": gb / ms * 1e3, "frac_of_hbm_peak": gb / ms * 1e3 / peak_gbs,
                                               "observations_per_policy": 1, "activation": "tanh", "params_per_policy": pol.parameter_length}
         # the same population on ONE shared minibatch of 256 observations (SupervisedNE, common_minibatch): the first layer of all
-        # 65 536 networks is a single (16.8 M x 376) x (376 x 256) product on the tcgen05 GEMM (3xTF32, weights read once)
+        # 65 536 networks is a single (16.8 M x 376) x (376 x 256) product on the tensor-core GEMM (3xTF32, weights read once)
         try:
             Bm = 256
             xb = torch.randn(Bm, 376, device=dev)
@@ -639,7 +669,7 @@ def other_config_legs(dev, peak_gbs: float) -> dict:
                 with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as fh:
                     tf32_peak = float(json.load(fh)["bf16_tflops"]) / 2.0
             except Exception:
-                tf32_peak = 1100.0
+                tf32_peak = 495.0  # H100 SXM data sheet, dense TF32
             out["cfg4_mlp_376_256_17_x_65536"]["shared_minibatch_B256"] = {
                 "ms_per_forward": ms_b, "useful_tflops_fp32_equivalent": useful / ms_b / 1e9, "tensor_tflops_3xtf32": tensor / ms_b / 1e9,
                 "frac_of_tf32_peak": tensor / ms_b / 1e9 / tf32_peak, "tf32_peak_tflops": tf32_peak, "parameter_gbs": gb / ms_b * 1e3,
@@ -656,7 +686,7 @@ def other_config_legs(dev, peak_gbs: float) -> dict:
 
 def run_reference(args):
     """The reference arm: the reference's own CPU implementation of the path (its torch-CPU op sequence, restated in
-    oracle/ref_cpu_path.py and checked bit-identical against the real reference in the build container), all host threads,
+    oracle/ref_cpu_path.py and checked bit-identical against the real reference's recorded trajectories in tests/golden), all host threads,
     same metric / config, SURVEY 8(d) protocol: populations of 10k / 30k / 100k rows at the full dimension, linearity check,
     extrapolation to the workload's population from the fitted line.  Rank 0 only."""
     if int(os.environ.get("RANK", "0")) != 0:

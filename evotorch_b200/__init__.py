@@ -1,5 +1,5 @@
 """evotorch_b200: the per-generation hot path of EvoTorch's distribution-based searchers (PGPE / SNES / CEM / XNES /
-CMA-ES) as hand-written sm_100a CUDA kernels behind the reference's Problem / SolutionBatch / SearchAlgorithm API.
+CMA-ES) as hand-written sm_90a (H100) CUDA kernels behind the reference's Problem / SolutionBatch / SearchAlgorithm API.
 
     from evotorch_b200 import Problem
     from evotorch_b200.algorithms import PGPE

@@ -97,7 +97,7 @@ def lib() -> ctypes.CDLL:
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise EvokError(
-                f"{LIB_PATH} is missing: the sm_100a kernel library has not been built. "
+                f"{LIB_PATH} is missing: the sm_90a kernel library has not been built. "
                 "Run `python -m evotorch_b200.build` (needs nvcc). There is no CPU/torch fallback for CUDA problems."
             )
         handle = ctypes.CDLL(LIB_PATH)

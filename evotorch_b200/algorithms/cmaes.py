@@ -7,13 +7,13 @@ Per generation (cmaes.py:567-606):
     weighted recombinations sum_i w_i z_i, sum_i w_i y_i (K4 weighted column sums)
     evolution paths, sigma, rank-1 + rank-mu update of C, Cholesky.
 The rank-mu term is computed as Y^T diag(w) Y (a weighted SYRK): the reference materialises an N x D x D broadcast
-temporary (cmaes.py:548; 16 GiB at D = 1024, N = 4096).  On CUDA fp32 both contractions run on the hand-written tcgen05
-kernel (csrc/evok_gemm.cu: TMA -> 128B-swizzled smem -> tcgen05.mma.kind::tf32 with 3xTF32 operand splitting -> TMEM ->
+temporary (cmaes.py:548; 16 GiB at D = 1024, N = 4096).  On CUDA fp32 both contractions run on the hand-written wgmma
+kernel (csrc/evok_gemm.cu: TMA -> 128B-swizzled smem -> wgmma.mma_async tf32 with 3xTF32 operand splitting -> registers ->
 register accumulation; the lo halves of the 3xTF32 operands are derived inside the kernel, so operands are read from HBM once); the
 glue between the contractions is fused into four small kernels (csrc/evok_cmaes.cu, evok_rank_table) and the covariance update is
 applied by the SYRK's epilogue, so a generation is ~14 launches with no host reads and replays from a CUDA graph
 (`enable_cuda_graph()`).  The Cholesky factorisation stays on cuSOLVER (torch.linalg.cholesky_ex): the repo's own persistent
-tile-dataflow kernel (csrc/evok_chol.cu, EVOTORCH_B200_EVOK_CHOLESKY=1) is correct but measured 2.2x slower at D = 1024.
+tile-dataflow kernel (csrc/evok_chol.cu, EVOTORCH_B200_EVOK_CHOLESKY=1) is correct but its 64 x 64 diagonal tiles form a serial critical path.
 """
 
 from __future__ import annotations
@@ -159,7 +159,7 @@ class CMAES(SearchAlgorithm, SinglePopulationAlgorithmMixin):
         if self.separable:
             ys = self.A.unsqueeze(0) * zs
         elif ops.uses_kernels(zs) and ops.uses_kernels(self.A):
-            # K6: one tcgen05 GEMM (3xTF32, fp32-accurate) with the affine epilogue xs = m + sigma * ys fused in; in the fused
+            # K6: one tensor-core GEMM (3xTF32, fp32-accurate) with the affine epilogue xs = m + sigma * ys fused in; in the fused
             # generation xs IS the population's value buffer
             ys = torch.empty_like(zs) if fs is None else fs["ys"]
             xs = torch.empty_like(zs) if fs is None else self._population._data
@@ -232,7 +232,7 @@ class CMAES(SearchAlgorithm, SinglePopulationAlgorithmMixin):
             pc = weighted_pc * self.p_c
             r1_update = c1a * (torch.outer(pc, pc) - self.C)
             if ops.uses_kernels(ys) and ops.uses_kernels(assigned_weights):
-                # K7: weighted SYRK Y^T diag(w) Y as one tcgen05 GEMM over K-major (w*Y)^T and Y^T (split-K over the population)
+                # K7: weighted SYRK Y^T diag(w) Y as one tensor-core GEMM over K-major (w*Y)^T and Y^T (split-K over the population)
                 syrk = ops.gemm_nt(ops.transpose_scale(ys.contiguous(), assigned_weights.contiguous()), ops.transpose_scale(ys.contiguous()))
             else:
                 syrk = (ys.T * assigned_weights) @ ys  # no N x D x D temporary either
@@ -305,8 +305,8 @@ class CMAES(SearchAlgorithm, SinglePopulationAlgorithmMixin):
         ops.weighted_syrk_update(ys, fs["w_act"], fs["k"], self.C, u=self.p_c, out=self.C)
         if fs["steps_dev"] is not None or (self._steps_count + 1) % self.decompose_C_freq == 0:
             if os.environ.get("EVOTORCH_B200_EVOK_CHOLESKY", "0") == "1":
-                ops.cholesky(self.C, out=self.A)  # the repo's own tile-dataflow kernel (csrc/evok_chol.cu): correct, but measured
-                # 2.2x SLOWER than cuSOLVER's potrf at D = 1024 (0.75 vs 0.34 ms, profiles/r02_cholesky.txt), so it is not the default
+                ops.cholesky(self.C, out=self.A)  # the repo's own tile-dataflow kernel (csrc/evok_chol.cu): correct, but
+                # its diagonal-tile factorisations are a serial critical path, so cuSOLVER's potrf stays the default
             else:
                 torch.linalg.cholesky_ex(self.C, check_errors=False, out=(self.A, fs["info"]))
 

@@ -1,9 +1,9 @@
-"""Build libevok.so (the C-ABI library of sm_100a kernels) in-tree with nvcc.
+"""Build libevok.so (the C-ABI library of sm_90a kernels) in-tree with nvcc.
 
     python -m evotorch_b200.build [--force] [--verbose]
 
-The library is written to evotorch_b200/lib/libevok.so; it is git-ignored but travels to the GPU box with
-the working tree.  nvcc cross-compiles for sm_100a without a GPU.
+The library is written to evotorch_b200/lib/libevok.so (git-ignored build product).  nvcc cross-compiles for sm_90a
+without a GPU.
 """
 
 from __future__ import annotations
@@ -24,7 +24,7 @@ NVCC_FLAGS = [
     "-O3",
     "-std=c++17",
     "-gencode",
-    "arch=compute_100a,code=sm_100a",
+    "arch=compute_90a,code=sm_90a",
     "-lineinfo",
     "-Xcompiler",
     "-fPIC",
@@ -78,7 +78,7 @@ def build(force: bool = False, verbose: bool = False, defines: tuple = (), tag: 
 
     with ThreadPoolExecutor(max_workers=min(8, len(sources()))) as ex:
         objs = list(ex.map(compile_one, sources()))
-    cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC", "-o", lib_path + ".tmp", *objs,
+    cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC", "-o", lib_path + ".tmp", *objs,
            "-lcuda"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:

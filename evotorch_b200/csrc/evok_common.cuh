@@ -1,4 +1,4 @@
-// Shared device helpers for libevok (sm_100a).  See include/evok.h for the ABI.
+// Shared device helpers for libevok (sm_90a).  See include/evok.h for the ABI.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -21,7 +21,7 @@ extern unsigned long long g_launch_count;
 inline void count_launches(int n) { __atomic_fetch_add(&g_launch_count, (unsigned long long)n, __ATOMIC_RELAXED); }
 
 constexpr int kWarp = 32;
-constexpr int kNumSMs = 148;  // B200
+constexpr int kNumSMs = 132;  // H100 SXM
 
 // ------------------------------------------------------------------------------------------------
 // Peer exchange over NVLink (evok_peer.cu): where a producing kernel's result is needed by every GPU, the kernel itself

@@ -1,25 +1,25 @@
-// K6 / K7: fp32-accurate GEMM on the 5th-generation tensor cores (tcgen05 + TMEM + TMA), for the dense contractions of
+// K6 / K7: fp32-accurate GEMM on the Hopper tensor cores (wgmma + TMA + mbarrier), for the dense contractions of
 // CMA-ES (cmaes.py:427 `Y = Z A^T`, :548 rank-mu update `Y^T diag(w) Y`) and XNES.
 //
 //   C[M x N] = A[M x K] * B[N x K]^T            (A, B row-major with K contiguous: "K-major"; fp32 in, fp32 out)
 //
 // Accuracy: every fp32 operand x is split as x = hi + lo with hi = x rounded down to TF32 (13 low mantissa bits cleared)
-// and lo = x - hi (exact); the kernel accumulates hi*hi + hi*lo + lo*hi in the fp32 TMEM accumulator with
-// tcgen05.mma.kind::tf32 ("3xTF32"), which restores ~2^-21 relative accuracy per product -- plain single-pass TF32 (2^-10)
-// would break the 1e-5 parity bar of the searchers' state.
+// and lo = x - hi (exact); the kernel accumulates hi*hi + hi*lo + lo*hi in fp32 with wgmma.mma_async...tf32 ("3xTF32"),
+// which restores ~2^-21 relative accuracy per product -- plain single-pass TF32 (2^-10) would break the 1e-5 parity bar of
+// the searchers' state.
 //
-// Structure (one CTA per 128 x 256 output tile, optional split-K over blockIdx.z):
-//   warp 0      TMA producer, 2-stage mbarrier ring.  CONVERT = true (operands 16-byte aligned, the normal case): TWO raw fp32
+// Structure (one CTA per 128 x 128 output tile, optional split-K over blockIdx.z; 384 threads = 3 warpgroups):
+//   warp 0      TMA producer, 3-stage mbarrier ring.  CONVERT = true (operands 16-byte aligned, the normal case): TWO raw fp32
 //               tile loads per K-block (A, B; 128-byte swizzle) -- the tensor core ignores the 13 low mantissa bits of a tf32
 //               operand, so the raw tile IS the hi operand, and two converter warps derive the lo tiles (x - trunc(x), same
 //               swizzled positions, element-wise) in shared memory while earlier MMAs run: the operands are read from HBM exactly
 //               once and no split copies exist.  CONVERT = false (unaligned operands): 4 loads of tiles pre-split by a pre-pass
-//   warp 1      TMEM allocation + single-thread tcgen05.mma issue (12 MMAs of 128 x 256 x 8 per K-block),
-//               tcgen05.commit releases the stage / signals the epilogue
+//   warp 1      idle (keeps the consumers on a warpgroup boundary)
 //   warps 2-3   converters (CONVERT only, see warp 0)
-//   warps 4-11  epilogue: the K loop is accumulated in TMEM in chunks of 4 K-blocks (two ping-pong accumulators); each finished
-//               chunk is folded into per-thread fp32 REGISTER accumulators (round-to-nearest) via tcgen05.ld, the final tile is
-//               written through a shared-memory transpose; optional second output C2 = alpha * acc + bias[col]
+//   warps 4-11  two consumer warpgroups, tile rows 0-63 and 64-127: each issues the 12 wgmma.m64n128k8 of a K-block (its half of
+//               the A tile against the whole B tile) and accumulates in registers in chunks of 4 K-blocks; each finished chunk
+//               is folded into a second register accumulator with round-to-nearest fp32 adds.  The final tile is written through
+//               a shared-memory transpose; optional second output C2 = alpha * acc + bias[col]
 #include <cuda.h>
 
 #include <cstdlib>
@@ -29,16 +29,19 @@
 namespace evok {
 
 constexpr int kGemmBM = 128;
-constexpr int kGemmBN = 256;
+constexpr int kGemmBN = 128;
 constexpr int kGemmBK = 32;  // floats = 128 bytes = one swizzle span
-constexpr int kGemmStages = 2;
-constexpr int kGemmThreads = 384;  // TMA warp, MMA warp, 2 converter warps, 8 epilogue warps (two aligned warpgroups: warp % 4 = TMEM lane quadrant)
-constexpr int kUmmaK = 8;  // tf32: 32 bytes of K per MMA
+constexpr int kGemmStages = 3;
+constexpr int kGemmThreads = 384;  // producer warpgroup (TMA warp, idle warp, 2 converter warps) + 2 consumer warpgroups
+constexpr int kWgmmaK = 8;         // tf32: 32 bytes of K per MMA
+constexpr int kAcc = kGemmBN / 2;  // fp32 accumulator registers per consumer thread (m64 x n128 over 128 threads)
 constexpr uint32_t kTileABytes = kGemmBM * kGemmBK * 4;  // 16 KB
-constexpr uint32_t kTileBBytes = kGemmBN * kGemmBK * 4;  // 32 KB
-constexpr uint32_t kStageBytes = 2 * kTileABytes + 2 * kTileBBytes;  // 96 KB
-constexpr int kEpiPitch = 36;  // floats per row of the epilogue transpose tile (144 B: keeps float4 alignment, spreads banks)
+constexpr uint32_t kTileBBytes = kGemmBN * kGemmBK * 4;  // 16 KB
+constexpr uint32_t kHalfABytes = kTileABytes / 2;        // the 64 rows of one consumer warpgroup
+constexpr uint32_t kStageBytes = 2 * kTileABytes + 2 * kTileBBytes;  // 64 KB
+constexpr int kEpiPitch = kGemmBN + 8;  // floats per row of the epilogue tile (the fragment's 8-byte stores of 8 rows hit 32 distinct banks)
 constexpr size_t kGemmSmemBytes = (size_t)kGemmStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+static_assert((size_t)kGemmBM * kEpiPitch * 4 <= (size_t)kGemmStages * kStageBytes, "epilogue tile reuses the stages");
 
 // ---- PTX wrappers ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t s32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -46,6 +49,7 @@ __device__ __forceinline__ void bar_init(uint64_t* b, uint32_t n) { asm volatile
 __device__ __forceinline__ void bar_expect_tx(uint64_t* b, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(s32(b)), "r"(bytes) : "memory");
 }
+__device__ __forceinline__ void bar_arrive(uint64_t* b) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(s32(b)) : "memory"); }
 __device__ __forceinline__ void bar_wait(uint64_t* b, uint32_t parity) {
   asm volatile(
       "{\n"
@@ -57,89 +61,71 @@ __device__ __forceinline__ void bar_wait(uint64_t* b, uint32_t parity) {
       "DONE:\n"
       "}" ::"r"(s32(b)), "r"(parity) : "memory");
 }
-// The same wait for warps that are NOT on the critical path (the epilogue warps waiting for an accumulator chunk): sleep between polls.  A tight try_wait loop issues continuously, and eight spinning epilogue warps share
-// the four schedulers with the two converter warps -- ncu showed the converters issue-starved at 0.13 IPC while the spin loops
-// executed more instructions than the rest of the kernel.
-__device__ __forceinline__ void bar_wait_relaxed(uint64_t* b, uint32_t parity) {
-  for (;;) {
-    uint32_t ok;
-    asm volatile(
-        "{\n"
-        ".reg .pred P1;\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%1], %2;\n"
-        "selp.u32 %0, 1, 0, P1;\n"
-        "}"
-        : "=r"(ok)
-        : "r"(s32(b)), "r"(parity)
-        : "memory");
-    if (ok) return;
-    __nanosleep(200);
-  }
-}
 __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int x, int y, uint64_t* bar) {
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(s32(dst)),
                "l"(reinterpret_cast<uint64_t>(map)), "r"(x), "r"(y), "r"(s32(bar))
                : "memory");
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s32(dst_smem)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t addr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(ncols) : "memory");
+// keeps the compiler from moving accesses of the accumulator registers across a wgmma fence / wait
+__device__ __forceinline__ void fence_acc(float (&d)[kAcc]) {
+#pragma unroll
+  for (int j = 0; j < kAcc; ++j) asm volatile("" : "+f"(d[j])::"memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(s32(bar)) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]^T, tf32 inputs, fp32 accumulate
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+// D (+)= A[smem desc, 64 x 8] * B[smem desc, 128 x 8]^T, tf32 inputs, fp32 accumulate in registers.  Fragment of thread t of the
+// warpgroup: d[4 j + 2 h + c] = D[16 (t / 32) + (t % 32) / 4 + 8 h][8 j + 2 (t % 4) + c]
+__device__ __forceinline__ void wgmma_tf32(float (&d)[kAcc], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-      "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+      "setp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, "
-      "%28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-        "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]),
-        "=r"(r[31])
-      : "r"(taddr)
+      "%28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, "
+      "%54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]),
+        "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]),
+        "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]),
+        "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+        "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]),
+        "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]),
+        "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate)
       : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
 }
 
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-        "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// shared-memory matrix descriptor of a K-major tile stored as rows of 128 bytes with the 128-byte swizzle
-// (cute::UMMA::SmemDescriptor: start>>4 | LBO<<16 | SBO<<32 | version(1)<<46 | layout(SWIZZLE_128B = 2)<<61)
+// shared-memory matrix descriptor (wgmma) of a K-major tile stored as rows of 128 bytes with the 128-byte swizzle:
+// start >> 4 | LBO (unused for swizzled K-major, canonical 1) << 16 | SBO (8 rows x 128 B between core-matrix groups) >> 4 << 32 |
+// layout SWIZZLE_128B (1) << 62.  Tiles are 1024-byte aligned, so the base offset field stays 0.
 __device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)1 << 16;            // leading byte offset (unused for swizzled K-major), canonical value 1
-  d |= (uint64_t)(1024 >> 4) << 32;  // stride byte offset: 8 rows x 128 B between core-matrix groups
-  d |= (uint64_t)1 << 46;            // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;            // SWIZZLE_128B
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)(1024 >> 4) << 32;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-// instruction descriptor (cute::UMMA::InstrDescriptor): D = F32, A = B = TF32, both K-major, M = 128, N = 256
-constexpr uint32_t kIdesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(kGemmBN >> 3) << 17) | ((uint32_t)(kGemmBM >> 4) << 24);
+
+// The 3xTF32 products of one K-block (32 floats = 4 wgmma K-steps) into the chunk accumulator d; small terms first, the dominant
+// hi*hi product last.  `first`: the chunk starts here (the first MMA overwrites d).
+__device__ __forceinline__ void mma_kblock(float (&d)[kAcc], uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo, bool first) {
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < kGemmBK / kWgmmaK; ++k) {
+    const uint64_t adv = (uint64_t)((k * kWgmmaK * 4) >> 4);  // advance the start address by 32 bytes per MMA along K
+    wgmma_tf32(d, a_hi + adv, b_lo + adv, (first && k == 0) ? 0u : 1u);
+    wgmma_tf32(d, a_lo + adv, b_hi + adv, 1u);
+    wgmma_tf32(d, a_hi + adv, b_hi + adv, 1u);
+  }
+  wgmma_commit();
+}
 
 // lo = x - trunc_tf32(x) of a whole tile, by 64 threads: thread ct handles the float4 at byte ct * 16 + j * 1024 (addresses in the shared
 // window); 16 loads are issued before the first use
@@ -186,27 +172,13 @@ struct GemmParams {
   const float* row_bias;
   int64_t rb_batch_stride;
   int row_act;
-  int debug;  // measurement only (EVOK_GATHER_DEBUG): 1 = skip the global loads of the gather, 2 = skip bias / activation
   int b_lo_tma;  // CONVERT: the lo tile of B comes from a pre-split copy (map_b_lo) instead of being derived by the converter warps
-  int c_unit_fastest;  // persistent gather kernel: C[(batch * N + col) * rows_per_batch + row_in_batch] (one cache line per store instruction)
-  long long* trace;  // -DEVOK_GEMM_TRACE builds only: clock64() stamps of CTA 0's roles per K-block (scripts/gather_trace.py)
+  int c_unit_fastest;  // persistent gather kernel: C[(batch * N + col) * rows_per_batch + row_in_batch]
 };
 
-#ifdef EVOK_GEMM_TRACE
-#define EVOK_TRACE(slot, idx)                                                                                      \
-  do {                                                                                                             \
-    if (p.trace && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && (idx) < 512u) p.trace[(size_t)(idx) * 16 + (slot)] = clock64();               \
-  } while (0)
-#else
-#define EVOK_TRACE(slot, idx) \
-  do {                        \
-  } while (0)
-#endif
-
-// The tensor core adds every MMA into the TMEM accumulator with round-toward-zero; over hundreds of MMAs that is a
-// systematic shrink of ~2e-8 per MMA (measured: -7e-6 relative after 384 MMAs).  The accumulation is therefore CHUNKED:
-// kGemmChunk K-blocks (48 MMAs) go into one of two TMEM accumulators, then the epilogue warps fold that partial into
-// register accumulators with ordinary round-to-nearest fp32 adds while the MMA warp fills the other TMEM accumulator.
+// The tensor core does not round its fp32 accumulation to nearest; over hundreds of MMAs that is a systematic drift of the
+// result.  The accumulation is therefore CHUNKED: kGemmChunk K-blocks (48 MMAs) go into the wgmma accumulator, which the consumer
+// threads then fold into a second register accumulator with ordinary round-to-nearest fp32 adds.
 constexpr int kGemmChunk = 4;
 
 __device__ __noinline__ float gemm_act(float v, int act) {
@@ -230,45 +202,31 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
   unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(gemm_smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full = reinterpret_cast<uint64_t*>(base + (size_t)kGemmStages * kStageBytes);
   uint64_t* empty = full + kGemmStages;
-  uint64_t* tmem_full = empty + kGemmStages;  // [2]
-  uint64_t* tmem_empty = tmem_full + 2;       // [2]
-  uint64_t* conv = tmem_empty + 2;            // [kGemmStages] lo tiles of the stage derived (CONVERT)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(conv + kGemmStages);
+  uint64_t* conv = empty + kGemmStages;  // [kGemmStages] lo tiles of the stage derived (CONVERT)
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;  // (uniform: keeps the wgmma path non-divergent)
   const int m0 = blockIdx.x * kGemmBM, n0 = blockIdx.y * kGemmBN;
   const int total_kb = (p.K + kGemmBK - 1) / kGemmBK;
   const int kb_begin = blockIdx.z * p.kblocks_per_split;
   const int kb_end = min(total_kb, kb_begin + p.kblocks_per_split);
   const int num_kb = max(kb_end - kb_begin, 0);
-  const int num_chunks = (num_kb + kGemmChunk - 1) / kGemmChunk;
-  if (threadIdx.x == 0) EVOK_TRACE(13, 0u);  // kernel start
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < kGemmStages; ++s) {
       bar_init(&full[s], 1);
-      bar_init(&empty[s], 1);
-      bar_init(&conv[s], 2);  // one arrival per converter warp
-    }
-    for (int t = 0; t < 2; ++t) {
-      bar_init(&tmem_full[t], 1);
-      bar_init(&tmem_empty[t], 8);  // one arrival per epilogue warp
+      bar_init(&empty[s], 8);  // one arrival per consumer warp
+      bar_init(&conv[s], 2);   // one arrival per converter warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 2 * kGemmBN);  // two accumulators of 256 fp32 columns x 128 lanes = all 512 columns
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp == 0) {
     if (lane == 0) {
       for (int i = 0; i < num_kb; ++i) {
         const int s = i % kGemmStages;
         const uint32_t use = i / kGemmStages;
-        bar_wait(&empty[s], (use & 1) ^ 1);  // first use of a stage passes immediately (tight poll: with two stages the wake-up is on the critical path)
-        EVOK_TRACE(9, (uint32_t)i);
+        bar_wait(&empty[s], (use & 1) ^ 1);  // first use of a stage passes immediately
         unsigned char* st = base + (size_t)s * kStageBytes;
         bar_expect_tx(&full[s], (GATHER ? kTileBBytes : (CONVERT ? kTileABytes + kTileBBytes : kStageBytes)) + ((CONVERT && p.b_lo_tma) ? kTileBBytes : 0u));
         const int kx = (kb_begin + i) * kGemmBK;
@@ -278,44 +236,12 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
         if (!CONVERT || p.b_lo_tma) tma_load_2d(st + 2 * kTileABytes + kTileBBytes, &map_b_lo, kx, n0, &full[s]);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      for (int i = 0; i < num_kb; ++i) {
-        const int s = i % kGemmStages;
-        const uint32_t use = i / kGemmStages;
-        const int ch = i / kGemmChunk, in_chunk = i % kGemmChunk;
-        const int buf = ch & 1;
-        if (in_chunk == 0 && ch >= 2) {  // the epilogue must have drained this accumulator (chunk ch - 2)
-          bar_wait(&tmem_empty[buf], ((ch >> 1) - 1) & 1);
-          tc_fence_after();
-        }
-        bar_wait(CONVERT ? &conv[s] : &full[s], use & 1);  // CONVERT: the converter warps have derived the lo tiles of this stage
-        EVOK_TRACE(6, (uint32_t)i);
-        tc_fence_after();
-        const uint32_t acc = tmem_base + (uint32_t)(buf * kGemmBN);
-        const uint32_t st = s32(base + (size_t)s * kStageBytes);
-        const uint64_t a_hi = make_sw128_desc(st), a_lo = make_sw128_desc(st + kTileABytes);
-        const uint64_t b_hi = make_sw128_desc(st + 2 * kTileABytes), b_lo = make_sw128_desc(st + 2 * kTileABytes + kTileBBytes);
-#pragma unroll
-        for (int k = 0; k < kGemmBK / kUmmaK; ++k) {
-          const uint64_t adv = (uint64_t)((k * kUmmaK * 4) >> 4);  // advance the start address by 32 bytes per MMA along K
-          // small terms first, the dominant hi*hi product last
-          umma_tf32(acc, a_hi + adv, b_lo + adv, kIdesc, (in_chunk | k) != 0);
-          umma_tf32(acc, a_lo + adv, b_hi + adv, kIdesc, 1);
-          umma_tf32(acc, a_hi + adv, b_hi + adv, kIdesc, 1);
-        }
-        umma_commit(&empty[s]);  // stage reusable once these MMAs have consumed it
-        if (in_chunk == kGemmChunk - 1 || i == num_kb - 1) umma_commit(&tmem_full[buf]);  // chunk accumulator complete
-        EVOK_TRACE(8, (uint32_t)i);
-      }
-    }
   } else if (warp < 4) {
     // ===== 2 converter warps (CONVERT): per K-block wait for the raw tiles, derive lo = x - trunc_tf32(x) for both operands
-    // (element-wise, so every element simply keeps its swizzled position: 3072 float4 per stage, 48 per thread), publish them to
-    // the tensor core (async proxy) and signal the MMA warp.  Runs one or two K-blocks ahead of the MMAs.
-    if (CONVERT) {
+    // (element-wise, so every element simply keeps its swizzled position: 2048 float4 per stage, 32 per thread), publish them to
+    // the tensor core (async proxy) and signal the consumers.  Runs up to two K-blocks ahead of the MMAs.
+    if (CONVERT && warp >= 2) {
       const int ct = threadIdx.x - 64;  // 0 .. 63
-      auto lo_of = [](float v) { return v - __uint_as_float(__float_as_uint(v) & 0xFFFFE000u); };
       // GATHER: the A tile of K-block i is fetched with 4-byte cp.async copies (global -> shared, no registers, zero fill outside
       // the matrix): one 128-byte row segment per warp instruction, 64 rows per warp, all in flight at once; element (r, k) of a
       // 128B-swizzled K-major tile sits at  r * 128 + ((k / 4) ^ (r % 8)) * 16 + (k % 4) * 4.  The copy of block i + 1 is issued
@@ -335,7 +261,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
 #pragma unroll 8
         for (int it = 0; it < 64; ++it) {
           const int r = wrow0 + it;
-          const bool ok = k_ok && (m0 + r < p.M) && p.debug != 1;
+          const bool ok = k_ok && (m0 + r < p.M);
           const uint32_t off = (uint32_t)r * 128u + ((((uint32_t)lane >> 2) ^ ((uint32_t)r & 7u)) << 4) + (((uint32_t)lane & 3u) << 2);
           const float* src = ok ? rowp : p.gather_a;  // a valid address even when nothing is read (src-size 0 -> zero fill)
           asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(st_a + off), "l"(src), "r"(ok ? 4 : 0) : "memory");
@@ -356,156 +282,167 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
           asm volatile("cp.async.wait_group 0;" ::: "memory");  // this thread's copies of block i have landed
           asm volatile("bar.sync 1, 64;" ::: "memory");         // ... and so have the other converter warp's
         }
-        if (threadIdx.x == 64) EVOK_TRACE(0, (uint32_t)i);
         bar_wait(&full[s], use & 1);
-        if (threadIdx.x == 64) EVOK_TRACE(1, (uint32_t)i);
         const float4* a_raw = reinterpret_cast<const float4*>(st);
         float4* a_lo = reinterpret_cast<float4*>(st + kTileABytes);
         const float4* b_raw = reinterpret_cast<const float4*>(st + 2 * kTileABytes);
         float4* b_lo = reinterpret_cast<float4*>(st + 2 * kTileABytes + kTileBBytes);
-        // (a single warp runs this dependent stream at ~0.2 IPC, so the instruction count per K-block is what matters: shared-space
-        // 16-byte loads / stores with immediate offsets, 16 loads in flight; B is skipped when its lo tile came by TMA)
+        // shared-space 16-byte loads / stores with immediate offsets, 16 loads in flight; B is skipped when its lo tile came by TMA
         split_lo_tile<kTileABytes>(s32(a_raw) + (uint32_t)ct * 16u, s32(a_lo) + (uint32_t)ct * 16u);
         if (!p.b_lo_tma) split_lo_tile<kTileBBytes>(s32(b_raw) + (uint32_t)ct * 16u, s32(b_lo) + (uint32_t)ct * 16u);
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy stores -> visible to the tensor core's reads
         __syncwarp();
-        if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(s32(&conv[s])) : "memory");
-        if (threadIdx.x == 64) EVOK_TRACE(3, (uint32_t)i);
-        // the next block's copy is issued AFTER this block has been handed to the tensor core (its stage frees up when the MMAs of
-        // block i - 1 retire, which overlaps with the MMAs of block i)
+        if (lane == 0) bar_arrive(&conv[s]);
+        // the next block's copy is issued AFTER this block has been handed to the tensor core
         if (GATHER && i + 1 < num_kb) issue_gather(i + 1);
       }
     }
   } else {
-    // ===== 8 epilogue warps: TMEM lane quadrant = warp % 4, column half = (warp - 4) / 4 =====
-    // Every thread keeps its row's 128 partial sums in REGISTERS and folds each finished TMEM chunk into them with
-    // round-to-nearest fp32 adds (no memory traffic); the final tile goes out through a padded shared-memory transpose so that a
-    // warp writes 4 rows x 128 contiguous bytes per instruction.
-    const int quad = warp & 3, half = (warp - 4) >> 2;
-    float acc[kGemmBN / 2];
+    // ===== 2 consumer warpgroups: warpgroup wg owns rows wg * 64 .. wg * 64 + 63 of the tile =====
+    const int wg = (warp - 4) >> 2;
+    float acc[kAcc], frag[kAcc];
 #pragma unroll
-    for (int j = 0; j < kGemmBN / 2; ++j) acc[j] = 0.0f;
-    auto fold_chunk = [&](int ch) {
-      const int buf = ch & 1;
-      if (threadIdx.x == 128) EVOK_TRACE(10, (uint32_t)ch);
-      bar_wait_relaxed(&tmem_full[buf], (ch >> 1) & 1);
-      if (threadIdx.x == 128) EVOK_TRACE(11, (uint32_t)ch);
-      tc_fence_after();
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        uint32_t r[32];
-        tmem_ld32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(buf * kGemmBN + half * (kGemmBN / 2) + g * 32), r);
-#pragma unroll
-        for (int j = 0; j < 32; ++j) acc[g * 32 + j] += __uint_as_float(r[j]);
-      }
-      tc_fence_before();
+    for (int j = 0; j < kAcc; ++j) acc[j] = 0.0f;
+    int pending = -1;  // stage whose MMAs may still be in flight (released once the next K-block's wait proves them done)
+    auto release = [&](int s) {
       __syncwarp();
-      if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(s32(&tmem_empty[buf])) : "memory");
+      if (lane == 0) bar_arrive(&empty[s]);
     };
-    for (int ch = 0; ch < num_chunks; ++ch) fold_chunk(ch);
-    if (threadIdx.x == 128) EVOK_TRACE(13, 1u);  // all chunks folded: the store phase starts
-    if (GATHER && p.row_bias && p.debug != 2) {  // C = act(acc + bias of this row): TMEM lane = row of the tile
-      const int64_t m = (int64_t)m0 + quad * 32 + lane;
-      if (m < p.M) {
-        const int64_t bi = m / p.ga_rows_per_batch;
-        const float b = __ldg(p.row_bias + bi * p.rb_batch_stride + (m - bi * p.ga_rows_per_batch));
-        // the activation switch is hoisted out of the unrolled loop: one 128-fold copy of ONE activation per branch, the common
-        // NONE case is a plain add (a per-element switch with an inlined tanhf was 15 k instructions: instruction-cache bound)
-        if (p.row_act == EVOK_ACT_NONE) {
+    for (int i = 0; i < num_kb; ++i) {
+      const int s = i % kGemmStages;
+      const uint32_t use = i / kGemmStages;
+      const int in_chunk = i % kGemmChunk;
+      bar_wait(CONVERT ? &conv[s] : &full[s], use & 1);  // CONVERT: the converter warps have derived the lo tiles of this stage
+      const uint32_t st = s32(base + (size_t)s * kStageBytes);
+      mma_kblock(frag, make_sw128_desc(st + wg * kHalfABytes), make_sw128_desc(st + kTileABytes + wg * kHalfABytes),
+                 make_sw128_desc(st + 2 * kTileABytes), make_sw128_desc(st + 2 * kTileABytes + kTileBBytes), in_chunk == 0);
+      if (in_chunk == kGemmChunk - 1 || i == num_kb - 1) {  // chunk complete: fold it
+        wgmma_wait<0>();
+        fence_acc(frag);
+        if (pending >= 0) release(pending);
+        release(s);
+        pending = -1;
 #pragma unroll
-          for (int j = 0; j < kGemmBN / 2; ++j) acc[j] += b;
-        } else if (p.row_act == EVOK_ACT_RELU) {
-#pragma unroll
-          for (int j = 0; j < kGemmBN / 2; ++j) acc[j] = fmaxf(acc[j] + b, 0.0f);
-        } else {
-#pragma unroll
-          for (int j = 0; j < kGemmBN / 2; ++j) acc[j] = gemm_act(acc[j] + b, p.row_act);  // 128 calls of the out-of-line function
-        }
+        for (int j = 0; j < kAcc; ++j) acc[j] += frag[j];
+      } else {
+        wgmma_wait<1>();  // the previous K-block's MMAs are done
+        if (pending >= 0) release(pending);
+        pending = s;
       }
     }
-    // all MMAs have completed (the last tmem_full has fired), so the pipeline stages are free: use them as transpose scratch
-    float* stile = reinterpret_cast<float*>(base) + (size_t)(warp - 4) * (32 * kEpiPitch);
+    wgmma_wait<0>();  // (the last K-block always waited already; this makes it visible to the compiler, which would insert its own)
+    // every MMA of both warpgroups has completed (and with them every load and conversion feeding them): the stages are free, use
+    // them as a transpose tile so that a warp writes 512 contiguous bytes of one row per instruction
+    asm volatile("bar.sync 2, 256;" ::: "memory");
+    float* stile = reinterpret_cast<float*>(base);
+    {
+      const int t = threadIdx.x & 127;
+      const int r = wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2), c = 2 * (t & 3);
+#pragma unroll
+      for (int j = 0; j < kAcc / 4; ++j) {
+        *reinterpret_cast<float2*>(stile + r * kEpiPitch + 8 * j + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        *reinterpret_cast<float2*>(stile + (r + 8) * kEpiPitch + 8 * j + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+      }
+    }
+    asm volatile("bar.sync 2, 256;" ::: "memory");
     const float alpha = (p.C2 && p.alpha_dev) ? *p.alpha_dev : 1.0f;
     const bool affine = p.affine_k != nullptr && gridDim.z == 1;
     const float k0 = affine ? p.affine_k[0] : 1.0f, k1 = affine ? p.affine_k[1] : 0.0f, k2 = affine ? p.affine_k[2] : 0.0f;
     float* cbase = p.C + (int64_t)blockIdx.z * p.split_stride;
     const bool vec_ok = ((reinterpret_cast<uintptr_t>(cbase) & 15) == 0) && (p.ldc % 4 == 0);
-    const int sub_row = lane >> 3, sub_col = (lane & 7) * 4;
-#pragma unroll
-    for (int g = 0; g < 4; ++g) {
-#pragma unroll
-      for (int j = 0; j < 32; j += 4)
-        *reinterpret_cast<float4*>(stile + lane * kEpiPitch + j) = make_float4(acc[g * 32 + j], acc[g * 32 + j + 1], acc[g * 32 + j + 2], acc[g * 32 + j + 3]);
-      __syncwarp();
-      const int col = n0 + half * (kGemmBN / 2) + g * 32 + sub_col;
-#pragma unroll
-      for (int it = 0; it < 8; ++it) {
-        const int rr = it * 4 + sub_row;
-        const int row = m0 + quad * 32 + rr;
-        const float4 v = *reinterpret_cast<const float4*>(stile + rr * kEpiPitch + sub_col);
-        if (row < p.M) {
-          float* cp = cbase + (int64_t)row * p.ldc + col;
-          float e[4] = {v.x, v.y, v.z, v.w};
-          if (affine) {
-            const float ur = p.affine_u ? __ldg(p.affine_u + row) : 0.0f;
-            for (int t = 0; t < 4; ++t)
-              if (col + t < p.N)
-                e[t] = fmaf(k0, e[t], fmaf(k1, p.affine_E ? p.affine_E[(int64_t)row * p.lde + col + t] : 0.0f,
-                                          k2 * ur * (p.affine_u ? __ldg(p.affine_u + col + t) : 0.0f)));
-          }
-          if (!affine && vec_ok && col + 4 <= p.N) {
-            *reinterpret_cast<float4*>(cp) = v;
-          } else {
-            for (int t = 0; t < 4; ++t)
-              if (col + t < p.N) cp[t] = e[t];
-          }
-          if (p.C2) {
-            float* c2 = p.C2 + (int64_t)row * p.ldc2 + col;
-            for (int t = 0; t < 4; ++t)
-              if (col + t < p.N) c2[t] = fmaf(alpha, e[t], p.bias ? __ldg(p.bias + col + t) : 0.0f);
-          }
-        }
+    const int col = n0 + lane * 4;
+    for (int rr = warp - 4; rr < kGemmBM && m0 + rr < p.M; rr += 8) {
+      const int row = m0 + rr;
+      const float4 v = *reinterpret_cast<const float4*>(stile + rr * kEpiPitch + lane * 4);
+      float e[4] = {v.x, v.y, v.z, v.w};
+      if (GATHER && p.row_bias) {  // C = act(acc + bias of this row)
+        const int64_t bi = row / p.ga_rows_per_batch;
+        const float b = __ldg(p.row_bias + bi * p.rb_batch_stride + (row - bi * p.ga_rows_per_batch));
+        for (int t = 0; t < 4; ++t) e[t] = p.row_act == EVOK_ACT_NONE ? e[t] + b : gemm_act(e[t] + b, p.row_act);
       }
-      __syncwarp();
+      if (affine) {
+        const float ur = p.affine_u ? __ldg(p.affine_u + row) : 0.0f;
+        for (int t = 0; t < 4; ++t)
+          if (col + t < p.N)
+            e[t] = fmaf(k0, e[t], fmaf(k1, p.affine_E ? p.affine_E[(int64_t)row * p.lde + col + t] : 0.0f,
+                                      k2 * ur * (p.affine_u ? __ldg(p.affine_u + col + t) : 0.0f)));
+      }
+      float* cp = cbase + (int64_t)row * p.ldc + col;
+      if (vec_ok && col + 4 <= p.N) {
+        *reinterpret_cast<float4*>(cp) = make_float4(e[0], e[1], e[2], e[3]);
+      } else {
+        for (int t = 0; t < 4; ++t)
+          if (col + t < p.N) cp[t] = e[t];
+      }
+      if (p.C2) {
+        float* c2 = p.C2 + (int64_t)row * p.ldc2 + col;
+        for (int t = 0; t < 4; ++t)
+          if (col + t < p.N) c2[t] = fmaf(alpha, e[t], p.bias ? __ldg(p.bias + col + t) : 0.0f);
+      }
     }
-  }
-  if (threadIdx.x == 128) EVOK_TRACE(13, 2u);  // stores issued
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 2 * kGemmBN);
   }
 }
 
 // ---- persistent gather GEMM (batched policy forward on ONE shared minibatch) ------------------------------------------------
 // Same arithmetic as gemm_tf32x3_kernel<true, true>, restructured for the shape this path has -- millions of A rows (the stacked
 // first-layer weights), a small B operand (the minibatch) that every tile re-reads:
-//   * PERSISTENT: one CTA per SM walks the output tiles (tile = blockIdx.x + q * gridDim.x), so barrier set-up and the TMEM allocation
-//     happen once, and the epilogue of tile q (bias, activation, 128 KB of stores) runs while the tensor core is already two
-//     accumulator chunks into tile q + 1 (the two TMEM accumulators of the chunked accumulation double as the overlap buffer);
+//   * PERSISTENT: one CTA per SM walks the output tiles (tile = blockIdx.x + q * gridDim.x), so barrier set-up happens once and the
+//     gather of the next tile's A operand is already in flight while the consumers store the previous tile;
 //   * the minibatch is split into hi / lo ONCE by a pre-pass (it is a few hundred KB) and both tiles arrive by TMA: the converter
 //     warps only derive the lo tile of the gathered A operand (a third of the element-wise work of the generic kernel);
 //   * the gathered A tiles live in a 4-deep ring of raw tiles (three 16 KB gathers in flight per SM while one is converted) with only
-//     two lo buffers behind it (a lo tile is derived right before its MMAs); the minibatch tiles (2 stages of hi + lo, 128 KB) come
-//     from L2;
-//   * the epilogue warps store their rows straight from registers (a row of the tile = 128 consecutive floats per thread).
+//     two lo buffers behind it (a lo tile is derived right before its MMAs); the minibatch tiles (3 stages of hi + lo) come from L2;
+//   * the consumers apply bias + activation to their accumulator fragments and store them straight from registers.
 // the minibatch operand, pre-split into hi / lo and stored four times, copy s shifted right by s floats (xs[b][k'] = x[b][k' - s], zero
-// outside): TMA needs 16-byte aligned box coordinates (an odd K coordinate is an illegal instruction), so a tile whose rows sit sh
-// floats past a 16-byte boundary reads copy sh at the aligned coordinate 32 i instead of the original at 32 i - sh
+// outside): TMA needs 16-byte aligned box coordinates, so a tile whose rows sit sh floats past a 16-byte boundary reads copy sh at the
+// aligned coordinate 32 i instead of the original at 32 i - sh
 struct GatherMaps {
   CUtensorMap hi[4];
   CUtensorMap lo[4];
 };
 
-// K-blocks per TMEM accumulator chunk, as in the generic kernel.  (6 -- two chunks per 12-block tile, so that the tensor core could finish
-// a whole tile while the epilogue stores the previous one -- was tried: 28.7 vs 29.0 ms, not worth the larger round-toward-zero error.
-// The timeline shows why: during the store phase the converter warps themselves slow down 3-5x -- the epilogue's row-per-thread 16-byte
-// stores are 32 cache-line operations per warp instruction, 8192 per tile, in the same LSU pipe as the converters' LDS / STS / LDGSTS.)
-constexpr int kPersChunk = 4;
-constexpr int kPersRawStages = 4, kPersLoStages = 2, kPersBStages = 2;
+constexpr int kPersChunk = 4;  // K-blocks per accumulator chunk, as in the generic kernel
+constexpr int kPersRawStages = 4, kPersLoStages = 2, kPersBStages = 3;
 constexpr uint32_t kPersBStageBytes = 2 * kTileBBytes;
 constexpr size_t kPersSmemBytes =
     (size_t)(kPersRawStages + kPersLoStages) * kTileABytes + (size_t)kPersBStages * kPersBStageBytes + 1024 /*align*/ + 256;
+
+// bias + activation of one accumulator fragment, stored on the way out (one unrolled copy per activation: a per-element switch would
+// not fit the instruction cache).  Rows r_first and r_first + 8 of the tile, columns n0 + 8 j + c and + 1.
+template <int ACT>
+__device__ __forceinline__ float pers_act(float v) {
+  if (ACT == EVOK_ACT_RELU) return fmaxf(v, 0.0f);
+  if (ACT == EVOK_ACT_TANH) return tanh_abs1e7(v);
+  if (ACT == EVOK_ACT_SIGMOID) return activate_fast(v, EVOK_ACT_SIGMOID);
+  return v;
+}
+template <int ACT>
+__device__ __forceinline__ void pers_store(const GemmParams& p, const float (&acc)[kAcc], int m0, int r_first, int n0, int c, bool vec_ok) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int64_t m = (int64_t)m0 + r_first + 8 * h;
+    if (m >= p.M) continue;
+    const int64_t bi = m / p.ga_rows_per_batch, hrow = m - bi * p.ga_rows_per_batch;
+    const float b = p.row_bias ? __ldg(p.row_bias + bi * p.rb_batch_stride + hrow) : 0.0f;
+    float* crow = p.C + m * p.ldc;
+    // unit-fastest layout: the 8 rows a warp holds per register are consecutive units of one batch (32 contiguous bytes per column)
+    float* ccol = p.C + (bi * p.N) * p.ga_rows_per_batch + hrow;
+#pragma unroll
+    for (int j = 0; j < kAcc / 4; ++j) {
+      const int col = n0 + 8 * j + c;
+      const float v0 = pers_act<ACT>(acc[4 * j + 2 * h] + b), v1 = pers_act<ACT>(acc[4 * j + 2 * h + 1] + b);
+      if (p.c_unit_fastest) {
+        if (col < p.N) ccol[(int64_t)col * p.ga_rows_per_batch] = v0;
+        if (col + 1 < p.N) ccol[(int64_t)(col + 1) * p.ga_rows_per_batch] = v1;
+      } else if (vec_ok && col + 2 <= p.N) {
+        *reinterpret_cast<float2*>(crow + col) = make_float2(v0, v1);
+      } else {
+        if (col < p.N) crow[col] = v0;
+        if (col + 1 < p.N) crow[col + 1] = v1;
+      }
+    }
+  }
+}
 
 __global__ void __launch_bounds__(kGemmThreads, 1)
     gemm_gather_persistent_kernel(const __grid_constant__ GatherMaps maps, const GemmParams p) {
@@ -519,20 +456,14 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
   uint64_t* empty_raw = empty_b + kPersBStages;
   uint64_t* empty_lo = empty_raw + kPersRawStages;
   uint64_t* conv_a = empty_lo + kPersLoStages;
-  uint64_t* tmem_full = conv_a + kPersLoStages;  // [2]
-  uint64_t* tmem_empty = tmem_full + 2;         // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;  // (uniform: keeps the wgmma path non-divergent)
   // VECTOR mode (rows of K % 4 == 0 floats at pitch K, a tile never straddles two batches): all rows of a tile share one misalignment
   // `sh` (0..3 floats past a 16-byte boundary), so the K axis of that tile is simply cut at 16-byte-aligned source addresses --
   // K-block i covers k = 32 i - sh .. 32 i - sh + 31 for BOTH operands (the minibatch tile comes from the copy shifted by sh floats,
-  // GatherMaps; zeros for k < 0 and k >= K) -- and the gather moves 16 bytes per copy.  4-byte cp.async copies turned out to cost ~57 issue
-  // cycles per warp instruction (ncu: 70 % of the converter warps' samples sat on the 64 LDGSTS of a K-block), which bounded the
-  // whole kernel at 2.6 us per K-block against 0.9 us of tensor-core work.
+  // GatherMaps; zeros for k < 0 and k >= K) -- and the gather moves 16 bytes per copy instead of 4.
   const bool vec_mode = (p.K % 4 == 0) && (p.ga_row_stride == p.K) && (p.ga_rows_per_batch % kGemmBM == 0);
   const int num_kb = (p.K + (vec_mode ? 3 : 0) + kGemmBK - 1) / kGemmBK;
-  const int num_chunks = (num_kb + kPersChunk - 1) / kPersChunk;
   const int n_tiles = (p.N + kGemmBN - 1) / kGemmBN;
   const int64_t total_tiles = (int64_t)((p.M + kGemmBM - 1) / kGemmBM) * n_tiles;
   auto tile_rows = [&](int64_t t, int& m0, int& sh) -> const float* {  // first row of tile t (VECTOR mode) and its misalignment
@@ -548,24 +479,16 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
   if (threadIdx.x == 0) {
     for (int s = 0; s < kPersBStages; ++s) {
       bar_init(&full_b[s], 1);
-      bar_init(&empty_b[s], 1);
+      bar_init(&empty_b[s], 8);  // one arrival per consumer warp
     }
-    for (int s = 0; s < kPersRawStages; ++s) bar_init(&empty_raw[s], 1);
+    for (int s = 0; s < kPersRawStages; ++s) bar_init(&empty_raw[s], 8);
     for (int s = 0; s < kPersLoStages; ++s) {
-      bar_init(&empty_lo[s], 1);
+      bar_init(&empty_lo[s], 8);
       bar_init(&conv_a[s], 2);  // one arrival per converter warp
-    }
-    for (int t = 0; t < 2; ++t) {
-      bar_init(&tmem_full[t], 1);
-      bar_init(&tmem_empty[t], 8);  // one arrival per epilogue warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 2 * kGemmBN);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp == 0) {
     // ===== TMA producer of the minibatch tiles (hi, lo) =====
@@ -578,60 +501,19 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
         tile_rows(t, m0_unused, sh);
         for (int i = 0; i < num_kb; ++i, ++g) {
           const int s = g % kPersBStages;
-          bar_wait(&empty_b[s], ((g / kPersBStages) & 1) ^ 1);  // tight poll: the minibatch tile of block g + 2 is needed ~1 block later
-          EVOK_TRACE(9, g);
+          bar_wait(&empty_b[s], ((g / kPersBStages) & 1) ^ 1);
           unsigned char* st = b_base + (size_t)s * kPersBStageBytes;
-          // (p.debug == 3, measurement only: the lo tile of the minibatch is not loaded -- wrong results, half the L2 -> SM traffic)
-          bar_expect_tx(&full_b[s], p.debug == 3 ? kTileBBytes : kPersBStageBytes);
+          bar_expect_tx(&full_b[s], kPersBStageBytes);
           tma_load_2d(st, &maps.hi[sh], i * kGemmBK, n0, &full_b[s]);
-          if (p.debug != 3) tma_load_2d(st + kTileBBytes, &maps.lo[sh], i * kGemmBK, n0, &full_b[s]);
+          tma_load_2d(st + kTileBBytes, &maps.lo[sh], i * kGemmBK, n0, &full_b[s]);
         }
       }
     }
   } else if (warp == 1) {
-    // ===== MMA issue =====
-    if (lane == 0) {
-      uint32_t g = 0, gch = 0;
-      for (int64_t q = 0; q < my_tiles; ++q) {
-        for (int i = 0; i < num_kb; ++i, ++g) {
-          const int sr = g % kPersRawStages, sl = g % kPersLoStages, sb = g % kPersBStages;
-          const int in_chunk = i % kPersChunk;
-          const int buf = gch & 1;
-          if (in_chunk == 0 && gch >= 2) {  // the epilogue must have folded the chunk that used this accumulator (two chunks ago)
-            bar_wait(&tmem_empty[buf], ((gch >> 1) - 1) & 1);
-            tc_fence_after();
-          }
-          bar_wait(&conv_a[sl], (g / kPersLoStages) & 1);
-          EVOK_TRACE(6, g);
-          bar_wait(&full_b[sb], (g / kPersBStages) & 1);
-          EVOK_TRACE(7, g);
-          tc_fence_after();
-          const uint32_t acc = tmem_base + (uint32_t)(buf * kGemmBN);
-          const uint32_t stb = s32(b_base + (size_t)sb * kPersBStageBytes);
-          const uint64_t a_hi = make_sw128_desc(s32(raw_base + (size_t)sr * kTileABytes));
-          const uint64_t a_lo = make_sw128_desc(s32(lo_base + (size_t)sl * kTileABytes));
-          const uint64_t b_hi = make_sw128_desc(stb), b_lo = make_sw128_desc(stb + kTileBBytes);
-#pragma unroll
-          for (int k = 0; k < kGemmBK / kUmmaK; ++k) {
-            const uint64_t adv = (uint64_t)((k * kUmmaK * 4) >> 4);
-            umma_tf32(acc, a_hi + adv, b_lo + adv, kIdesc, (in_chunk | k) != 0);
-            umma_tf32(acc, a_lo + adv, b_hi + adv, kIdesc, 1);
-            umma_tf32(acc, a_hi + adv, b_hi + adv, kIdesc, 1);
-          }
-          umma_commit(&empty_raw[sr]);
-          umma_commit(&empty_lo[sl]);
-          umma_commit(&empty_b[sb]);
-          EVOK_TRACE(8, g);
-          if (in_chunk == kPersChunk - 1 || i == num_kb - 1) {
-            umma_commit(&tmem_full[buf]);
-            ++gch;
-          }
-        }
-      }
-    }
+    // idle
   } else if (warp < 4) {
     // ===== 2 converter warps: gather the A tile of K-block g (64 rows per warp), derive its lo tile =====
-    // One warp executes a dependent instruction stream at ~0.2 IPC, so what bounds this role is its instruction COUNT per K-block:
+    // One warp executes a dependent instruction stream at low IPC, so what bounds this role is its instruction COUNT per K-block:
     // everything that does not change between K-blocks is hoisted (lane offsets, per-tile base / misalignment), shared memory is
     // addressed through 32-bit shared-space addresses (LDS / STS / LDGSTS with immediate offsets), and the rare cases (first chunk of a
     // misaligned row, partial tiles) live in their own branches.
@@ -657,7 +539,6 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
     auto issue_gather = [&](uint32_t g) {
       const int s = g % kPersRawStages;
       bar_wait(&empty_raw[s], ((g / kPersRawStages) & 1) ^ 1);
-      if (threadIdx.x == 64) EVOK_TRACE(4, g);
       const uint32_t st_a = raw_s + (uint32_t)s * kTileABytes;
       const int i = is_i, m0 = is_m0;
       if (vec_mode) {
@@ -736,110 +617,72 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
     if (total_g > 2) issue_gather(2);
     for (uint32_t g = 0; g < total_g; ++g) {
       const int sr = g % kPersRawStages, sl = g % kPersLoStages;
-      if (threadIdx.x == 64) EVOK_TRACE(0, g);
       // block g has landed (blocks g + 1, g + 2 may still be in flight)
       if (g + 2 < total_g) asm volatile("cp.async.wait_group 2;" ::: "memory");
       else if (g + 1 < total_g) asm volatile("cp.async.wait_group 1;" ::: "memory");
       else asm volatile("cp.async.wait_group 0;" ::: "memory");
-      if (threadIdx.x == 64) EVOK_TRACE(14, g);
       asm volatile("bar.sync 1, 64;" ::: "memory");  // ... and so have the other converter warp's rows
-      if (threadIdx.x == 64) EVOK_TRACE(1, g);
       bar_wait(&empty_lo[sl], ((g / kPersLoStages) & 1) ^ 1);  // the MMAs of block g - 2 are done with this lo buffer
-      if (threadIdx.x == 64) EVOK_TRACE(2, g);
       // lo = x - trunc_tf32(x), element-wise (every element keeps its swizzled position): 16 float4 per thread, all loads first
       const uint32_t ra = raw_s + (uint32_t)sr * kTileABytes + (uint32_t)ct * 16u, la = lo_s + (uint32_t)sl * kTileABytes + (uint32_t)ct * 16u;
       split_lo_tile<kTileABytes>(ra, la);
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
       __syncwarp();
       if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(s32(&conv_a[sl])) : "memory");
-      if (threadIdx.x == 64) EVOK_TRACE(3, g);
       if (g + 3 < total_g) issue_gather(g + 3);
-      if (threadIdx.x == 64) EVOK_TRACE(5, g);
     }
   } else {
-    // ===== 8 epilogue warps: TMEM lane quadrant = warp % 4 (tile row = quadrant * 32 + lane), column half = (warp - 4) / 4 =====
-    const int quad = warp & 3, half = (warp - 4) >> 2;
+    // ===== 2 consumer warpgroups: warpgroup wg owns rows wg * 64 .. wg * 64 + 63 of every tile =====
+    const int wg = (warp - 4) >> 2, t = threadIdx.x & 127;
+    const int r_first = wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2), c = 2 * (t & 3);  // accumulator fragment position (wgmma_tf32)
     const bool vec_ok = ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0) && (p.ldc % 4 == 0);
-    uint32_t gch = 0;
-    for (int64_t q = 0; q < my_tiles; ++q) {
-      const int64_t t = blockIdx.x + q * gridDim.x;
-      const int m0 = (int)(t / n_tiles) * kGemmBM, n0 = (int)(t % n_tiles) * kGemmBN;
-      float acc[kGemmBN / 2];
-#pragma unroll
-      for (int j = 0; j < kGemmBN / 2; ++j) acc[j] = 0.0f;
-      for (int ch = 0; ch < num_chunks; ++ch, ++gch) {
-        const int buf = gch & 1;
-        if (threadIdx.x == 128) EVOK_TRACE(10, gch);
-        bar_wait_relaxed(&tmem_full[buf], (gch >> 1) & 1);
-        if (threadIdx.x == 128) EVOK_TRACE(11, gch);
-        tc_fence_after();
-#pragma unroll
-        for (int g8 = 0; g8 < 8; ++g8) {
-          uint32_t r[16];
-          tmem_ld16(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(buf * kGemmBN + half * (kGemmBN / 2) + g8 * 16), r);
-#pragma unroll
-          for (int j = 0; j < 16; ++j) acc[g8 * 16 + j] += __uint_as_float(r[j]);
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(s32(&tmem_empty[buf])) : "memory");
-        if (threadIdx.x == 128) EVOK_TRACE(12, gch);
+    auto release = [&](uint32_t g) {  // the MMAs of block g are done with its raw, lo and minibatch stages
+      __syncwarp();
+      if (lane == 0) {
+        bar_arrive(&empty_raw[g % kPersRawStages]);
+        bar_arrive(&empty_lo[g % kPersLoStages]);
+        bar_arrive(&empty_b[g % kPersBStages]);
       }
-      const int64_t m = (int64_t)m0 + quad * 32 + lane;
-      if (m < p.M) {
-        float b = 0.0f;
-        if (p.row_bias) {
-          const int64_t bi = m / p.ga_rows_per_batch;
-          b = __ldg(p.row_bias + bi * p.rb_batch_stride + (m - bi * p.ga_rows_per_batch));
-        }
-        // bias + activation applied four values at a time on the way out; one unrolled copy of the store loop per activation (a
-        // per-element switch would not fit the instruction cache)
-        float* crow = p.C + m * p.ldc;
-        const int col0 = n0 + half * (kGemmBN / 2);
-        // unit-fastest layout: the 32 lanes of a warp (consecutive rows of one batch) write 128 consecutive bytes per instruction
-        const int64_t bi_c = m / p.ga_rows_per_batch;
-        float* ccol = p.C + (bi_c * p.N + col0) * p.ga_rows_per_batch + (m - bi_c * p.ga_rows_per_batch);
-        const int64_t cstride = p.ga_rows_per_batch;
-        auto store4 = [&](int j, float v0, float v1, float v2, float v3) {
-          const int col = col0 + j;
-          if (p.c_unit_fastest) {
-            const float v[4] = {v0, v1, v2, v3};
+    };
+    uint32_t g = 0;
+    for (int64_t q = 0; q < my_tiles; ++q) {
+      const int64_t tile = blockIdx.x + q * gridDim.x;
+      const int m0 = (int)(tile / n_tiles) * kGemmBM, n0 = (int)(tile % n_tiles) * kGemmBN;
+      float acc[kAcc], frag[kAcc];
 #pragma unroll
-            for (int u = 0; u < 4; ++u)
-              if (col + u < p.N) ccol[(int64_t)(j + u) * cstride] = v[u];
-          } else if (vec_ok && col + 4 <= p.N) {
-            *reinterpret_cast<float4*>(crow + col) = make_float4(v0, v1, v2, v3);
-          } else {
-            const float v[4] = {v0, v1, v2, v3};
+      for (int j = 0; j < kAcc; ++j) acc[j] = 0.0f;
+      bool pending = false;  // block g - 1 may still be in flight
+      for (int i = 0; i < num_kb; ++i, ++g) {
+        const int sr = g % kPersRawStages, sl = g % kPersLoStages, sb = g % kPersBStages;
+        const int in_chunk = i % kPersChunk;
+        bar_wait(&conv_a[sl], (g / kPersLoStages) & 1);
+        bar_wait(&full_b[sb], (g / kPersBStages) & 1);
+        const uint32_t stb = s32(b_base + (size_t)sb * kPersBStageBytes);
+        mma_kblock(frag, make_sw128_desc(s32(raw_base + (size_t)sr * kTileABytes) + wg * kHalfABytes),
+                   make_sw128_desc(s32(lo_base + (size_t)sl * kTileABytes) + wg * kHalfABytes), make_sw128_desc(stb),
+                   make_sw128_desc(stb + kTileBBytes), in_chunk == 0);
+        if (in_chunk == kPersChunk - 1 || i == num_kb - 1) {  // chunk complete: fold it
+          wgmma_wait<0>();
+          fence_acc(frag);
+          if (pending) release(g - 1);
+          release(g);
+          pending = false;
 #pragma unroll
-            for (int u = 0; u < 4; ++u)
-              if (col + u < p.N) crow[col + u] = v[u];
-          }
-        };
-        if (p.row_act == EVOK_ACT_NONE) {
-#pragma unroll
-          for (int j = 0; j < kGemmBN / 2; j += 4) store4(j, acc[j] + b, acc[j + 1] + b, acc[j + 2] + b, acc[j + 3] + b);
-        } else if (p.row_act == EVOK_ACT_RELU) {
-#pragma unroll
-          for (int j = 0; j < kGemmBN / 2; j += 4)
-            store4(j, fmaxf(acc[j] + b, 0.0f), fmaxf(acc[j + 1] + b, 0.0f), fmaxf(acc[j + 2] + b, 0.0f), fmaxf(acc[j + 3] + b, 0.0f));
-        } else if (p.row_act == EVOK_ACT_TANH) {
-#pragma unroll
-          for (int j = 0; j < kGemmBN / 2; j += 4)
-            store4(j, tanh_abs1e7(acc[j] + b), tanh_abs1e7(acc[j + 1] + b), tanh_abs1e7(acc[j + 2] + b), tanh_abs1e7(acc[j + 3] + b));
+          for (int j = 0; j < kAcc; ++j) acc[j] += frag[j];
         } else {
-#pragma unroll
-          for (int j = 0; j < kGemmBN / 2; j += 4)
-            store4(j, activate_fast(acc[j] + b, EVOK_ACT_SIGMOID), activate_fast(acc[j + 1] + b, EVOK_ACT_SIGMOID),
-                   activate_fast(acc[j + 2] + b, EVOK_ACT_SIGMOID), activate_fast(acc[j + 3] + b, EVOK_ACT_SIGMOID));
+          wgmma_wait<1>();
+          if (pending) release(g - 1);
+          pending = true;
         }
+      }
+      wgmma_wait<0>();  // (as in gemm_tf32x3_kernel: already true, stated for the compiler)
+      switch (p.row_act) {
+        case EVOK_ACT_RELU: pers_store<EVOK_ACT_RELU>(p, acc, m0, r_first, n0, c, vec_ok); break;
+        case EVOK_ACT_TANH: pers_store<EVOK_ACT_TANH>(p, acc, m0, r_first, n0, c, vec_ok); break;
+        case EVOK_ACT_SIGMOID: pers_store<EVOK_ACT_SIGMOID>(p, acc, m0, r_first, n0, c, vec_ok); break;
+        default: pers_store<EVOK_ACT_NONE>(p, acc, m0, r_first, n0, c, vec_ok); break;
       }
     }
-  }
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 2 * kGemmBN);
   }
 }
 
@@ -1030,8 +873,8 @@ static int gemm_impl(const float* A, int64_t lda, const float* B, int64_t ldb, i
   }();
   const bool convert = allow_convert && tma_ok(A, lda) && tma_ok(B, ldb);
   static const int allow_b_lo = [] {
-    // =1: B's lo tile by TMA from a pre-split copy instead of the converter warps.  Measured: 8192^3 4.94 vs 5.05 ms, but 52 vs 44 us at
-    // the CMA-ES sizes (the extra pre-pass launch), and the K loop is bound by the 2-stage load latency either way -- off by default
+    // =1: B's lo tile by TMA from a pre-split copy instead of the converter warps: half the conversion work, but one more pre-pass
+    // launch, which small (CMA-ES-sized) products feel -- off by default
     const char* e = getenv("EVOK_GEMM_B_LO_TMA");
     return e ? atoi(e) : 0;
   }();
@@ -1081,15 +924,7 @@ static int gemm_impl(const float* A, int64_t lda, const float* B, int64_t ldb, i
   p.ga_rows_per_batch = p.ga_batch_stride = p.ga_row_stride = p.rb_batch_stride = 0;
   p.row_bias = nullptr;
   p.row_act = 0;
-  p.debug = 0;
   p.b_lo_tma = b_lo_tma ? 1 : 0;
-  p.trace = nullptr;
-#ifdef EVOK_GEMM_TRACE
-  {
-    const char* e = getenv("EVOK_GATHER_TRACE_PTR");
-    p.trace = e ? reinterpret_cast<long long*>(strtoull(e, nullptr, 16)) : nullptr;
-  }
-#endif
   static bool attr_set = false;
   if (!attr_set) {
     if (cudaFuncSetAttribute(gemm_tf32x3_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kGemmSmemBytes) != cudaSuccess ||
@@ -1149,10 +984,6 @@ extern "C" EVOK_API int evok_gemm_gather_rows(const float* params, int64_t batch
   p.row_bias = bias_offset >= 0 ? params + bias_offset : nullptr;
   p.rb_batch_stride = batch_stride;
   p.row_act = act;
-  {
-    const char* e = getenv("EVOK_GATHER_DEBUG");
-    p.debug = e ? atoi(e) : 0;
-  }
   static bool attr_set = false;
   if (!attr_set) {
     if (cudaFuncSetAttribute(gemm_tf32x3_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kGemmSmemBytes) != cudaSuccess)
@@ -1172,7 +1003,7 @@ extern "C" EVOK_API size_t evok_gemm_gather_rows_workspace_bytes(int64_t n_cols,
 
 // The same product on the persistent kernel (gemm_gather_persistent_kernel): X is split into hi / lo copies in `ws` first (any
 // alignment / pitch of X is fine).  unit_fastest = 1 writes C[(batch * n_cols + col) * rows_per_batch + row] instead of the row-major
-// C[(batch * rows_per_batch + row) * ldc + col]: one cache line per store instruction of the epilogue instead of 32.
+// C[(batch * rows_per_batch + row) * ldc + col]: the rows a warp stores per instruction are consecutive floats.
 // EVOK_GATHER_PERSISTENT=0 routes the row-major case to the one-tile-per-CTA kernel instead (measurement only).
 extern "C" EVOK_API int evok_gemm_gather_rows_ws(const float* params, int64_t batch_stride, int64_t w_offset, int64_t rows_per_batch,
                                                  int64_t n_batches, const float* X, int64_t ldx, int64_t n_cols, int64_t K, int64_t bias_offset,
@@ -1213,21 +1044,11 @@ extern "C" EVOK_API int evok_gemm_gather_rows_ws(const float* params, int64_t ba
   p.rb_batch_stride = batch_stride;
   p.row_act = act;
   p.c_unit_fastest = unit_fastest ? 1 : 0;
-  {
-    const char* e = getenv("EVOK_GATHER_DEBUG");
-    p.debug = e ? atoi(e) : 0;
-  }
-#ifdef EVOK_GEMM_TRACE
-  {
-    const char* e = getenv("EVOK_GATHER_TRACE_PTR");  // device pointer (hex) of a 512 x 16 int64 buffer
-    p.trace = e ? reinterpret_cast<long long*>(strtoull(e, nullptr, 16)) : nullptr;
-  }
-#endif
   static int sm_count = 0;
   if (!sm_count) {
     int dev = 0;
     cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sm_count <= 0) sm_count = 148;
+    if (cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sm_count <= 0) sm_count = kNumSMs;
     if (cudaFuncSetAttribute(gemm_gather_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPersSmemBytes) != cudaSuccess) {
       sm_count = 0;
       return (int)cudaGetLastError();

@@ -25,7 +25,7 @@ namespace evok {
 #endif
 constexpr int kGradThreads = 256;
 constexpr int kGradUnroll = EVOK_GRAD_UNROLL;
-constexpr int kMaxResidentCtas = 148 * 8;
+constexpr int kMaxResidentCtas = kNumSMs * 8;
 
 template <int VEC>
 struct VecF;

@@ -251,7 +251,7 @@ constexpr int kTail2MaxOut = 32;
 
 // The hidden tile of 64 samples (h1 x 64 floats) is brought into shared memory with 16-byte cp.async copies, all of them issued up
 // front in four commit groups (streaming the rows from inside the accumulation loop, or filling the tile with plain loads, was
-// latency-bound: 35 ms of a 74 ms forward); each thread applies act_0 in place to the pieces it copied as its group lands, and the
+// latency-bound); each thread applies act_0 in place to the pieces it copied as its group lands, and the
 // accumulation over a quarter of the hidden units starts while the other quarters are still in flight.  Thread = (sample pair,
 // output group): per hidden unit two activation reads and one or two 16-byte broadcast weight reads serve 2 x OG FMAs.  96 KB of
 // shared memory per CTA: two CTAs per SM cover each other's fill latency.

@@ -309,8 +309,7 @@ __global__ void __launch_bounds__(256) elite_mask_kernel(const uint32_t* __restr
 }
 
 // ---- small populations: rank by counting, ONE launch -------------------------------------------------
-// For N <= kSmallRankMax the 14-launch radix pipeline is pure launch latency (about 60 us inside a CUDA graph, more in eager
-// mode), while the stable rank of element i is simply  #{j : key_j < key_i} + #{j < i : key_j == key_i}.  All N^2 comparisons
+// For N <= kSmallRankMax the 14-launch radix pipeline is pure launch latency (even inside a CUDA graph), while the stable rank of element i is simply  #{j : key_j < key_i} + #{j < i : key_j == key_i}.  All N^2 comparisons
 // (67 M at N = 8192) spread over the whole GPU take a few microseconds: 4 lanes share one element (interleaved quarters of
 // the key tile staged in shared memory: conflict-free, broadcast reads; 8 or 16 lanes for larger N, so that the grid always
 // covers the GPU), 256 / lanes elements per CTA.  The utility (or the elite flag,

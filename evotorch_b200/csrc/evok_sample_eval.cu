@@ -18,7 +18,7 @@ static int sm_count() {
   return g_sm_count;
 }
 
-// tunables (profiles/ records the sweep that chose the defaults)
+// tunables (build-time, for measurement builds: scripts/build_variants.py, scripts/kbench.py)
 #ifndef EVOK_SAMPLE_THREADS
 #define EVOK_SAMPLE_THREADS 256
 #endif
@@ -36,7 +36,7 @@ static int sm_count() {
 #endif
 constexpr int kSampleThreads = EVOK_SAMPLE_THREADS;
 // the fused kernels are issue/XU bound (two independent Philox chains per lane help); the sample-only kernel is store
-// bound and prefers occupancy (kbench sweep in profiles/)
+// bound and prefers occupancy
 template <int OBJ>
 struct SampleTune {
   static constexpr int kUnroll = OBJ == EVOK_OBJ_NONE ? EVOK_SAMPLEONLY_UNR : EVOK_SAMPLE_UNR;

@@ -169,7 +169,7 @@ def sharded_sample_and_gradients(problem, distribution, popsize: int, *, obj_ind
     method = "raw" if ranking_method is None else ranking_method
     # sharded ranking: sort locally, exchange sorted keys, rank the local rows against the world (no GPU holds all fitnesses)
     sharded_rank = (peer is not None and method in ("centered", "linear", "nes") and dev_dist.accepts_local_weights(method)
-                    and os.environ.get("EVOTORCH_B200_SHARDED_RANK", "0") == "1")  # opt-in: measured equal to the replicated sort at 8 GPUs
+                    and os.environ.get("EVOTORCH_B200_SHARDED_RANK", "0") == "1")  # opt-in; the replicated sort is the default
     # the fitness all-gather: either stores from inside the sampler (EVOTORCH_B200_PUSH_IN_SAMPLER=1, the round-1 protocol) or, by
     # default, the plain sampler followed by one 8-CTA push kernel (coalesced 16-byte stores, one system fence per peer)
     push_in_sampler = peer is not None and not sharded_rank and os.environ.get("EVOTORCH_B200_PUSH_IN_SAMPLER", "0") == "1"

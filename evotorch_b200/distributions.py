@@ -437,7 +437,7 @@ class ExpGaussian(Distribution):
         return self.sigma.transpose(0, 1) @ self.sigma
 
     def to_global_coordinates(self, local_coordinates: torch.Tensor) -> torch.Tensor:
-        """mu + z A^T (distributions.py:928-938); the tcgen05 GEMM with the `+ mu` epilogue on CUDA fp32."""
+        """mu + z A^T (distributions.py:928-938); the tensor-core GEMM with the `+ mu` epilogue on CUDA fp32."""
         if ops.uses_kernels(local_coordinates) and ops.uses_kernels(self.A) and local_coordinates.ndim == 2:
             z = local_coordinates.contiguous()
             out = torch.empty_like(z)

@@ -169,7 +169,7 @@ class NEProblem(BaseNEProblem):
         """Row i of `parameters` (N x L) applied to the SHARED input batch `x` (B x ...) -> N x B x out.
         This is the one place where the policy forward of a population is a dense contraction: for a feed-forward net the first
         layer of all N networks is ONE product (N*H x in) * (in x B) of the stacked weight rows with the shared batch; on CUDA
-        float32 it runs on the tcgen05 GEMM kernel with the weights read once (`Policy.forward_shared`)."""
+        float32 it runs on the tensor-core GEMM kernel with the weights read once (`Policy.forward_shared`)."""
         return self.policy.forward_shared(parameters, x)
 
     def to_policy(self, solution) -> nn.Module:

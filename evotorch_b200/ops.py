@@ -1,4 +1,4 @@
-"""Tensor-level entry points of the sm_100a kernels (CUDA, fp32 only).
+"""Tensor-level entry points of the sm_90a kernels (CUDA, fp32 only).
 
 Each function validates its tensors, pulls raw pointers + the current stream and calls the C ABI of
 libevok.so (include/evok.h).  Callers in this package decide *whether* a tensor goes to these kernels

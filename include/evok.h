@@ -1,5 +1,5 @@
 /*
- * evok.h -- C ABI of libevok.so: the sm_100a kernels behind the per-generation hot path of
+ * evok.h -- C ABI of libevok.so: the sm_90a kernels behind the per-generation hot path of
  * EvoTorch's distribution-based searchers (PGPE / SNES / CEM / XNES / CMA-ES).
  *
  * The reference (nnaisense/evotorch @ cebcac4f) has no FFI: its "plugin interface" on this path is a
@@ -216,7 +216,7 @@ size_t evok_mlp_forward_shared_workspace_bytes(int64_t N, int64_t B, int n_layer
 int evok_mlp_forward_shared(const float* params, int64_t ldp, int64_t N, const float* X, int64_t ldx, int64_t B, int n_layers,
                             const int32_t* dims_host, const int32_t* acts_host, float* out, void* ws, size_t ws_bytes, void* stream);
 /* C[(i, h), b] = act(sum_k W_i[h, k] X[b, k] + bias_i[h]),  W_i = params + i * batch_stride + w_offset (rows_per_batch x K, row-major),
- * bias_i = params + i * batch_stride + bias_offset (bias_offset < 0: none).  3xTF32 on tcgen05, fp32 accuracy. */
+ * bias_i = params + i * batch_stride + bias_offset (bias_offset < 0: none).  3xTF32 on wgmma, fp32 accuracy. */
 int evok_gemm_gather_rows(const float* params, int64_t batch_stride, int64_t w_offset, int64_t rows_per_batch, int64_t n_batches, const float* X,
                           int64_t ldx, int64_t n_cols, int64_t K, int64_t bias_offset, int act, float* C, int64_t ldc, void* stream);
 /* The same product on the PERSISTENT kernel (one CTA per SM walks the tiles; X pre-split into hi / lo copies in `ws`, so X may have any
@@ -228,7 +228,7 @@ int evok_gemm_gather_rows_ws(const float* params, int64_t batch_stride, int64_t 
                              size_t ws_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
- * K6 / K7: fp32-accurate tensor-core GEMM (tcgen05 + TMEM + TMA, 3xTF32 operand splitting).
+ * K6 / K7: fp32-accurate tensor-core GEMM (wgmma + TMA, 3xTF32 operand splitting).
  *   C[M x N] = A[M x K] * B[N x K]^T        A, B, C row-major fp32 (lda, ldb >= K; ldc >= N)
  *   optional C2[M x N] = alpha_dev[0] * (A B^T) + bias[col]    (C2 / alpha_dev / bias nullable)
  * Replaces the dense contractions of CMA-ES: `ys = (A @ zs.T).T`, `xs = m + sigma * ys` (cmaes.py:427-429; call with

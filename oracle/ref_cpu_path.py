@@ -3,7 +3,7 @@ INFRASTRUCTURE ONLY (see oracle/es_oracle.py for the rules: never imported by th
 
 Why this exists next to the numpy oracle: the reference IS a sequence of multi-threaded torch ops; timing a numpy port would
 understate its speed.  `bench.py --impl reference` and the `cpu_baseline` leg therefore time THIS restatement with all host
-threads (`kind: "port"`).  It is validated against the real reference in the build container (bit-identical trajectories,
+threads (`kind: "port"`).  It is validated against the real reference's recorded runs in tests/golden (bit-identical trajectories,
 tests/test_ref_cpu_port.py) and against the golden trajectories everywhere.
 
 Op sequence per generation (gaussian.py:351-367 of the reference):
@@ -35,7 +35,7 @@ class PGPEReferencePath:
                  seed: int, stdev_max_change: Optional[float] = 0.2, momentum: float = 0.9, sense: str = "min",
                  center_init: Optional[torch.Tensor] = None, objective=rastrigin, device: str = "cpu"):
         # `device="cuda"` runs the very same torch op sequence on a GPU (the reference is device-agnostic): the "PyTorch eager
-        # on the same B200" comparator of SURVEY 8(d).  The CPU trajectory is what the golden tests pin.
+        # on the same GPU" comparator of SURVEY 8(d).  The CPU trajectory is what the golden tests pin.
         self.n, self.d = int(popsize), int(solution_length)
         self.device = torch.device(device)
         self.gen = torch.Generator(device=self.device).manual_seed(int(seed))

@@ -1,4 +1,4 @@
-"""BASELINE config 1 shape (the reference README's SNES: popsize 1000, dim 100, Rastrigin) on one B200: generations/s with
+"""BASELINE config 1 shape (the reference README's SNES: popsize 1000, dim 100, Rastrigin) on one GPU: generations/s with
 eager stepping and with CUDA-graph replay."""
 import json
 import sys

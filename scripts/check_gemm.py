@@ -1,4 +1,4 @@
-"""GPU check of the tcgen05 3xTF32 GEMM against float64 (run on the B200 box)."""
+"""GPU check of the wgmma 3xTF32 GEMM against float64."""
 import os, sys, time
 import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -1,4 +1,4 @@
-"""K6 throughput: ops.gemm_nt at CMA-ES and square sizes (3xTF32 on tcgen05), torch fp32 matmul (no TF32) beside it."""
+"""K6 throughput: ops.gemm_nt at CMA-ES and square sizes (3xTF32 on wgmma), torch fp32 matmul (no TF32) beside it."""
 import json
 import sys
 

@@ -1,5 +1,5 @@
-"""Parity of the sm_100a kernels (called through the C ABI of libevok.so via evotorch_b200.ops) against the numpy oracle
-and the golden vectors produced by the real reference.  Needs a CUDA device: run with `-m gpu` on the B200 box."""
+"""Parity of the sm_90a kernels (called through the C ABI of libevok.so via evotorch_b200.ops) against the numpy oracle
+and the golden vectors produced by the real reference.  Needs a CUDA device (H100): run with `-m gpu`."""
 
 import os
 import math
@@ -507,7 +507,7 @@ def test_user_objective_and_torch_rng_paths_on_cuda():
 
 
 @pytest.mark.parametrize("M,N,K", [(128, 256, 32), (4096, 1024, 1024), (1024, 1024, 4096), (100, 70, 36), (129, 257, 40), (12, 6, 6), (300, 513, 1000)])
-def test_tcgen05_gemm_matches_float64(M, N, K):
+def test_tensor_core_gemm_matches_float64(M, N, K):
     g = torch.Generator(device=DEV).manual_seed(M + N + K)
     A = torch.randn(M, K, device=DEV, generator=g)
     B = torch.randn(N, K, device=DEV, generator=g)
@@ -672,7 +672,7 @@ def test_config2_size_properties():
 
 
 def test_metric_size_properties():
-    """BASELINE metric size: PGPE, popsize 1 000 000 x dim 10 000 (40 GB population on one B200) -- size-independent properties."""
+    """BASELINE metric size: PGPE, popsize 1 000 000 x dim 10 000 (40 GB population on one 80 GB H100) -- size-independent properties."""
     free, _total = torch.cuda.mem_get_info()
     if free < 60e9:
         pytest.skip("needs 60 GB of free device memory")
@@ -791,7 +791,7 @@ def single_rank_group(tmp_path):
 def test_peer_exchange_kernels_single_rank(single_rank_group):
     """World size 1 runs the very same kernels as the multi-GPU exchange (push stores + flag raise, flag wait, slot
     reduction); the results must equal the plain kernels bit for bit, generation after generation, also from a CUDA graph.
-    (2- and 8-GPU parity: scripts/check_peer_exchange.py, profiles/r01_peer_exchange_*.txt.)"""
+    (2- and 8-GPU parity: scripts/check_peer_exchange.py.)"""
     from evotorch_b200.peer import PeerExchange
 
     n, d = 4096, 515

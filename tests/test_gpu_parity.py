@@ -1,4 +1,4 @@
-"""Parity tests at the sizes and modes the hot path actually runs in (GPU box, `-m gpu`).
+"""Parity tests at the sizes and modes the hot path actually runs in (on the GPU, `-m gpu`).
 
   * same-seed contract: `Problem(device="cuda", rng="torch", seed=S)` + PGPE beside the reference's torch op sequence
     (`oracle/ref_cpu_path.PGPEReferencePath(device="cuda", seed=S)`, bit-identical to the live reference on CPU,

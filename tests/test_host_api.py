@@ -474,8 +474,7 @@ def test_searcher_option_variants_match_reference(tag):
 
 def test_decorators_and_device_aware_evaluation():
     """decorators.py:170-960: vectorized / rowwise / expects_ndim / on_device / on_cuda / on_aux_device markers and how `Problem`
-    honours them (core.py:2502-2585).  (The reference's own tests/test_decorators.py, test_expects_ndim.py and test_func_alg.py pass
-    against this package through scripts/run_reference_tests.py.)"""
+    honours them (core.py:2502-2585)."""
     from evotorch_b200.decorators import expects_ndim, on_aux_device, on_cuda, on_device, pass_info, rowwise, vectorized
 
     @rowwise

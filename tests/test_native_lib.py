@@ -1,4 +1,4 @@
-"""The C-ABI library builds for sm_100a without a GPU, loads, and exports every symbol include/evok.h declares."""
+"""The C-ABI library builds for sm_90a without a GPU, loads, and exports every symbol include/evok.h declares."""
 
 import ctypes
 import os
@@ -45,7 +45,7 @@ def test_host_side_argument_checks_need_no_gpu(libpath):
     assert lib.evok_clipup_step(None, 4, None, 0.1, 0.9, 0.2, None, None, None) == -1
 
 
-def test_kernels_are_sm100a_sass(libpath):
+def test_kernels_are_sm90a_sass(libpath):
     import shutil
     import subprocess
 
@@ -53,4 +53,4 @@ def test_kernels_are_sm100a_sass(libpath):
     if not os.path.exists(cuobjdump):
         pytest.skip("cuobjdump not available")
     out = subprocess.run([cuobjdump, "-lelf", libpath], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out

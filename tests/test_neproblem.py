@@ -1,6 +1,6 @@
 """NEProblem / SupervisedNE against golden fitnesses produced by the REAL reference's one-solution-at-a-time loop
 (tests/golden/gen_ne_golden.py; neproblem.py:407-429, supervisedne.py:327-347), through the batched route of this package;
-CPU here, CUDA (kernel path: K8 / tcgen05 GEMM) when a GPU is present."""
+CPU here, CUDA (kernel path: K8 / tensor-core GEMM) when a GPU is present."""
 
 import os
 

@@ -1,14 +1,9 @@
-"""oracle/ref_cpu_path.py (the torch-CPU restatement timed as the CPU baseline) against the real reference: golden
-trajectories everywhere, and a live side-by-side run where /root/reference is mounted (the build container)."""
+"""oracle/ref_cpu_path.py (the torch-CPU restatement timed as the CPU baseline) against the real reference's recorded
+trajectories (tests/golden)."""
 
 import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
-import torch
-
 from oracle.ref_cpu_path import PGPEReferencePath
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -24,26 +19,15 @@ def test_port_reproduces_golden_trajectory(golden, tag, sense):
         np.testing.assert_allclose(p.X.numpy(), golden[f"traj/{tag}/X"][t], rtol=1e-6, atol=2e-6)
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/src/evotorch"), reason="the reference is only mounted in the build container")
-def test_port_is_bit_identical_to_the_live_reference():
-    code = r"""
-import sys, numpy as np, torch
-sys.path.insert(0, %r)
-import evotorch
-from evotorch import Problem
-from evotorch.algorithms import PGPE
-from oracle.ref_cpu_path import PGPEReferencePath, rastrigin
-prob = Problem("min", rastrigin, initial_bounds=(-5.12, 5.12), solution_length=300, vectorized=True, seed=5, dtype=torch.float32)
-s = PGPE(prob, popsize=200, center_learning_rate=0.5, stdev_learning_rate=0.1, stdev_init=1.0)
-p = PGPEReferencePath(300, 200, center_learning_rate=0.5, stdev_learning_rate=0.1, stdev_init=1.0, seed=5)
-for t in range(8):
-    s.step(); p.step()
-    assert torch.equal(s.status["center"], p.mu), t
-    assert torch.equal(s.status["stdev"], p.sigma), t
-    assert torch.equal(s.population.values, p.X), t
-print("IDENTICAL")
-""" % ROOT
-    env = dict(os.environ, PYTHONPATH=os.pathsep.join([os.path.join(ROOT, "tests", "golden", "_refstubs"), "/root/reference/src"]),
-               EVOTORCH_VERBOSE_LEVEL="0")
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=env, timeout=300)
-    assert "IDENTICAL" in r.stdout, r.stdout + r.stderr
+def test_port_is_bit_identical_to_the_reference():
+    """The reference's own PGPE run (tests/golden/gen_ref_cpu_port_golden.py), generation by generation, bit for bit."""
+    with np.load(os.path.join(ROOT, "tests", "golden", "ref_cpu_port_golden.npz")) as z:
+        ref = {k: z[k] for k in z.files}
+    p = PGPEReferencePath(300, 200, center_learning_rate=0.5, stdev_learning_rate=0.1, stdev_init=1.0, seed=5)
+    for t in range(len(ref["mu"])):
+        p.step()
+        assert np.array_equal(p.mu.numpy(), ref["mu"][t]), t
+        assert np.array_equal(p.sigma.numpy(), ref["sigma"][t]), t
+        if t == 0:
+            assert np.array_equal(p.X.numpy(), ref["X_first"])
+    assert np.array_equal(p.X.numpy(), ref["X_last"])
