@@ -48,6 +48,8 @@ _SIGNATURES = {
     "evok_grad": (c_int, [c_int, _P, c_int64, _P, _P, _P, c_int64, c_int64, c_float, c_float, _P, _P, _P, c_size_t, _P]),
     "evok_grad_regen": (c_int, [c_int, _P, _P, _P, c_int64, c_int64, c_int64, c_uint64, c_uint64, _P, c_float, c_float, _P, _P, _P,
                                 c_size_t, _P]),
+    "evok_grad_hybrid": (c_int, [c_int, _P, c_int64, _P, _P, _P, c_int64, c_int64, c_int64, c_uint64, c_uint64, _P, c_int, c_float, c_float, _P,
+                                 _P, _P, c_size_t, _P]),
     "evok_clipup_step": (c_int, [_P, c_int64, _P, c_float, c_float, c_float, _P, _P, _P]),
     "evok_adam_step": (c_int, [_P, c_int64, _P, _P, c_int64, c_float, c_float, c_float, c_float, _P, _P, _P]),
     "evok_sgd_step": (c_int, [_P, c_int64, _P, c_int, c_float, c_float, _P, _P, _P]),

@@ -20,7 +20,7 @@ from typing import Optional
 import torch
 
 from .. import ops
-from ..core import LazySolutionBatch, PhiloxRecipe, Problem, SolutionBatch
+from ..core import LazySolutionBatch, PhiloxRecipe, PhiloxSamples, Problem, SolutionBatch
 from ..distributed import world
 from ..distributions import Distribution, ExpGaussian, ExpSeparableGaussian, SeparableGaussian, SymmetricSeparableGaussian
 from ..optimizers import get_optimizer_class
@@ -183,20 +183,18 @@ class GaussianSearchAlgorithm(SearchAlgorithm, SinglePopulationAlgorithmMixin):
         lazy = isinstance(pop, LazySolutionBatch)
         n = len(pop)
         fitnesses = pop._evdata.view(-1)
-        if lazy:
-            # the population consumed here was drawn one stream id earlier (by the eager step before the capture, or by the previous replay)
-            samples = PhiloxRecipe(seed=prob._philox_seed, stream_id=base_stream - 1, row0=0, n_rows=n, solution_length=prob.solution_length,
-                                   symmetric=dist.SYMMETRIC, stream_offset=counter, mu=dist.mu, sigma=dist.sigma)
-        else:
-            samples = pop._data
+        # the population consumed here was drawn one stream id earlier (by the eager step before the capture, or by the previous
+        # replay); a materialised one is rebuilt in part from the same counters (`_step_graph` drops the graph if it was modified)
+        recipe = PhiloxRecipe(seed=prob._philox_seed, stream_id=base_stream - 1, row0=0, n_rows=n, solution_length=prob.solution_length,
+                              symmetric=dist.SYMMETRIC, stream_offset=counter, mu=dist.mu, sigma=dist.sigma)
+        samples = recipe if lazy else PhiloxSamples(pop._data, recipe)
         gradients = dist.compute_gradients(samples, fitnesses, objective_sense=prob.senses[self._obj_index], ranking_method=self._ranking_method)
         self._update_in_place(gradients)
-        ops.sample_eval(prob.evok_objective_id, None if lazy else samples, dist.mu, dist.sigma, n_rows=n, symmetric=dist.SYMMETRIC,
+        ops.sample_eval(prob.evok_objective_id, None if lazy else pop._data, dist.mu, dist.sigma, n_rows=n, symmetric=dist.SYMMETRIC,
                         seed=prob._philox_seed, stream_id=base_stream, f=fitnesses, stream_offset=counter)
         counter.add_(1)
         if lazy:
-            pop.recipe = PhiloxRecipe(seed=prob._philox_seed, stream_id=base_stream - 1, row0=0, n_rows=n, solution_length=prob.solution_length,
-                                      symmetric=dist.SYMMETRIC, stream_offset=counter, mu=dist.mu, sigma=dist.sigma)
+            pop.recipe = recipe
 
     def _capture_graph(self):
         prob = self.problem
@@ -217,9 +215,19 @@ class GaussianSearchAlgorithm(SearchAlgorithm, SinglePopulationAlgorithmMixin):
         ops.count_replayed_launches(-self._graph_kernels)  # the capture itself executed nothing
         self._graph_counter.zero_()
         self._graph = graph
+        pop = self._population
+        # replays resample the population without passing through Python: the eager record goes stale with the first one
+        pop._philox_record = None
+        self._graph_values_version = None if isinstance(pop, LazySolutionBatch) else pop._data._version
 
     def _step_graph(self):
         prob, pop = self.problem, self._population
+        if self._graph is not None and self._graph_values_version is not None and pop._data._version != self._graph_values_version:
+            # the population was modified in place since the last replay: the graph would rebuild rows from their Philox
+            # counters, so this generation runs eagerly (reading the modified rows) and the next one captures a new graph
+            self._graph = None
+            self._step_eager()
+            return
         if self._graph is None:
             # one more eager generation right before the capture: warms every kernel and workspace that the graph will use
             self._step_eager()
@@ -244,7 +252,8 @@ class GaussianSearchAlgorithm(SearchAlgorithm, SinglePopulationAlgorithmMixin):
 
     def _step_eager(self):
         lazy = isinstance(self._population, LazySolutionBatch)
-        samples = self._population.recipe if lazy else self._population.access_values(keep_evals=True)
+        dist = self._distribution
+        samples = self._population.recipe if lazy else self._population.gradient_samples(dist.mu, dist.sigma)
         fitnesses = self._population.access_evals()[:, self._obj_index]
         gradients = self._distribution.compute_gradients(samples, fitnesses, objective_sense=self.problem.senses[self._obj_index],
                                                          ranking_method=self._ranking_method)

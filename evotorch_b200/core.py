@@ -554,6 +554,7 @@ class Problem(Clonable):
                                 row0=self.philox_row0, f=batch._evdata.view(-1), stream_offset=self.philox_stream_offset)
             self._finish_evaluation(batch)
             return
+        batch._philox_record = None  # only the fused sampler below leaves a record that the gradient pass may rebuild rows from
         values = batch.access_values()
         # before-eval hooks must see (and may edit) the freshly sampled values before they are evaluated (core.py:2559 of the
         # reference: the hook is called inside evaluate(), after distribution.sample): with hooks registered the sampling and the
@@ -578,9 +579,12 @@ class Problem(Clonable):
                                  stream_offset=self.philox_stream_offset)
             self._finish_evaluation(batch)
             return
-        ops.sample_eval(obj, values, distribution.mu.contiguous(), distribution.sigma.contiguous(), n_rows=n,
-                        symmetric=distribution.SYMMETRIC, seed=seed, stream_id=stream_id, row0=self.philox_row0, f=f,
-                        stream_offset=self.philox_stream_offset)
+        mu, sigma = distribution.mu.contiguous(), distribution.sigma.contiguous()
+        ops.sample_eval(obj, values, mu, sigma, n_rows=n, symmetric=distribution.SYMMETRIC, seed=seed, stream_id=stream_id,
+                        row0=self.philox_row0, f=f, stream_offset=self.philox_stream_offset)
+        recipe = PhiloxRecipe(seed=seed, stream_id=stream_id, row0=self.philox_row0, n_rows=n, solution_length=self._solution_length,
+                              symmetric=distribution.SYMMETRIC, stream_offset=self.philox_stream_offset, mu=mu, sigma=sigma)
+        batch._philox_record = (PhiloxSamples(values, recipe), values._version, mu._version, sigma._version)
         if not direct:
             batch.set_evals(f)
         self._finish_evaluation(batch)
@@ -743,6 +747,26 @@ class SolutionBatch:
         """Mutable view of the decision values; evaluations are forgotten (NaN) unless `keep_evals` (core.py:4166-4195)."""
         if not keep_evals:
             self.forget_evals()
+        return self._data
+
+    def gradient_samples(self, mu: torch.Tensor, sigma: torch.Tensor) -> Union[torch.Tensor, "PhiloxSamples"]:
+        """The decision values as the input of a gradient pass over the distribution (`mu`, `sigma`).
+
+        While the values are still exactly what the fused sampler of `Problem.sample_and_evaluate` wrote from these very `mu`
+        and `sigma` tensors, this returns a `PhiloxSamples`: the values plus the Philox recipe that produced them, from which
+        the gradient kernel rebuilds part of the rows instead of reading them back.  Otherwise it returns the mutable values
+        tensor, as `access_values(keep_evals=True)` does.  The record is dropped when torch bumps the version counter of the
+        values (in-place ops on `access_values()`, `set_values`), when `mu` or `sigma` is another tensor than the sampler used
+        or was modified in place, and when the batch was sampled otherwise; batches made by slicing or concatenation carry
+        none.  Writes that bypass torch (a kernel writing through a raw pointer) are NOT detected: after such a write, pass
+        `access_values(keep_evals=True)` to the gradient computation instead."""
+        record = self.__dict__.get("_philox_record")
+        if record is not None:
+            samples, v_values, v_mu, v_sigma = record
+            r = samples.recipe
+            if (samples.values is self._data and self._data._version == v_values and r.mu is mu and r.sigma is sigma
+                    and mu._version == v_mu and sigma._version == v_sigma):
+                return samples
         return self._data
 
     def access_evals(self, obj_index: Optional[int] = None) -> torch.Tensor:
@@ -910,6 +934,18 @@ class PhiloxRecipe:
         ops.sample_eval(ops.OBJ_NONE, out, self.mu, self.sigma, n_rows=self.n_rows, symmetric=self.symmetric, seed=self.seed,
                         stream_id=self.stream_id, row0=self.row0, stream_offset=self.stream_offset)
         return out
+
+
+class PhiloxSamples:
+    """A materialised population together with the PhiloxRecipe that sampled it (see `SolutionBatch.gradient_samples`): the
+    gradient kernel reads part of the rows from `values` and rebuilds the rest, bit for bit, from `recipe`."""
+
+    def __init__(self, values: torch.Tensor, recipe: PhiloxRecipe):
+        self.values, self.recipe = values, recipe
+
+    @property
+    def shape(self) -> torch.Size:
+        return self.values.shape
 
 
 class LazySolutionBatch(SolutionBatch):

@@ -257,6 +257,9 @@ static int launch_finalize(const float* partial, int n_chunks, int64_t D, float 
 #ifndef EVOK_GRAD_TMA_CTAS_PER_SM
 #define EVOK_GRAD_TMA_CTAS_PER_SM 3
 #endif
+#ifndef EVOK_GRAD_AUTO_SPLIT
+#define EVOK_GRAD_AUTO_SPLIT 2
+#endif
 constexpr int kTmaRows = EVOK_GRAD_TMA_ROWS;
 constexpr int kTmaStages = EVOK_GRAD_TMA_STAGES;
 constexpr int kTmaCols = 1024;
@@ -291,11 +294,22 @@ __device__ __forceinline__ void bulk_load(void* dst_smem, const void* src_gmem, 
                : "memory");
 }
 
+// Hybrid schedule: streaming leaves the SMs' issue slots nearly idle, so part of the row groups (kTmaRows rows each) are
+// rebuilt on the SMs from the Philox counters that produced them instead of being streamed (see kAutoSplit for how much).  `split` of every kSplitPeriod
+// consecutive groups of a chunk are rebuilt, spread evenly over the period (the same mix in every CTA); split 0 streams every
+// group, kSplitPeriod rebuilds every group.  A rebuilt row is bit-identical to the stored one (same normals4 call, same
+// fmaf(sigma, z, mu) as sample_group) and the accumulation order does not depend on the schedule, so neither does the result.
+constexpr int kSplitPeriod = 16;
+__device__ __forceinline__ bool group_rebuilt(int64_t g, int split) {
+  const int k = (int)(g % kSplitPeriod);
+  return (k + 1) * split / kSplitPeriod > k * split / kSplitPeriod;
+}
+
 template <bool SYM>
 __global__ void __launch_bounds__(kTmaThreads, EVOK_GRAD_TMA_CTAS_PER_SM)
     grad_partial_tma_kernel(int form, const float* __restrict__ X, int64_t ldx, const float* __restrict__ w, const float* __restrict__ mu,
-                            const float* __restrict__ sigma, int64_t n_units, int64_t D, int64_t units_per_chunk,
-                            float* __restrict__ partial) {
+                            const float* __restrict__ sigma, int64_t n_units, int64_t D, int64_t units_per_chunk, int split, uint64_t unit0,
+                            const __grid_constant__ PhiloxKey key, const uint32_t* __restrict__ stream_off, float* __restrict__ partial) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   float* tiles = reinterpret_cast<float*>(smem_raw);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + (size_t)kTmaStages * kTmaRows * kTmaCols * sizeof(float));
@@ -323,9 +337,12 @@ __global__ void __launch_bounds__(kTmaThreads, EVOK_GRAD_TMA_CTAS_PER_SM)
     // ===== producer warp: one elected lane issues the bulk copies =====
     if (lane == 0) {
       const uint32_t row_bytes = (uint32_t)(width * sizeof(float));
+      int64_t t = 0;  // streamed groups so far: the ring advances only on these
       for (int64_t g = 0; g < n_groups; ++g) {
-        const int s = (int)(g % kTmaStages);
-        const uint32_t use = (uint32_t)(g / kTmaStages);
+        if (group_rebuilt(g, split)) continue;
+        const int s = (int)(t % kTmaStages);
+        const uint32_t use = (uint32_t)(t / kTmaStages);
+        ++t;
         if (use > 0) mbar_wait(&empty[s], (use - 1) & 1);
         const int64_t r0 = r_begin + g * kTmaRows;
         const int rows = (int)min((int64_t)kTmaRows, r_end - r0);
@@ -340,27 +357,27 @@ __global__ void __launch_bounds__(kTmaThreads, EVOK_GRAD_TMA_CTAS_PER_SM)
   // ===== consumer warps =====
   const int64_t col = col0 + (int64_t)tid * 4;
   const bool active = col < D;
-  float m[4], c1[4], c0[4];
+  const uint32_t sw = key.stream_lo + (stream_off ? __ldg(stream_off) : 0u);
+  float m[4], sg[4], c1[4], c0[4];
 #pragma unroll
   for (int c = 0; c < 4; ++c) {
-    const float sg = active ? __ldg(sigma + col + c) : 1.0f;
+    sg[c] = active ? __ldg(sigma + col + c) : 1.0f;
     m[c] = active ? __ldg(mu + col + c) : 0.0f;
     if (form == EVOK_GRAD_EXP) {
-      c1[c] = __fdiv_rn(1.0f, sg * sg);
+      c1[c] = __fdiv_rn(1.0f, sg[c] * sg[c]);
       c0[c] = 1.0f;
     } else if (form == EVOK_GRAD_MOMENTS) {
       c1[c] = 1.0f;
       c0[c] = 0.0f;
     } else {
-      c1[c] = __fdiv_rn(1.0f, sg);
-      c0[c] = sg;
+      c1[c] = __fdiv_rn(1.0f, sg[c]);
+      c0[c] = sg[c];
     }
   }
   float s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
 
+  int64_t t = 0;  // streamed groups consumed so far (the producer's ring position)
   for (int64_t g = 0; g < n_groups; ++g) {
-    const int s = (int)(g % kTmaStages);
-    const uint32_t use = (uint32_t)(g / kTmaStages);
     const int64_t r0 = r_begin + g * kTmaRows;
     const int rows = (int)min((int64_t)kTmaRows, r_end - r0);
     float a[kTmaRows], b[kTmaRows];
@@ -377,6 +394,36 @@ __global__ void __launch_bounds__(kTmaThreads, EVOK_GRAD_TMA_CTAS_PER_SM)
         }
       }
     }
+    if (group_rebuilt(g, split)) {
+      if (active) {
+        // all rows' Philox chains first (independent: they overlap in the pipeline), then the same FMA chain as below
+        float x[kTmaRows][4];
+#pragma unroll
+        for (int i = 0; i < kTmaRows; ++i) {
+          if (i < rows) {
+            float z[4];
+            normals4(key, sw, unit0 + (uint64_t)(r0 + i), (uint32_t)(col >> 2), z);
+#pragma unroll
+            for (int c = 0; c < 4; ++c) x[i][c] = fmaf(sg[c], z[c], m[c]);
+          }
+        }
+#pragma unroll
+        for (int i = 0; i < kTmaRows; ++i) {
+          if (i < rows) {
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {
+              const float e = x[i][c] - m[c];
+              s1[c] = fmaf(a[i], e, s1[c]);
+              s2[c] = fmaf(b[i], fmaf(e * e, c1[c], -c0[c]), s2[c]);
+            }
+          }
+        }
+      }
+      continue;
+    }
+    const int s = (int)(t % kTmaStages);
+    const uint32_t use = (uint32_t)(t / kTmaStages);
+    ++t;
     mbar_wait(&full[s], use & 1);
     const float4* tile = reinterpret_cast<const float4*>(tiles + (size_t)s * kTmaRows * kTmaCols) + tid;
     if (active) {
@@ -452,12 +499,21 @@ static void launch_partial(const GradPlan& p, int form, const float* X, int64_t 
 #undef EVOK_LAUNCH_TX
 }
 
+// Rebuilt groups per kSplitPeriod when the caller leaves the choice to the library (scripts/grad_hybrid_bench.py).  On an H100
+// SXM capped at 400 W the pass is bound by power, not by bandwidth or issue: streaming alone already draws the cap (the SM clock
+// drops to ~1.1 GHz), rebuilding alone draws it at ~1.9 GHz, and both cost about the same energy per element.  A small rebuilt
+// share fills the idle issue slots of the streaming pass; more shifts the pass towards the slower all-rebuild end
+// (1 M x 10 k symmetric: split 0 7.31-7.39 ms, 2 6.72 ms, 4 6.80-6.87 ms, 8 7.30 ms, 16 7.78-7.82 ms).
+constexpr int kAutoSplit = EVOK_GRAD_AUTO_SPLIT;
+
+// split: rebuilt groups per kSplitPeriod in the TMA kernel (0 = stream every row, -1 = kAutoSplit); rows are rebuilt from
+// (seed, stream_id, *stream_off, row0), which must be the counters that sampled X from this mu and sigma.
 static int grad_impl(int form, const float* X, int64_t ldx, const float* w, const float* mu, const float* sigma, int64_t row0, int64_t n_rows,
                      int64_t D, bool regen, uint64_t seed, uint64_t stream_id, const uint32_t* stream_off, float scale_mu, float scale_sigma, float* out_mu,
-                     float* out_sigma, void* ws, size_t ws_bytes, void* stream, const GradPush* push = nullptr) {
+                     float* out_sigma, void* ws, size_t ws_bytes, void* stream, const GradPush* push = nullptr, int split = 0) {
   if (!w || !mu || !sigma || !ws || (!regen && !X) || (!push && (!out_mu || !out_sigma))) return EVOK_E_NULLPTR;
   if (form < EVOK_GRAD_SEPARABLE || form > EVOK_GRAD_MOMENTS) return EVOK_E_BADENUM;
-  if (n_rows < 0 || D <= 0 || row0 < 0 || (!regen && ldx < D)) return EVOK_E_BADSIZE;
+  if (n_rows < 0 || D <= 0 || row0 < 0 || (!regen && ldx < D) || split < -1 || split > kSplitPeriod) return EVOK_E_BADSIZE;
   const bool sym = form == EVOK_GRAD_SYMMETRIC;
   if (sym && ((n_rows & 1) || (row0 & 1))) return EVOK_E_ODDROWS;
   if (ws_bytes < evok_grad_workspace_bytes(n_rows, D)) return EVOK_E_WORKSPACE;
@@ -485,13 +541,11 @@ static int grad_impl(int form, const float* X, int64_t ldx, const float* w, cons
     const int64_t upc = (n_units + chunks - 1) / chunks;
     const int n_chunks = (int)((n_units + upc - 1) / upc);
     dim3 grid(n_coltiles, n_chunks);
-    if (sym) {
-      cudaFuncSetAttribute(grad_partial_tma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTmaSmemBytes);
-      grad_partial_tma_kernel<true><<<grid, kTmaThreads, kTmaSmemBytes, st>>>(form, X, ldx, w, mu, sigma, n_units, D, upc, partial);
-    } else {
-      cudaFuncSetAttribute(grad_partial_tma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTmaSmemBytes);
-      grad_partial_tma_kernel<false><<<grid, kTmaThreads, kTmaSmemBytes, st>>>(form, X, ldx, w, mu, sigma, n_units, D, upc, partial);
-    }
+    const int rebuilt = split < 0 ? kAutoSplit : split;
+    const PhiloxKey key = make_philox_key(seed, stream_id);
+    auto kernel = sym ? grad_partial_tma_kernel<true> : grad_partial_tma_kernel<false>;
+    cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTmaSmemBytes);
+    kernel<<<grid, kTmaThreads, kTmaSmemBytes, st>>>(form, X, ldx, w, mu, sigma, n_units, D, upc, rebuilt, unit0, key, stream_off, partial);
     EVOK_CHECK_LAUNCH();
     return launch_finalize(partial, n_chunks, D, scale_mu, scale_sigma, out_mu, out_sigma, push, st);
   }
@@ -531,6 +585,13 @@ extern "C" EVOK_API int evok_grad_regen(int form, const float* w, const float* m
                                float* out_mu, float* out_sigma, void* ws, size_t ws_bytes, void* stream) {
   return grad_impl(form, nullptr, 0, w, mu, sigma, row0, n_rows, D, true, seed, stream_id, stream_offset_dev, scale_mu, scale_sigma, out_mu, out_sigma, ws,
                    ws_bytes, stream);
+}
+
+extern "C" EVOK_API int evok_grad_hybrid(int form, const float* X, int64_t ldx, const float* w, const float* mu, const float* sigma, int64_t row0,
+                                         int64_t n_rows, int64_t D, uint64_t seed, uint64_t stream_id, const uint32_t* stream_offset_dev, int split,
+                                         float scale_mu, float scale_sigma, float* out_mu, float* out_sigma, void* ws, size_t ws_bytes, void* stream) {
+  return grad_impl(form, X, ldx, w, mu, sigma, row0, n_rows, D, false, seed, stream_id, stream_offset_dev, scale_mu, scale_sigma, out_mu, out_sigma, ws,
+                   ws_bytes, stream, nullptr, split);
 }
 
 extern "C" EVOK_API int evok_grad_push(int form, const float* X, int64_t ldx, const float* w, const float* mu, const float* sigma, int64_t row0,

@@ -181,7 +181,7 @@ def sharded_sample_and_gradients(problem, distribution, popsize: int, *, obj_ind
         problem.philox_row0 = 0
         problem._active_peer = None
 
-    samples = batch.recipe if isinstance(batch, LazySolutionBatch) else batch.access_values(keep_evals=True)
+    samples = batch.recipe if isinstance(batch, LazySolutionBatch) else batch.gradient_samples(dev_dist.mu, dev_dist.sigma)
     if sharded_rank:
         offsets = [0]
         for c in counts:

@@ -22,7 +22,7 @@ from typing import Any, Iterable, Optional
 import torch
 
 from . import ops
-from .core import PhiloxRecipe
+from .core import PhiloxRecipe, PhiloxSamples
 from .tools.cloning import Clonable
 from .tools.readonlytensor import as_plain_tensor
 from .tools.misc import extract_generator, make_gaussian, to_torch_dtype
@@ -256,6 +256,12 @@ class SeparableGaussian(Distribution):
         """(scale_mu * sum_r a_r eps_r, scale_sigma * sum_r b_r g(eps_r)) -- the K4 kernel, or its torch restatement."""
         mu, sigma = self.mu, self.sigma
         peer = getattr(self, "_peer", None)
+        if isinstance(samples, PhiloxSamples):  # a population the fused sampler wrote from mu / sigma, untouched since
+            r = samples.recipe
+            if peer is None and ops.uses_kernels(w):
+                return ops.grad_hybrid(form, samples.values, w.contiguous(), mu.contiguous(), sigma.contiguous(), seed=r.seed, stream_id=r.stream_id, row0=r.row0,
+                                       scale_mu=scale_mu, scale_sigma=scale_sigma, stream_offset=r.stream_offset)
+            samples = samples.values
         if peer is not None:  # sharded generation: the kernel pushes this shard's sums to every GPU, the reduction returns the global sums
             if isinstance(samples, PhiloxRecipe):
                 ops.grad_push(form, None, w.contiguous(), mu.contiguous(), sigma.contiguous(), scale_mu=scale_mu, scale_sigma=scale_sigma, peer=peer,

@@ -310,6 +310,32 @@ def grad_regen(form: int, w: torch.Tensor, mu: torch.Tensor, sigma: torch.Tensor
     return out_mu, out_sigma
 
 
+GRAD_SPLIT_PERIOD = 16  # `split` of grad_hybrid counts rebuilt row groups per this many
+
+
+def grad_hybrid(form: int, X: torch.Tensor, w: torch.Tensor, mu: torch.Tensor, sigma: torch.Tensor, *, seed: int, stream_id: int, row0: int,
+                scale_mu: float, scale_sigma: float, split: int = -1, out_mu: Optional[torch.Tensor] = None,
+                out_sigma: Optional[torch.Tensor] = None, stream_offset: Optional[torch.Tensor] = None) -> tuple:
+    """`grad` over an X that `sample_eval` wrote from this very `mu` / `sigma` with the same seed, stream_id, row0 and
+    stream_offset: `split` of every GRAD_SPLIT_PERIOD row groups are rebuilt from their Philox counters instead of being read
+    (-1 = the library's choice).  Bit-identical to `grad(form, X, ...)` for every split."""
+    _mat(X, "samples")
+    n, D = X.shape
+    _vec(w, "weights", n); _vec(mu, "mu", D); _vec(sigma, "sigma", D)
+    if not -1 <= split <= GRAD_SPLIT_PERIOD:
+        raise ValueError(f"split: expected -1 .. {GRAD_SPLIT_PERIOD}, got {split}")
+    out_mu = torch.empty_like(mu) if out_mu is None else _vec(out_mu, "out_mu", D)
+    out_sigma = torch.empty_like(mu) if out_sigma is None else _vec(out_sigma, "out_sigma", D)
+    ws = nat.workspace(X.device, nat.lib().evok_grad_workspace_bytes(n, D), "grad")
+    with _timed("grad_hybrid"):
+        rc = nat.lib().evok_grad_hybrid(form, X.data_ptr(), X.stride(0), w.data_ptr(), mu.data_ptr(), sigma.data_ptr(), row0, n, D,
+                                        seed & 0xFFFFFFFFFFFFFFFF, stream_id & 0xFFFFFFFFFFFFFFFF, _offset_ptr(stream_offset), int(split),
+                                        scale_mu, scale_sigma, out_mu.data_ptr(), out_sigma.data_ptr(), ws.data_ptr(), ws.numel(),
+                                        nat.stream_of(X))
+    nat.check(rc, "evok_grad_hybrid")
+    return out_mu, out_sigma
+
+
 # ------------------------------------------------------------------------------------------------ K5
 def clipup_step(g: torch.Tensor, velocity: torch.Tensor, stepsize: float, momentum: float, max_speed: float,
                 step_out: Optional[torch.Tensor] = None, mu: Optional[torch.Tensor] = None) -> None:

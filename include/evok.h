@@ -146,6 +146,15 @@ int evok_grad_regen(int form, const float* w, const float* mu, const float* sigm
                     int64_t D, uint64_t seed, uint64_t stream_id, const uint32_t* stream_offset_dev, float scale_mu,
                     float scale_sigma, float* out_mu, float* out_sigma, void* ws, size_t ws_bytes, void* stream);
 
+/* evok_grad over a materialised population X that evok_sample_eval wrote from this mu and sigma with the same (seed,
+ * stream_id, stream_offset_dev, row0): part of the rows are rebuilt from their Philox counters on the SMs while the rest
+ * stream from X, which cuts the bytes read.  The result is bit-identical to evok_grad for every split.
+ * split = rebuilt row groups per 16 (0 = read every row, 16 = rebuild every row, -1 = the library's choice).  Shapes the
+ * TMA-staged kernel does not take (D % 4, alignment, D < 512, fewer than 4096 units, EVOK_GRAD_MOMENTS) read every row. */
+int evok_grad_hybrid(int form, const float* X, int64_t ldx, const float* w, const float* mu, const float* sigma, int64_t row0,
+                     int64_t n_rows, int64_t D, uint64_t seed, uint64_t stream_id, const uint32_t* stream_offset_dev, int split,
+                     float scale_mu, float scale_sigma, float* out_mu, float* out_sigma, void* ws, size_t ws_bytes, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * K5: D-vector updates (no host synchronisation; norms are reduced on the device).
  * --------------------------------------------------------------------------------------------- */
