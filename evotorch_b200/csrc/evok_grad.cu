@@ -381,6 +381,7 @@ __global__ void __launch_bounds__(kTmaThreads, EVOK_GRAD_TMA_CTAS_PER_SM)
     const int64_t r0 = r_begin + g * kTmaRows;
     const int rows = (int)min((int64_t)kTmaRows, r_end - r0);
     float a[kTmaRows], b[kTmaRows];
+    bool need[kTmaRows];  // rows whose weights are both zero are skipped, as in grad_partial_kernel: their values never matter
 #pragma unroll
     for (int i = 0; i < kTmaRows; ++i) {
       a[i] = b[i] = 0.0f;
@@ -393,6 +394,7 @@ __global__ void __launch_bounds__(kTmaThreads, EVOK_GRAD_TMA_CTAS_PER_SM)
           a[i] = b[i] = __ldg(w + r0 + i);
         }
       }
+      need[i] = a[i] != 0.0f || b[i] != 0.0f;
     }
     if (group_rebuilt(g, split)) {
       if (active) {
@@ -400,7 +402,7 @@ __global__ void __launch_bounds__(kTmaThreads, EVOK_GRAD_TMA_CTAS_PER_SM)
         float x[kTmaRows][4];
 #pragma unroll
         for (int i = 0; i < kTmaRows; ++i) {
-          if (i < rows) {
+          if (need[i]) {
             float z[4];
             normals4(key, sw, unit0 + (uint64_t)(r0 + i), (uint32_t)(col >> 2), z);
 #pragma unroll
@@ -409,7 +411,7 @@ __global__ void __launch_bounds__(kTmaThreads, EVOK_GRAD_TMA_CTAS_PER_SM)
         }
 #pragma unroll
         for (int i = 0; i < kTmaRows; ++i) {
-          if (i < rows) {
+          if (need[i]) {
 #pragma unroll
             for (int c = 0; c < 4; ++c) {
               const float e = x[i][c] - m[c];
@@ -427,10 +429,13 @@ __global__ void __launch_bounds__(kTmaThreads, EVOK_GRAD_TMA_CTAS_PER_SM)
     mbar_wait(&full[s], use & 1);
     const float4* tile = reinterpret_cast<const float4*>(tiles + (size_t)s * kTmaRows * kTmaCols) + tid;
     if (active) {
+      float4 v4[kTmaRows];  // every slot of the stage is loaded (a slot past `rows` holds stale data that is never used)
+#pragma unroll
+      for (int i = 0; i < kTmaRows; ++i) v4[i] = tile[(size_t)i * (kTmaCols / 4)];
 #pragma unroll
       for (int i = 0; i < kTmaRows; ++i) {
-        if (i < rows) {
-          const float4 v = tile[(size_t)i * (kTmaCols / 4)];
+        if (need[i]) {
+          const float4 v = v4[i];
           const float x[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
           for (int c = 0; c < 4; ++c) {
