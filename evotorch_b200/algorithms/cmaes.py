@@ -14,6 +14,10 @@ glue between the contractions is fused into four small kernels (csrc/evok_cmaes.
 applied by the SYRK's epilogue, so a generation is ~14 launches with no host reads and replays from a CUDA graph
 (`enable_cuda_graph()`).  The Cholesky factorisation stays on cuSOLVER (torch.linalg.cholesky_ex): the repo's own persistent
 tile-dataflow kernel (csrc/evok_chol.cu, EVOTORCH_B200_EVOK_CHOLESKY=1) is correct but its 64 x 64 diagonal tiles form a serial critical path.
+
+Separable CMA-ES (`separable=True`, diagonal C) has its own fused generation on CUDA fp32 (`_step_sep_fused`): four kernels, no
+host reads, the population written once (or never, with `Problem(lazy_population=True)`) and never read back, stdev bounds
+included, CUDA-graph capturable at any `decompose_C_freq`.  The op-by-op path stays for CPU, rng="torch" and other dtypes.
 """
 
 from __future__ import annotations
@@ -26,7 +30,7 @@ import numpy as np
 import torch
 
 from .. import ops
-from ..core import Problem, Solution, SolutionBatch
+from ..core import LazySolutionBatch, PhiloxRecipe, Problem, Solution, SolutionBatch
 from .searchalgorithm import SearchAlgorithm, SinglePopulationAlgorithmMixin
 
 
@@ -53,8 +57,17 @@ class CMAES(SearchAlgorithm, SinglePopulationAlgorithmMixin):
             popsize = 4 + int(np.floor(3 * np.log(d)))  # cmaes.py:270-272
         self.popsize = int(popsize)
         self.mu = int(np.floor(popsize / 2))
-        self._population = problem.generate_batch(popsize=popsize)
         self.separable = bool(separable)
+        if self.separable and problem.lazy_population:
+            # the fused separable generation never reads the population back, so it can stay a function of the Philox counters.
+            # No initial values are drawn for it, so with center_init=None the random centre below differs from the one of a
+            # materialised run with the same seed (whose initial population consumes the generator first, as in the reference).
+            if not (problem.evok_objective_id is not None and problem.rng == "philox" and len(problem.senses) == 1
+                    and problem.eval_data_length == 0 and problem.device.type == "cuda" and problem.dtype == torch.float32):
+                raise ValueError("a lazy population needs a built-in objective, rng='philox', a separable Gaussian and CUDA float32")
+            self._population = LazySolutionBatch(problem, popsize)
+        else:
+            self._population = problem.generate_batch(popsize=popsize)
 
         if center_init is None:
             center_init = problem.generate_values(1)
@@ -147,7 +160,8 @@ class CMAES(SearchAlgorithm, SinglePopulationAlgorithmMixin):
         n = self.popsize if num_samples is None else int(num_samples)
         problem = self._problem
         d = problem.solution_length
-        fs = self.__dict__.get("_fused") if n == self.popsize else None  # persistent buffers of the fused generation
+        # persistent buffers of the fused generation (the separable one draws inside its own sampler and keeps no zs)
+        fs = self.__dict__.get("_fused") if n == self.popsize and not self.separable else None
         zs = problem.make_empty(num_solutions=n) if fs is None else fs["zs"]
         if ops.uses_kernels(zs) and problem.rng == "philox":
             seed, stream_id = problem.next_philox_stream()
@@ -258,15 +272,34 @@ class CMAES(SearchAlgorithm, SinglePopulationAlgorithmMixin):
         else:
             self.A = torch.linalg.cholesky(self.C)
 
-    # ------------------------------------------------------------------ fused generation (CUDA float32, full covariance)
+    # ------------------------------------------------------------------ fused generation (CUDA float32)
     def _fused_ok(self) -> bool:
-        return (not self.separable and self.stdev_min is None and self.stdev_max is None and ops.uses_kernels(self.m) and ops.uses_kernels(self.C)
-                and self._problem.rng == "philox" and self._population._data.is_contiguous()
-                and self._population._evdata.shape[1] == 1 and self._population._evdata.dtype == torch.float32)
+        pop = self._population
+        if self.separable:  # stdev bounds are applied by the update kernel; the sampler is built in, so an override stays op-by-op
+            return (ops.uses_kernels(self.m) and ops.uses_kernels(self.C) and self._problem.rng == "philox"
+                    and (isinstance(pop, LazySolutionBatch) or pop._data.is_contiguous()) and pop._evdata.shape[1] == 1
+                    and pop._evdata.dtype == torch.float32 and "sample_distribution" not in self.__dict__
+                    and type(self).sample_distribution is CMAES.sample_distribution)
+        return (self.stdev_min is None and self.stdev_max is None and ops.uses_kernels(self.m) and ops.uses_kernels(self.C)
+                and self._problem.rng == "philox" and pop._data.is_contiguous()
+                and pop._evdata.shape[1] == 1 and pop._evdata.dtype == torch.float32)
 
     def _fused_state(self) -> dict:
         fs = self.__dict__.get("_fused")
-        if fs is None:
+        if fs is None and self.separable:
+            n, d, dev = self.popsize, self._problem.solution_length, self.m.device
+            new = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=dev)  # noqa: E731
+            lazy = isinstance(self._population, LazySolutionBatch)
+            # m_draw / s_draw: the centre and stdev the current (lazy) population was drawn from, written by the update kernel
+            fs = self._fused = dict(q=new(n), aw=new(n), local=new(d), S2=new(d), wsum=new(1), m_draw=new(d) if lazy else None,
+                                    s_draw=new(d) if lazy else None, steps_dev=None)
+            self.m, self.p_sigma, self.p_c = self.m.contiguous().clone(), self.p_sigma.contiguous().clone(), self.p_c.contiguous().clone()
+            self.sigma = self.sigma.reshape(()).clone()
+            self.C, self.A = self.C.contiguous().clone(), self.A.contiguous().clone()
+            fs["s"] = (self.sigma * self.A).contiguous()  # the sampler's per-column stdev; the update kernel keeps it = sigma * A
+            self._consts = (self.c_m, self.c_sigma, self.damp_sigma, self.c_c, self.c_1, self.c_mu, self.variance_discount_sigma,
+                            self.variance_discount_c, float(self.unbiased_expectation), self._weights_sum)
+        elif fs is None:
             p, n, d = self._problem, self.popsize, self._problem.solution_length
             dev = self.m.device
             new = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=dev)  # noqa: E731
@@ -287,6 +320,9 @@ class CMAES(SearchAlgorithm, SinglePopulationAlgorithmMixin):
         -> row weights (positive part / active reweighting, one pass over Z) -> two weighted row sums (K4) -> fused vector update
         (m, p_sigma, sigma, h_sig, p_c + the covariance coefficients) -> weighted SYRK with the covariance update in its epilogue ->
         Cholesky.  Every state tensor is updated in place."""
+        if self.separable:
+            self._step_sep_fused()
+            return
         fs = self._fused_state()
         zs, ys, xs = self.sample_distribution()
         pop = self._population
@@ -310,20 +346,62 @@ class CMAES(SearchAlgorithm, SinglePopulationAlgorithmMixin):
             else:
                 torch.linalg.cholesky_ex(self.C, check_errors=False, out=(self.A, fs["info"]))
 
+    def _step_sep_fused(self):
+        """One separable generation (cmaes.py:567-606 with diagonal C) as four kernels with no host reads.  With s = sigma * A:
+        sample x_i = m + s z_i and evaluate it in one pass that also keeps q_i = ||z_i||^2 (the population is written once, or not
+        at all when it is lazy) -> rank-to-weights -> the moments sum a_i z_i, sum b_i z_i^2, sum b_i over z regenerated from the
+        same Philox counters (never read back) -> one update kernel for m, p_sigma, sigma, p_c, C, the stdev bounds, A and s.
+        The draw takes one Philox stream id, the one the op-by-op path takes for its zs, so both paths see the same z."""
+        fs = self._fused_state()
+        prob, pop, n, d = self._problem, self._population, self.popsize, self._problem.solution_length
+        lazy = isinstance(pop, LazySolutionBatch)
+        seed, stream_id = prob.next_philox_stream()
+        offset = prob.philox_stream_offset
+        f = pop._evdata.view(-1)
+        obj = prob.evok_objective_id
+        if lazy:
+            # until the update below the live m and s ARE the draw's centre and stdev (what a before-eval hook or the best / worst
+            # bookkeeping regenerates rows from)
+            pop.recipe = PhiloxRecipe(seed=seed, stream_id=stream_id, row0=0, n_rows=n, solution_length=d, symmetric=False, stream_offset=offset,
+                                      mu=self.m, sigma=fs["s"])
+            prob._before_eval_hook(pop)
+            ops.sample_eval_sq(obj, None, self.m, fs["s"], fs["q"], n_rows=n, seed=seed, stream_id=stream_id, f=f, stream_offset=offset)
+            prob._finish_evaluation(pop)
+        elif obj is not None and len(prob.before_eval_hook) == 0:
+            ops.sample_eval_sq(obj, pop._data, self.m, fs["s"], fs["q"], n_rows=n, seed=seed, stream_id=stream_id, f=f, stream_offset=offset)
+            prob._finish_evaluation(pop)
+        else:  # custom objective or before-eval hooks: sample (and keep q), then the problem's own evaluation
+            ops.sample_eval_sq(ops.OBJ_NONE, pop._data, self.m, fs["s"], fs["q"], n_rows=n, seed=seed, stream_id=stream_id, stream_offset=offset)
+            pop._evdata.fill_(float("nan"))
+            prob.evaluate(pop)
+        ops.rank_table(f, prob.senses[self._obj_index] == "max", self.weights, out=fs["aw"])
+        ops.sepcma_moments(fs["aw"], fs["q"], self.active, d, seed=seed, stream_id=stream_id, stream_offset=offset, local=fs["local"], S2=fs["S2"],
+                           wsum=fs["wsum"])
+        ops.sepcma_update(fs["local"], fs["S2"], fs["wsum"], self.m, self.p_sigma, self.p_c, self.sigma, self.C, self.A, fs["s"], self._consts,
+                          self.csa_squared, decompose_C_freq=self.decompose_C_freq, steps=self._steps_count, steps_dev=fs["steps_dev"],
+                          stdev_min=self.stdev_min, stdev_max=self.stdev_max, m_prev=fs["m_draw"], s_prev=fs["s_draw"])
+        if lazy:
+            # from here on the population is the one drawn from the snapshots.  Under a CUDA graph the stream offset counter is
+            # advanced right after this body, so the draw is (stream_id - 1) + counter: the recipe then follows every replay.
+            pop.recipe = PhiloxRecipe(seed=seed, stream_id=stream_id if offset is None else stream_id - 1, row0=0, n_rows=n, solution_length=d,
+                                      symmetric=False, stream_offset=offset, mu=fs["m_draw"], sigma=fs["s_draw"])
+
     # ------------------------------------------------------------------ CUDA-graph replay of the fused generation
     def enable_cuda_graph(self, enabled: bool = True):
         """Capture the fused generation into a CUDA graph and replay it from `step()` (one graph launch per generation; the
         z-sampler reads a device-side generation counter, `_h_sig` a device-side step counter, so the replayed trajectory equals
-        eager stepping).  Used when the configuration is capturable: fused path, built-in objective, no evaluation hooks, Cholesky
-        every generation (`decompose_C_freq == 1`); otherwise stepping stays eager."""
+        eager stepping).  Used when the configuration is capturable: fused path, built-in objective, no evaluation hooks, and for
+        the full covariance a Cholesky every generation (`decompose_C_freq == 1`; the separable update kernel reads the step
+        counter itself, so it replays at any frequency); otherwise stepping stays eager."""
         self._use_graph = bool(enabled)
         self._graph = None
         return self
 
     def _graph_capturable(self) -> bool:
         prob = self._problem
-        return (self._fused_ok() and self.decompose_C_freq == 1 and prob.evok_objective_id is not None and len(prob.before_eval_hook) == 0
-                and len(prob.after_eval_hook) == 0 and not prob.stores_solution_stats and "sample_distribution" not in self.__dict__)
+        return (self._fused_ok() and (self.separable or self.decompose_C_freq == 1) and prob.evok_objective_id is not None
+                and len(prob.before_eval_hook) == 0 and len(prob.after_eval_hook) == 0 and not prob.stores_solution_stats
+                and "sample_distribution" not in self.__dict__)
 
     def _step_graph(self):
         from .. import _native as nat
@@ -376,6 +454,8 @@ class CMAES(SearchAlgorithm, SinglePopulationAlgorithmMixin):
                     self._fused["steps_dev"], self._problem.philox_stream_offset = None, None
                 self._step_fused()
             return
+        if self.separable:
+            self._fused = None  # the op-by-op step replaces the state tensors: the fused buffers (and s = sigma * A) are rebuilt
         zs, ys, xs = self.sample_distribution()
         assigned_weights = self.get_population_weights(xs)
         local_m_displacement, shaped_m_displacement = self.update_m(zs, ys, assigned_weights)

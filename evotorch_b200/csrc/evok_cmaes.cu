@@ -48,17 +48,27 @@ struct CmaesConsts {
 
 constexpr int kCmaThreads = 1024;
 
-__global__ void __launch_bounds__(kCmaThreads)
-    cmaes_vector_update_kernel(const float* __restrict__ local_disp, const float* __restrict__ shaped_disp, int64_t D, float* __restrict__ m,
-                               float* __restrict__ p_sigma, float* __restrict__ p_c, float* __restrict__ sigma, long long* steps_dev,
-                               long long steps_host, const __grid_constant__ CmaesConsts c, float* __restrict__ k_out, float* __restrict__ h_sig_out) {
-  __shared__ double sm[33];
+struct CmaVectorStep {
+  float new_sigma, h;
+  long long steps;  // generation counter before this generation's increment
+};
+
+// update_m, update_p_sigma, update_sigma, _h_sig, update_p_c (cmaes.py:454-517, :31-46) on one CTA, in place; element i belongs
+// to thread i % kCmaThreads.  The shaped displacement sum_i w_i y_i is `shaped_disp` or, separable (SEP), A * local_disp (y = A z
+// elementwise).  m_prev (SEP, nullable) receives m before the update.  *sigma is left to the caller (read by every thread first).
+template <bool SEP>
+__device__ __forceinline__ CmaVectorStep cma_vector_step(const float* __restrict__ local_disp, const float* __restrict__ shaped_disp,
+                                                         const float* __restrict__ A, int64_t D, float* __restrict__ m, float* __restrict__ p_sigma,
+                                                         float* __restrict__ p_c, const float* sigma, const long long* steps_dev, long long steps_host,
+                                                         const CmaesConsts& c, double* sm, float* __restrict__ m_prev) {
   const float sig = *sigma;
   const long long steps = steps_dev ? *steps_dev : steps_host;
   // update_m (cmaes.py:477-479, uses the OLD sigma) and update_p_sigma (:483-490)
   double acc = 0.0;
   for (int64_t i = threadIdx.x; i < D; i += kCmaThreads) {
-    m[i] = m[i] + c.c_m * sig * shaped_disp[i];
+    const float mi = m[i];
+    if (SEP && m_prev) m_prev[i] = mi;
+    m[i] = mi + c.c_m * sig * (SEP ? A[i] * local_disp[i] : shaped_disp[i]);
     const float ps = (1.0f - c.c_sigma) * p_sigma[i] + c.vd_sigma * local_disp[i];
     p_sigma[i] = ps;
     acc += (double)ps * (double)ps;
@@ -73,7 +83,19 @@ __global__ void __launch_bounds__(kCmaThreads)
   const float squared_sum = (float)((double)(pnorm * pnorm) / decay);
   const float h = ((squared_sum / dn) - 1.0f < 1.0f + 4.0f / (dn + 1.0f)) ? 1.0f : 0.0f;
   // update_p_c (:509-517)
-  for (int64_t i = threadIdx.x; i < D; i += kCmaThreads) p_c[i] = (1.0f - c.c_c) * p_c[i] + h * c.vd_c * shaped_disp[i];
+  for (int64_t i = threadIdx.x; i < D; i += kCmaThreads)
+    p_c[i] = (1.0f - c.c_c) * p_c[i] + h * c.vd_c * (SEP ? A[i] * local_disp[i] : shaped_disp[i]);
+  return CmaVectorStep{new_sigma, h, steps};
+}
+
+__global__ void __launch_bounds__(kCmaThreads)
+    cmaes_vector_update_kernel(const float* __restrict__ local_disp, const float* __restrict__ shaped_disp, int64_t D, float* __restrict__ m,
+                               float* __restrict__ p_sigma, float* __restrict__ p_c, float* __restrict__ sigma, long long* steps_dev,
+                               long long steps_host, const __grid_constant__ CmaesConsts c, float* __restrict__ k_out, float* __restrict__ h_sig_out) {
+  __shared__ double sm[33];
+  const CmaVectorStep v = cma_vector_step<false>(local_disp, shaped_disp, nullptr, D, m, p_sigma, p_c, sigma, steps_dev, steps_host, c, sm, nullptr);
+  const float new_sigma = v.new_sigma, h = v.h;
+  const long long steps = v.steps;
   if (threadIdx.x == 0) {
     *sigma = new_sigma;
     if (steps_dev) *steps_dev = steps + 1;
@@ -83,6 +105,48 @@ __global__ void __launch_bounds__(kCmaThreads)
     k_out[0] = c.c_mu;
     k_out[1] = 1.0f - c1a - c.c_mu * c.weights_sum;
     k_out[2] = c1a * wpc2;
+    if (h_sig_out) *h_sig_out = h;
+  }
+}
+
+// Separable CMA-ES, everything after the moments in one CTA: cma_vector_step, then per element (cmaes.py:536-545, separable
+// branch, and :49-79, :555-565 of the reference)
+//   C <- C + c1a (p_c^2 - C) + c_mu (A^2 S2 - wsum C)              (S2 = sum_i b_i z_i^2, so A^2 S2 = sum_i b_i y_i^2)
+//   stdev bounds with the new sigma: C <- (clamp(sigma' sqrt(C), lo, hi) / sigma')^2
+//   A <- sqrt(C) on the generations where (steps + 1) % decompose_freq == 0;   s <- sigma' A  (the sampler's per-column stdev)
+// s_prev (nullable) receives s before the update.  lo / hi: NaN = no bound.
+__global__ void __launch_bounds__(kCmaThreads)
+    sepcma_update_kernel(const float* __restrict__ local_disp, const float* __restrict__ S2, const float* __restrict__ wsum, int64_t D,
+                         float* __restrict__ m, float* __restrict__ p_sigma, float* __restrict__ p_c, float* __restrict__ sigma, float* __restrict__ C,
+                         float* __restrict__ A, float* __restrict__ s, float* __restrict__ m_prev, float* __restrict__ s_prev, long long* steps_dev,
+                         long long steps_host, const __grid_constant__ CmaesConsts c, long long decompose_freq, float lo, float hi,
+                         float* __restrict__ h_sig_out) {
+  __shared__ double sm[33];
+  const CmaVectorStep v = cma_vector_step<true>(local_disp, nullptr, A, D, m, p_sigma, p_c, sigma, steps_dev, steps_host, c, sm, m_prev);
+  const float sg = v.new_sigma, h = v.h;
+  const float c1a = c.c_1 * (1.0f - (1.0f - h * h) * c.c_c * (2.0f - c.c_c));
+  const float ws = *wsum;
+  const bool has_lo = !isnan(lo), has_hi = !isnan(hi);
+  const bool decompose = (v.steps + 1) % decompose_freq == 0;
+  for (int64_t i = threadIdx.x; i < D; i += kCmaThreads) {
+    const float Ci = C[i], Ai = A[i], pc = p_c[i];  // p_c[i] was just written by this thread
+    float Cn = Ci + c1a * (pc * pc - Ci) + c.c_mu * (Ai * Ai * S2[i] - ws * Ci);
+    if (has_lo || has_hi) {
+      float sd = sg * sqrtf(Cn);
+      if (has_lo && sd < lo) sd = lo;  // NaN stays NaN, like torch.clamp
+      if (has_hi && sd > hi) sd = hi;
+      const float u = __fdiv_rn(sd, sg);
+      Cn = u * u;
+    }
+    C[i] = Cn;
+    const float An = decompose ? sqrtf(Cn) : Ai;
+    A[i] = An;
+    if (s_prev) s_prev[i] = s[i];
+    s[i] = sg * An;
+  }
+  if (threadIdx.x == 0) {
+    *sigma = sg;
+    if (steps_dev) *steps_dev = v.steps + 1;
     if (h_sig_out) *h_sig_out = h;
   }
 }
@@ -100,19 +164,38 @@ extern "C" EVOK_API int evok_cmaes_row_weights(const float* assigned_weights, co
   return 0;
 }
 
-extern "C" EVOK_API int evok_cmaes_vector_update(const float* local_disp, const float* shaped_disp, int64_t D, float* m, float* p_sigma, float* p_c,
-                                                 float* sigma_dev, int64_t* steps_dev, int64_t steps_host, const float* consts_host, int csa_squared,
-                                                 float* k_out, float* h_sig_out, void* stream) {
-  if (!local_disp || !shaped_disp || !m || !p_sigma || !p_c || !sigma_dev || !consts_host || !k_out) return EVOK_E_NULLPTR;
-  if (D <= 0) return EVOK_E_BADSIZE;
+static CmaesConsts cmaes_consts(const float* consts_host, int csa_squared) {
   CmaesConsts c;
   c.c_m = consts_host[0]; c.c_sigma = consts_host[1]; c.damp_sigma = consts_host[2]; c.c_c = consts_host[3]; c.c_1 = consts_host[4];
   c.c_mu = consts_host[5]; c.vd_sigma = consts_host[6]; c.vd_c = consts_host[7]; c.unbiased_expectation = consts_host[8];
   c.weights_sum = consts_host[9];
   c.csa_squared = csa_squared;
+  return c;
+}
+
+extern "C" EVOK_API int evok_cmaes_vector_update(const float* local_disp, const float* shaped_disp, int64_t D, float* m, float* p_sigma, float* p_c,
+                                                 float* sigma_dev, int64_t* steps_dev, int64_t steps_host, const float* consts_host, int csa_squared,
+                                                 float* k_out, float* h_sig_out, void* stream) {
+  if (!local_disp || !shaped_disp || !m || !p_sigma || !p_c || !sigma_dev || !consts_host || !k_out) return EVOK_E_NULLPTR;
+  if (D <= 0) return EVOK_E_BADSIZE;
+  const CmaesConsts c = cmaes_consts(consts_host, csa_squared);
   cmaes_vector_update_kernel<<<1, kCmaThreads, 0, (cudaStream_t)stream>>>(local_disp, shaped_disp, D, m, p_sigma, p_c, sigma_dev,
                                                                          reinterpret_cast<long long*>(steps_dev), (long long)steps_host, c, k_out,
                                                                          h_sig_out);
+  EVOK_CHECK_LAUNCH();
+  return 0;
+}
+
+extern "C" EVOK_API int evok_sepcma_update(const float* local_disp, const float* S2, const float* wsum, int64_t D, float* m, float* p_sigma, float* p_c,
+                                           float* sigma_dev, float* C, float* A, float* s, float* m_prev, float* s_prev, int64_t* steps_dev,
+                                           int64_t steps_host, const float* consts_host, int csa_squared, int64_t decompose_C_freq, float stdev_min,
+                                           float stdev_max, float* h_sig_out, void* stream) {
+  if (!local_disp || !S2 || !wsum || !m || !p_sigma || !p_c || !sigma_dev || !C || !A || !s || !consts_host) return EVOK_E_NULLPTR;
+  if (D <= 0 || decompose_C_freq < 1) return EVOK_E_BADSIZE;
+  const CmaesConsts c = cmaes_consts(consts_host, csa_squared);
+  sepcma_update_kernel<<<1, kCmaThreads, 0, (cudaStream_t)stream>>>(local_disp, S2, wsum, D, m, p_sigma, p_c, sigma_dev, C, A, s, m_prev, s_prev,
+                                                                   reinterpret_cast<long long*>(steps_dev), (long long)steps_host, c,
+                                                                   (long long)decompose_C_freq, stdev_min, stdev_max, h_sig_out);
   EVOK_CHECK_LAUNCH();
   return 0;
 }

@@ -55,13 +55,24 @@ struct GradItems {
   int64_t x, w, mu, sigma, partial;
 };
 
+// Separable CMA-ES row weights (SEPW mode): w holds the rank-assigned weights aw; row r contributes a = max(aw, 0) to S1
+// (recombination) and b = aw, or with active weights b = aw > 0 ? aw : D * aw / q[r] (q = ||z_r||^2, cmaes.py:531-535 of the
+// reference), to S2; the CTAs of column tile 0 also add up b per row chunk into wsum_partial[chunk].
+struct SepWeights {
+  const float* q;
+  int active;
+  float* wsum_partial;
+};
+
 // SYM: unit r = direction (rows 2r, 2r+1), else unit r = row r.  REGEN: eps = sigma * z regenerated from Philox.
-template <int VEC, int TX, bool SYM, bool REGEN>
+// SEPW (with REGEN, non-symmetric, form MOMENTS, mu = sigma = NULL): the weights above, eps = z.
+template <int VEC, int TX, bool SYM, bool REGEN, bool SEPW = false>
 __global__ void __launch_bounds__(kGradThreads, EVOK_GRAD_MINB)
     grad_partial_kernel(int form, const float* __restrict__ X, int64_t ldx, const float* __restrict__ w, const float* __restrict__ mu,
                         const float* __restrict__ sigma, int64_t n_units, int64_t D, int64_t units_per_chunk, uint64_t unit0,
                         const __grid_constant__ PhiloxKey key, const uint32_t* __restrict__ stream_off, float* __restrict__ partial,
-                        const __grid_constant__ GradItems items) {
+                        const __grid_constant__ GradItems items, const __grid_constant__ SepWeights sepw) {
+  static_assert(!SEPW || (REGEN && !SYM), "the CMA-ES weight mode regenerates non-symmetric rows");
   constexpr int TY = kGradThreads / TX;
   if (gridDim.z > 1) {
     const int64_t item = blockIdx.z;
@@ -79,7 +90,7 @@ __global__ void __launch_bounds__(kGradThreads, EVOK_GRAD_MINB)
   float m[VEC], c1[VEC], c0[VEC], sg[VEC];
 #pragma unroll
   for (int c = 0; c < VEC; ++c) {
-    const bool ok = active && (col + c < D);
+    const bool ok = active && (col + c < D) && !SEPW;
     const float s = ok ? __ldg(sigma + col + c) : 1.0f;
     m[c] = ok ? __ldg(mu + col + c) : 0.0f;
     sg[c] = s;
@@ -101,6 +112,7 @@ __global__ void __launch_bounds__(kGradThreads, EVOK_GRAD_MINB)
 
   const int64_t r_begin = (int64_t)blockIdx.y * units_per_chunk;
   const int64_t r_end = min(n_units, r_begin + units_per_chunk);
+  float wb = 0.0f;  // SEPW: sum of this thread's b (rows in a fixed order)
 
   for (int64_t r0 = r_begin + ty; r0 < r_end; r0 += (int64_t)TY * kGradUnroll) {
     float a[kGradUnroll], b[kGradUnroll];
@@ -111,7 +123,13 @@ __global__ void __launch_bounds__(kGradThreads, EVOK_GRAD_MINB)
       const int64_t r = r0 + (int64_t)u * TY;
       a[u] = b[u] = 0.0f;
       if (r < r_end) {
-        if (SYM) {
+        if (SEPW) {
+          const float aw = __ldg(w + r);
+          a[u] = fmaxf(aw, 0.0f);
+          // q is read only for the negative weights: a zero-weight row is never regenerated and never looks at its norm
+          b[u] = (sepw.active && aw < 0.0f) ? __fdiv_rn((float)D * aw, __ldg(sepw.q + r)) : aw;
+          wb += b[u];
+        } else if (SYM) {
           const float wp = __ldg(w + 2 * r), wm = __ldg(w + 2 * r + 1);
           a[u] = 0.5f * (wp - wm);
           b[u] = 0.5f * (wp + wm);
@@ -184,12 +202,30 @@ __global__ void __launch_bounds__(kGradThreads, EVOK_GRAD_MINB)
       }
     }
   }
+  if (SEPW && blockIdx.x == 0) {  // uniform per CTA: every tile's row threads see the same rows, tile 0 reports their b sum
+    __shared__ float wred[TY];
+    if (tx == 0) wred[ty] = wb;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      float t = wred[0];
+      for (int y = 1; y < TY; ++y) t += wred[y];
+      sepw.wsum_partial[blockIdx.y] = t;
+    }
+  }
 }
 
+// WSUM: block 0 also adds the per-chunk sums of the separable CMA-ES weight mode, in chunk order, into *wsum_out
+template <bool WSUM = false>
 __global__ void __launch_bounds__(256) grad_finalize_kernel(const float* __restrict__ partial, int n_chunks, int64_t D, float scale_mu,
                                                             float scale_sigma, float* __restrict__ out_mu, float* __restrict__ out_sigma,
-                                                            int64_t item_stride_partial = 0) {
+                                                            int64_t item_stride_partial = 0, const float* __restrict__ wsum_partial = nullptr,
+                                                            float* __restrict__ wsum_out = nullptr) {
   const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (WSUM && j == 0) {
+    float t = 0.0f;
+    for (int c = 0; c < n_chunks; ++c) t += wsum_partial[c];
+    *wsum_out = t;
+  }
   if (j >= D) return;
   partial += (int64_t)blockIdx.y * item_stride_partial;  // batched: blockIdx.y = item, outputs contiguous [items][D]
   out_mu += (int64_t)blockIdx.y * D;
@@ -485,16 +521,17 @@ static GradPlan plan_grad(int64_t n_units, int64_t D, bool vec_ok) {
   return p;
 }
 
-template <int VEC, bool SYM, bool REGEN>
+template <int VEC, bool SYM, bool REGEN, bool SEPW = false>
 static void launch_partial(const GradPlan& p, int form, const float* X, int64_t ldx, const float* w, const float* mu, const float* sigma,
                            int64_t n_units, int64_t D, uint64_t unit0, uint64_t seed, uint64_t stream_id, const uint32_t* stream_off, float* partial,
-                           cudaStream_t st, int64_t n_items = 1, const GradItems* items = nullptr) {
+                           cudaStream_t st, int64_t n_items = 1, const GradItems* items = nullptr, const SepWeights* sep = nullptr) {
   dim3 grid(p.n_coltiles, p.n_chunks, (unsigned)n_items);
   const PhiloxKey key = make_philox_key(seed, stream_id);
   const GradItems it = items ? *items : GradItems{0, 0, 0, 0, 0};
-#define EVOK_LAUNCH_TX(TXV)                                                                                                         \
-  grad_partial_kernel<VEC, TXV, SYM, REGEN><<<grid, kGradThreads, 0, st>>>(form, X, ldx, w, mu, sigma, n_units, D, p.units_per_chunk, \
-                                                                           unit0, key, stream_off, partial, it)
+  const SepWeights sw = sep ? *sep : SepWeights{nullptr, 0, nullptr};
+#define EVOK_LAUNCH_TX(TXV)                                                                                                               \
+  grad_partial_kernel<VEC, TXV, SYM, REGEN, SEPW><<<grid, kGradThreads, 0, st>>>(form, X, ldx, w, mu, sigma, n_units, D, p.units_per_chunk, \
+                                                                                 unit0, key, stream_off, partial, it, sw)
   switch (p.tx) {
     case 32: EVOK_LAUNCH_TX(32); break;
     case 64: EVOK_LAUNCH_TX(64); break;
@@ -597,6 +634,29 @@ extern "C" EVOK_API int evok_grad_hybrid(int form, const float* X, int64_t ldx, 
                                          float scale_mu, float scale_sigma, float* out_mu, float* out_sigma, void* ws, size_t ws_bytes, void* stream) {
   return grad_impl(form, X, ldx, w, mu, sigma, row0, n_rows, D, false, seed, stream_id, stream_offset_dev, scale_mu, scale_sigma, out_mu, out_sigma, ws,
                    ws_bytes, stream, nullptr, split);
+}
+
+extern "C" EVOK_API size_t evok_sepcma_workspace_bytes(int64_t n_rows, int64_t D) {
+  // the gradient partials, then one float per row chunk (plan_grad: at most kNumSMs * EVOK_GRAD_CTAS_PER_SM chunks)
+  return evok_grad_workspace_bytes(n_rows, D) + (size_t)kMaxResidentCtas * sizeof(float);
+}
+
+extern "C" EVOK_API int evok_sepcma_moments(const float* aw, const float* q, int active, int64_t row0, int64_t n_rows, int64_t D, uint64_t seed,
+                                            uint64_t stream_id, const uint32_t* stream_offset_dev, float* local, float* S2, float* wsum, void* ws,
+                                            size_t ws_bytes, void* stream) {
+  if (!aw || (active && !q) || !local || !S2 || !wsum || !ws) return EVOK_E_NULLPTR;
+  if (n_rows <= 0 || D <= 0 || row0 < 0) return EVOK_E_BADSIZE;
+  if (ws_bytes < evok_sepcma_workspace_bytes(n_rows, D)) return EVOK_E_WORKSPACE;
+  cudaStream_t st = (cudaStream_t)stream;
+  const GradPlan p = plan_grad(n_rows, D, true);
+  float* partial = (float*)ws;
+  const SepWeights sep{q, active, partial + evok_grad_workspace_bytes(n_rows, D) / sizeof(float)};
+  launch_partial<4, false, true, true>(p, EVOK_GRAD_MOMENTS, nullptr, 0, aw, nullptr, nullptr, n_rows, D, (uint64_t)row0, seed, stream_id,
+                                       stream_offset_dev, partial, st, 1, nullptr, &sep);
+  EVOK_CHECK_LAUNCH();
+  grad_finalize_kernel<true><<<(unsigned)((D + 255) / 256), 256, 0, st>>>(partial, p.n_chunks, D, 1.0f, 1.0f, local, S2, 0, sep.wsum_partial, wsum);
+  EVOK_CHECK_LAUNCH();
+  return 0;
 }
 
 extern "C" EVOK_API int evok_grad_push(int form, const float* X, int64_t ldx, const float* w, const float* mu, const float* sigma, int64_t row0,

@@ -43,15 +43,19 @@ struct SampleTune {
   static constexpr int kMinBlocks = OBJ == EVOK_OBJ_NONE ? EVOK_SAMPLEONLY_MINB : EVOK_SAMPLE_MINB;
 };
 
-// one column group (4 columns) of one unit: sample, store, accumulate
-template <int OBJ, bool SYM, bool STORE, bool VEC>
+// one column group (4 columns) of one unit: sample, store, accumulate.  SQ: also *zsq += z^2 (the unscaled normals; the
+// squared norm that separable CMA-ES's active reweighting needs), in column order
+template <int OBJ, bool SYM, bool STORE, bool VEC, bool SQ = false>
 __device__ __forceinline__ void sample_group(const PhiloxKey& key, uint32_t sw, uint64_t unit, uint32_t q, int64_t D,
                                              const float* __restrict__ mu, const float* __restrict__ sigma, float* xp, float* xm,
-                                             ObjAcc<OBJ>& accp, ObjAcc<OBJ>& accm) {
+                                             ObjAcc<OBJ>& accp, ObjAcc<OBJ>& accm, float* zsq = nullptr) {
   float z[4];
   normals4(key, sw, unit, q, z);
   const int64_t j = (int64_t)q << 2;
   if (VEC) {
+    if (SQ) {
+      *zsq = fmaf(z[0], z[0], *zsq); *zsq = fmaf(z[1], z[1], *zsq); *zsq = fmaf(z[2], z[2], *zsq); *zsq = fmaf(z[3], z[3], *zsq);
+    }
     const float4 m = __ldg(reinterpret_cast<const float4*>(mu + j));
     const float4 s = __ldg(reinterpret_cast<const float4*>(sigma + j));
     const float p0 = fmaf(s.x, z[0], m.x), p1 = fmaf(s.y, z[1], m.y), p2 = fmaf(s.z, z[2], m.z), p3 = fmaf(s.w, z[3], m.w);
@@ -66,6 +70,7 @@ __device__ __forceinline__ void sample_group(const PhiloxKey& key, uint32_t sw, 
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
       if (j + c < D) {
+        if (SQ) *zsq = fmaf(z[c], z[c], *zsq);
         const float m = __ldg(mu + j + c), s = __ldg(sigma + j + c);
         const float p = fmaf(s, z[c], m);
         if (STORE) st_stream1(xp + j + c, p);
@@ -82,11 +87,14 @@ __device__ __forceinline__ void sample_group(const PhiloxKey& key, uint32_t sw, 
 
 // PUSH: the fitness of row i goes to row (row0 + i) of EVERY peer's fitness vector (the all-gather of the sharded
 // generation, fused into the producer) and the last CTA raises this rank's flag on every peer.
-template <int OBJ, bool SYM, bool STORE, bool VEC, bool PUSH>
+// SQ (non-symmetric only): q[r] = sum_j z_rj^2 of the unscaled normals, accumulated in registers next to the objective.
+template <int OBJ, bool SYM, bool STORE, bool VEC, bool PUSH, bool SQ = false>
 __global__ void __launch_bounds__(kSampleThreads, SampleTune<OBJ>::kMinBlocks)
     sample_eval_kernel(float* __restrict__ X, int64_t ldx, const float* __restrict__ mu, const float* __restrict__ sigma,
                        int64_t row0, int64_t n_units, int64_t D, const __grid_constant__ PhiloxKey key, const uint32_t* __restrict__ stream_off,
-                       float* __restrict__ f, const __grid_constant__ PeerSink sink, const unsigned long long* epoch, unsigned int* done) {
+                       float* __restrict__ f, const __grid_constant__ PeerSink sink, const unsigned long long* epoch, unsigned int* done,
+                       float* __restrict__ q_out) {
+  static_assert(!(SQ && (SYM || PUSH)), "the squared norms are produced by the plain non-symmetric sampler only");
   const int lane = threadIdx.x & 31;
   const uint32_t sw = key.stream_lo + (stream_off ? __ldg(stream_off) : 0u);
   const int64_t warps_total = (int64_t)gridDim.x * (kSampleThreads / 32);
@@ -101,16 +109,21 @@ __global__ void __launch_bounds__(kSampleThreads, SampleTune<OBJ>::kMinBlocks)
     float* xm = STORE ? xp + ldx : nullptr;
     const uint64_t unit = unit0 + (uint64_t)u;
     constexpr int kSampleUnroll = SampleTune<OBJ>::kUnroll;
+    float zsq = 0.f;
     uint32_t q = lane;
     if (kSampleUnroll > 1) {
       // independent Philox chains in flight per lane
       for (; q + 32u * (kSampleUnroll - 1) < nq; q += 32u * kSampleUnroll) {
 #pragma unroll
         for (int uu = 0; uu < kSampleUnroll; ++uu)
-          sample_group<OBJ, SYM, STORE, VEC>(key, sw, unit, q + 32u * uu, D, mu, sigma, xp, xm, accp, accm);
+          sample_group<OBJ, SYM, STORE, VEC, SQ>(key, sw, unit, q + 32u * uu, D, mu, sigma, xp, xm, accp, accm, &zsq);
       }
     }
-    for (; q < nq; q += 32) sample_group<OBJ, SYM, STORE, VEC>(key, sw, unit, q, D, mu, sigma, xp, xm, accp, accm);
+    for (; q < nq; q += 32) sample_group<OBJ, SYM, STORE, VEC, SQ>(key, sw, unit, q, D, mu, sigma, xp, xm, accp, accm, &zsq);
+    if (SQ) {
+      zsq = warp_sum(zsq);
+      if (lane == 0) q_out[r] = zsq;
+    }
     if (OBJ != EVOK_OBJ_NONE) {
       const float fp = accp.finish(D);
       float fm = 0.f;
@@ -207,10 +220,10 @@ struct PushArgs {
   unsigned int* done;
 };
 
-template <int OBJ, bool SYM, bool STORE, bool PUSH = false>
+template <int OBJ, bool SYM, bool STORE, bool PUSH = false, bool SQ = false>
 static int launch_sample(float* X, int64_t ldx, const float* mu, const float* sigma, int64_t row0, int64_t n_rows, int64_t D,
                          uint64_t seed, uint64_t stream_id, const uint32_t* stream_off, float* f, cudaStream_t st,
-                         const PushArgs* push = nullptr) {
+                         const PushArgs* push = nullptr, float* q = nullptr) {
   const int64_t n_units = SYM ? n_rows / 2 : n_rows;
   const bool vec = (D % 4 == 0) && aligned16(mu) && aligned16(sigma) && (!STORE || (aligned16(X) && ldx % 4 == 0));
   const int64_t ctas_needed = (n_units + (kSampleThreads / 32) - 1) / (kSampleThreads / 32);
@@ -218,13 +231,13 @@ static int launch_sample(float* X, int64_t ldx, const float* mu, const float* si
   PushArgs none{};
   const PushArgs& pa = PUSH ? *push : none;
   if (vec) {
-    auto k = sample_eval_kernel<OBJ, SYM, STORE, true, PUSH>;
+    auto k = sample_eval_kernel<OBJ, SYM, STORE, true, PUSH, SQ>;
     k<<<resident_grid(k, kSampleThreads, ctas_needed), kSampleThreads, 0, st>>>(X, ldx, mu, sigma, row0, n_units, D, key, stream_off, f, pa.sink,
-                                                                                pa.epoch, pa.done);
+                                                                                pa.epoch, pa.done, q);
   } else {
-    auto k = sample_eval_kernel<OBJ, SYM, STORE, false, PUSH>;
+    auto k = sample_eval_kernel<OBJ, SYM, STORE, false, PUSH, SQ>;
     k<<<resident_grid(k, kSampleThreads, ctas_needed), kSampleThreads, 0, st>>>(X, ldx, mu, sigma, row0, n_units, D, key, stream_off, f, pa.sink,
-                                                                                pa.epoch, pa.done);
+                                                                                pa.epoch, pa.done, q);
   }
   EVOK_CHECK_LAUNCH();
   return 0;
@@ -239,6 +252,14 @@ static int dispatch_sample(float* X, int64_t ldx, const float* mu, const float* 
   }
   return X ? launch_sample<OBJ, false, true>(X, ldx, mu, sigma, row0, n_rows, D, seed, stream_id, stream_off, f, st)
            : launch_sample<OBJ, false, false>(X, ldx, mu, sigma, row0, n_rows, D, seed, stream_id, stream_off, f, st);
+}
+
+template <int OBJ>
+static int dispatch_sample_sq(float* X, int64_t ldx, const float* mu, const float* sigma, int64_t row0, int64_t n_rows, int64_t D, uint64_t seed,
+                              uint64_t stream_id, const uint32_t* stream_off, float* f, float* q, cudaStream_t st) {
+  if (X) return launch_sample<OBJ, false, true, false, true>(X, ldx, mu, sigma, row0, n_rows, D, seed, stream_id, stream_off, f, st, nullptr, q);
+  if constexpr (OBJ == EVOK_OBJ_NONE) return EVOK_E_NULLPTR;  // rejected by the entry point: no kernel for "q only"
+  else return launch_sample<OBJ, false, false, false, true>(X, ldx, mu, sigma, row0, n_rows, D, seed, stream_id, stream_off, f, st, nullptr, q);
 }
 
 template <int OBJ>
@@ -288,6 +309,25 @@ extern "C" EVOK_API int evok_sample_eval(int objective, float* X, int64_t ldx, c
     case EVOK_OBJ_SPHERE: return dispatch_sample<EVOK_OBJ_SPHERE>(X, ldx, mu, sigma, row0, n_rows, D, symmetric, seed, stream_id, stream_off, f, st);
     case EVOK_OBJ_RASTRIGIN: return dispatch_sample<EVOK_OBJ_RASTRIGIN>(X, ldx, mu, sigma, row0, n_rows, D, symmetric, seed, stream_id, stream_off, f, st);
     case EVOK_OBJ_ACKLEY: return dispatch_sample<EVOK_OBJ_ACKLEY>(X, ldx, mu, sigma, row0, n_rows, D, symmetric, seed, stream_id, stream_off, f, st);
+  }
+  return EVOK_E_BADENUM;
+}
+
+extern "C" EVOK_API int evok_sample_eval_sq(int objective, float* X, int64_t ldx, const float* mu, const float* sigma, int64_t row0, int64_t n_rows,
+                                            int64_t D, uint64_t seed, uint64_t stream_id, const uint32_t* stream_offset_dev, float* f, float* q,
+                                            void* stream) {
+  if (!mu || !sigma || !q) return EVOK_E_NULLPTR;
+  if (objective < 0 || objective >= EVOK_OBJ_COUNT) return EVOK_E_BADENUM;
+  if (objective == EVOK_OBJ_NONE && !X) return EVOK_E_NULLPTR;
+  if (objective != EVOK_OBJ_NONE && !f) return EVOK_E_NULLPTR;
+  if (n_rows < 0 || D <= 0 || row0 < 0 || (X && ldx < D)) return EVOK_E_BADSIZE;
+  if (n_rows == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  switch (objective) {
+    case EVOK_OBJ_NONE: return dispatch_sample_sq<EVOK_OBJ_NONE>(X, ldx, mu, sigma, row0, n_rows, D, seed, stream_id, stream_offset_dev, f, q, st);
+    case EVOK_OBJ_SPHERE: return dispatch_sample_sq<EVOK_OBJ_SPHERE>(X, ldx, mu, sigma, row0, n_rows, D, seed, stream_id, stream_offset_dev, f, q, st);
+    case EVOK_OBJ_RASTRIGIN: return dispatch_sample_sq<EVOK_OBJ_RASTRIGIN>(X, ldx, mu, sigma, row0, n_rows, D, seed, stream_id, stream_offset_dev, f, q, st);
+    case EVOK_OBJ_ACKLEY: return dispatch_sample_sq<EVOK_OBJ_ACKLEY>(X, ldx, mu, sigma, row0, n_rows, D, seed, stream_id, stream_offset_dev, f, q, st);
   }
   return EVOK_E_BADENUM;
 }

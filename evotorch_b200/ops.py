@@ -262,6 +262,91 @@ def cmaes_vector_update(local_disp: torch.Tensor, shaped_disp: torch.Tensor, m: 
                                                  nat.ptr(h_sig_out), nat.stream_of(m)), "evok_cmaes_vector_update")
 
 
+def sample_eval_sq(objective: int, X: Optional[torch.Tensor], mu: torch.Tensor, sigma: torch.Tensor, q: torch.Tensor, *, n_rows: int,
+                   seed: int, stream_id: int, row0: int = 0, f: Optional[torch.Tensor] = None,
+                   stream_offset: Optional[torch.Tensor] = None) -> None:
+    """`sample_eval` (non-symmetric) that also writes q[i] = ||z_i||^2 of the unscaled normals; X / f are the same bits as
+    `sample_eval` with the same arguments.  X = None: lazy population (needs a built-in objective)."""
+    D = mu.numel()
+    _vec(mu, "mu"); _vec(sigma, "sigma", D); _vec(q, "q", n_rows)
+    ldx = 0
+    if X is not None:
+        _mat(X, "X")
+        if X.shape != (n_rows, D):
+            raise ValueError(f"X: expected shape {(n_rows, D)}, got {tuple(X.shape)}")
+        ldx = X.stride(0)
+    elif objective == OBJ_NONE:
+        raise ValueError("X: the samples must be written somewhere when no objective is fused into the sampler")
+    if f is not None:
+        _vec(f, "f", n_rows)
+    if objective != OBJ_NONE and f is None:
+        raise ValueError("f: a fitness buffer is required when an objective is fused into the sampler")
+    if n_rows == 0:
+        return
+    with _timed("sepcma_sample"):
+        rc = nat.lib().evok_sample_eval_sq(objective, nat.ptr(X), ldx, mu.data_ptr(), sigma.data_ptr(), row0, n_rows, D,
+                                           seed & 0xFFFFFFFFFFFFFFFF, stream_id & 0xFFFFFFFFFFFFFFFF, _offset_ptr(stream_offset), nat.ptr(f),
+                                           q.data_ptr(), nat.stream_of(mu))
+    nat.check(rc, "evok_sample_eval_sq")
+
+
+def sepcma_moments(aw: torch.Tensor, q: Optional[torch.Tensor], active: bool, D: int, *, seed: int, stream_id: int, row0: int = 0,
+                   stream_offset: Optional[torch.Tensor] = None, local: Optional[torch.Tensor] = None, S2: Optional[torch.Tensor] = None,
+                   wsum: Optional[torch.Tensor] = None) -> tuple:
+    """Separable CMA-ES moments over the population that `sample_eval_sq` drew with the same (seed, stream_id, row0, stream_offset),
+    regenerated from Philox: local = sum_i a_i z_i, S2 = sum_i b_i z_i^2, wsum = sum_i b_i (1 element), with a_i = max(aw_i, 0) and
+    b_i = aw_i, or with `active` b_i = aw_i > 0 ? aw_i : D aw_i / q_i.  Returns (local, S2, wsum)."""
+    n = aw.numel()
+    _vec(aw, "aw")
+    if active:
+        if q is None:
+            raise ValueError("q: the squared norms are required with active weights")
+        _vec(q, "q", n)
+    dev = aw.device
+    local = torch.empty(D, dtype=torch.float32, device=dev) if local is None else _vec(local, "local", D)
+    S2 = torch.empty(D, dtype=torch.float32, device=dev) if S2 is None else _vec(S2, "S2", D)
+    wsum = torch.empty(1, dtype=torch.float32, device=dev) if wsum is None else _vec(wsum, "wsum", 1)
+    ws = nat.workspace(dev, nat.lib().evok_sepcma_workspace_bytes(n, D), "grad")
+    with _timed("sepcma_moments"):
+        rc = nat.lib().evok_sepcma_moments(aw.data_ptr(), nat.ptr(q), int(bool(active)), row0, n, D, seed & 0xFFFFFFFFFFFFFFFF,
+                                           stream_id & 0xFFFFFFFFFFFFFFFF, _offset_ptr(stream_offset), local.data_ptr(), S2.data_ptr(),
+                                           wsum.data_ptr(), ws.data_ptr(), ws.numel(), nat.stream_of(aw))
+    nat.check(rc, "evok_sepcma_moments")
+    return local, S2, wsum
+
+
+def sepcma_update(local: torch.Tensor, S2: torch.Tensor, wsum: torch.Tensor, m: torch.Tensor, p_sigma: torch.Tensor, p_c: torch.Tensor,
+                  sigma: torch.Tensor, C: torch.Tensor, A: torch.Tensor, s: torch.Tensor, consts, csa_squared: bool, *, decompose_C_freq: int,
+                  steps: int = 0, steps_dev: Optional[torch.Tensor] = None, stdev_min: Optional[float] = None, stdev_max: Optional[float] = None,
+                  m_prev: Optional[torch.Tensor] = None, s_prev: Optional[torch.Tensor] = None, h_sig_out: Optional[torch.Tensor] = None) -> None:
+    """In place, one kernel: m, p_sigma, sigma (1-element tensor), p_c, C, A (diagonal, D-vectors) and s = sigma * A after one separable
+    CMA-ES generation with the given moments (see `sepcma_moments`).  `consts` as for `cmaes_vector_update`.  m_prev / s_prev receive
+    m and s from before the update."""
+    import ctypes
+
+    d = m.numel()
+    _vec(local, "local", d); _vec(S2, "S2", d); _vec(wsum, "wsum", 1); _vec(m, "m"); _vec(p_sigma, "p_sigma", d); _vec(p_c, "p_c", d)
+    _vec(C, "C", d); _vec(A, "A", d); _vec(s, "s", d)
+    for t, name in ((m_prev, "m_prev"), (s_prev, "s_prev")):
+        if t is not None:
+            _vec(t, name, d)
+    if not (sigma.is_cuda and sigma.dtype == torch.float32 and sigma.numel() == 1):
+        raise ValueError("sigma: expected a 1-element float32 CUDA tensor")
+    if steps_dev is not None and not (steps_dev.is_cuda and steps_dev.dtype == torch.int64 and steps_dev.numel() == 1):
+        raise ValueError("steps_dev: expected a 1-element int64 CUDA tensor")
+    if int(decompose_C_freq) < 1:
+        raise ValueError("decompose_C_freq: expected a positive integer")
+    carr = (ctypes.c_float * 10)(*[float(x) for x in consts])
+    lo = NAN if stdev_min is None else float(stdev_min)
+    hi = NAN if stdev_max is None else float(stdev_max)
+    with _timed("sepcma_update"):
+        rc = nat.lib().evok_sepcma_update(local.data_ptr(), S2.data_ptr(), wsum.data_ptr(), d, m.data_ptr(), p_sigma.data_ptr(), p_c.data_ptr(),
+                                          sigma.data_ptr(), C.data_ptr(), A.data_ptr(), s.data_ptr(), nat.ptr(m_prev), nat.ptr(s_prev),
+                                          nat.ptr(steps_dev), int(steps), carr, int(bool(csa_squared)), int(decompose_C_freq), lo, hi,
+                                          nat.ptr(h_sig_out), nat.stream_of(m))
+    nat.check(rc, "evok_sepcma_update")
+
+
 def weights_adjust_(w: torch.Tensor, mode: int) -> torch.Tensor:
     _vec(w, "weights")
     nat.check(nat.lib().evok_weights_adjust(w.data_ptr(), w.numel(), mode, nat.stream_of(w)), "evok_weights_adjust")

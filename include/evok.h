@@ -303,6 +303,33 @@ int evok_cmaes_vector_update(const float* local_disp, const float* shaped_disp, 
                              int64_t* steps_dev, int64_t steps_host, const float* consts_host, int csa_squared, float* k_out, float* h_sig_out,
                              void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Separable CMA-ES (diagonal C, algorithms/cmaes.py with separable=True) as three kernels plus evok_rank_table, with no host
+ * reads.  With s = sigma * A (the per-column stdev of the sampler) one generation is
+ *   evok_sample_eval_sq : x_i = fmaf(s, z_i, m) (X nullable: lazy population), f_i = objective(x_i), q_i = ||z_i||^2
+ *   evok_rank_table     : aw = weights[rank(f)]
+ *   evok_sepcma_moments : regenerates z_i from Philox and reduces local = sum_i a_i z_i, S2 = sum_i b_i z_i^2, wsum = sum_i b_i with
+ *                         a_i = max(aw_i, 0), b_i = active ? (aw_i > 0 ? aw_i : D aw_i / q_i) : aw_i   (cmaes.py:454-481, :519-535);
+ *                         rows with a_i = b_i = 0 are not regenerated (their q_i is not read).  Fixed summation order, no atomics.
+ *   evok_sepcma_update  : m, p_sigma, sigma, h_sig, p_c (the arithmetic of evok_cmaes_vector_update, with shaped = A * local), then
+ *                         C <- C + c1a (p_c^2 - C) + c_mu (A^2 S2 - wsum C) (cmaes.py:536-545, separable branch), the stdev bounds
+ *                         with the new sigma (cmaes.py:49-79; NaN = no bound), A <- sqrt(C) when (steps + 1) % decompose_C_freq == 0,
+ *                         s <- sigma A.  One CTA.  m_prev / s_prev (nullable) receive m and s before the update: the centre and stdev
+ *                         the population of this generation was drawn from.  Step counter as in evok_cmaes_vector_update.
+ * --------------------------------------------------------------------------------------------- */
+/* evok_sample_eval for a non-symmetric population that also writes q[i] = sum_j z_ij^2 of the unscaled normals.  X and f are
+ * bit-identical to evok_sample_eval with the same arguments.  objective may be EVOK_OBJ_NONE only when X is given. */
+int evok_sample_eval_sq(int objective, float* X, int64_t ldx, const float* mu, const float* sigma, int64_t row0, int64_t n_rows, int64_t D,
+                        uint64_t seed, uint64_t stream_id, const uint32_t* stream_offset_dev, float* f, float* q, void* stream);
+size_t evok_sepcma_workspace_bytes(int64_t n_rows, int64_t D);
+/* aw: the n_rows assigned weights; q: nullable when active == 0; (seed, stream_id, stream_offset_dev, row0) as for the sampler */
+int evok_sepcma_moments(const float* aw, const float* q, int active, int64_t row0, int64_t n_rows, int64_t D, uint64_t seed, uint64_t stream_id,
+                        const uint32_t* stream_offset_dev, float* local, float* S2, float* wsum, void* ws, size_t ws_bytes, void* stream);
+/* consts_host: the 10 floats of evok_cmaes_vector_update (the last one, sum(weights), is not used: wsum comes from the device) */
+int evok_sepcma_update(const float* local, const float* S2, const float* wsum, int64_t D, float* m, float* p_sigma, float* p_c, float* sigma_dev,
+                       float* C, float* A, float* s, float* m_prev, float* s_prev, int64_t* steps_dev, int64_t steps_host, const float* consts_host,
+                       int csa_squared, int64_t decompose_C_freq, float stdev_min, float stdev_max, float* h_sig_out, void* stream);
+
 /* Cholesky factorisation A = L L^T (fp32, lower; the strictly upper part of L is zeroed, like torch.linalg.cholesky).  Replaces
  * CMAES.decompose_C (cmaes.py:555-565, torch.linalg.cholesky -> cuSOLVER potrf).  ONE persistent kernel: 64 x 64 tiles, left-looking
  * tile dataflow with per-tile release / acquire flags instead of a launch (or grid barrier) per panel step.  Only the lower triangle
