@@ -31,7 +31,8 @@ import torch
 
 from .. import ops
 from ..core import LazySolutionBatch, PhiloxRecipe, Problem, Solution, SolutionBatch
-from .searchalgorithm import SearchAlgorithm, SinglePopulationAlgorithmMixin
+from .cudagraph import GenerationGraph
+from .searchalgorithm import CUDAGraphMixin, SearchAlgorithm, SinglePopulationAlgorithmMixin
 
 
 def _safe_divide(a, b):
@@ -41,7 +42,7 @@ def _safe_divide(a, b):
     return a / b
 
 
-class CMAES(SearchAlgorithm, SinglePopulationAlgorithmMixin):
+class CMAES(SearchAlgorithm, SinglePopulationAlgorithmMixin, CUDAGraphMixin):
     def __init__(self, problem: Problem, *, stdev_init, popsize: Optional[int] = None, center_init=None, c_m: float = 1.0,
                  c_sigma: Optional[float] = None, c_sigma_ratio: float = 1.0, damp_sigma: Optional[float] = None,
                  damp_sigma_ratio: float = 1.0, c_c: Optional[float] = None, c_c_ratio: float = 1.0, c_1: Optional[float] = None,
@@ -136,7 +137,7 @@ class CMAES(SearchAlgorithm, SinglePopulationAlgorithmMixin):
             self.decompose_C_freq = max(1, int(np.floor(_safe_divide(1, 10 * d * (self.c_1 + self.c_mu)))))
         else:
             self.decompose_C_freq = 1
-        self._use_graph, self._graph = os.environ.get("EVOTORCH_B200_CUDA_GRAPH", "0") == "1", None
+        CUDAGraphMixin.__init__(self)
         SinglePopulationAlgorithmMixin.__init__(self)
 
     # ------------------------------------------------------------------ accessors
@@ -286,42 +287,37 @@ class CMAES(SearchAlgorithm, SinglePopulationAlgorithmMixin):
 
     def _fused_state(self) -> dict:
         fs = self.__dict__.get("_fused")
-        if fs is None and self.separable:
-            n, d, dev = self.popsize, self._problem.solution_length, self.m.device
-            new = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=dev)  # noqa: E731
+        if fs is not None:
+            return fs
+        p, n, d, dev = self._problem, self.popsize, self._problem.solution_length, self.m.device
+        new = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=dev)  # noqa: E731
+        if self.separable:
             lazy = isinstance(self._population, LazySolutionBatch)
             # m_draw / s_draw: the centre and stdev the current (lazy) population was drawn from, written by the update kernel
-            fs = self._fused = dict(q=new(n), aw=new(n), local=new(d), S2=new(d), wsum=new(1), m_draw=new(d) if lazy else None,
-                                    s_draw=new(d) if lazy else None, steps_dev=None)
-            self.m, self.p_sigma, self.p_c = self.m.contiguous().clone(), self.p_sigma.contiguous().clone(), self.p_c.contiguous().clone()
-            self.sigma = self.sigma.reshape(()).clone()
-            self.C, self.A = self.C.contiguous().clone(), self.A.contiguous().clone()
+            fs = dict(q=new(n), aw=new(n), local=new(d), S2=new(d), wsum=new(1), m_draw=new(d) if lazy else None, s_draw=new(d) if lazy else None)
+        else:
+            fs = dict(zs=new(n, d), ys=new(n, d), aw=new(n), w_pos=new(n), w_act=new(n), local=new(d), shaped=new(d), scratch=new(d), k=new(3),
+                      zero=p.make_zeros(d), one=p.make_ones(d), info=torch.zeros((), dtype=torch.int32, device=dev))
+        # state tensors become persistent buffers that the kernels update in place (pointer-stable: CUDA-graph replay)
+        self.m, self.p_sigma, self.p_c = self.m.contiguous().clone(), self.p_sigma.contiguous().clone(), self.p_c.contiguous().clone()
+        self.sigma = self.sigma.reshape(()).clone()
+        self.C, self.A = self.C.contiguous().clone(), self.A.contiguous().clone()
+        if self.separable:
             fs["s"] = (self.sigma * self.A).contiguous()  # the sampler's per-column stdev; the update kernel keeps it = sigma * A
-            self._consts = (self.c_m, self.c_sigma, self.damp_sigma, self.c_c, self.c_1, self.c_mu, self.variance_discount_sigma,
-                            self.variance_discount_c, float(self.unbiased_expectation), self._weights_sum)
-        elif fs is None:
-            p, n, d = self._problem, self.popsize, self._problem.solution_length
-            dev = self.m.device
-            new = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=dev)  # noqa: E731
-            fs = self._fused = dict(zs=new(n, d), ys=new(n, d), aw=new(n), w_pos=new(n), w_act=new(n), local=new(d), shaped=new(d), scratch=new(d),
-                                    k=new(3), zero=p.make_zeros(d), one=p.make_ones(d), info=torch.zeros((), dtype=torch.int32, device=dev),
-                                    steps_dev=None)
-            # state tensors become persistent buffers that the kernels update in place (pointer-stable: CUDA-graph replay)
-            self.m, self.p_sigma, self.p_c = self.m.contiguous().clone(), self.p_sigma.contiguous().clone(), self.p_c.contiguous().clone()
-            self.sigma = self.sigma.reshape(()).clone()
-            self.C, self.A = self.C.contiguous().clone(), self.A.contiguous().clone()
-            self._consts = (self.c_m, self.c_sigma, self.damp_sigma, self.c_c, self.c_1, self.c_mu, self.variance_discount_sigma,
-                            self.variance_discount_c, float(self.unbiased_expectation), self._weights_sum)
+        self._consts = (self.c_m, self.c_sigma, self.damp_sigma, self.c_c, self.c_1, self.c_mu, self.variance_discount_sigma,
+                        self.variance_discount_c, float(self.unbiased_expectation), self._weights_sum)
+        self._fused = fs
         return fs
 
-    def _step_fused(self):
+    def _step_fused(self, steps_dev: Optional[torch.Tensor] = None):
         """One generation as a short chain of kernels with no host reads (cmaes.py:567-606):
         K1 z-sampling -> GEMM (Y = Z A^T, X = m + sigma Y straight into the population) -> evaluate -> rank-to-weights (K3, one launch)
         -> row weights (positive part / active reweighting, one pass over Z) -> two weighted row sums (K4) -> fused vector update
         (m, p_sigma, sigma, h_sig, p_c + the covariance coefficients) -> weighted SYRK with the covariance update in its epilogue ->
-        Cholesky.  Every state tensor is updated in place."""
+        Cholesky.  Every state tensor is updated in place.  Under a CUDA-graph capture `steps_dev` is the device-side step
+        counter that the vector update reads and increments (`_h_sig`, the decomposition schedule); eager steps use `_steps_count`."""
         if self.separable:
-            self._step_sep_fused()
+            self._step_sep_fused(steps_dev)
             return
         fs = self._fused_state()
         zs, ys, xs = self.sample_distribution()
@@ -337,16 +333,16 @@ class CMAES(SearchAlgorithm, SinglePopulationAlgorithmMixin):
         ops.grad(ops.GRAD_MOMENTS, zs, fs["w_pos"], fs["zero"], fs["one"], 1.0, 1.0, out_mu=fs["local"], out_sigma=fs["scratch"])
         ops.grad(ops.GRAD_MOMENTS, ys, fs["w_pos"], fs["zero"], fs["one"], 1.0, 1.0, out_mu=fs["shaped"], out_sigma=fs["scratch"])
         ops.cmaes_vector_update(fs["local"], fs["shaped"], self.m, self.p_sigma, self.p_c, self.sigma, self._consts, self.csa_squared, fs["k"],
-                                steps=self._steps_count, steps_dev=fs["steps_dev"])
+                                steps=self._steps_count, steps_dev=steps_dev)
         ops.weighted_syrk_update(ys, fs["w_act"], fs["k"], self.C, u=self.p_c, out=self.C)
-        if fs["steps_dev"] is not None or (self._steps_count + 1) % self.decompose_C_freq == 0:
+        if steps_dev is not None or (self._steps_count + 1) % self.decompose_C_freq == 0:
             if os.environ.get("EVOTORCH_B200_EVOK_CHOLESKY", "0") == "1":
                 ops.cholesky(self.C, out=self.A)  # the repo's own tile-dataflow kernel (csrc/evok_chol.cu): correct, but
                 # its diagonal-tile factorisations are a serial critical path, so cuSOLVER's potrf stays the default
             else:
                 torch.linalg.cholesky_ex(self.C, check_errors=False, out=(self.A, fs["info"]))
 
-    def _step_sep_fused(self):
+    def _step_sep_fused(self, steps_dev: Optional[torch.Tensor] = None):
         """One separable generation (cmaes.py:567-606 with diagonal C) as four kernels with no host reads.  With s = sigma * A:
         sample x_i = m + s z_i and evaluate it in one pass that also keeps q_i = ||z_i||^2 (the population is written once, or not
         at all when it is lazy) -> rank-to-weights -> the moments sum a_i z_i, sum b_i z_i^2, sum b_i over z regenerated from the
@@ -378,7 +374,7 @@ class CMAES(SearchAlgorithm, SinglePopulationAlgorithmMixin):
         ops.sepcma_moments(fs["aw"], fs["q"], self.active, d, seed=seed, stream_id=stream_id, stream_offset=offset, local=fs["local"], S2=fs["S2"],
                            wsum=fs["wsum"])
         ops.sepcma_update(fs["local"], fs["S2"], fs["wsum"], self.m, self.p_sigma, self.p_c, self.sigma, self.C, self.A, fs["s"], self._consts,
-                          self.csa_squared, decompose_C_freq=self.decompose_C_freq, steps=self._steps_count, steps_dev=fs["steps_dev"],
+                          self.csa_squared, decompose_C_freq=self.decompose_C_freq, steps=self._steps_count, steps_dev=steps_dev,
                           stdev_min=self.stdev_min, stdev_max=self.stdev_max, m_prev=fs["m_draw"], s_prev=fs["s_draw"])
         if lazy:
             # from here on the population is the one drawn from the snapshots.  Under a CUDA graph the stream offset counter is
@@ -387,71 +383,39 @@ class CMAES(SearchAlgorithm, SinglePopulationAlgorithmMixin):
                                       symmetric=False, stream_offset=offset, mu=fs["m_draw"], sigma=fs["s_draw"])
 
     # ------------------------------------------------------------------ CUDA-graph replay of the fused generation
-    def enable_cuda_graph(self, enabled: bool = True):
-        """Capture the fused generation into a CUDA graph and replay it from `step()` (one graph launch per generation; the
-        z-sampler reads a device-side generation counter, `_h_sig` a device-side step counter, so the replayed trajectory equals
-        eager stepping).  Used when the configuration is capturable: fused path, built-in objective, no evaluation hooks, and for
-        the full covariance a Cholesky every generation (`decompose_C_freq == 1`; the separable update kernel reads the step
-        counter itself, so it replays at any frequency); otherwise stepping stays eager."""
-        self._use_graph = bool(enabled)
-        self._graph = None
-        return self
-
     def _graph_capturable(self) -> bool:
+        """The fused path with a built-in objective and no evaluation hooks, and for the full covariance a Cholesky every
+        generation (`decompose_C_freq == 1`; the separable update kernel schedules the decomposition from the device-side step
+        counter, so it replays at any frequency)."""
         prob = self._problem
         return (self._fused_ok() and (self.separable or self.decompose_C_freq == 1) and prob.evok_objective_id is not None
                 and len(prob.before_eval_hook) == 0 and len(prob.after_eval_hook) == 0 and not prob.stores_solution_stats
                 and "sample_distribution" not in self.__dict__)
 
     def _step_graph(self):
-        from .. import _native as nat
-
-        prob = self._problem
         if self._graph is None:
             self._step_fused()  # warm every kernel / workspace / cuSOLVER handle eagerly, right before the capture
-            fs = self._fused_state()
-            prob.philox_stream_offset = torch.zeros(1, dtype=torch.int32, device=self.m.device)
-            fs["steps_dev"] = torch.full((1,), self._steps_count + 1, dtype=torch.int64, device=self.m.device)
-            base = prob._philox_stream
-            torch.cuda.synchronize()
-            graph = torch.cuda.CUDAGraph()
-            before = ops.launch_count()
+            steps_dev = torch.full((1,), self._steps_count + 1, dtype=torch.int64, device=self.m.device)
             try:
-                with nat.private_workspaces() as store, torch.cuda.graph(graph):
-                    self._step_fused()
-                    prob.philox_stream_offset.add_(1)
+                self._graph = GenerationGraph(self._problem, lambda: self._step_fused(steps_dev), buffers=(steps_dev,))
             except Exception:  # e.g. a library call inside the step that cannot be captured on this build: stay eager
-                prob.philox_stream_offset, fs["steps_dev"] = None, None
-                prob._philox_stream = base
                 self._use_graph = False
                 torch.cuda.synchronize()
-                return
-            self._graph_kernels = ops.launch_count() - before
-            ops.count_replayed_launches(-self._graph_kernels)
-            prob._philox_stream = base  # the capture consumed a host-side stream id without running anything
-            prob.philox_stream_offset.zero_()
-            self._graph, self._graph_workspaces = graph, store
             return
         self._graph.replay()
-        ops.count_replayed_launches(self._graph_kernels)
-        prob._philox_stream += 1
 
     def __getstate__(self) -> dict:
-        state = dict(self.__dict__)
-        state["_graph"] = None
-        state.pop("_graph_workspaces", None)
+        state = super().__getstate__()
         if state.get("_fused") is not None:
             state["_fused"] = None  # scratch buffers are rebuilt on the first step after loading
         return state
 
     def _step(self):
         if self._fused_ok():
-            if self.__dict__.get("_use_graph") and self._graph_capturable():
+            if self._use_graph and self._graph_capturable():
                 self._step_graph()
             else:
                 self._graph = None
-                if self.__dict__.get("_fused") is not None and self._fused.get("steps_dev") is not None:
-                    self._fused["steps_dev"], self._problem.philox_stream_offset = None, None
                 self._step_fused()
             return
         if self.separable:

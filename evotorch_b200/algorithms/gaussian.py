@@ -25,10 +25,11 @@ from ..distributed import world
 from ..distributions import Distribution, ExpGaussian, ExpSeparableGaussian, SeparableGaussian, SymmetricSeparableGaussian
 from ..optimizers import get_optimizer_class
 from ..tools.misc import modify_tensor, to_stdev_init
-from .searchalgorithm import SearchAlgorithm, SinglePopulationAlgorithmMixin
+from .cudagraph import GenerationGraph
+from .searchalgorithm import CUDAGraphMixin, SearchAlgorithm, SinglePopulationAlgorithmMixin
 
 
-class GaussianSearchAlgorithm(SearchAlgorithm, SinglePopulationAlgorithmMixin):
+class GaussianSearchAlgorithm(SearchAlgorithm, SinglePopulationAlgorithmMixin, CUDAGraphMixin):
     """Base class of the Gaussian-distribution searchers (gaussian.py:35-501)."""
 
     DISTRIBUTION_TYPE = NotImplemented
@@ -92,8 +93,7 @@ class GaussianSearchAlgorithm(SearchAlgorithm, SinglePopulationAlgorithmMixin):
         self._mean_eval = None
         self._population: Optional[SolutionBatch] = None
         self._first_iter = True
-        self._use_graph = os.environ.get("EVOTORCH_B200_CUDA_GRAPH", "0") == "1"
-        self._graph = None
+        CUDAGraphMixin.__init__(self)
         SinglePopulationAlgorithmMixin.__init__(self, exclude="mean_eval", enable=(not self._distributed))
 
     def _initialize_optimizer(self, learning_rate: float, optimizer=None, optimizer_config: Optional[dict] = None):
@@ -104,14 +104,6 @@ class GaussianSearchAlgorithm(SearchAlgorithm, SinglePopulationAlgorithmMixin):
             return cls(stepsize=float(learning_rate), dtype=self._distribution.dtype, solution_length=self._distribution.solution_length,
                        device=self._distribution.device)
         return optimizer
-
-    # ------------------------------------------------------------------ pickling (checkpoints: logging.PicklingLogger(checkpoint=True))
-    def __getstate__(self) -> dict:
-        """Everything but the captured CUDA graph (re-captured on the first step after loading)."""
-        state = dict(self.__dict__)
-        state["_graph"] = None
-        state.pop("_graph_workspaces", None)
-        return state
 
     # ------------------------------------------------------------------ generations
     def _fill_and_eval_pop(self):
@@ -145,15 +137,6 @@ class GaussianSearchAlgorithm(SearchAlgorithm, SinglePopulationAlgorithmMixin):
         self._population = populations[0] if len(populations) == 1 else SolutionBatch.cat(populations)
 
     # ------------------------------------------------------------------ CUDA-graph replay of a whole generation
-    def enable_cuda_graph(self, enabled: bool = True):
-        """Capture one generation (rank -> gradients -> update -> fused sample/evaluate) into a CUDA graph and replay it from
-        `step()`: one graph launch instead of ~20 kernel launches and their Python glue.  The trajectory is bit-identical to
-        the eager path: the sampler reads a device-side generation counter that an in-graph kernel increments.  Falls back to
-        eager stepping whenever the configuration is not capturable (see `_graph_capturable`)."""
-        self._use_graph = bool(enabled)
-        self._graph = None
-        return self
-
     def _graph_capturable(self) -> bool:
         from ..optimizers import ClipUp
 
@@ -167,61 +150,27 @@ class GaussianSearchAlgorithm(SearchAlgorithm, SinglePopulationAlgorithmMixin):
                     and len(prob.before_grad_hook) == 0 and len(prob.after_grad_hook) == 0)  # Python hooks do not replay
         return ok and self._population is not None
 
-    def _update_in_place(self, gradients: dict):
-        """Same arithmetic as `_update_distribution` on CUDA, but writing into the live mu / sigma buffers (replayable)."""
-        dist = self._distribution
-        gmu = gradients["mu"].contiguous()
-        if self._optimizer is not None:
-            self._optimizer.ascent_into_(gmu, dist.mu)
-        else:
-            ops.axpy_(dist.mu, gmu, self._center_learning_rate)
-        ops.sigma_update_(dist.sigma, gradients["sigma"].contiguous(), self._stdev_learning_rate, isinstance(dist, ExpSeparableGaussian),
-                          **self._kernel_bounds)
-
-    def _graph_body(self, base_stream: int, counter: torch.Tensor):
+    def _graph_body(self):
         dist, prob, pop = self._distribution, self.problem, self._population
         lazy = isinstance(pop, LazySolutionBatch)
         n = len(pop)
         fitnesses = pop._evdata.view(-1)
+        seed, sid = prob.next_philox_stream()
+        counter = prob.philox_stream_offset
         # the population consumed here was drawn one stream id earlier (by the eager step before the capture, or by the previous
         # replay); a materialised one is rebuilt in part from the same counters (`_step_graph` drops the graph if it was modified)
-        recipe = PhiloxRecipe(seed=prob._philox_seed, stream_id=base_stream - 1, row0=0, n_rows=n, solution_length=prob.solution_length,
+        recipe = PhiloxRecipe(seed=seed, stream_id=sid - 1, row0=0, n_rows=n, solution_length=prob.solution_length,
                               symmetric=dist.SYMMETRIC, stream_offset=counter, mu=dist.mu, sigma=dist.sigma)
         samples = recipe if lazy else PhiloxSamples(pop._data, recipe)
         gradients = dist.compute_gradients(samples, fitnesses, objective_sense=prob.senses[self._obj_index], ranking_method=self._ranking_method)
-        self._update_in_place(gradients)
+        self._update_into(dist.mu, dist.sigma, gradients)
         ops.sample_eval(prob.evok_objective_id, None if lazy else pop._data, dist.mu, dist.sigma, n_rows=n, symmetric=dist.SYMMETRIC,
-                        seed=prob._philox_seed, stream_id=base_stream, f=fitnesses, stream_offset=counter)
-        counter.add_(1)
+                        seed=seed, stream_id=sid, f=fitnesses, stream_offset=counter)
         if lazy:
             pop.recipe = recipe
 
-    def _capture_graph(self):
-        prob = self.problem
-        # the distribution's tensors become the persistent, in-place-updated buffers of the graph
-        dist = self._distribution
-        if not (dist.mu.is_contiguous() and dist.sigma.is_contiguous()):
-            self._distribution = dist = dist.modified_copy(mu=dist.mu.contiguous(), sigma=dist.sigma.contiguous())
-        self._graph_counter = torch.zeros(1, dtype=torch.int32, device=dist.mu.device)
-        self._graph_base_stream = prob._philox_stream
-        graph = torch.cuda.CUDAGraph()
-        before = ops.launch_count()
-        from .. import _native as nat
-
-        with nat.private_workspaces() as store, torch.cuda.graph(graph):  # the graph owns the scratch buffers it writes to
-            self._graph_body(self._graph_base_stream, self._graph_counter)
-        self._graph_workspaces = store
-        self._graph_kernels = ops.launch_count() - before  # kernels of libevok.so inside one replay
-        ops.count_replayed_launches(-self._graph_kernels)  # the capture itself executed nothing
-        self._graph_counter.zero_()
-        self._graph = graph
-        pop = self._population
-        # replays resample the population without passing through Python: the eager record goes stale with the first one
-        pop._philox_record = None
-        self._graph_values_version = None if isinstance(pop, LazySolutionBatch) else pop._data._version
-
     def _step_graph(self):
-        prob, pop = self.problem, self._population
+        pop = self._population
         if self._graph is not None and self._graph_values_version is not None and pop._data._version != self._graph_values_version:
             # the population was modified in place since the last replay: the graph would rebuild rows from their Philox
             # counters, so this generation runs eagerly (reading the modified rows) and the next one captures a new graph
@@ -231,12 +180,17 @@ class GaussianSearchAlgorithm(SearchAlgorithm, SinglePopulationAlgorithmMixin):
         if self._graph is None:
             # one more eager generation right before the capture: warms every kernel and workspace that the graph will use
             self._step_eager()
-            self._capture_graph()
+            # the distribution's tensors become the persistent, in-place-updated buffers of the graph
+            dist, pop = self._distribution, self._population
+            if not (dist.mu.is_contiguous() and dist.sigma.is_contiguous()):
+                self._distribution = dist.modified_copy(mu=dist.mu.contiguous(), sigma=dist.sigma.contiguous())
+            self._graph = GenerationGraph(self.problem, self._graph_body)
+            # replays resample the population without passing through Python: the eager record goes stale with the first one
+            pop._philox_record = None
+            self._graph_values_version = None if isinstance(pop, LazySolutionBatch) else pop._data._version
             return
         self._graph.replay()
-        ops.count_replayed_launches(self._graph_kernels)
-        prob._philox_stream += 1  # keep the host-side stream counter in step with the device-side one
-        prob._finish_evaluation(pop)
+        self.problem._finish_evaluation(pop)
 
     def _step_non_distributed(self):
         """gaussian.py:274-367."""
@@ -266,7 +220,7 @@ class GaussianSearchAlgorithm(SearchAlgorithm, SinglePopulationAlgorithmMixin):
                                                             ranking_method=self._ranking_method,
                                                             ensure_even_popsize=self._ensure_even_popsize)
         if in_place:
-            self._update_in_place(fetched[0]["gradients"])
+            self._update_into(self._distribution.mu, self._distribution.sigma, fetched[0]["gradients"])
         else:
             self._update_distribution(fetched[0]["gradients"])
         self._mean_eval = fetched[0]["mean_eval"]
@@ -311,44 +265,32 @@ class GaussianSearchAlgorithm(SearchAlgorithm, SinglePopulationAlgorithmMixin):
                 self._distributed_body(in_place=False)
                 return
             dist = self._distribution
-            self._distribution = dist = dist.modified_copy(mu=dist.mu.contiguous().clone(), sigma=dist.sigma.contiguous().clone())
-            prob.philox_stream_offset = torch.zeros(1, dtype=torch.int32, device=dist.mu.device)
-            base = prob._philox_stream
-            torch.cuda.synchronize()
-            graph = torch.cuda.CUDAGraph()
-            before = ops.launch_count()
-            from .. import _native as nat
-
-            with nat.private_workspaces() as store, torch.cuda.graph(graph):
-                self._distributed_body(in_place=True)
-                prob.philox_stream_offset.add_(1)
-            self._graph_workspaces = store
-            self._graph_kernels = ops.launch_count() - before
-            ops.count_replayed_launches(-self._graph_kernels)
-            prob._philox_stream = base  # the capture consumed one host-side stream id without running anything
-            prob.philox_stream_offset.zero_()
-            self._graph = graph
+            self._distribution = dist.modified_copy(mu=dist.mu.contiguous().clone(), sigma=dist.sigma.contiguous().clone())
+            self._graph = GenerationGraph(prob, lambda: self._distributed_body(in_place=True))
         self._graph.replay()
-        ops.count_replayed_launches(self._graph_kernels)
-        prob._philox_stream += 1
 
     # ------------------------------------------------------------------ distribution update (K5)
+    def _update_into(self, mu: torch.Tensor, sigma: torch.Tensor, gradients: dict):
+        """The CUDA update of a separable distribution as two launches that write into `mu` and `sigma`: follow the gradients,
+        then clamp sigma against its pre-update value."""
+        gmu = gradients["mu"].contiguous()
+        if self._optimizer is not None and hasattr(self._optimizer, "ascent_into_"):
+            self._optimizer.ascent_into_(gmu, mu)
+        elif self._optimizer is not None:
+            mu += self._optimizer.ascent(gmu)
+        else:
+            ops.axpy_(mu, gmu, self._center_learning_rate)
+        ops.sigma_update_(sigma, gradients["sigma"].contiguous(), self._stdev_learning_rate, isinstance(self._distribution, ExpSeparableGaussian),
+                          **self._kernel_bounds)
+
     def _update_distribution(self, gradients: dict):
         """gaussian.py:369-419: follow the gradients, then clamp sigma against its pre-update value."""
         dist = self._distribution
         separable = isinstance(dist, SeparableGaussian)
         if separable and ops.uses_kernels(dist.mu) and ops.uses_kernels(gradients["mu"]):
-            # two launches, in place on copies (the previous generation's tensors stay valid for whoever holds them)
+            # on copies: the previous generation's tensors stay valid for whoever holds them
             new_mu, new_sigma = dist.mu.clone(), dist.sigma.clone()
-            gmu = gradients["mu"].contiguous()
-            if self._optimizer is not None and hasattr(self._optimizer, "ascent_into_"):
-                self._optimizer.ascent_into_(gmu, new_mu)
-            elif self._optimizer is not None:
-                new_mu += self._optimizer.ascent(gmu)
-            else:
-                ops.axpy_(new_mu, gmu, self._center_learning_rate)
-            ops.sigma_update_(new_sigma, gradients["sigma"].contiguous(), self._stdev_learning_rate,
-                              isinstance(dist, ExpSeparableGaussian), **self._kernel_bounds)
+            self._update_into(new_mu, new_sigma, gradients)
             self._distribution = dist.modified_copy(mu=new_mu, sigma=new_sigma)
             return
 

@@ -5,6 +5,7 @@ only computed when something (a logger, the user) reads them, so reading nothing
 from __future__ import annotations
 
 import io
+import os
 from collections.abc import Mapping
 from datetime import datetime
 from typing import Any, Iterable, Optional
@@ -158,6 +159,30 @@ class SearchAlgorithm(LazyReporter):
     @property
     def is_terminated(self) -> bool:
         return False
+
+
+class CUDAGraphMixin:
+    """`enable_cuda_graph()` for the searchers that can replay a whole generation from one CUDA graph (`.cudagraph`).
+    `_graph` is the captured `GenerationGraph` or None; each searcher's `_graph_capturable()` says when it may be used."""
+
+    def __init__(self):
+        self._use_graph = os.environ.get("EVOTORCH_B200_CUDA_GRAPH", "0") == "1"
+        self._graph = None
+
+    def enable_cuda_graph(self, enabled: bool = True):
+        """Capture one generation into a CUDA graph and replay it from `step()`: one graph launch per generation instead of
+        the kernel launches and their Python glue.  The trajectory is bit-identical to eager stepping: the sampler reads a
+        device-side generation counter that an in-graph kernel increments.  Stepping stays eager while the configuration is
+        not capturable (hooks, non-fused paths, ...); calling this again drops the captured graph."""
+        self._use_graph = bool(enabled)
+        self._graph = None
+        return self
+
+    def __getstate__(self) -> dict:
+        """Everything but the captured CUDA graph (re-captured on the first step after loading)."""
+        state = dict(self.__dict__)
+        state["_graph"] = None
+        return state
 
 
 class SinglePopulationAlgorithmMixin:

@@ -138,7 +138,7 @@ class Problem(Clonable):
         self._philox_seed = int(seed) & 0xFFFFFFFFFFFFFFFF
         self._philox_stream = 0
         self.philox_row0 = 0  # global index of the first local row when the population is sharded over ranks
-        self.philox_stream_offset = None  # optional device-side generation counter (set while a CUDA graph is captured / replayed)
+        self.philox_stream_offset = None  # device-side generation counter, set only while a CUDA graph is captured (algorithms/cudagraph.py)
 
     def next_philox_stream(self) -> tuple:
         """(seed, stream_id) for the next kernel-sampled population; every call uses a fresh Philox stream."""
@@ -518,12 +518,9 @@ class Problem(Clonable):
     _TRANSIENT = ("_peer_exchange", "_active_peer", "_grad_batches", "_grad_scratch", "_d2h_stage")
 
     def __getstate__(self) -> dict:
-        """Device-mapped and cached objects (peer-exchange buffers, gradient batches, the CUDA-graph generation counter) are
-        not part of a pickled problem; the Philox key and the host-side generation counter are, so an unpickled problem
-        continues the same random stream."""
-        state = {k: v for k, v in self.__dict__.items() if k not in self._TRANSIENT}
-        state["philox_stream_offset"] = None
-        return state
+        """Device-mapped and cached objects (peer-exchange buffers, gradient batches) are not part of a pickled problem; the
+        Philox key and the host-side generation counter are, so an unpickled problem continues the same random stream."""
+        return {k: v for k, v in self.__dict__.items() if k not in self._TRANSIENT}
 
     # ------------------------------------------------------------------ fused sample + evaluate, gradient service
     def sample_and_evaluate(self, distribution, batch: "SolutionBatch"):

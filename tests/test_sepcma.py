@@ -166,14 +166,15 @@ def test_lazy_separable_population_needs_the_fused_prerequisites():
     assert full.population.values.shape == (10, 8)
 
 
-def test_getstate_drops_the_fused_scratch_buffers():
+def test_getstate_drops_the_fused_buffers_and_the_graph():
     """Pickles hold the search state, not the fused generation's scratch buffers or graph: those (and s = sigma * A) are
-    rebuilt on the first step after loading."""
+    rebuilt on the first step after loading.  The device-side step counter of a captured generation belongs to its graph,
+    not to these buffers."""
     prob = Problem("min", _torch_sphere, initial_bounds=(-3, 3), solution_length=6, vectorized=True, seed=2, dtype=torch.float32)
     c = CMAES(prob, stdev_init=0.8, popsize=10, separable=True)
     c.step()
     fs = c._fused_state()  # the buffers exist whether or not this device runs the fused path
-    assert set(fs) >= {"q", "aw", "local", "S2", "wsum", "s", "steps_dev"}
+    assert set(fs) >= {"q", "aw", "local", "S2", "wsum", "s"}
     assert torch.equal(fs["s"], c.sigma * c.A)
     state = c.__getstate__()
     assert state["_fused"] is None and state["_graph"] is None and "_graph_workspaces" not in state
