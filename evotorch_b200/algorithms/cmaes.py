@@ -30,7 +30,7 @@ import numpy as np
 import torch
 
 from .. import ops
-from ..core import LazySolutionBatch, PhiloxRecipe, Problem, Solution, SolutionBatch
+from ..core import LazySolutionBatch, Problem, Solution, SolutionBatch
 from .cudagraph import GenerationGraph
 from .searchalgorithm import CUDAGraphMixin, SearchAlgorithm, SinglePopulationAlgorithmMixin
 
@@ -165,10 +165,8 @@ class CMAES(SearchAlgorithm, SinglePopulationAlgorithmMixin, CUDAGraphMixin):
         fs = self.__dict__.get("_fused") if n == self.popsize and not self.separable else None
         zs = problem.make_empty(num_solutions=n) if fs is None else fs["zs"]
         if ops.uses_kernels(zs) and problem.rng == "philox":
-            seed, stream_id = problem.next_philox_stream()
             zero, one = (problem.make_zeros(d), problem.make_ones(d)) if fs is None else (fs["zero"], fs["one"])
-            ops.sample_eval(ops.OBJ_NONE, zs, zero, one, n_rows=n, symmetric=False, seed=seed, stream_id=stream_id,
-                            stream_offset=problem.philox_stream_offset)
+            ops.sample_eval(ops.OBJ_NONE, zs, zero, one, n_rows=n, symmetric=False, **problem.next_philox_draw().kwargs)
         else:
             problem.make_gaussian(out=zs)
         if self.separable:
@@ -351,36 +349,31 @@ class CMAES(SearchAlgorithm, SinglePopulationAlgorithmMixin, CUDAGraphMixin):
         fs = self._fused_state()
         prob, pop, n, d = self._problem, self._population, self.popsize, self._problem.solution_length
         lazy = isinstance(pop, LazySolutionBatch)
-        seed, stream_id = prob.next_philox_stream()
-        offset = prob.philox_stream_offset
+        draw = prob.next_philox_draw()
         f = pop._evdata.view(-1)
         obj = prob.evok_objective_id
         if lazy:
             # until the update below the live m and s ARE the draw's centre and stdev (what a before-eval hook or the best / worst
             # bookkeeping regenerates rows from)
-            pop.recipe = PhiloxRecipe(seed=seed, stream_id=stream_id, row0=0, n_rows=n, solution_length=d, symmetric=False, stream_offset=offset,
-                                      mu=self.m, sigma=fs["s"])
+            pop.recipe = draw.recipe(n, False, self.m, fs["s"])
             prob._before_eval_hook(pop)
-            ops.sample_eval_sq(obj, None, self.m, fs["s"], fs["q"], n_rows=n, seed=seed, stream_id=stream_id, f=f, stream_offset=offset)
+            ops.sample_eval_sq(obj, None, self.m, fs["s"], fs["q"], n_rows=n, f=f, **draw.kwargs)
             prob._finish_evaluation(pop)
         elif obj is not None and len(prob.before_eval_hook) == 0:
-            ops.sample_eval_sq(obj, pop._data, self.m, fs["s"], fs["q"], n_rows=n, seed=seed, stream_id=stream_id, f=f, stream_offset=offset)
+            ops.sample_eval_sq(obj, pop._data, self.m, fs["s"], fs["q"], n_rows=n, f=f, **draw.kwargs)
             prob._finish_evaluation(pop)
         else:  # custom objective or before-eval hooks: sample (and keep q), then the problem's own evaluation
-            ops.sample_eval_sq(ops.OBJ_NONE, pop._data, self.m, fs["s"], fs["q"], n_rows=n, seed=seed, stream_id=stream_id, stream_offset=offset)
+            ops.sample_eval_sq(ops.OBJ_NONE, pop._data, self.m, fs["s"], fs["q"], n_rows=n, **draw.kwargs)
             pop._evdata.fill_(float("nan"))
             prob.evaluate(pop)
         ops.rank_table(f, prob.senses[self._obj_index] == "max", self.weights, out=fs["aw"])
-        ops.sepcma_moments(fs["aw"], fs["q"], self.active, d, seed=seed, stream_id=stream_id, stream_offset=offset, local=fs["local"], S2=fs["S2"],
-                           wsum=fs["wsum"])
+        ops.sepcma_moments(fs["aw"], fs["q"], self.active, d, local=fs["local"], S2=fs["S2"], wsum=fs["wsum"], **draw.kwargs)
         ops.sepcma_update(fs["local"], fs["S2"], fs["wsum"], self.m, self.p_sigma, self.p_c, self.sigma, self.C, self.A, fs["s"], self._consts,
                           self.csa_squared, decompose_C_freq=self.decompose_C_freq, steps=self._steps_count, steps_dev=steps_dev,
                           stdev_min=self.stdev_min, stdev_max=self.stdev_max, m_prev=fs["m_draw"], s_prev=fs["s_draw"])
         if lazy:
-            # from here on the population is the one drawn from the snapshots.  Under a CUDA graph the stream offset counter is
-            # advanced right after this body, so the draw is (stream_id - 1) + counter: the recipe then follows every replay.
-            pop.recipe = PhiloxRecipe(seed=seed, stream_id=stream_id if offset is None else stream_id - 1, row0=0, n_rows=n, solution_length=d,
-                                      symmetric=False, stream_offset=offset, mu=fs["m_draw"], sigma=fs["s_draw"])
+            # from here on the population is the one drawn from the snapshots; under a CUDA graph its recipe follows every replay
+            pop.recipe = draw.between_generations().recipe(n, False, fs["m_draw"], fs["s_draw"])
 
     # ------------------------------------------------------------------ CUDA-graph replay of the fused generation
     def _graph_capturable(self) -> bool:

@@ -14,13 +14,16 @@ from ..core import Problem
 class GenerationGraph:
     """One generation of a searcher captured into a CUDA graph; `replay()` runs the next generation.
 
-    The body draws its Philox stream as an eager step does (`problem.next_philox_stream()`) and passes
-    `problem.philox_stream_offset` to every kernel that samples or regenerates the population.  While the capture runs, that
-    attribute is a fresh device-side int32 generation counter, zero until the first replay and incremented by the graph after
-    the body, so the k-th replay (k = 0, 1, ...) draws from stream `base + k`, `base` being the host stream id the capture started
-    from; `replay()` advances the host counter alongside.  Outside the capture the attribute is None again: the graph reads the counter through the pointer it
-    baked in, and an eager step after any number of replays continues on the next host stream id.  Every capture allocates its
-    own counter, because a lazy population's `PhiloxRecipe` may still reference the one of an earlier graph.
+    The body takes its draw as an eager step does (`problem.next_philox_draw()`) and hands it to every kernel that samples or
+    regenerates the population.  While the capture runs, `problem.philox_stream_offset`, and so the draw's `stream_offset`, is a
+    fresh device-side int32 generation counter, zero until the first replay and incremented by the graph after the body, so the
+    k-th replay (k = 0, 1, ...) draws from stream `base + k`, `base` being the host stream id the capture started from;
+    `replay()` advances the host counter alongside.  The population that exists between two generations is therefore keyed
+    `(base - 1) + counter` (`PhiloxDraw.between_generations()`): read while replay k runs, the counter is k and that is the
+    previous replay's population, the one the body consumes; read after it, the counter is k + 1 and that is the population
+    replay k drew.  Outside the capture the attribute is None again: the graph reads the counter through the pointer it baked
+    in, and an eager step after any number of replays continues on the next host stream id.  Every capture allocates its own
+    counter, because a lazy population's `PhiloxRecipe` may still reference the one of an earlier graph.
 
     The body runs under `private_workspaces()`, so the graph owns the scratch buffers it writes to.  `buffers` are tensors made
     outside the capture that nothing but the graph uses any more: the graph keeps them alive, because its kernels read and write

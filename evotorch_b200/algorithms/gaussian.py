@@ -20,7 +20,7 @@ from typing import Optional
 import torch
 
 from .. import ops
-from ..core import LazySolutionBatch, PhiloxRecipe, PhiloxSamples, Problem, SolutionBatch
+from ..core import LazySolutionBatch, PhiloxSamples, Problem, SolutionBatch
 from ..distributed import world
 from ..distributions import Distribution, ExpGaussian, ExpSeparableGaussian, SeparableGaussian, SymmetricSeparableGaussian
 from ..optimizers import get_optimizer_class
@@ -155,17 +155,15 @@ class GaussianSearchAlgorithm(SearchAlgorithm, SinglePopulationAlgorithmMixin, C
         lazy = isinstance(pop, LazySolutionBatch)
         n = len(pop)
         fitnesses = pop._evdata.view(-1)
-        seed, sid = prob.next_philox_stream()
-        counter = prob.philox_stream_offset
-        # the population consumed here was drawn one stream id earlier (by the eager step before the capture, or by the previous
-        # replay); a materialised one is rebuilt in part from the same counters (`_step_graph` drops the graph if it was modified)
-        recipe = PhiloxRecipe(seed=seed, stream_id=sid - 1, row0=0, n_rows=n, solution_length=prob.solution_length,
-                              symmetric=dist.SYMMETRIC, stream_offset=counter, mu=dist.mu, sigma=dist.sigma)
+        draw = prob.next_philox_draw()
+        # the population consumed here is the previous generation's (the eager step before the capture, or the previous replay);
+        # a materialised one is rebuilt in part from the same counters (`_step_graph` drops the graph if it was modified)
+        recipe = draw.between_generations().recipe(n, dist.SYMMETRIC, dist.mu, dist.sigma)
         samples = recipe if lazy else PhiloxSamples(pop._data, recipe)
         gradients = dist.compute_gradients(samples, fitnesses, objective_sense=prob.senses[self._obj_index], ranking_method=self._ranking_method)
         self._update_into(dist.mu, dist.sigma, gradients)
         ops.sample_eval(prob.evok_objective_id, None if lazy else pop._data, dist.mu, dist.sigma, n_rows=n, symmetric=dist.SYMMETRIC,
-                        seed=seed, stream_id=sid, f=fitnesses, stream_offset=counter)
+                        f=fitnesses, **draw.kwargs)
         if lazy:
             pop.recipe = recipe
 
@@ -205,9 +203,8 @@ class GaussianSearchAlgorithm(SearchAlgorithm, SinglePopulationAlgorithmMixin, C
             self._step_eager()
 
     def _step_eager(self):
-        lazy = isinstance(self._population, LazySolutionBatch)
         dist = self._distribution
-        samples = self._population.recipe if lazy else self._population.gradient_samples(dist.mu, dist.sigma)
+        samples = self._population.gradient_samples(dist.mu, dist.sigma)
         fitnesses = self._population.access_evals()[:, self._obj_index]
         gradients = self._distribution.compute_gradients(samples, fitnesses, objective_sense=self.problem.senses[self._obj_index],
                                                          ranking_method=self._ranking_method)

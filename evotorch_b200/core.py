@@ -13,6 +13,7 @@ multi-objective pareto utilities.  Population sharding across GPUs is done with 
 from __future__ import annotations
 
 import math
+from dataclasses import dataclass, replace
 from typing import Any, Callable, Iterable, Optional, Union
 
 import torch
@@ -140,11 +141,12 @@ class Problem(Clonable):
         self.philox_row0 = 0  # global index of the first local row when the population is sharded over ranks
         self.philox_stream_offset = None  # device-side generation counter, set only while a CUDA graph is captured (algorithms/cudagraph.py)
 
-    def next_philox_stream(self) -> tuple:
-        """(seed, stream_id) for the next kernel-sampled population; every call uses a fresh Philox stream."""
+    def next_philox_draw(self) -> "PhiloxDraw":
+        """The draw of the next kernel-sampled population: a fresh Philox stream (the host-side stream id advances by one),
+        starting at global row `philox_row0`, with the device-side `philox_stream_offset` of the moment."""
         sid = self._philox_stream
         self._philox_stream += 1
-        return self._philox_seed, sid
+        return PhiloxDraw(self._philox_seed, sid, self.philox_row0, self.philox_stream_offset)
 
     # ------------------------------------------------------------------ properties
     @property
@@ -526,64 +528,48 @@ class Problem(Clonable):
     def sample_and_evaluate(self, distribution, batch: "SolutionBatch"):
         """Fill `batch` with samples of `distribution` and evaluate it.  With a built-in objective, the Philox sampler and
         a separable Gaussian this is ONE kernel (K1+K2 fused: the population is written once and evaluated from registers);
-        otherwise `distribution.sample(out=...)` followed by `evaluate` (gaussian.py:292-295 of the reference)."""
+        otherwise `distribution.sample(out=...)` followed by `evaluate` (gaussian.py:292-295 of the reference).  A lazy population
+        (`LazySolutionBatch`) has no such fall-back: it exists only as the fused sampler's draw."""
         obj = self.evok_objective_id
-        if isinstance(batch, LazySolutionBatch):
-            if not (obj is not None and self.rng == "philox" and len(self._senses) == 1 and hasattr(distribution, "SYMMETRIC")
-                    and ops.uses_kernels(distribution.mu)):
-                raise ValueError("a lazy population needs a built-in objective, rng='philox', a separable Gaussian and CUDA float32")
-            n = len(batch)
-            if distribution.SYMMETRIC and n % 2 != 0:
-                raise ValueError(f"Symmetric sampling cannot be done if the number of solutions is odd: {n}")
-            seed, stream_id = self.next_philox_stream()
-            mu, sigma = distribution.mu.contiguous(), distribution.sigma.contiguous()
-            batch.recipe = PhiloxRecipe(seed=seed, stream_id=stream_id, row0=self.philox_row0, n_rows=n, solution_length=self._solution_length,
-                                        symmetric=distribution.SYMMETRIC, stream_offset=self.philox_stream_offset, mu=mu, sigma=sigma)
-            # the hook runs AFTER the new population is defined (core.py:2559 of the reference calls it inside evaluate(), after
-            # distribution.sample): `batch.values` regenerates the new samples from the recipe.  A lazy batch is read-only.
-            self._before_eval_hook(batch)
-            peer = getattr(self, "_active_peer", None)
-            if peer is not None:  # sharded generation over NVLink peer memory: the fitness all-gather happens inside the kernel
-                ops.sample_eval_push(obj, None, mu, sigma, n_rows=n, symmetric=distribution.SYMMETRIC, seed=seed, stream_id=stream_id,
-                                     row0=self.philox_row0, peer=peer, stream_offset=self.philox_stream_offset)
-            else:
-                ops.sample_eval(obj, None, mu, sigma, n_rows=n, symmetric=distribution.SYMMETRIC, seed=seed, stream_id=stream_id,
-                                row0=self.philox_row0, f=batch._evdata.view(-1), stream_offset=self.philox_stream_offset)
-            self._finish_evaluation(batch)
-            return
-        batch._philox_record = None  # only the fused sampler below leaves a record that the gradient pass may rebuild rows from
-        values = batch.access_values()
+        lazy = isinstance(batch, LazySolutionBatch)
+        values = None if lazy else batch.access_values()
         # before-eval hooks must see (and may edit) the freshly sampled values before they are evaluated (core.py:2559 of the
         # reference: the hook is called inside evaluate(), after distribution.sample): with hooks registered the sampling and the
-        # evaluation stay two kernels with the hook in between
-        fused = (obj is not None and self.rng == "philox" and ops.uses_kernels(values) and len(self._senses) == 1
-                 and hasattr(distribution, "SYMMETRIC") and ops.uses_kernels(distribution.mu) and len(self._before_eval_hook) == 0)
+        # evaluation of a materialised population stay two kernels with the hook in between
+        fused = (obj is not None and self.rng == "philox" and len(self._senses) == 1 and hasattr(distribution, "SYMMETRIC")
+                 and ops.uses_kernels(distribution.mu) and (lazy or (ops.uses_kernels(values) and len(self._before_eval_hook) == 0)))
+        if not lazy:
+            batch._philox_record = None  # only the fused sampler below leaves a record that the gradient pass may rebuild rows from
         if not fused:
+            if lazy:
+                raise ValueError("a lazy population needs a built-in objective, rng='philox', a separable Gaussian and CUDA float32")
             distribution.sample(out=values, generator=self)
             self.evaluate(batch)
             return
-        n = values.shape[0]
+        n = len(batch)
         if distribution.SYMMETRIC and n % 2 != 0:
-            raise ValueError(f"Symmetric sampling cannot be done if the leftmost dimension of the target tensor is odd: {tuple(values.shape)}")
-        seed, stream_id = self.next_philox_stream()
-        evdata = batch._evdata
-        direct = evdata.shape[1] == 1 and evdata.dtype == torch.float32 and evdata.is_contiguous()
-        f = evdata.view(-1) if direct else torch.empty(n, dtype=torch.float32, device=values.device)
-        peer = getattr(self, "_active_peer", None)
-        if peer is not None:  # sharded generation over NVLink peer memory (evdata IS this rank's slice of peer.f_all)
-            ops.sample_eval_push(obj, values, distribution.mu.contiguous(), distribution.sigma.contiguous(), n_rows=n,
-                                 symmetric=distribution.SYMMETRIC, seed=seed, stream_id=stream_id, row0=self.philox_row0, peer=peer,
-                                 stream_offset=self.philox_stream_offset)
-            self._finish_evaluation(batch)
-            return
+            raise ValueError(f"Symmetric sampling cannot be done if the number of solutions is odd: {n}")
+        draw = self.next_philox_draw()
         mu, sigma = distribution.mu.contiguous(), distribution.sigma.contiguous()
-        ops.sample_eval(obj, values, mu, sigma, n_rows=n, symmetric=distribution.SYMMETRIC, seed=seed, stream_id=stream_id,
-                        row0=self.philox_row0, f=f, stream_offset=self.philox_stream_offset)
-        recipe = PhiloxRecipe(seed=seed, stream_id=stream_id, row0=self.philox_row0, n_rows=n, solution_length=self._solution_length,
-                              symmetric=distribution.SYMMETRIC, stream_offset=self.philox_stream_offset, mu=mu, sigma=sigma)
-        batch._philox_record = (PhiloxSamples(values, recipe), values._version, mu._version, sigma._version)
-        if not direct:
-            batch.set_evals(f)
+        recipe = draw.recipe(n, distribution.SYMMETRIC, mu, sigma)
+        if lazy:
+            # the hook runs AFTER the new population is defined (core.py:2559 of the reference calls it inside evaluate(), after
+            # distribution.sample): `batch.values` regenerates the new samples from the recipe.  A lazy batch is read-only.
+            batch.recipe = recipe
+            self._before_eval_hook(batch)
+        peer = getattr(self, "_active_peer", None)
+        if peer is not None:  # sharded generation over NVLink peer memory: the fitness all-gather happens inside the kernel
+            # (the batch's evaluations ARE this rank's slice of peer.f_all)
+            ops.sample_eval_push(obj, values, mu, sigma, n_rows=n, symmetric=distribution.SYMMETRIC, peer=peer, **draw.kwargs)
+        else:
+            evdata = batch._evdata
+            direct = lazy or (evdata.shape[1] == 1 and evdata.dtype == torch.float32 and evdata.is_contiguous())
+            f = evdata.view(-1) if direct else torch.empty(n, dtype=torch.float32, device=evdata.device)
+            ops.sample_eval(obj, values, mu, sigma, n_rows=n, symmetric=distribution.SYMMETRIC, f=f, **draw.kwargs)
+            if not direct:
+                batch.set_evals(f)
+        if not lazy:
+            batch._philox_record = (PhiloxSamples(values, recipe), values._version, mu._version, sigma._version)
         self._finish_evaluation(batch)
 
     def sample_and_compute_gradients(self, distribution, popsize: int, *, num_interactions: Optional[int] = None,
@@ -912,24 +898,54 @@ class SolutionBatch:
         return f"<SolutionBatch: {len(self)} x {self.solution_length}, {self.dtype}, {self.device}>"
 
 
+@dataclass(frozen=True, eq=False)
+class PhiloxDraw:
+    """The Philox counters of one kernel-sampled population: key, stream id, global index of the first row (non-zero for a
+    rank's shard) and the optional device-side stream offset (a CUDA graph's generation counter, added to the stream id by the
+    kernels).  `kwargs` are the keyword arguments of every `ops` function that samples or regenerates a population."""
+
+    seed: int
+    stream_id: int
+    row0: int = 0
+    stream_offset: Optional[torch.Tensor] = None
+
+    @property
+    def kwargs(self) -> dict:
+        return dict(seed=self.seed, stream_id=self.stream_id, row0=self.row0, stream_offset=self.stream_offset)
+
+    def between_generations(self) -> "PhiloxDraw":
+        """The draw of the population that exists between two generations, seen from a generation that drew `self`: `self`
+        when stepping eagerly; under a CUDA graph (`stream_offset` set) one stream id lower with the same counter, which the
+        graph advances after every replay (the rule is derived in `algorithms/cudagraph.py::GenerationGraph`)."""
+        return self if self.stream_offset is None else replace(self, stream_id=self.stream_id - 1)
+
+    def recipe(self, n_rows: int, symmetric: bool, mu: torch.Tensor, sigma: torch.Tensor) -> "PhiloxRecipe":
+        """The population of `n_rows` rows that this draw samples from N(mu, diag(sigma^2))."""
+        return PhiloxRecipe(self, n_rows, mu.numel(), symmetric, mu, sigma)
+
+
+@dataclass(eq=False)
 class PhiloxRecipe:
     """How a population was (and can again be) generated: stands in for the N x D sample matrix in the gradient calls."""
 
-    def __init__(self, *, seed: int, stream_id: int, row0: int, n_rows: int, solution_length: int, symmetric: bool,
-                 stream_offset: Optional[torch.Tensor], mu: torch.Tensor, sigma: torch.Tensor):
-        self.seed, self.stream_id, self.row0, self.n_rows = seed, stream_id, row0, n_rows
-        self.solution_length, self.symmetric, self.stream_offset = solution_length, symmetric, stream_offset
-        self.mu, self.sigma = mu, sigma
+    draw: PhiloxDraw
+    n_rows: int
+    solution_length: int
+    symmetric: bool
+    mu: torch.Tensor
+    sigma: torch.Tensor
 
     @property
     def shape(self) -> tuple:
         return (self.n_rows, self.solution_length)
 
-    def materialize(self) -> torch.Tensor:
-        """Regenerate the decision values (allocates n_rows x solution_length floats)."""
-        out = torch.empty(self.n_rows, self.solution_length, dtype=torch.float32, device=self.mu.device)
-        ops.sample_eval(ops.OBJ_NONE, out, self.mu, self.sigma, n_rows=self.n_rows, symmetric=self.symmetric, seed=self.seed,
-                        stream_id=self.stream_id, row0=self.row0, stream_offset=self.stream_offset)
+    def materialize(self, first: int = 0, rows: Optional[int] = None) -> torch.Tensor:
+        """Regenerate the decision values of rows [first, first + rows), by default all of them (allocates rows x
+        solution_length floats).  With a symmetric recipe `first` and `rows` are even."""
+        rows = self.n_rows - first if rows is None else rows
+        out = torch.empty(rows, self.solution_length, dtype=torch.float32, device=self.mu.device)
+        ops.sample_eval(ops.OBJ_NONE, out, self.mu, self.sigma, n_rows=rows, symmetric=self.symmetric,
+                        **replace(self.draw, row0=self.draw.row0 + first).kwargs)
         return out
 
 
@@ -994,6 +1010,10 @@ class LazySolutionBatch(SolutionBatch):
     def set_values(self, values: Any, *, solutions=None):
         raise ValueError("The decision values of a lazy population are read-only (they are a function of the Philox counters).")
 
+    def gradient_samples(self, mu: torch.Tensor, sigma: torch.Tensor) -> Optional[PhiloxRecipe]:
+        """The recipe: the gradient pass regenerates every row from its Philox counters (there are no values to read)."""
+        return self.recipe
+
     def __getitem__(self, i):
         if isinstance(i, (slice, list, torch.Tensor)):
             raise NotImplementedError("slicing a lazy population is not supported; use `.values` to materialise it")
@@ -1011,11 +1031,7 @@ class _Materialized:
     def __init__(self, lazy: LazySolutionBatch, i: int):
         r = lazy.recipe
         first = (i // 2) * 2 if r.symmetric else i
-        rows = 2 if r.symmetric else 1
-        block = torch.empty(rows, r.solution_length, dtype=torch.float32, device=r.mu.device)
-        ops.sample_eval(ops.OBJ_NONE, block, r.mu, r.sigma, n_rows=rows, symmetric=r.symmetric, seed=r.seed, stream_id=r.stream_id,
-                        row0=r.row0 + first, stream_offset=r.stream_offset)
-        self._data = block[i - first: i - first + 1]
+        self._data = r.materialize(first, 2 if r.symmetric else 1)[i - first: i - first + 1]
         self._evdata = lazy._evdata[i: i + 1]
         self._senses, self._num_objs = lazy._senses, lazy._num_objs
 

@@ -181,7 +181,7 @@ def sharded_sample_and_gradients(problem, distribution, popsize: int, *, obj_ind
         problem.philox_row0 = 0
         problem._active_peer = None
 
-    samples = batch.recipe if isinstance(batch, LazySolutionBatch) else batch.gradient_samples(dev_dist.mu, dev_dist.sigma)
+    samples = batch.gradient_samples(dev_dist.mu, dev_dist.sigma)
     if sharded_rank:
         offsets = [0]
         for c in counts:
@@ -191,11 +191,7 @@ def sharded_sample_and_gradients(problem, distribution, popsize: int, *, obj_ind
         if w_local is None:
             w_local = scratch[n_local] = torch.empty(n_local, dtype=torch.float32, device=problem.device)
         w_local, mean_buf = peer.rank_sharded(batch._evdata.view(-1), method, sense == "max", offsets, w_local)
-        dev_dist._peer = peer
-        try:
-            summed = dev_dist.partial_gradients(samples, w_local, row0, method, local_weights_of=popsize)  # already summed over the ranks
-        finally:
-            dev_dist._peer = None
+        summed = dev_dist.partial_gradients(samples, w_local, row0, method, local_weights_of=popsize, peer=peer)  # already summed over the ranks
         grads = dev_dist.finalize_gradients(summed, popsize)
         mean_eval = mean_buf.reshape(())  # live 1-element buffer: holds the latest generation's global mean fitness
         grads, mean_eval = _results_to_home(problem, grads, mean_eval, home_device)
@@ -210,11 +206,7 @@ def sharded_sample_and_gradients(problem, distribution, popsize: int, *, obj_ind
     weights_all = rank(f_all, method, higher_is_better=(sense == "max"))
 
     if peer is not None:
-        dev_dist._peer = peer
-        try:
-            summed = dev_dist.partial_gradients(samples, weights_all, row0, method)  # already summed over the ranks
-        finally:
-            dev_dist._peer = None
+        summed = dev_dist.partial_gradients(samples, weights_all, row0, method, peer=peer)  # already summed over the ranks
         grads = dev_dist.finalize_gradients(summed, popsize)
     elif hasattr(dev_dist, "partial_gradients"):
         partial = dev_dist.partial_gradients(samples, weights_all, row0, method)

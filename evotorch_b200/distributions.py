@@ -30,9 +30,9 @@ from .tools.ranking import rank
 
 
 def _philox_source(generator: Any):
-    """Objects that hand out Philox (seed, stream_id) pairs (our Problem with rng="philox") select the K1 sampler;
-    a bare torch.Generator (or None) selects torch's own RNG."""
-    return generator if (generator is not None and hasattr(generator, "next_philox_stream")
+    """Objects that hand out Philox draws (our Problem with rng="philox") select the K1 sampler; a bare torch.Generator (or
+    None) selects torch's own RNG."""
+    return generator if (generator is not None and hasattr(generator, "next_philox_draw")
                          and getattr(generator, "rng", "philox") == "philox") else None
 
 
@@ -218,9 +218,8 @@ class SeparableGaussian(Distribution):
         if src is not None and ops.uses_kernels(out) and out.stride(1) == 1:
             if self.SYMMETRIC and out.shape[0] % 2 != 0:
                 raise ValueError(f"Symmetric sampling cannot be done if the leftmost dimension of the target tensor is odd: {tuple(out.shape)}")
-            seed, stream_id = src.next_philox_stream()
             ops.sample_eval(ops.OBJ_NONE, out, self.mu.contiguous(), self.sigma.contiguous(), n_rows=out.shape[0],
-                            symmetric=self.SYMMETRIC, seed=seed, stream_id=stream_id, row0=getattr(src, "philox_row0", 0))
+                            symmetric=self.SYMMETRIC, **src.next_philox_draw().kwargs)
         else:
             make_gaussian(out=out, center=self.mu, stdev=self.sigma, symmetric=self.SYMMETRIC, generator=extract_generator(generator))
 
@@ -252,33 +251,33 @@ class SeparableGaussian(Distribution):
 
     _UNTOUCHED_RANKINGS = ("centered", "normalized")  # utilities that `_prepared_weights` passes through unchanged
 
-    def _weighted_sums(self, form: int, samples: torch.Tensor, w: torch.Tensor, scale_mu: float, scale_sigma: float) -> tuple:
-        """(scale_mu * sum_r a_r eps_r, scale_sigma * sum_r b_r g(eps_r)) -- the K4 kernel, or its torch restatement."""
-        mu, sigma = self.mu, self.sigma
-        peer = getattr(self, "_peer", None)
-        if isinstance(samples, PhiloxSamples):  # a population the fused sampler wrote from mu / sigma, untouched since
-            r = samples.recipe
-            if peer is None and ops.uses_kernels(w):
-                return ops.grad_hybrid(form, samples.values, w.contiguous(), mu.contiguous(), sigma.contiguous(), seed=r.seed, stream_id=r.stream_id, row0=r.row0,
-                                       scale_mu=scale_mu, scale_sigma=scale_sigma, stream_offset=r.stream_offset)
-            samples = samples.values
-        if peer is not None:  # sharded generation: the kernel pushes this shard's sums to every GPU, the reduction returns the global sums
-            if isinstance(samples, PhiloxRecipe):
-                ops.grad_push(form, None, w.contiguous(), mu.contiguous(), sigma.contiguous(), scale_mu=scale_mu, scale_sigma=scale_sigma, peer=peer,
-                              seed=samples.seed, stream_id=samples.stream_id, row0=samples.row0, stream_offset=samples.stream_offset)
-            else:
-                ops.grad_push(form, samples, w.contiguous(), mu.contiguous(), sigma.contiguous(), scale_mu=scale_mu, scale_sigma=scale_sigma, peer=peer)
+    def _weighted_sums(self, form: int, samples, w: torch.Tensor, scale_mu: float, scale_sigma: float, peer=None) -> tuple:
+        """(scale_mu * sum_r a_r eps_r, scale_sigma * sum_r b_r g(eps_r)) -- the K4 kernel, or its torch restatement.
+        `samples` is a values tensor, a `PhiloxRecipe` (lazy population: every row is regenerated) or a `PhiloxSamples` (values
+        the fused sampler wrote from mu / sigma, untouched since: part of the rows is rebuilt).  `peer`: a sharded generation
+        over NVLink peer memory, where the kernel pushes this shard's sums to every GPU and the result is the global sums."""
+        if isinstance(samples, PhiloxSamples):
+            values, recipe = samples.values, samples.recipe
+        elif isinstance(samples, PhiloxRecipe):
+            values, recipe = None, samples
+        else:
+            values, recipe = samples, None
+        w, mu, sigma = w.contiguous(), self.mu.contiguous(), self.sigma.contiguous()
+        if peer is not None:  # reads the values where there are any, regenerates them otherwise
+            ops.grad_push(form, values, w, mu, sigma, scale_mu=scale_mu, scale_sigma=scale_sigma, peer=peer,
+                          **(recipe.draw.kwargs if values is None else {}))
             return peer.reduce_gradients()
-        if isinstance(samples, PhiloxRecipe):  # lazy population: regenerate eps = sigma * z from the Philox counters
-            return ops.grad_regen(form, w.contiguous(), mu.contiguous(), sigma.contiguous(), seed=samples.seed, stream_id=samples.stream_id,
-                                  row0=samples.row0, scale_mu=scale_mu, scale_sigma=scale_sigma, stream_offset=samples.stream_offset)
-        if ops.uses_kernels(samples) and ops.uses_kernels(w):
-            return ops.grad(form, samples, w.contiguous(), mu.contiguous(), sigma.contiguous(), scale_mu, scale_sigma)
+        if values is None:
+            return ops.grad_regen(form, w, mu, sigma, scale_mu=scale_mu, scale_sigma=scale_sigma, **recipe.draw.kwargs)
+        if recipe is not None and ops.uses_kernels(w):
+            return ops.grad_hybrid(form, values, w, mu, sigma, scale_mu=scale_mu, scale_sigma=scale_sigma, **recipe.draw.kwargs)
+        if ops.uses_kernels(values) and ops.uses_kernels(w):
+            return ops.grad(form, values, w, mu, sigma, scale_mu, scale_sigma)
         if form == ops.GRAD_SYMMETRIC:
-            eps = samples[0::2] - mu
+            eps = values[0::2] - mu
             a, b = (w[0::2] - w[1::2]) / 2, (w[0::2] + w[1::2]) / 2
         else:
-            eps = samples - mu
+            eps = values - mu
             a = b = w
         if form == ops.GRAD_EXP:
             g = ((eps / sigma) ** 2) - 1
@@ -300,19 +299,20 @@ class SeparableGaussian(Distribution):
         return ranking_used in self._UNTOUCHED_RANKINGS and ranking_used in ("centered", "linear", "nes")
 
     def partial_gradients(self, samples: torch.Tensor, all_weights: torch.Tensor, row0: int, ranking_used: Optional[str],
-                          local_weights_of: Optional[int] = None) -> dict:
+                          local_weights_of: Optional[int] = None, peer=None) -> dict:
         """Gradient contribution of a row shard.  `samples` are rows [row0, row0 + n) of a population whose utilities are
         `all_weights` (ranked over the WHOLE population).  The dictionaries of all shards add up (all-reduce) to what
         `finalize_gradients` turns into the result of `compute_gradients` on the whole population.
         `local_weights_of=N`: `all_weights` holds only the utilities of THIS shard's rows, of a population of N solutions
-        (sharded ranking; see `accepts_local_weights`)."""
+        (sharded ranking; see `accepts_local_weights`).  With `peer` (an evotorch_b200.peer.PeerExchange) the kernels do the
+        all-reduce: the result is already summed over the ranks."""
         n_local = samples.shape[0]
         if local_weights_of is not None:
             if not self.accepts_local_weights(ranking_used):
                 raise ValueError("this distribution / ranking needs the utilities of the whole population")
             smu, _ = self._grad_scale("mu", all_weights, local_weights_of)
             ssig, _ = self._grad_scale("sigma", all_weights, local_weights_of)
-            gmu, gsig = self._weighted_sums(self.GRAD_FORM, samples, all_weights, smu, ssig)
+            gmu, gsig = self._weighted_sums(self.GRAD_FORM, samples, all_weights, smu, ssig, peer)
             return {"mu": gmu, "sigma": gsig}
         if "parenthood_ratio" in self.parameters:  # CEM elite moments (distributions.py:538-546)
             num_elites = math.floor(all_weights.shape[0] * self.parameters["parenthood_ratio"])
@@ -321,12 +321,12 @@ class SeparableGaussian(Distribution):
             else:
                 mask = torch.zeros_like(all_weights)
                 mask[torch.argsort(all_weights, descending=True, stable=True)[:num_elites]] = 1
-            s1, s2 = self._weighted_sums(ops.GRAD_MOMENTS, samples, mask[row0:row0 + n_local], 1.0, 1.0)
+            s1, s2 = self._weighted_sums(ops.GRAD_MOMENTS, samples, mask[row0:row0 + n_local], 1.0, 1.0, peer)
             return {"elite_sum": s1, "elite_sqsum": s2}
         w = self._prepared_weights(all_weights, ranking_used)
         smu, dmu = self._grad_scale("mu", w)
         ssig, dsig = self._grad_scale("sigma", w)
-        gmu, gsig = self._weighted_sums(self.GRAD_FORM, samples, w[row0:row0 + n_local], smu, ssig)
+        gmu, gsig = self._weighted_sums(self.GRAD_FORM, samples, w[row0:row0 + n_local], smu, ssig, peer)
         if dmu is not None:
             gmu = gmu / dmu
         if dsig is not None:

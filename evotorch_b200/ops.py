@@ -7,6 +7,7 @@ libevok.so (include/evok.h).  Callers in this package decide *whether* a tensor 
 
 from __future__ import annotations
 
+import ctypes
 import math
 from typing import Optional
 
@@ -100,6 +101,41 @@ def _mat(t: torch.Tensor, name: str) -> torch.Tensor:
     return as_plain_tensor(t)
 
 
+def _ldx(X: Optional[torch.Tensor], n_rows: int, D: int) -> int:
+    """Leading dimension of the optional population operand X (n_rows x D); 0 for X = None (nothing stored or read)."""
+    if X is None:
+        return 0
+    _mat(X, "X")
+    if X.shape != (n_rows, D):
+        raise ValueError(f"X: expected shape {(n_rows, D)}, got {tuple(X.shape)}")
+    return X.stride(0)
+
+
+def _out_pair(mu: torch.Tensor, out_mu: Optional[torch.Tensor], out_sigma: Optional[torch.Tensor]) -> tuple:
+    """The (mu, sigma) gradient outputs: the given D-vectors, or new ones."""
+    D = mu.numel()
+    return (torch.empty_like(mu) if out_mu is None else _vec(out_mu, "out_mu", D),
+            torch.empty_like(mu) if out_sigma is None else _vec(out_sigma, "out_sigma", D))
+
+
+def _check_scalar_sigma(sigma: torch.Tensor) -> None:
+    if not (sigma.is_cuda and sigma.dtype == torch.float32 and sigma.numel() == 1):
+        raise ValueError("sigma: expected a 1-element float32 CUDA tensor")
+
+
+def _check_steps_dev(steps_dev: Optional[torch.Tensor]) -> None:
+    if steps_dev is not None and not (steps_dev.is_cuda and steps_dev.dtype == torch.int64 and steps_dev.numel() == 1):
+        raise ValueError("steps_dev: expected a 1-element int64 CUDA tensor")
+
+
+def _host_floats(values, n: int):
+    """The n host scalars `values` as a C float array (passed by pointer, read by the launch)."""
+    vals = [float(v) for v in values]
+    if len(vals) != n:
+        raise ValueError(f"expected {n} host scalars, got {len(vals)}")
+    return (ctypes.c_float * n)(*vals)
+
+
 # ------------------------------------------------------------------------------------------------ K1 / K2
 def _offset_ptr(stream_offset: Optional[torch.Tensor]) -> Optional[int]:
     if stream_offset is None:
@@ -114,12 +150,7 @@ def sample_eval(objective: int, X: Optional[torch.Tensor], mu: torch.Tensor, sig
                 stream_offset: Optional[torch.Tensor] = None) -> None:
     D = mu.numel()
     _vec(mu, "mu"); _vec(sigma, "sigma", D)
-    ldx = 0
-    if X is not None:
-        _mat(X, "X")
-        if X.shape != (n_rows, D):
-            raise ValueError(f"X: expected shape {(n_rows, D)}, got {tuple(X.shape)}")
-        ldx = X.stride(0)
+    ldx = _ldx(X, n_rows, D)
     if f is not None:
         _vec(f, "f", n_rows)
     if objective != OBJ_NONE and f is None:
@@ -130,8 +161,7 @@ def sample_eval(objective: int, X: Optional[torch.Tensor], mu: torch.Tensor, sig
         return
     with _timed("sample_eval" if objective != OBJ_NONE else "sample"):
         rc = nat.lib().evok_sample_eval(objective, nat.ptr(X), ldx, mu.data_ptr(), sigma.data_ptr(), row0, n_rows, D, int(symmetric),
-                                        seed & 0xFFFFFFFFFFFFFFFF, stream_id & 0xFFFFFFFFFFFFFFFF, _offset_ptr(stream_offset), nat.ptr(f),
-                                        nat.stream_of(mu))
+                                        seed, stream_id, _offset_ptr(stream_offset), nat.ptr(f), nat.stream_of(mu))
     nat.check(rc, "evok_sample_eval")
 
 
@@ -141,18 +171,13 @@ def sample_eval_push(objective: int, X: Optional[torch.Tensor], mu: torch.Tensor
     evotorch_b200.peer.PeerExchange).  Follow with `peer.wait_fitness()` before reading `peer.f_all`."""
     D = mu.numel()
     _vec(mu, "mu"); _vec(sigma, "sigma", D)
-    ldx = 0
-    if X is not None:
-        _mat(X, "X")
-        if X.shape != (n_rows, D):
-            raise ValueError(f"X: expected shape {(n_rows, D)}, got {tuple(X.shape)}")
-        ldx = X.stride(0)
+    ldx = _ldx(X, n_rows, D)
     if row0 + n_rows > peer.popsize:
         raise ValueError("rows beyond the population the peer exchange was sized for")
     with _timed("sample_eval"):
         rc = nat.lib().evok_sample_eval_push(objective, nat.ptr(X), ldx, mu.data_ptr(), sigma.data_ptr(), row0, n_rows, D, int(symmetric),
-                                             seed & 0xFFFFFFFFFFFFFFFF, stream_id & 0xFFFFFFFFFFFFFFFF, _offset_ptr(stream_offset), peer.world,
-                                             peer.rank, peer.peer_f, peer.peer_flags_f, peer.epoch_f, peer._counter(0), nat.stream_of(mu))
+                                             seed, stream_id, _offset_ptr(stream_offset), peer.world, peer.rank, peer.peer_f,
+                                             peer.peer_flags_f, peer.epoch_f, peer._counter(0), nat.stream_of(mu))
     nat.check(rc, "evok_sample_eval_push")
 
 
@@ -162,18 +187,12 @@ def grad_push(form: int, X: Optional[torch.Tensor], w: torch.Tensor, mu: torch.T
     Follow with `peer.reduce_gradients()`."""
     n, D = w.numel(), mu.numel()
     _vec(w, "weights"); _vec(mu, "mu"); _vec(sigma, "sigma", D)
-    ldx = 0
-    if X is not None:
-        _mat(X, "X")
-        if X.shape != (n, D):
-            raise ValueError(f"X: expected shape {(n, D)}, got {tuple(X.shape)}")
-        ldx = X.stride(0)
+    ldx = _ldx(X, n, D)
     ws = nat.workspace(mu.device, nat.lib().evok_grad_workspace_bytes(n, D), "grad")
     with _timed("grad" if X is not None else "grad_regen"):
-        rc = nat.lib().evok_grad_push(form, nat.ptr(X), ldx, w.data_ptr(), mu.data_ptr(), sigma.data_ptr(), row0, n, D, seed & 0xFFFFFFFFFFFFFFFF,
-                                      stream_id & 0xFFFFFFFFFFFFFFFF, _offset_ptr(stream_offset), scale_mu, scale_sigma, peer.world, peer.rank,
-                                      peer.peer_slots, peer.peer_flags_g, peer.epoch_g, peer._counter(1), ws.data_ptr(), ws.numel(),
-                                      nat.stream_of(mu))
+        rc = nat.lib().evok_grad_push(form, nat.ptr(X), ldx, w.data_ptr(), mu.data_ptr(), sigma.data_ptr(), row0, n, D, seed, stream_id,
+                                      _offset_ptr(stream_offset), scale_mu, scale_sigma, peer.world, peer.rank, peer.peer_slots,
+                                      peer.peer_flags_g, peer.epoch_g, peer._counter(1), ws.data_ptr(), ws.numel(), nat.stream_of(mu))
     nat.check(rc, "evok_grad_push")
 
 
@@ -247,19 +266,14 @@ def cmaes_vector_update(local_disp: torch.Tensor, shaped_disp: torch.Tensor, m: 
                         sigma: torch.Tensor, consts, csa_squared: bool, k_out: torch.Tensor, *, steps: int = 0,
                         steps_dev: Optional[torch.Tensor] = None, h_sig_out: Optional[torch.Tensor] = None) -> None:
     """In place: m, p_sigma, sigma (1-element tensor), p_c; k_out (3 floats) = coefficients of the covariance update."""
-    import ctypes
-
     d = m.numel()
     _vec(local_disp, "local_disp", d); _vec(shaped_disp, "shaped_disp", d); _vec(m, "m"); _vec(p_sigma, "p_sigma", d); _vec(p_c, "p_c", d)
     _vec(k_out, "k_out", 3)
-    if not (sigma.is_cuda and sigma.dtype == torch.float32 and sigma.numel() == 1):
-        raise ValueError("sigma: expected a 1-element float32 CUDA tensor")
-    if steps_dev is not None and not (steps_dev.is_cuda and steps_dev.dtype == torch.int64 and steps_dev.numel() == 1):
-        raise ValueError("steps_dev: expected a 1-element int64 CUDA tensor")
-    carr = (ctypes.c_float * 10)(*[float(x) for x in consts])
+    _check_scalar_sigma(sigma)
+    _check_steps_dev(steps_dev)
     nat.check(nat.lib().evok_cmaes_vector_update(local_disp.data_ptr(), shaped_disp.data_ptr(), d, m.data_ptr(), p_sigma.data_ptr(), p_c.data_ptr(),
-                                                 sigma.data_ptr(), nat.ptr(steps_dev), int(steps), carr, int(bool(csa_squared)), k_out.data_ptr(),
-                                                 nat.ptr(h_sig_out), nat.stream_of(m)), "evok_cmaes_vector_update")
+                                                 sigma.data_ptr(), nat.ptr(steps_dev), int(steps), _host_floats(consts, 10), int(bool(csa_squared)),
+                                                 k_out.data_ptr(), nat.ptr(h_sig_out), nat.stream_of(m)), "evok_cmaes_vector_update")
 
 
 def sample_eval_sq(objective: int, X: Optional[torch.Tensor], mu: torch.Tensor, sigma: torch.Tensor, q: torch.Tensor, *, n_rows: int,
@@ -269,13 +283,8 @@ def sample_eval_sq(objective: int, X: Optional[torch.Tensor], mu: torch.Tensor, 
     `sample_eval` with the same arguments.  X = None: lazy population (needs a built-in objective)."""
     D = mu.numel()
     _vec(mu, "mu"); _vec(sigma, "sigma", D); _vec(q, "q", n_rows)
-    ldx = 0
-    if X is not None:
-        _mat(X, "X")
-        if X.shape != (n_rows, D):
-            raise ValueError(f"X: expected shape {(n_rows, D)}, got {tuple(X.shape)}")
-        ldx = X.stride(0)
-    elif objective == OBJ_NONE:
+    ldx = _ldx(X, n_rows, D)
+    if X is None and objective == OBJ_NONE:
         raise ValueError("X: the samples must be written somewhere when no objective is fused into the sampler")
     if f is not None:
         _vec(f, "f", n_rows)
@@ -284,9 +293,8 @@ def sample_eval_sq(objective: int, X: Optional[torch.Tensor], mu: torch.Tensor, 
     if n_rows == 0:
         return
     with _timed("sepcma_sample"):
-        rc = nat.lib().evok_sample_eval_sq(objective, nat.ptr(X), ldx, mu.data_ptr(), sigma.data_ptr(), row0, n_rows, D,
-                                           seed & 0xFFFFFFFFFFFFFFFF, stream_id & 0xFFFFFFFFFFFFFFFF, _offset_ptr(stream_offset), nat.ptr(f),
-                                           q.data_ptr(), nat.stream_of(mu))
+        rc = nat.lib().evok_sample_eval_sq(objective, nat.ptr(X), ldx, mu.data_ptr(), sigma.data_ptr(), row0, n_rows, D, seed, stream_id,
+                                           _offset_ptr(stream_offset), nat.ptr(f), q.data_ptr(), nat.stream_of(mu))
     nat.check(rc, "evok_sample_eval_sq")
 
 
@@ -308,9 +316,9 @@ def sepcma_moments(aw: torch.Tensor, q: Optional[torch.Tensor], active: bool, D:
     wsum = torch.empty(1, dtype=torch.float32, device=dev) if wsum is None else _vec(wsum, "wsum", 1)
     ws = nat.workspace(dev, nat.lib().evok_sepcma_workspace_bytes(n, D), "grad")
     with _timed("sepcma_moments"):
-        rc = nat.lib().evok_sepcma_moments(aw.data_ptr(), nat.ptr(q), int(bool(active)), row0, n, D, seed & 0xFFFFFFFFFFFFFFFF,
-                                           stream_id & 0xFFFFFFFFFFFFFFFF, _offset_ptr(stream_offset), local.data_ptr(), S2.data_ptr(),
-                                           wsum.data_ptr(), ws.data_ptr(), ws.numel(), nat.stream_of(aw))
+        rc = nat.lib().evok_sepcma_moments(aw.data_ptr(), nat.ptr(q), int(bool(active)), row0, n, D, seed, stream_id,
+                                           _offset_ptr(stream_offset), local.data_ptr(), S2.data_ptr(), wsum.data_ptr(), ws.data_ptr(),
+                                           ws.numel(), nat.stream_of(aw))
     nat.check(rc, "evok_sepcma_moments")
     return local, S2, wsum
 
@@ -322,28 +330,23 @@ def sepcma_update(local: torch.Tensor, S2: torch.Tensor, wsum: torch.Tensor, m: 
     """In place, one kernel: m, p_sigma, sigma (1-element tensor), p_c, C, A (diagonal, D-vectors) and s = sigma * A after one separable
     CMA-ES generation with the given moments (see `sepcma_moments`).  `consts` as for `cmaes_vector_update`.  m_prev / s_prev receive
     m and s from before the update."""
-    import ctypes
-
     d = m.numel()
     _vec(local, "local", d); _vec(S2, "S2", d); _vec(wsum, "wsum", 1); _vec(m, "m"); _vec(p_sigma, "p_sigma", d); _vec(p_c, "p_c", d)
     _vec(C, "C", d); _vec(A, "A", d); _vec(s, "s", d)
     for t, name in ((m_prev, "m_prev"), (s_prev, "s_prev")):
         if t is not None:
             _vec(t, name, d)
-    if not (sigma.is_cuda and sigma.dtype == torch.float32 and sigma.numel() == 1):
-        raise ValueError("sigma: expected a 1-element float32 CUDA tensor")
-    if steps_dev is not None and not (steps_dev.is_cuda and steps_dev.dtype == torch.int64 and steps_dev.numel() == 1):
-        raise ValueError("steps_dev: expected a 1-element int64 CUDA tensor")
+    _check_scalar_sigma(sigma)
+    _check_steps_dev(steps_dev)
     if int(decompose_C_freq) < 1:
         raise ValueError("decompose_C_freq: expected a positive integer")
-    carr = (ctypes.c_float * 10)(*[float(x) for x in consts])
     lo = NAN if stdev_min is None else float(stdev_min)
     hi = NAN if stdev_max is None else float(stdev_max)
     with _timed("sepcma_update"):
         rc = nat.lib().evok_sepcma_update(local.data_ptr(), S2.data_ptr(), wsum.data_ptr(), d, m.data_ptr(), p_sigma.data_ptr(), p_c.data_ptr(),
                                           sigma.data_ptr(), C.data_ptr(), A.data_ptr(), s.data_ptr(), nat.ptr(m_prev), nat.ptr(s_prev),
-                                          nat.ptr(steps_dev), int(steps), carr, int(bool(csa_squared)), int(decompose_C_freq), lo, hi,
-                                          nat.ptr(h_sig_out), nat.stream_of(m))
+                                          nat.ptr(steps_dev), int(steps), _host_floats(consts, 10), int(bool(csa_squared)),
+                                          int(decompose_C_freq), lo, hi, nat.ptr(h_sig_out), nat.stream_of(m))
     nat.check(rc, "evok_sepcma_update")
 
 
@@ -369,8 +372,7 @@ def grad(form: int, X: torch.Tensor, w: torch.Tensor, mu: torch.Tensor, sigma: t
     _mat(X, "samples")
     n, D = X.shape
     _vec(w, "weights", n); _vec(mu, "mu", D); _vec(sigma, "sigma", D)
-    out_mu = torch.empty_like(mu) if out_mu is None else _vec(out_mu, "out_mu", D)
-    out_sigma = torch.empty_like(mu) if out_sigma is None else _vec(out_sigma, "out_sigma", D)
+    out_mu, out_sigma = _out_pair(mu, out_mu, out_sigma)
     ws = nat.workspace(X.device, nat.lib().evok_grad_workspace_bytes(n, D), "grad")
     with _timed("grad"):
         rc = nat.lib().evok_grad(form, X.data_ptr(), X.stride(0), w.data_ptr(), mu.data_ptr(), sigma.data_ptr(), n, D, scale_mu,
@@ -384,13 +386,12 @@ def grad_regen(form: int, w: torch.Tensor, mu: torch.Tensor, sigma: torch.Tensor
                out_sigma: Optional[torch.Tensor] = None, stream_offset: Optional[torch.Tensor] = None) -> tuple:
     n, D = w.numel(), mu.numel()
     _vec(w, "weights"); _vec(mu, "mu"); _vec(sigma, "sigma", D)
-    out_mu = torch.empty_like(mu) if out_mu is None else _vec(out_mu, "out_mu", D)
-    out_sigma = torch.empty_like(mu) if out_sigma is None else _vec(out_sigma, "out_sigma", D)
+    out_mu, out_sigma = _out_pair(mu, out_mu, out_sigma)
     ws = nat.workspace(mu.device, nat.lib().evok_grad_workspace_bytes(n, D), "grad")
     with _timed("grad_regen"):
-        rc = nat.lib().evok_grad_regen(form, w.data_ptr(), mu.data_ptr(), sigma.data_ptr(), row0, n, D, seed & 0xFFFFFFFFFFFFFFFF,
-                                       stream_id & 0xFFFFFFFFFFFFFFFF, _offset_ptr(stream_offset), scale_mu, scale_sigma, out_mu.data_ptr(),
-                                       out_sigma.data_ptr(), ws.data_ptr(), ws.numel(), nat.stream_of(mu))
+        rc = nat.lib().evok_grad_regen(form, w.data_ptr(), mu.data_ptr(), sigma.data_ptr(), row0, n, D, seed, stream_id,
+                                       _offset_ptr(stream_offset), scale_mu, scale_sigma, out_mu.data_ptr(), out_sigma.data_ptr(),
+                                       ws.data_ptr(), ws.numel(), nat.stream_of(mu))
     nat.check(rc, "evok_grad_regen")
     return out_mu, out_sigma
 
@@ -409,14 +410,12 @@ def grad_hybrid(form: int, X: torch.Tensor, w: torch.Tensor, mu: torch.Tensor, s
     _vec(w, "weights", n); _vec(mu, "mu", D); _vec(sigma, "sigma", D)
     if not -1 <= split <= GRAD_SPLIT_PERIOD:
         raise ValueError(f"split: expected -1 .. {GRAD_SPLIT_PERIOD}, got {split}")
-    out_mu = torch.empty_like(mu) if out_mu is None else _vec(out_mu, "out_mu", D)
-    out_sigma = torch.empty_like(mu) if out_sigma is None else _vec(out_sigma, "out_sigma", D)
+    out_mu, out_sigma = _out_pair(mu, out_mu, out_sigma)
     ws = nat.workspace(X.device, nat.lib().evok_grad_workspace_bytes(n, D), "grad")
     with _timed("grad_hybrid"):
         rc = nat.lib().evok_grad_hybrid(form, X.data_ptr(), X.stride(0), w.data_ptr(), mu.data_ptr(), sigma.data_ptr(), row0, n, D,
-                                        seed & 0xFFFFFFFFFFFFFFFF, stream_id & 0xFFFFFFFFFFFFFFFF, _offset_ptr(stream_offset), int(split),
-                                        scale_mu, scale_sigma, out_mu.data_ptr(), out_sigma.data_ptr(), ws.data_ptr(), ws.numel(),
-                                        nat.stream_of(X))
+                                        seed, stream_id, _offset_ptr(stream_offset), int(split), scale_mu, scale_sigma,
+                                        out_mu.data_ptr(), out_sigma.data_ptr(), ws.data_ptr(), ws.numel(), nat.stream_of(X))
     nat.check(rc, "evok_grad_hybrid")
     return out_mu, out_sigma
 
@@ -517,7 +516,7 @@ def sample_batched(out: torch.Tensor, mu: torch.Tensor, sigma: torch.Tensor, *, 
         raise ValueError(f"Symmetric sampling cannot be done if the number of solutions is odd: {n}")
     with _timed("sample"):
         rc = nat.lib().evok_sample_batched(out.data_ptr(), n * d, d, mu.data_ptr(), sm, sigma.data_ptr(), ss, B, n, d, int(symmetric),
-                                           seed & 0xFFFFFFFFFFFFFFFF, stream_id0 & 0xFFFFFFFFFFFFFFFF, nat.stream_of(out))
+                                           seed, stream_id0, nat.stream_of(out))
     nat.check(rc, "evok_sample_batched")
     return out
 
@@ -576,15 +575,6 @@ def grad_batched(form: int, X: torch.Tensor, w: torch.Tensor, mu: torch.Tensor, 
     return out_mu, out_sigma
 
 
-def _host_floats(values, n: int):
-    import ctypes
-
-    vals = [float(v) for v in values]
-    if len(vals) != n:
-        raise ValueError(f"expected {n} per-item scalars, got {len(vals)}")
-    return (ctypes.c_float * n)(*vals)
-
-
 def clipup_batched_(g: torch.Tensor, velocity: torch.Tensor, center: torch.Tensor, stepsizes, momenta, max_speeds) -> None:
     """In place on contiguous (items, D) tensors: one CTA per item (per-item hyper-parameters are host scalars)."""
     B, d = center.shape
@@ -616,8 +606,6 @@ def mlp_forward(params: torch.Tensor, obs: torch.Tensor, dims, acts, out: Option
     """Batched policy forward: row i of `params` (flat Linear-layer parameters) applied to row i of `obs`.
     With `obs_sum / obs_sumsq / obs_count` (the RunningNorm sums, all on the device) the observations are normalised and
     clipped while they are loaded; with `active` (bool / uint8, N) inactive policies are skipped and get zero actions."""
-    import ctypes
-
     _mat(params, "parameters"); _mat(obs, "observations")
     n = params.shape[0]
     dims = [int(d) for d in dims]
@@ -662,8 +650,6 @@ def mlp_forward_shared(params: torch.Tensor, x: torch.Tensor, dims, acts) -> tor
     """Row i of `params` (N x L flat feed-forward parameters) applied to the SHARED input batch `x` (B x in) -> N x B x out.
     First layer: one tensor-core product of the stacked weight rows of all N networks with the batch (weights read from HBM once,
     3xTF32 = fp32 accuracy); remaining layers: per-network fp32 kernel."""
-    import ctypes
-
     _mat(params, "parameters"); _mat(x, "x")
     dims = [int(d) for d in dims]
     act_ids = [ACT_IDS[a] if isinstance(a, str) else int(a) for a in acts]
