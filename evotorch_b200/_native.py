@@ -55,6 +55,8 @@ _SIGNATURES = {
                                 c_size_t, _P]),
     "evok_grad_hybrid": (c_int, [c_int, _P, c_int64, _P, _P, _P, c_int64, c_int64, c_int64, c_uint64, c_uint64, _P, c_int, c_float, c_float, _P,
                                  _P, _P, c_size_t, _P]),
+    "evok_grad_auto_split": (c_int, [c_int64]),
+    "evok_grad_power_limit_mw": (c_int64, [c_int]),
     "evok_clipup_step": (c_int, [_P, c_int64, _P, c_float, c_float, c_float, _P, _P, _P]),
     "evok_adam_step": (c_int, [_P, c_int64, _P, _P, c_int64, c_float, c_float, c_float, c_float, _P, _P, _P]),
     "evok_sgd_step": (c_int, [_P, c_int64, _P, c_int, c_float, c_float, _P, _P, _P]),

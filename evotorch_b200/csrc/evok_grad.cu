@@ -4,6 +4,9 @@
 // HBM-bound: each CTA owns a column tile (128-bit loads, 4 rows in flight per thread) and a contiguous chunk of
 // rows; partial sums go to a [chunk][2][D] workspace and a second tiny kernel adds the chunks in a fixed order
 // (deterministic, no atomics).  In the symmetric form only the even ("+") rows are read.
+#include <dlfcn.h>
+
+#include <atomic>
 #include <cstdlib>
 
 #include "evok_common.cuh"
@@ -293,9 +296,6 @@ static int launch_finalize(const float* partial, int n_chunks, int64_t D, float 
 #ifndef EVOK_GRAD_TMA_CTAS_PER_SM
 #define EVOK_GRAD_TMA_CTAS_PER_SM 3
 #endif
-#ifndef EVOK_GRAD_AUTO_SPLIT
-#define EVOK_GRAD_AUTO_SPLIT 2
-#endif
 constexpr int kTmaRows = EVOK_GRAD_TMA_ROWS;
 constexpr int kTmaStages = EVOK_GRAD_TMA_STAGES;
 constexpr int kTmaCols = 1024;
@@ -331,15 +331,20 @@ __device__ __forceinline__ void bulk_load(void* dst_smem, const void* src_gmem, 
 }
 
 // Hybrid schedule: streaming leaves the SMs' issue slots nearly idle, so part of the row groups (kTmaRows rows each) are
-// rebuilt on the SMs from the Philox counters that produced them instead of being streamed (see kAutoSplit for how much).  `split` of every kSplitPeriod
+// rebuilt on the SMs from the Philox counters that produced them instead of being streamed (see kAutoSplitFull for how much).  `split` of every kSplitPeriod
 // consecutive groups of a chunk are rebuilt, spread evenly over the period (the same mix in every CTA); split 0 streams every
 // group, kSplitPeriod rebuilds every group.  A rebuilt row is bit-identical to the stored one (same normals4 call, same
 // fmaf(sigma, z, mu) as sample_group) and the accumulation order does not depend on the schedule, so neither does the result.
+// The schedule is one kSplitPeriod-bit mask, built once per thread: bit k set = group k of every period is rebuilt.
 constexpr int kSplitPeriod = 16;
-__device__ __forceinline__ bool group_rebuilt(int64_t g, int split) {
-  const int k = (int)(g % kSplitPeriod);
-  return (k + 1) * split / kSplitPeriod > k * split / kSplitPeriod;
+__device__ __forceinline__ uint32_t rebuilt_mask(int split) {
+  uint32_t m = 0;
+#pragma unroll
+  for (int k = 0; k < kSplitPeriod; ++k)
+    if ((k + 1) * split / kSplitPeriod > k * split / kSplitPeriod) m |= 1u << k;
+  return m;
 }
+__device__ __forceinline__ bool group_rebuilt(uint32_t mask, int64_t g) { return (mask >> ((int)g & (kSplitPeriod - 1))) & 1u; }
 
 template <bool SYM>
 __global__ void __launch_bounds__(kTmaThreads, EVOK_GRAD_TMA_CTAS_PER_SM)
@@ -359,6 +364,7 @@ __global__ void __launch_bounds__(kTmaThreads, EVOK_GRAD_TMA_CTAS_PER_SM)
   const int64_t n_rows = r_end - r_begin;
   const int64_t n_groups = (n_rows + kTmaRows - 1) / kTmaRows;
   const int64_t row_stride = (SYM ? 2 : 1) * ldx;
+  const uint32_t mask = rebuilt_mask(split);
 
   if (tid == 0) {
     for (int s = 0; s < kTmaStages; ++s) {
@@ -375,7 +381,7 @@ __global__ void __launch_bounds__(kTmaThreads, EVOK_GRAD_TMA_CTAS_PER_SM)
       const uint32_t row_bytes = (uint32_t)(width * sizeof(float));
       int64_t t = 0;  // streamed groups so far: the ring advances only on these
       for (int64_t g = 0; g < n_groups; ++g) {
-        if (group_rebuilt(g, split)) continue;
+        if (group_rebuilt(mask, g)) continue;
         const int s = (int)(t % kTmaStages);
         const uint32_t use = (uint32_t)(t / kTmaStages);
         ++t;
@@ -394,15 +400,17 @@ __global__ void __launch_bounds__(kTmaThreads, EVOK_GRAD_TMA_CTAS_PER_SM)
   const int64_t col = col0 + (int64_t)tid * 4;
   const bool active = col < D;
   const uint32_t sw = key.stream_lo + (stream_off ? __ldg(stream_off) : 0u);
+  // the symmetric instantiation only ever runs the symmetric form: saying so lets c0 share sg's registers
+  const int frm = SYM ? EVOK_GRAD_SYMMETRIC : form;
   float m[4], sg[4], c1[4], c0[4];
 #pragma unroll
   for (int c = 0; c < 4; ++c) {
     sg[c] = active ? __ldg(sigma + col + c) : 1.0f;
     m[c] = active ? __ldg(mu + col + c) : 0.0f;
-    if (form == EVOK_GRAD_EXP) {
+    if (frm == EVOK_GRAD_EXP) {
       c1[c] = __fdiv_rn(1.0f, sg[c] * sg[c]);
       c0[c] = 1.0f;
-    } else if (form == EVOK_GRAD_MOMENTS) {
+    } else if (frm == EVOK_GRAD_MOMENTS) {
       c1[c] = 1.0f;
       c0[c] = 0.0f;
     } else {
@@ -432,18 +440,17 @@ __global__ void __launch_bounds__(kTmaThreads, EVOK_GRAD_TMA_CTAS_PER_SM)
       }
       need[i] = a[i] != 0.0f || b[i] != 0.0f;
     }
-    if (group_rebuilt(g, split)) {
+    if (group_rebuilt(mask, g)) {
       if (active) {
-        // all rows' Philox chains first (independent: they overlap in the pipeline), then the same FMA chain as below
+        // every row's Philox chain, unconditionally: one straight-line block keeps kTmaRows independent chains in flight per
+        // thread (their latencies overlap) and none of them waits for the weights; `need` gates only the FMA chain, the same as below
         float x[kTmaRows][4];
 #pragma unroll
         for (int i = 0; i < kTmaRows; ++i) {
-          if (need[i]) {
-            float z[4];
-            normals4(key, sw, unit0 + (uint64_t)(r0 + i), (uint32_t)(col >> 2), z);
+          float z[4];
+          normals4(key, sw, unit0 + (uint64_t)(r0 + i), (uint32_t)(col >> 2), z);
 #pragma unroll
-            for (int c = 0; c < 4; ++c) x[i][c] = fmaf(sg[c], z[c], m[c]);
-          }
+          for (int c = 0; c < 4; ++c) x[i][c] = fmaf(sg[c], z[c], m[c]);
         }
 #pragma unroll
         for (int i = 0; i < kTmaRows; ++i) {
@@ -541,14 +548,68 @@ static void launch_partial(const GradPlan& p, int form, const float* X, int64_t 
 #undef EVOK_LAUNCH_TX
 }
 
-// Rebuilt groups per kSplitPeriod when the caller leaves the choice to the library (scripts/grad_hybrid_bench.py).  On an H100
-// SXM capped at 400 W the pass is bound by power, not by bandwidth or issue: streaming alone already draws the cap (the SM clock
-// drops to ~1.1 GHz), rebuilding alone draws it at ~1.9 GHz, and both cost about the same energy per element.  A small rebuilt
-// share fills the idle issue slots of the streaming pass; more shifts the pass towards the slower all-rebuild end
-// (1 M x 10 k symmetric: split 0 7.31-7.39 ms, 2 6.72 ms, 4 6.80-6.87 ms, 8 7.30 ms, 16 7.78-7.82 ms).
-constexpr int kAutoSplit = EVOK_GRAD_AUTO_SPLIT;
+// Rebuilt groups per kSplitPeriod when the caller leaves the choice to the library, by the card's enforced power limit
+// (scripts/grad_hybrid_bench.py, 1 M x 10 k symmetric).
+// - H100 SXM capped at 400 W (kAutoSplitCapped): the pass is bound by power, not by bandwidth or issue.  Streaming alone
+//   already draws the cap (the SM clock drops to ~1.1 GHz), rebuilding alone draws it at ~1.9 GHz, and both cost about the
+//   same energy per element.  A small rebuilt share fills the idle issue slots of the streaming pass; more shifts the pass
+//   towards the slower all-rebuild end (split 0 7.31-7.39 ms, 2 6.72 ms, 4 6.80-6.87 ms, 8 7.30 ms, 16 7.78-7.82 ms; measured
+//   before the straight-line rebuild, not re-measured since).
+// - H100 80 GB HBM3 at 700 W, 1980 MHz (kAutoSplitFull): the clock holds and the two ends overlap (two sweeps: split 0
+//   6.34-6.35 ms, 2 5.63 ms, 4 4.96-4.97 ms, 5 4.65-4.67 ms, 6 4.81-5.00 ms, 8 5.25-5.31 ms, 16 7.00-7.02 ms).
+// The limit is read once per device through NVML (read-only); when it cannot be read the capped value is used.
+constexpr int kAutoSplitCapped = 2;
+constexpr int kAutoSplitFull = 5;
+constexpr int64_t kFullPowerMilliwatts = 550000;  // at or above: the full-power sweep applies
 
-// split: rebuilt groups per kSplitPeriod in the TMA kernel (0 = stream every row, -1 = kAutoSplit); rows are rebuilt from
+static int auto_split_for_power(int64_t milliwatts) { return milliwatts >= kFullPowerMilliwatts ? kAutoSplitFull : kAutoSplitCapped; }
+
+// The enforced power limit of CUDA device `device` in mW, or -1 when NVML or the device is not available.  NVML is opened
+// at run time (the library does not link it) and only read.
+static int64_t enforced_power_limit_mw(int device) {
+  char bus_id[32];
+  if (cudaDeviceGetPCIBusId(bus_id, (int)sizeof(bus_id), device) != cudaSuccess) {
+    cudaGetLastError();
+    return -1;
+  }
+  void* nvml = dlopen("libnvidia-ml.so.1", RTLD_NOW | RTLD_LOCAL);
+  if (!nvml) return -1;
+  using init_t = int (*)();
+  using by_bus_t = int (*)(const char*, void**);
+  using limit_t = int (*)(void*, unsigned int*);
+  const auto init = reinterpret_cast<init_t>(dlsym(nvml, "nvmlInit_v2"));
+  const auto shutdown = reinterpret_cast<init_t>(dlsym(nvml, "nvmlShutdown"));
+  const auto by_bus = reinterpret_cast<by_bus_t>(dlsym(nvml, "nvmlDeviceGetHandleByPciBusId_v2"));
+  const auto limit = reinterpret_cast<limit_t>(dlsym(nvml, "nvmlDeviceGetEnforcedPowerLimit"));
+  int64_t mw = -1;
+  if (init && shutdown && by_bus && limit && init() == 0) {
+    void* handle = nullptr;
+    unsigned int v = 0;
+    if (by_bus(bus_id, &handle) == 0 && limit(handle, &v) == 0) mw = v;
+    shutdown();
+  }
+  dlclose(nvml);
+  return mw;
+}
+
+// split -1 on the current device: resolved on the first call and kept for the life of the process
+static int device_auto_split() {
+  constexpr int kMaxDevices = 64;
+  static std::atomic<int> resolved[kMaxDevices];  // 0 = not yet, else split + 1
+  int device = 0;
+  if (cudaGetDevice(&device) != cudaSuccess || device < 0 || device >= kMaxDevices) {
+    cudaGetLastError();
+    return kAutoSplitCapped;
+  }
+  int s = resolved[device].load(std::memory_order_relaxed);
+  if (s == 0) {
+    s = auto_split_for_power(enforced_power_limit_mw(device)) + 1;
+    resolved[device].store(s, std::memory_order_relaxed);
+  }
+  return s - 1;
+}
+
+// split: rebuilt groups per kSplitPeriod in the TMA kernel (0 = stream every row, -1 = device_auto_split()); rows are rebuilt from
 // (seed, stream_id, *stream_off, row0), which must be the counters that sampled X from this mu and sigma.
 static int grad_impl(int form, const float* X, int64_t ldx, const float* w, const float* mu, const float* sigma, int64_t row0, int64_t n_rows,
                      int64_t D, bool regen, uint64_t seed, uint64_t stream_id, const uint32_t* stream_off, float scale_mu, float scale_sigma, float* out_mu,
@@ -583,7 +644,7 @@ static int grad_impl(int form, const float* X, int64_t ldx, const float* w, cons
     const int64_t upc = (n_units + chunks - 1) / chunks;
     const int n_chunks = (int)((n_units + upc - 1) / upc);
     dim3 grid(n_coltiles, n_chunks);
-    const int rebuilt = split < 0 ? kAutoSplit : split;
+    const int rebuilt = split < 0 ? device_auto_split() : split;
     const PhiloxKey key = make_philox_key(seed, stream_id);
     auto kernel = sym ? grad_partial_tma_kernel<true> : grad_partial_tma_kernel<false>;
     cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTmaSmemBytes);
@@ -635,6 +696,10 @@ extern "C" EVOK_API int evok_grad_hybrid(int form, const float* X, int64_t ldx, 
   return grad_impl(form, X, ldx, w, mu, sigma, row0, n_rows, D, false, seed, stream_id, stream_offset_dev, scale_mu, scale_sigma, out_mu, out_sigma, ws,
                    ws_bytes, stream, nullptr, split);
 }
+
+extern "C" EVOK_API int evok_grad_auto_split(int64_t power_limit_mw) { return auto_split_for_power(power_limit_mw); }
+
+extern "C" EVOK_API int64_t evok_grad_power_limit_mw(int device) { return enforced_power_limit_mw(device); }
 
 extern "C" EVOK_API size_t evok_sepcma_workspace_bytes(int64_t n_rows, int64_t D) {
   // the gradient partials, then one float per row chunk (plan_grad: at most kNumSMs * EVOK_GRAD_CTAS_PER_SM chunks)

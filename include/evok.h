@@ -155,6 +155,13 @@ int evok_grad_hybrid(int form, const float* X, int64_t ldx, const float* w, cons
                      int64_t n_rows, int64_t D, uint64_t seed, uint64_t stream_id, const uint32_t* stream_offset_dev, int split,
                      float scale_mu, float scale_sigma, float* out_mu, float* out_sigma, void* ws, size_t ws_bytes, void* stream);
 
+/* The split evok_grad_hybrid uses for split = -1 on a card whose enforced power limit is power_limit_mw milliwatts
+ * (<= 0: unknown, which takes the value of a power-capped card).  The choice is made once per device. */
+int evok_grad_auto_split(int64_t power_limit_mw);
+
+/* The enforced power limit of CUDA device `device` in milliwatts, read through NVML, or -1 when it cannot be read. */
+int64_t evok_grad_power_limit_mw(int device);
+
 /* ---------------------------------------------------------------------------------------------
  * K5: D-vector updates (no host synchronisation; norms are reduced on the device).
  * --------------------------------------------------------------------------------------------- */
