@@ -67,6 +67,7 @@ _SIGNATURES = {
     "evok_mlp_forward": (c_int, [_P, c_int64, _P, c_int64, _P, c_int64, c_int64, c_int, _P, _P, _P]),
     "evok_mlp_forward_prep": (c_int, [_P, c_int64, _P, c_int64, _P, c_int64, c_int64, c_int, _P, _P, _P, _P, _P, c_float, c_float, c_float, _P, _P,
                                       c_size_t, _P]),
+    "evok_mlp_forward_shared_supported": (c_int, [c_int, _P]),
     "evok_mlp_forward_shared_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int, _P]),
     "evok_mlp_forward_shared": (c_int, [_P, c_int64, c_int64, _P, c_int64, c_int64, c_int, _P, _P, _P, _P, c_size_t, _P]),
     "evok_gemm_gather_rows": (c_int, [_P, c_int64, c_int64, c_int64, c_int64, _P, c_int64, c_int64, c_int64, c_int64, c_int, _P, c_int64, _P]),

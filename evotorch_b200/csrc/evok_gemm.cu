@@ -355,9 +355,12 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
       const int row = m0 + rr;
       const float4 v = *reinterpret_cast<const float4*>(stile + rr * kEpiPitch + lane * 4);
       float e[4] = {v.x, v.y, v.z, v.w};
-      if (GATHER && p.row_bias) {  // C = act(acc + bias of this row)
-        const int64_t bi = row / p.ga_rows_per_batch;
-        const float b = __ldg(p.row_bias + bi * p.rb_batch_stride + (row - bi * p.ga_rows_per_batch));
+      if (GATHER && (p.row_bias || p.row_act != EVOK_ACT_NONE)) {  // C = act(acc + bias of this row), bias 0 without one
+        float b = 0.0f;
+        if (p.row_bias) {
+          const int64_t bi = row / p.ga_rows_per_batch;
+          b = __ldg(p.row_bias + bi * p.rb_batch_stride + (row - bi * p.ga_rows_per_batch));
+        }
         for (int t = 0; t < 4; ++t) e[t] = p.row_act == EVOK_ACT_NONE ? e[t] + b : gemm_act(e[t] + b, p.row_act);
       }
       if (affine) {

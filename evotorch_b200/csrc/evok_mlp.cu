@@ -411,23 +411,42 @@ extern "C" EVOK_API size_t evok_mlp_forward_shared_workspace_bytes(int64_t N, in
   return (size_t)chunk * dims_host[1] * ldh * 4 + 256 + evok_gemm_gather_rows_workspace_bytes(B, dims_host[0]);
 }
 
+// Shared memory of mlp_tail_kernel: two [width][33] activation tiles of the widest layer after the input, and the largest staged
+// layer (weights + bias) among the layers 1 .. n-1.  mlp_tail2_kernel, where it is taken instead, never needs more.
+constexpr size_t kTailMaxSmem = 200 * 1024;
+static size_t mlp_tail_smem_bytes(int n_layers, const int32_t* dims) {
+  size_t maxw = 0, wmax = 0;
+  for (int l = 1; l <= n_layers; ++l) maxw = dims[l] > (int)maxw ? (size_t)dims[l] : maxw;
+  for (int l = 1; l < n_layers; ++l) {
+    const size_t wl = (size_t)dims[l] * dims[l + 1] + dims[l + 1];
+    if (wl > wmax) wmax = wl;
+  }
+  return (2 * maxw * (kTailSamples + 1) + wmax) * sizeof(float);
+}
+
+extern "C" EVOK_API int evok_mlp_forward_shared_supported(int n_layers, const int32_t* dims_host) {
+  if (!dims_host || n_layers < 2 || n_layers > kMlpMaxLayers) return 0;
+  for (int l = 0; l <= n_layers; ++l) {
+    if (dims_host[l] < 1 || dims_host[l] > kMlpMaxWidth) return 0;
+    if (l >= 1 && dims_host[l] > kTailMaxWidth) return 0;
+  }
+  return mlp_tail_smem_bytes(n_layers, dims_host) <= kTailMaxSmem ? 1 : 0;
+}
+
 // out[i, b, :] = net_i(X[b, :]) for N flat parameter rows and ONE shared input batch X (B x dims[0], 16-byte aligned rows).
 extern "C" EVOK_API int evok_mlp_forward_shared(const float* params, int64_t ldp, int64_t N, const float* X, int64_t ldx, int64_t B, int n_layers,
                                                 const int32_t* dims_host, const int32_t* acts_host, float* out, void* ws, size_t ws_bytes,
                                                 void* stream) {
   if (!params || !X || !out || !dims_host || !acts_host || !ws) return EVOK_E_NULLPTR;
-  if (n_layers < 2 || n_layers > kMlpMaxLayers || N < 0 || B <= 0) return EVOK_E_BADSIZE;
+  if (!evok_mlp_forward_shared_supported(n_layers, dims_host) || N < 0 || B <= 0) return EVOK_E_BADSIZE;
   MlpSpec spec;
   spec.n_layers = n_layers;
   int64_t off = 0;
   int maxw = 0;
   for (int l = 0; l <= n_layers; ++l) {
-    const int d = dims_host[l];
-    if (d < 1 || d > kMlpMaxWidth) return EVOK_E_BADSIZE;
-    spec.dims[l] = d;
-    if (l >= 1 && d > maxw) maxw = d;
+    spec.dims[l] = dims_host[l];
+    if (l >= 1 && dims_host[l] > maxw) maxw = dims_host[l];
   }
-  if (maxw > kTailMaxWidth) return EVOK_E_BADSIZE;
   for (int l = 0; l < n_layers; ++l) {
     if (acts_host[l] < EVOK_ACT_NONE || acts_host[l] > EVOK_ACT_SIGMOID) return EVOK_E_BADENUM;
     spec.acts[l] = acts_host[l];
@@ -452,13 +471,7 @@ extern "C" EVOK_API int evok_mlp_forward_shared(const float* params, int64_t ldp
   // read activations
   MlpSpec tail_spec = spec;
   tail_spec.acts[0] = EVOK_ACT_NONE;
-  size_t wmax = 0;  // largest staged layer (weights + bias) among the layers 1 .. n-1
-  for (int l = 1; l < n_layers; ++l) {
-    const size_t wl = (size_t)spec.dims[l] * spec.dims[l + 1] + spec.dims[l + 1];
-    if (wl > wmax) wmax = wl;
-  }
-  const size_t smem = (2 * (size_t)maxw * (kTailSamples + 1) + wmax) * sizeof(float);
-  if (smem > 200 * 1024) return EVOK_E_BADSIZE;  // a hidden layer too wide to stage: the caller falls back to the generic path
+  const size_t smem = mlp_tail_smem_bytes(n_layers, dims_host);  // <= kTailMaxSmem: checked above
   static size_t attr_smem = 0;
   if (smem > attr_smem) {
     if (cudaFuncSetAttribute(mlp_tail_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return (int)cudaGetLastError();

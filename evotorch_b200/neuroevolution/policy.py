@@ -127,12 +127,13 @@ class Policy:
         """Row i of `parameters` (N x L) applied to the SAME input batch `x` (B x in) -> N x B x out: a population scored on a
         common minibatch (supervisedne.py:337-347).  For feed-forward nets on CUDA float32 the layers run on the kernels of
         `ops.mlp_forward_shared` (first layer: one tensor-core product of the stacked weight rows of all N networks with the
-        shared batch); anything else goes through `vmap(functional_call)`."""
+        shared batch); anything else, including nets those kernels cannot take (`ops.mlp_forward_shared_supported`), goes
+        through `vmap(functional_call)`."""
         if parameters.ndim != 2 or parameters.shape[1] != self.parameter_length:
             raise ValueError(f"Expected parameters of shape (N, {self.parameter_length}), got {tuple(parameters.shape)}")
         if self._spec is not None and ops.uses_kernels(parameters) and ops.uses_kernels(x) and x.ndim == 2 and parameters.stride(1) == 1:
             dims, acts = self._spec
-            if len(acts) >= 2 and max(dims[1:]) <= 512:
+            if ops.mlp_forward_shared_supported(dims):
                 return ops.mlp_forward_shared(parameters, x.contiguous(), dims, acts)
         return vmap(self._call_one, in_dims=(0, None))(parameters, x)
 

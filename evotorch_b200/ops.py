@@ -646,18 +646,27 @@ def mlp_forward(params: torch.Tensor, obs: torch.Tensor, dims, acts, out: Option
     return out
 
 
+def mlp_forward_shared_supported(dims) -> bool:
+    """Whether `mlp_forward_shared` takes a net with these layer widths (the library's own rule: 2 to 8 layers, hidden and output
+    widths <= 512, and every layer after the first small enough for its kernel to stage in shared memory)."""
+    dims = [int(d) for d in dims]
+    return bool(nat.lib().evok_mlp_forward_shared_supported(len(dims) - 1, (ctypes.c_int32 * len(dims))(*dims)))
+
+
 def mlp_forward_shared(params: torch.Tensor, x: torch.Tensor, dims, acts) -> torch.Tensor:
     """Row i of `params` (N x L flat feed-forward parameters) applied to the SHARED input batch `x` (B x in) -> N x B x out.
     First layer: one tensor-core product of the stacked weight rows of all N networks with the batch (weights read from HBM once,
-    3xTF32 = fp32 accuracy); remaining layers: per-network fp32 kernel."""
+    3xTF32 = fp32 accuracy); remaining layers: per-network fp32 kernel.  Nets outside `mlp_forward_shared_supported` raise."""
     _mat(params, "parameters"); _mat(x, "x")
     dims = [int(d) for d in dims]
     act_ids = [ACT_IDS[a] if isinstance(a, str) else int(a) for a in acts]
     n, B = params.shape[0], x.shape[0]
     if x.shape[1] != dims[0]:
         raise ValueError(f"x: expected {dims[0]} columns, got {x.shape[1]}")
-    if len(act_ids) < 2 or max(dims[1:]) > 512:
-        raise ValueError("mlp_forward_shared handles nets with >= 2 layers and widths <= 512")
+    if len(act_ids) != len(dims) - 1 or not mlp_forward_shared_supported(dims):
+        raise ValueError(f"mlp_forward_shared does not handle layer widths {dims}: it takes 2 to 8 layers, widths <= 512 after the "
+                         "input, and layers after the first that fit its shared-memory staging (use Policy.forward_shared, which "
+                         "falls back to vmap)")
     d_arr = (ctypes.c_int32 * len(dims))(*dims)
     a_arr = (ctypes.c_int32 * len(act_ids))(*act_ids)
     lib = nat.lib()

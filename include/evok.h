@@ -227,7 +227,10 @@ int evok_mlp_forward_prep(const float* params, int64_t ldp, const float* obs, in
  * (evok_gemm_gather_rows: the weight rows are gathered from the flat parameter rows -- any 4-byte alignment -- straight into the swizzled
  * operand tiles, so every parameter is read from HBM once; bias and activation in the epilogue), the remaining (small, per-network)
  * layers run in a second kernel on the staged activations.  out: [N][B][dims[n_layers]].  n_layers >= 2, hidden widths <= 512,
- * X 16-byte aligned with ldx % 4 == 0. */
+ * X 16-byte aligned with ldx % 4 == 0.  evok_mlp_forward_shared_supported: 1 if evok_mlp_forward_shared takes these layer widths,
+ * 0 if it would return EVOK_E_BADSIZE (also when a layer after the first is too wide for its second kernel to stage in shared memory:
+ * e.g. 8-256-256-2 or 8-512-34); needs no device. */
+int evok_mlp_forward_shared_supported(int n_layers, const int32_t* dims_host);
 size_t evok_mlp_forward_shared_workspace_bytes(int64_t N, int64_t B, int n_layers, const int32_t* dims_host);
 int evok_mlp_forward_shared(const float* params, int64_t ldp, int64_t N, const float* X, int64_t ldx, int64_t B, int n_layers,
                             const int32_t* dims_host, const int32_t* acts_host, float* out, void* ws, size_t ws_bytes, void* stream);

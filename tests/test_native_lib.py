@@ -45,6 +45,24 @@ def test_host_side_argument_checks_need_no_gpu(libpath):
     assert lib.evok_clipup_step(None, 4, None, 0.1, 0.9, 0.2, None, None, None) == -1
 
 
+def test_shared_forward_eligibility_needs_no_gpu(libpath):
+    """evok_mlp_forward_shared_supported: the nets the shared-minibatch forward takes.  Its second kernel stages two [width][33]
+    activation tiles and the largest later layer in at most 200 KB of shared memory; the pairs below sit on either side of that."""
+    from evotorch_b200 import ops
+
+    def ok(*dims):
+        return bool(nat.lib().evok_mlp_forward_shared_supported(len(dims) - 1, (ctypes.c_int32 * len(dims))(*dims)))
+
+    assert ok(376, 256, 17) and ok(6, 16, 3) and ok(33, 40, 24, 5) and ok(8, 512, 2) and ok(2048, 508, 32)
+    assert ok(8, 512, 33) and not ok(8, 512, 34)  # 202 884 B / 204 936 B
+    assert ok(8, 195, 195, 2) and not ok(8, 196, 196, 2)  # 204 360 B / 206 192 B
+    assert not ok(8, 256, 256, 2) and not ok(8, 512, 40) and not ok(8, 200, 200, 2)
+    assert not ok(8, 513, 2) and not ok(2049, 16, 2) and not ok(8, 0, 2)  # widths
+    assert not ok(8, 16) and ok(*([8] * 9)) and not ok(*([8] * 10))  # 2 .. 8 layers
+    assert not nat.lib().evok_mlp_forward_shared_supported(2, None)
+    assert ops.mlp_forward_shared_supported([8, 512, 33]) and not ops.mlp_forward_shared_supported([8, 512, 34])
+
+
 def test_kernels_are_sm90a_sass(libpath):
     import shutil
     import subprocess
