@@ -614,7 +614,8 @@ static int device_auto_split() {
 static int grad_impl(int form, const float* X, int64_t ldx, const float* w, const float* mu, const float* sigma, int64_t row0, int64_t n_rows,
                      int64_t D, bool regen, uint64_t seed, uint64_t stream_id, const uint32_t* stream_off, float scale_mu, float scale_sigma, float* out_mu,
                      float* out_sigma, void* ws, size_t ws_bytes, void* stream, const GradPush* push = nullptr, int split = 0) {
-  if (!w || !mu || !sigma || !ws || (!regen && !X) || (!push && (!out_mu || !out_sigma))) return EVOK_E_NULLPTR;
+  // an empty shard has no weights to point at (an empty CUDA tensor's data pointer is NULL)
+  if ((!w && n_rows != 0) || !mu || !sigma || !ws || (!regen && !X) || (!push && (!out_mu || !out_sigma))) return EVOK_E_NULLPTR;
   if (form < EVOK_GRAD_SEPARABLE || form > EVOK_GRAD_MOMENTS) return EVOK_E_BADENUM;
   if (n_rows < 0 || D <= 0 || row0 < 0 || (!regen && ldx < D) || split < -1 || split > kSplitPeriod) return EVOK_E_BADSIZE;
   const bool sym = form == EVOK_GRAD_SYMMETRIC;
@@ -625,7 +626,6 @@ static int grad_impl(int form, const float* X, int64_t ldx, const float* w, cons
   const bool vec_ok = regen ? true : ((D % 4 == 0) && (ldx % 4 == 0) && aligned16(X));
   // symmetric sampling keys its counters by direction; the regenerating kernel must use the same unit index
   const uint64_t unit0 = (uint64_t)(sym ? row0 / 2 : row0);
-  GradPlan p = plan_grad(n_units, D, vec_ok);
   float* partial = (float*)ws;
   if (n_units == 0 && push) return launch_finalize(partial, 0, D, scale_mu, scale_sigma, nullptr, nullptr, push, st);  // zeros + this rank's flag
   if (n_units == 0) {
@@ -633,6 +633,7 @@ static int grad_impl(int form, const float* X, int64_t ldx, const float* w, cons
     cudaMemsetAsync(out_sigma, 0, (size_t)D * 4, st);
     return 0;
   }
+  const GradPlan p = plan_grad(n_units, D, vec_ok);  // after the empty case: plan_grad divides by the units per chunk
   // read per call (a getenv is ~100 ns): the parity tests run both implementations in one process
   const char* tma_env = getenv("EVOK_GRAD_TMA");
   const int use_tma = tma_env ? atoi(tma_env) : EVOK_GRAD_TMA_DEFAULT;

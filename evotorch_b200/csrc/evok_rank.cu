@@ -696,7 +696,7 @@ extern "C" EVOK_API int evok_rank_sharded(int method, const float* f_local, int6
                                           const int64_t* row_offsets_host, void* const* peer_keys_host, void* const* peer_fsum_host,
                                           void* const* peer_flags_host, uint64_t* epoch_dev, uint32_t* done_dev, uint32_t* err_dev,
                                           uint64_t timeout_ns, float* w_local, float* mean_out, void* ws, size_t ws_bytes, void* stream) {
-  if (!f_local || !row_offsets_host || !peer_keys_host || !peer_fsum_host || !peer_flags_host || !epoch_dev || !done_dev || !err_dev || !w_local || !ws)
+  if (!row_offsets_host || !peer_keys_host || !peer_fsum_host || !peer_flags_host || !epoch_dev || !done_dev || !err_dev || !ws)
     return EVOK_E_NULLPTR;
   if (method != EVOK_RANK_CENTERED && method != EVOK_RANK_LINEAR && method != EVOK_RANK_NES) return EVOK_E_BADENUM;
   if (world < 1 || world > EVOK_MAX_PEERS || rank < 0 || rank >= world) return EVOK_E_BADSIZE;
@@ -707,6 +707,8 @@ extern "C" EVOK_API int evok_rank_sharded(int method, const float* f_local, int6
     tab.off[r] = row_offsets_host[r];
   }
   const int64_t my_off = tab.off[rank], n_local = tab.off[rank + 1] - my_off;
+  // an empty shard has no fitnesses or utilities to point at (an empty CUDA tensor's data pointer is NULL)
+  if (n_local > 0 && (!f_local || !w_local)) return EVOK_E_NULLPTR;
   const SortPlan p = make_plan(n_local > 0 ? n_local : 1);
   if (ws_bytes < p.total) return EVOK_E_WORKSPACE;
   PeerSink keys_sink{}, fsum_sink{};

@@ -51,9 +51,30 @@ class PeerExchange:
     def __init__(self, popsize: int, solution_length: int, device: torch.device, *, timeout_ns: int = DEFAULT_TIMEOUT_NS):
         if not (dist.is_available() and dist.is_initialized()):
             raise RuntimeError("PeerExchange needs an initialised torch.distributed process group (it carries the IPC handles)")
-        self.rank, self.world = dist.get_rank(), dist.get_world_size()
-        if self.world > 16:
+        self._configure(popsize, solution_length, device, dist.get_rank(), dist.get_world_size(), timeout_ns)
+        lib = nat.lib()
+        with torch.cuda.device(self.device):
+            base, handle = ctypes.c_void_p(), ctypes.create_string_buffer(64)
+            nat.check(lib.evok_peer_alloc(self.nbytes, ctypes.byref(base), handle), "evok_peer_alloc")
+            handles = [None] * self.world
+            dist.all_gather_object(handles, handle.raw)
+            peer_bases = []
+            for p in range(self.world):
+                if p == self.rank:
+                    peer_bases.append(int(base.value))
+                    continue
+                mapped = ctypes.c_void_p()
+                nat.check(lib.evok_peer_open(ctypes.create_string_buffer(handles[p], 64), ctypes.byref(mapped)), "evok_peer_open")
+                peer_bases.append(int(mapped.value))
+            self._lay_out(int(base.value), peer_bases)
+        torch.cuda.synchronize(self.device)
+        dist.barrier()  # nobody writes into a peer before that peer has zeroed and published its buffer
+
+    def _configure(self, popsize: int, solution_length: int, device, rank: int, world: int, timeout_ns: int) -> None:
+        """Sizes and the byte offsets of the buffer sections; `nbytes` is the size of every rank's exchange buffer."""
+        if world > 16:
             raise ValueError("a peer exchange spans at most 16 GPUs (one NVLink domain)")
+        self.rank, self.world = int(rank), int(world)
         self.device = torch.device(device)
         self.popsize, self.solution_length, self.timeout_ns = int(popsize), int(solution_length), int(timeout_ns)
         n, d, r = self.popsize, self.solution_length, self.world
@@ -65,21 +86,11 @@ class PeerExchange:
         self._off_fsum = self._off_keys + _align(4 * n)         # ... and one local fitness sum (f64) per rank
         self.nbytes = self._off_fsum + _align(8 * r)
 
-        lib = nat.lib()
-        with torch.cuda.device(self.device):
-            base, handle = ctypes.c_void_p(), ctypes.create_string_buffer(64)
-            nat.check(lib.evok_peer_alloc(self.nbytes, ctypes.byref(base), handle), "evok_peer_alloc")
-            self._base = int(base.value)
-            handles = [None] * r
-            dist.all_gather_object(handles, handle.raw)
-            self._peer_bases = []
-            for p in range(r):
-                if p == self.rank:
-                    self._peer_bases.append(self._base)
-                    continue
-                mapped = ctypes.c_void_p()
-                nat.check(lib.evok_peer_open(ctypes.create_string_buffer(handles[p], 64), ctypes.byref(mapped)), "evok_peer_open")
-                self._peer_bases.append(int(mapped.value))
+    def _lay_out(self, base: int, peer_bases: list) -> None:
+        """The pointer tables the kernels take, the local views and the local (unshared) state, from this rank's buffer `base`
+        (zeroed, `nbytes` long) and every rank's buffer address as mapped in this process (`peer_bases[self.rank] == base`)."""
+        n, d, r = self.popsize, self.solution_length, self.world
+        self._base, self._peer_bases = int(base), [int(b) for b in peer_bases]
 
         def table(offset: int):
             return (ctypes.c_void_p * r)(*[b + offset for b in self._peer_bases])
@@ -97,8 +108,6 @@ class PeerExchange:
         self._rank_counters = torch.zeros(4, dtype=torch.int32, device=self.device)  # sharded ranking: hist-scan / push / merge
         self._mean_eval = torch.zeros(1, dtype=torch.float32, device=self.device)
         self.reduced = torch.empty(2 * d, dtype=torch.float32, device=self.device)
-        torch.cuda.synchronize(self.device)
-        dist.barrier()  # nobody writes into a peer before that peer has zeroed and published its buffer
 
     # pointers of the local state
     @property
