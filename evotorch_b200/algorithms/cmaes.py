@@ -74,7 +74,8 @@ class CMAES(SearchAlgorithm, SinglePopulationAlgorithmMixin, CUDAGraphMixin):
             center_init = problem.generate_values(1)
         elif isinstance(center_init, Solution):
             center_init = center_init.values.clone()
-        self.m = problem.make_tensor(center_init).squeeze().clone()
+        # reshape, not squeeze: with solution_length 1 a squeezed (1, 1) centre would be a 0-d tensor and fail the check below
+        self.m = problem.make_tensor(center_init).reshape(-1).clone()
         if not (self.m.ndim == 1 and len(self.m) == d):
             raise ValueError(f"The initial center point was expected as a vector of length {d}."
                              " However, the provided `center_init` has (or implies) a different shape.")

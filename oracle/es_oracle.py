@@ -479,10 +479,14 @@ def update_exp_gaussian(mu, A, A_inv, grads, lr_mu, lr_sigma, opt_mu=None) -> tu
 
 class CMAESState:
     """Hyper-parameters and state of the reference CMAES for the non-separable case
-    (algorithms/cmaes.py:279-385), computed in float64 then held as python floats / fp32 arrays."""
+    (algorithms/cmaes.py:279-385), computed in float64 then held as python floats / fp32 arrays.
+    The `*_ratio` arguments scale the default hyper-parameters as the reference's do (each one before the
+    defaults that depend on it); `stdev_min` / `stdev_max` bound sqrt(diag(C)) * sigma (`cmaes_limit_stdev`)."""
 
     def __init__(self, d: int, popsize: int, stdev_init: float, center, active: bool = True, c_m: float = 1.0,
-                 csa_squared: bool = False, limit_C_decomposition: bool = True):
+                 csa_squared: bool = False, limit_C_decomposition: bool = True, c_sigma_ratio: float = 1.0,
+                 damp_sigma_ratio: float = 1.0, c_c_ratio: float = 1.0, c_1_ratio: float = 1.0, c_mu_ratio: float = 1.0,
+                 stdev_min: Optional[float] = None, stdev_max: Optional[float] = None):
         self.d = int(d)
         self.popsize = int(popsize)
         self.mu_count = int(math.floor(popsize / 2))
@@ -498,11 +502,12 @@ class CMAESState:
         self.c_m = c_m
         self.active = active
         self.csa_squared = csa_squared
-        self.c_sigma = (mu_eff + 2.0) / (d + mu_eff + 3)
-        self.damp_sigma = 1 + 2 * max(0.0, math.sqrt((mu_eff - 1) / (d + 1)) - 1) + self.c_sigma
-        self.c_c = (4 + mu_eff / d) / (d + (4 + 2 * mu_eff / d))
-        self.c_1 = min(1, popsize / 6) * 2 / ((d + 1.3) ** 2.0 + mu_eff)
-        self.c_mu = min(1 - self.c_1, 2 * ((0.25 + mu_eff - 2 + (1 / mu_eff)) / ((d + 2) ** 2.0 + mu_eff)))
+        self.stdev_min, self.stdev_max = stdev_min, stdev_max
+        self.c_sigma = c_sigma_ratio * ((mu_eff + 2.0) / (d + mu_eff + 3))
+        self.damp_sigma = damp_sigma_ratio * (1 + 2 * max(0.0, math.sqrt((mu_eff - 1) / (d + 1)) - 1) + self.c_sigma)
+        self.c_c = c_c_ratio * ((4 + mu_eff / d) / (d + (4 + 2 * mu_eff / d)))
+        self.c_1 = c_1_ratio * (min(1, popsize / 6) * 2 / ((d + 1.3) ** 2.0 + mu_eff))
+        self.c_mu = c_mu_ratio * min(1 - self.c_1, 2 * ((0.25 + mu_eff - 2 + (1 / mu_eff)) / ((d + 2) ** 2.0 + mu_eff)))
         self.variance_discount_sigma = math.sqrt(self.c_sigma * (2 - self.c_sigma) * mu_eff)
         self.variance_discount_c = math.sqrt(self.c_c * (2 - self.c_c) * mu_eff)
         pos = pos / np.sum(pos, dtype=F32)
@@ -545,20 +550,34 @@ def cmaes_assign_weights(state: CMAESState, f, sense: str) -> np.ndarray:
     return state.weights[ranks]
 
 
-def cmaes_update(state: CMAESState, Z, Y, assigned_weights) -> None:
-    """cmaes.py:454-606 (_step after evaluation), non-separable branch; float64 accumulation,
-    fp32 state."""
+def cmaes_recombine(state: CMAESState, Z, Y, assigned_weights) -> tuple:
+    """update_m :454-481, the sums only: local = sum_i w_i z_i and shaped = sum_i w_i y_i over the mu best (the top-mu
+    weights are exactly the positive ones: stable order by weight desc), in float64."""
     Z, Y, aw = _f32(Z), _f32(Y), _f32(assigned_weights)
-    d = state.d
-    # update_m :454-481 (top-mu weights are exactly the positive ones: stable order by weight desc)
     top = np.argsort(-aw.astype(np.float64), kind="stable")[: state.mu_count]
     tw = aw[top].astype(np.float64)
     local_disp = (tw[:, None] * Z[top].astype(np.float64)).sum(axis=0)
     shaped_disp = (tw[:, None] * Y[top].astype(np.float64)).sum(axis=0)
-    state.m = (state.m + F32(state.c_m) * state.sigma * shaped_disp.astype(F32)).astype(F32)
+    return local_disp, shaped_disp
+
+
+def cmaes_h_sig(state: CMAESState, pnorm: float) -> tuple:
+    """_h_sig :31-46 from ||p_sigma|| after this generation's update and the generation counter BEFORE its increment.
+    Returns (h_sig, margin): margin = |lhs - rhs| / rhs of the comparison lhs < rhs that decides it."""
+    d = state.d
+    squared_sum = pnorm**2 / (1 - (1 - state.c_sigma) ** (2 * state.steps + 1))
+    lhs, rhs = (squared_sum / d) - 1, 1 + 4.0 / (d + 1)
+    return (1.0 if lhs < rhs else 0.0), abs(lhs - rhs) / rhs
+
+
+def cmaes_vector_step(state: CMAESState, local_disp, shaped_disp) -> float:
+    """update_m (with the OLD sigma), update_p_sigma, update_sigma, _h_sig and update_p_c (:454-517, :31-46): the work of
+    evok_cmaes_vector_update.  Updates the state; returns h_sig."""
+    d = state.d
+    state.m = (state.m + F32(state.c_m) * state.sigma * np.asarray(shaped_disp).astype(F32)).astype(F32)
     # update_p_sigma :483-490
     state.p_sigma = (F32(1 - state.c_sigma) * state.p_sigma
-                     + F32(state.variance_discount_sigma) * local_disp.astype(F32)).astype(F32)
+                     + F32(state.variance_discount_sigma) * np.asarray(local_disp).astype(F32)).astype(F32)
     # update_sigma :492-507
     pnorm = float(np.sqrt(np.sum(state.p_sigma.astype(np.float64) ** 2)))
     if state.csa_squared:
@@ -566,28 +585,76 @@ def cmaes_update(state: CMAESState, Z, Y, assigned_weights) -> None:
     else:
         expo = pnorm / state.unbiased_expectation - 1
     state.sigma = F32(state.sigma * np.exp(F32((state.c_sigma / state.damp_sigma) * expo)))
-    # _h_sig :31-46 (uses the generation counter BEFORE increment)
-    squared_sum = pnorm**2 / (1 - (1 - state.c_sigma) ** (2 * state.steps + 1))
-    h_sig = 1.0 if (squared_sum / d) - 1 < 1 + 4.0 / (d + 1) else 0.0
+    h_sig, _ = cmaes_h_sig(state, pnorm)
     # update_p_c :509-517
     state.p_c = (F32(1 - state.c_c) * state.p_c
-                 + F32(h_sig * state.variance_discount_c) * shaped_disp.astype(F32)).astype(F32)
-    # update_C :519-553
-    w = aw.astype(np.float64)
-    if state.active:
-        zn2 = (Z.astype(np.float64) ** 2).sum(axis=1)
-        w = np.where(w > 0, w, d * w / zn2)
+                 + F32(h_sig * state.variance_discount_c) * np.asarray(shaped_disp).astype(F32)).astype(F32)
+    return h_sig
+
+
+def cmaes_covariance_coefficients(state: CMAESState, h_sig: float) -> tuple:
+    """update_C :537-541: (c1a, weighted_pc).  The update C <- C + c1a (pc pc^T - C) + c_mu (S - sum(w) C), pc =
+    weighted_pc p_c, is k1 C + k0 S + k2 p_c p_c^T with the three coefficients of `cmaes_k`."""
     c1a = state.c_1 * (1 - (1 - h_sig**2) * state.c_c * (2 - state.c_c))
     weighted_pc = (state.c_1 / (c1a + 1e-23)) ** 0.5
+    return c1a, weighted_pc
+
+
+def cmaes_k(state: CMAESState, h_sig: float) -> tuple:
+    """(k0, k1, k2) = (c_mu, 1 - c1a - c_mu sum(w), c1a weighted_pc^2): what evok_cmaes_vector_update writes to `k_out`."""
+    c1a, weighted_pc = cmaes_covariance_coefficients(state, h_sig)
+    return state.c_mu, 1 - c1a - state.c_mu * float(np.sum(state.weights, dtype=F32)), c1a * weighted_pc**2
+
+
+def cmaes_active_weights(state: CMAESState, Z, assigned_weights) -> np.ndarray:
+    """update_C :531-535: w_i > 0 ? w_i : d w_i / ||z_i||^2 with active weights, w unchanged otherwise (float64)."""
+    w = _f32(assigned_weights).astype(np.float64)
+    if state.active:
+        zn2 = (_f32(Z).astype(np.float64) ** 2).sum(axis=1)
+        w = np.where(w > 0, w, state.d * w / zn2)
+    return w
+
+
+def cmaes_covariance_update(state: CMAESState, Y, w, c1a: float, weighted_pc: float) -> None:
+    """update_C :543-553: the rank-1 and rank-mu update of C with the (active-reweighted) weights `w`."""
     pc = weighted_pc * state.p_c.astype(np.float64)
     C64 = state.C.astype(np.float64)
     r1 = c1a * (np.outer(pc, pc) - C64)
-    Y64 = Y.astype(np.float64)
+    Y64 = _f32(Y).astype(np.float64)
     rmu = state.c_mu * ((Y64.T * w) @ Y64 - float(np.sum(state.weights, dtype=F32)) * C64)
     state.C = (C64 + r1 + rmu).astype(F32)
-    # decompose_C :555-565
-    if (state.steps + 1) % state.decompose_C_freq == 0:
-        state.A = np.linalg.cholesky(state.C.astype(np.float64)).astype(F32)
+
+
+def cmaes_limit_stdev(state: CMAESState) -> None:
+    """_limit_stdev :49-79, non-separable: only the diagonal of C is rewritten, to (clamp(sigma sqrt(C_ii), lo, hi) / sigma)^2."""
+    if state.stdev_min is None and state.stdev_max is None:
+        return
+    sigma = np.float64(state.sigma)
+    stdevs = np.clip(sigma * np.sqrt(np.diag(state.C).astype(np.float64)), state.stdev_min, state.stdev_max)
+    C = state.C.copy()
+    np.fill_diagonal(C, ((stdevs / sigma) ** 2).astype(F32))
+    state.C = C
+
+
+def cmaes_decomposition_due(state: CMAESState) -> bool:
+    """decompose_C :555-565: A is refactorised on the generations where (steps + 1) % decompose_C_freq == 0."""
+    return (state.steps + 1) % state.decompose_C_freq == 0
+
+
+def cmaes_decompose(state: CMAESState) -> None:
+    state.A = np.linalg.cholesky(state.C.astype(np.float64)).astype(F32)
+
+
+def cmaes_update(state: CMAESState, Z, Y, assigned_weights) -> None:
+    """cmaes.py:454-606 (_step after evaluation), non-separable branch; float64 accumulation,
+    fp32 state."""
+    local_disp, shaped_disp = cmaes_recombine(state, Z, Y, assigned_weights)
+    h_sig = cmaes_vector_step(state, local_disp, shaped_disp)
+    c1a, weighted_pc = cmaes_covariance_coefficients(state, h_sig)
+    cmaes_covariance_update(state, Y, cmaes_active_weights(state, Z, assigned_weights), c1a, weighted_pc)
+    cmaes_limit_stdev(state)
+    if cmaes_decomposition_due(state):
+        cmaes_decompose(state)
     state.steps += 1
 
 

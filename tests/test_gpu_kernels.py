@@ -506,7 +506,8 @@ def test_user_objective_and_torch_rng_paths_on_cuda():
     close(N(X[0::2] + X[1::2]), np.broadcast_to(2 * N(st.status["center"]), (250, 64)), rtol=0, atol=1e-5)
 
 
-@pytest.mark.parametrize("M,N,K", [(128, 256, 32), (4096, 1024, 1024), (1024, 1024, 4096), (100, 70, 36), (129, 257, 40), (12, 6, 6), (300, 513, 1000)])
+@pytest.mark.parametrize("M,N,K", [(128, 256, 32), (4096, 1024, 1024), (1024, 1024, 4096), (100, 70, 36), (129, 257, 40), (12, 6, 6), (300, 513, 1000),
+                                   (7, 3, 3), (24, 1025, 1025), (8193, 129, 129), (4, 1, 1)])  # CMA-ES sampling shapes: Z (n x D) A^T
 def test_tensor_core_gemm_matches_float64(M, N, K):
     g = torch.Generator(device=DEV).manual_seed(M + N + K)
     A = torch.randn(M, K, device=DEV, generator=g)

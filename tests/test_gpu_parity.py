@@ -407,29 +407,40 @@ def test_cmaes_cuda_graph_replay_equals_eager_stepping():
 
 def test_rank_table_and_affine_syrk_kernels():
     """evok_rank_table == weights[rank] by argsort / scatter / gather (cmaes.py:445-451) bit for bit; evok_gemm_nt_affine ==
-    k0 Y^T diag(w) Y + k1 C + k2 u u^T in float64 (direct epilogue and split-K reduction, in place)."""
+    k0 Y^T diag(w) Y + k1 C + k2 u u^T in float64 (direct epilogue and split-K reduction, in place).  The ranking runs on both
+    sides of the counting / radix switch (8192 / 8193) with +-0, NaN and +-inf keys in both senses; the SYRK also at the (d, n)
+    shapes CMA-ES runs (default popsizes, 8193 rows), in place, into a separate `out` and without the rank-1 vector."""
     g = torch.Generator(device=DEV).manual_seed(3)
-    for n in (12, 4096, 20000):
-        f = torch.round(torch.randn(n, device=DEV, generator=g) * 100) / 100
-        table = torch.randn(n, device=DEV, generator=g)
-        for desc in (False, True):
-            idx = torch.argsort(f, descending=desc, stable=True)
-            ranks = torch.empty_like(idx)
-            ranks[idx] = torch.arange(n, device=DEV)
-            assert torch.equal(ops.rank_table(f, desc, table), table[ranks])
-    for n, d in ((12, 6), (4096, 1024), (300, 130), (5000, 256)):
+    for n in (12, 4096, 8192, 8193, 20000):
+        for special in (False, True):
+            f = torch.round(torch.randn(n, device=DEV, generator=g) * 100) / 100
+            if special:  # stable ties between +0 and -0, NaN ranked as the largest value, both infinities
+                vals = torch.tensor([0.0, -0.0, float("nan"), float("inf"), float("-inf")], device=DEV)
+                pick = torch.randint(0, 6, (n,), device=DEV, generator=g)
+                f = torch.where(pick < 5, vals[pick.clamp_max(4)], f)
+            table = torch.randn(n, device=DEV, generator=g)
+            for desc in (False, True):
+                idx = torch.argsort(f, descending=desc, stable=True)
+                ranks = torch.empty_like(idx)
+                ranks[idx] = torch.arange(n, device=DEV)
+                assert torch.equal(ops.rank_table(f, desc, table), table[ranks]), (n, special, desc)
+    for n, d in ((12, 6), (4096, 1024), (300, 130), (5000, 256), (4, 1), (7, 3), (14, 33), (19, 200), (24, 1025), (8193, 129), (1000, 200)):
         Y = torch.randn(n, d, device=DEV, generator=g)
         w = torch.randn(n, device=DEV, generator=g) / n
         Cm = torch.randn(d, d, device=DEV, generator=g)
         u = torch.randn(d, device=DEV, generator=g)
         k = torch.tensor([0.7, 0.9, 0.05], device=DEV)
-        ref = 0.7 * (Y.double().T * w.double()) @ Y.double() + 0.9 * Cm.double() + 0.05 * torch.outer(u.double(), u.double())
-        out = ops.weighted_syrk_update(Y, w, k, Cm, u=u)
-        scale = float(ref.abs().max())
-        assert float((out.double() - ref).abs().max()) / scale < 3e-6
-        C2 = Cm.clone()
-        ops.weighted_syrk_update(Y, w, k, C2, u=u, out=C2)  # in place
-        assert torch.equal(C2, out)
+        S = 0.7 * (Y.double().T * w.double()) @ Y.double() + 0.9 * Cm.double()
+        for uu in (u, None):
+            ref = S + 0.05 * torch.outer(u.double(), u.double()) if uu is not None else S
+            out = ops.weighted_syrk_update(Y, w, k, Cm, u=uu)
+            scale = float(ref.abs().max())
+            assert float((out.double() - ref).abs().max()) / scale < 3e-6, (n, d, uu is None)
+            sep = torch.full_like(Cm, float("nan"))
+            assert ops.weighted_syrk_update(Y, w, k, Cm, u=uu, out=sep) is sep and torch.equal(sep, out)
+            C2 = Cm.clone()
+            ops.weighted_syrk_update(Y, w, k, C2, u=uu, out=C2)  # in place
+            assert torch.equal(C2, out)
 
 
 # ------------------------------------------------------------------------------------------------ batched functional kernels
