@@ -1,8 +1,13 @@
 // K1 / K2: fused Philox sampling -> perturbation write -> objective row-reduction, and the stand-alone
-// evaluation kernel.  HBM-bound design: one warp owns one direction (a +/- row pair) or one row; every
-// lane produces 4 consecutive columns per step from ONE Philox4x32-10 call, writes them with 128-bit
-// streaming stores (512 contiguous bytes per warp-row) and folds them into the objective accumulators
-// while they are still in registers, so the population is written once and never re-read for evaluation.
+// evaluation kernel: the host side of the kernels in evok_sampler.cuh, for the built-in objectives and for the objectives
+// registered at run time (evok_objective_register: NVRTC-compiled instantiations of the same kernels).
+#include <cuda.h>
+
+#include <atomic>
+#include <mutex>
+#include <string>
+#include <vector>
+
 #include "evok_common.cuh"
 
 namespace evok {
@@ -18,138 +23,11 @@ static int sm_count() {
   return g_sm_count;
 }
 
-// tunables (build-time, for measurement builds: scripts/build_variants.py, scripts/kbench.py)
-#ifndef EVOK_SAMPLE_THREADS
-#define EVOK_SAMPLE_THREADS 256
-#endif
-#ifndef EVOK_SAMPLE_MINB
-#define EVOK_SAMPLE_MINB 3
-#endif
-#ifndef EVOK_SAMPLE_UNR
-#define EVOK_SAMPLE_UNR 2
-#endif
-#ifndef EVOK_SAMPLEONLY_MINB
-#define EVOK_SAMPLEONLY_MINB 5
-#endif
-#ifndef EVOK_SAMPLEONLY_UNR
-#define EVOK_SAMPLEONLY_UNR 1
-#endif
-constexpr int kSampleThreads = EVOK_SAMPLE_THREADS;
-// the fused kernels are issue/XU bound (two independent Philox chains per lane help); the sample-only kernel is store
-// bound and prefers occupancy
-template <int OBJ>
-struct SampleTune {
-  static constexpr int kUnroll = OBJ == EVOK_OBJ_NONE ? EVOK_SAMPLEONLY_UNR : EVOK_SAMPLE_UNR;
-  static constexpr int kMinBlocks = OBJ == EVOK_OBJ_NONE ? EVOK_SAMPLEONLY_MINB : EVOK_SAMPLE_MINB;
-};
-
-// one column group (4 columns) of one unit: sample, store, accumulate.  SQ: also *zsq += z^2 (the unscaled normals; the
-// squared norm that separable CMA-ES's active reweighting needs), in column order
-template <int OBJ, bool SYM, bool STORE, bool VEC, bool SQ = false>
-__device__ __forceinline__ void sample_group(const PhiloxKey& key, uint32_t sw, uint64_t unit, uint32_t q, int64_t D,
-                                             const float* __restrict__ mu, const float* __restrict__ sigma, float* xp, float* xm,
-                                             ObjAcc<OBJ>& accp, ObjAcc<OBJ>& accm, float* zsq = nullptr) {
-  float z[4];
-  normals4(key, sw, unit, q, z);
-  const int64_t j = (int64_t)q << 2;
-  if (VEC) {
-    if (SQ) {
-      *zsq = fmaf(z[0], z[0], *zsq); *zsq = fmaf(z[1], z[1], *zsq); *zsq = fmaf(z[2], z[2], *zsq); *zsq = fmaf(z[3], z[3], *zsq);
-    }
-    const float4 m = __ldg(reinterpret_cast<const float4*>(mu + j));
-    const float4 s = __ldg(reinterpret_cast<const float4*>(sigma + j));
-    const float p0 = fmaf(s.x, z[0], m.x), p1 = fmaf(s.y, z[1], m.y), p2 = fmaf(s.z, z[2], m.z), p3 = fmaf(s.w, z[3], m.w);
-    if (STORE) st_stream4(xp + j, p0, p1, p2, p3);
-    accp.add(p0); accp.add(p1); accp.add(p2); accp.add(p3);
-    if (SYM) {
-      const float n0 = fmaf(-s.x, z[0], m.x), n1 = fmaf(-s.y, z[1], m.y), n2 = fmaf(-s.z, z[2], m.z), n3 = fmaf(-s.w, z[3], m.w);
-      if (STORE) st_stream4(xm + j, n0, n1, n2, n3);
-      accm.add(n0); accm.add(n1); accm.add(n2); accm.add(n3);
-    }
-  } else {
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      if (j + c < D) {
-        if (SQ) *zsq = fmaf(z[c], z[c], *zsq);
-        const float m = __ldg(mu + j + c), s = __ldg(sigma + j + c);
-        const float p = fmaf(s, z[c], m);
-        if (STORE) st_stream1(xp + j + c, p);
-        accp.add(p);
-        if (SYM) {
-          const float n = fmaf(-s, z[c], m);
-          if (STORE) st_stream1(xm + j + c, n);
-          accm.add(n);
-        }
-      }
-    }
-  }
-}
-
-// PUSH: the fitness of row i goes to row (row0 + i) of EVERY peer's fitness vector (the all-gather of the sharded
-// generation, fused into the producer) and the last CTA raises this rank's flag on every peer.
-// SQ (non-symmetric only): q[r] = sum_j z_rj^2 of the unscaled normals, accumulated in registers next to the objective.
-template <int OBJ, bool SYM, bool STORE, bool VEC, bool PUSH, bool SQ = false>
-__global__ void __launch_bounds__(kSampleThreads, SampleTune<OBJ>::kMinBlocks)
-    sample_eval_kernel(float* __restrict__ X, int64_t ldx, const float* __restrict__ mu, const float* __restrict__ sigma,
-                       int64_t row0, int64_t n_units, int64_t D, const __grid_constant__ PhiloxKey key, const uint32_t* __restrict__ stream_off,
-                       float* __restrict__ f, const __grid_constant__ PeerSink sink, const unsigned long long* epoch, unsigned int* done,
-                       float* __restrict__ q_out) {
-  static_assert(!(SQ && (SYM || PUSH)), "the squared norms are produced by the plain non-symmetric sampler only");
-  const int lane = threadIdx.x & 31;
-  const uint32_t sw = key.stream_lo + (stream_off ? __ldg(stream_off) : 0u);
-  const int64_t warps_total = (int64_t)gridDim.x * (kSampleThreads / 32);
-  const int64_t gw = (int64_t)blockIdx.x * (kSampleThreads / 32) + (threadIdx.x >> 5);
-  const uint32_t nq = (uint32_t)((D + 3) >> 2);
-  const uint64_t unit0 = (uint64_t)(SYM ? (row0 >> 1) : row0);
-
-  for (int64_t u = gw; u < n_units; u += warps_total) {
-    ObjAcc<OBJ> accp, accm;
-    const int64_t r = SYM ? 2 * u : u;
-    float* xp = STORE ? X + r * ldx : nullptr;
-    float* xm = STORE ? xp + ldx : nullptr;
-    const uint64_t unit = unit0 + (uint64_t)u;
-    constexpr int kSampleUnroll = SampleTune<OBJ>::kUnroll;
-    float zsq = 0.f;
-    uint32_t q = lane;
-    if (kSampleUnroll > 1) {
-      // independent Philox chains in flight per lane
-      for (; q + 32u * (kSampleUnroll - 1) < nq; q += 32u * kSampleUnroll) {
-#pragma unroll
-        for (int uu = 0; uu < kSampleUnroll; ++uu)
-          sample_group<OBJ, SYM, STORE, VEC, SQ>(key, sw, unit, q + 32u * uu, D, mu, sigma, xp, xm, accp, accm, &zsq);
-      }
-    }
-    for (; q < nq; q += 32) sample_group<OBJ, SYM, STORE, VEC, SQ>(key, sw, unit, q, D, mu, sigma, xp, xm, accp, accm, &zsq);
-    if (SQ) {
-      zsq = warp_sum(zsq);
-      if (lane == 0) q_out[r] = zsq;
-    }
-    if (OBJ != EVOK_OBJ_NONE) {
-      const float fp = accp.finish(D);
-      float fm = 0.f;
-      if (SYM) fm = accm.finish(D);
-      if (lane == 0) {
-        if (PUSH) {
-          for (int p = 0; p < sink.world; ++p) {
-            float* fr = static_cast<float*>(sink.data[p]) + row0 + r;
-            fr[0] = fp;
-            if (SYM) fr[1] = fm;
-          }
-        } else {
-          f[r] = fp;
-          if (SYM) f[r + 1] = fm;
-        }
-      }
-    }
-  }
-  if (PUSH) peer_signal_tail(sink, epoch, done);
-}
-
 // Batched searches (functional ask/tell API with leading batch dimensions, funcpgpe.py:301-327): blockIdx.y = batch item, every
 // item has its own centre / stdev row (item stride 0 = shared) and its own Philox stream (stream word + item), so one launch
 // draws the populations of all items -- bit-identical to one evok_sample_eval call per item with stream_id = item.
 template <bool SYM, bool VEC>
-__global__ void __launch_bounds__(kSampleThreads, SampleTune<EVOK_OBJ_NONE>::kMinBlocks)
+__global__ void __launch_bounds__(kSampleThreads, SampleTune<ObjAcc<EVOK_OBJ_NONE>>::kMinBlocks)
     sample_batched_kernel(float* __restrict__ X, int64_t item_stride_x, int64_t ldx, const float* __restrict__ mu, int64_t item_stride_mu,
                           const float* __restrict__ sigma, int64_t item_stride_sigma, int64_t n_units, int64_t D, const __grid_constant__ PhiloxKey key) {
   const int lane = threadIdx.x & 31;
@@ -162,45 +40,10 @@ __global__ void __launch_bounds__(kSampleThreads, SampleTune<EVOK_OBJ_NONE>::kMi
   const int64_t gw = (int64_t)blockIdx.x * (kSampleThreads / 32) + (threadIdx.x >> 5);
   const uint32_t nq = (uint32_t)((D + 3) >> 2);
   for (int64_t u = gw; u < n_units; u += warps_total) {
-    ObjAcc<EVOK_OBJ_NONE> accp, accm;
+    ObjAcc<EVOK_OBJ_NONE> accp(D), accm(D);
     float* xp = X + (SYM ? 2 * u : u) * ldx;
     float* xm = xp + ldx;
-    for (uint32_t q = lane; q < nq; q += 32) sample_group<EVOK_OBJ_NONE, SYM, true, VEC>(key, sw, (uint64_t)u, q, D, mu, sigma, xp, xm, accp, accm);
-  }
-}
-
-constexpr int kEvalThreads = 256;
-
-template <int OBJ, bool VEC>
-__global__ void __launch_bounds__(kEvalThreads)
-    eval_kernel(const float* __restrict__ X, int64_t ldx, int64_t n_rows, int64_t D, float* __restrict__ f) {
-  const int lane = threadIdx.x & 31;
-  const int64_t warps_total = (int64_t)gridDim.x * (kEvalThreads / 32);
-  const int64_t gw = (int64_t)blockIdx.x * (kEvalThreads / 32) + (threadIdx.x >> 5);
-  for (int64_t r = gw; r < n_rows; r += warps_total) {
-    ObjAcc<OBJ> acc;
-    const float* x = X + r * ldx;
-    if (VEC) {
-      const int64_t nq = D >> 2;
-      int64_t q = lane;
-      // 4 independent 128-bit loads in flight per lane
-      for (; q + 96 < nq; q += 128) {
-        const float4 a = ld_stream4(x + 4 * q), b = ld_stream4(x + 4 * (q + 32)), c = ld_stream4(x + 4 * (q + 64)),
-                     d = ld_stream4(x + 4 * (q + 96));
-        acc.add(a.x); acc.add(a.y); acc.add(a.z); acc.add(a.w);
-        acc.add(b.x); acc.add(b.y); acc.add(b.z); acc.add(b.w);
-        acc.add(c.x); acc.add(c.y); acc.add(c.z); acc.add(c.w);
-        acc.add(d.x); acc.add(d.y); acc.add(d.z); acc.add(d.w);
-      }
-      for (; q < nq; q += 32) {
-        const float4 a = ld_stream4(x + 4 * q);
-        acc.add(a.x); acc.add(a.y); acc.add(a.z); acc.add(a.w);
-      }
-    } else {
-      for (int64_t j = lane; j < D; j += 32) acc.add(ld_stream1(x + j));
-    }
-    const float v = acc.finish(D);
-    if (lane == 0) f[r] = v;
+    for (uint32_t q = lane; q < nq; q += 32) sample_group<ObjAcc<EVOK_OBJ_NONE>, SYM, true, VEC>(key, sw, (uint64_t)u, q, D, mu, sigma, xp, xm, accp, accm);
   }
 }
 
@@ -231,11 +74,11 @@ static int launch_sample(float* X, int64_t ldx, const float* mu, const float* si
   PushArgs none{};
   const PushArgs& pa = PUSH ? *push : none;
   if (vec) {
-    auto k = sample_eval_kernel<OBJ, SYM, STORE, true, PUSH, SQ>;
+    auto k = sample_eval_kernel<ObjAcc<OBJ>, SYM, STORE, true, PUSH, SQ>;
     k<<<resident_grid(k, kSampleThreads, ctas_needed), kSampleThreads, 0, st>>>(X, ldx, mu, sigma, row0, n_units, D, key, stream_off, f, pa.sink,
                                                                                 pa.epoch, pa.done, q);
   } else {
-    auto k = sample_eval_kernel<OBJ, SYM, STORE, false, PUSH, SQ>;
+    auto k = sample_eval_kernel<ObjAcc<OBJ>, SYM, STORE, false, PUSH, SQ>;
     k<<<resident_grid(k, kSampleThreads, ctas_needed), kSampleThreads, 0, st>>>(X, ldx, mu, sigma, row0, n_units, D, key, stream_off, f, pa.sink,
                                                                                 pa.epoch, pa.done, q);
   }
@@ -278,32 +121,196 @@ static int launch_eval(const float* X, int64_t ldx, int64_t n_rows, int64_t D, f
   const bool vec = (D % 4 == 0) && aligned16(X) && (ldx % 4 == 0);
   const int64_t ctas_needed = (n_rows + (kEvalThreads / 32) - 1) / (kEvalThreads / 32);
   if (vec) {
-    auto k = eval_kernel<OBJ, true>;
+    auto k = eval_kernel<ObjAcc<OBJ>, true>;
     k<<<resident_grid(k, kEvalThreads, ctas_needed), kEvalThreads, 0, st>>>(X, ldx, n_rows, D, f);
   } else {
-    auto k = eval_kernel<OBJ, false>;
+    auto k = eval_kernel<ObjAcc<OBJ>, false>;
     k<<<resident_grid(k, kEvalThreads, ctas_needed), kEvalThreads, 0, st>>>(X, ldx, n_rows, D, f);
   }
   EVOK_CHECK_LAUNCH();
   return 0;
 }
 
+// ------------------------------------------------------------------------------------------------
+// Objectives registered at run time.  A registration keeps a copy of the cubin and the lowered names of its kernels (in the
+// EVOK_OBJ_KERNEL_* order); the module is loaded into the current device's primary context on the first use on that device
+// (each device has its own module, functions, occupancy and SM count).  Loaded modules stay until the process ends.
+// ------------------------------------------------------------------------------------------------
+constexpr int kMaxDevices = 64;
+
+struct UserDevice {
+  int state = 0;  // 0: not loaded; 1: loaded; EVOK_E_NOKERNEL: the cubin lacks a kernel (a permanent failure)
+  CUmodule module = nullptr;
+  CUfunction fn[EVOK_OBJ_KERNELS] = {};
+  int per_sm[EVOK_OBJ_KERNELS] = {};
+  int sms = 0;
+};
+
+struct UserObjective {
+  std::vector<char> image;
+  std::vector<std::string> names;
+  UserDevice dev[kMaxDevices];
+};
+
+// the driver API through the runtime's entry points (the library does not link libcuda)
+struct DriverApi {
+  decltype(&cuDeviceGet) device_get = nullptr;
+  decltype(&cuDeviceGetAttribute) device_attribute = nullptr;
+  decltype(&cuModuleLoadData) module_load = nullptr;
+  decltype(&cuModuleGetFunction) module_function = nullptr;
+  decltype(&cuModuleUnload) module_unload = nullptr;
+  decltype(&cuOccupancyMaxActiveBlocksPerMultiprocessor) occupancy = nullptr;
+  decltype(&cuLaunchKernel) launch = nullptr;
+};
+static DriverApi g_driver;
+
+template <typename F>
+static bool driver_symbol(const char* name, F& fn) {
+  void* p = nullptr;
+  cudaDriverEntryPointQueryResult q;
+  if (cudaGetDriverEntryPoint(name, &p, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess || !p) return false;
+  fn = reinterpret_cast<F>(p);
+  return true;
+}
+
+static bool driver_api() {
+  DriverApi& d = g_driver;
+  if (d.launch) return true;
+  return driver_symbol("cuDeviceGet", d.device_get) && driver_symbol("cuDeviceGetAttribute", d.device_attribute) &&
+         driver_symbol("cuModuleLoadData", d.module_load) && driver_symbol("cuModuleGetFunction", d.module_function) &&
+         driver_symbol("cuModuleUnload", d.module_unload) && driver_symbol("cuOccupancyMaxActiveBlocksPerMultiprocessor", d.occupancy) &&
+         driver_symbol("cuLaunchKernel", d.launch);
+}
+
+static std::mutex g_user_mutex;
+static UserObjective* g_user[EVOK_OBJ_USER_CAPACITY];
+static std::atomic<int> g_user_count{0};
+
+static bool is_user(int objective) {
+  return objective >= EVOK_OBJ_USER_BASE && objective - EVOK_OBJ_USER_BASE < g_user_count.load(std::memory_order_acquire);
+}
+
+static int kernel_threads(int k) { return k >= EVOK_OBJ_KERNEL_EVAL ? kEvalThreads : kSampleThreads; }
+
+// The loaded module of a registered objective on the current device (loaded here on the first call for that device).
+static int user_device(int objective, const UserDevice** out) {
+  int dev = 0;
+  cudaError_t ce = cudaGetDevice(&dev);
+  if (ce != cudaSuccess) return (int)ce;
+  if (dev < 0 || dev >= kMaxDevices) return EVOK_E_BADSIZE;
+  std::lock_guard<std::mutex> lock(g_user_mutex);
+  UserObjective& obj = *g_user[objective - EVOK_OBJ_USER_BASE];
+  UserDevice& d = obj.dev[dev];
+  if (d.state == 0) {
+    ce = cudaSetDevice(dev);  // makes the device's primary context (the runtime's) current, creating it if needed
+    if (ce != cudaSuccess) return (int)ce;
+    if (!driver_api()) return (int)cudaErrorNotSupported;
+    const DriverApi& api = g_driver;
+    CUdevice cu_dev;
+    CUresult r = api.device_get(&cu_dev, dev);
+    if (r == CUDA_SUCCESS) r = api.device_attribute(&d.sms, CU_DEVICE_ATTRIBUTE_MULTIPROCESSOR_COUNT, cu_dev);
+    if (r == CUDA_SUCCESS) r = api.module_load(&d.module, obj.image.data());
+    if (r != CUDA_SUCCESS) return (int)r;  // CUresult and cudaError_t share their codes
+    for (int k = 0; k < EVOK_OBJ_KERNELS; ++k) {
+      if (api.module_function(&d.fn[k], d.module, obj.names[k].c_str()) != CUDA_SUCCESS) {
+        api.module_unload(d.module);
+        d.module = nullptr;
+        d.state = EVOK_E_NOKERNEL;
+        return d.state;
+      }
+      if (api.occupancy(&d.per_sm[k], d.fn[k], kernel_threads(k), 0) != CUDA_SUCCESS || d.per_sm[k] <= 0) d.per_sm[k] = 4;
+    }
+    if (d.sms <= 0) d.sms = kNumSMs;
+    d.state = 1;
+  }
+  if (d.state != 1) return d.state;
+  *out = &d;
+  return 0;
+}
+
+// the launch of kernel k with the grid rule of resident_grid (the driver API is resolved: user_device succeeded)
+static int user_launch(const UserDevice& d, int k, int64_t ctas_needed, void** args, cudaStream_t st) {
+  int64_t g = (int64_t)d.per_sm[k] * d.sms;
+  if (g > ctas_needed) g = ctas_needed;
+  if (g < 1) g = 1;
+  const CUresult r = g_driver.launch(d.fn[k], (unsigned)g, 1, 1, kernel_threads(k), 1, 1, 0, (CUstream)st, args, nullptr);
+  if (r != CUDA_SUCCESS) return (int)r;
+  count_launches(1);
+  return 0;
+}
+
+// launch_sample for a registered objective: the same kernel choice (symmetric, store, VEC, PUSH, SQ) and grid
+static int user_sample(int objective, float* X, int64_t ldx, const float* mu, const float* sigma, int64_t row0, int64_t n_rows, int64_t D,
+                       bool sym, uint64_t seed, uint64_t stream_id, const uint32_t* stream_off, float* f, cudaStream_t st,
+                       const PushArgs* push = nullptr, float* q = nullptr) {
+  const UserDevice* d = nullptr;
+  const int rc = user_device(objective, &d);
+  if (rc != 0) return rc;
+  const bool store = X != nullptr;
+  int64_t n_units = sym ? n_rows / 2 : n_rows;
+  const bool vec = (D % 4 == 0) && aligned16(mu) && aligned16(sigma) && (!store || (aligned16(X) && ldx % 4 == 0));
+  const int64_t ctas_needed = (n_units + (kSampleThreads / 32) - 1) / (kSampleThreads / 32);
+  PhiloxKey key = make_philox_key(seed, stream_id);
+  PushArgs pa{};
+  if (push) pa = *push;
+  const int variant = (store ? 2 : 0) + (vec ? 1 : 0);
+  const int k = q ? EVOK_OBJ_KERNEL_SQ + variant : (push ? EVOK_OBJ_KERNEL_PUSH : EVOK_OBJ_KERNEL_SAMPLE) + (sym ? 4 : 0) + variant;
+  void* args[] = {&X, &ldx, &mu, &sigma, &row0, &n_units, &D, &key, &stream_off, &f, &pa.sink, &pa.epoch, &pa.done, &q};
+  return user_launch(*d, k, ctas_needed, args, st);
+}
+
+static int user_eval(int objective, const float* X, int64_t ldx, int64_t n_rows, int64_t D, float* f, cudaStream_t st) {
+  const UserDevice* d = nullptr;
+  const int rc = user_device(objective, &d);
+  if (rc != 0) return rc;
+  const bool vec = (D % 4 == 0) && aligned16(X) && (ldx % 4 == 0);
+  const int64_t ctas_needed = (n_rows + (kEvalThreads / 32) - 1) / (kEvalThreads / 32);
+  void* args[] = {&X, &ldx, &n_rows, &D, &f};
+  return user_launch(*d, EVOK_OBJ_KERNEL_EVAL + (vec ? 1 : 0), ctas_needed, args, st);
+}
+
 }  // namespace evok
 
 using namespace evok;
+
+extern "C" EVOK_API int evok_objective_register(const void* cubin, size_t bytes, const char* const* kernel_names_host, int n_kernels,
+                                                int* id_out_host) {
+  if (!cubin || !kernel_names_host || !id_out_host) return EVOK_E_NULLPTR;
+  if (bytes == 0 || n_kernels != EVOK_OBJ_KERNELS) return EVOK_E_BADSIZE;
+  for (int k = 0; k < n_kernels; ++k)
+    if (!kernel_names_host[k]) return EVOK_E_NULLPTR;
+  std::lock_guard<std::mutex> lock(g_user_mutex);
+  const int n = g_user_count.load(std::memory_order_relaxed);
+  if (n >= EVOK_OBJ_USER_CAPACITY) return EVOK_E_BADSIZE;
+  UserObjective* obj = new UserObjective;
+  obj->image.assign(static_cast<const char*>(cubin), static_cast<const char*>(cubin) + bytes);
+  for (int k = 0; k < n_kernels; ++k) obj->names.emplace_back(kernel_names_host[k]);
+  g_user[n] = obj;
+  g_user_count.store(n + 1, std::memory_order_release);
+  *id_out_host = EVOK_OBJ_USER_BASE + n;
+  return 0;
+}
+
+extern "C" EVOK_API int evok_objective_load(int objective) {
+  if (!is_user(objective)) return EVOK_E_BADENUM;
+  const UserDevice* d = nullptr;
+  return user_device(objective, &d);
+}
 
 extern "C" EVOK_API int evok_sample_eval(int objective, float* X, int64_t ldx, const float* mu, const float* sigma, int64_t row0,
                                 int64_t n_rows, int64_t D, int symmetric, uint64_t seed, uint64_t stream_id,
                                 const uint32_t* stream_offset_dev, float* f, void* stream) {
   const uint32_t* stream_off = stream_offset_dev;
   if (!mu || !sigma) return EVOK_E_NULLPTR;
-  if (objective < 0 || objective >= EVOK_OBJ_COUNT) return EVOK_E_BADENUM;
+  const bool user = is_user(objective);
+  if ((objective < 0 || objective >= EVOK_OBJ_COUNT) && !user) return EVOK_E_BADENUM;
   if (objective == EVOK_OBJ_NONE && !X) return EVOK_E_NULLPTR;
   if (objective != EVOK_OBJ_NONE && !f) return EVOK_E_NULLPTR;
   if (n_rows < 0 || D <= 0 || row0 < 0 || (X && ldx < D)) return EVOK_E_BADSIZE;
   if (symmetric && ((n_rows & 1) || (row0 & 1))) return EVOK_E_ODDROWS;
   if (n_rows == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
+  if (user) return user_sample(objective, X, ldx, mu, sigma, row0, n_rows, D, symmetric != 0, seed, stream_id, stream_off, f, st);
   switch (objective) {
     case EVOK_OBJ_NONE: return dispatch_sample<EVOK_OBJ_NONE>(X, ldx, mu, sigma, row0, n_rows, D, symmetric, seed, stream_id, stream_off, f, st);
     case EVOK_OBJ_SPHERE: return dispatch_sample<EVOK_OBJ_SPHERE>(X, ldx, mu, sigma, row0, n_rows, D, symmetric, seed, stream_id, stream_off, f, st);
@@ -317,12 +324,14 @@ extern "C" EVOK_API int evok_sample_eval_sq(int objective, float* X, int64_t ldx
                                             int64_t D, uint64_t seed, uint64_t stream_id, const uint32_t* stream_offset_dev, float* f, float* q,
                                             void* stream) {
   if (!mu || !sigma || !q) return EVOK_E_NULLPTR;
-  if (objective < 0 || objective >= EVOK_OBJ_COUNT) return EVOK_E_BADENUM;
+  const bool user = is_user(objective);
+  if ((objective < 0 || objective >= EVOK_OBJ_COUNT) && !user) return EVOK_E_BADENUM;
   if (objective == EVOK_OBJ_NONE && !X) return EVOK_E_NULLPTR;
   if (objective != EVOK_OBJ_NONE && !f) return EVOK_E_NULLPTR;
   if (n_rows < 0 || D <= 0 || row0 < 0 || (X && ldx < D)) return EVOK_E_BADSIZE;
   if (n_rows == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
+  if (user) return user_sample(objective, X, ldx, mu, sigma, row0, n_rows, D, false, seed, stream_id, stream_offset_dev, f, st, nullptr, q);
   switch (objective) {
     case EVOK_OBJ_NONE: return dispatch_sample_sq<EVOK_OBJ_NONE>(X, ldx, mu, sigma, row0, n_rows, D, seed, stream_id, stream_offset_dev, f, q, st);
     case EVOK_OBJ_SPHERE: return dispatch_sample_sq<EVOK_OBJ_SPHERE>(X, ldx, mu, sigma, row0, n_rows, D, seed, stream_id, stream_offset_dev, f, q, st);
@@ -337,7 +346,8 @@ extern "C" EVOK_API int evok_sample_eval_push(int objective, float* X, int64_t l
                                               int world, int rank, void* const* peer_f, void* const* peer_flags, const uint64_t* epoch_dev,
                                               uint32_t* done_dev, void* stream) {
   if (!mu || !sigma || !peer_f || !peer_flags || !epoch_dev || !done_dev) return EVOK_E_NULLPTR;
-  if (objective <= EVOK_OBJ_NONE || objective >= EVOK_OBJ_COUNT) return EVOK_E_BADENUM;
+  const bool user = is_user(objective);
+  if ((objective <= EVOK_OBJ_NONE || objective >= EVOK_OBJ_COUNT) && !user) return EVOK_E_BADENUM;
   if (world < 1 || world > EVOK_MAX_PEERS || rank < 0 || rank >= world) return EVOK_E_BADSIZE;
   if (n_rows < 0 || D <= 0 || row0 < 0 || (X && ldx < D)) return EVOK_E_BADSIZE;
   if (symmetric && ((n_rows & 1) || (row0 & 1))) return EVOK_E_ODDROWS;
@@ -353,6 +363,7 @@ extern "C" EVOK_API int evok_sample_eval_push(int objective, float* X, int64_t l
   push.done = done_dev;
   // n_rows == 0 still launches one CTA: the peers wait for this rank's flag
   cudaStream_t st = (cudaStream_t)stream;
+  if (user) return user_sample(objective, X, ldx, mu, sigma, row0, n_rows, D, symmetric != 0, seed, stream_id, stream_offset_dev, nullptr, st, &push);
   switch (objective) {
     case EVOK_OBJ_SPHERE: return dispatch_sample_push<EVOK_OBJ_SPHERE>(X, ldx, mu, sigma, row0, n_rows, D, symmetric, seed, stream_id, stream_offset_dev, push, st);
     case EVOK_OBJ_RASTRIGIN: return dispatch_sample_push<EVOK_OBJ_RASTRIGIN>(X, ldx, mu, sigma, row0, n_rows, D, symmetric, seed, stream_id, stream_offset_dev, push, st);
@@ -363,10 +374,12 @@ extern "C" EVOK_API int evok_sample_eval_push(int objective, float* X, int64_t l
 
 extern "C" EVOK_API int evok_eval(int objective, const float* X, int64_t ldx, int64_t n_rows, int64_t D, float* f, void* stream) {
   if (!X || !f) return EVOK_E_NULLPTR;
-  if (objective <= EVOK_OBJ_NONE || objective >= EVOK_OBJ_COUNT) return EVOK_E_BADENUM;
+  const bool user = is_user(objective);
+  if ((objective <= EVOK_OBJ_NONE || objective >= EVOK_OBJ_COUNT) && !user) return EVOK_E_BADENUM;
   if (n_rows < 0 || D <= 0 || ldx < D) return EVOK_E_BADSIZE;
   if (n_rows == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
+  if (user) return user_eval(objective, X, ldx, n_rows, D, f, st);
   switch (objective) {
     case EVOK_OBJ_SPHERE: return launch_eval<EVOK_OBJ_SPHERE>(X, ldx, n_rows, D, f, st);
     case EVOK_OBJ_RASTRIGIN: return launch_eval<EVOK_OBJ_RASTRIGIN>(X, ldx, n_rows, D, f, st);

@@ -1,0 +1,395 @@
+// The device-only half of K1 / K2: Philox normals, the streaming stores, the peer-exchange sink, the objective accumulators
+// and the sampling / evaluation kernels.  nvcc compiles it into libevok.so (evok_sample_eval.cu, with the built-in
+// objectives) and NVRTC compiles it at run time with a user-defined accumulator (evotorch_b200/jit.py), so it has no host
+// includes and no host code: under NVRTC the integer types come from the typedefs below.
+#pragma once
+
+#ifdef __CUDACC_RTC__
+typedef signed char int8_t;
+typedef unsigned char uint8_t;
+typedef int int32_t;
+typedef unsigned int uint32_t;
+typedef long long int64_t;
+typedef unsigned long long uint64_t;
+#endif
+
+#include "../../include/evok.h"
+
+namespace evok {
+
+// ------------------------------------------------------------------------------------------------
+// Peer exchange over NVLink (evok_peer.cu): where a producing kernel's result is needed by every GPU, the kernel itself
+// stores it into every peer's buffer and the LAST CTA to finish raises this rank's flag in every peer's flag array.
+// ------------------------------------------------------------------------------------------------
+struct PeerSink {
+  void* data[EVOK_MAX_PEERS];                 // peer p's destination buffer (this rank's own buffer at p == rank)
+  unsigned long long* flags[EVOK_MAX_PEERS];  // peer p's flag array (one 64-bit epoch per source rank)
+  int world, rank;
+};
+
+__device__ __forceinline__ void st_release_sys(unsigned long long* p, unsigned long long v) {
+  asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
+__device__ __forceinline__ unsigned long long ld_acquire_sys(const unsigned long long* p) {
+  unsigned long long v;
+  asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+  return v;
+}
+
+// Call from ALL threads of EVERY CTA of a 1-D grid after the CTA's last peer store.  `epoch` (local) holds the number of
+// completed exchanges; the flag value raised is epoch + 1 (the waiting kernel advances `epoch`).  `done` is a local counter
+// that returns to 0 for the next launch.
+static __device__ __noinline__ void peer_signal_tail(const PeerSink& s, const unsigned long long* epoch, unsigned int* done) {
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence_system();  // this CTA's peer stores are visible system-wide before the counter moves
+    const unsigned int prev = atomicAdd(done, 1u);
+    if (prev == gridDim.x - 1) {
+      *done = 0;
+      __threadfence_system();
+      const unsigned long long e = *epoch + 1ull;
+      for (int p = 0; p < s.world; ++p) st_release_sys(s.flags[p] + s.rank, e);
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Philox4x32-10 (Salmon et al., SC'11).  One call -> 4 x 32 random bits.
+// ------------------------------------------------------------------------------------------------
+struct U4 {
+  uint32_t x, y, z, w;
+};
+
+// The 10 round keys of one (seed, stream) pair, precomputed on the host and passed to the kernels BY VALUE: they live in
+// the constant bank, so each round's key XOR takes its operand straight from c[][] (no per-thread key-schedule adds).
+struct PhiloxKey {
+  uint32_t k0[10], k1[10];
+  uint32_t stream_lo;
+};
+
+// EVOK_PHILOX_ROUNDS exists for MEASUREMENT builds only (scripts/build_variants.py: what would fewer rounds buy?); the
+// product is Philox4x32-10, the variant cuRAND / torch use, and the oracle restates exactly that.
+#ifndef EVOK_PHILOX_ROUNDS
+#define EVOK_PHILOX_ROUNDS 10
+#endif
+__device__ __forceinline__ U4 philox4x32_10(U4 c, const PhiloxKey& key) {
+  constexpr uint32_t M0 = 0xD2511F53u, M1 = 0xCD9E8D57u;
+#pragma unroll
+  for (int r = 0; r < EVOK_PHILOX_ROUNDS; ++r) {
+    const uint32_t hi0 = __umulhi(M0, c.x), lo0 = M0 * c.x;
+    const uint32_t hi1 = __umulhi(M1, c.z), lo1 = M1 * c.z;
+    U4 n;
+    n.x = hi1 ^ c.y ^ key.k0[r];
+    n.y = lo1;
+    n.z = hi0 ^ c.w ^ key.k1[r];
+    n.w = lo0;
+    c = n;
+  }
+  return c;
+}
+
+__device__ __forceinline__ float sqrt_approx(float x) {
+  float r;
+  asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
+  return r;
+}
+
+__device__ __forceinline__ float lg2_approx(float x) {
+  float r;
+  asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
+  return r;
+}
+
+// Box-Muller on 32+32 random bits -> two standard normals.
+//   u1 = 2^-33 + a * 2^-32 in (0, 1]  (never 0, so the log is finite);  r = sqrt(-2 ln u1) = sqrt(lg2(u1) * (-2 ln 2))
+//   theta = 2 pi (2^-33 + b * 2^-32): the 2 pi is folded into the conversion constants.
+__device__ __forceinline__ void box_muller(uint32_t a, uint32_t b, float& z0, float& z1) {
+  const float u1 = fmaf((float)a, 2.3283064365386963e-10f, 1.1641532182693481e-10f);
+  const float th = fmaf((float)b, 1.4629180792671596e-09f, 7.314590396335798e-10f);
+  const float r = sqrt_approx(lg2_approx(u1) * -1.3862943611198906f);
+  float s, c;
+  __sincosf(th, &s, &c);
+  z0 = r * c;
+  z1 = r * s;
+}
+
+// The four standard normals of (unit, column group q): `unit` is the GLOBAL direction index (symmetric
+// sampling: rows 2*unit and 2*unit+1) or the global row index (non-symmetric); columns 4q .. 4q+3.
+// `stream_word` = low 32 bits of the stream id (key.stream_lo plus an optional device-side generation offset, which lets a
+// CUDA graph that was captured once draw a fresh population on every replay)
+__device__ __forceinline__ void normals4(const PhiloxKey& key, uint32_t stream_word, uint64_t unit, uint32_t q, float z[4]) {
+  U4 c;
+  c.x = q;
+  c.y = (uint32_t)unit;
+  c.z = (uint32_t)(unit >> 32);
+  c.w = stream_word;
+  const U4 r = philox4x32_10(c, key);
+  box_muller(r.x, r.y, z[0], z[1]);
+  box_muller(r.z, r.w, z[2], z[3]);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Warp reductions
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+__device__ __forceinline__ double warp_sum(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// streaming 128-bit accesses: the population is touched once per kernel, keep it out of L1
+__device__ __forceinline__ float4 ld_stream4(const float* p) {
+  float4 v;
+  asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
+  return v;
+}
+__device__ __forceinline__ float ld_stream1(const float* p) {
+  float v;
+  asm volatile("ld.global.nc.L1::no_allocate.f32 %0, [%1];" : "=f"(v) : "l"(p));
+  return v;
+}
+__device__ __forceinline__ void st_stream4(float* p, float a, float b, float c, float d) {
+  asm volatile("st.global.cs.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+}
+__device__ __forceinline__ void st_stream1(float* p, float a) {
+  asm volatile("st.global.cs.f32 [%0], %1;" ::"l"(p), "f"(a) : "memory");
+}
+
+// ------------------------------------------------------------------------------------------------
+// Objective accumulators.  An accumulator is a type with
+//   Acc(D)      : a fresh accumulator for one row of D columns (one per row and lane);
+//   add(x, j)   : fold element x of column j (0-based, global) into this lane's partial sums;
+//   finish(D)   : warp-reduce the partials and return the fitness of the row (every lane gets it; lane 0 stores it).
+// A row's elements reach add() in no fixed column order (strided over the lanes of a warp), so an accumulator holds sums.
+// The built-in ones are ObjAcc<EVOK_OBJ_*>; a user-defined one is generated by evotorch_b200/jit.py.
+// ------------------------------------------------------------------------------------------------
+template <int OBJ>
+struct ObjAcc;
+
+template <>
+struct ObjAcc<EVOK_OBJ_NONE> {
+  __device__ __forceinline__ explicit ObjAcc(int64_t) {}
+  __device__ __forceinline__ void add(float, int64_t) {}
+  __device__ __forceinline__ float finish(int64_t) { return 0.f; }
+};
+template <>
+struct ObjAcc<EVOK_OBJ_SPHERE> {
+  __device__ __forceinline__ explicit ObjAcc(int64_t) {}
+  float s2 = 0.f;
+  __device__ __forceinline__ void add(float x, int64_t) { s2 = fmaf(x, x, s2); }
+  __device__ __forceinline__ float finish(int64_t) { return warp_sum(s2); }
+};
+template <>
+struct ObjAcc<EVOK_OBJ_RASTRIGIN> {
+  __device__ __forceinline__ explicit ObjAcc(int64_t) {}
+  float s2 = 0.f, sc = 0.f;
+  __device__ __forceinline__ void add(float x, int64_t) {
+    s2 = fmaf(x, x, s2);
+    sc += __cosf(6.2831853071795865f * x);
+  }
+  __device__ __forceinline__ float finish(int64_t D) {
+    const float a = warp_sum(s2), c = warp_sum(sc);
+    return fmaf(-10.f, c, a) + 10.f * (float)D;
+  }
+};
+template <>
+struct ObjAcc<EVOK_OBJ_ACKLEY> {
+  __device__ __forceinline__ explicit ObjAcc(int64_t) {}
+  float s2 = 0.f, sc = 0.f;
+  __device__ __forceinline__ void add(float x, int64_t) {
+    s2 = fmaf(x, x, s2);
+    sc += __cosf(6.2831853071795865f * x);
+  }
+  __device__ __forceinline__ float finish(int64_t D) {
+    const float a = warp_sum(s2), c = warp_sum(sc);
+    const float invD = 1.0f / (float)D;
+    return -20.f * expf(-0.2f * sqrtf(a * invD)) - expf(c * invD) + 20.f + 2.718281828459045f;
+  }
+};
+
+// true only for ObjAcc<EVOK_OBJ_NONE> (sample without evaluating)
+template <typename Acc>
+struct SampleOnly {
+  static constexpr bool value = false;
+};
+template <>
+struct SampleOnly<ObjAcc<EVOK_OBJ_NONE>> {
+  static constexpr bool value = true;
+};
+
+// ------------------------------------------------------------------------------------------------
+// K1 / K2 kernels.  HBM-bound design: one warp owns one direction (a +/- row pair) or one row; every lane produces 4
+// consecutive columns per step from ONE Philox4x32-10 call, writes them with 128-bit streaming stores (512 contiguous bytes
+// per warp-row) and folds them into the objective accumulators while they are still in registers, so the population is
+// written once and never re-read for evaluation.
+// ------------------------------------------------------------------------------------------------
+// tunables (build-time, for measurement builds: scripts/build_variants.py, scripts/kbench.py)
+#ifndef EVOK_SAMPLE_THREADS
+#define EVOK_SAMPLE_THREADS 256
+#endif
+#ifndef EVOK_SAMPLE_MINB
+#define EVOK_SAMPLE_MINB 3
+#endif
+#ifndef EVOK_SAMPLE_UNR
+#define EVOK_SAMPLE_UNR 2
+#endif
+#ifndef EVOK_SAMPLEONLY_MINB
+#define EVOK_SAMPLEONLY_MINB 5
+#endif
+#ifndef EVOK_SAMPLEONLY_UNR
+#define EVOK_SAMPLEONLY_UNR 1
+#endif
+constexpr int kSampleThreads = EVOK_SAMPLE_THREADS;
+// the fused kernels are issue/XU bound (two independent Philox chains per lane help); the sample-only kernel is store
+// bound and prefers occupancy
+template <typename Acc>
+struct SampleTune {
+  static constexpr int kUnroll = SampleOnly<Acc>::value ? EVOK_SAMPLEONLY_UNR : EVOK_SAMPLE_UNR;
+  static constexpr int kMinBlocks = SampleOnly<Acc>::value ? EVOK_SAMPLEONLY_MINB : EVOK_SAMPLE_MINB;
+};
+
+// one column group (4 columns) of one unit: sample, store, accumulate.  SQ: also *zsq += z^2 (the unscaled normals; the
+// squared norm that separable CMA-ES's active reweighting needs), in column order
+template <typename Acc, bool SYM, bool STORE, bool VEC, bool SQ = false>
+__device__ __forceinline__ void sample_group(const PhiloxKey& key, uint32_t sw, uint64_t unit, uint32_t q, int64_t D,
+                                             const float* __restrict__ mu, const float* __restrict__ sigma, float* xp, float* xm,
+                                             Acc& accp, Acc& accm, float* zsq = nullptr) {
+  float z[4];
+  normals4(key, sw, unit, q, z);
+  const int64_t j = (int64_t)q << 2;
+  if (VEC) {
+    if (SQ) {
+      *zsq = fmaf(z[0], z[0], *zsq); *zsq = fmaf(z[1], z[1], *zsq); *zsq = fmaf(z[2], z[2], *zsq); *zsq = fmaf(z[3], z[3], *zsq);
+    }
+    const float4 m = __ldg(reinterpret_cast<const float4*>(mu + j));
+    const float4 s = __ldg(reinterpret_cast<const float4*>(sigma + j));
+    const float p0 = fmaf(s.x, z[0], m.x), p1 = fmaf(s.y, z[1], m.y), p2 = fmaf(s.z, z[2], m.z), p3 = fmaf(s.w, z[3], m.w);
+    if (STORE) st_stream4(xp + j, p0, p1, p2, p3);
+    accp.add(p0, j); accp.add(p1, j + 1); accp.add(p2, j + 2); accp.add(p3, j + 3);
+    if (SYM) {
+      const float n0 = fmaf(-s.x, z[0], m.x), n1 = fmaf(-s.y, z[1], m.y), n2 = fmaf(-s.z, z[2], m.z), n3 = fmaf(-s.w, z[3], m.w);
+      if (STORE) st_stream4(xm + j, n0, n1, n2, n3);
+      accm.add(n0, j); accm.add(n1, j + 1); accm.add(n2, j + 2); accm.add(n3, j + 3);
+    }
+  } else {
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      if (j + c < D) {
+        if (SQ) *zsq = fmaf(z[c], z[c], *zsq);
+        const float m = __ldg(mu + j + c), s = __ldg(sigma + j + c);
+        const float p = fmaf(s, z[c], m);
+        if (STORE) st_stream1(xp + j + c, p);
+        accp.add(p, j + c);
+        if (SYM) {
+          const float n = fmaf(-s, z[c], m);
+          if (STORE) st_stream1(xm + j + c, n);
+          accm.add(n, j + c);
+        }
+      }
+    }
+  }
+}
+
+// PUSH: the fitness of row i goes to row (row0 + i) of EVERY peer's fitness vector (the all-gather of the sharded
+// generation, fused into the producer) and the last CTA raises this rank's flag on every peer.
+// SQ (non-symmetric only): q[r] = sum_j z_rj^2 of the unscaled normals, accumulated in registers next to the objective.
+template <typename Acc, bool SYM, bool STORE, bool VEC, bool PUSH, bool SQ = false>
+__global__ void __launch_bounds__(kSampleThreads, SampleTune<Acc>::kMinBlocks)
+    sample_eval_kernel(float* __restrict__ X, int64_t ldx, const float* __restrict__ mu, const float* __restrict__ sigma,
+                       int64_t row0, int64_t n_units, int64_t D, const __grid_constant__ PhiloxKey key, const uint32_t* __restrict__ stream_off,
+                       float* __restrict__ f, const __grid_constant__ PeerSink sink, const unsigned long long* epoch, unsigned int* done,
+                       float* __restrict__ q_out) {
+  static_assert(!(SQ && (SYM || PUSH)), "the squared norms are produced by the plain non-symmetric sampler only");
+  const int lane = threadIdx.x & 31;
+  const uint32_t sw = key.stream_lo + (stream_off ? __ldg(stream_off) : 0u);
+  const int64_t warps_total = (int64_t)gridDim.x * (kSampleThreads / 32);
+  const int64_t gw = (int64_t)blockIdx.x * (kSampleThreads / 32) + (threadIdx.x >> 5);
+  const uint32_t nq = (uint32_t)((D + 3) >> 2);
+  const uint64_t unit0 = (uint64_t)(SYM ? (row0 >> 1) : row0);
+
+  for (int64_t u = gw; u < n_units; u += warps_total) {
+    Acc accp(D), accm(D);
+    const int64_t r = SYM ? 2 * u : u;
+    float* xp = STORE ? X + r * ldx : nullptr;
+    float* xm = STORE ? xp + ldx : nullptr;
+    const uint64_t unit = unit0 + (uint64_t)u;
+    constexpr int kSampleUnroll = SampleTune<Acc>::kUnroll;
+    float zsq = 0.f;
+    uint32_t q = lane;
+    if (kSampleUnroll > 1) {
+      // independent Philox chains in flight per lane
+      for (; q + 32u * (kSampleUnroll - 1) < nq; q += 32u * kSampleUnroll) {
+#pragma unroll
+        for (int uu = 0; uu < kSampleUnroll; ++uu)
+          sample_group<Acc, SYM, STORE, VEC, SQ>(key, sw, unit, q + 32u * uu, D, mu, sigma, xp, xm, accp, accm, &zsq);
+      }
+    }
+    for (; q < nq; q += 32) sample_group<Acc, SYM, STORE, VEC, SQ>(key, sw, unit, q, D, mu, sigma, xp, xm, accp, accm, &zsq);
+    if (SQ) {
+      zsq = warp_sum(zsq);
+      if (lane == 0) q_out[r] = zsq;
+    }
+    if (!SampleOnly<Acc>::value) {
+      const float fp = accp.finish(D);
+      float fm = 0.f;
+      if (SYM) fm = accm.finish(D);
+      if (lane == 0) {
+        if (PUSH) {
+          for (int p = 0; p < sink.world; ++p) {
+            float* fr = static_cast<float*>(sink.data[p]) + row0 + r;
+            fr[0] = fp;
+            if (SYM) fr[1] = fm;
+          }
+        } else {
+          f[r] = fp;
+          if (SYM) f[r + 1] = fm;
+        }
+      }
+    }
+  }
+  if (PUSH) peer_signal_tail(sink, epoch, done);
+}
+
+constexpr int kEvalThreads = 256;
+
+template <typename Acc, bool VEC>
+__global__ void __launch_bounds__(kEvalThreads)
+    eval_kernel(const float* __restrict__ X, int64_t ldx, int64_t n_rows, int64_t D, float* __restrict__ f) {
+  const int lane = threadIdx.x & 31;
+  const int64_t warps_total = (int64_t)gridDim.x * (kEvalThreads / 32);
+  const int64_t gw = (int64_t)blockIdx.x * (kEvalThreads / 32) + (threadIdx.x >> 5);
+  for (int64_t r = gw; r < n_rows; r += warps_total) {
+    Acc acc(D);
+    const float* x = X + r * ldx;
+    if (VEC) {
+      const int64_t nq = D >> 2;
+      int64_t q = lane;
+      // 4 independent 128-bit loads in flight per lane
+      for (; q + 96 < nq; q += 128) {
+        const float4 a = ld_stream4(x + 4 * q), b = ld_stream4(x + 4 * (q + 32)), c = ld_stream4(x + 4 * (q + 64)),
+                     d = ld_stream4(x + 4 * (q + 96));
+        const int64_t ja = 4 * q, jb = 4 * (q + 32), jc = 4 * (q + 64), jd = 4 * (q + 96);
+        acc.add(a.x, ja); acc.add(a.y, ja + 1); acc.add(a.z, ja + 2); acc.add(a.w, ja + 3);
+        acc.add(b.x, jb); acc.add(b.y, jb + 1); acc.add(b.z, jb + 2); acc.add(b.w, jb + 3);
+        acc.add(c.x, jc); acc.add(c.y, jc + 1); acc.add(c.z, jc + 2); acc.add(c.w, jc + 3);
+        acc.add(d.x, jd); acc.add(d.y, jd + 1); acc.add(d.z, jd + 2); acc.add(d.w, jd + 3);
+      }
+      for (; q < nq; q += 32) {
+        const float4 a = ld_stream4(x + 4 * q);
+        const int64_t ja = 4 * q;
+        acc.add(a.x, ja); acc.add(a.y, ja + 1); acc.add(a.z, ja + 2); acc.add(a.w, ja + 3);
+      }
+    } else {
+      for (int64_t j = lane; j < D; j += 32) acc.add(ld_stream1(x + j), j);
+    }
+    const float v = acc.finish(D);
+    if (lane == 0) f[r] = v;
+  }
+}
+
+}  // namespace evok

@@ -285,6 +285,7 @@ extern "C" EVOK_API const char* evok_error_string(int code) {
     case EVOK_E_WORKSPACE: return "workspace too small";
     case EVOK_E_ODDROWS: return "symmetric sampling needs an even number of rows";
     case EVOK_E_ALIGN: return "misaligned pointer";
+    case EVOK_E_NOKERNEL: return "the cubin of the registered objective lacks one of its kernels";
     default: return code > 0 ? cudaGetErrorString((cudaError_t)code) : "unknown error";
   }
 }

@@ -1,0 +1,361 @@
+"""Run-time compiled objectives: a sum-separable function given as Python expressions becomes an accumulator of the fused
+sampler (csrc/evok_sampler.cuh), compiled with NVRTC for sm_90a and registered with libevok.so.
+
+    f(x) = value(S_1, ..., S_k, D),    S_i = sum_j term_i(x_j, j, D),    k <= 4
+
+One parse of the expressions gives both the CUDA accumulator and a torch function of the same formula (the evaluation of
+CPU problems, other dtypes, rng="torch" and before-eval hooks; the float64 reference of the tests).
+
+The expression language (anything else raises ValueError):
+  - operators  + - * /, unary -, ** (an integer literal exponent expands to products, any other exponent is powf / torch.pow);
+  - functions  abs sqrt exp log sin cos tan tanh floor minimum maximum  (minimum / maximum return the other operand when
+    one is NaN, like fminf / fmaxf and torch.fmin / torch.fmax);
+  - constants  pi, e, numeric literals;
+  - names      x (the element), j (its 0-based column) and D (the row length) in a term; the sum names and D in `value`.
+The CUDA side evaluates in float32 with the precise libdevice functions (no fast math) and contracts a * b + c into fma.
+"""
+
+from __future__ import annotations
+
+import ast
+import ctypes
+import math
+import os
+import re
+import threading
+from ctypes import c_char_p, c_int, c_size_t, c_void_p
+from typing import Callable, Dict, Optional
+
+import numpy as np
+import torch
+
+from . import _native as nat
+
+_PKG = os.path.dirname(os.path.abspath(__file__))
+CSRC = os.path.join(_PKG, "csrc")
+INCLUDE = os.path.join(os.path.dirname(_PKG), "include")
+
+MAX_SUMS = 4
+MAX_INT_POWER = 16
+
+FUNCTIONS = {
+    "abs": ("fabsf", torch.abs), "sqrt": ("sqrtf", torch.sqrt), "exp": ("expf", torch.exp), "log": ("logf", torch.log),
+    "sin": ("sinf", torch.sin), "cos": ("cosf", torch.cos), "tan": ("tanf", torch.tan), "tanh": ("tanhf", torch.tanh),
+    "floor": ("floorf", torch.floor), "minimum": ("fminf", torch.fmin), "maximum": ("fmaxf", torch.fmax),
+}
+CONSTANTS = {"pi": math.pi, "e": math.e}
+_ARITY = {"minimum": 2, "maximum": 2}
+_BINOPS = {ast.Add: "+", ast.Sub: "-", ast.Mult: "*", ast.Div: "/"}
+_ALLOWED_TEXT = ("allowed: + - * / ** and unary -, the functions " + " ".join(FUNCTIONS) + ", the constants pi and e, numeric "
+                 "literals and the names {names}")
+
+
+def _float_literal(v: float) -> str:
+    with np.errstate(over="ignore"):
+        f = float(np.float32(v))
+    if not math.isfinite(f):
+        raise ValueError(f"the literal {v!r} is not a finite float32")
+    return repr(f) + "f"
+
+
+class _Expr:
+    """One parsed expression: `cuda` is its CUDA text over the given identifiers, `torch(env)` evaluates it on tensors."""
+
+    def __init__(self, cuda: str, fn: Callable):
+        self.cuda, self.torch = cuda, fn
+
+
+def _as_tensor(v, env):
+    return v if isinstance(v, torch.Tensor) else torch.as_tensor(v, dtype=env["_dtype"], device=env["_device"])
+
+
+def _int_exponent(node) -> Optional[int]:
+    """The integer value of a literal exponent (2, -3, 2.0), else None."""
+    sign = 1
+    if isinstance(node, ast.UnaryOp) and isinstance(node.op, (ast.USub, ast.UAdd)):
+        sign = -1 if isinstance(node.op, ast.USub) else 1
+        node = node.operand
+    if isinstance(node, ast.Constant) and type(node.value) in (int, float) and float(node.value).is_integer():
+        n = sign * int(node.value)
+        return n if abs(n) <= MAX_INT_POWER else None
+    return None
+
+
+def _translate(node, names: Dict[str, str], where: str) -> _Expr:
+    """names: the Python names allowed here -> their CUDA identifiers."""
+    allowed = _ALLOWED_TEXT.format(names=", ".join(names))
+    if isinstance(node, ast.Expression):
+        return _translate(node.body, names, where)
+    if isinstance(node, ast.Constant):
+        if type(node.value) not in (int, float):
+            raise ValueError(f"{where}: the literal {node.value!r} is not a number; {allowed}")
+        v = float(node.value)
+        return _Expr(_float_literal(v), lambda env, v=v: v)
+    if isinstance(node, ast.Name):
+        if node.id in names:
+            return _Expr(names[node.id], lambda env, n=node.id: env[n])
+        if node.id in CONSTANTS:
+            v = CONSTANTS[node.id]
+            return _Expr(_float_literal(v), lambda env, v=v: v)
+        raise ValueError(f"{where}: unknown name {node.id!r}; {allowed}")
+    if isinstance(node, ast.UnaryOp):
+        a = _translate(node.operand, names, where)
+        if isinstance(node.op, ast.USub):
+            return _Expr(f"(-{a.cuda})", lambda env: -a.torch(env))
+        if isinstance(node.op, ast.UAdd):
+            return a
+        raise ValueError(f"{where}: the operator {type(node.op).__name__} is not supported; {allowed}")
+    if isinstance(node, ast.BinOp):
+        a = _translate(node.left, names, where)
+        if isinstance(node.op, ast.Pow):
+            n = _int_exponent(node.right)
+            if n is not None:
+                if n == 0:
+                    return _Expr("1.0f", lambda env: 1.0)
+                prod = "(" + " * ".join([a.cuda] * abs(n)) + ")"
+                return _Expr(prod if n > 0 else f"(1.0f / {prod})", lambda env: a.torch(env) ** n)
+            b = _translate(node.right, names, where)
+            return _Expr(f"powf({a.cuda}, {b.cuda})", lambda env: torch.pow(_as_tensor(a.torch(env), env), b.torch(env)))
+        if type(node.op) not in _BINOPS:
+            raise ValueError(f"{where}: the operator {type(node.op).__name__} is not supported; {allowed}")
+        b = _translate(node.right, names, where)
+        op = _BINOPS[type(node.op)]
+        fn = {"+": lambda env: a.torch(env) + b.torch(env), "-": lambda env: a.torch(env) - b.torch(env),
+              "*": lambda env: a.torch(env) * b.torch(env), "/": lambda env: a.torch(env) / b.torch(env)}[op]
+        return _Expr(f"({a.cuda} {op} {b.cuda})", fn)
+    if isinstance(node, ast.Call):
+        if not isinstance(node.func, ast.Name) or node.func.id not in FUNCTIONS:
+            what = node.func.id if isinstance(node.func, ast.Name) else ast.unparse(node.func)
+            raise ValueError(f"{where}: the function {what!r} is not supported; {allowed}")
+        if node.keywords:
+            raise ValueError(f"{where}: keyword arguments are not supported; {allowed}")
+        name = node.func.id
+        arity = _ARITY.get(name, 1)
+        if len(node.args) != arity:
+            raise ValueError(f"{where}: {name} takes {arity} argument(s), got {len(node.args)}")
+        args = [_translate(a, names, where) for a in node.args]
+        cname, tfn = FUNCTIONS[name]
+        return _Expr(f"{cname}(" + ", ".join(a.cuda for a in args) + ")",
+                     lambda env: tfn(*[_as_tensor(a.torch(env), env) for a in args]))
+    raise ValueError(f"{where}: {type(node).__name__} ({ast.unparse(node)!r}) is not supported; {allowed}")
+
+
+def _parse(text: str, names: Dict[str, str], where: str) -> _Expr:
+    if not isinstance(text, str):
+        raise ValueError(f"{where}: expected an expression string, got {type(text).__name__}")
+    try:
+        tree = ast.parse(text, mode="eval")
+    except SyntaxError as e:
+        raise ValueError(f"{where}: not a Python expression: {text!r} ({e.msg})") from None
+    return _translate(tree, names, where)
+
+
+_RESERVED = {"x", "j", "D"} | set(CONSTANTS) | set(FUNCTIONS)
+
+
+class ObjectiveSpec:
+    """The parsed form of a sum-separable objective: `source` is the CUDA translation unit, `torch_fn(X)` the torch function."""
+
+    def __init__(self, sums: Dict[str, str], value: str):
+        if not isinstance(sums, dict) or not 1 <= len(sums) <= MAX_SUMS:
+            raise ValueError(f"sums: expected a dict of 1 to {MAX_SUMS} named term expressions")
+        for s in sums:
+            if not (isinstance(s, str) and s.isidentifier()) or s in _RESERVED:
+                raise ValueError(f"sums: {s!r} cannot name a sum (a sum name is an identifier other than {sorted(_RESERVED)})")
+        self.sums, self.value = dict(sums), value
+        term_names = {"x": "x", "j": "jf", "D": "Df"}
+        self.terms = {s: _parse(t, term_names, f"sums[{s!r}]") for s, t in sums.items()}
+        value_names = {s: f"S_{s}" for s in sums}
+        value_names["D"] = "Df"
+        self.value_expr = _parse(value, value_names, "value")
+        self.source = self._cuda_source()
+
+    def _cuda_source(self) -> str:
+        k = range(len(self.terms))
+        exprs = list(self.terms.values())
+        lines = ['#include "evok_sampler.cuh"', "", "namespace evok_user {", "struct Acc {"]
+        lines.append("  float Df;")
+        lines.append("  float " + ", ".join(f"s{i} = 0.f" for i in k) + ";")
+        lines.append("  __device__ __forceinline__ explicit Acc(int64_t D) : Df((float)D) {}")
+        lines.append("  __device__ __forceinline__ void add(float x, int64_t j) {")
+        if any(re.search(r"\bjf\b", e.cuda) for e in exprs):
+            lines.append("    const float jf = (float)j;")
+        lines += [f"    s{i} += {e.cuda};" for i, e in zip(k, exprs)]
+        lines.append("  }")
+        lines.append("  __device__ __forceinline__ float finish(int64_t) {")
+        lines += [f"    const float S_{s} = evok::warp_sum(s{i});" for i, s in zip(k, self.terms)]
+        lines.append(f"    return {self.value_expr.cuda};")
+        lines += ["  }", "};", "}  // namespace evok_user", ""]
+        return "\n".join(lines)
+
+    def torch_fn(self, X: torch.Tensor) -> torch.Tensor:
+        D = X.shape[-1]
+        env = {"x": X, "j": torch.arange(D, dtype=X.dtype, device=X.device), "D": torch.tensor(float(D), dtype=X.dtype, device=X.device),
+               "_dtype": X.dtype, "_device": X.device}
+        venv = {s: torch.broadcast_to(_as_tensor(e.torch(env), env), X.shape).sum(dim=-1) for s, e in self.terms.items()}
+        venv.update(D=env["D"], _dtype=X.dtype, _device=X.device)
+        return torch.broadcast_to(_as_tensor(self.value_expr.torch(venv), venv), X.shape[:-1])
+
+
+# ------------------------------------------------------------------------------------------------ NVRTC
+def kernel_expressions() -> list:
+    """The 22 kernels of a registered objective, in the EVOK_OBJ_KERNEL_* order of include/evok.h."""
+    b = lambda v: "true" if v else "false"  # noqa: E731
+    out = []
+    for push in (False, True):  # EVOK_OBJ_KERNEL_SAMPLE, EVOK_OBJ_KERNEL_PUSH: + 4 sym + 2 store + vec
+        for sym in (False, True):
+            for store in (False, True):
+                for vec in (False, True):
+                    out.append(f"evok::sample_eval_kernel<evok_user::Acc, {b(sym)}, {b(store)}, {b(vec)}, {b(push)}, false>")
+    for store in (False, True):  # EVOK_OBJ_KERNEL_SQ: + 2 store + vec
+        for vec in (False, True):
+            out.append(f"evok::sample_eval_kernel<evok_user::Acc, false, {b(store)}, {b(vec)}, false, true>")
+    for vec in (False, True):  # EVOK_OBJ_KERNEL_EVAL: + vec
+        out.append(f"evok::eval_kernel<evok_user::Acc, {b(vec)}>")
+    return out
+
+
+N_KERNELS = 22
+# -default-device: the declarations of the C ABI in include/evok.h (reached through evok_sampler.cuh) are unannotated
+NVRTC_OPTIONS = ("--gpu-architecture=sm_90a", "-std=c++17", "--fmad=true", "--ptxas-options=-v", "-default-device", f"-I{CSRC}",
+                 f"-I{INCLUDE}")
+
+_nvrtc: Optional[ctypes.CDLL] = None
+
+
+def _nvrtc_candidates() -> list:
+    cands = []
+    try:
+        import nvidia.cuda_nvrtc as m  # the NVRTC wheel torch depends on
+
+        for d in m.__path__:
+            cands += sorted((os.path.join(d, "lib", f) for f in os.listdir(os.path.join(d, "lib")) if re.fullmatch(r"libnvrtc\.so\.\d+", f)),
+                            reverse=True)
+    except (ImportError, OSError):
+        pass
+    from torch.utils.cpp_extension import CUDA_HOME
+
+    for home in (CUDA_HOME, "/usr/local/cuda"):
+        if home:
+            cands.append(os.path.join(home, "lib64", "libnvrtc.so"))
+    return cands
+
+
+def nvrtc() -> ctypes.CDLL:
+    global _nvrtc
+    if _nvrtc is None:
+        for path in _nvrtc_candidates():
+            if os.path.exists(path):
+                _nvrtc = ctypes.CDLL(path)
+                break
+        else:
+            raise RuntimeError("NVRTC not found: a fused objective is compiled with the libnvrtc of torch's nvidia-cuda-nvrtc wheel or "
+                               "of the CUDA toolkit")
+        P = ctypes.POINTER
+        for name, res, args in (
+            ("nvrtcCreateProgram", c_int, [P(c_void_p), c_char_p, c_char_p, c_int, c_void_p, c_void_p]),
+            ("nvrtcAddNameExpression", c_int, [c_void_p, c_char_p]),
+            ("nvrtcCompileProgram", c_int, [c_void_p, c_int, P(c_char_p)]),
+            ("nvrtcGetLoweredName", c_int, [c_void_p, c_char_p, P(c_char_p)]),
+            ("nvrtcGetProgramLogSize", c_int, [c_void_p, P(c_size_t)]),
+            ("nvrtcGetProgramLog", c_int, [c_void_p, c_char_p]),
+            ("nvrtcGetCUBINSize", c_int, [c_void_p, P(c_size_t)]),
+            ("nvrtcGetCUBIN", c_int, [c_void_p, c_char_p]),
+            ("nvrtcDestroyProgram", c_int, [P(c_void_p)]),
+            ("nvrtcGetErrorString", c_char_p, [c_int]),
+        ):
+            fn = getattr(_nvrtc, name)
+            fn.restype, fn.argtypes = res, args
+    return _nvrtc
+
+
+class CompiledObjective:
+    """An NVRTC compilation of one generated source: the cubin, the lowered kernel names, the ptxas info per kernel
+    ({expression: {"registers", "spill_stores", "spill_loads", "stack"}}), the compile wall time and, once registered, the id."""
+
+    def __init__(self, cubin: bytes, names: list, kernel_info: dict, seconds: float):
+        self.cubin, self.names, self.kernel_info, self.seconds = cubin, names, kernel_info, seconds
+        self.objective_id: Optional[int] = None
+
+
+def _ptxas_info(log: str, lowered: Dict[str, str]) -> dict:
+    by_lowered = {v: k for k, v in lowered.items()}
+    info, cur = {}, None
+    for line in log.splitlines():
+        m = re.search(r"Compiling entry function '([^']+)'", line)
+        if m:
+            cur = by_lowered.get(m.group(1))
+            if cur is not None:
+                info[cur] = {}
+            continue
+        if cur is None:
+            continue
+        m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", line)
+        if m:
+            info[cur].update(stack=int(m.group(1)), spill_stores=int(m.group(2)), spill_loads=int(m.group(3)))
+        m = re.search(r"Used (\d+) registers", line)
+        if m:
+            info[cur]["registers"] = int(m.group(1))
+    return info
+
+
+def compile_source(source: str, expressions: Optional[list] = None) -> CompiledObjective:
+    """Compile `source` with NVRTC for sm_90a and lower the names of `expressions` (default: the 22 objective kernels)."""
+    import time
+
+    lib = nvrtc()
+    expressions = kernel_expressions() if expressions is None else expressions
+    t0 = time.perf_counter()
+    prog = c_void_p()
+
+    def ok(rc, what):
+        if rc != 0:
+            raise RuntimeError(f"{what}: {lib.nvrtcGetErrorString(rc).decode()}")
+
+    ok(lib.nvrtcCreateProgram(ctypes.byref(prog), source.encode(), b"evok_objective.cu", 0, None, None), "nvrtcCreateProgram")
+    try:
+        for e in expressions:
+            ok(lib.nvrtcAddNameExpression(prog, f"&{e}".encode()), "nvrtcAddNameExpression")
+        opts = (c_char_p * len(NVRTC_OPTIONS))(*[o.encode() for o in NVRTC_OPTIONS])
+        rc = lib.nvrtcCompileProgram(prog, len(NVRTC_OPTIONS), opts)
+        size = c_size_t()
+        lib.nvrtcGetProgramLogSize(prog, ctypes.byref(size))
+        buf = ctypes.create_string_buffer(size.value)
+        lib.nvrtcGetProgramLog(prog, buf)
+        log = buf.value.decode(errors="replace")
+        if rc != 0:
+            raise RuntimeError(f"NVRTC could not compile the objective:\n{log}\n--- source ---\n{source}")
+        lowered = {}
+        for e in expressions:
+            name = c_char_p()
+            ok(lib.nvrtcGetLoweredName(prog, f"&{e}".encode(), ctypes.byref(name)), "nvrtcGetLoweredName")
+            lowered[e] = name.value.decode()
+        ok(lib.nvrtcGetCUBINSize(prog, ctypes.byref(size)), "nvrtcGetCUBINSize")
+        cubin = ctypes.create_string_buffer(size.value)
+        ok(lib.nvrtcGetCUBIN(prog, cubin), "nvrtcGetCUBIN")
+    finally:
+        lib.nvrtcDestroyProgram(ctypes.byref(prog))
+    return CompiledObjective(cubin.raw, [lowered[e] for e in expressions], _ptxas_info(log, lowered), time.perf_counter() - t0)
+
+
+def register(cubin: bytes, names: list) -> int:
+    """evok_objective_register: the id of the objective whose kernels (in EVOK_OBJ_KERNEL_* order) are in `cubin`."""
+    arr = (c_char_p * len(names))(*[n.encode() for n in names])
+    out = c_int()
+    nat.check(nat.lib().evok_objective_register(cubin, len(cubin), arr, len(names), ctypes.byref(out)), "evok_objective_register")
+    return out.value
+
+
+_cache: Dict[str, CompiledObjective] = {}
+_cache_lock = threading.Lock()
+
+
+def compile_objective(spec: ObjectiveSpec) -> CompiledObjective:
+    """Compile and register the objective of `spec`, once per process for one generated source."""
+    with _cache_lock:
+        c = _cache.get(spec.source)
+        if c is None:
+            c = compile_source(spec.source)
+            c.objective_id = register(c.cubin, c.names)
+            _cache[spec.source] = c
+        return c

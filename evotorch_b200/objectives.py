@@ -7,6 +7,9 @@ evaluate the population *inside* the sampling kernel (K1+K2 fused, csrc/evok_sam
 written once and never re-read for evaluation.  Called directly on a CUDA fp32 population they run the stand-alone
 row-reduction kernel (K2); on any other tensor the plain torch expression (same formula as the reference's README
 example, README.md:86-89).
+
+`FusedObjective` is the same for a user-defined sum-separable function: its expressions are compiled at run time into the
+same kernels (evotorch_b200/jit.py), so every fused path of the package takes it.
 """
 
 from __future__ import annotations
@@ -54,8 +57,37 @@ def _ackley(x: torch.Tensor) -> torch.Tensor:
             + 20.0 + math.e)
 
 
+class FusedObjective(BuiltinObjective):
+    """A user-defined objective f(x) = value(S_1, ..., S_k, D) with S_i = sum_j term_i(x_j, j, D), k <= 4, fused into the sampler.
+
+        styblinski_tang = FusedObjective("styblinski_tang", sums={"s": "x**4 - 16*x**2 + 5*x"}, value="0.5 * s")
+
+    `sums` maps each sum's name to its term (an expression of x, j and D), `value` is an expression of the sums and D; the
+    language is described in evotorch_b200.jit.  Construction parses both (ValueError for anything outside the language),
+    compiles the kernels with NVRTC for sm_90a and registers them with libevok.so; `kernel_info` holds the registers and
+    spills of every kernel.  The same source compiles once per process.  A FusedObjective pickles as its expressions."""
+
+    def __init__(self, name: str, sums: dict, value: str):
+        from . import jit
+
+        spec = jit.ObjectiveSpec(sums, value)
+        if name in ops.OBJECTIVE_IDS and ops.OBJECTIVE_IDS[name] < ops.OBJ_USER_BASE:
+            raise ValueError(f"{name!r} is the name of a built-in objective")
+        compiled = jit.compile_objective(spec)
+        super().__init__(name, compiled.objective_id, spec.torch_fn)
+        self.sums, self.value, self.source = dict(spec.sums), spec.value, spec.source
+        self.kernel_info = compiled.kernel_info
+        ops.OBJECTIVE_IDS[name] = compiled.objective_id
+
+    def __reduce__(self):
+        return (FusedObjective, (self.name, self.sums, self.value))
+
+    def __repr__(self) -> str:
+        return f"FusedObjective({self.name!r}, sums={self.sums!r}, value={self.value!r})"
+
+
 sphere = BuiltinObjective("sphere", ops.OBJ_SPHERE, _sphere)
 rastrigin = BuiltinObjective("rastrigin", ops.OBJ_RASTRIGIN, _rastrigin)
 ackley = BuiltinObjective("ackley", ops.OBJ_ACKLEY, _ackley)
 
-__all__ = ["sphere", "rastrigin", "ackley", "BuiltinObjective"]
+__all__ = ["sphere", "rastrigin", "ackley", "BuiltinObjective", "FusedObjective"]

@@ -17,6 +17,8 @@ from . import _native as nat
 from .tools.readonlytensor import as_plain_tensor
 
 OBJ_NONE, OBJ_SPHERE, OBJ_RASTRIGIN, OBJ_ACKLEY = 0, 1, 2, 3
+OBJ_USER_BASE = 64  # EVOK_OBJ_USER_BASE: the first id of an objective registered at run time (objectives.FusedObjective)
+# name -> id; a FusedObjective adds its own name here
 OBJECTIVE_IDS = {"sphere": OBJ_SPHERE, "rastrigin": OBJ_RASTRIGIN, "ackley": OBJ_ACKLEY}
 RANK_IDS = {"centered": 0, "linear": 1, "nes": 2, "normalized": 3, "raw": 4}
 GRAD_SEPARABLE, GRAD_SYMMETRIC, GRAD_EXP, GRAD_MOMENTS = 0, 1, 2, 3
@@ -137,6 +139,20 @@ def _host_floats(values, n: int):
 
 
 # ------------------------------------------------------------------------------------------------ K1 / K2
+_loaded_objectives: set = set()
+
+
+def _load_objective(objective: int, t: torch.Tensor) -> None:
+    """Load a registered objective's module on the device of `t` before its first launch there (evok_objective_load)."""
+    if objective < OBJ_USER_BASE:
+        return
+    key = (objective, t.device.index)
+    if key not in _loaded_objectives:
+        with torch.cuda.device(t.device):
+            nat.check(nat.lib().evok_objective_load(objective), "evok_objective_load")
+        _loaded_objectives.add(key)
+
+
 def _offset_ptr(stream_offset: Optional[torch.Tensor]) -> Optional[int]:
     if stream_offset is None:
         return None
@@ -159,6 +175,7 @@ def sample_eval(objective: int, X: Optional[torch.Tensor], mu: torch.Tensor, sig
         raise ValueError("symmetric sampling needs an even number of rows and an even first row")
     if n_rows == 0:
         return
+    _load_objective(objective, mu)
     with _timed("sample_eval" if objective != OBJ_NONE else "sample"):
         rc = nat.lib().evok_sample_eval(objective, nat.ptr(X), ldx, mu.data_ptr(), sigma.data_ptr(), row0, n_rows, D, int(symmetric),
                                         seed, stream_id, _offset_ptr(stream_offset), nat.ptr(f), nat.stream_of(mu))
@@ -174,6 +191,7 @@ def sample_eval_push(objective: int, X: Optional[torch.Tensor], mu: torch.Tensor
     ldx = _ldx(X, n_rows, D)
     if row0 + n_rows > peer.popsize:
         raise ValueError("rows beyond the population the peer exchange was sized for")
+    _load_objective(objective, mu)
     with _timed("sample_eval"):
         rc = nat.lib().evok_sample_eval_push(objective, nat.ptr(X), ldx, mu.data_ptr(), sigma.data_ptr(), row0, n_rows, D, int(symmetric),
                                              seed, stream_id, _offset_ptr(stream_offset), peer.world, peer.rank, peer.peer_f,
@@ -202,6 +220,7 @@ def evaluate(objective: int, X: torch.Tensor, f: Optional[torch.Tensor] = None) 
     if f is None:
         f = torch.empty(n, dtype=torch.float32, device=X.device)
     _vec(f, "f", n)
+    _load_objective(objective, X)
     with _timed("eval"):
         rc = nat.lib().evok_eval(objective, X.data_ptr(), X.stride(0), n, D, f.data_ptr(), nat.stream_of(X))
     nat.check(rc, "evok_eval")
@@ -280,7 +299,7 @@ def sample_eval_sq(objective: int, X: Optional[torch.Tensor], mu: torch.Tensor, 
                    seed: int, stream_id: int, row0: int = 0, f: Optional[torch.Tensor] = None,
                    stream_offset: Optional[torch.Tensor] = None) -> None:
     """`sample_eval` (non-symmetric) that also writes q[i] = ||z_i||^2 of the unscaled normals; X / f are the same bits as
-    `sample_eval` with the same arguments.  X = None: lazy population (needs a built-in objective)."""
+    `sample_eval` with the same arguments.  X = None: lazy population (needs an objective with a fused kernel)."""
     D = mu.numel()
     _vec(mu, "mu"); _vec(sigma, "sigma", D); _vec(q, "q", n_rows)
     ldx = _ldx(X, n_rows, D)
@@ -292,6 +311,7 @@ def sample_eval_sq(objective: int, X: Optional[torch.Tensor], mu: torch.Tensor, 
         raise ValueError("f: a fitness buffer is required when an objective is fused into the sampler")
     if n_rows == 0:
         return
+    _load_objective(objective, mu)
     with _timed("sepcma_sample"):
         rc = nat.lib().evok_sample_eval_sq(objective, nat.ptr(X), ldx, mu.data_ptr(), sigma.data_ptr(), row0, n_rows, D, seed, stream_id,
                                            _offset_ptr(stream_offset), nat.ptr(f), q.data_ptr(), nat.stream_of(mu))

@@ -19,8 +19,10 @@
 #ifndef EVOK_H_
 #define EVOK_H_
 
+#ifndef __CUDACC_RTC__ /* NVRTC compiles this header as part of evotorch_b200/csrc/evok_sampler.cuh, which defines the integer types */
 #include <stddef.h>
 #include <stdint.h>
+#endif
 
 #ifdef __cplusplus
 extern "C" {
@@ -41,6 +43,7 @@ extern "C" {
 #define EVOK_E_WORKSPACE (-4)
 #define EVOK_E_ODDROWS (-5) /* symmetric sampling / gradients need an even number of rows */
 #define EVOK_E_ALIGN (-6)
+#define EVOK_E_NOKERNEL (-7) /* the cubin of a registered objective lacks one of its EVOK_OBJ_KERNELS kernels */
 
 #define EVOK_MAX_PEERS 16 /* GPUs of one NVLink domain that can take part in a peer exchange */
 
@@ -50,6 +53,10 @@ extern "C" {
 #define EVOK_OBJ_RASTRIGIN 2 /* 10 D + sum(x^2 - 10 cos(2 pi x))  (reference README.md:86-89) */
 #define EVOK_OBJ_ACKLEY 3    /* -20 exp(-0.2 sqrt(mean x^2)) - exp(mean cos(2 pi x)) + 20 + e */
 #define EVOK_OBJ_COUNT 4
+/* objectives registered at run time (evok_objective_register) take the ids EVOK_OBJ_USER_BASE, EVOK_OBJ_USER_BASE + 1, ...
+ * in registration order, at most EVOK_OBJ_USER_CAPACITY of them per process; every id in between is EVOK_E_BADENUM */
+#define EVOK_OBJ_USER_BASE 64
+#define EVOK_OBJ_USER_CAPACITY 256
 
 /* ranking methods (tools/ranking.py:186) */
 #define EVOK_RANK_CENTERED 0
@@ -91,6 +98,30 @@ int evok_sample_eval(int objective, float* X, int64_t ldx, const float* mu, cons
 /* K2 alone: f[i] = objective(X[i, :]) for an already materialised population (torch-RNG parity mode,
  * CMA-ES / XNES populations).  Replaces the user's vectorised torch objective at core.py:2604. */
 int evok_eval(int objective, const float* X, int64_t ldx, int64_t n_rows, int64_t D, float* f, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Objectives defined at run time (evotorch_b200/jit.py compiles them with NVRTC from csrc/evok_sampler.cuh).
+ * evok_objective_register takes an sm_90a cubin and the lowered names of its EVOK_OBJ_KERNELS kernels, in this order:
+ *   EVOK_OBJ_KERNEL_SAMPLE + 4 sym + 2 store + vec : sample_eval_kernel<Acc, sym, store, vec, PUSH = false, SQ = false>
+ *   EVOK_OBJ_KERNEL_PUSH   + 4 sym + 2 store + vec : sample_eval_kernel<Acc, sym, store, vec, PUSH = true,  SQ = false>
+ *   EVOK_OBJ_KERNEL_SQ     + 2 store + vec         : sample_eval_kernel<Acc, false, store, vec, PUSH = false, SQ = true>
+ *   EVOK_OBJ_KERNEL_EVAL   + vec                   : eval_kernel<Acc, vec>
+ * It copies the image and the names, writes the new id to *id_out_host and needs no device.  The id is then accepted by
+ * evok_sample_eval, evok_sample_eval_sq, evok_sample_eval_push and evok_eval, which launch the registered kernels exactly
+ * as they launch a built-in objective's (same argument checks, kernel choice and grid).
+ * The module is loaded on a device by the first call that uses the id there, or by evok_objective_load (on the current
+ * device), which a caller about to capture a CUDA graph uses to keep the loading out of the capture.  A cubin without one
+ * of the kernels yields EVOK_E_NOKERNEL from every call on that device, and nothing is launched.
+ * Errors: EVOK_E_NULLPTR, EVOK_E_BADSIZE (bytes == 0, n_kernels != EVOK_OBJ_KERNELS, registry full), EVOK_E_BADENUM
+ * (evok_objective_load of an id that is not registered).
+ * --------------------------------------------------------------------------------------------- */
+#define EVOK_OBJ_KERNEL_SAMPLE 0
+#define EVOK_OBJ_KERNEL_PUSH 8
+#define EVOK_OBJ_KERNEL_SQ 16
+#define EVOK_OBJ_KERNEL_EVAL 20
+#define EVOK_OBJ_KERNELS 22
+int evok_objective_register(const void* cubin, size_t bytes, const char* const* kernel_names_host, int n_kernels, int* id_out_host);
+int evok_objective_load(int objective);
 
 /* ---------------------------------------------------------------------------------------------
  * K3: fitness -> utilities.  Replaces tools/ranking.py:24-183 (`rank` :189).
