@@ -24,6 +24,8 @@ inline void count_launches(int n) { __atomic_fetch_add(&g_launch_count, (unsigne
 
 constexpr int kWarp = 32;
 constexpr int kNumSMs = 132;  // H100 SXM
+// largest grid y / z: the batched entry points launch item chunks of at most this many items, one after another on the stream
+constexpr int64_t kMaxGridY = 65535;
 
 inline PhiloxKey make_philox_key(uint64_t seed, uint64_t stream_id) {
   PhiloxKey k;

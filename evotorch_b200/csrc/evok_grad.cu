@@ -761,7 +761,7 @@ extern "C" EVOK_API int evok_grad_batched(int form, const float* X, int64_t item
                                           void* stream) {
   if (!X || !w || !mu || !sigma || !out_mu || !out_sigma || !ws) return EVOK_E_NULLPTR;
   if (form < EVOK_GRAD_SEPARABLE || form > EVOK_GRAD_MOMENTS) return EVOK_E_BADENUM;
-  if (n_items < 0 || n_items > 65535 || n_rows < 0 || D <= 0 || ldx < D) return EVOK_E_BADSIZE;
+  if (n_items < 0 || n_rows < 0 || D <= 0 || ldx < D) return EVOK_E_BADSIZE;
   const bool sym = form == EVOK_GRAD_SYMMETRIC;
   if (sym && (n_rows & 1)) return EVOK_E_ODDROWS;
   if (n_items == 0) return 0;
@@ -787,18 +787,28 @@ extern "C" EVOK_API int evok_grad_batched(int form, const float* X, int64_t item
   items.mu = item_stride_mu;
   items.sigma = item_stride_sigma;
   items.partial = (int64_t)p.n_chunks * 2 * D;
-  if (ws_bytes < (size_t)n_items * items.partial * sizeof(float)) return EVOK_E_WORKSPACE;
+  // grid z / y hold at most kMaxGridY items: larger batches run as item chunks with the plan above, in order on the stream, each
+  // reusing the partial sums of the previous one
+  const int64_t chunk = n_items < kMaxGridY ? n_items : kMaxGridY;
+  if (ws_bytes < (size_t)chunk * items.partial * sizeof(float)) return EVOK_E_WORKSPACE;
   float* partial = (float*)ws;
-  if (vec_ok) {
-    if (sym) launch_partial<4, true, false>(p, form, X, ldx, w, mu, sigma, n_units, D, 0, 0, 0, nullptr, partial, st, n_items, &items);
-    else launch_partial<4, false, false>(p, form, X, ldx, w, mu, sigma, n_units, D, 0, 0, 0, nullptr, partial, st, n_items, &items);
-  } else {
-    if (sym) launch_partial<1, true, false>(p, form, X, ldx, w, mu, sigma, n_units, D, 0, 0, 0, nullptr, partial, st, n_items, &items);
-    else launch_partial<1, false, false>(p, form, X, ldx, w, mu, sigma, n_units, D, 0, 0, 0, nullptr, partial, st, n_items, &items);
+  for (int64_t b0 = 0; b0 < n_items; b0 += kMaxGridY) {
+    const int64_t nb = n_items - b0 < kMaxGridY ? n_items - b0 : kMaxGridY;
+    const float* Xc = X + b0 * item_stride_x;
+    const float* wc = w + b0 * n_rows;
+    const float* muc = mu + b0 * item_stride_mu;
+    const float* sgc = sigma + b0 * item_stride_sigma;
+    if (vec_ok) {
+      if (sym) launch_partial<4, true, false>(p, form, Xc, ldx, wc, muc, sgc, n_units, D, 0, 0, 0, nullptr, partial, st, nb, &items);
+      else launch_partial<4, false, false>(p, form, Xc, ldx, wc, muc, sgc, n_units, D, 0, 0, 0, nullptr, partial, st, nb, &items);
+    } else {
+      if (sym) launch_partial<1, true, false>(p, form, Xc, ldx, wc, muc, sgc, n_units, D, 0, 0, 0, nullptr, partial, st, nb, &items);
+      else launch_partial<1, false, false>(p, form, Xc, ldx, wc, muc, sgc, n_units, D, 0, 0, 0, nullptr, partial, st, nb, &items);
+    }
+    EVOK_CHECK_LAUNCH();
+    grad_finalize_kernel<<<dim3((unsigned)((D + 255) / 256), (unsigned)nb), 256, 0, st>>>(partial, p.n_chunks, D, scale_mu, scale_sigma,
+                                                                                          out_mu + b0 * D, out_sigma + b0 * D, items.partial);
+    EVOK_CHECK_LAUNCH();
   }
-  EVOK_CHECK_LAUNCH();
-  grad_finalize_kernel<<<dim3((unsigned)((D + 255) / 256), (unsigned)n_items), 256, 0, st>>>(partial, p.n_chunks, D, scale_mu, scale_sigma, out_mu,
-                                                                                             out_sigma, items.partial);
-  EVOK_CHECK_LAUNCH();
   return 0;
 }

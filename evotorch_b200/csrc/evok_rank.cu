@@ -762,24 +762,37 @@ extern "C" EVOK_API int evok_rank_table(const float* keys, int64_t N, int descen
 
 // ---- batched searches (functional API with leading batch dimensions): n_items independent rankings of N fitnesses each, f and w
 // contiguous [n_items][N].  N <= 8192: ONE launch for all items (the counting rank with blockIdx.y = item); larger N: the radix
-// pipeline item by item on the same workspace.
+// pipeline item by item on the same workspace.  Batches above kMaxGridY items run as item chunks of at most kMaxGridY, in order on
+// the stream, so the chunks reuse the workspace.
 extern "C" EVOK_API int evok_rank_batched(int method, const float* f, int64_t N, int64_t n_items, int higher_is_better, float* w, void* ws,
                                           size_t ws_bytes, void* stream) {
   if (!f || !w || !ws) return EVOK_E_NULLPTR;
   if (method < EVOK_RANK_CENTERED || method > EVOK_RANK_RAW) return EVOK_E_BADENUM;
-  if (N < 0 || N >= (int64_t)1 << 32 || n_items < 0 || n_items > 65535) return EVOK_E_BADSIZE;
+  if (N < 0 || N >= (int64_t)1 << 32 || n_items < 0) return EVOK_E_BADSIZE;
   if (N == 0 || n_items == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   if (method == EVOK_RANK_NORMALIZED || method == EVOK_RANK_RAW) {
-    if (ws_bytes < (size_t)n_items * 8 + 256) return EVOK_E_WORKSPACE;
+    const int64_t chunk = n_items < kMaxGridY ? n_items : kMaxGridY;
+    if (ws_bytes < (size_t)chunk * 8 + 256) return EVOK_E_WORKSPACE;
     float* stats = (float*)ws;
     const float sign = higher_is_better ? 1.0f : -1.0f;
-    if (method == EVOK_RANK_NORMALIZED) mean_std_kernel<<<(unsigned)n_items, 1024, 0, st>>>(f, N, sign, stats);
-    affine_kernel<<<dim3((unsigned)((N + 255) / 256), (unsigned)n_items), 256, 0, st>>>(f, N, sign, stats, method == EVOK_RANK_NORMALIZED, w);
-    EVOK_CHECK_LAUNCH_N(method == EVOK_RANK_NORMALIZED ? 2 : 1);
+    for (int64_t b0 = 0; b0 < n_items; b0 += kMaxGridY) {
+      const int64_t nb = n_items - b0 < kMaxGridY ? n_items - b0 : kMaxGridY;
+      const float* fc = f + b0 * N;
+      if (method == EVOK_RANK_NORMALIZED) mean_std_kernel<<<(unsigned)nb, 1024, 0, st>>>(fc, N, sign, stats);
+      affine_kernel<<<dim3((unsigned)((N + 255) / 256), (unsigned)nb), 256, 0, st>>>(fc, N, sign, stats, method == EVOK_RANK_NORMALIZED, w + b0 * N);
+      EVOK_CHECK_LAUNCH_N(method == EVOK_RANK_NORMALIZED ? 2 : 1);
+    }
     return 0;
   }
-  if (use_small_rank(N)) return rank_small(f, N, !higher_is_better, kSmallUtilities, method, 0, w, nullptr, st, nullptr, n_items);
+  if (use_small_rank(N)) {
+    for (int64_t b0 = 0; b0 < n_items; b0 += kMaxGridY) {
+      const int64_t nb = n_items - b0 < kMaxGridY ? n_items - b0 : kMaxGridY;
+      const int rc = rank_small(f + b0 * N, N, !higher_is_better, kSmallUtilities, method, 0, w + b0 * N, nullptr, st, nullptr, nb);
+      if (rc) return rc;
+    }
+    return 0;
+  }
   for (int64_t b = 0; b < n_items; ++b) {
     const int rc = evok_rank(method, f + b * N, N, higher_is_better, w + b * N, nullptr, ws, ws_bytes, stream);
     if (rc) return rc;
@@ -790,9 +803,17 @@ extern "C" EVOK_API int evok_rank_batched(int method, const float* f, int64_t N,
 extern "C" EVOK_API int evok_elite_mask_batched(const float* w, int64_t N, int64_t n_items, int64_t num_elites, float* mask, void* ws,
                                                 size_t ws_bytes, void* stream) {
   if (!w || !mask || !ws) return EVOK_E_NULLPTR;
-  if (N < 0 || N >= (int64_t)1 << 32 || n_items < 0 || n_items > 65535 || num_elites < 0 || num_elites > N) return EVOK_E_BADSIZE;
+  if (N < 0 || N >= (int64_t)1 << 32 || n_items < 0 || num_elites < 0 || num_elites > N) return EVOK_E_BADSIZE;
   if (N == 0 || n_items == 0) return 0;
-  if (use_small_rank(N)) return rank_small(w, N, /*descending=*/1, kSmallEliteMask, 0, num_elites, mask, nullptr, (cudaStream_t)stream, nullptr, n_items);
+  if (use_small_rank(N)) {
+    for (int64_t b0 = 0; b0 < n_items; b0 += kMaxGridY) {
+      const int64_t nb = n_items - b0 < kMaxGridY ? n_items - b0 : kMaxGridY;
+      const int rc = rank_small(w + b0 * N, N, /*descending=*/1, kSmallEliteMask, 0, num_elites, mask + b0 * N, nullptr, (cudaStream_t)stream,
+                                nullptr, nb);
+      if (rc) return rc;
+    }
+    return 0;
+  }
   for (int64_t b = 0; b < n_items; ++b) {
     const int rc = evok_elite_mask(w + b * N, N, num_elites, mask + b * N, ws, ws_bytes, stream);
     if (rc) return rc;
@@ -803,9 +824,12 @@ extern "C" EVOK_API int evok_elite_mask_batched(const float* w, int64_t N, int64
 extern "C" EVOK_API int evok_weights_adjust_batched(float* w, int64_t N, int64_t n_items, int mode, void* stream) {
   if (!w) return EVOK_E_NULLPTR;
   if (mode != 1 && mode != 2) return EVOK_E_BADENUM;
-  if (N < 0 || n_items < 0 || n_items > 65535) return EVOK_E_BADSIZE;
+  if (N < 0 || n_items < 0) return EVOK_E_BADSIZE;
   if (N == 0 || n_items == 0) return 0;
-  weights_adjust_kernel<<<(unsigned)n_items, 1024, 0, (cudaStream_t)stream>>>(w, N, mode);
-  EVOK_CHECK_LAUNCH();
+  for (int64_t b0 = 0; b0 < n_items; b0 += kMaxGridY) {
+    const int64_t nb = n_items - b0 < kMaxGridY ? n_items - b0 : kMaxGridY;
+    weights_adjust_kernel<<<(unsigned)nb, 1024, 0, (cudaStream_t)stream>>>(w + b0 * N, N, mode);
+    EVOK_CHECK_LAUNCH();
+  }
   return 0;
 }

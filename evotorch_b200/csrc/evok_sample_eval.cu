@@ -392,7 +392,7 @@ extern "C" EVOK_API int evok_sample_batched(float* X, int64_t item_stride_x, int
                                             int64_t item_stride_sigma, int64_t n_items, int64_t n_rows, int64_t D, int symmetric, uint64_t seed,
                                             uint64_t stream_id0, void* stream) {
   if (!X || !mu || !sigma) return EVOK_E_NULLPTR;
-  if (n_items < 0 || n_items > 65535 || n_rows < 0 || D <= 0 || ldx < D || item_stride_x < 0 || item_stride_mu < 0 || item_stride_sigma < 0)
+  if (n_items < 0 || n_rows < 0 || D <= 0 || ldx < D || item_stride_x < 0 || item_stride_mu < 0 || item_stride_sigma < 0)
     return EVOK_E_BADSIZE;
   if (symmetric && (n_rows & 1)) return EVOK_E_ODDROWS;
   if (n_items == 0 || n_rows == 0) return 0;
@@ -403,19 +403,28 @@ extern "C" EVOK_API int evok_sample_batched(float* X, int64_t item_stride_x, int
   const int64_t cap = ((int64_t)sm_count() * 8 + n_items - 1) / n_items;  // about 8 CTAs per SM over all items
   if (ctas > cap) ctas = cap < 1 ? 1 : cap;
   const PhiloxKey key = make_philox_key(seed, stream_id0);
-  dim3 grid((unsigned)ctas, (unsigned)n_items);
   cudaStream_t st = (cudaStream_t)stream;
-#define EVOK_LAUNCH_SB(SYMV, VECV)                                                                                                    \
-  sample_batched_kernel<SYMV, VECV><<<grid, kSampleThreads, 0, st>>>(X, item_stride_x, ldx, mu, item_stride_mu, sigma, item_stride_sigma, \
-                                                                     n_units, D, key)
-  if (symmetric) {
-    if (vec) EVOK_LAUNCH_SB(true, true);
-    else EVOK_LAUNCH_SB(true, false);
-  } else {
-    if (vec) EVOK_LAUNCH_SB(false, true);
-    else EVOK_LAUNCH_SB(false, false);
-  }
+  // grid y is at most kMaxGridY items: larger batches go in item chunks, chunk b0 starting at stream word stream_lo + b0, so item b
+  // keeps its Philox stream stream_id0 + b
+  for (int64_t b0 = 0; b0 < n_items; b0 += kMaxGridY) {
+    const int64_t nb = n_items - b0 < kMaxGridY ? n_items - b0 : kMaxGridY;
+    PhiloxKey kc = key;
+    kc.stream_lo += (uint32_t)b0;
+    const dim3 grid((unsigned)ctas, (unsigned)nb);
+    float* Xc = X + b0 * item_stride_x;
+    const float* muc = mu + b0 * item_stride_mu;
+    const float* sgc = sigma + b0 * item_stride_sigma;
+#define EVOK_LAUNCH_SB(SYMV, VECV) \
+  sample_batched_kernel<SYMV, VECV><<<grid, kSampleThreads, 0, st>>>(Xc, item_stride_x, ldx, muc, item_stride_mu, sgc, item_stride_sigma, n_units, D, kc)
+    if (symmetric) {
+      if (vec) EVOK_LAUNCH_SB(true, true);
+      else EVOK_LAUNCH_SB(true, false);
+    } else {
+      if (vec) EVOK_LAUNCH_SB(false, true);
+      else EVOK_LAUNCH_SB(false, false);
+    }
 #undef EVOK_LAUNCH_SB
-  EVOK_CHECK_LAUNCH();
+    EVOK_CHECK_LAUNCH();
+  }
   return 0;
 }

@@ -75,6 +75,21 @@ __global__ void __launch_bounds__(256) axpy_kernel(const float* __restrict__ g, 
   if (i < D) mu[i] += lr * g[i];
 }
 
+// torch.max / torch.min: NaN if either operand is NaN (fmaxf / fminf would return the other one)
+__device__ __forceinline__ float torch_max(float a, float b) { return (a != a || b != b) ? NAN : fmaxf(a, b); }
+__device__ __forceinline__ float torch_min(float a, float b) { return (a != a || b != b) ? NAN : fminf(a, b); }
+
+// modify_tensor (tools/misc.py) on one element: every operand the caller supplied takes part in torch.max / torch.min, so a NaN
+// target, a NaN bound or a NaN allowed change (|0| * inf) gives NaN; an absent bound is -inf / +inf, an absent max_change no limit
+__device__ __forceinline__ float clamp_sigma(float s, float target, float lo, float hi, bool has_mc, float c) {
+  if (has_mc) {
+    const float allowed = fabsf(s) * c;
+    lo = torch_max(lo, s - allowed);
+    hi = torch_min(hi, s + allowed);
+  }
+  return torch_min(torch_max(target, lo), hi);
+}
+
 __global__ void __launch_bounds__(256) sigma_update_kernel(float* __restrict__ sigma, const float* __restrict__ g, int64_t D, float lr,
                                                            int exp_form, const float* __restrict__ lb_vec, float lb,
                                                            const float* __restrict__ ub_vec, float ub, const float* __restrict__ mc_vec,
@@ -83,21 +98,12 @@ __global__ void __launch_bounds__(256) sigma_update_kernel(float* __restrict__ s
   if (i >= D) return;
   const float s = sigma[i];
   const float step = lr * g[i];
-  float target = exp_form ? s * expf(0.5f * step) : s + step;
-  float lo = lb_vec ? lb_vec[i] : lb;
-  float hi = ub_vec ? ub_vec[i] : ub;
-  if (lo != lo) lo = -INFINITY;  // NaN == "not set"
-  if (hi != hi) hi = INFINITY;
-  const float c = mc_vec ? mc_vec[i] : mc;
-  if (c == c) {
-    const float allowed = fabsf(s) * c;
-    lo = fmaxf(lo, s - allowed);
-    hi = fminf(hi, s + allowed);
-  }
-  // torch.max / torch.min propagate NaN from `target`; fmaxf would drop it
-  float r = (target != target) ? target : fmaxf(target, lo);
-  r = (r != r) ? r : fminf(r, hi);
-  sigma[i] = r;
+  const float target = exp_form ? s * expf(0.5f * step) : s + step;
+  // a NaN scalar means "not set"; vector entries are user data and keep their NaNs
+  const float lo = lb_vec ? lb_vec[i] : (lb != lb ? -INFINITY : lb);
+  const float hi = ub_vec ? ub_vec[i] : (ub != ub ? INFINITY : ub);
+  const bool has_mc = mc_vec != nullptr || mc == mc;
+  sigma[i] = clamp_sigma(s, target, lo, hi, has_mc, mc_vec ? mc_vec[i] : mc);
 }
 
 // Batched searches: per-item scalar hyper-parameters travel BY VALUE in the launch parameters (no device copy, no sync)
@@ -149,31 +155,21 @@ __global__ void __launch_bounds__(256) sigma_update_batched_kernel(float* __rest
   const int64_t i = (int64_t)blockIdx.y * D + j;
   const float s = sigma[i];
   const float step = sc.a[blockIdx.y] * g[i];
-  float target = exp_form ? s * expf(0.5f * step) : s + step;
-  float lo = lb_vec ? lb_vec[i] : -INFINITY;
-  float hi = ub_vec ? ub_vec[i] : INFINITY;
-  if (lo != lo) lo = -INFINITY;
-  if (hi != hi) hi = INFINITY;
-  const float c = mc_vec ? mc_vec[i] : NAN;
-  if (c == c) {
-    const float allowed = fabsf(s) * c;
-    lo = fmaxf(lo, s - allowed);
-    hi = fminf(hi, s + allowed);
-  }
-  float r = (target != target) ? target : fmaxf(target, lo);
-  r = (r != r) ? r : fminf(r, hi);
-  sigma[i] = r;
+  const float target = exp_form ? s * expf(0.5f * step) : s + step;
+  sigma[i] = clamp_sigma(s, target, lb_vec ? lb_vec[i] : -INFINITY, ub_vec ? ub_vec[i] : INFINITY, mc_vec != nullptr, mc_vec ? mc_vec[i] : 0.0f);
 }
 
+// E elites: grad_mu = S1 / E, grad_sigma = unbiased std - sigma.  As torch.std: E = 1 (a zero divisor) and E = 0 give NaN, and a NaN
+// variance stays NaN through the clamp at 0 (torch.clamp_min); without the E = 1 case the fp32 rounding error of S2 over 0 gave +-inf.
 __global__ void __launch_bounds__(256) cem_finalize_kernel(const float* __restrict__ s1, const float* __restrict__ s2,
                                                            const float* __restrict__ sigma, int64_t D, float E, float* __restrict__ grad_mu,
                                                            float* __restrict__ grad_sigma) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= D) return;
   const double a = (double)s1[i], b = (double)s2[i], e = (double)E;
-  const double var = (b - a * a / e) / (e - 1.0);
+  const double var = e > 1.0 ? (b - a * a / e) / (e - 1.0) : (double)NAN;
   grad_mu[i] = (float)(a / e);
-  grad_sigma[i] = (float)sqrt(var > 0.0 ? var : 0.0) - sigma[i];
+  grad_sigma[i] = (float)sqrt(var > 0.0 || var != var ? var : 0.0) - sigma[i];
 }
 
 }  // namespace evok
@@ -232,7 +228,7 @@ extern "C" EVOK_API int evok_sigma_update(float* sigma, const float* g, int64_t 
 extern "C" EVOK_API int evok_cem_finalize(const float* s1, const float* s2, const float* sigma, int64_t D, int64_t num_elites, float* grad_mu,
                                  float* grad_sigma, void* stream) {
   if (!s1 || !s2 || !sigma || !grad_mu || !grad_sigma) return EVOK_E_NULLPTR;
-  if (D <= 0 || num_elites < 1) return EVOK_E_BADSIZE;
+  if (D <= 0 || num_elites < 0) return EVOK_E_BADSIZE;
   cem_finalize_kernel<<<nblk(D), 256, 0, (cudaStream_t)stream>>>(s1, s2, sigma, D, (float)num_elites, grad_mu, grad_sigma);
   EVOK_CHECK_LAUNCH();
   return 0;

@@ -215,12 +215,14 @@ int evok_axpy(const float* g, int64_t D, float lr, float* mu, void* stream);
  *   exp_form == 0: target = sigma + lr*g          exp_form != 0: target = sigma * exp(0.5*lr*g)
  *   lo = max(lb, sigma - |sigma|*mc), hi = min(ub, sigma + |sigma|*mc); sigma <- min(max(target, lo), hi)
  * lb / ub / mc: device vectors (length D) or NULL; when NULL the scalar is used; a NaN scalar means
- * "not set" (-inf / +inf / no max-change limit). */
+ * "not set" (-inf / +inf / no max-change limit).  max / min are torch.max / torch.min: a NaN in any operand that is
+ * set (target, a vector entry, |sigma|*mc = 0*inf) makes the result NaN. */
 int evok_sigma_update(float* sigma, const float* g, int64_t D, float lr, int exp_form, const float* lb_vec,
                       float lb, const float* ub_vec, float ub, const float* mc_vec, float mc, void* stream);
 
 /* CEM finalisation from elite moments (distributions.py:543-546): given S1 = sum eps, S2 = sum eps^2 over
- * the E elites, writes grad_mu = S1/E and grad_sigma = sqrt((S2 - S1^2/E)/(E-1)) - sigma. */
+ * the E elites, writes grad_mu = S1/E and grad_sigma = sqrt(max((S2 - S1^2/E)/(E-1), 0)) - sigma.  As torch.std of
+ * E < 2 rows, E = 1 gives grad_sigma = NaN and E = 0 NaN in both; a NaN variance stays NaN (torch.clamp_min). */
 int evok_cem_finalize(const float* s1, const float* s2, const float* sigma, int64_t D, int64_t num_elites,
                       float* grad_mu, float* grad_sigma, void* stream);
 
@@ -304,7 +306,8 @@ int evok_transpose_pair(const float* in, int64_t ldi, int64_t rows, int64_t cols
 /* ---------------------------------------------------------------------------------------------
  * Batched searches: the functional ask / tell API with leading batch dimensions (algorithms/functional/funcpgpe.py:67, :301, :330,
  * funccem.py, funcclipup.py:95-108; `expects_ndim`, decorators.py:613).  n_items independent searches of the same shape run in ONE
- * launch per stage (grid y / z = item) instead of one launch chain per item.  Tensors are contiguous [items][...] unless an item
+ * launch per stage (grid y / z = item) instead of one launch chain per item; above 65535 items (the grid y / z limit) a stage runs
+ * as item chunks of at most 65535, in order on the stream, reusing one workspace.  Tensors are contiguous [items][...] unless an item
  * stride is given (stride 0 = the operand is shared by all items).  Per-item scalar hyper-parameters are HOST arrays (they travel in
  * the launch parameters).  Every stage computes exactly what its single-search entry point computes per item.
  * --------------------------------------------------------------------------------------------- */
@@ -312,7 +315,7 @@ int evok_transpose_pair(const float* in, int64_t ldi, int64_t rows, int64_t cols
 int evok_sample_batched(float* X, int64_t item_stride_x, int64_t ldx, const float* mu, int64_t item_stride_mu, const float* sigma,
                         int64_t item_stride_sigma, int64_t n_items, int64_t n_rows, int64_t D, int symmetric, uint64_t seed, uint64_t stream_id0,
                         void* stream);
-/* K3: f, w: [items][N].  ws: max(evok_rank_workspace_bytes(N), 8 * n_items + 256) bytes */
+/* K3: f, w: [items][N].  ws: max(evok_rank_workspace_bytes(N), 8 * min(n_items, 65535) + 256) bytes */
 int evok_rank_batched(int method, const float* f, int64_t N, int64_t n_items, int higher_is_better, float* w, void* ws, size_t ws_bytes,
                       void* stream);
 int evok_elite_mask_batched(const float* w, int64_t N, int64_t n_items, int64_t num_elites, float* mask, void* ws, size_t ws_bytes, void* stream);

@@ -103,5 +103,23 @@ for tag, case in cem_cases.items():
     for k, v in rec.items():
         out[f"cem/{tag}/{k}"] = np.stack(v)
 
+# ---------------------------------------------------------------- functional CEM at its edges (one tell each; drawn after every case
+# above, so the keys above do not change).  One elite: std of one row is NaN.  No elite: mean and std of no rows are NaN.  A zero in
+# `stdev_init` with the default stdev_max_change=None (inf): the allowed change |0| * inf is NaN, and torch.max / torch.min keep it.
+cem_edge_cases = {
+    "one_elite": dict(kw=dict(parenthood_ratio=0.03, objective_sense="min", stdev_init=1.0), batch=()),
+    "zero_elites": dict(kw=dict(parenthood_ratio=0.01, objective_sense="max", stdev_init=1.0), batch=()),
+    "zero_stdev": dict(kw=dict(parenthood_ratio=0.25, objective_sense="min", stdev_init=T([1.0, 0.0] * (D // 2))), batch=()),
+}
+for tag, case in cem_edge_cases.items():
+    center0 = T(rng.uniform(-3, 3, size=case["batch"] + (D,)))
+    st = cem(center_init=center0, **case["kw"])
+    out[f"cem/{tag}/center0"], out[f"cem/{tag}/stdev0"] = npy(center0), npy(st.stdev)
+    values = cem_ask(st, popsize=N)
+    evals = rastrigin(values)
+    st = cem_tell(st, values, evals)
+    for k, v in (("values", values), ("evals", evals), ("center", st.center), ("stdev", st.stdev)):
+        out[f"cem/{tag}/{k}"] = npy(v)[None]
+
 np.savez_compressed(os.path.join(HERE, "functional_golden.npz"), **out)
 print("wrote", len(out), "arrays ->", os.path.join(HERE, "functional_golden.npz"), file=sys.stderr)

@@ -72,6 +72,10 @@ CEM_CASES = {
     "plain": dict(parenthood_ratio=0.25, objective_sense="min", stdev_init=2.0, stdev_max_change=0.3),
     "max_bounds": dict(parenthood_ratio=0.5, objective_sense="max", stdev_init=1.0, stdev_min=0.4, stdev_max=1.5),
     "batched": dict(parenthood_ratio=0.25, objective_sense="min"),
+    # the edges, where the reference gives NaN: one elite (std of one row), no elite, a zero stdev with an unlimited max change
+    "one_elite": dict(parenthood_ratio=0.03, objective_sense="min", stdev_init=1.0),
+    "zero_elites": dict(parenthood_ratio=0.01, objective_sense="max", stdev_init=1.0),
+    "zero_stdev": dict(parenthood_ratio=0.25, objective_sense="min"),
 }
 
 
@@ -79,8 +83,8 @@ CEM_CASES = {
 @pytest.mark.parametrize("tag", list(CEM_CASES))
 def test_functional_cem_tell_matches_reference(tag, device):
     kw = dict(CEM_CASES[tag])
-    if tag == "batched":
-        kw["stdev_init"] = T(GOLD["cem/batched/stdev0"], device)
+    if tag in ("batched", "zero_stdev"):
+        kw["stdev_init"] = T(GOLD[f"cem/{tag}/stdev0"], device)
     state = F.cem(center_init=T(GOLD[f"cem/{tag}/center0"], device), **kw)
     for g in range(GOLD[f"cem/{tag}/values"].shape[0]):
         state = F.cem_tell(state, T(GOLD[f"cem/{tag}/values"][g], device), T(GOLD[f"cem/{tag}/evals"][g], device))
