@@ -166,6 +166,9 @@ __device__ __forceinline__ void st_stream1(float* p, float a) {
 //   add(x, j)   : fold element x of column j (0-based, global) into this lane's partial sums;
 //   finish(D)   : warp-reduce the partials and return the fitness of the row (every lane gets it; lane 0 stores it).
 // A row's elements reach add() in no fixed column order (strided over the lanes of a warp), so an accumulator holds sums.
+// A generated accumulator may also have pair terms (`static constexpr bool kPairs = true`, see PairTerms below):
+//   add_pair(x, xn, j) : fold the neighbour pair (x_j, x_{j+1}); it is called exactly once for every j in [0, D-2] of a row,
+//                        by the lane that holds column j+1, also in no fixed order across lanes (fold_pairs).
 // The built-in ones are ObjAcc<EVOK_OBJ_*>; a user-defined one is generated by evotorch_b200/jit.py.
 // ------------------------------------------------------------------------------------------------
 template <int OBJ>
@@ -221,6 +224,35 @@ template <>
 struct SampleOnly<ObjAcc<EVOK_OBJ_NONE>> {
   static constexpr bool value = true;
 };
+
+// true for an accumulator that declares `static constexpr bool kPairs = true` (a generated one whose terms use x_{j+1});
+// false for every ObjAcc<> and every accumulator without the marker.  All pair code is under `if constexpr` on it.
+template <typename Acc, typename = void>
+struct PairTerms {
+  static constexpr bool value = false;
+};
+template <typename Acc>
+struct PairTerms<Acc, decltype(void(Acc::kPairs))> {
+  static constexpr bool value = Acc::kPairs;
+};
+
+// One warp step of pair folds: this lane holds the N consecutive columns j .. j+N-1 of a row (v[]), of which the first
+// n_valid exist (0 for a lane past the row's end).  The lane holding column c + 1 folds (x_c, x_{c+1}): inside v[] from
+// registers, and for its first column with x_{j-1} = the last column of lane - 1, or for lane 0 the last column lane 31
+// held in the previous step of the same row (`carry`, zero-initialised per row and advanced here).  Every lane of the warp
+// must call it on every step, in the same order (it shuffles); a column's left neighbour is always in the previous lane
+// or the previous step because each step covers 32 * N consecutive columns.
+template <int N, typename Acc>
+__device__ __forceinline__ void fold_pairs(Acc& acc, const float (&v)[N], int64_t j, int n_valid, float& carry) {
+  const int lane = threadIdx.x & 31;
+  const float rot = __shfl_sync(0xffffffffu, v[N - 1], (lane + 31) & 31);  // lane 0 receives lane 31's: next step's carry
+  const float left = lane == 0 ? carry : rot;
+  carry = rot;
+  if (n_valid > 0 && j > 0) acc.add_pair(left, v[0], j - 1);
+#pragma unroll
+  for (int c = 1; c < N; ++c)
+    if (c < n_valid) acc.add_pair(v[c - 1], v[c], j + c - 1);
+}
 
 // ------------------------------------------------------------------------------------------------
 // K1 / K2 kernels.  HBM-bound design: one warp owns one direction (a +/- row pair) or one row; every lane produces 4
@@ -295,6 +327,57 @@ __device__ __forceinline__ void sample_group(const PhiloxKey& key, uint32_t sw, 
   }
 }
 
+// sample_group for an accumulator with pair terms, called by EVERY lane of the warp on every step (fold_pairs shuffles): a
+// lane whose group lies past the row's end (!active) draws, loads and stores nothing and folds nothing.  The samples and the
+// element adds are those of sample_group, in the same order; the + and - rows have their own neighbours and carries.
+template <typename Acc, bool SYM, bool STORE, bool VEC, bool SQ>
+__device__ __forceinline__ void sample_group_pairs(const PhiloxKey& key, uint32_t sw, uint64_t unit, uint32_t q, int64_t D,
+                                                   const float* __restrict__ mu, const float* __restrict__ sigma, float* xp, float* xm,
+                                                   Acc& accp, Acc& accm, float* zsq, bool active, float& carry_p, float& carry_m) {
+  float p[4] = {0.f, 0.f, 0.f, 0.f}, n[4] = {0.f, 0.f, 0.f, 0.f};
+  const int64_t j = (int64_t)q << 2;
+  int n_valid = 0;
+  if (active) {
+    float z[4];
+    normals4(key, sw, unit, q, z);
+    if (VEC) {
+      if (SQ) {
+        *zsq = fmaf(z[0], z[0], *zsq); *zsq = fmaf(z[1], z[1], *zsq); *zsq = fmaf(z[2], z[2], *zsq); *zsq = fmaf(z[3], z[3], *zsq);
+      }
+      const float4 m = __ldg(reinterpret_cast<const float4*>(mu + j));
+      const float4 s = __ldg(reinterpret_cast<const float4*>(sigma + j));
+      p[0] = fmaf(s.x, z[0], m.x); p[1] = fmaf(s.y, z[1], m.y); p[2] = fmaf(s.z, z[2], m.z); p[3] = fmaf(s.w, z[3], m.w);
+      if (STORE) st_stream4(xp + j, p[0], p[1], p[2], p[3]);
+      accp.add(p[0], j); accp.add(p[1], j + 1); accp.add(p[2], j + 2); accp.add(p[3], j + 3);
+      if (SYM) {
+        n[0] = fmaf(-s.x, z[0], m.x); n[1] = fmaf(-s.y, z[1], m.y); n[2] = fmaf(-s.z, z[2], m.z); n[3] = fmaf(-s.w, z[3], m.w);
+        if (STORE) st_stream4(xm + j, n[0], n[1], n[2], n[3]);
+        accm.add(n[0], j); accm.add(n[1], j + 1); accm.add(n[2], j + 2); accm.add(n[3], j + 3);
+      }
+      n_valid = 4;
+    } else {
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+        if (j + c < D) {
+          if (SQ) *zsq = fmaf(z[c], z[c], *zsq);
+          const float m = __ldg(mu + j + c), s = __ldg(sigma + j + c);
+          p[c] = fmaf(s, z[c], m);
+          if (STORE) st_stream1(xp + j + c, p[c]);
+          accp.add(p[c], j + c);
+          if (SYM) {
+            n[c] = fmaf(-s, z[c], m);
+            if (STORE) st_stream1(xm + j + c, n[c]);
+            accm.add(n[c], j + c);
+          }
+        }
+      }
+      n_valid = D - j < 4 ? (int)(D - j) : 4;  // the partial last group: a pair is folded only where column j + 1 < D
+    }
+  }
+  fold_pairs<4>(accp, p, j, n_valid, carry_p);
+  if (SYM) fold_pairs<4>(accm, n, j, n_valid, carry_m);
+}
+
 // PUSH: the fitness of row i goes to row (row0 + i) of EVERY peer's fitness vector (the all-gather of the sharded
 // generation, fused into the producer) and the last CTA raises this rank's flag on every peer.
 // SQ (non-symmetric only): q[r] = sum_j z_rj^2 of the unscaled normals, accumulated in registers next to the objective.
@@ -320,16 +403,32 @@ __global__ void __launch_bounds__(kSampleThreads, SampleTune<Acc>::kMinBlocks)
     const uint64_t unit = unit0 + (uint64_t)u;
     constexpr int kSampleUnroll = SampleTune<Acc>::kUnroll;
     float zsq = 0.f;
-    uint32_t q = lane;
-    if (kSampleUnroll > 1) {
-      // independent Philox chains in flight per lane
-      for (; q + 32u * (kSampleUnroll - 1) < nq; q += 32u * kSampleUnroll) {
+    if constexpr (PairTerms<Acc>::value) {
+      // warp-uniform steps of 32 groups (fold_pairs shuffles); each lane still visits its groups lane, lane + 32, ... in
+      // increasing order, the order of the loops below and of eval_kernel
+      float carry_p = 0.f, carry_m = 0.f;
+      uint32_t b = 0;
+      for (; b + 32u * kSampleUnroll <= nq; b += 32u * kSampleUnroll) {
 #pragma unroll
         for (int uu = 0; uu < kSampleUnroll; ++uu)
-          sample_group<Acc, SYM, STORE, VEC, SQ>(key, sw, unit, q + 32u * uu, D, mu, sigma, xp, xm, accp, accm, &zsq);
+          sample_group_pairs<Acc, SYM, STORE, VEC, SQ>(key, sw, unit, b + 32u * uu + lane, D, mu, sigma, xp, xm, accp, accm, &zsq, true,
+                                                       carry_p, carry_m);
       }
+      for (; b < nq; b += 32)
+        sample_group_pairs<Acc, SYM, STORE, VEC, SQ>(key, sw, unit, b + lane, D, mu, sigma, xp, xm, accp, accm, &zsq, b + lane < nq,
+                                                     carry_p, carry_m);
+    } else {
+      uint32_t q = lane;
+      if (kSampleUnroll > 1) {
+        // independent Philox chains in flight per lane
+        for (; q + 32u * (kSampleUnroll - 1) < nq; q += 32u * kSampleUnroll) {
+#pragma unroll
+          for (int uu = 0; uu < kSampleUnroll; ++uu)
+            sample_group<Acc, SYM, STORE, VEC, SQ>(key, sw, unit, q + 32u * uu, D, mu, sigma, xp, xm, accp, accm, &zsq);
+        }
+      }
+      for (; q < nq; q += 32) sample_group<Acc, SYM, STORE, VEC, SQ>(key, sw, unit, q, D, mu, sigma, xp, xm, accp, accm, &zsq);
     }
-    for (; q < nq; q += 32) sample_group<Acc, SYM, STORE, VEC, SQ>(key, sw, unit, q, D, mu, sigma, xp, xm, accp, accm, &zsq);
     if (SQ) {
       zsq = warp_sum(zsq);
       if (lane == 0) q_out[r] = zsq;
@@ -366,7 +465,47 @@ __global__ void __launch_bounds__(kEvalThreads)
   for (int64_t r = gw; r < n_rows; r += warps_total) {
     Acc acc(D);
     const float* x = X + r * ldx;
-    if (VEC) {
+    if constexpr (PairTerms<Acc>::value) {
+      // warp-uniform steps (fold_pairs shuffles); per lane the groups, element adds and pair folds of sample_eval_kernel's
+      // VEC path in the same order, so both kernels give the same fitness bit for bit on the same X
+      float carry = 0.f;
+      if (VEC) {
+        const int64_t nq = D >> 2;
+        int64_t b = 0;
+        for (; b + 128 <= nq; b += 128) {
+          const int64_t q = b + lane;
+          float4 g[4];
+#pragma unroll
+          for (int k = 0; k < 4; ++k) g[k] = ld_stream4(x + 4 * (q + 32 * k));
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const int64_t jk = 4 * (q + 32 * k);
+            const float v[4] = {g[k].x, g[k].y, g[k].z, g[k].w};
+            acc.add(v[0], jk); acc.add(v[1], jk + 1); acc.add(v[2], jk + 2); acc.add(v[3], jk + 3);
+            fold_pairs<4>(acc, v, jk, 4, carry);
+          }
+        }
+        for (; b < nq; b += 32) {
+          const int64_t q = b + lane;
+          const bool active = q < nq;
+          const float4 a = active ? ld_stream4(x + 4 * q) : make_float4(0.f, 0.f, 0.f, 0.f);
+          const float v[4] = {a.x, a.y, a.z, a.w};
+          const int64_t ja = 4 * q;
+          if (active) {
+            acc.add(v[0], ja); acc.add(v[1], ja + 1); acc.add(v[2], ja + 2); acc.add(v[3], ja + 3);
+          }
+          fold_pairs<4>(acc, v, ja, active ? 4 : 0, carry);
+        }
+      } else {
+        for (int64_t b = 0; b < D; b += 32) {
+          const int64_t j = b + lane;
+          const bool active = j < D;
+          const float v[1] = {active ? ld_stream1(x + j) : 0.f};
+          if (active) acc.add(v[0], j);
+          fold_pairs<1>(acc, v, j, active ? 1 : 0, carry);
+        }
+      }
+    } else if (VEC) {
       const int64_t nq = D >> 2;
       int64_t q = lane;
       // 4 independent 128-bit loads in flight per lane

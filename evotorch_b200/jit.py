@@ -1,7 +1,13 @@
-"""Run-time compiled objectives: a sum-separable function given as Python expressions becomes an accumulator of the fused
-sampler (csrc/evok_sampler.cuh), compiled with NVRTC for sm_90a and registered with libevok.so.
+"""Run-time compiled objectives: a function of sums over the elements or neighbour pairs of a row, given as Python
+expressions, becomes an accumulator of the fused sampler (csrc/evok_sampler.cuh), compiled with NVRTC for sm_90a and
+registered with libevok.so.
 
-    f(x) = value(S_1, ..., S_k, D),    S_i = sum_j term_i(x_j, j, D),    k <= 4
+    f(x) = value(S_1, ..., S_k, D),    k <= 4,
+    S_i = sum_{j=0}^{D-1} term_i(x_j, j, D)              (an element term), or
+    S_i = sum_{j=0}^{D-2} term_i(x_j, x_{j+1}, j, D)     (a pair term: one that uses xn; 0 when D = 1)
+
+Pair terms give the chained test functions, e.g. Rosenbrock: {"s": "100*(xn - x**2)**2 + (1 - x)**2"}, value "s".  One
+objective may mix both kinds.
 
 One parse of the expressions gives both the CUDA accumulator and a torch function of the same formula (the evaluation of
 CPU problems, other dtypes, rng="torch" and before-eval hooks; the float64 reference of the tests).
@@ -11,8 +17,10 @@ The expression language (anything else raises ValueError):
   - functions  abs sqrt exp log sin cos tan tanh floor minimum maximum  (minimum / maximum return the other operand when
     one is NaN, like fminf / fmaxf and torch.fmin / torch.fmax);
   - constants  pi, e, numeric literals;
-  - names      x (the element), j (its 0-based column) and D (the row length) in a term; the sum names and D in `value`.
+  - names      x (the element), xn (the next element x_{j+1}), j (the 0-based column of x) and D (the row length) in a
+    term; the sum names and D in `value`.
 The CUDA side evaluates in float32 with the precise libdevice functions (no fast math) and contracts a * b + c into fma.
+The source of an objective without pair terms is exactly that of the element-only language (no pair code in it).
 """
 
 from __future__ import annotations
@@ -154,7 +162,8 @@ _RESERVED = {"x", "j", "D"} | set(CONSTANTS) | set(FUNCTIONS)
 
 
 class ObjectiveSpec:
-    """The parsed form of a sum-separable objective: `source` is the CUDA translation unit, `torch_fn(X)` the torch function."""
+    """The parsed form of an objective: `source` is the CUDA translation unit, `torch_fn(X)` the torch function.  `pairs` names
+    the sums whose term uses xn (summed over the neighbour pairs of a row); the others are summed over its elements."""
 
     def __init__(self, sums: Dict[str, str], value: str):
         if not isinstance(sums, dict) or not 1 <= len(sums) <= MAX_SUMS:
@@ -163,8 +172,9 @@ class ObjectiveSpec:
             if not (isinstance(s, str) and s.isidentifier()) or s in _RESERVED:
                 raise ValueError(f"sums: {s!r} cannot name a sum (a sum name is an identifier other than {sorted(_RESERVED)})")
         self.sums, self.value = dict(sums), value
-        term_names = {"x": "x", "j": "jf", "D": "Df"}
+        term_names = {"x": "x", "xn": "xn", "j": "jf", "D": "Df"}
         self.terms = {s: _parse(t, term_names, f"sums[{s!r}]") for s, t in sums.items()}
+        self.pairs = frozenset(s for s, e in self.terms.items() if re.search(r"\bxn\b", e.cuda))
         value_names = {s: f"S_{s}" for s in sums}
         value_names["D"] = "Df"
         self.value_expr = _parse(value, value_names, "value")
@@ -172,16 +182,26 @@ class ObjectiveSpec:
 
     def _cuda_source(self) -> str:
         k = range(len(self.terms))
-        exprs = list(self.terms.values())
+        uses_j = lambda es: any(re.search(r"\bjf\b", e.cuda) for e in es)  # noqa: E731
+        element = [(i, e) for i, (s, e) in zip(k, self.terms.items()) if s not in self.pairs]
+        pair = [(i, e) for i, (s, e) in zip(k, self.terms.items()) if s in self.pairs]
         lines = ['#include "evok_sampler.cuh"', "", "namespace evok_user {", "struct Acc {"]
+        if pair:
+            lines.append("  static constexpr bool kPairs = true;")
         lines.append("  float Df;")
         lines.append("  float " + ", ".join(f"s{i} = 0.f" for i in k) + ";")
         lines.append("  __device__ __forceinline__ explicit Acc(int64_t D) : Df((float)D) {}")
         lines.append("  __device__ __forceinline__ void add(float x, int64_t j) {")
-        if any(re.search(r"\bjf\b", e.cuda) for e in exprs):
+        if uses_j(e for _, e in element):
             lines.append("    const float jf = (float)j;")
-        lines += [f"    s{i} += {e.cuda};" for i, e in zip(k, exprs)]
+        lines += [f"    s{i} += {e.cuda};" for i, e in element]
         lines.append("  }")
+        if pair:
+            lines.append("  __device__ __forceinline__ void add_pair(float x, float xn, int64_t j) {")
+            if uses_j(e for _, e in pair):
+                lines.append("    const float jf = (float)j;")
+            lines += [f"    s{i} += {e.cuda};" for i, e in pair]
+            lines.append("  }")
         lines.append("  __device__ __forceinline__ float finish(int64_t) {")
         lines += [f"    const float S_{s} = evok::warp_sum(s{i});" for i, s in zip(k, self.terms)]
         lines.append(f"    return {self.value_expr.cuda};")
@@ -190,10 +210,16 @@ class ObjectiveSpec:
 
     def torch_fn(self, X: torch.Tensor) -> torch.Tensor:
         D = X.shape[-1]
-        env = {"x": X, "j": torch.arange(D, dtype=X.dtype, device=X.device), "D": torch.tensor(float(D), dtype=X.dtype, device=X.device),
-               "_dtype": X.dtype, "_device": X.device}
-        venv = {s: torch.broadcast_to(_as_tensor(e.torch(env), env), X.shape).sum(dim=-1) for s, e in self.terms.items()}
-        venv.update(D=env["D"], _dtype=X.dtype, _device=X.device)
+        Dt = torch.tensor(float(D), dtype=X.dtype, device=X.device)
+        env = {"x": X, "j": torch.arange(D, dtype=X.dtype, device=X.device), "D": Dt, "_dtype": X.dtype, "_device": X.device}
+        # a pair term on (x_j, x_{j+1}) for j = 0 .. D-2: an empty sum when D = 1
+        penv = {"x": X[..., :-1], "xn": X[..., 1:], "j": torch.arange(max(D - 1, 0), dtype=X.dtype, device=X.device), "D": Dt,
+                "_dtype": X.dtype, "_device": X.device}
+        venv = {}
+        for s, e in self.terms.items():
+            en = penv if s in self.pairs else env
+            venv[s] = torch.broadcast_to(_as_tensor(e.torch(en), en), en["x"].shape).sum(dim=-1)
+        venv.update(D=Dt, _dtype=X.dtype, _device=X.device)
         return torch.broadcast_to(_as_tensor(self.value_expr.torch(venv), venv), X.shape[:-1])
 
 

@@ -8,8 +8,9 @@ written once and never re-read for evaluation.  Called directly on a CUDA fp32 p
 row-reduction kernel (K2); on any other tensor the plain torch expression (same formula as the reference's README
 example, README.md:86-89).
 
-`FusedObjective` is the same for a user-defined sum-separable function: its expressions are compiled at run time into the
-same kernels (evotorch_b200/jit.py), so every fused path of the package takes it.
+`FusedObjective` is the same for a user-defined function of sums over the elements (sum-separable) or over the neighbour
+pairs (x_j, x_{j+1}) of a row (Rosenbrock, Trid, Dixon-Price): its expressions are compiled at run time into the same kernels
+(evotorch_b200/jit.py), so every fused path of the package takes it.
 """
 
 from __future__ import annotations
@@ -58,11 +59,13 @@ def _ackley(x: torch.Tensor) -> torch.Tensor:
 
 
 class FusedObjective(BuiltinObjective):
-    """A user-defined objective f(x) = value(S_1, ..., S_k, D) with S_i = sum_j term_i(x_j, j, D), k <= 4, fused into the sampler.
+    """A user-defined objective f(x) = value(S_1, ..., S_k, D), k <= 4, fused into the sampler, where S_i is either
+    sum_{j<D} term_i(x_j, j, D) or, for a term that uses xn = x_{j+1}, the pair sum sum_{j<D-1} term_i(x_j, x_{j+1}, j, D).
 
         styblinski_tang = FusedObjective("styblinski_tang", sums={"s": "x**4 - 16*x**2 + 5*x"}, value="0.5 * s")
+        rosenbrock = FusedObjective("rosenbrock", sums={"s": "100*(xn - x**2)**2 + (1 - x)**2"}, value="s")
 
-    `sums` maps each sum's name to its term (an expression of x, j and D), `value` is an expression of the sums and D; the
+    `sums` maps each sum's name to its term (an expression of x, xn, j and D), `value` is an expression of the sums and D; the
     language is described in evotorch_b200.jit.  Construction parses both (ValueError for anything outside the language),
     compiles the kernels with NVRTC for sm_90a and registers them with libevok.so; `kernel_info` holds the registers and
     spills of every kernel.  The same source compiles once per process.  A FusedObjective pickles as its expressions."""

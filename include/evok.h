@@ -106,6 +106,8 @@ int evok_eval(int objective, const float* X, int64_t ldx, int64_t n_rows, int64_
  *   EVOK_OBJ_KERNEL_PUSH   + 4 sym + 2 store + vec : sample_eval_kernel<Acc, sym, store, vec, PUSH = true,  SQ = false>
  *   EVOK_OBJ_KERNEL_SQ     + 2 store + vec         : sample_eval_kernel<Acc, false, store, vec, PUSH = false, SQ = true>
  *   EVOK_OBJ_KERNEL_EVAL   + vec                   : eval_kernel<Acc, vec>
+ * The fitness of a row is Acc's function of sums over the row's elements x_j and, for an Acc with pair terms (kPairs), over
+ * its neighbour pairs (x_j, x_{j+1}), j = 0 .. D-2; the kernels fold each element and each pair exactly once.
  * It copies the image and the names, writes the new id to *id_out_host and needs no device.  The id is then accepted by
  * evok_sample_eval, evok_sample_eval_sq, evok_sample_eval_push and evok_eval, which launch the registered kernels exactly
  * as they launch a built-in objective's (same argument checks, kernel choice and grid).

@@ -42,6 +42,22 @@ for sym in (True, False):
         ops.axpy_(mu.clone(), g, 0.1)
         ops.sigma_update_(sg.clone(), g, 0.1, False, lb=0.01, ub=2.0, max_change=0.2)
         ops.cem_finalize(g, g * g + 1, sg, 5)
+# a run-time compiled objective with pair terms (x_j, x_{j+1}): the shuffles of the warp-uniform steps, the carry and the
+# partial groups, on the vectorised and the scalar paths of every sampling kernel and of the evaluation
+from evotorch_b200.objectives import FusedObjective  # noqa: E402
+
+pair_obj = FusedObjective("sanitize_pairs", {"s": "100*(xn - x**2)**2 + (1 - x)**2", "a": "abs(x)"}, "s + a").evok_objective_id
+for sym in (True, False):
+    for n, D in ((6, 1), (10, 7), (64, 16), (48, 130), (34, 1000), (4100, 1028), (40, 257), (40, 516)):
+        for off in (0, 1):  # off = 1: mu / sigma / X one float into their allocations, the scalar path
+            mu, sg = torch.randn(D + off, device=dev)[off:], (torch.rand(D + off, device=dev) + 0.1)[off:]
+            X, f = torch.empty(n, D + off, device=dev)[:, off:], torch.empty(n, device=dev)
+            ops.sample_eval(pair_obj, X, mu, sg, n_rows=n, symmetric=sym, seed=1, stream_id=2, f=f)
+            ops.sample_eval(pair_obj, None, mu, sg, n_rows=n, symmetric=sym, seed=1, stream_id=2, f=f)
+            if not sym:
+                ops.sample_eval_sq(pair_obj, X, mu, sg, torch.empty(n, device=dev), n_rows=n, seed=1, stream_id=2, f=f)
+                ops.sample_eval_sq(pair_obj, None, mu, sg, torch.empty(n, device=dev), n_rows=n, seed=1, stream_id=2, f=f)
+            ops.evaluate(pair_obj, X)
 # big-enough rank to use several tiles
 ops.rank(torch.randn(10_000, device=dev), "centered", False)
 # MLP: aligned and odd-length rows
