@@ -6,22 +6,12 @@
 #include <atomic>
 #include <mutex>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "evok_common.cuh"
 
 namespace evok {
-
-static int g_sm_count = 0;
-static int sm_count() {
-  if (g_sm_count == 0) {
-    int dev = 0, n = 0;
-    cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = kNumSMs;
-    g_sm_count = n;
-  }
-  return g_sm_count;
-}
 
 // Batched searches (functional ask/tell API with leading batch dimensions, funcpgpe.py:301-327): blockIdx.y = batch item, every
 // item has its own centre / stdev row (item stride 0 = shared) and its own Philox stream (stream word + item), so one launch
@@ -47,109 +37,72 @@ __global__ void __launch_bounds__(kSampleThreads, SampleTune<ObjAcc<EVOK_OBJ_NON
   }
 }
 
-template <typename K>
-static int resident_grid(K kernel, int threads, int64_t units_per_cta_needed) {
-  int per_sm = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, 0) != cudaSuccess || per_sm <= 0) per_sm = 4;
-  int64_t g = (int64_t)per_sm * sm_count();
-  if (g > units_per_cta_needed) g = units_per_cta_needed;
-  if (g < 1) g = 1;
-  return (int)g;
-}
-
 struct PushArgs {
   PeerSink sink;
   const unsigned long long* epoch;
   unsigned int* done;
 };
 
-template <int OBJ, bool SYM, bool STORE, bool PUSH = false, bool SQ = false>
-static int launch_sample(float* X, int64_t ldx, const float* mu, const float* sigma, int64_t row0, int64_t n_rows, int64_t D,
-                         uint64_t seed, uint64_t stream_id, const uint32_t* stream_off, float* f, cudaStream_t st,
-                         const PushArgs* push = nullptr, float* q = nullptr) {
-  const int64_t n_units = SYM ? n_rows / 2 : n_rows;
-  const bool vec = (D % 4 == 0) && aligned16(mu) && aligned16(sigma) && (!STORE || (aligned16(X) && ldx % 4 == 0));
-  const int64_t ctas_needed = (n_units + (kSampleThreads / 32) - 1) / (kSampleThreads / 32);
-  const PhiloxKey key = make_philox_key(seed, stream_id);
-  PushArgs none{};
-  const PushArgs& pa = PUSH ? *push : none;
-  if (vec) {
-    auto k = sample_eval_kernel<ObjAcc<OBJ>, SYM, STORE, true, PUSH, SQ>;
-    k<<<resident_grid(k, kSampleThreads, ctas_needed), kSampleThreads, 0, st>>>(X, ldx, mu, sigma, row0, n_units, D, key, stream_off, f, pa.sink,
-                                                                                pa.epoch, pa.done, q);
-  } else {
-    auto k = sample_eval_kernel<ObjAcc<OBJ>, SYM, STORE, false, PUSH, SQ>;
-    k<<<resident_grid(k, kSampleThreads, ctas_needed), kSampleThreads, 0, st>>>(X, ldx, mu, sigma, row0, n_units, D, key, stream_off, f, pa.sink,
-                                                                                pa.epoch, pa.done, q);
-  }
-  EVOK_CHECK_LAUNCH();
-  return 0;
-}
-
-template <int OBJ>
-static int dispatch_sample(float* X, int64_t ldx, const float* mu, const float* sigma, int64_t row0, int64_t n_rows, int64_t D,
-                           int symmetric, uint64_t seed, uint64_t stream_id, const uint32_t* stream_off, float* f, cudaStream_t st) {
-  if (symmetric) {
-    return X ? launch_sample<OBJ, true, true>(X, ldx, mu, sigma, row0, n_rows, D, seed, stream_id, stream_off, f, st)
-             : launch_sample<OBJ, true, false>(X, ldx, mu, sigma, row0, n_rows, D, seed, stream_id, stream_off, f, st);
-  }
-  return X ? launch_sample<OBJ, false, true>(X, ldx, mu, sigma, row0, n_rows, D, seed, stream_id, stream_off, f, st)
-           : launch_sample<OBJ, false, false>(X, ldx, mu, sigma, row0, n_rows, D, seed, stream_id, stream_off, f, st);
-}
-
-template <int OBJ>
-static int dispatch_sample_sq(float* X, int64_t ldx, const float* mu, const float* sigma, int64_t row0, int64_t n_rows, int64_t D, uint64_t seed,
-                              uint64_t stream_id, const uint32_t* stream_off, float* f, float* q, cudaStream_t st) {
-  if (X) return launch_sample<OBJ, false, true, false, true>(X, ldx, mu, sigma, row0, n_rows, D, seed, stream_id, stream_off, f, st, nullptr, q);
-  if constexpr (OBJ == EVOK_OBJ_NONE) return EVOK_E_NULLPTR;  // rejected by the entry point: no kernel for "q only"
-  else return launch_sample<OBJ, false, false, false, true>(X, ldx, mu, sigma, row0, n_rows, D, seed, stream_id, stream_off, f, st, nullptr, q);
-}
-
-template <int OBJ>
-static int dispatch_sample_push(float* X, int64_t ldx, const float* mu, const float* sigma, int64_t row0, int64_t n_rows, int64_t D,
-                                int symmetric, uint64_t seed, uint64_t stream_id, const uint32_t* stream_off, const PushArgs& push, cudaStream_t st) {
-  if (symmetric) {
-    return X ? launch_sample<OBJ, true, true, true>(X, ldx, mu, sigma, row0, n_rows, D, seed, stream_id, stream_off, nullptr, st, &push)
-             : launch_sample<OBJ, true, false, true>(X, ldx, mu, sigma, row0, n_rows, D, seed, stream_id, stream_off, nullptr, st, &push);
-  }
-  return X ? launch_sample<OBJ, false, true, true>(X, ldx, mu, sigma, row0, n_rows, D, seed, stream_id, stream_off, nullptr, st, &push)
-           : launch_sample<OBJ, false, false, true>(X, ldx, mu, sigma, row0, n_rows, D, seed, stream_id, stream_off, nullptr, st, &push);
-}
-
-template <int OBJ>
-static int launch_eval(const float* X, int64_t ldx, int64_t n_rows, int64_t D, float* f, cudaStream_t st) {
-  const bool vec = (D % 4 == 0) && aligned16(X) && (ldx % 4 == 0);
-  const int64_t ctas_needed = (n_rows + (kEvalThreads / 32) - 1) / (kEvalThreads / 32);
-  if (vec) {
-    auto k = eval_kernel<ObjAcc<OBJ>, true>;
-    k<<<resident_grid(k, kEvalThreads, ctas_needed), kEvalThreads, 0, st>>>(X, ldx, n_rows, D, f);
-  } else {
-    auto k = eval_kernel<ObjAcc<OBJ>, false>;
-    k<<<resident_grid(k, kEvalThreads, ctas_needed), kEvalThreads, 0, st>>>(X, ldx, n_rows, D, f);
-  }
-  EVOK_CHECK_LAUNCH();
-  return 0;
-}
-
 // ------------------------------------------------------------------------------------------------
-// Objectives registered at run time.  A registration keeps a copy of the cubin and the lowered names of its kernels (in the
-// EVOK_OBJ_KERNEL_* order); the module is loaded into the current device's primary context on the first use on that device
-// (each device has its own module, functions, occupancy and SM count).  Loaded modules stay until the process ends.
+// The kernel table.  Every objective, built-in or registered at run time (evok_objective_register: NVRTC-compiled
+// instantiations of the same kernels), has the EVOK_OBJ_KERNELS kernels of include/evok.h on each device.  One rule picks the
+// kernel of a call (choose_kernel) and one function launches it (launch).
 // ------------------------------------------------------------------------------------------------
+
+// The position of a kernel in the EVOK_OBJ_KERNEL_* order: its family (EVOK_OBJ_KERNEL_SAMPLE, _PUSH, _SQ or _EVAL), then
+// + 4 sym (SAMPLE and PUSH), + 2 store (all but EVAL), + vec.  jit.kernel_expressions() lists a registered objective's kernels
+// in the same order.
+constexpr int kernel_index(int family, bool sym, bool store, bool vec) {
+  return family + (sym && family < EVOK_OBJ_KERNEL_SQ ? 4 : 0) + (store && family < EVOK_OBJ_KERNEL_EVAL ? 2 : 0) + (vec ? 1 : 0);
+}
+
+static int kernel_threads(int k) { return k >= EVOK_OBJ_KERNEL_EVAL ? kEvalThreads : kSampleThreads; }
+
+// The sampler of built-in objective OBJ with the variant bits V = sym | store << 1 | vec << 2 | push << 3 | sq << 4, if it
+// exists (the SQ sampler is plain and non-symmetric) and can be reached: EVOK_OBJ_NONE only stores samples, since
+// evok_sample_eval and _sq refuse it without X, and _push refuses it always.
+template <int OBJ, int V>
+static void put_builtin_sampler(void** fn) {
+  constexpr bool sym = V & 1, store = V & 2, vec = V & 4, push = V & 8, sq = V & 16;
+  if constexpr (!(sq && (sym || push)) && (OBJ != EVOK_OBJ_NONE || (store && !push)))
+    fn[kernel_index(sq ? EVOK_OBJ_KERNEL_SQ : push ? EVOK_OBJ_KERNEL_PUSH : EVOK_OBJ_KERNEL_SAMPLE, sym, store, vec)] =
+        reinterpret_cast<void*>(sample_eval_kernel<ObjAcc<OBJ>, sym, store, vec, push, sq>);
+}
+
+template <int OBJ, int... V>
+static void put_builtin_kernels(void** fn, std::integer_sequence<int, V...>) {
+  (put_builtin_sampler<OBJ, V>(fn), ...);
+  if constexpr (OBJ != EVOK_OBJ_NONE) {  // evok_eval refuses EVOK_OBJ_NONE
+    fn[kernel_index(EVOK_OBJ_KERNEL_EVAL, false, true, false)] = reinterpret_cast<void*>(eval_kernel<ObjAcc<OBJ>, false>);
+    fn[kernel_index(EVOK_OBJ_KERNEL_EVAL, false, true, true)] = reinterpret_cast<void*>(eval_kernel<ObjAcc<OBJ>, true>);
+  }
+}
+
+template <int OBJ>
+static void builtin_kernels(void** fn) {
+  put_builtin_kernels<OBJ>(fn, std::make_integer_sequence<int, 32>());
+}
+
+static void (*const kBuiltinKernels[EVOK_OBJ_COUNT])(void**) = {builtin_kernels<EVOK_OBJ_NONE>, builtin_kernels<EVOK_OBJ_SPHERE>,
+                                                                 builtin_kernels<EVOK_OBJ_RASTRIGIN>, builtin_kernels<EVOK_OBJ_ACKLEY>};
+
 constexpr int kMaxDevices = 64;
 
-struct UserDevice {
-  int state = 0;  // 0: not loaded; 1: loaded; EVOK_E_NOKERNEL: the cubin lacks a kernel (a permanent failure)
-  CUmodule module = nullptr;
-  CUfunction fn[EVOK_OBJ_KERNELS] = {};
-  int per_sm[EVOK_OBJ_KERNELS] = {};
+// The kernels of one objective on one device, filled on the first use there and kept until the process ends.  A built-in
+// objective's entries are its nvcc-compiled kernels (null where no entry point reaches them); a registered objective's are the
+// functions of its module, loaded into the device's primary context.
+struct DeviceKernels {
+  int state = 0;              // 0: not filled; 1: filled; EVOK_E_NOKERNEL: the cubin lacks a kernel (a permanent failure)
+  CUmodule module = nullptr;  // set for a registered objective: fn holds CUfunctions, launched through the driver
+  void* fn[EVOK_OBJ_KERNELS] = {};
+  int per_sm[EVOK_OBJ_KERNELS] = {};  // resident CTAs per SM
   int sms = 0;
 };
 
-struct UserObjective {
-  std::vector<char> image;
+struct Objective {
+  std::vector<char> image;  // a registered objective's cubin and the lowered names of its kernels (in the EVOK_OBJ_KERNEL_* order)
   std::vector<std::string> names;
-  UserDevice dev[kMaxDevices];
+  DeviceKernels dev[kMaxDevices];
 };
 
 // the driver API through the runtime's entry points (the library does not link libcuda)
@@ -182,91 +135,141 @@ static bool driver_api() {
          driver_symbol("cuLaunchKernel", d.launch);
 }
 
-static std::mutex g_user_mutex;
-static UserObjective* g_user[EVOK_OBJ_USER_CAPACITY];
+static std::mutex g_objective_mutex;
+static Objective g_builtin[EVOK_OBJ_COUNT];
+static Objective* g_user[EVOK_OBJ_USER_CAPACITY];
 static std::atomic<int> g_user_count{0};
 
 static bool is_user(int objective) {
   return objective >= EVOK_OBJ_USER_BASE && objective - EVOK_OBJ_USER_BASE < g_user_count.load(std::memory_order_acquire);
 }
 
-static int kernel_threads(int k) { return k >= EVOK_OBJ_KERNEL_EVAL ? kEvalThreads : kSampleThreads; }
+static void fill_builtin(int objective, int dev, DeviceKernels& d) {
+  kBuiltinKernels[objective](d.fn);
+  for (int k = 0; k < EVOK_OBJ_KERNELS; ++k)
+    if (d.fn[k] && (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&d.per_sm[k], d.fn[k], kernel_threads(k), 0) != cudaSuccess || d.per_sm[k] <= 0))
+      d.per_sm[k] = 4;
+  if (cudaDeviceGetAttribute(&d.sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || d.sms <= 0) d.sms = kNumSMs;
+  d.state = 1;
+}
 
-// The loaded module of a registered objective on the current device (loaded here on the first call for that device).
-static int user_device(int objective, const UserDevice** out) {
+static int load_module(const Objective& obj, int dev, DeviceKernels& d) {
+  cudaError_t ce = cudaSetDevice(dev);  // makes the device's primary context (the runtime's) current, creating it if needed
+  if (ce != cudaSuccess) return (int)ce;
+  if (!driver_api()) return (int)cudaErrorNotSupported;
+  const DriverApi& api = g_driver;
+  CUdevice cu_dev;
+  CUresult r = api.device_get(&cu_dev, dev);
+  if (r == CUDA_SUCCESS) r = api.device_attribute(&d.sms, CU_DEVICE_ATTRIBUTE_MULTIPROCESSOR_COUNT, cu_dev);
+  if (r == CUDA_SUCCESS) r = api.module_load(&d.module, obj.image.data());
+  if (r != CUDA_SUCCESS) return (int)r;  // CUresult and cudaError_t share their codes
+  for (int k = 0; k < EVOK_OBJ_KERNELS; ++k) {
+    CUfunction fn = nullptr;
+    if (api.module_function(&fn, d.module, obj.names[k].c_str()) != CUDA_SUCCESS) {
+      api.module_unload(d.module);
+      d.module = nullptr;
+      d.state = EVOK_E_NOKERNEL;
+      return d.state;
+    }
+    d.fn[k] = fn;
+    if (api.occupancy(&d.per_sm[k], fn, kernel_threads(k), 0) != CUDA_SUCCESS || d.per_sm[k] <= 0) d.per_sm[k] = 4;
+  }
+  if (d.sms <= 0) d.sms = kNumSMs;
+  d.state = 1;
+  return 0;
+}
+
+// The kernel table of an objective (a built-in id or a registered one) on the current device, filled here on the first call
+// for that device.
+static int device_kernels(int objective, const DeviceKernels** out) {
   int dev = 0;
-  cudaError_t ce = cudaGetDevice(&dev);
+  const cudaError_t ce = cudaGetDevice(&dev);
   if (ce != cudaSuccess) return (int)ce;
   if (dev < 0 || dev >= kMaxDevices) return EVOK_E_BADSIZE;
-  std::lock_guard<std::mutex> lock(g_user_mutex);
-  UserObjective& obj = *g_user[objective - EVOK_OBJ_USER_BASE];
-  UserDevice& d = obj.dev[dev];
+  std::lock_guard<std::mutex> lock(g_objective_mutex);
+  const bool user = objective >= EVOK_OBJ_USER_BASE;
+  Objective& obj = user ? *g_user[objective - EVOK_OBJ_USER_BASE] : g_builtin[objective];
+  DeviceKernels& d = obj.dev[dev];
   if (d.state == 0) {
-    ce = cudaSetDevice(dev);  // makes the device's primary context (the runtime's) current, creating it if needed
-    if (ce != cudaSuccess) return (int)ce;
-    if (!driver_api()) return (int)cudaErrorNotSupported;
-    const DriverApi& api = g_driver;
-    CUdevice cu_dev;
-    CUresult r = api.device_get(&cu_dev, dev);
-    if (r == CUDA_SUCCESS) r = api.device_attribute(&d.sms, CU_DEVICE_ATTRIBUTE_MULTIPROCESSOR_COUNT, cu_dev);
-    if (r == CUDA_SUCCESS) r = api.module_load(&d.module, obj.image.data());
-    if (r != CUDA_SUCCESS) return (int)r;  // CUresult and cudaError_t share their codes
-    for (int k = 0; k < EVOK_OBJ_KERNELS; ++k) {
-      if (api.module_function(&d.fn[k], d.module, obj.names[k].c_str()) != CUDA_SUCCESS) {
-        api.module_unload(d.module);
-        d.module = nullptr;
-        d.state = EVOK_E_NOKERNEL;
-        return d.state;
-      }
-      if (api.occupancy(&d.per_sm[k], d.fn[k], kernel_threads(k), 0) != CUDA_SUCCESS || d.per_sm[k] <= 0) d.per_sm[k] = 4;
-    }
-    if (d.sms <= 0) d.sms = kNumSMs;
-    d.state = 1;
+    if (!user) fill_builtin(objective, dev, d);
+    else if (const int rc = load_module(obj, dev, d)) return rc;
   }
   if (d.state != 1) return d.state;
   *out = &d;
   return 0;
 }
 
-// the launch of kernel k with the grid rule of resident_grid (the driver API is resolved: user_device succeeded)
-static int user_launch(const UserDevice& d, int k, int64_t ctas_needed, void** args, cudaStream_t st) {
-  int64_t g = (int64_t)d.per_sm[k] * d.sms;
-  if (g > ctas_needed) g = ctas_needed;
+struct KernelChoice {
+  int k;                // index in the EVOK_OBJ_KERNEL_* order
+  int64_t n_units;      // rows, or antithetic row pairs for symmetric sampling; one warp each
+  int64_t ctas_needed;  // CTAs that give every unit its own warp
+};
+
+// The kernel of a call: family (EVOK_OBJ_KERNEL_*) and sym; stored samples when X is given; the vectorised variant when
+// D % 4 == 0 and every operand read or written with float4 loads / stores is 16-byte aligned with 16-byte aligned rows (mu and
+// sigma are null for the evaluation kernel, which reads X only).
+static KernelChoice choose_kernel(int family, bool sym, const float* X, int64_t ldx, const float* mu, const float* sigma, int64_t n_rows,
+                                  int64_t D) {
+  const bool store = X != nullptr;
+  const bool vec = (D % 4 == 0) && aligned16(mu) && aligned16(sigma) && (!store || (aligned16(X) && ldx % 4 == 0));
+  KernelChoice c;
+  c.k = kernel_index(family, sym, store, vec);
+  c.n_units = sym ? n_rows / 2 : n_rows;
+  const int warps = kernel_threads(c.k) / 32;
+  c.ctas_needed = (c.n_units + warps - 1) / warps;
+  return c;
+}
+
+// Launches kernel c.k of an objective on the current device with `args` in the kernel's parameter order, on as many CTAs as
+// stay resident but no more than the units need, and at least one (the push sampler with no rows still raises this rank's
+// flag).  A built-in kernel goes through the runtime, a registered one through the driver.
+static int launch(int objective, const KernelChoice& c, void** args, cudaStream_t st) {
+  const DeviceKernels* d = nullptr;
+  const int rc = device_kernels(objective, &d);
+  if (rc != 0) return rc;
+  int64_t g = (int64_t)d->per_sm[c.k] * d->sms;
+  if (g > c.ctas_needed) g = c.ctas_needed;
   if (g < 1) g = 1;
-  const CUresult r = g_driver.launch(d.fn[k], (unsigned)g, 1, 1, kernel_threads(k), 1, 1, 0, (CUstream)st, args, nullptr);
-  if (r != CUDA_SUCCESS) return (int)r;
-  count_launches(1);
+  const int threads = kernel_threads(c.k);
+  if (d->module) {
+    const CUresult r = g_driver.launch(static_cast<CUfunction>(d->fn[c.k]), (unsigned)g, 1, 1, threads, 1, 1, 0, (CUstream)st, args, nullptr);
+    if (r != CUDA_SUCCESS) return (int)r;
+    count_launches(1);
+    return 0;
+  }
+  cudaLaunchKernel(d->fn[c.k], dim3((unsigned)g), dim3(threads), args, 0, st);
+  EVOK_CHECK_LAUNCH();
   return 0;
 }
 
-// launch_sample for a registered objective: the same kernel choice (symmetric, store, VEC, PUSH, SQ) and grid
-static int user_sample(int objective, float* X, int64_t ldx, const float* mu, const float* sigma, int64_t row0, int64_t n_rows, int64_t D,
-                       bool sym, uint64_t seed, uint64_t stream_id, const uint32_t* stream_off, float* f, cudaStream_t st,
-                       const PushArgs* push = nullptr, float* q = nullptr) {
-  const UserDevice* d = nullptr;
-  const int rc = user_device(objective, &d);
-  if (rc != 0) return rc;
-  const bool store = X != nullptr;
-  int64_t n_units = sym ? n_rows / 2 : n_rows;
-  const bool vec = (D % 4 == 0) && aligned16(mu) && aligned16(sigma) && (!store || (aligned16(X) && ldx % 4 == 0));
-  const int64_t ctas_needed = (n_units + (kSampleThreads / 32) - 1) / (kSampleThreads / 32);
-  PhiloxKey key = make_philox_key(seed, stream_id);
-  PushArgs pa{};
-  if (push) pa = *push;
-  const int variant = (store ? 2 : 0) + (vec ? 1 : 0);
-  const int k = q ? EVOK_OBJ_KERNEL_SQ + variant : (push ? EVOK_OBJ_KERNEL_PUSH : EVOK_OBJ_KERNEL_SAMPLE) + (sym ? 4 : 0) + variant;
-  void* args[] = {&X, &ldx, &mu, &sigma, &row0, &n_units, &D, &key, &stream_off, &f, &pa.sink, &pa.epoch, &pa.done, &q};
-  return user_launch(*d, k, ctas_needed, args, st);
+// The argument checks of evok_sample_eval, _sq and _push, in the order of include/evok.h's error codes for them: the first
+// check that fails gives the code (the pointers only one entry point takes are checked there first, with mu and sigma).
+// push: the peer-exchange sampler, which takes no f, has no kernels for EVOK_OBJ_NONE and checks its world and rank.
+static int check_sample(int objective, const float* X, int64_t ldx, const float* mu, const float* sigma, int64_t row0, int64_t n_rows,
+                        int64_t D, bool sym, const float* f, const PushArgs* push) {
+  if (!mu || !sigma) return EVOK_E_NULLPTR;
+  const int first = push ? EVOK_OBJ_NONE + 1 : EVOK_OBJ_NONE;
+  if ((objective < first || objective >= EVOK_OBJ_COUNT) && !is_user(objective)) return EVOK_E_BADENUM;
+  if (push) {
+    if (push->sink.world < 1 || push->sink.world > EVOK_MAX_PEERS || push->sink.rank < 0 || push->sink.rank >= push->sink.world)
+      return EVOK_E_BADSIZE;
+  } else {
+    if (objective == EVOK_OBJ_NONE && !X) return EVOK_E_NULLPTR;
+    if (objective != EVOK_OBJ_NONE && !f) return EVOK_E_NULLPTR;
+  }
+  if (n_rows < 0 || D <= 0 || row0 < 0 || (X && ldx < D)) return EVOK_E_BADSIZE;
+  if (sym && ((n_rows & 1) || (row0 & 1))) return EVOK_E_ODDROWS;
+  return 0;
 }
 
-static int user_eval(int objective, const float* X, int64_t ldx, int64_t n_rows, int64_t D, float* f, cudaStream_t st) {
-  const UserDevice* d = nullptr;
-  const int rc = user_device(objective, &d);
-  if (rc != 0) return rc;
-  const bool vec = (D % 4 == 0) && aligned16(X) && (ldx % 4 == 0);
-  const int64_t ctas_needed = (n_rows + (kEvalThreads / 32) - 1) / (kEvalThreads / 32);
-  void* args[] = {&X, &ldx, &n_rows, &D, &f};
-  return user_launch(*d, EVOK_OBJ_KERNEL_EVAL + (vec ? 1 : 0), ctas_needed, args, st);
+// One launch of a sampler of family EVOK_OBJ_KERNEL_SAMPLE, _PUSH (push set) or _SQ (q set).
+static int sample(int objective, int family, float* X, int64_t ldx, const float* mu, const float* sigma, int64_t row0, int64_t n_rows,
+                  int64_t D, bool sym, uint64_t seed, uint64_t stream_id, const uint32_t* stream_off, float* f, float* q, PushArgs push,
+                  cudaStream_t st) {
+  KernelChoice c = choose_kernel(family, sym, X, ldx, mu, sigma, n_rows, D);
+  PhiloxKey key = make_philox_key(seed, stream_id);
+  void* args[] = {&X, &ldx, &mu, &sigma, &row0, &c.n_units, &D, &key, &stream_off, &f, &push.sink, &push.epoch, &push.done, &q};
+  return launch(objective, c, args, st);
 }
 
 }  // namespace evok
@@ -279,10 +282,10 @@ extern "C" EVOK_API int evok_objective_register(const void* cubin, size_t bytes,
   if (bytes == 0 || n_kernels != EVOK_OBJ_KERNELS) return EVOK_E_BADSIZE;
   for (int k = 0; k < n_kernels; ++k)
     if (!kernel_names_host[k]) return EVOK_E_NULLPTR;
-  std::lock_guard<std::mutex> lock(g_user_mutex);
+  std::lock_guard<std::mutex> lock(g_objective_mutex);
   const int n = g_user_count.load(std::memory_order_relaxed);
   if (n >= EVOK_OBJ_USER_CAPACITY) return EVOK_E_BADSIZE;
-  UserObjective* obj = new UserObjective;
+  Objective* obj = new Objective;
   obj->image.assign(static_cast<const char*>(cubin), static_cast<const char*>(cubin) + bytes);
   for (int k = 0; k < n_kernels; ++k) obj->names.emplace_back(kernel_names_host[k]);
   g_user[n] = obj;
@@ -293,99 +296,59 @@ extern "C" EVOK_API int evok_objective_register(const void* cubin, size_t bytes,
 
 extern "C" EVOK_API int evok_objective_load(int objective) {
   if (!is_user(objective)) return EVOK_E_BADENUM;
-  const UserDevice* d = nullptr;
-  return user_device(objective, &d);
+  const DeviceKernels* d = nullptr;
+  return device_kernels(objective, &d);
 }
 
 extern "C" EVOK_API int evok_sample_eval(int objective, float* X, int64_t ldx, const float* mu, const float* sigma, int64_t row0,
                                 int64_t n_rows, int64_t D, int symmetric, uint64_t seed, uint64_t stream_id,
                                 const uint32_t* stream_offset_dev, float* f, void* stream) {
-  const uint32_t* stream_off = stream_offset_dev;
-  if (!mu || !sigma) return EVOK_E_NULLPTR;
-  const bool user = is_user(objective);
-  if ((objective < 0 || objective >= EVOK_OBJ_COUNT) && !user) return EVOK_E_BADENUM;
-  if (objective == EVOK_OBJ_NONE && !X) return EVOK_E_NULLPTR;
-  if (objective != EVOK_OBJ_NONE && !f) return EVOK_E_NULLPTR;
-  if (n_rows < 0 || D <= 0 || row0 < 0 || (X && ldx < D)) return EVOK_E_BADSIZE;
-  if (symmetric && ((n_rows & 1) || (row0 & 1))) return EVOK_E_ODDROWS;
-  if (n_rows == 0) return 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (user) return user_sample(objective, X, ldx, mu, sigma, row0, n_rows, D, symmetric != 0, seed, stream_id, stream_off, f, st);
-  switch (objective) {
-    case EVOK_OBJ_NONE: return dispatch_sample<EVOK_OBJ_NONE>(X, ldx, mu, sigma, row0, n_rows, D, symmetric, seed, stream_id, stream_off, f, st);
-    case EVOK_OBJ_SPHERE: return dispatch_sample<EVOK_OBJ_SPHERE>(X, ldx, mu, sigma, row0, n_rows, D, symmetric, seed, stream_id, stream_off, f, st);
-    case EVOK_OBJ_RASTRIGIN: return dispatch_sample<EVOK_OBJ_RASTRIGIN>(X, ldx, mu, sigma, row0, n_rows, D, symmetric, seed, stream_id, stream_off, f, st);
-    case EVOK_OBJ_ACKLEY: return dispatch_sample<EVOK_OBJ_ACKLEY>(X, ldx, mu, sigma, row0, n_rows, D, symmetric, seed, stream_id, stream_off, f, st);
-  }
-  return EVOK_E_BADENUM;
+  const int rc = check_sample(objective, X, ldx, mu, sigma, row0, n_rows, D, symmetric != 0, f, nullptr);
+  if (rc != 0 || n_rows == 0) return rc;
+  return sample(objective, EVOK_OBJ_KERNEL_SAMPLE, X, ldx, mu, sigma, row0, n_rows, D, symmetric != 0, seed, stream_id, stream_offset_dev, f,
+                nullptr, PushArgs{}, (cudaStream_t)stream);
 }
 
 extern "C" EVOK_API int evok_sample_eval_sq(int objective, float* X, int64_t ldx, const float* mu, const float* sigma, int64_t row0, int64_t n_rows,
                                             int64_t D, uint64_t seed, uint64_t stream_id, const uint32_t* stream_offset_dev, float* f, float* q,
                                             void* stream) {
-  if (!mu || !sigma || !q) return EVOK_E_NULLPTR;
-  const bool user = is_user(objective);
-  if ((objective < 0 || objective >= EVOK_OBJ_COUNT) && !user) return EVOK_E_BADENUM;
-  if (objective == EVOK_OBJ_NONE && !X) return EVOK_E_NULLPTR;
-  if (objective != EVOK_OBJ_NONE && !f) return EVOK_E_NULLPTR;
-  if (n_rows < 0 || D <= 0 || row0 < 0 || (X && ldx < D)) return EVOK_E_BADSIZE;
-  if (n_rows == 0) return 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (user) return user_sample(objective, X, ldx, mu, sigma, row0, n_rows, D, false, seed, stream_id, stream_offset_dev, f, st, nullptr, q);
-  switch (objective) {
-    case EVOK_OBJ_NONE: return dispatch_sample_sq<EVOK_OBJ_NONE>(X, ldx, mu, sigma, row0, n_rows, D, seed, stream_id, stream_offset_dev, f, q, st);
-    case EVOK_OBJ_SPHERE: return dispatch_sample_sq<EVOK_OBJ_SPHERE>(X, ldx, mu, sigma, row0, n_rows, D, seed, stream_id, stream_offset_dev, f, q, st);
-    case EVOK_OBJ_RASTRIGIN: return dispatch_sample_sq<EVOK_OBJ_RASTRIGIN>(X, ldx, mu, sigma, row0, n_rows, D, seed, stream_id, stream_offset_dev, f, q, st);
-    case EVOK_OBJ_ACKLEY: return dispatch_sample_sq<EVOK_OBJ_ACKLEY>(X, ldx, mu, sigma, row0, n_rows, D, seed, stream_id, stream_offset_dev, f, q, st);
-  }
-  return EVOK_E_BADENUM;
+  if (!q) return EVOK_E_NULLPTR;
+  const int rc = check_sample(objective, X, ldx, mu, sigma, row0, n_rows, D, false, f, nullptr);
+  if (rc != 0 || n_rows == 0) return rc;
+  return sample(objective, EVOK_OBJ_KERNEL_SQ, X, ldx, mu, sigma, row0, n_rows, D, false, seed, stream_id, stream_offset_dev, f, q, PushArgs{},
+                (cudaStream_t)stream);
 }
 
 extern "C" EVOK_API int evok_sample_eval_push(int objective, float* X, int64_t ldx, const float* mu, const float* sigma, int64_t row0, int64_t n_rows,
                                               int64_t D, int symmetric, uint64_t seed, uint64_t stream_id, const uint32_t* stream_offset_dev,
                                               int world, int rank, void* const* peer_f, void* const* peer_flags, const uint64_t* epoch_dev,
                                               uint32_t* done_dev, void* stream) {
-  if (!mu || !sigma || !peer_f || !peer_flags || !epoch_dev || !done_dev) return EVOK_E_NULLPTR;
-  const bool user = is_user(objective);
-  if ((objective <= EVOK_OBJ_NONE || objective >= EVOK_OBJ_COUNT) && !user) return EVOK_E_BADENUM;
-  if (world < 1 || world > EVOK_MAX_PEERS || rank < 0 || rank >= world) return EVOK_E_BADSIZE;
-  if (n_rows < 0 || D <= 0 || row0 < 0 || (X && ldx < D)) return EVOK_E_BADSIZE;
-  if (symmetric && ((n_rows & 1) || (row0 & 1))) return EVOK_E_ODDROWS;
+  if (!peer_f || !peer_flags || !epoch_dev || !done_dev) return EVOK_E_NULLPTR;
   PushArgs push{};
   push.sink.world = world;
   push.sink.rank = rank;
+  push.epoch = reinterpret_cast<const unsigned long long*>(epoch_dev);
+  push.done = done_dev;
+  const int rc = check_sample(objective, X, ldx, mu, sigma, row0, n_rows, D, symmetric != 0, nullptr, &push);
+  if (rc != 0) return rc;
   for (int p = 0; p < world; ++p) {
     if (!peer_f[p] || !peer_flags[p]) return EVOK_E_NULLPTR;
     push.sink.data[p] = peer_f[p];
     push.sink.flags[p] = static_cast<unsigned long long*>(peer_flags[p]);
   }
-  push.epoch = reinterpret_cast<const unsigned long long*>(epoch_dev);
-  push.done = done_dev;
   // n_rows == 0 still launches one CTA: the peers wait for this rank's flag
-  cudaStream_t st = (cudaStream_t)stream;
-  if (user) return user_sample(objective, X, ldx, mu, sigma, row0, n_rows, D, symmetric != 0, seed, stream_id, stream_offset_dev, nullptr, st, &push);
-  switch (objective) {
-    case EVOK_OBJ_SPHERE: return dispatch_sample_push<EVOK_OBJ_SPHERE>(X, ldx, mu, sigma, row0, n_rows, D, symmetric, seed, stream_id, stream_offset_dev, push, st);
-    case EVOK_OBJ_RASTRIGIN: return dispatch_sample_push<EVOK_OBJ_RASTRIGIN>(X, ldx, mu, sigma, row0, n_rows, D, symmetric, seed, stream_id, stream_offset_dev, push, st);
-    case EVOK_OBJ_ACKLEY: return dispatch_sample_push<EVOK_OBJ_ACKLEY>(X, ldx, mu, sigma, row0, n_rows, D, symmetric, seed, stream_id, stream_offset_dev, push, st);
-  }
-  return EVOK_E_BADENUM;
+  return sample(objective, EVOK_OBJ_KERNEL_PUSH, X, ldx, mu, sigma, row0, n_rows, D, symmetric != 0, seed, stream_id, stream_offset_dev,
+                nullptr, nullptr, push, (cudaStream_t)stream);
 }
 
 extern "C" EVOK_API int evok_eval(int objective, const float* X, int64_t ldx, int64_t n_rows, int64_t D, float* f, void* stream) {
   if (!X || !f) return EVOK_E_NULLPTR;
-  const bool user = is_user(objective);
-  if ((objective <= EVOK_OBJ_NONE || objective >= EVOK_OBJ_COUNT) && !user) return EVOK_E_BADENUM;
+  if ((objective <= EVOK_OBJ_NONE || objective >= EVOK_OBJ_COUNT) && !is_user(objective)) return EVOK_E_BADENUM;
   if (n_rows < 0 || D <= 0 || ldx < D) return EVOK_E_BADSIZE;
   if (n_rows == 0) return 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (user) return user_eval(objective, X, ldx, n_rows, D, f, st);
-  switch (objective) {
-    case EVOK_OBJ_SPHERE: return launch_eval<EVOK_OBJ_SPHERE>(X, ldx, n_rows, D, f, st);
-    case EVOK_OBJ_RASTRIGIN: return launch_eval<EVOK_OBJ_RASTRIGIN>(X, ldx, n_rows, D, f, st);
-    case EVOK_OBJ_ACKLEY: return launch_eval<EVOK_OBJ_ACKLEY>(X, ldx, n_rows, D, f, st);
-  }
-  return EVOK_E_BADENUM;
+  const KernelChoice c = choose_kernel(EVOK_OBJ_KERNEL_EVAL, false, X, ldx, nullptr, nullptr, n_rows, D);
+  void* args[] = {&X, &ldx, &n_rows, &D, &f};
+  return launch(objective, c, args, (cudaStream_t)stream);
 }
 
 extern "C" EVOK_API int evok_sample_batched(float* X, int64_t item_stride_x, int64_t ldx, const float* mu, int64_t item_stride_mu, const float* sigma,
@@ -400,7 +363,10 @@ extern "C" EVOK_API int evok_sample_batched(float* X, int64_t item_stride_x, int
   const bool vec = (D % 4 == 0) && aligned16(mu) && aligned16(sigma) && aligned16(X) && ldx % 4 == 0 && item_stride_x % 4 == 0 &&
                    item_stride_mu % 4 == 0 && item_stride_sigma % 4 == 0;
   int64_t ctas = (n_units + (kSampleThreads / 32) - 1) / (kSampleThreads / 32);
-  const int64_t cap = ((int64_t)sm_count() * 8 + n_items - 1) / n_items;  // about 8 CTAs per SM over all items
+  const DeviceKernels* d = nullptr;
+  const int rc = device_kernels(EVOK_OBJ_NONE, &d);
+  if (rc != 0) return rc;
+  const int64_t cap = ((int64_t)d->sms * 8 + n_items - 1) / n_items;  // about 8 CTAs per SM over all items
   if (ctas > cap) ctas = cap < 1 ? 1 : cap;
   const PhiloxKey key = make_philox_key(seed, stream_id0);
   cudaStream_t st = (cudaStream_t)stream;

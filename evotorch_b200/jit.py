@@ -225,7 +225,8 @@ class ObjectiveSpec:
 
 # ------------------------------------------------------------------------------------------------ NVRTC
 def kernel_expressions() -> list:
-    """The 22 kernels of a registered objective, in the EVOK_OBJ_KERNEL_* order of include/evok.h."""
+    """The 22 kernels of a registered objective, in the EVOK_OBJ_KERNEL_* order of include/evok.h (kernel_index in
+    csrc/evok_sample_eval.cu computes the same positions)."""
     b = lambda v: "true" if v else "false"  # noqa: E731
     out = []
     for push in (False, True):  # EVOK_OBJ_KERNEL_SAMPLE, EVOK_OBJ_KERNEL_PUSH: + 4 sym + 2 store + vec

@@ -161,24 +161,38 @@ def _offset_ptr(stream_offset: Optional[torch.Tensor]) -> Optional[int]:
     return stream_offset.data_ptr()
 
 
-def sample_eval(objective: int, X: Optional[torch.Tensor], mu: torch.Tensor, sigma: torch.Tensor, *, n_rows: int, symmetric: bool,
-                seed: int, stream_id: int, row0: int = 0, f: Optional[torch.Tensor] = None,
-                stream_offset: Optional[torch.Tensor] = None) -> None:
+def _sampler_args(objective: int, X, mu, sigma, n_rows: int, *, f=None, q=None, symmetric=False, row0=0, peer=None) -> Optional[int]:
+    """The checks of `sample_eval`, `sample_eval_sq` (q) and `sample_eval_push` (peer) in their order, then `_load_objective`.
+    Returns X's leading dimension, or None with no rows to sample (the push always launches: the peers wait for this rank's flag)."""
     D = mu.numel()
     _vec(mu, "mu"); _vec(sigma, "sigma", D)
+    if q is not None:
+        _vec(q, "q", n_rows)
     ldx = _ldx(X, n_rows, D)
+    if peer is not None and row0 + n_rows > peer.popsize:
+        raise ValueError("rows beyond the population the peer exchange was sized for")
+    if q is not None and X is None and objective == OBJ_NONE:
+        raise ValueError("X: the samples must be written somewhere when no objective is fused into the sampler")
     if f is not None:
         _vec(f, "f", n_rows)
-    if objective != OBJ_NONE and f is None:
+    if peer is None and objective != OBJ_NONE and f is None:
         raise ValueError("f: a fitness buffer is required when an objective is fused into the sampler")
     if symmetric and (n_rows % 2 or row0 % 2):
         raise ValueError("symmetric sampling needs an even number of rows and an even first row")
-    if n_rows == 0:
-        return
+    if peer is None and n_rows == 0:
+        return None
     _load_objective(objective, mu)
+    return ldx
+
+
+def sample_eval(objective: int, X: Optional[torch.Tensor], mu: torch.Tensor, sigma: torch.Tensor, *, n_rows: int, symmetric: bool,
+                seed: int, stream_id: int, row0: int = 0, f: Optional[torch.Tensor] = None,
+                stream_offset: Optional[torch.Tensor] = None) -> None:
+    if (ldx := _sampler_args(objective, X, mu, sigma, n_rows, f=f, symmetric=symmetric, row0=row0)) is None:
+        return
     with _timed("sample_eval" if objective != OBJ_NONE else "sample"):
-        rc = nat.lib().evok_sample_eval(objective, nat.ptr(X), ldx, mu.data_ptr(), sigma.data_ptr(), row0, n_rows, D, int(symmetric),
-                                        seed, stream_id, _offset_ptr(stream_offset), nat.ptr(f), nat.stream_of(mu))
+        rc = nat.lib().evok_sample_eval(objective, nat.ptr(X), ldx, mu.data_ptr(), sigma.data_ptr(), row0, n_rows, mu.numel(),
+                                        int(symmetric), seed, stream_id, _offset_ptr(stream_offset), nat.ptr(f), nat.stream_of(mu))
     nat.check(rc, "evok_sample_eval")
 
 
@@ -186,14 +200,9 @@ def sample_eval_push(objective: int, X: Optional[torch.Tensor], mu: torch.Tensor
                      seed: int, stream_id: int, row0: int, peer, stream_offset: Optional[torch.Tensor] = None) -> None:
     """K1+K2 with the fitness all-gather fused in: row i's fitness lands in `f_all[row0 + i]` of every rank (`peer` is a
     evotorch_b200.peer.PeerExchange).  Follow with `peer.wait_fitness()` before reading `peer.f_all`."""
-    D = mu.numel()
-    _vec(mu, "mu"); _vec(sigma, "sigma", D)
-    ldx = _ldx(X, n_rows, D)
-    if row0 + n_rows > peer.popsize:
-        raise ValueError("rows beyond the population the peer exchange was sized for")
-    _load_objective(objective, mu)
+    ldx = _sampler_args(objective, X, mu, sigma, n_rows, row0=row0, peer=peer)
     with _timed("sample_eval"):
-        rc = nat.lib().evok_sample_eval_push(objective, nat.ptr(X), ldx, mu.data_ptr(), sigma.data_ptr(), row0, n_rows, D, int(symmetric),
+        rc = nat.lib().evok_sample_eval_push(objective, nat.ptr(X), ldx, mu.data_ptr(), sigma.data_ptr(), row0, n_rows, mu.numel(), int(symmetric),
                                              seed, stream_id, _offset_ptr(stream_offset), peer.world, peer.rank, peer.peer_f,
                                              peer.peer_flags_f, peer.epoch_f, peer._counter(0), nat.stream_of(mu))
     nat.check(rc, "evok_sample_eval_push")
@@ -300,20 +309,10 @@ def sample_eval_sq(objective: int, X: Optional[torch.Tensor], mu: torch.Tensor, 
                    stream_offset: Optional[torch.Tensor] = None) -> None:
     """`sample_eval` (non-symmetric) that also writes q[i] = ||z_i||^2 of the unscaled normals; X / f are the same bits as
     `sample_eval` with the same arguments.  X = None: lazy population (needs an objective with a fused kernel)."""
-    D = mu.numel()
-    _vec(mu, "mu"); _vec(sigma, "sigma", D); _vec(q, "q", n_rows)
-    ldx = _ldx(X, n_rows, D)
-    if X is None and objective == OBJ_NONE:
-        raise ValueError("X: the samples must be written somewhere when no objective is fused into the sampler")
-    if f is not None:
-        _vec(f, "f", n_rows)
-    if objective != OBJ_NONE and f is None:
-        raise ValueError("f: a fitness buffer is required when an objective is fused into the sampler")
-    if n_rows == 0:
+    if (ldx := _sampler_args(objective, X, mu, sigma, n_rows, f=f, q=q)) is None:
         return
-    _load_objective(objective, mu)
     with _timed("sepcma_sample"):
-        rc = nat.lib().evok_sample_eval_sq(objective, nat.ptr(X), ldx, mu.data_ptr(), sigma.data_ptr(), row0, n_rows, D, seed, stream_id,
+        rc = nat.lib().evok_sample_eval_sq(objective, nat.ptr(X), ldx, mu.data_ptr(), sigma.data_ptr(), row0, n_rows, mu.numel(), seed, stream_id,
                                            _offset_ptr(stream_offset), nat.ptr(f), q.data_ptr(), nat.stream_of(mu))
     nat.check(rc, "evok_sample_eval_sq")
 
