@@ -27,6 +27,16 @@ constexpr int kNumSMs = 132;  // H100 SXM
 // largest grid y / z: the batched entry points launch item chunks of at most this many items, one after another on the stream
 constexpr int64_t kMaxGridY = 65535;
 
+// fn(b0, nb) for the item chunks [b0, b0 + nb) of a batch, nb <= max_items, in order; returns the first non-zero code of fn
+template <typename Fn>
+inline int for_item_chunks(int64_t n_items, int64_t max_items, Fn&& fn) {
+  for (int64_t b0 = 0; b0 < n_items; b0 += max_items) {
+    const int rc = fn(b0, n_items - b0 < max_items ? n_items - b0 : max_items);
+    if (rc) return rc;
+  }
+  return 0;
+}
+
 inline PhiloxKey make_philox_key(uint64_t seed, uint64_t stream_id) {
   PhiloxKey k;
   uint32_t a = (uint32_t)seed, b = (uint32_t)(seed >> 32) ^ (uint32_t)(stream_id >> 32);

@@ -792,8 +792,7 @@ extern "C" EVOK_API int evok_grad_batched(int form, const float* X, int64_t item
   const int64_t chunk = n_items < kMaxGridY ? n_items : kMaxGridY;
   if (ws_bytes < (size_t)chunk * items.partial * sizeof(float)) return EVOK_E_WORKSPACE;
   float* partial = (float*)ws;
-  for (int64_t b0 = 0; b0 < n_items; b0 += kMaxGridY) {
-    const int64_t nb = n_items - b0 < kMaxGridY ? n_items - b0 : kMaxGridY;
+  return for_item_chunks(n_items, kMaxGridY, [&](int64_t b0, int64_t nb) {
     const float* Xc = X + b0 * item_stride_x;
     const float* wc = w + b0 * n_rows;
     const float* muc = mu + b0 * item_stride_mu;
@@ -809,6 +808,6 @@ extern "C" EVOK_API int evok_grad_batched(int form, const float* X, int64_t item
     grad_finalize_kernel<<<dim3((unsigned)((D + 255) / 256), (unsigned)nb), 256, 0, st>>>(partial, p.n_chunks, D, scale_mu, scale_sigma,
                                                                                           out_mu + b0 * D, out_sigma + b0 * D, items.partial);
     EVOK_CHECK_LAUNCH();
-  }
-  return 0;
+    return 0;
+  });
 }

@@ -1,9 +1,7 @@
 // K3: fitness -> utilities.  A hand-written stable LSD radix sort of (orderable fp32 key, index) pairs
 // (4 passes x 8 bits; per pass: per-tile digit histogram -> per-digit exclusive scan -> stable scatter using
-// warp match/ballot ranking), followed by a fused utility-table scatter.  N is the population size
+// warp match/ballot ranking), followed by one scatter of what each sorted position writes (emit_at).  N is the population size
 // (<= a few million): the whole working set lives in L2, the kernels are latency-, not bandwidth-bound.
-#include <cstdlib>
-
 #include "evok_common.cuh"
 
 namespace evok {
@@ -23,12 +21,17 @@ __device__ __forceinline__ uint32_t orderable(float v) {
   return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
 
+// the sort key of fitness f: descending + stable == ascending on the complemented key
+__device__ __forceinline__ uint32_t sort_key(float f, int descending) {
+  const uint32_t k = orderable(f);
+  return descending ? ~k : k;
+}
+
 __global__ void __launch_bounds__(256) make_keys_kernel(const float* __restrict__ f, int64_t N, int descending,
                                                         uint32_t* __restrict__ keys, uint32_t* __restrict__ idx) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < N) {
-    const uint32_t k = orderable(f[i]);
-    keys[i] = descending ? ~k : k;  // descending + stable == ascending on the complemented key
+    keys[i] = sort_key(f[i], descending);
     idx[i] = (uint32_t)i;
   }
 }
@@ -69,8 +72,7 @@ __global__ void __launch_bounds__(kSortThreads)
     if (i < N) {
       uint32_t k;
       if (FIRST) {
-        k = orderable(f[i]);
-        if (descending) k = ~k;
+        k = sort_key(f[i], descending);
         keys[i] = k;
         idx[i] = (uint32_t)i;
       } else {
@@ -211,49 +213,70 @@ __global__ void __launch_bounds__(kSortThreads)
   }
 }
 
-// ---- utility tables -------------------------------------------------------------------------------
-// sum over p of max(0, ln(N/2+1) - ln(N-p)) (fp32 terms, double accumulation); single CTA.
+// ---- what a sorted position writes -----------------------------------------------------------------
+// NES utility of sorted position p (0 = worst) of N before normalisation: max(0, top - ln(N-p)), Nf = N, top = ln(N/2+1)
+__device__ __forceinline__ float nes_term(int64_t p, float Nf, float top) { return fmaxf(0.0f, top - logf(Nf - (float)p)); }
+
+// this thread's share of the NES table sum: positions first, first + stride, ... (fp32 terms, double accumulation in that order)
+__device__ __forceinline__ double nes_partial_sum(int64_t N, int64_t first, int stride) {
+  const float Nf = (float)N, top = logf(Nf / 2.0f + 1.0f);
+  double acc = 0.0;
+  for (int64_t p = first; p < N; p += stride) acc += (double)nes_term(p, Nf, top);
+  return acc;
+}
+
+// utility of sorted position p of N; *nes_sum (the table sum) is read for NES only
+__device__ __forceinline__ float utility_at(int64_t p, int64_t N, int method, const float* nes_sum) {
+  if (method == EVOK_RANK_CENTERED) return __fdiv_rn((float)p, (float)(N - 1)) - 0.5f;
+  if (method == EVOK_RANK_LINEAR) return __fdiv_rn((float)p, (float)(N - 1));
+  const float Nf = (float)N;
+  return __fdiv_rn(nes_term(p, Nf, logf(Nf / 2.0f + 1.0f)), *nes_sum) - __fdiv_rn(1.0f, Nf);
+}
+
+enum { kUtilities = 0, kArgsort = 1, kEliteMask = 2, kTable = 3 };
+
+// The outputs of a ranking, [items][N] like its keys; the table is shared by the items.
+struct Emit {
+  int mode;            // kUtilities / kArgsort / kEliteMask / kTable
+  int method;          // kUtilities: the ranking method
+  int64_t num_elites;  // kEliteMask
+  float* out;          // utility / elite flag / table entry, in the solution's slot (unused by kArgsort)
+  int64_t* perm;       // nullable: the solution at each sorted position
+  const float* table;  // kTable: the value of each sorted position (CMA-ES: weight of a solution = weights[its rank], cmaes.py:445-451)
+  __host__ __device__ Emit item(int64_t off) const {
+    Emit e = *this;
+    if (out) e.out += off;
+    if (perm) e.perm += off;
+    return e;
+  }
+};
+
+// the four kinds of output (out / perm [items][N]; perm may be null for utilities)
+static Emit utilities(int method, float* w, int64_t* perm) { return Emit{kUtilities, method, 0, w, perm, nullptr}; }
+static Emit permutation(int64_t* perm) { return Emit{kArgsort, 0, 0, nullptr, perm, nullptr}; }
+static Emit elite_flags(int64_t num_elites, float* mask) { return Emit{kEliteMask, 0, num_elites, mask, nullptr, nullptr}; }
+static Emit table_entries(const float* table, float* out) { return Emit{kTable, 0, 0, out, nullptr, table}; }
+
+// solution i sits at sorted position p (0 = first in the stable order): write what `mode` asks for
+__device__ __forceinline__ void emit_at(int64_t p, uint32_t i, int64_t N, const Emit& e, const float* nes_sum) {
+  if (e.perm) e.perm[p] = (int64_t)i;
+  if (e.mode == kUtilities) e.out[i] = utility_at(p, N, e.method, nes_sum);
+  else if (e.mode == kEliteMask) e.out[i] = p < e.num_elites ? 1.0f : 0.0f;
+  else if (e.mode == kTable) e.out[i] = e.table[p];
+}
+
+// the NES table sum of N positions; single CTA
 __global__ void __launch_bounds__(1024) nes_table_sum_kernel(int64_t N, float* __restrict__ out_sum) {
   __shared__ double sm[33];
-  const float Nf = (float)N;
-  const float top = logf(Nf / 2.0f + 1.0f);
-  double acc = 0.0;
-  for (int64_t p = threadIdx.x; p < N; p += 1024) acc += (double)fmaxf(0.0f, top - logf(Nf - (float)p));
-  const double tot = block_sum<double>(acc, sm);
+  const double tot = block_sum<double>(nes_partial_sum(N, threadIdx.x, 1024), sm);
   if (threadIdx.x == 0) *out_sum = (float)tot;
 }
 
-// position p in sorted order (worst first) -> utility, scattered to the solution's slot
-__global__ void __launch_bounds__(256) scatter_utilities_kernel(const uint32_t* __restrict__ idx, int64_t N, int method,
-                                                                const float* __restrict__ nes_sum, float* __restrict__ w,
-                                                                int64_t* __restrict__ perm) {
+// after the radix sort: emit_at for every position p of the sorted index array
+__global__ void __launch_bounds__(256) scatter_sorted_kernel(const uint32_t* __restrict__ idx, int64_t N, const Emit e,
+                                                             const float* __restrict__ nes_sum) {
   const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= N) return;
-  const uint32_t i = idx[p];
-  float u;
-  if (method == EVOK_RANK_CENTERED) {
-    u = __fdiv_rn((float)p, (float)(N - 1)) - 0.5f;
-  } else if (method == EVOK_RANK_LINEAR) {
-    u = __fdiv_rn((float)p, (float)(N - 1));
-  } else {  // NES
-    const float Nf = (float)N;
-    const float t = fmaxf(0.0f, logf(Nf / 2.0f + 1.0f) - logf(Nf - (float)p));
-    u = __fdiv_rn(t, *nes_sum) - __fdiv_rn(1.0f, Nf);
-  }
-  w[i] = u;
-  if (perm) perm[p] = (int64_t)i;
-}
-
-// out[solution at sorted position p] = table[p]   (CMA-ES: weight of a solution = weights[its rank], cmaes.py:445-451)
-__global__ void __launch_bounds__(256) scatter_table_kernel(const uint32_t* __restrict__ idx, int64_t N, const float* __restrict__ table,
-                                                            float* __restrict__ out) {
-  const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (p < N) out[idx[p]] = table[p];
-}
-
-__global__ void __launch_bounds__(256) write_perm_kernel(const uint32_t* __restrict__ idx, int64_t N, int64_t* __restrict__ perm) {
-  const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (p < N) perm[p] = (int64_t)idx[p];
+  if (p < N) emit_at(p, idx[p], N, e, nes_sum);
 }
 
 // normalized / raw: no sort.  stats[0] = mean, stats[1] = unbiased std of g = +-f (double accumulation).
@@ -302,12 +325,6 @@ __global__ void __launch_bounds__(1024) weights_adjust_kernel(float* __restrict_
   }
 }
 
-__global__ void __launch_bounds__(256) elite_mask_kernel(const uint32_t* __restrict__ idx, int64_t N, int64_t num_elites,
-                                                         float* __restrict__ mask) {
-  const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (p < N) mask[idx[p]] = p < num_elites ? 1.0f : 0.0f;
-}
-
 // ---- small populations: rank by counting, ONE launch -------------------------------------------------
 // For N <= kSmallRankMax the 14-launch radix pipeline is pure launch latency (even inside a CUDA graph), while the stable rank of element i is simply  #{j : key_j < key_i} + #{j < i : key_j == key_i}.  All N^2 comparisons
 // (67 M at N = 8192) spread over the whole GPU take a few microseconds: 4 lanes share one element (interleaved quarters of
@@ -318,39 +335,23 @@ constexpr int kSmallRankMax = 8192;
 constexpr int kSmallThreads = 256;
 constexpr int kSmallTile = 2048;
 
-enum { kSmallUtilities = 0, kSmallArgsort = 1, kSmallEliteMask = 2, kSmallTable = 3 };
-
 template <int PARTS>
-__global__ void __launch_bounds__(kSmallThreads)
-    rank_small_kernel(const float* __restrict__ f, int N, int descending, int mode, int method, int64_t num_elites, float* __restrict__ out,
-                      int64_t* __restrict__ perm, const float* __restrict__ table = nullptr) {
+__global__ void __launch_bounds__(kSmallThreads) rank_small_kernel(const float* __restrict__ f, int N, int descending, Emit e) {
   __shared__ uint32_t tile[kSmallTile];
   __shared__ double red[33];
   constexpr int kElems = kSmallThreads / PARTS;
-  {  // batched searches: blockIdx.y = batch item, every item ranks its own N fitnesses (the table, if any, is shared)
-    const int64_t item_off = (int64_t)blockIdx.y * N;
-    f += item_off;
-    if (out) out += item_off;
-    if (perm) perm += item_off;
-  }
+  // batched searches: blockIdx.y = batch item, every item ranks its own N fitnesses
+  f += (int64_t)blockIdx.y * N;
+  e = e.item((int64_t)blockIdx.y * N);
   const int part = threadIdx.x % PARTS;
   const int i = blockIdx.x * kElems + threadIdx.x / PARTS;
-  uint32_t ki = 0;
-  if (i < N) {
-    ki = orderable(f[i]);
-    if (descending) ki = ~ki;
-  }
+  const uint32_t ki = i < N ? sort_key(f[i], descending) : 0u;
   uint32_t cnt = 0;
   for (int base = 0; base < N; base += kSmallTile) {
     __syncthreads();
     for (int t = threadIdx.x; t < kSmallTile; t += kSmallThreads) {
       const int j = base + t;
-      uint32_t k = 0xFFFFFFFFu;  // padding: never below a real key, and never "equal with a lower index"
-      if (j < N) {
-        k = orderable(f[j]);
-        if (descending) k = ~k;
-      }
-      tile[t] = k;
+      tile[t] = j < N ? sort_key(f[j], descending) : 0xFFFFFFFFu;  // padding: never below a real key, never "equal with a lower index"
     }
     __syncthreads();
     const int lim = min(kSmallTile, N - base);
@@ -364,54 +365,23 @@ __global__ void __launch_bounds__(kSmallThreads)
   for (int o = 1; o < PARTS; o <<= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
 
   float nes_sum = 0.0f;
-  if (mode == kSmallUtilities && method == EVOK_RANK_NES) {  // the table sum of nes_table_sum_kernel, once per CTA
-    const float Nf = (float)N, top = logf(Nf / 2.0f + 1.0f);
-    double acc = 0.0;
-    for (int p = threadIdx.x; p < N; p += kSmallThreads) acc += (double)fmaxf(0.0f, top - logf(Nf - (float)p));
-    nes_sum = (float)block_sum<double>(acc, red);
-  }
-  if (i >= N || part != 0) return;
-  const uint32_t p = cnt;  // position in sorted order
-  if (perm) perm[p] = (int64_t)i;
-  if (mode == kSmallUtilities) {
-    float u;
-    if (method == EVOK_RANK_CENTERED) {
-      u = __fdiv_rn((float)p, (float)(N - 1)) - 0.5f;
-    } else if (method == EVOK_RANK_LINEAR) {
-      u = __fdiv_rn((float)p, (float)(N - 1));
-    } else {
-      const float Nf = (float)N;
-      const float t = fmaxf(0.0f, logf(Nf / 2.0f + 1.0f) - logf(Nf - (float)p));
-      u = __fdiv_rn(t, nes_sum) - __fdiv_rn(1.0f, Nf);
-    }
-    out[i] = u;
-  } else if (mode == kSmallEliteMask) {
-    out[i] = (int64_t)p < num_elites ? 1.0f : 0.0f;
-  } else if (mode == kSmallTable) {
-    out[i] = table[p];
-  }
+  if (e.mode == kUtilities && e.method == EVOK_RANK_NES)  // the table sum of nes_table_sum_kernel, once per CTA
+    nes_sum = (float)block_sum<double>(nes_partial_sum(N, threadIdx.x, kSmallThreads), red);
+  if (i < N && part == 0) emit_at(cnt, (uint32_t)i, N, e, &nes_sum);  // cnt: position in sorted order
 }
 
-static int rank_small(const float* f, int64_t N, int descending, int mode, int method, int64_t num_elites, float* out, int64_t* perm, cudaStream_t st,
-                      const float* table = nullptr, int64_t n_items = 1) {
+// one launch for n_items rows of N <= kSmallRankMax keys
+static int rank_small(const float* f, int64_t N, int64_t n_items, int descending, const Emit& e, cudaStream_t st) {
   // lanes per element grow with N: the work per thread stays <= 512 comparisons and the grid >= N / 64 CTAs
   if (N <= 1024) {
-    rank_small_kernel<4><<<dim3((unsigned)((N + 63) / 64), (unsigned)n_items), kSmallThreads, 0, st>>>(f, (int)N, descending, mode, method, num_elites, out, perm, table);
+    rank_small_kernel<4><<<dim3((unsigned)((N + 63) / 64), (unsigned)n_items), kSmallThreads, 0, st>>>(f, (int)N, descending, e);
   } else if (N <= 4096) {
-    rank_small_kernel<8><<<dim3((unsigned)((N + 31) / 32), (unsigned)n_items), kSmallThreads, 0, st>>>(f, (int)N, descending, mode, method, num_elites, out, perm, table);
+    rank_small_kernel<8><<<dim3((unsigned)((N + 31) / 32), (unsigned)n_items), kSmallThreads, 0, st>>>(f, (int)N, descending, e);
   } else {
-    rank_small_kernel<16><<<dim3((unsigned)((N + 15) / 16), (unsigned)n_items), kSmallThreads, 0, st>>>(f, (int)N, descending, mode, method, num_elites, out, perm, table);
+    rank_small_kernel<16><<<dim3((unsigned)((N + 15) / 16), (unsigned)n_items), kSmallThreads, 0, st>>>(f, (int)N, descending, e);
   }
   EVOK_CHECK_LAUNCH();
   return 0;
-}
-
-static bool use_small_rank(int64_t N) {
-  static const int enabled = [] {
-    const char* e = getenv("EVOK_RANK_SMALL");
-    return e ? atoi(e) : 1;
-  }();
-  return enabled && N <= kSmallRankMax;
 }
 
 // ---- host side ------------------------------------------------------------------------------------
@@ -441,7 +411,7 @@ static SortPlan make_plan(int64_t N) {
 
 // sorts; returns the device pointer (inside ws) of the sorted index array (and of the sorted keys).
 // Up to kSelfScanMaxTiles tiles (512 k keys) the 13-launch pipeline (make_keys + 4 x (hist, scan, scatter)) shrinks to 8
-// (4 x (hist [+ keys], self-scanning scatter)); EVOK_RANK_SELF_SCAN=0 forces the 3-kernel passes.
+// (4 x (hist [+ keys], self-scanning scatter)).
 static int sort_pairs(const float* f, int64_t N, int descending, void* ws, const SortPlan& p, cudaStream_t st, uint32_t** sorted_idx,
                       uint32_t** sorted_keys = nullptr) {
   char* base = (char*)ws;
@@ -449,38 +419,67 @@ static int sort_pairs(const float* f, int64_t N, int descending, void* ws, const
   uint32_t* idx[2] = {(uint32_t*)(base + p.off_idx0), (uint32_t*)(base + p.off_idx1)};
   uint32_t* counts = (uint32_t*)(base + p.off_counts);
   uint32_t* totals = (uint32_t*)(base + p.off_totals);
-  static const int self_scan = [] {
-    const char* e = getenv("EVOK_RANK_SELF_SCAN");
-    return e ? atoi(e) : 1;
-  }();
-  if (self_scan && p.n_tiles <= kSelfScanMaxTiles) {
-    int cur = 0;
-    for (int pass = 0; pass < 32 / kRadixBits; ++pass) {
-      const int shift = pass * kRadixBits;
+  const bool self_scan = p.n_tiles <= kSelfScanMaxTiles;
+  if (!self_scan) {
+    make_keys_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(f, N, descending, keys[0], idx[0]);
+    EVOK_CHECK_LAUNCH();
+  }
+  int cur = 0;
+  for (int pass = 0; pass < 32 / kRadixBits; ++pass) {
+    const int shift = pass * kRadixBits;
+    if (self_scan) {
       if (pass == 0) radix_hist_t_kernel<true><<<p.n_tiles, kSortThreads, 0, st>>>(f, descending, keys[0], idx[0], N, shift, counts);
       else radix_hist_t_kernel<false><<<p.n_tiles, kSortThreads, 0, st>>>(nullptr, 0, keys[cur], nullptr, N, shift, counts);
       radix_scatter_kernel<true><<<p.n_tiles, kSortThreads, 0, st>>>(keys[cur], idx[cur], keys[cur ^ 1], idx[cur ^ 1], N, shift, counts, p.n_tiles, totals);
       EVOK_CHECK_LAUNCH_N(2);
-      cur ^= 1;
+    } else {
+      radix_hist_kernel<<<p.n_tiles, kSortThreads, 0, st>>>(keys[cur], N, shift, counts, p.n_tiles);
+      digit_scan_kernel<<<kRadix, 256, 0, st>>>(counts, p.n_tiles, totals);
+      radix_scatter_kernel<false><<<p.n_tiles, kSortThreads, 0, st>>>(keys[cur], idx[cur], keys[cur ^ 1], idx[cur ^ 1], N, shift, counts, p.n_tiles, totals);
+      EVOK_CHECK_LAUNCH_N(3);
     }
-    *sorted_idx = idx[cur];
-    if (sorted_keys) *sorted_keys = keys[cur];
-    return 0;
-  }
-  make_keys_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(f, N, descending, keys[0], idx[0]);
-  EVOK_CHECK_LAUNCH();
-  int cur = 0;
-  for (int pass = 0; pass < 32 / kRadixBits; ++pass) {
-    const int shift = pass * kRadixBits;
-    radix_hist_kernel<<<p.n_tiles, kSortThreads, 0, st>>>(keys[cur], N, shift, counts, p.n_tiles);
-    digit_scan_kernel<<<kRadix, 256, 0, st>>>(counts, p.n_tiles, totals);
-    radix_scatter_kernel<false><<<p.n_tiles, kSortThreads, 0, st>>>(keys[cur], idx[cur], keys[cur ^ 1], idx[cur ^ 1], N, shift, counts, p.n_tiles, totals);
-    EVOK_CHECK_LAUNCH_N(3);
     cur ^= 1;
   }
   *sorted_idx = idx[cur];
   if (sorted_keys) *sorted_keys = keys[cur];
   return 0;
+}
+
+// n_items rankings of N keys each ([items][N], like the outputs of e): for N <= kSmallRankMax the counting rank, one launch per item
+// chunk; above, per item on the one workspace, the radix sort, the NES table sum if the utilities need it, and the scatter.  The
+// single-search entry points check the workspace for every N; the batched ones need it, and check it, for the sort only.
+static int rank_rows(const float* keys, int64_t N, int64_t n_items, int descending, const Emit& e, void* ws, size_t ws_bytes,
+                     cudaStream_t st) {
+  if (N <= kSmallRankMax)
+    return for_item_chunks(n_items, kMaxGridY, [&](int64_t b0, int64_t nb) {
+      return rank_small(keys + b0 * N, N, nb, descending, e.item(b0 * N), st);
+    });
+  const SortPlan p = make_plan(N);
+  if (ws_bytes < p.total) return EVOK_E_WORKSPACE;
+  float* nes_sum = (float*)((char*)ws + p.off_scalar);
+  const bool nes = e.mode == kUtilities && e.method == EVOK_RANK_NES;
+  for (int64_t b = 0; b < n_items; ++b) {
+    uint32_t* sidx = nullptr;
+    const int rc = sort_pairs(keys + b * N, N, descending, ws, p, st, &sidx);
+    if (rc) return rc;
+    if (nes) nes_table_sum_kernel<<<1, 1024, 0, st>>>(N, nes_sum);
+    scatter_sorted_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(sidx, N, e.item(b * N), nes_sum);
+    EVOK_CHECK_LAUNCH_N(nes ? 2 : 1);
+  }
+  return 0;
+}
+
+// normalized / raw (no sort) for n_items rows of N: stats holds (mean, std) of +-f for each item of a chunk
+static int affine_rows(int method, const float* f, int64_t N, int64_t n_items, int higher_is_better, float* w, float* stats, cudaStream_t st) {
+  const float sign = higher_is_better ? 1.0f : -1.0f;
+  const int normalized = method == EVOK_RANK_NORMALIZED;
+  return for_item_chunks(n_items, kMaxGridY, [&](int64_t b0, int64_t nb) {
+    const float* fc = f + b0 * N;
+    if (normalized) mean_std_kernel<<<(unsigned)nb, 1024, 0, st>>>(fc, N, sign, stats);
+    affine_kernel<<<dim3((unsigned)((N + 255) / 256), (unsigned)nb), 256, 0, st>>>(fc, N, sign, stats, normalized, w + b0 * N);
+    EVOK_CHECK_LAUNCH_N(normalized ? 2 : 1);
+    return 0;
+  });
 }
 
 // ---- sharded ranking over peer memory ----------------------------------------------------------------
@@ -578,17 +577,7 @@ __global__ void __launch_bounds__(256)
 #pragma unroll
     for (int s = 0; s < EVOK_MAX_PEERS; ++s)
       if (s < world && s != rank) pos += lo[s];
-    float u;
-    if (method == EVOK_RANK_CENTERED) {
-      u = __fdiv_rn((float)pos, (float)(N - 1)) - 0.5f;
-    } else if (method == EVOK_RANK_LINEAR) {
-      u = __fdiv_rn((float)pos, (float)(N - 1));
-    } else {
-      const float Nf = (float)N;
-      const float t = fmaxf(0.0f, logf(Nf / 2.0f + 1.0f) - logf(Nf - (float)pos));
-      u = __fdiv_rn(t, *nes_sum) - __fdiv_rn(1.0f, Nf);
-    }
-    w_local[sorted_idx[p]] = u;
+    w_local[sorted_idx[p]] = utility_at(pos, N, method, nes_sum);
   }
   if (blockIdx.x == 0 && threadIdx.x == 0 && mean_out) {
     double tot = 0.0;
@@ -623,73 +612,30 @@ extern "C" EVOK_API int evok_rank(int method, const float* f, int64_t N, int hig
   const SortPlan p = make_plan(N);
   if (ws_bytes < p.total) return EVOK_E_WORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
-  float* scalar = (float*)((char*)ws + p.off_scalar);
-  const unsigned nb = (unsigned)((N + 255) / 256);
   if (method == EVOK_RANK_NORMALIZED || method == EVOK_RANK_RAW) {
-    const float sign = higher_is_better ? 1.0f : -1.0f;
-    if (method == EVOK_RANK_NORMALIZED) mean_std_kernel<<<1, 1024, 0, st>>>(f, N, sign, scalar);
-    affine_kernel<<<nb, 256, 0, st>>>(f, N, sign, scalar, method == EVOK_RANK_NORMALIZED, w);
-    EVOK_CHECK_LAUNCH_N(method == EVOK_RANK_NORMALIZED ? 2 : 1);
-    if (perm && use_small_rank(N)) return rank_small(f, N, !higher_is_better, kSmallArgsort, 0, 0, nullptr, perm, st);
-    if (perm) {
-      uint32_t* sidx = nullptr;
-      int rc = sort_pairs(f, N, !higher_is_better, ws, p, st, &sidx);
-      if (rc) return rc;
-      write_perm_kernel<<<nb, 256, 0, st>>>(sidx, N, perm);
-      EVOK_CHECK_LAUNCH();
-    }
-    return 0;
+    const int rc = affine_rows(method, f, N, 1, higher_is_better, w, (float*)((char*)ws + p.off_scalar), st);
+    if (rc || !perm) return rc;
+    return rank_rows(f, N, 1, !higher_is_better, permutation(perm), ws, ws_bytes, st);
   }
-  if (use_small_rank(N)) return rank_small(f, N, !higher_is_better, kSmallUtilities, method, 0, w, perm, st);
-  uint32_t* sidx = nullptr;
-  int rc = sort_pairs(f, N, !higher_is_better, ws, p, st, &sidx);
-  if (rc) return rc;
-  if (method == EVOK_RANK_NES) nes_table_sum_kernel<<<1, 1024, 0, st>>>(N, scalar);
-  scatter_utilities_kernel<<<nb, 256, 0, st>>>(sidx, N, method, scalar, w, perm);
-  EVOK_CHECK_LAUNCH_N(method == EVOK_RANK_NES ? 2 : 1);
-  return 0;
+  return rank_rows(f, N, 1, !higher_is_better, utilities(method, w, perm), ws, ws_bytes, st);
 }
 
 extern "C" EVOK_API int evok_argsort(const float* keys, int64_t N, int descending, int64_t* perm, void* ws, size_t ws_bytes, void* stream) {
   if (!keys || !perm || !ws) return EVOK_E_NULLPTR;
   if (N < 0 || N >= (int64_t)1 << 32) return EVOK_E_BADSIZE;
   if (N == 0) return 0;
-  const SortPlan p = make_plan(N);
-  if (ws_bytes < p.total) return EVOK_E_WORKSPACE;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (use_small_rank(N)) return rank_small(keys, N, descending, kSmallArgsort, 0, 0, nullptr, perm, st);
-  uint32_t* sidx = nullptr;
-  int rc = sort_pairs(keys, N, descending, ws, p, st, &sidx);
-  if (rc) return rc;
-  write_perm_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(sidx, N, perm);
-  EVOK_CHECK_LAUNCH();
-  return 0;
+  if (ws_bytes < make_plan(N).total) return EVOK_E_WORKSPACE;
+  return rank_rows(keys, N, 1, descending, permutation(perm), ws, ws_bytes, (cudaStream_t)stream);
 }
 
-extern "C" EVOK_API int evok_weights_adjust(float* w, int64_t N, int mode, void* stream) {
-  if (!w) return EVOK_E_NULLPTR;
-  if (mode != 1 && mode != 2) return EVOK_E_BADENUM;
-  if (N < 0) return EVOK_E_BADSIZE;
-  if (N == 0) return 0;
-  weights_adjust_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(w, N, mode);
-  EVOK_CHECK_LAUNCH();
-  return 0;
-}
+extern "C" EVOK_API int evok_weights_adjust(float* w, int64_t N, int mode, void* stream) { return evok_weights_adjust_batched(w, N, 1, mode, stream); }
 
 extern "C" EVOK_API int evok_elite_mask(const float* w, int64_t N, int64_t num_elites, float* mask, void* ws, size_t ws_bytes, void* stream) {
   if (!w || !mask || !ws) return EVOK_E_NULLPTR;
   if (N < 0 || N >= (int64_t)1 << 32 || num_elites < 0 || num_elites > N) return EVOK_E_BADSIZE;
   if (N == 0) return 0;
-  const SortPlan p = make_plan(N);
-  if (ws_bytes < p.total) return EVOK_E_WORKSPACE;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (use_small_rank(N)) return rank_small(w, N, /*descending=*/1, kSmallEliteMask, 0, num_elites, mask, nullptr, st);
-  uint32_t* sidx = nullptr;
-  int rc = sort_pairs(w, N, /*descending=*/1, ws, p, st, &sidx);
-  if (rc) return rc;
-  elite_mask_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(sidx, N, num_elites, mask);
-  EVOK_CHECK_LAUNCH();
-  return 0;
+  if (ws_bytes < make_plan(N).total) return EVOK_E_WORKSPACE;
+  return rank_rows(w, N, 1, /*descending=*/1, elite_flags(num_elites, mask), ws, ws_bytes, (cudaStream_t)stream);
 }
 
 extern "C" EVOK_API int evok_rank_sharded(int method, const float* f_local, int64_t N, int higher_is_better, int world, int rank,
@@ -748,22 +694,12 @@ extern "C" EVOK_API int evok_rank_table(const float* keys, int64_t N, int descen
   if (!keys || !table || !out || !ws) return EVOK_E_NULLPTR;
   if (N < 0 || N >= (int64_t)1 << 32) return EVOK_E_BADSIZE;
   if (N == 0) return 0;
-  const SortPlan p = make_plan(N);
-  if (ws_bytes < p.total) return EVOK_E_WORKSPACE;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (use_small_rank(N)) return rank_small(keys, N, descending, kSmallTable, 0, 0, out, nullptr, st, table);
-  uint32_t* sidx = nullptr;
-  int rc = sort_pairs(keys, N, descending, ws, p, st, &sidx);
-  if (rc) return rc;
-  scatter_table_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(sidx, N, table, out);
-  EVOK_CHECK_LAUNCH();
-  return 0;
+  if (ws_bytes < make_plan(N).total) return EVOK_E_WORKSPACE;
+  return rank_rows(keys, N, 1, descending, table_entries(table, out), ws, ws_bytes, (cudaStream_t)stream);
 }
 
 // ---- batched searches (functional API with leading batch dimensions): n_items independent rankings of N fitnesses each, f and w
-// contiguous [n_items][N].  N <= 8192: ONE launch for all items (the counting rank with blockIdx.y = item); larger N: the radix
-// pipeline item by item on the same workspace.  Batches above kMaxGridY items run as item chunks of at most kMaxGridY, in order on
-// the stream, so the chunks reuse the workspace.
+// contiguous [n_items][N], through the same path as the single searches (see rank_rows).
 extern "C" EVOK_API int evok_rank_batched(int method, const float* f, int64_t N, int64_t n_items, int higher_is_better, float* w, void* ws,
                                           size_t ws_bytes, void* stream) {
   if (!f || !w || !ws) return EVOK_E_NULLPTR;
@@ -774,30 +710,9 @@ extern "C" EVOK_API int evok_rank_batched(int method, const float* f, int64_t N,
   if (method == EVOK_RANK_NORMALIZED || method == EVOK_RANK_RAW) {
     const int64_t chunk = n_items < kMaxGridY ? n_items : kMaxGridY;
     if (ws_bytes < (size_t)chunk * 8 + 256) return EVOK_E_WORKSPACE;
-    float* stats = (float*)ws;
-    const float sign = higher_is_better ? 1.0f : -1.0f;
-    for (int64_t b0 = 0; b0 < n_items; b0 += kMaxGridY) {
-      const int64_t nb = n_items - b0 < kMaxGridY ? n_items - b0 : kMaxGridY;
-      const float* fc = f + b0 * N;
-      if (method == EVOK_RANK_NORMALIZED) mean_std_kernel<<<(unsigned)nb, 1024, 0, st>>>(fc, N, sign, stats);
-      affine_kernel<<<dim3((unsigned)((N + 255) / 256), (unsigned)nb), 256, 0, st>>>(fc, N, sign, stats, method == EVOK_RANK_NORMALIZED, w + b0 * N);
-      EVOK_CHECK_LAUNCH_N(method == EVOK_RANK_NORMALIZED ? 2 : 1);
-    }
-    return 0;
+    return affine_rows(method, f, N, n_items, higher_is_better, w, (float*)ws, st);
   }
-  if (use_small_rank(N)) {
-    for (int64_t b0 = 0; b0 < n_items; b0 += kMaxGridY) {
-      const int64_t nb = n_items - b0 < kMaxGridY ? n_items - b0 : kMaxGridY;
-      const int rc = rank_small(f + b0 * N, N, !higher_is_better, kSmallUtilities, method, 0, w + b0 * N, nullptr, st, nullptr, nb);
-      if (rc) return rc;
-    }
-    return 0;
-  }
-  for (int64_t b = 0; b < n_items; ++b) {
-    const int rc = evok_rank(method, f + b * N, N, higher_is_better, w + b * N, nullptr, ws, ws_bytes, stream);
-    if (rc) return rc;
-  }
-  return 0;
+  return rank_rows(f, N, n_items, !higher_is_better, utilities(method, w, nullptr), ws, ws_bytes, st);
 }
 
 extern "C" EVOK_API int evok_elite_mask_batched(const float* w, int64_t N, int64_t n_items, int64_t num_elites, float* mask, void* ws,
@@ -805,20 +720,7 @@ extern "C" EVOK_API int evok_elite_mask_batched(const float* w, int64_t N, int64
   if (!w || !mask || !ws) return EVOK_E_NULLPTR;
   if (N < 0 || N >= (int64_t)1 << 32 || n_items < 0 || num_elites < 0 || num_elites > N) return EVOK_E_BADSIZE;
   if (N == 0 || n_items == 0) return 0;
-  if (use_small_rank(N)) {
-    for (int64_t b0 = 0; b0 < n_items; b0 += kMaxGridY) {
-      const int64_t nb = n_items - b0 < kMaxGridY ? n_items - b0 : kMaxGridY;
-      const int rc = rank_small(w + b0 * N, N, /*descending=*/1, kSmallEliteMask, 0, num_elites, mask + b0 * N, nullptr, (cudaStream_t)stream,
-                                nullptr, nb);
-      if (rc) return rc;
-    }
-    return 0;
-  }
-  for (int64_t b = 0; b < n_items; ++b) {
-    const int rc = evok_elite_mask(w + b * N, N, num_elites, mask + b * N, ws, ws_bytes, stream);
-    if (rc) return rc;
-  }
-  return 0;
+  return rank_rows(w, N, n_items, /*descending=*/1, elite_flags(num_elites, mask), ws, ws_bytes, (cudaStream_t)stream);
 }
 
 extern "C" EVOK_API int evok_weights_adjust_batched(float* w, int64_t N, int64_t n_items, int mode, void* stream) {
@@ -826,10 +728,9 @@ extern "C" EVOK_API int evok_weights_adjust_batched(float* w, int64_t N, int64_t
   if (mode != 1 && mode != 2) return EVOK_E_BADENUM;
   if (N < 0 || n_items < 0) return EVOK_E_BADSIZE;
   if (N == 0 || n_items == 0) return 0;
-  for (int64_t b0 = 0; b0 < n_items; b0 += kMaxGridY) {
-    const int64_t nb = n_items - b0 < kMaxGridY ? n_items - b0 : kMaxGridY;
+  return for_item_chunks(n_items, kMaxGridY, [&](int64_t b0, int64_t nb) {
     weights_adjust_kernel<<<(unsigned)nb, 1024, 0, (cudaStream_t)stream>>>(w + b0 * N, N, mode);
     EVOK_CHECK_LAUNCH();
-  }
-  return 0;
+    return 0;
+  });
 }

@@ -372,8 +372,7 @@ extern "C" EVOK_API int evok_sample_batched(float* X, int64_t item_stride_x, int
   cudaStream_t st = (cudaStream_t)stream;
   // grid y is at most kMaxGridY items: larger batches go in item chunks, chunk b0 starting at stream word stream_lo + b0, so item b
   // keeps its Philox stream stream_id0 + b
-  for (int64_t b0 = 0; b0 < n_items; b0 += kMaxGridY) {
-    const int64_t nb = n_items - b0 < kMaxGridY ? n_items - b0 : kMaxGridY;
+  return for_item_chunks(n_items, kMaxGridY, [&](int64_t b0, int64_t nb) {
     PhiloxKey kc = key;
     kc.stream_lo += (uint32_t)b0;
     const dim3 grid((unsigned)ctas, (unsigned)nb);
@@ -391,6 +390,6 @@ extern "C" EVOK_API int evok_sample_batched(float* X, int64_t item_stride_x, int
     }
 #undef EVOK_LAUNCH_SB
     EVOK_CHECK_LAUNCH();
-  }
-  return 0;
+    return 0;
+  });
 }

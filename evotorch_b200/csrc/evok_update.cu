@@ -9,9 +9,10 @@ unsigned long long g_launch_count = 0;
 
 constexpr int kUpdThreads = 1024;
 
-__global__ void __launch_bounds__(kUpdThreads) clipup_kernel(const float* __restrict__ g, int64_t D, float* __restrict__ velocity,
-                                                             float stepsize, float momentum, float max_speed, float* __restrict__ step_out,
-                                                             float* __restrict__ mu) {
+// ClipUp on one D-vector, by one CTA of kUpdThreads; store(i, step) writes step i where the caller wants it
+template <typename Store>
+__device__ __forceinline__ void clipup(const float* __restrict__ g, int64_t D, float* __restrict__ velocity, float stepsize, float momentum,
+                                       float max_speed, Store store) {
   __shared__ double sm[33];
   double acc = 0.0;
   for (int64_t i = threadIdx.x; i < D; i += kUpdThreads) {
@@ -35,9 +36,17 @@ __global__ void __launch_bounds__(kUpdThreads) clipup_kernel(const float* __rest
       nv *= ratio;
       velocity[i] = nv;
     }
+    store(i, nv);
+  }
+}
+
+__global__ void __launch_bounds__(kUpdThreads) clipup_kernel(const float* __restrict__ g, int64_t D, float* __restrict__ velocity,
+                                                             float stepsize, float momentum, float max_speed, float* __restrict__ step_out,
+                                                             float* __restrict__ mu) {
+  clipup(g, D, velocity, stepsize, momentum, max_speed, [&](int64_t i, float nv) {
     if (step_out) step_out[i] = nv;
     if (mu) mu[i] += nv;
-  }
+  });
 }
 
 __global__ void __launch_bounds__(256) adam_kernel(const float* __restrict__ g, int64_t D, float* __restrict__ m, float* __restrict__ v,
@@ -90,12 +99,10 @@ __device__ __forceinline__ float clamp_sigma(float s, float target, float lo, fl
   return torch_min(torch_max(target, lo), hi);
 }
 
-__global__ void __launch_bounds__(256) sigma_update_kernel(float* __restrict__ sigma, const float* __restrict__ g, int64_t D, float lr,
-                                                           int exp_form, const float* __restrict__ lb_vec, float lb,
-                                                           const float* __restrict__ ub_vec, float ub, const float* __restrict__ mc_vec,
-                                                           float mc) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= D) return;
+// sigma[i] after the step lr * g[i]: the target sigma + step (or sigma * exp(step / 2)), then clamp_sigma
+__device__ __forceinline__ void sigma_step(float* __restrict__ sigma, const float* __restrict__ g, int64_t i, float lr, int exp_form,
+                                           const float* __restrict__ lb_vec, float lb, const float* __restrict__ ub_vec, float ub,
+                                           const float* __restrict__ mc_vec, float mc) {
   const float s = sigma[i];
   const float step = lr * g[i];
   const float target = exp_form ? s * expf(0.5f * step) : s + step;
@@ -106,44 +113,27 @@ __global__ void __launch_bounds__(256) sigma_update_kernel(float* __restrict__ s
   sigma[i] = clamp_sigma(s, target, lo, hi, has_mc, mc_vec ? mc_vec[i] : mc);
 }
 
+__global__ void __launch_bounds__(256) sigma_update_kernel(float* __restrict__ sigma, const float* __restrict__ g, int64_t D, float lr,
+                                                           int exp_form, const float* __restrict__ lb_vec, float lb,
+                                                           const float* __restrict__ ub_vec, float ub, const float* __restrict__ mc_vec,
+                                                           float mc) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= D) return;
+  sigma_step(sigma, g, i, lr, exp_form, lb_vec, lb, ub_vec, ub, mc_vec, mc);
+}
+
 // Batched searches: per-item scalar hyper-parameters travel BY VALUE in the launch parameters (no device copy, no sync)
 constexpr int kItemsPerLaunch = 256;
 struct ItemScalars {
   float a[kItemsPerLaunch], b[kItemsPerLaunch], c[kItemsPerLaunch];
 };
 
-// one CTA per item: the ClipUp step of clipup_kernel on row blockIdx.x of [items][D] tensors, with that item's (lr, momentum, max_speed)
+// one CTA per item: clipup on row blockIdx.x of [items][D] tensors, with that item's (lr, momentum, max_speed)
 __global__ void __launch_bounds__(kUpdThreads) clipup_batched_kernel(const float* __restrict__ g, int64_t D, float* __restrict__ velocity,
                                                                      float* __restrict__ center, const __grid_constant__ ItemScalars sc) {
-  __shared__ double sm[33];
   const int item = blockIdx.x;
-  const float stepsize = sc.a[item], momentum = sc.b[item], max_speed = sc.c[item];
-  g += (int64_t)item * D;
-  velocity += (int64_t)item * D;
-  center += (int64_t)item * D;
-  double acc = 0.0;
-  for (int64_t i = threadIdx.x; i < D; i += kUpdThreads) {
-    const double v = (double)g[i];
-    acc += v * v;
-  }
-  const float gnorm = (float)sqrt(block_sum<double>(acc, sm));
-  acc = 0.0;
-  for (int64_t i = threadIdx.x; i < D; i += kUpdThreads) {
-    const float nv = momentum * velocity[i] + __fdiv_rn(g[i], gnorm) * stepsize;
-    velocity[i] = nv;
-    acc += (double)nv * (double)nv;
-  }
-  const float vnorm = (float)sqrt(block_sum<double>(acc, sm));
-  const bool clip = vnorm > max_speed;
-  const float ratio = clip ? __fdiv_rn(max_speed, vnorm) : 1.0f;
-  for (int64_t i = threadIdx.x; i < D; i += kUpdThreads) {
-    float nv = velocity[i];
-    if (clip) {
-      nv *= ratio;
-      velocity[i] = nv;
-    }
-    center[i] += nv;
-  }
+  const int64_t off = (int64_t)item * D;
+  clipup(g + off, D, velocity + off, sc.a[item], sc.b[item], sc.c[item], [&](int64_t i, float nv) { center[off + i] += nv; });
 }
 
 // sigma_update_kernel on [items][D] tensors with a per-item learning rate (blockIdx.y = item)
@@ -152,11 +142,8 @@ __global__ void __launch_bounds__(256) sigma_update_batched_kernel(float* __rest
                                                                    const float* __restrict__ mc_vec, const __grid_constant__ ItemScalars sc) {
   const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= D) return;
-  const int64_t i = (int64_t)blockIdx.y * D + j;
-  const float s = sigma[i];
-  const float step = sc.a[blockIdx.y] * g[i];
-  const float target = exp_form ? s * expf(0.5f * step) : s + step;
-  sigma[i] = clamp_sigma(s, target, lb_vec ? lb_vec[i] : -INFINITY, ub_vec ? ub_vec[i] : INFINITY, mc_vec != nullptr, mc_vec ? mc_vec[i] : 0.0f);
+  // absent bounds and max_change: the NaN scalars
+  sigma_step(sigma, g, (int64_t)blockIdx.y * D + j, sc.a[blockIdx.y], exp_form, lb_vec, NAN, ub_vec, NAN, mc_vec, NAN);
 }
 
 // E elites: grad_mu = S1 / E, grad_sigma = unbiased std - sigma.  As torch.std: E = 1 (a zero divisor) and E = 0 give NaN, and a NaN
@@ -238,34 +225,32 @@ extern "C" EVOK_API int evok_clipup_batched(const float* g, int64_t n_items, int
                                             const float* momentum_host, const float* max_speed_host, void* stream) {
   if (!g || !velocity || !center || !stepsize_host || !momentum_host || !max_speed_host) return EVOK_E_NULLPTR;
   if (D <= 0 || n_items < 0) return EVOK_E_BADSIZE;
-  for (int64_t b0 = 0; b0 < n_items; b0 += kItemsPerLaunch) {
-    const int n = (int)((n_items - b0) < kItemsPerLaunch ? (n_items - b0) : kItemsPerLaunch);
+  return for_item_chunks(n_items, kItemsPerLaunch, [&](int64_t b0, int64_t n) {
     ItemScalars sc;
     for (int i = 0; i < n; ++i) {
       sc.a[i] = stepsize_host[b0 + i];
       sc.b[i] = momentum_host[b0 + i];
       sc.c[i] = max_speed_host[b0 + i];
     }
-    clipup_batched_kernel<<<n, kUpdThreads, 0, (cudaStream_t)stream>>>(g + b0 * D, D, velocity + b0 * D, center + b0 * D, sc);
+    clipup_batched_kernel<<<(unsigned)n, kUpdThreads, 0, (cudaStream_t)stream>>>(g + b0 * D, D, velocity + b0 * D, center + b0 * D, sc);
     EVOK_CHECK_LAUNCH();
-  }
-  return 0;
+    return 0;
+  });
 }
 
 extern "C" EVOK_API int evok_sigma_update_batched(float* sigma, const float* g, int64_t n_items, int64_t D, const float* lr_host, int exp_form,
                                                   const float* lb_vec, const float* ub_vec, const float* mc_vec, void* stream) {
   if (!sigma || !g || !lr_host) return EVOK_E_NULLPTR;
   if (D <= 0 || n_items < 0) return EVOK_E_BADSIZE;
-  for (int64_t b0 = 0; b0 < n_items; b0 += kItemsPerLaunch) {
-    const int n = (int)((n_items - b0) < kItemsPerLaunch ? (n_items - b0) : kItemsPerLaunch);
+  return for_item_chunks(n_items, kItemsPerLaunch, [&](int64_t b0, int64_t n) {
     ItemScalars sc;
     for (int i = 0; i < n; ++i) sc.a[i] = lr_host[b0 + i];
     const int64_t off = b0 * D;
     sigma_update_batched_kernel<<<dim3(nblk(D), (unsigned)n), 256, 0, (cudaStream_t)stream>>>(
         sigma + off, g + off, D, exp_form, lb_vec ? lb_vec + off : nullptr, ub_vec ? ub_vec + off : nullptr, mc_vec ? mc_vec + off : nullptr, sc);
     EVOK_CHECK_LAUNCH();
-  }
-  return 0;
+    return 0;
+  });
 }
 
 extern "C" EVOK_API int evok_abi_version(void) { return EVOK_ABI_VERSION; }

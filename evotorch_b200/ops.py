@@ -7,6 +7,7 @@ libevok.so (include/evok.h).  Callers in this package decide *whether* a tensor 
 
 from __future__ import annotations
 
+import contextlib
 import ctypes
 import math
 from typing import Optional
@@ -241,6 +242,14 @@ def _rank_ws(device: torch.device, n: int) -> torch.Tensor:
     return nat.workspace(device, nat.lib().evok_rank_workspace_bytes(n), "rank")
 
 
+def _rank_call(entry: str, keys: torch.Tensor, *args, timed: bool = True) -> None:
+    """`entry`(*args, workspace, its size, stream) for a K3 entry point that sorts `keys`, timed as "rank" if `timed`."""
+    ws = _rank_ws(keys.device, keys.shape[-1])
+    with _timed("rank") if timed else contextlib.nullcontext():
+        rc = getattr(nat.lib(), entry)(*args, ws.data_ptr(), ws.numel(), nat.stream_of(keys))
+    nat.check(rc, entry)
+
+
 def rank(f: torch.Tensor, method: str, higher_is_better: bool, out: Optional[torch.Tensor] = None,
          perm: Optional[torch.Tensor] = None) -> torch.Tensor:
     f = _vec(f, "fitnesses")
@@ -248,22 +257,14 @@ def rank(f: torch.Tensor, method: str, higher_is_better: bool, out: Optional[tor
     w = torch.empty_like(f) if out is None else _vec(out, "out", n)
     if perm is not None and not (perm.is_cuda and perm.dtype == torch.int64 and perm.is_contiguous() and perm.numel() == n):
         raise ValueError("perm: expected a contiguous int64 CUDA tensor of the same length")
-    ws = _rank_ws(f.device, n)
-    method_id = RANK_IDS[method]
-    with _timed("rank"):
-        rc = nat.lib().evok_rank(method_id, f.data_ptr(), n, int(bool(higher_is_better)), w.data_ptr(), nat.ptr(perm), ws.data_ptr(),
-                                 ws.numel(), nat.stream_of(f))
-    nat.check(rc, "evok_rank")
+    _rank_call("evok_rank", f, RANK_IDS[method], f.data_ptr(), n, int(bool(higher_is_better)), w.data_ptr(), nat.ptr(perm))
     return w
 
 
 def argsort(keys: torch.Tensor, descending: bool) -> torch.Tensor:
     keys = _vec(keys, "keys")
-    n = keys.numel()
-    perm = torch.empty(n, dtype=torch.int64, device=keys.device)
-    ws = _rank_ws(keys.device, n)
-    nat.check(nat.lib().evok_argsort(keys.data_ptr(), n, int(bool(descending)), perm.data_ptr(), ws.data_ptr(), ws.numel(),
-                                     nat.stream_of(keys)), "evok_argsort")
+    perm = torch.empty(keys.numel(), dtype=torch.int64, device=keys.device)
+    _rank_call("evok_argsort", keys, keys.data_ptr(), keys.numel(), int(bool(descending)), perm.data_ptr(), timed=False)
     return perm
 
 
@@ -273,11 +274,7 @@ def rank_table(keys: torch.Tensor, descending: bool, table: torch.Tensor, out: O
     n = keys.numel()
     _vec(table, "table", n)
     out = torch.empty_like(keys) if out is None else _vec(out, "out", n)
-    ws = _rank_ws(keys.device, n)
-    with _timed("rank"):
-        rc = nat.lib().evok_rank_table(keys.data_ptr(), n, int(bool(descending)), table.data_ptr(), out.data_ptr(), ws.data_ptr(), ws.numel(),
-                                       nat.stream_of(keys))
-    nat.check(rc, "evok_rank_table")
+    _rank_call("evok_rank_table", keys, keys.data_ptr(), n, int(bool(descending)), table.data_ptr(), out.data_ptr())
     return out
 
 
@@ -377,11 +374,8 @@ def weights_adjust_(w: torch.Tensor, mode: int) -> torch.Tensor:
 
 def elite_mask(w: torch.Tensor, num_elites: int) -> torch.Tensor:
     w = _vec(w, "weights")
-    n = w.numel()
     mask = torch.empty_like(w)
-    ws = _rank_ws(w.device, n)
-    nat.check(nat.lib().evok_elite_mask(w.data_ptr(), n, num_elites, mask.data_ptr(), ws.data_ptr(), ws.numel(), nat.stream_of(w)),
-              "evok_elite_mask")
+    _rank_call("evok_elite_mask", w, w.data_ptr(), w.numel(), num_elites, mask.data_ptr(), timed=False)
     return mask
 
 
@@ -521,6 +515,13 @@ def _items(t: torch.Tensor, core_shape: tuple, name: str) -> tuple:
     return t, t.shape[0], int(t.stride(0))
 
 
+def _rows(t: torch.Tensor, name: str, shape: tuple) -> torch.Tensor:
+    """A 2-D operand of the batched stages: contiguous float32 CUDA of shape (items, n)."""
+    if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and tuple(t.shape) == shape):
+        raise ValueError(f"{name}: expected a contiguous float32 CUDA tensor of shape {shape}")
+    return as_plain_tensor(t)
+
+
 def sample_batched(out: torch.Tensor, mu: torch.Tensor, sigma: torch.Tensor, *, symmetric: bool, seed: int, stream_id0: int = 0) -> torch.Tensor:
     """out[b] ~ N(mu[b], diag(sigma[b]^2)) for every batch item in one launch; item b uses Philox stream stream_id0 + b."""
     if not (out.is_cuda and out.dtype == torch.float32 and out.ndim == 3 and out.is_contiguous()):
@@ -557,17 +558,16 @@ def rank_batched(f: torch.Tensor, method: str, higher_is_better: bool) -> torch.
 
 
 def elite_mask_batched(w: torch.Tensor, num_elites: int) -> torch.Tensor:
-    w = as_plain_tensor(w).contiguous()
     B, n = w.shape
+    w = _rows(w, "weights", (B, n))
     mask = torch.empty_like(w)
-    ws = _rank_ws(w.device, n)
-    nat.check(nat.lib().evok_elite_mask_batched(w.data_ptr(), n, B, num_elites, mask.data_ptr(), ws.data_ptr(), ws.numel(), nat.stream_of(w)),
-              "evok_elite_mask_batched")
+    _rank_call("evok_elite_mask_batched", w, w.data_ptr(), n, B, num_elites, mask.data_ptr(), timed=False)
     return mask
 
 
 def weights_adjust_batched_(w: torch.Tensor, mode: int) -> torch.Tensor:
     B, n = w.shape
+    _rows(w, "weights", (B, n))
     nat.check(nat.lib().evok_weights_adjust_batched(w.data_ptr(), n, B, mode, nat.stream_of(w)), "evok_weights_adjust_batched")
     return w
 
@@ -598,8 +598,7 @@ def clipup_batched_(g: torch.Tensor, velocity: torch.Tensor, center: torch.Tenso
     """In place on contiguous (items, D) tensors: one CTA per item (per-item hyper-parameters are host scalars)."""
     B, d = center.shape
     for t, name in ((g, "g"), (velocity, "velocity"), (center, "center")):
-        if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and tuple(t.shape) == (B, d)):
-            raise ValueError(f"{name}: expected a contiguous float32 CUDA tensor of shape {(B, d)}")
+        _rows(t, name, (B, d))
     nat.check(nat.lib().evok_clipup_batched(g.data_ptr(), B, d, velocity.data_ptr(), center.data_ptr(), _host_floats(stepsizes, B),
                                             _host_floats(momenta, B), _host_floats(max_speeds, B), nat.stream_of(g)), "evok_clipup_batched")
 
@@ -609,8 +608,8 @@ def sigma_update_batched_(sigma: torch.Tensor, g: torch.Tensor, lrs, exp_form: b
     """In place on contiguous (items, D) tensors; lb / ub / max_change: (items, D) tensors or None."""
     B, d = sigma.shape
     for t, name in ((sigma, "sigma"), (g, "g"), (lb, "lb"), (ub, "ub"), (max_change, "max_change")):
-        if t is not None and not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and tuple(t.shape) == (B, d)):
-            raise ValueError(f"{name}: expected a contiguous float32 CUDA tensor of shape {(B, d)}")
+        if t is not None:
+            _rows(t, name, (B, d))
     nat.check(nat.lib().evok_sigma_update_batched(sigma.data_ptr(), g.data_ptr(), B, d, _host_floats(lrs, B), int(bool(exp_form)), nat.ptr(lb),
                                                   nat.ptr(ub), nat.ptr(max_change), nat.stream_of(sigma)), "evok_sigma_update_batched")
 

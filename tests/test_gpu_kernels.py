@@ -175,7 +175,7 @@ def test_rank_matches_reference_golden(golden, name, method, hib):
     np.testing.assert_array_equal(N(perm), O.argsort_for_ranking(f, hib))  # bit-exact ranking indices
 
 
-@pytest.mark.parametrize("n", [1, 2, 31, 1024, 1025, 2049, 4096, 4097, 8192, 8193, 100_003, 1_000_000])  # <= 8192: the single-launch counting rank; above: radix
+@pytest.mark.parametrize("n", [1, 2, 31, 1024, 1025, 2049, 4096, 4097, 8192, 8193, 100_003, 524_288, 524_289, 1_000_000])  # <= 8192: the single-launch counting rank; above: radix (self-scanning up to 524 288)
 @pytest.mark.parametrize("hib", [True, False])
 def test_rank_large_with_ties_nan_and_signed_zero(n, hib):
     rng = np.random.default_rng(n)

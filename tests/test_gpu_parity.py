@@ -444,7 +444,7 @@ def test_rank_table_and_affine_syrk_kernels():
 
 
 # ------------------------------------------------------------------------------------------------ batched functional kernels
-@pytest.mark.parametrize("shape", [(5, 40, 12), (3, 1000, 100), (2, 20000, 64), (1, 30, 7)])
+@pytest.mark.parametrize("shape", [(5, 40, 12), (3, 1000, 100), (2, 20000, 64), (1, 30, 7), (2, 524290, 8)])
 def test_batched_stage_kernels_equal_the_per_item_kernels(shape):
     """SURVEY 8(f2): every batched stage (grid y / z = batch item) computes exactly what its single-search entry point computes per
     item: K1 bit-identical, K3 bit-identical, K4 / K5 to fp32 summation order."""

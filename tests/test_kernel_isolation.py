@@ -475,7 +475,7 @@ def _check_workspace_independence(call, large=None):
 RANK_METHODS = ("centered", "linear", "nes", "normalized", "raw")
 
 
-@pytest.mark.parametrize("n", [1000, 8192, 20000, 700000])  # counting path (n <= 8192), self-scanning and three-kernel radix sort
+@pytest.mark.parametrize("n", [1000, 8192, 20000, 524288, 524289, 700000])  # counting path (n <= 8192), self-scanning (n <= 524288) and three-kernel radix sort
 def test_ranking_does_not_depend_on_workspace_contents(n):
     g = gen(n)
     f = torch.round(torch.randn(n, device=DEV, generator=g) * 20) / 20  # ties
