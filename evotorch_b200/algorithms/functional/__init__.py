@@ -6,15 +6,22 @@
         population = pgpe_ask(state, popsize=1000)
         state = pgpe_tell(state, population, f(population))
     best_guess = state.optimizer_state.center
+
+With an objective that has a fused kernel, `pgpe_ask_and_evaluate` / `cem_ask_and_evaluate` sample and evaluate all batch items
+in one launch, and with `lazy=True` never store the population:
+
+    population, evals = pgpe_ask_and_evaluate(state, popsize=1000, objective=rastrigin, lazy=True)
+    state = pgpe_tell(state, population, evals)
 """
 
 from .funcadam import AdamState, adam, adam_ask, adam_tell
-from .funccem import CEMState, cem, cem_ask, cem_tell
+from .funccem import CEMState, cem, cem_ask, cem_ask_and_evaluate, cem_tell
 from .funcclipup import ClipUpState, clipup, clipup_ask, clipup_tell
-from .funcpgpe import PGPEState, pgpe, pgpe_ask, pgpe_tell
+from .funcpgpe import PGPEState, pgpe, pgpe_ask, pgpe_ask_and_evaluate, pgpe_tell
+from .fused import LazyPopulation
 from .funcsgd import SGDState, sgd, sgd_ask, sgd_tell
 from .misc import OptimizerFunctions, get_functional_optimizer
 
-__all__ = ["AdamState", "adam", "adam_ask", "adam_tell", "CEMState", "cem", "cem_ask", "cem_tell", "ClipUpState", "clipup", "clipup_ask",
-           "clipup_tell", "PGPEState", "pgpe", "pgpe_ask", "pgpe_tell", "SGDState", "sgd", "sgd_ask", "sgd_tell", "OptimizerFunctions",
-           "get_functional_optimizer"]
+__all__ = ["AdamState", "adam", "adam_ask", "adam_tell", "CEMState", "cem", "cem_ask", "cem_ask_and_evaluate", "cem_tell", "ClipUpState",
+           "clipup", "clipup_ask", "clipup_tell", "LazyPopulation", "PGPEState", "pgpe", "pgpe_ask", "pgpe_ask_and_evaluate", "pgpe_tell",
+           "SGDState", "sgd", "sgd_ask", "sgd_tell", "OptimizerFunctions", "get_functional_optimizer"]

@@ -9,7 +9,7 @@ from __future__ import annotations
 
 import os
 
-from typing import NamedTuple
+from typing import Callable, NamedTuple, Union
 
 import torch
 
@@ -17,6 +17,7 @@ from ... import ops
 from ...distributions import SeparableGaussian
 from ...tools import modify_tensor
 from .funcpgpe import sample_separable
+from .fused import LazyPopulation, ask_and_evaluate
 from .misc import batch_shape_of, expand_to, flat_items, get_stdev_init, on_kernels, vector_like_center
 
 
@@ -55,31 +56,49 @@ def cem_ask(state: CEMState, *, popsize: int) -> torch.Tensor:
     return sample_separable(state.center, state.stdev, popsize, False)
 
 
-def cem_tell(state: CEMState, values: torch.Tensor, evals: torch.Tensor) -> CEMState:
+def cem_ask_and_evaluate(state: CEMState, *, popsize: int, objective: Callable, lazy: bool = False) -> tuple:
+    """`cem_ask` and the fitnesses of the population, fused into one launch where the kernels and the objective allow it; see
+    `pgpe_ask_and_evaluate`.  With `lazy=True` the tell rebuilds only the elites."""
+    return ask_and_evaluate(lambda: cem_ask(state, popsize=popsize), state.center, state.stdev, popsize, False, objective, lazy)
+
+
+def cem_tell(state: CEMState, values: Union[torch.Tensor, LazyPopulation], evals: torch.Tensor) -> CEMState:
     center = state.center
-    values = torch.as_tensor(values, dtype=center.dtype, device=center.device)
+    lazy = isinstance(values, LazyPopulation)
+    if lazy:
+        values.check_drawn_from(center, state.stdev, False)
+    else:
+        values = torch.as_tensor(values, dtype=center.dtype, device=center.device)
     evals = torch.as_tensor(evals, dtype=center.dtype, device=center.device)
     batch = batch_shape_of((center, 1), (state.stdev, 1), (values, 2), (evals, 1), (state.stdev_min, 1), (state.stdev_max, 1),
                            (state.stdev_max_change, 1))
+    if lazy and tuple(batch) != tuple(values.shape[:-2]):
+        # batched hyper-parameters or fitnesses over fewer population items: the tell broadcasts a drawn item to several of its
+        # items, which the rebuild (item b on stream b) cannot; the population is regenerated bit for bit for this tell instead
+        values, lazy = values.materialize(), False
     d = center.shape[-1]
     mus, sigmas = flat_items(center, batch, 1), flat_items(state.stdev, batch, 1)
-    xs, fs = flat_items(values, batch, 2), flat_items(evals, batch, 1)
+    xs = None if lazy else flat_items(values, batch, 2)
+    fs = flat_items(evals, batch, 1)
     lbs, ubs, mcs = (flat_items(t, batch, 1) for t in (state.stdev_min, state.stdev_max, state.stdev_max_change))
     new_center = expand_to(center, batch, 1).contiguous().clone()
     new_stdev = expand_to(state.stdev, batch, 1).contiguous().clone()
     new_mus, new_sigmas = new_center.view(-1, d), new_stdev.view(-1, d)
-    kernels = on_kernels(center, values)
+    kernels = lazy or on_kernels(center, values)
     sense = "max" if state.maximize else "min"
-    if kernels and os.environ.get("EVOTORCH_B200_FUNCTIONAL_LOOP", "0") != "1":  # (=1: the per-item launch chains, for comparison)
+    if lazy or (kernels and os.environ.get("EVOTORCH_B200_FUNCTIONAL_LOOP", "0") != "1"):  # (=1: the per-item launch chains, for comparison)
         # one launch per stage for ALL batch items: raw utilities, elite flags, elite moments, mean / std of the elites, clamped update
         import math
 
-        n = xs.shape[1]
+        n = fs.shape[1]
         num_elites = math.floor(n * state.parenthood_ratio)
         w = ops.rank_batched(fs, "raw", state.maximize)
         mask = ops.elite_mask_batched(w, num_elites)
-        s1, s2 = ops.grad_batched(ops.GRAD_MOMENTS, xs, mask, mus if center.ndim > 1 else center, sigmas if state.stdev.ndim > 1 else state.stdev,
-                                  1.0, 1.0)
+        mu_items, sigma_items = mus if center.ndim > 1 else center, sigmas if state.stdev.ndim > 1 else state.stdev
+        if lazy:  # only the elites (non-zero mask) are rebuilt from their Philox counters
+            s1, s2 = ops.grad_batched_regen(ops.GRAD_MOMENTS, mask, mu_items, sigma_items, 1.0, 1.0, seed=values.seed)
+        else:
+            s1, s2 = ops.grad_batched(ops.GRAD_MOMENTS, xs, mask, mu_items, sigma_items, 1.0, 1.0)
         B = s1.shape[0]
         gmu, gsig = ops.cem_finalize(s1.view(-1), s2.view(-1), new_sigmas.reshape(-1), num_elites)
         ops.axpy_(new_mus.view(-1), gmu, 1.0)

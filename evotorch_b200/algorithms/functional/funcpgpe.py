@@ -9,13 +9,14 @@ from __future__ import annotations
 
 import os
 
-from typing import NamedTuple, Optional, Union
+from typing import Callable, NamedTuple, Optional, Union
 
 import torch
 
 from ... import ops
 from ...distributions import SeparableGaussian, SymmetricSeparableGaussian
 from ...tools import modify_tensor
+from .fused import LazyPopulation, ask_and_evaluate
 from .misc import (batch_shape_of, draw_philox_seed, expand_to, flat_items, get_functional_optimizer, get_stdev_init, host_scalar, on_kernels,
                    scalar_items, vector_like_center)
 
@@ -95,34 +96,63 @@ def pgpe_ask(state: PGPEState, *, popsize: int) -> torch.Tensor:
     return sample_separable(ask(state.optimizer_state), state.stdev, popsize, state.symmetric)
 
 
-def pgpe_tell(state: PGPEState, values: torch.Tensor, evals: torch.Tensor) -> PGPEState:
-    """The next state, given the population `values` (..., N, L) and its fitnesses `evals` (..., N)."""
+def pgpe_ask_and_evaluate(state: PGPEState, *, popsize: int, objective: Callable, lazy: bool = False) -> tuple:
+    """`pgpe_ask` and the fitnesses of the population: (values (..., popsize, L), evals (..., popsize)).
+
+    With the centre and stdev on the kernels (float32 CUDA) and an objective with a fused kernel (`evok_objective_id`: the
+    objectives of evotorch_b200.objectives and every FusedObjective), the populations of all batch items are sampled and evaluated
+    in one launch: the population is written once and not read back for the evaluation, and under the same torch.manual_seed it
+    is the population `pgpe_ask` would return.  `lazy=True` does not store it either: `values` is then a `LazyPopulation`, which
+    `pgpe_tell` takes in place of the tensor and whose gradient rows are rebuilt from their Philox counters, bit-identical to the
+    stored population's.  (A tell whose batch is larger than the population's -- batched hyper-parameters over an unbatched
+    centre and stdev -- regenerates the population for that tell: it broadcasts one drawn item to several.)  Otherwise this is `pgpe_ask` followed by `objective(values)`, and `lazy=True` raises ValueError."""
+    _, ask, _ = get_functional_optimizer(state.optimizer)
+    return ask_and_evaluate(lambda: pgpe_ask(state, popsize=popsize), ask(state.optimizer_state), state.stdev, popsize, state.symmetric, objective,
+                            lazy)
+
+
+def pgpe_tell(state: PGPEState, values: Union[torch.Tensor, LazyPopulation], evals: torch.Tensor) -> PGPEState:
+    """The next state, given the population `values` (..., N, L) and its fitnesses `evals` (..., N).  `values` may be the
+    LazyPopulation of `pgpe_ask_and_evaluate(..., lazy=True)` on this very state."""
     _, ask, tell = get_functional_optimizer(state.optimizer)
     center = ask(state.optimizer_state)
-    values = torch.as_tensor(values, dtype=center.dtype, device=center.device)
+    lazy = isinstance(values, LazyPopulation)
+    if lazy:
+        values.check_drawn_from(center, state.stdev, state.symmetric)
+    else:
+        values = torch.as_tensor(values, dtype=center.dtype, device=center.device)
     evals = torch.as_tensor(evals, dtype=center.dtype, device=center.device)
     lr_sigma = state.stdev_learning_rate
     batch = batch_shape_of((center, 1), (state.stdev, 1), (values, 2), (evals, 1), (lr_sigma, 0), (state.stdev_min, 1), (state.stdev_max, 1),
                            (state.stdev_max_change, 1))
+    if lazy and tuple(batch) != tuple(values.shape[:-2]):
+        # batched hyper-parameters or fitnesses over fewer population items: the tell broadcasts a drawn item to several of its
+        # items, which the rebuild (item b on stream b) cannot; the population is regenerated bit for bit for this tell instead
+        values, lazy = values.materialize(), False
     d = center.shape[-1]
     mus, sigmas = flat_items(center, batch, 1), flat_items(state.stdev, batch, 1)
-    xs, fs = flat_items(values, batch, 2), flat_items(evals, batch, 1)
+    xs = None if lazy else flat_items(values, batch, 2)
+    fs = flat_items(evals, batch, 1)
     lbs, ubs, mcs = (flat_items(t, batch, 1) for t in (state.stdev_min, state.stdev_max, state.stdev_max_change))
     sense = "max" if state.maximize else "min"
     n_items = mus.shape[0]
     grad_mu = torch.empty(n_items, d, dtype=center.dtype, device=center.device)
     new_stdev = expand_to(state.stdev, batch, 1).contiguous().clone()
     new_sigmas = new_stdev.view(-1, d)
-    kernels = on_kernels(center, values)
-    if kernels and os.environ.get("EVOTORCH_B200_FUNCTIONAL_LOOP", "0") != "1":  # (=1: the per-item launch chains, for comparison)
+    kernels = lazy or on_kernels(center, values)
+    if lazy or (kernels and os.environ.get("EVOTORCH_B200_FUNCTIONAL_LOOP", "0") != "1"):  # (=1: the per-item launch chains, for comparison)
         # one launch per stage for ALL batch items (grid y / z = item): K3 ranking, K4 weighted reductions, K5 sigma update
-        n = xs.shape[1]
+        n = fs.shape[1]
         w = ops.rank_batched(fs, state.ranking_method, state.maximize)
         if state.ranking_method not in ("centered", "normalized"):  # distributions.py:562-563 / :722-723: w - mean(w)
             ops.weights_adjust_batched_(w, 1)
         scale = 1.0 / (n // 2) if state.symmetric else 1.0 / n  # divide by num_directions / num_solutions (funcpgpe.py defaults)
         form = ops.GRAD_SYMMETRIC if state.symmetric else ops.GRAD_SEPARABLE
-        gmu, gsig = ops.grad_batched(form, xs, w, mus if center.ndim > 1 else center, sigmas if state.stdev.ndim > 1 else state.stdev, scale, scale)
+        mu_items, sigma_items = mus if center.ndim > 1 else center, sigmas if state.stdev.ndim > 1 else state.stdev
+        if lazy:  # the rows with a non-zero weight, rebuilt from their Philox counters: the bits of the stored population's gradient
+            gmu, gsig = ops.grad_batched_regen(form, w, mu_items, sigma_items, scale, scale, seed=values.seed)
+        else:
+            gmu, gsig = ops.grad_batched(form, xs, w, mu_items, sigma_items, scale, scale)
         ops.sigma_update_batched_(new_sigmas, gsig, scalar_items(lr_sigma, batch), False, lb=lbs.contiguous(), ub=ubs.contiguous(),
                                   max_change=mcs.contiguous())
         new_optimizer_state = tell(state.optimizer_state, follow_grad=gmu.view(tuple(batch) + (d,)))

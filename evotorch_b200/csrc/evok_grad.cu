@@ -67,15 +67,20 @@ struct SepWeights {
   float* wsum_partial;
 };
 
-// SYM: unit r = direction (rows 2r, 2r+1), else unit r = row r.  REGEN: eps = sigma * z regenerated from Philox.
-// SEPW (with REGEN, non-symmetric, form MOMENTS, mu = sigma = NULL): the weights above, eps = z.
-template <int VEC, int TX, bool SYM, bool REGEN, bool SEPW = false>
+// Where eps comes from (EPS): kEpsRead: eps = X - mu from the stored rows; kEpsRegen: eps = sigma * z regenerated from Philox
+// (the lazy population of evok_sample_eval); kEpsRebuild: the row rebuilt as the sampler stored it, x = fmaf(sigma, z, mu), then
+// eps = x - mu, bit-identical to kEpsRead over the stored rows, with item b of a batch (blockIdx.z) on stream word stream_lo + b.
+constexpr int kEpsRead = 0, kEpsRegen = 1, kEpsRebuild = 2;
+
+// SYM: unit r = direction (rows 2r, 2r+1), else unit r = row r.
+// SEPW (with kEpsRegen, non-symmetric, form MOMENTS, mu = sigma = NULL): the weights above, eps = z.
+template <int VEC, int TX, bool SYM, int EPS, bool SEPW = false>
 __global__ void __launch_bounds__(kGradThreads, EVOK_GRAD_MINB)
     grad_partial_kernel(int form, const float* __restrict__ X, int64_t ldx, const float* __restrict__ w, const float* __restrict__ mu,
                         const float* __restrict__ sigma, int64_t n_units, int64_t D, int64_t units_per_chunk, uint64_t unit0,
                         const __grid_constant__ PhiloxKey key, const uint32_t* __restrict__ stream_off, float* __restrict__ partial,
                         const __grid_constant__ GradItems items, const __grid_constant__ SepWeights sepw) {
-  static_assert(!SEPW || (REGEN && !SYM), "the CMA-ES weight mode regenerates non-symmetric rows");
+  static_assert(!SEPW || (EPS == kEpsRegen && !SYM), "the CMA-ES weight mode regenerates non-symmetric rows");
   constexpr int TY = kGradThreads / TX;
   if (gridDim.z > 1) {
     const int64_t item = blockIdx.z;
@@ -85,7 +90,7 @@ __global__ void __launch_bounds__(kGradThreads, EVOK_GRAD_MINB)
     sigma += item * items.sigma;
     partial += item * items.partial;
   }
-  const uint32_t sw = key.stream_lo + ((REGEN && stream_off) ? __ldg(stream_off) : 0u);
+  const uint32_t sw = key.stream_lo + ((EPS != kEpsRead && stream_off) ? __ldg(stream_off) : 0u) + (EPS == kEpsRebuild ? (uint32_t)blockIdx.z : 0u);
   const int tx = threadIdx.x % TX, ty = threadIdx.x / TX;
   const int64_t col = ((int64_t)blockIdx.x * TX + tx) * VEC;
   const bool active = col < D;
@@ -146,7 +151,7 @@ __global__ void __launch_bounds__(kGradThreads, EVOK_GRAD_MINB)
     for (int u = 0; u < kGradUnroll; ++u) {
       const int64_t r = r0 + (int64_t)u * TY;
       if (need[u]) {
-        if (REGEN) {
+        if (EPS != kEpsRead) {
           if (VEC == 4) {
             normals4(key, sw, unit0 + (uint64_t)r, (uint32_t)(col >> 2), x[u].v);
           } else {
@@ -164,7 +169,7 @@ __global__ void __launch_bounds__(kGradThreads, EVOK_GRAD_MINB)
       if (need[u]) {
 #pragma unroll
         for (int c = 0; c < VEC; ++c) {
-          const float e = REGEN ? sg[c] * x[u].v[c] : x[u].v[c] - m[c];
+          const float e = EPS == kEpsRegen ? sg[c] * x[u].v[c] : EPS == kEpsRebuild ? fmaf(sg[c], x[u].v[c], m[c]) - m[c] : x[u].v[c] - m[c];
           s1[c] = fmaf(a[u], e, s1[c]);
           s2[c] = fmaf(b[u], fmaf(e * e, c1[c], -c0[c]), s2[c]);
         }
@@ -528,7 +533,7 @@ static GradPlan plan_grad(int64_t n_units, int64_t D, bool vec_ok) {
   return p;
 }
 
-template <int VEC, bool SYM, bool REGEN, bool SEPW = false>
+template <int VEC, bool SYM, int EPS, bool SEPW = false>
 static void launch_partial(const GradPlan& p, int form, const float* X, int64_t ldx, const float* w, const float* mu, const float* sigma,
                            int64_t n_units, int64_t D, uint64_t unit0, uint64_t seed, uint64_t stream_id, const uint32_t* stream_off, float* partial,
                            cudaStream_t st, int64_t n_items = 1, const GradItems* items = nullptr, const SepWeights* sep = nullptr) {
@@ -537,7 +542,7 @@ static void launch_partial(const GradPlan& p, int form, const float* X, int64_t 
   const GradItems it = items ? *items : GradItems{0, 0, 0, 0, 0};
   const SepWeights sw = sep ? *sep : SepWeights{nullptr, 0, nullptr};
 #define EVOK_LAUNCH_TX(TXV)                                                                                                               \
-  grad_partial_kernel<VEC, TXV, SYM, REGEN, SEPW><<<grid, kGradThreads, 0, st>>>(form, X, ldx, w, mu, sigma, n_units, D, p.units_per_chunk, \
+  grad_partial_kernel<VEC, TXV, SYM, EPS, SEPW><<<grid, kGradThreads, 0, st>>>(form, X, ldx, w, mu, sigma, n_units, D, p.units_per_chunk, \
                                                                                  unit0, key, stream_off, partial, it, sw)
   switch (p.tx) {
     case 32: EVOK_LAUNCH_TX(32); break;
@@ -654,14 +659,14 @@ static int grad_impl(int form, const float* X, int64_t ldx, const float* w, cons
     return launch_finalize(partial, n_chunks, D, scale_mu, scale_sigma, out_mu, out_sigma, push, st);
   }
   if (regen) {
-    if (sym) launch_partial<4, true, true>(p, form, X, ldx, w, mu, sigma, n_units, D, unit0, seed, stream_id, stream_off, partial, st);
-    else launch_partial<4, false, true>(p, form, X, ldx, w, mu, sigma, n_units, D, unit0, seed, stream_id, stream_off, partial, st);
+    if (sym) launch_partial<4, true, kEpsRegen>(p, form, X, ldx, w, mu, sigma, n_units, D, unit0, seed, stream_id, stream_off, partial, st);
+    else launch_partial<4, false, kEpsRegen>(p, form, X, ldx, w, mu, sigma, n_units, D, unit0, seed, stream_id, stream_off, partial, st);
   } else if (vec_ok) {
-    if (sym) launch_partial<4, true, false>(p, form, X, ldx, w, mu, sigma, n_units, D, unit0, seed, stream_id, stream_off, partial, st);
-    else launch_partial<4, false, false>(p, form, X, ldx, w, mu, sigma, n_units, D, unit0, seed, stream_id, stream_off, partial, st);
+    if (sym) launch_partial<4, true, kEpsRead>(p, form, X, ldx, w, mu, sigma, n_units, D, unit0, seed, stream_id, stream_off, partial, st);
+    else launch_partial<4, false, kEpsRead>(p, form, X, ldx, w, mu, sigma, n_units, D, unit0, seed, stream_id, stream_off, partial, st);
   } else {
-    if (sym) launch_partial<1, true, false>(p, form, X, ldx, w, mu, sigma, n_units, D, unit0, seed, stream_id, stream_off, partial, st);
-    else launch_partial<1, false, false>(p, form, X, ldx, w, mu, sigma, n_units, D, unit0, seed, stream_id, stream_off, partial, st);
+    if (sym) launch_partial<1, true, kEpsRead>(p, form, X, ldx, w, mu, sigma, n_units, D, unit0, seed, stream_id, stream_off, partial, st);
+    else launch_partial<1, false, kEpsRead>(p, form, X, ldx, w, mu, sigma, n_units, D, unit0, seed, stream_id, stream_off, partial, st);
   }
   EVOK_CHECK_LAUNCH();
   return launch_finalize(partial, p.n_chunks, D, scale_mu, scale_sigma, out_mu, out_sigma, push, st);
@@ -717,7 +722,7 @@ extern "C" EVOK_API int evok_sepcma_moments(const float* aw, const float* q, int
   const GradPlan p = plan_grad(n_rows, D, true);
   float* partial = (float*)ws;
   const SepWeights sep{q, active, partial + evok_grad_workspace_bytes(n_rows, D) / sizeof(float)};
-  launch_partial<4, false, true, true>(p, EVOK_GRAD_MOMENTS, nullptr, 0, aw, nullptr, nullptr, n_rows, D, (uint64_t)row0, seed, stream_id,
+  launch_partial<4, false, kEpsRegen, true>(p, EVOK_GRAD_MOMENTS, nullptr, 0, aw, nullptr, nullptr, n_rows, D, (uint64_t)row0, seed, stream_id,
                                        stream_offset_dev, partial, st, 1, nullptr, &sep);
   EVOK_CHECK_LAUNCH();
   grad_finalize_kernel<true><<<(unsigned)((D + 255) / 256), 256, 0, st>>>(partial, p.n_chunks, D, 1.0f, 1.0f, local, S2, 0, sep.wsum_partial, wsum);
@@ -755,24 +760,22 @@ extern "C" EVOK_API size_t evok_grad_batched_workspace_bytes(int64_t n_items, in
   return ((size_t)kMaxResidentCtas * 1024 + 4 * (size_t)n_items * (size_t)D + 64) * sizeof(float);
 }
 
-extern "C" EVOK_API int evok_grad_batched(int form, const float* X, int64_t item_stride_x, int64_t ldx, const float* w, const float* mu,
-                                          int64_t item_stride_mu, const float* sigma, int64_t item_stride_sigma, int64_t n_items, int64_t n_rows,
-                                          int64_t D, float scale_mu, float scale_sigma, float* out_mu, float* out_sigma, void* ws, size_t ws_bytes,
-                                          void* stream) {
-  if (!X || !w || !mu || !sigma || !out_mu || !out_sigma || !ws) return EVOK_E_NULLPTR;
-  if (form < EVOK_GRAD_SEPARABLE || form > EVOK_GRAD_MOMENTS) return EVOK_E_BADENUM;
-  if (n_items < 0 || n_rows < 0 || D <= 0 || ldx < D) return EVOK_E_BADSIZE;
+// evok_grad_batched (X given) and evok_grad_batched_regen (X null: every needed row rebuilt from (seed, stream_id0 + item) as
+// the batched sampler stored it) after their argument checks: one plan, one workspace layout, one launch chain per item chunk.
+// The rebuilt rows take the plan of a contiguous, 16-byte aligned X [items][n_rows][D], so both give the same bits.
+static int grad_batched_impl(int form, const float* X, int64_t item_stride_x, int64_t ldx, const float* w, const float* mu, int64_t item_stride_mu,
+                             const float* sigma, int64_t item_stride_sigma, int64_t n_items, int64_t n_rows, int64_t D, uint64_t seed, uint64_t stream_id0,
+                             float scale_mu, float scale_sigma, float* out_mu, float* out_sigma, void* ws, size_t ws_bytes, cudaStream_t st) {
   const bool sym = form == EVOK_GRAD_SYMMETRIC;
-  if (sym && (n_rows & 1)) return EVOK_E_ODDROWS;
-  if (n_items == 0) return 0;
-  cudaStream_t st = (cudaStream_t)stream;
   const int64_t n_units = sym ? n_rows / 2 : n_rows;
   if (n_units == 0) {
     cudaMemsetAsync(out_mu, 0, (size_t)n_items * D * 4, st);
     cudaMemsetAsync(out_sigma, 0, (size_t)n_items * D * 4, st);
     return 0;
   }
-  const bool vec_ok = (D % 4 == 0) && (ldx % 4 == 0) && aligned16(X) && item_stride_x % 4 == 0 && item_stride_mu % 4 == 0 && item_stride_sigma % 4 == 0;
+  const bool rebuild = X == nullptr;
+  const bool x_vec = rebuild || ((ldx % 4 == 0) && aligned16(X) && item_stride_x % 4 == 0);
+  const bool vec_ok = (D % 4 == 0) && x_vec && item_stride_mu % 4 == 0 && item_stride_sigma % 4 == 0;
   GradPlan p = plan_grad(n_units, D, vec_ok);
   // the batch fills the GPU: fewer row chunks per item keep the fixed-order finalisation short
   int64_t chunks = ((int64_t)kNumSMs * EVOK_GRAD_CTAS_PER_SM + (int64_t)p.n_coltiles * n_items - 1) / ((int64_t)p.n_coltiles * n_items);
@@ -782,7 +785,7 @@ extern "C" EVOK_API int evok_grad_batched(int form, const float* X, int64_t item
     p.n_chunks = (int)((n_units + p.units_per_chunk - 1) / p.units_per_chunk);
   }
   GradItems items;
-  items.x = item_stride_x;
+  items.x = rebuild ? 0 : item_stride_x;
   items.w = n_rows;
   items.mu = item_stride_mu;
   items.sigma = item_stride_sigma;
@@ -792,17 +795,27 @@ extern "C" EVOK_API int evok_grad_batched(int form, const float* X, int64_t item
   const int64_t chunk = n_items < kMaxGridY ? n_items : kMaxGridY;
   if (ws_bytes < (size_t)chunk * items.partial * sizeof(float)) return EVOK_E_WORKSPACE;
   float* partial = (float*)ws;
+  // The rebuild always runs 4 columns per thread: one Philox group gives all 4 (a thread per column would draw each group 4
+  // times).  A column's sum depends only on the row threads per CTA (kGradThreads / tx) and the row chunks, so for the scalar
+  // plan it keeps that plan's tx and chunks, with a quarter of its column tiles, and gives the scalar read path's bits.
+  GradPlan rp = p;
+  if (rebuild && !vec_ok) rp.n_coltiles = (int)(((D + 3) / 4 + p.tx - 1) / p.tx);
   return for_item_chunks(n_items, kMaxGridY, [&](int64_t b0, int64_t nb) {
-    const float* Xc = X + b0 * item_stride_x;
+    const float* Xc = rebuild ? nullptr : X + b0 * item_stride_x;
     const float* wc = w + b0 * n_rows;
     const float* muc = mu + b0 * item_stride_mu;
     const float* sgc = sigma + b0 * item_stride_sigma;
-    if (vec_ok) {
-      if (sym) launch_partial<4, true, false>(p, form, Xc, ldx, wc, muc, sgc, n_units, D, 0, 0, 0, nullptr, partial, st, nb, &items);
-      else launch_partial<4, false, false>(p, form, Xc, ldx, wc, muc, sgc, n_units, D, 0, 0, 0, nullptr, partial, st, nb, &items);
+    // item b0 + z rebuilds on stream word (stream_lo of stream_id0) + b0 + z, as the batched sampler draws it
+    const uint64_t sid = (stream_id0 & ~0xffffffffull) | (uint32_t)(stream_id0 + (uint64_t)b0);
+    if (rebuild) {
+      if (sym) launch_partial<4, true, kEpsRebuild>(rp, form, Xc, ldx, wc, muc, sgc, n_units, D, 0, seed, sid, nullptr, partial, st, nb, &items);
+      else launch_partial<4, false, kEpsRebuild>(rp, form, Xc, ldx, wc, muc, sgc, n_units, D, 0, seed, sid, nullptr, partial, st, nb, &items);
+    } else if (vec_ok) {
+      if (sym) launch_partial<4, true, kEpsRead>(p, form, Xc, ldx, wc, muc, sgc, n_units, D, 0, 0, 0, nullptr, partial, st, nb, &items);
+      else launch_partial<4, false, kEpsRead>(p, form, Xc, ldx, wc, muc, sgc, n_units, D, 0, 0, 0, nullptr, partial, st, nb, &items);
     } else {
-      if (sym) launch_partial<1, true, false>(p, form, Xc, ldx, wc, muc, sgc, n_units, D, 0, 0, 0, nullptr, partial, st, nb, &items);
-      else launch_partial<1, false, false>(p, form, Xc, ldx, wc, muc, sgc, n_units, D, 0, 0, 0, nullptr, partial, st, nb, &items);
+      if (sym) launch_partial<1, true, kEpsRead>(p, form, Xc, ldx, wc, muc, sgc, n_units, D, 0, 0, 0, nullptr, partial, st, nb, &items);
+      else launch_partial<1, false, kEpsRead>(p, form, Xc, ldx, wc, muc, sgc, n_units, D, 0, 0, 0, nullptr, partial, st, nb, &items);
     }
     EVOK_CHECK_LAUNCH();
     grad_finalize_kernel<<<dim3((unsigned)((D + 255) / 256), (unsigned)nb), 256, 0, st>>>(partial, p.n_chunks, D, scale_mu, scale_sigma,
@@ -810,4 +823,30 @@ extern "C" EVOK_API int evok_grad_batched(int form, const float* X, int64_t item
     EVOK_CHECK_LAUNCH();
     return 0;
   });
+}
+
+extern "C" EVOK_API int evok_grad_batched(int form, const float* X, int64_t item_stride_x, int64_t ldx, const float* w, const float* mu,
+                                          int64_t item_stride_mu, const float* sigma, int64_t item_stride_sigma, int64_t n_items, int64_t n_rows,
+                                          int64_t D, float scale_mu, float scale_sigma, float* out_mu, float* out_sigma, void* ws, size_t ws_bytes,
+                                          void* stream) {
+  if (!X || !w || !mu || !sigma || !out_mu || !out_sigma || !ws) return EVOK_E_NULLPTR;
+  if (form < EVOK_GRAD_SEPARABLE || form > EVOK_GRAD_MOMENTS) return EVOK_E_BADENUM;
+  if (n_items < 0 || n_rows < 0 || D <= 0 || ldx < D) return EVOK_E_BADSIZE;
+  if (form == EVOK_GRAD_SYMMETRIC && (n_rows & 1)) return EVOK_E_ODDROWS;
+  if (n_items == 0) return 0;
+  return grad_batched_impl(form, X, item_stride_x, ldx, w, mu, item_stride_mu, sigma, item_stride_sigma, n_items, n_rows, D, 0, 0, scale_mu,
+                           scale_sigma, out_mu, out_sigma, ws, ws_bytes, (cudaStream_t)stream);
+}
+
+extern "C" EVOK_API int evok_grad_batched_regen(int form, const float* w, const float* mu, int64_t item_stride_mu, const float* sigma,
+                                                int64_t item_stride_sigma, int64_t n_items, int64_t n_rows, int64_t D, uint64_t seed,
+                                                uint64_t stream_id0, float scale_mu, float scale_sigma, float* out_mu, float* out_sigma, void* ws,
+                                                size_t ws_bytes, void* stream) {
+  if (!w || !mu || !sigma || !out_mu || !out_sigma || !ws) return EVOK_E_NULLPTR;
+  if (form < EVOK_GRAD_SEPARABLE || form > EVOK_GRAD_MOMENTS) return EVOK_E_BADENUM;
+  if (n_items < 0 || n_rows < 0 || D <= 0 || item_stride_mu < 0 || item_stride_sigma < 0) return EVOK_E_BADSIZE;
+  if (form == EVOK_GRAD_SYMMETRIC && (n_rows & 1)) return EVOK_E_ODDROWS;
+  if (n_items == 0) return 0;
+  return grad_batched_impl(form, nullptr, 0, D, w, mu, item_stride_mu, sigma, item_stride_sigma, n_items, n_rows, D, seed, stream_id0, scale_mu,
+                           scale_sigma, out_mu, out_sigma, ws, ws_bytes, (cudaStream_t)stream);
 }

@@ -13,30 +13,6 @@
 
 namespace evok {
 
-// Batched searches (functional ask/tell API with leading batch dimensions, funcpgpe.py:301-327): blockIdx.y = batch item, every
-// item has its own centre / stdev row (item stride 0 = shared) and its own Philox stream (stream word + item), so one launch
-// draws the populations of all items -- bit-identical to one evok_sample_eval call per item with stream_id = item.
-template <bool SYM, bool VEC>
-__global__ void __launch_bounds__(kSampleThreads, SampleTune<ObjAcc<EVOK_OBJ_NONE>>::kMinBlocks)
-    sample_batched_kernel(float* __restrict__ X, int64_t item_stride_x, int64_t ldx, const float* __restrict__ mu, int64_t item_stride_mu,
-                          const float* __restrict__ sigma, int64_t item_stride_sigma, int64_t n_units, int64_t D, const __grid_constant__ PhiloxKey key) {
-  const int lane = threadIdx.x & 31;
-  const int64_t item = blockIdx.y;
-  X += item * item_stride_x;
-  mu += item * item_stride_mu;
-  sigma += item * item_stride_sigma;
-  const uint32_t sw = key.stream_lo + (uint32_t)item;
-  const int64_t warps_total = (int64_t)gridDim.x * (kSampleThreads / 32);
-  const int64_t gw = (int64_t)blockIdx.x * (kSampleThreads / 32) + (threadIdx.x >> 5);
-  const uint32_t nq = (uint32_t)((D + 3) >> 2);
-  for (int64_t u = gw; u < n_units; u += warps_total) {
-    ObjAcc<EVOK_OBJ_NONE> accp(D), accm(D);
-    float* xp = X + (SYM ? 2 * u : u) * ldx;
-    float* xm = xp + ldx;
-    for (uint32_t q = lane; q < nq; q += 32) sample_group<ObjAcc<EVOK_OBJ_NONE>, SYM, true, VEC>(key, sw, (uint64_t)u, q, D, mu, sigma, xp, xm, accp, accm);
-  }
-}
-
 struct PushArgs {
   PeerSink sink;
   const unsigned long long* epoch;
@@ -49,14 +25,22 @@ struct PushArgs {
 // kernel of a call (choose_kernel) and one function launches it (launch).
 // ------------------------------------------------------------------------------------------------
 
-// The position of a kernel in the EVOK_OBJ_KERNEL_* order: its family (EVOK_OBJ_KERNEL_SAMPLE, _PUSH, _SQ or _EVAL), then
-// + 4 sym (SAMPLE and PUSH), + 2 store (all but EVAL), + vec.  jit.kernel_expressions() lists a registered objective's kernels
-// in the same order.
+// The position of a kernel in the EVOK_OBJ_KERNEL_* order: its family (EVOK_OBJ_KERNEL_SAMPLE, _PUSH, _SQ, _EVAL or
+// _BATCHED), then + 4 sym (SAMPLE, PUSH and BATCHED), + 2 store (all but EVAL), + vec.  jit.kernel_expressions() lists a
+// registered objective's first EVOK_OBJ_KERNELS kernels in the same order, jit.batched_kernel_expressions() its batched ones.
 constexpr int kernel_index(int family, bool sym, bool store, bool vec) {
-  return family + (sym && family < EVOK_OBJ_KERNEL_SQ ? 4 : 0) + (store && family < EVOK_OBJ_KERNEL_EVAL ? 2 : 0) + (vec ? 1 : 0);
+  return family + (sym && (family < EVOK_OBJ_KERNEL_SQ || family == EVOK_OBJ_KERNEL_BATCHED) ? 4 : 0) +
+         (store && family != EVOK_OBJ_KERNEL_EVAL ? 2 : 0) + (vec ? 1 : 0);
 }
 
-static int kernel_threads(int k) { return k >= EVOK_OBJ_KERNEL_EVAL ? kEvalThreads : kSampleThreads; }
+// every kernel of an objective's table: the EVOK_OBJ_KERNELS of its first image, then the batched family of its second
+constexpr int kTableKernels = EVOK_OBJ_KERNEL_BATCHED + EVOK_OBJ_BATCHED_KERNELS;
+static_assert(EVOK_OBJ_KERNEL_BATCHED == EVOK_OBJ_KERNELS, "the batched family follows the first image's kernels");
+
+static int kernel_threads(int k) { return k >= EVOK_OBJ_KERNEL_EVAL && k < EVOK_OBJ_KERNEL_BATCHED ? kEvalThreads : kSampleThreads; }
+
+// the image of a registered objective that holds kernel k: 0 = the one of evok_objective_register, 1 = the batched one
+static int image_of(int k) { return k >= EVOK_OBJ_KERNEL_BATCHED ? 1 : 0; }
 
 // The sampler of built-in objective OBJ with the variant bits V = sym | store << 1 | vec << 2 | push << 3 | sq << 4, if it
 // exists (the SQ sampler is plain and non-symmetric) and can be reached: EVOK_OBJ_NONE only stores samples, since
@@ -69,9 +53,18 @@ static void put_builtin_sampler(void** fn) {
         reinterpret_cast<void*>(sample_eval_kernel<ObjAcc<OBJ>, sym, store, vec, push, sq>);
 }
 
+// The batched sampler of built-in objective OBJ with V = sym | store << 1 | vec << 2 (V < 8); EVOK_OBJ_NONE only stores samples.
+template <int OBJ, int V>
+static void put_builtin_batched(void** fn) {
+  constexpr bool sym = V & 1, store = V & 2, vec = V & 4;
+  if constexpr (V < EVOK_OBJ_BATCHED_KERNELS && (OBJ != EVOK_OBJ_NONE || store))
+    fn[kernel_index(EVOK_OBJ_KERNEL_BATCHED, sym, store, vec)] = reinterpret_cast<void*>(sample_eval_batched_kernel<ObjAcc<OBJ>, sym, store, vec>);
+}
+
 template <int OBJ, int... V>
 static void put_builtin_kernels(void** fn, std::integer_sequence<int, V...>) {
   (put_builtin_sampler<OBJ, V>(fn), ...);
+  (put_builtin_batched<OBJ, V>(fn), ...);
   if constexpr (OBJ != EVOK_OBJ_NONE) {  // evok_eval refuses EVOK_OBJ_NONE
     fn[kernel_index(EVOK_OBJ_KERNEL_EVAL, false, true, false)] = reinterpret_cast<void*>(eval_kernel<ObjAcc<OBJ>, false>);
     fn[kernel_index(EVOK_OBJ_KERNEL_EVAL, false, true, true)] = reinterpret_cast<void*>(eval_kernel<ObjAcc<OBJ>, true>);
@@ -90,18 +83,21 @@ constexpr int kMaxDevices = 64;
 
 // The kernels of one objective on one device, filled on the first use there and kept until the process ends.  A built-in
 // objective's entries are its nvcc-compiled kernels (null where no entry point reaches them); a registered objective's are the
-// functions of its module, loaded into the device's primary context.
+// functions of its modules, loaded into the device's primary context: the first image's on the first use of the id, the
+// batched image's on the first batched use.
 struct DeviceKernels {
-  int state = 0;              // 0: not filled; 1: filled; EVOK_E_NOKERNEL: the cubin lacks a kernel (a permanent failure)
-  CUmodule module = nullptr;  // set for a registered objective: fn holds CUfunctions, launched through the driver
-  void* fn[EVOK_OBJ_KERNELS] = {};
-  int per_sm[EVOK_OBJ_KERNELS] = {};  // resident CTAs per SM
+  int state[2] = {};             // per image: 0: not filled; 1: filled; EVOK_E_NOKERNEL: the cubin lacks a kernel (a permanent failure)
+  CUmodule module[2] = {};       // set for a registered objective: fn holds CUfunctions, launched through the driver
+  void* fn[kTableKernels] = {};
+  int per_sm[kTableKernels] = {};  // resident CTAs per SM
   int sms = 0;
 };
 
 struct Objective {
-  std::vector<char> image;  // a registered objective's cubin and the lowered names of its kernels (in the EVOK_OBJ_KERNEL_* order)
-  std::vector<std::string> names;
+  // a registered objective's cubins and the lowered names of their kernels (in the EVOK_OBJ_KERNEL_* order): [0] from
+  // evok_objective_register, [1] (the batched family, empty until attached) from evok_objective_register_batched
+  std::vector<char> image[2];
+  std::vector<std::string> names[2];
   DeviceKernels dev[kMaxDevices];
 };
 
@@ -146,14 +142,16 @@ static bool is_user(int objective) {
 
 static void fill_builtin(int objective, int dev, DeviceKernels& d) {
   kBuiltinKernels[objective](d.fn);
-  for (int k = 0; k < EVOK_OBJ_KERNELS; ++k)
+  for (int k = 0; k < kTableKernels; ++k)
     if (d.fn[k] && (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&d.per_sm[k], d.fn[k], kernel_threads(k), 0) != cudaSuccess || d.per_sm[k] <= 0))
       d.per_sm[k] = 4;
   if (cudaDeviceGetAttribute(&d.sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || d.sms <= 0) d.sms = kNumSMs;
-  d.state = 1;
+  d.state[0] = d.state[1] = 1;
 }
 
-static int load_module(const Objective& obj, int dev, DeviceKernels& d) {
+// Loads image `part` of a registered objective on device `dev` into its table positions (EVOK_OBJ_KERNELS kernels from 0 for
+// part 0, EVOK_OBJ_BATCHED_KERNELS from EVOK_OBJ_KERNEL_BATCHED for part 1).
+static int load_module(const Objective& obj, int part, int dev, DeviceKernels& d) {
   cudaError_t ce = cudaSetDevice(dev);  // makes the device's primary context (the runtime's) current, creating it if needed
   if (ce != cudaSuccess) return (int)ce;
   if (!driver_api()) return (int)cudaErrorNotSupported;
@@ -161,27 +159,31 @@ static int load_module(const Objective& obj, int dev, DeviceKernels& d) {
   CUdevice cu_dev;
   CUresult r = api.device_get(&cu_dev, dev);
   if (r == CUDA_SUCCESS) r = api.device_attribute(&d.sms, CU_DEVICE_ATTRIBUTE_MULTIPROCESSOR_COUNT, cu_dev);
-  if (r == CUDA_SUCCESS) r = api.module_load(&d.module, obj.image.data());
+  if (r == CUDA_SUCCESS) r = api.module_load(&d.module[part], obj.image[part].data());
   if (r != CUDA_SUCCESS) return (int)r;  // CUresult and cudaError_t share their codes
-  for (int k = 0; k < EVOK_OBJ_KERNELS; ++k) {
+  const int k0 = part ? EVOK_OBJ_KERNEL_BATCHED : 0;
+  const int n = part ? EVOK_OBJ_BATCHED_KERNELS : EVOK_OBJ_KERNELS;
+  for (int i = 0; i < n; ++i) {
+    const int k = k0 + i;
     CUfunction fn = nullptr;
-    if (api.module_function(&fn, d.module, obj.names[k].c_str()) != CUDA_SUCCESS) {
-      api.module_unload(d.module);
-      d.module = nullptr;
-      d.state = EVOK_E_NOKERNEL;
-      return d.state;
+    if (api.module_function(&fn, d.module[part], obj.names[part][i].c_str()) != CUDA_SUCCESS) {
+      api.module_unload(d.module[part]);
+      d.module[part] = nullptr;
+      d.state[part] = EVOK_E_NOKERNEL;
+      return d.state[part];
     }
     d.fn[k] = fn;
     if (api.occupancy(&d.per_sm[k], fn, kernel_threads(k), 0) != CUDA_SUCCESS || d.per_sm[k] <= 0) d.per_sm[k] = 4;
   }
   if (d.sms <= 0) d.sms = kNumSMs;
-  d.state = 1;
+  d.state[part] = 1;
   return 0;
 }
 
-// The kernel table of an objective (a built-in id or a registered one) on the current device, filled here on the first call
-// for that device.
-static int device_kernels(int objective, const DeviceKernels** out) {
+// The kernel table of an objective (a built-in id or a registered one) on the current device, with the kernels of image `part`
+// (image_of) filled here on the first call that needs them on that device.  A registered id without a batched image gives
+// EVOK_E_NOKERNEL for part 1 (not kept: the image may be attached later).
+static int device_kernels(int objective, int part, const DeviceKernels** out) {
   int dev = 0;
   const cudaError_t ce = cudaGetDevice(&dev);
   if (ce != cudaSuccess) return (int)ce;
@@ -190,28 +192,30 @@ static int device_kernels(int objective, const DeviceKernels** out) {
   const bool user = objective >= EVOK_OBJ_USER_BASE;
   Objective& obj = user ? *g_user[objective - EVOK_OBJ_USER_BASE] : g_builtin[objective];
   DeviceKernels& d = obj.dev[dev];
-  if (d.state == 0) {
+  if (d.state[part] == 0) {
     if (!user) fill_builtin(objective, dev, d);
-    else if (const int rc = load_module(obj, dev, d)) return rc;
+    else if (obj.image[part].empty()) return EVOK_E_NOKERNEL;
+    else if (const int rc = load_module(obj, part, dev, d)) return rc;
   }
-  if (d.state != 1) return d.state;
+  if (d.state[part] != 1) return d.state[part];
   *out = &d;
   return 0;
 }
 
 struct KernelChoice {
   int k;                // index in the EVOK_OBJ_KERNEL_* order
-  int64_t n_units;      // rows, or antithetic row pairs for symmetric sampling; one warp each
-  int64_t ctas_needed;  // CTAs that give every unit its own warp
+  int64_t n_units;      // rows, or antithetic row pairs for symmetric sampling; one warp each (per item)
+  int64_t ctas_needed;  // CTAs that give every unit of an item its own warp
 };
 
 // The kernel of a call: family (EVOK_OBJ_KERNEL_*) and sym; stored samples when X is given; the vectorised variant when
 // D % 4 == 0 and every operand read or written with float4 loads / stores is 16-byte aligned with 16-byte aligned rows (mu and
-// sigma are null for the evaluation kernel, which reads X only).
+// sigma are null for the evaluation kernel, which reads X only) in every item: `item_strides` is the bitwise OR of the item
+// strides of the batched family (0 for one item), a multiple of 4 when each of them is.
 static KernelChoice choose_kernel(int family, bool sym, const float* X, int64_t ldx, const float* mu, const float* sigma, int64_t n_rows,
-                                  int64_t D) {
+                                  int64_t D, int64_t item_strides = 0) {
   const bool store = X != nullptr;
-  const bool vec = (D % 4 == 0) && aligned16(mu) && aligned16(sigma) && (!store || (aligned16(X) && ldx % 4 == 0));
+  const bool vec = (D % 4 == 0) && aligned16(mu) && aligned16(sigma) && (!store || (aligned16(X) && ldx % 4 == 0)) && item_strides % 4 == 0;
   KernelChoice c;
   c.k = kernel_index(family, sym, store, vec);
   c.n_units = sym ? n_rows / 2 : n_rows;
@@ -220,24 +224,26 @@ static KernelChoice choose_kernel(int family, bool sym, const float* X, int64_t 
   return c;
 }
 
-// Launches kernel c.k of an objective on the current device with `args` in the kernel's parameter order, on as many CTAs as
-// stay resident but no more than the units need, and at least one (the push sampler with no rows still raises this rank's
-// flag).  A built-in kernel goes through the runtime, a registered one through the driver.
-static int launch(int objective, const KernelChoice& c, void** args, cudaStream_t st) {
+// Launches kernel c.k of an objective on the current device with `args` in the kernel's parameter order, for `items` items
+// (grid y, at most kMaxGridY), on as many CTAs per item as stay resident when the items share the device, but no more than the
+// units need, and at least one (the push sampler with no rows still raises this rank's flag).  A built-in kernel goes through
+// the runtime, a registered one through the driver.
+static int launch(int objective, const KernelChoice& c, void** args, cudaStream_t st, int64_t items = 1) {
   const DeviceKernels* d = nullptr;
-  const int rc = device_kernels(objective, &d);
+  const int rc = device_kernels(objective, image_of(c.k), &d);
   if (rc != 0) return rc;
-  int64_t g = (int64_t)d->per_sm[c.k] * d->sms;
+  int64_t g = (int64_t)d->per_sm[c.k] * d->sms / items;
   if (g > c.ctas_needed) g = c.ctas_needed;
   if (g < 1) g = 1;
   const int threads = kernel_threads(c.k);
-  if (d->module) {
-    const CUresult r = g_driver.launch(static_cast<CUfunction>(d->fn[c.k]), (unsigned)g, 1, 1, threads, 1, 1, 0, (CUstream)st, args, nullptr);
+  if (d->module[image_of(c.k)]) {
+    const CUresult r = g_driver.launch(static_cast<CUfunction>(d->fn[c.k]), (unsigned)g, (unsigned)items, 1, threads, 1, 1, 0, (CUstream)st, args,
+                                       nullptr);
     if (r != CUDA_SUCCESS) return (int)r;
     count_launches(1);
     return 0;
   }
-  cudaLaunchKernel(d->fn[c.k], dim3((unsigned)g), dim3(threads), args, 0, st);
+  cudaLaunchKernel(d->fn[c.k], dim3((unsigned)g, (unsigned)items), dim3(threads), args, 0, st);
   EVOK_CHECK_LAUNCH();
   return 0;
 }
@@ -286,8 +292,8 @@ extern "C" EVOK_API int evok_objective_register(const void* cubin, size_t bytes,
   const int n = g_user_count.load(std::memory_order_relaxed);
   if (n >= EVOK_OBJ_USER_CAPACITY) return EVOK_E_BADSIZE;
   Objective* obj = new Objective;
-  obj->image.assign(static_cast<const char*>(cubin), static_cast<const char*>(cubin) + bytes);
-  for (int k = 0; k < n_kernels; ++k) obj->names.emplace_back(kernel_names_host[k]);
+  obj->image[0].assign(static_cast<const char*>(cubin), static_cast<const char*>(cubin) + bytes);
+  for (int k = 0; k < n_kernels; ++k) obj->names[0].emplace_back(kernel_names_host[k]);
   g_user[n] = obj;
   g_user_count.store(n + 1, std::memory_order_release);
   *id_out_host = EVOK_OBJ_USER_BASE + n;
@@ -297,7 +303,21 @@ extern "C" EVOK_API int evok_objective_register(const void* cubin, size_t bytes,
 extern "C" EVOK_API int evok_objective_load(int objective) {
   if (!is_user(objective)) return EVOK_E_BADENUM;
   const DeviceKernels* d = nullptr;
-  return device_kernels(objective, &d);
+  return device_kernels(objective, 0, &d);
+}
+
+extern "C" EVOK_API int evok_objective_register_batched(int objective, const void* cubin, size_t bytes, const char* const* kernel_names_host,
+                                                        int n_kernels) {
+  if (!cubin || !kernel_names_host) return EVOK_E_NULLPTR;
+  if (bytes == 0 || n_kernels != EVOK_OBJ_BATCHED_KERNELS) return EVOK_E_BADSIZE;
+  for (int k = 0; k < n_kernels; ++k)
+    if (!kernel_names_host[k]) return EVOK_E_NULLPTR;
+  if (!is_user(objective)) return EVOK_E_BADENUM;
+  std::lock_guard<std::mutex> lock(g_objective_mutex);
+  Objective& obj = *g_user[objective - EVOK_OBJ_USER_BASE];
+  obj.image[1].assign(static_cast<const char*>(cubin), static_cast<const char*>(cubin) + bytes);
+  obj.names[1].assign(kernel_names_host, kernel_names_host + n_kernels);
+  return 0;
 }
 
 extern "C" EVOK_API int evok_sample_eval(int objective, float* X, int64_t ldx, const float* mu, const float* sigma, int64_t row0,
@@ -351,6 +371,26 @@ extern "C" EVOK_API int evok_eval(int objective, const float* X, int64_t ldx, in
   return launch(objective, c, args, (cudaStream_t)stream);
 }
 
+// One launch per item chunk of the batched family: item b of the batch samples with stream word (stream_id0 + b), chunk b0 of
+// at most kMaxGridY items (grid y) starting at stream word stream_lo + b0; f (null for EVOK_OBJ_NONE) is [items][n_rows].
+static int sample_items(int objective, float* X, int64_t item_stride_x, int64_t ldx, const float* mu, int64_t item_stride_mu, const float* sigma,
+                        int64_t item_stride_sigma, int64_t n_items, int64_t n_rows, int64_t D, bool sym, uint64_t seed, uint64_t stream_id0, float* f,
+                        cudaStream_t st) {
+  KernelChoice c = choose_kernel(EVOK_OBJ_KERNEL_BATCHED, sym, X, ldx, mu, sigma, n_rows, D,
+                                 (X ? item_stride_x : 0) | item_stride_mu | item_stride_sigma);
+  const PhiloxKey key = make_philox_key(seed, stream_id0);
+  return for_item_chunks(n_items, kMaxGridY, [&](int64_t b0, int64_t nb) {
+    PhiloxKey kc = key;
+    kc.stream_lo += (uint32_t)b0;
+    float* Xc = X ? X + b0 * item_stride_x : nullptr;
+    const float* muc = mu + b0 * item_stride_mu;
+    const float* sgc = sigma + b0 * item_stride_sigma;
+    float* fc = f ? f + b0 * n_rows : nullptr;
+    void* args[] = {&Xc, &item_stride_x, &ldx, &muc, &item_stride_mu, &sgc, &item_stride_sigma, &c.n_units, &D, &kc, &fc};
+    return launch(objective, c, args, st, nb);
+  });
+}
+
 extern "C" EVOK_API int evok_sample_batched(float* X, int64_t item_stride_x, int64_t ldx, const float* mu, int64_t item_stride_mu, const float* sigma,
                                             int64_t item_stride_sigma, int64_t n_items, int64_t n_rows, int64_t D, int symmetric, uint64_t seed,
                                             uint64_t stream_id0, void* stream) {
@@ -359,37 +399,31 @@ extern "C" EVOK_API int evok_sample_batched(float* X, int64_t item_stride_x, int
     return EVOK_E_BADSIZE;
   if (symmetric && (n_rows & 1)) return EVOK_E_ODDROWS;
   if (n_items == 0 || n_rows == 0) return 0;
-  const int64_t n_units = symmetric ? n_rows / 2 : n_rows;
-  const bool vec = (D % 4 == 0) && aligned16(mu) && aligned16(sigma) && aligned16(X) && ldx % 4 == 0 && item_stride_x % 4 == 0 &&
-                   item_stride_mu % 4 == 0 && item_stride_sigma % 4 == 0;
-  int64_t ctas = (n_units + (kSampleThreads / 32) - 1) / (kSampleThreads / 32);
-  const DeviceKernels* d = nullptr;
-  const int rc = device_kernels(EVOK_OBJ_NONE, &d);
-  if (rc != 0) return rc;
-  const int64_t cap = ((int64_t)d->sms * 8 + n_items - 1) / n_items;  // about 8 CTAs per SM over all items
-  if (ctas > cap) ctas = cap < 1 ? 1 : cap;
-  const PhiloxKey key = make_philox_key(seed, stream_id0);
-  cudaStream_t st = (cudaStream_t)stream;
-  // grid y is at most kMaxGridY items: larger batches go in item chunks, chunk b0 starting at stream word stream_lo + b0, so item b
-  // keeps its Philox stream stream_id0 + b
-  return for_item_chunks(n_items, kMaxGridY, [&](int64_t b0, int64_t nb) {
-    PhiloxKey kc = key;
-    kc.stream_lo += (uint32_t)b0;
-    const dim3 grid((unsigned)ctas, (unsigned)nb);
-    float* Xc = X + b0 * item_stride_x;
-    const float* muc = mu + b0 * item_stride_mu;
-    const float* sgc = sigma + b0 * item_stride_sigma;
-#define EVOK_LAUNCH_SB(SYMV, VECV) \
-  sample_batched_kernel<SYMV, VECV><<<grid, kSampleThreads, 0, st>>>(Xc, item_stride_x, ldx, muc, item_stride_mu, sgc, item_stride_sigma, n_units, D, kc)
-    if (symmetric) {
-      if (vec) EVOK_LAUNCH_SB(true, true);
-      else EVOK_LAUNCH_SB(true, false);
-    } else {
-      if (vec) EVOK_LAUNCH_SB(false, true);
-      else EVOK_LAUNCH_SB(false, false);
-    }
-#undef EVOK_LAUNCH_SB
-    EVOK_CHECK_LAUNCH();
-    return 0;
-  });
+  return sample_items(EVOK_OBJ_NONE, X, item_stride_x, ldx, mu, item_stride_mu, sigma, item_stride_sigma, n_items, n_rows, D, symmetric != 0, seed,
+                      stream_id0, nullptr, (cudaStream_t)stream);
+}
+
+// The argument checks of evok_sample_eval_batched, in the order of include/evok.h.
+static int check_sample_batched(int objective, const float* X, int64_t item_stride_x, int64_t ldx, const float* mu, int64_t item_stride_mu,
+                                const float* sigma, int64_t item_stride_sigma, int64_t n_items, int64_t n_rows, int64_t D, bool sym, const float* f) {
+  if (!mu || !sigma || !f) return EVOK_E_NULLPTR;
+  if ((objective <= EVOK_OBJ_NONE || objective >= EVOK_OBJ_COUNT) && !is_user(objective)) return EVOK_E_BADENUM;
+  if (n_items < 0 || n_rows < 0 || D <= 0 || (X && (ldx < D || item_stride_x < 0)) || item_stride_mu < 0 || item_stride_sigma < 0)
+    return EVOK_E_BADSIZE;
+  if (sym && (n_rows & 1)) return EVOK_E_ODDROWS;
+  if (is_user(objective)) {  // a registered id samples batched only with its batched image: nothing is launched without it
+    std::lock_guard<std::mutex> lock(g_objective_mutex);
+    if (g_user[objective - EVOK_OBJ_USER_BASE]->image[1].empty()) return EVOK_E_NOKERNEL;
+  }
+  return 0;
+}
+
+extern "C" EVOK_API int evok_sample_eval_batched(int objective, float* X, int64_t item_stride_x, int64_t ldx, const float* mu, int64_t item_stride_mu,
+                                                 const float* sigma, int64_t item_stride_sigma, int64_t n_items, int64_t n_rows, int64_t D,
+                                                 int symmetric, uint64_t seed, uint64_t stream_id0, float* f, void* stream) {
+  const int rc = check_sample_batched(objective, X, item_stride_x, ldx, mu, item_stride_mu, sigma, item_stride_sigma, n_items, n_rows, D,
+                                      symmetric != 0, f);
+  if (rc != 0 || n_items == 0 || n_rows == 0) return rc;
+  return sample_items(objective, X, item_stride_x, ldx, mu, item_stride_mu, sigma, item_stride_sigma, n_items, n_rows, D, symmetric != 0, seed,
+                      stream_id0, f, (cudaStream_t)stream);
 }

@@ -378,6 +378,70 @@ __device__ __forceinline__ void sample_group_pairs(const PhiloxKey& key, uint32_
   if (SYM) fold_pairs<4>(accm, n, j, n_valid, carry_m);
 }
 
+// One unit u (a direction of symmetric sampling, else a row) of the warp of lane `lane`: sample its row(s) from (key, stream word sw, unit
+// unit0 + u), store them at row r = (SYM ? 2u : u) of X when STORE, fold them into the objective and store the fitness at f[r]
+// (or, PUSH, at row0 + r of every peer's vector); SQ: q_out[r] = sum of z^2.  The body of sample_eval_kernel and of
+// sample_eval_batched_kernel, so both give the same bits for the same operands and counters.
+template <typename Acc, bool SYM, bool STORE, bool VEC, bool PUSH, bool SQ>
+__device__ __forceinline__ void sample_eval_unit(int lane, float* __restrict__ X, int64_t ldx, const float* __restrict__ mu,
+                                                 const float* __restrict__ sigma, int64_t row0, int64_t u, int64_t D, const PhiloxKey& key, uint32_t sw,
+                                                 uint32_t nq, uint64_t unit0, float* __restrict__ f, const PeerSink& sink, float* __restrict__ q_out) {
+  Acc accp(D), accm(D);
+  const int64_t r = SYM ? 2 * u : u;
+  float* xp = STORE ? X + r * ldx : nullptr;
+  float* xm = STORE ? xp + ldx : nullptr;
+  const uint64_t unit = unit0 + (uint64_t)u;
+  constexpr int kSampleUnroll = SampleTune<Acc>::kUnroll;
+  float zsq = 0.f;
+  if constexpr (PairTerms<Acc>::value) {
+    // warp-uniform steps of 32 groups (fold_pairs shuffles); each lane still visits its groups lane, lane + 32, ... in
+    // increasing order, the order of the loops below and of eval_kernel
+    float carry_p = 0.f, carry_m = 0.f;
+    uint32_t b = 0;
+    for (; b + 32u * kSampleUnroll <= nq; b += 32u * kSampleUnroll) {
+#pragma unroll
+      for (int uu = 0; uu < kSampleUnroll; ++uu)
+        sample_group_pairs<Acc, SYM, STORE, VEC, SQ>(key, sw, unit, b + 32u * uu + lane, D, mu, sigma, xp, xm, accp, accm, &zsq, true,
+                                                     carry_p, carry_m);
+    }
+    for (; b < nq; b += 32)
+      sample_group_pairs<Acc, SYM, STORE, VEC, SQ>(key, sw, unit, b + lane, D, mu, sigma, xp, xm, accp, accm, &zsq, b + lane < nq,
+                                                   carry_p, carry_m);
+  } else {
+    uint32_t q = lane;
+    if (kSampleUnroll > 1) {
+      // independent Philox chains in flight per lane
+      for (; q + 32u * (kSampleUnroll - 1) < nq; q += 32u * kSampleUnroll) {
+#pragma unroll
+        for (int uu = 0; uu < kSampleUnroll; ++uu)
+          sample_group<Acc, SYM, STORE, VEC, SQ>(key, sw, unit, q + 32u * uu, D, mu, sigma, xp, xm, accp, accm, &zsq);
+      }
+    }
+    for (; q < nq; q += 32) sample_group<Acc, SYM, STORE, VEC, SQ>(key, sw, unit, q, D, mu, sigma, xp, xm, accp, accm, &zsq);
+  }
+  if (SQ) {
+    zsq = warp_sum(zsq);
+    if (lane == 0) q_out[r] = zsq;
+  }
+  if (!SampleOnly<Acc>::value) {
+    const float fp = accp.finish(D);
+    float fm = 0.f;
+    if (SYM) fm = accm.finish(D);
+    if (lane == 0) {
+      if (PUSH) {
+        for (int p = 0; p < sink.world; ++p) {
+          float* fr = static_cast<float*>(sink.data[p]) + row0 + r;
+          fr[0] = fp;
+          if (SYM) fr[1] = fm;
+        }
+      } else {
+        f[r] = fp;
+        if (SYM) f[r + 1] = fm;
+      }
+    }
+  }
+}
+
 // PUSH: the fitness of row i goes to row (row0 + i) of EVERY peer's fitness vector (the all-gather of the sharded
 // generation, fused into the producer) and the last CTA raises this rank's flag on every peer.
 // SQ (non-symmetric only): q[r] = sum_j z_rj^2 of the unscaled normals, accumulated in registers next to the objective.
@@ -395,63 +459,33 @@ __global__ void __launch_bounds__(kSampleThreads, SampleTune<Acc>::kMinBlocks)
   const uint32_t nq = (uint32_t)((D + 3) >> 2);
   const uint64_t unit0 = (uint64_t)(SYM ? (row0 >> 1) : row0);
 
-  for (int64_t u = gw; u < n_units; u += warps_total) {
-    Acc accp(D), accm(D);
-    const int64_t r = SYM ? 2 * u : u;
-    float* xp = STORE ? X + r * ldx : nullptr;
-    float* xm = STORE ? xp + ldx : nullptr;
-    const uint64_t unit = unit0 + (uint64_t)u;
-    constexpr int kSampleUnroll = SampleTune<Acc>::kUnroll;
-    float zsq = 0.f;
-    if constexpr (PairTerms<Acc>::value) {
-      // warp-uniform steps of 32 groups (fold_pairs shuffles); each lane still visits its groups lane, lane + 32, ... in
-      // increasing order, the order of the loops below and of eval_kernel
-      float carry_p = 0.f, carry_m = 0.f;
-      uint32_t b = 0;
-      for (; b + 32u * kSampleUnroll <= nq; b += 32u * kSampleUnroll) {
-#pragma unroll
-        for (int uu = 0; uu < kSampleUnroll; ++uu)
-          sample_group_pairs<Acc, SYM, STORE, VEC, SQ>(key, sw, unit, b + 32u * uu + lane, D, mu, sigma, xp, xm, accp, accm, &zsq, true,
-                                                       carry_p, carry_m);
-      }
-      for (; b < nq; b += 32)
-        sample_group_pairs<Acc, SYM, STORE, VEC, SQ>(key, sw, unit, b + lane, D, mu, sigma, xp, xm, accp, accm, &zsq, b + lane < nq,
-                                                     carry_p, carry_m);
-    } else {
-      uint32_t q = lane;
-      if (kSampleUnroll > 1) {
-        // independent Philox chains in flight per lane
-        for (; q + 32u * (kSampleUnroll - 1) < nq; q += 32u * kSampleUnroll) {
-#pragma unroll
-          for (int uu = 0; uu < kSampleUnroll; ++uu)
-            sample_group<Acc, SYM, STORE, VEC, SQ>(key, sw, unit, q + 32u * uu, D, mu, sigma, xp, xm, accp, accm, &zsq);
-        }
-      }
-      for (; q < nq; q += 32) sample_group<Acc, SYM, STORE, VEC, SQ>(key, sw, unit, q, D, mu, sigma, xp, xm, accp, accm, &zsq);
-    }
-    if (SQ) {
-      zsq = warp_sum(zsq);
-      if (lane == 0) q_out[r] = zsq;
-    }
-    if (!SampleOnly<Acc>::value) {
-      const float fp = accp.finish(D);
-      float fm = 0.f;
-      if (SYM) fm = accm.finish(D);
-      if (lane == 0) {
-        if (PUSH) {
-          for (int p = 0; p < sink.world; ++p) {
-            float* fr = static_cast<float*>(sink.data[p]) + row0 + r;
-            fr[0] = fp;
-            if (SYM) fr[1] = fm;
-          }
-        } else {
-          f[r] = fp;
-          if (SYM) f[r + 1] = fm;
-        }
-      }
-    }
-  }
+  for (int64_t u = gw; u < n_units; u += warps_total)
+    sample_eval_unit<Acc, SYM, STORE, VEC, PUSH, SQ>(lane, X, ldx, mu, sigma, row0, u, D, key, sw, nq, unit0, f, sink, q_out);
   if (PUSH) peer_signal_tail(sink, epoch, done);
+}
+
+// Batched searches (the functional ask / tell API with leading batch dimensions): blockIdx.y = item b of the launch.  Every
+// item has its own X, mu and sigma at an item stride (0 = the operand is shared by all items), its fitnesses at row b of
+// f [items][n_rows], and its own Philox stream word key.stream_lo + b, so one launch samples and evaluates the populations of
+// all items, bit-identical to one sample_eval_kernel launch per item with stream id (stream id of the key) + b.
+template <typename Acc, bool SYM, bool STORE, bool VEC>
+__global__ void __launch_bounds__(kSampleThreads, SampleTune<Acc>::kMinBlocks)
+    sample_eval_batched_kernel(float* __restrict__ X, int64_t item_stride_x, int64_t ldx, const float* __restrict__ mu, int64_t item_stride_mu,
+                               const float* __restrict__ sigma, int64_t item_stride_sigma, int64_t n_units, int64_t D,
+                               const __grid_constant__ PhiloxKey key, float* __restrict__ f) {
+  const int lane = threadIdx.x & 31;
+  const int64_t item = blockIdx.y;
+  if (STORE) X += item * item_stride_x;
+  mu += item * item_stride_mu;
+  sigma += item * item_stride_sigma;
+  if (!SampleOnly<Acc>::value) f += item * (SYM ? 2 * n_units : n_units);
+  const uint32_t sw = key.stream_lo + (uint32_t)item;
+  const int64_t warps_total = (int64_t)gridDim.x * (kSampleThreads / 32);
+  const int64_t gw = (int64_t)blockIdx.x * (kSampleThreads / 32) + (threadIdx.x >> 5);
+  const uint32_t nq = (uint32_t)((D + 3) >> 2);
+  const PeerSink no_sink{};
+  for (int64_t u = gw; u < n_units; u += warps_total)
+    sample_eval_unit<Acc, SYM, STORE, VEC, false, false>(lane, X, ldx, mu, sigma, 0, u, D, key, sw, nq, 0, f, no_sink, nullptr);
 }
 
 constexpr int kEvalThreads = 256;

@@ -242,7 +242,17 @@ def kernel_expressions() -> list:
     return out
 
 
+def batched_kernel_expressions() -> list:
+    """The 8 batched samplers of a registered objective, in the order of EVOK_OBJ_KERNEL_BATCHED + 4 sym + 2 store + vec of
+    include/evok.h (kernel_index in csrc/evok_sample_eval.cu computes the same positions).  They are compiled from the same
+    source as `kernel_expressions`, as a second image, on the first batched use (`compile_batched`)."""
+    b = lambda v: "true" if v else "false"  # noqa: E731
+    return [f"evok::sample_eval_batched_kernel<evok_user::Acc, {b(sym)}, {b(store)}, {b(vec)}>"
+            for sym in (False, True) for store in (False, True) for vec in (False, True)]
+
+
 N_KERNELS = 22
+N_BATCHED_KERNELS = 8
 # -default-device: the declarations of the C ABI in include/evok.h (reached through evok_sampler.cuh) are unannotated
 NVRTC_OPTIONS = ("--gpu-architecture=sm_90a", "-std=c++17", "--fmad=true", "--ptxas-options=-v", "-default-device", f"-I{CSRC}",
                  f"-I{INCLUDE}")
@@ -373,7 +383,14 @@ def register(cubin: bytes, names: list) -> int:
     return out.value
 
 
+def register_batched(objective_id: int, cubin: bytes, names: list) -> None:
+    """evok_objective_register_batched: attach the batched kernels (in `batched_kernel_expressions` order) to a registered id."""
+    arr = (c_char_p * len(names))(*[n.encode() for n in names])
+    nat.check(nat.lib().evok_objective_register_batched(objective_id, cubin, len(cubin), arr, len(names)), "evok_objective_register_batched")
+
+
 _cache: Dict[str, CompiledObjective] = {}
+_batched_cache: Dict[str, CompiledObjective] = {}
 _cache_lock = threading.Lock()
 
 
@@ -385,4 +402,17 @@ def compile_objective(spec: ObjectiveSpec) -> CompiledObjective:
             c = compile_source(spec.source)
             c.objective_id = register(c.cubin, c.names)
             _cache[spec.source] = c
+        return c
+
+
+def compile_batched(spec: ObjectiveSpec) -> CompiledObjective:
+    """Compile the batched samplers of `spec` and attach them to its registered id, once per process for one generated source."""
+    base = compile_objective(spec)
+    with _cache_lock:
+        c = _batched_cache.get(spec.source)
+        if c is None:
+            c = compile_source(spec.source, batched_kernel_expressions())
+            register_batched(base.objective_id, c.cubin, c.names)
+            c.objective_id = base.objective_id
+            _batched_cache[spec.source] = c
         return c

@@ -68,7 +68,10 @@ class FusedObjective(BuiltinObjective):
     `sums` maps each sum's name to its term (an expression of x, xn, j and D), `value` is an expression of the sums and D; the
     language is described in evotorch_b200.jit.  Construction parses both (ValueError for anything outside the language),
     compiles the kernels with NVRTC for sm_90a and registers them with libevok.so; `kernel_info` holds the registers and
-    spills of every kernel.  The same source compiles once per process.  A FusedObjective pickles as its expressions."""
+    spills of every kernel.  The same source compiles once per process.  A FusedObjective pickles as its expressions.
+
+    The batched samplers of the functional API (`pgpe_ask_and_evaluate`, `cem_ask_and_evaluate`) are 8 more kernels of the same
+    source, compiled on the first batched use (`compile_batched`); `batched_kernel_info` then holds their registers and spills."""
 
     def __init__(self, name: str, sums: dict, value: str):
         from . import jit
@@ -80,7 +83,16 @@ class FusedObjective(BuiltinObjective):
         super().__init__(name, compiled.objective_id, spec.torch_fn)
         self.sums, self.value, self.source = dict(spec.sums), spec.value, spec.source
         self.kernel_info = compiled.kernel_info
+        self.batched_kernel_info = None
+        self._spec = spec
         ops.OBJECTIVE_IDS[name] = compiled.objective_id
+
+    def compile_batched(self) -> None:
+        """Compile and attach the batched samplers (once per process for one source); fills `batched_kernel_info`."""
+        if self.batched_kernel_info is None:
+            from . import jit
+
+            self.batched_kernel_info = jit.compile_batched(self._spec).kernel_info
 
     def __reduce__(self):
         return (FusedObjective, (self.name, self.sums, self.value))

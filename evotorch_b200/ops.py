@@ -541,6 +541,37 @@ def sample_batched(out: torch.Tensor, mu: torch.Tensor, sigma: torch.Tensor, *, 
     return out
 
 
+def sample_eval_batched(objective: int, X: Optional[torch.Tensor], mu: torch.Tensor, sigma: torch.Tensor, f: torch.Tensor, *, symmetric: bool,
+                        seed: int, stream_id0: int = 0) -> torch.Tensor:
+    """K1+K2 for every batch item in one launch: item b samples with Philox stream stream_id0 + b into X[b] (X = None: a lazy
+    population, evaluated and not stored) and writes its fitnesses to f[b].  X: (items, N, D) or None, f: (items, N), mu / sigma:
+    (D,) or (items, D).  Per item, X and f are the bits of `sample_eval(..., stream_id=stream_id0 + b)`.  A registered objective
+    needs its batched kernels (`FusedObjective.compile_batched`)."""
+    if objective == OBJ_NONE:
+        raise ValueError("objective: EVOK_OBJ_NONE only samples; use sample_batched")
+    if not (f.is_cuda and f.dtype == torch.float32 and f.ndim == 2):
+        raise ValueError("f: expected a contiguous float32 CUDA tensor of shape (items, popsize)")
+    B, n = f.shape
+    d = mu.shape[-1]
+    f = _rows(f, "f", (B, n))
+    if X is not None:
+        if not (X.is_cuda and X.dtype == torch.float32 and X.is_contiguous() and tuple(X.shape) == (B, n, d)):
+            raise ValueError(f"X: expected a contiguous float32 CUDA tensor of shape {(B, n, d)}")
+        X = as_plain_tensor(X)
+    mu, bm, sm = _items(mu, (d,), "mu")
+    sigma, bs, ss = _items(sigma, (d,), "sigma")
+    for cnt in (bm, bs):
+        if cnt is not None and cnt != B:
+            raise ValueError("mu / sigma: number of items differs from f")
+    if symmetric and n % 2:
+        raise ValueError(f"Symmetric sampling cannot be done if the number of solutions is odd: {n}")
+    with _timed("sample_eval"):
+        rc = nat.lib().evok_sample_eval_batched(objective, nat.ptr(X), n * d, d, mu.data_ptr(), sm, sigma.data_ptr(), ss, B, n, d, int(symmetric),
+                                                seed, stream_id0, f.data_ptr(), nat.stream_of(f))
+    nat.check(rc, "evok_sample_eval_batched")
+    return f
+
+
 def rank_batched(f: torch.Tensor, method: str, higher_is_better: bool) -> torch.Tensor:
     """Utilities of `items` independent fitness vectors, f: (items, N)."""
     if not (f.is_cuda and f.dtype == torch.float32 and f.ndim == 2):
@@ -591,6 +622,32 @@ def grad_batched(form: int, X: torch.Tensor, w: torch.Tensor, mu: torch.Tensor, 
         rc = lib.evok_grad_batched(form, X.data_ptr(), n * d, d, w.data_ptr(), mu.data_ptr(), sm, sigma.data_ptr(), ss, B, n, d, scale_mu, scale_sigma,
                                    out_mu.data_ptr(), out_sigma.data_ptr(), ws.data_ptr(), ws.numel(), nat.stream_of(X))
     nat.check(rc, "evok_grad_batched")
+    return out_mu, out_sigma
+
+
+def grad_batched_regen(form: int, w: torch.Tensor, mu: torch.Tensor, sigma: torch.Tensor, scale_mu: float, scale_sigma: float, *, seed: int,
+                       stream_id0: int = 0) -> tuple:
+    """`grad_batched` over the population that `sample_eval_batched` / `sample_batched` drew from these mu and sigma with this seed
+    and stream_id0, without reading it: the rows with a non-zero weight are rebuilt from their Philox counters.  Bit-identical to
+    `grad_batched` over the stored population.  w: (items, N), mu / sigma: (D,) or (items, D)."""
+    if not (w.is_cuda and w.dtype == torch.float32 and w.ndim == 2):
+        raise ValueError("w: expected a float32 CUDA tensor of shape (items, N)")
+    B, n = w.shape
+    w = _rows(w, "w", (B, n))
+    d = mu.shape[-1]
+    mu, bm, sm = _items(mu, (d,), "mu")
+    sigma, bs, ss = _items(sigma, (d,), "sigma")
+    for cnt in (bm, bs):
+        if cnt is not None and cnt != B:
+            raise ValueError("mu / sigma: number of items differs from w")
+    out_mu = torch.empty(B, d, dtype=torch.float32, device=w.device)
+    out_sigma = torch.empty_like(out_mu)
+    lib = nat.lib()
+    ws = nat.workspace(w.device, lib.evok_grad_batched_workspace_bytes(B, n, d), "grad_batched")
+    with _timed("grad_regen"):
+        rc = lib.evok_grad_batched_regen(form, w.data_ptr(), mu.data_ptr(), sm, sigma.data_ptr(), ss, B, n, d, seed, stream_id0, scale_mu,
+                                         scale_sigma, out_mu.data_ptr(), out_sigma.data_ptr(), ws.data_ptr(), ws.numel(), nat.stream_of(w))
+    nat.check(rc, "evok_grad_batched_regen")
     return out_mu, out_sigma
 
 

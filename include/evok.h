@@ -125,6 +125,20 @@ int evok_eval(int objective, const float* X, int64_t ldx, int64_t n_rows, int64_
 int evok_objective_register(const void* cubin, size_t bytes, const char* const* kernel_names_host, int n_kernels, int* id_out_host);
 int evok_objective_load(int objective);
 
+/* The batched sampler of an objective (evok_sample_eval_batched) is a second family of kernels, kept in a second image so
+ * that a registered objective that never runs batched searches compiles and loads only the EVOK_OBJ_KERNELS above:
+ *   EVOK_OBJ_KERNEL_BATCHED + 4 sym + 2 store + vec : sample_eval_batched_kernel<Acc, sym, store, vec>
+ * evok_objective_register_batched attaches the sm_90a cubin of these EVOK_OBJ_BATCHED_KERNELS kernels (lowered names in this
+ * order, positions counted from EVOK_OBJ_KERNEL_BATCHED) to the registered id `objective`.  It copies the image and the names
+ * and needs no device; the module is loaded on a device by the first batched call there.  Attaching again replaces the image
+ * for the devices that have not loaded it yet.  A registered id without a batched image yields EVOK_E_NOKERNEL from
+ * evok_sample_eval_batched, which then launches nothing.
+ * Errors: EVOK_E_NULLPTR, EVOK_E_BADSIZE (bytes == 0, n_kernels != EVOK_OBJ_BATCHED_KERNELS), EVOK_E_BADENUM (`objective` is
+ * a built-in id or is not registered). */
+#define EVOK_OBJ_KERNEL_BATCHED 22
+#define EVOK_OBJ_BATCHED_KERNELS 8
+int evok_objective_register_batched(int objective, const void* cubin, size_t bytes, const char* const* kernel_names_host, int n_kernels);
+
 /* ---------------------------------------------------------------------------------------------
  * K3: fitness -> utilities.  Replaces tools/ranking.py:24-183 (`rank` :189).
  * Sort semantics: STABLE (equal fitnesses keep ascending index order), -0 == +0, NaN largest;
@@ -313,10 +327,22 @@ int evok_transpose_pair(const float* in, int64_t ldi, int64_t rows, int64_t cols
  * stride is given (stride 0 = the operand is shared by all items).  Per-item scalar hyper-parameters are HOST arrays (they travel in
  * the launch parameters).  Every stage computes exactly what its single-search entry point computes per item.
  * --------------------------------------------------------------------------------------------- */
-/* K1: item b draws with Philox stream (stream_id0 + b): same bits as evok_sample_eval(..., stream_id = stream_id0 + b) per item */
+/* K1: item b draws with Philox stream (stream_id0 + b): same bits as evok_sample_eval(..., stream_id = stream_id0 + b) per item.
+ * Launches the EVOK_OBJ_NONE kernels of the batched family (grid y = item, grid x = the resident CTAs of the kernel shared over
+ * the items of a launch, at least 1 and at most what the rows need). */
 int evok_sample_batched(float* X, int64_t item_stride_x, int64_t ldx, const float* mu, int64_t item_stride_mu, const float* sigma,
                         int64_t item_stride_sigma, int64_t n_items, int64_t n_rows, int64_t D, int symmetric, uint64_t seed, uint64_t stream_id0,
                         void* stream);
+/* K1+K2 for a batch of searches in one launch per 65535 items: item b samples with Philox stream (stream_id0 + b) and writes its
+ * n_rows fitnesses to f[b * n_rows ...] (f: [items][n_rows], contiguous).  For every item, X and f are bit-identical to
+ * evok_sample_eval(objective, ..., row0 = 0, stream_id = stream_id0 + b) on that item's operands, and X to evok_sample_batched.
+ * objective: a built-in id other than EVOK_OBJ_NONE (which goes through evok_sample_batched), or a registered id with a batched
+ * image (evok_objective_register_batched; else EVOK_E_NOKERNEL).  X may be NULL: a lazy population, evaluated and not stored
+ * (evok_grad_batched_regen rebuilds the rows its gradient needs).  Errors in this order: EVOK_E_NULLPTR (mu, sigma, f),
+ * EVOK_E_BADENUM, EVOK_E_BADSIZE (negative counts or strides, D <= 0, ldx < D with X), EVOK_E_ODDROWS, EVOK_E_NOKERNEL. */
+int evok_sample_eval_batched(int objective, float* X, int64_t item_stride_x, int64_t ldx, const float* mu, int64_t item_stride_mu,
+                             const float* sigma, int64_t item_stride_sigma, int64_t n_items, int64_t n_rows, int64_t D, int symmetric,
+                             uint64_t seed, uint64_t stream_id0, float* f, void* stream);
 /* K3: f, w: [items][N].  ws: max(evok_rank_workspace_bytes(N), 8 * min(n_items, 65535) + 256) bytes */
 int evok_rank_batched(int method, const float* f, int64_t N, int64_t n_items, int higher_is_better, float* w, void* ws, size_t ws_bytes,
                       void* stream);
@@ -327,6 +353,14 @@ size_t evok_grad_batched_workspace_bytes(int64_t n_items, int64_t n_rows, int64_
 int evok_grad_batched(int form, const float* X, int64_t item_stride_x, int64_t ldx, const float* w, const float* mu, int64_t item_stride_mu,
                       const float* sigma, int64_t item_stride_sigma, int64_t n_items, int64_t n_rows, int64_t D, float scale_mu, float scale_sigma,
                       float* out_mu, float* out_sigma, void* ws, size_t ws_bytes, void* stream);
+/* K4 over the population that evok_sample_eval_batched / evok_sample_batched drew from these mu and sigma with this (seed,
+ * stream_id0), without reading it: every row with a non-zero weight is rebuilt from its Philox counters as
+ * x = fmaf(sigma, z, mu) (item b on stream stream_id0 + b) and eps = x - mu, with the plan and workspace of evok_grad_batched.
+ * The result is bit-identical to evok_grad_batched over the contiguous, 16-byte aligned X [items][n_rows][D] that the sampler
+ * would have written.  Errors as evok_grad_batched, and EVOK_E_BADSIZE for a negative item stride. */
+int evok_grad_batched_regen(int form, const float* w, const float* mu, int64_t item_stride_mu, const float* sigma, int64_t item_stride_sigma,
+                            int64_t n_items, int64_t n_rows, int64_t D, uint64_t seed, uint64_t stream_id0, float scale_mu, float scale_sigma,
+                            float* out_mu, float* out_sigma, void* ws, size_t ws_bytes, void* stream);
 /* K5: g, velocity, center [items][D]; center += step.  sigma, g, lb / ub / mc vectors (nullable) [items][D] */
 int evok_clipup_batched(const float* g, int64_t n_items, int64_t D, float* velocity, float* center, const float* stepsize_host,
                         const float* momentum_host, const float* max_speed_host, void* stream);
