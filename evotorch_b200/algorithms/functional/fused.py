@@ -3,6 +3,10 @@ fused kernel (`evok_objective_id`: the built-in objectives and every `FusedObjec
 drawn and evaluated in one launch of the batched sampler, which writes the population once and never reads it back for the
 evaluation.  With `lazy=True` the population is not stored at all: the tell rebuilds the rows its gradient needs from their
 Philox counters (`LazyPopulation`).
+
+A `FusedObjective` whose data tensors have batch dimensions gives every batch item its own data, so one launch solves as many
+problem instances as it has items.  The batch shape of the data is then the batch shape of the populations and fitnesses: the
+centre and stdev are broadcast to it (`data_batch`).
 """
 
 from __future__ import annotations
@@ -76,10 +80,27 @@ def fused_objective_id(objective: Callable, center: torch.Tensor, stdev: torch.T
     return int(oid)
 
 
+def data_batch(objective: Callable, batch: torch.Size) -> torch.Size:
+    """The batch shape of a search whose centre and stdev have batch shape `batch` on `objective`: `batch` itself, or for an
+    objective with per-item data the batch shape of the data, to which `batch` must broadcast (ValueError naming both if not)."""
+    per_item = getattr(objective, "data_batch_shape", torch.Size())
+    if not per_item:
+        return batch
+    try:
+        ok = tuple(torch.broadcast_shapes(batch, per_item)) == tuple(per_item)
+    except RuntimeError:
+        ok = False
+    if not ok:
+        raise ValueError(f"the batch shape {tuple(batch)} of the centre and stdev does not broadcast to the batch shape {tuple(per_item)} "
+                         f"of the data of {objective!r}")
+    return per_item
+
+
 def ask_and_evaluate(ask: Callable, center: torch.Tensor, stdev: torch.Tensor, popsize: int, symmetric: bool, objective: Callable,
                      lazy: bool) -> tuple:
     """(population, fitnesses) of one ask: fused when `fused_objective_id` applies, else `ask()` followed by `objective`."""
     oid = fused_objective_id(objective, center, stdev)
+    batch = data_batch(objective, batch_shape_of((center, 1), (stdev, 1)))
     if oid is None:
         if lazy:
             oid = getattr(objective, "evok_objective_id", None)
@@ -87,8 +108,7 @@ def ask_and_evaluate(ask: Callable, center: torch.Tensor, stdev: torch.Tensor, p
                    if oid is None or oid == ops.OBJ_NONE else "the centre and stdev are not float32 CUDA tensors")
             raise ValueError(f"lazy=True needs the fused sampler, which does not apply here: {why}")
         values = ask()
-        return values, objective(values)
-    batch = batch_shape_of((center, 1), (stdev, 1))
+        return values.expand(tuple(batch) + values.shape[-2:]), objective(values)
     d = center.shape[-1]
     popsize = int(popsize)
     if symmetric and popsize % 2 != 0:

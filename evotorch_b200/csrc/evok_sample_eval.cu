@@ -98,7 +98,18 @@ struct Objective {
   // evok_objective_register, [1] (the batched family, empty until attached) from evok_objective_register_batched
   std::vector<char> image[2];
   std::vector<std::string> names[2];
+  // evok_objective_declare_data: the data names of its accumulator (0: none) and which of them are vectors of the row length
+  int n_data = 0;
+  bool is_vector[EVOK_MAX_DATA] = {};
   DeviceKernels dev[kMaxDevices];
+};
+
+// An instance of a registered objective with data (evok_objective_instance): the kernels of `base`, its own binding.
+struct Instance {
+  int base = -1;  // -1: the slot is free
+  const float* p[EVOK_MAX_DATA] = {};
+  int64_t len[EVOK_MAX_DATA] = {}, stride[EVOK_MAX_DATA] = {};
+  int64_t n_items = 1;
 };
 
 // the driver API through the runtime's entry points (the library does not link libcuda)
@@ -136,8 +147,58 @@ static Objective g_builtin[EVOK_OBJ_COUNT];
 static Objective* g_user[EVOK_OBJ_USER_CAPACITY];
 static std::atomic<int> g_user_count{0};
 
+static std::vector<Instance> g_instances;  // slot i is the id EVOK_OBJ_INSTANCE_BASE + i; guarded by g_objective_mutex
+static std::vector<int> g_free_instances;
+
 static bool is_user(int objective) {
   return objective >= EVOK_OBJ_USER_BASE && objective - EVOK_OBJ_USER_BASE < g_user_count.load(std::memory_order_acquire);
+}
+
+// the live instance of an id, else null; call with g_objective_mutex held
+static const Instance* instance_of(int objective) {
+  const int64_t slot = (int64_t)objective - EVOK_OBJ_INSTANCE_BASE;
+  return slot >= 0 && slot < (int64_t)g_instances.size() && g_instances[slot].base >= 0 ? &g_instances[slot] : nullptr;
+}
+
+// The id whose kernels `objective` launches: the base of a live instance, else `objective` itself (an id that is neither an
+// instance nor an objective then fails the enum check of its entry point).
+static int base_of(int objective) {
+  if (objective < EVOK_OBJ_INSTANCE_BASE) return objective;
+  std::lock_guard<std::mutex> lock(g_objective_mutex);
+  const Instance* inst = instance_of(objective);
+  return inst ? inst->base : objective;
+}
+
+// The data of one call: the kernels' last argument, the id that holds the kernels, and whether every vector allows the 16-byte
+// loads of the vectorised kernels (its base 16-byte aligned, its item stride a multiple of 4).
+struct LaunchData {
+  DataBinding binding{};
+  int base = 0;
+  bool vec_ok = true;
+};
+
+// The data checks of a call with row length D on `items` items (0: an entry point that is not batched), after the entry point's
+// own checks: EVOK_E_NODATA for an objective that declares data and is not launched through an instance; EVOK_E_BADSIZE for a
+// vector whose length is not D, and for a per-item binding on a non-batched entry or on another number of items.
+static int bind_data(int objective, int64_t D, int64_t items, LaunchData* out) {
+  out->base = objective;
+  if (objective < EVOK_OBJ_USER_BASE) return 0;
+  std::lock_guard<std::mutex> lock(g_objective_mutex);
+  const Instance* inst = instance_of(objective);
+  if (!inst) return is_user(objective) && g_user[objective - EVOK_OBJ_USER_BASE]->n_data > 0 ? EVOK_E_NODATA : 0;
+  const Objective& obj = *g_user[inst->base - EVOK_OBJ_USER_BASE];
+  out->base = inst->base;
+  if (inst->n_items > 1 && items != inst->n_items) return EVOK_E_BADSIZE;
+  for (int i = 0; i < obj.n_data; ++i) {
+    const int64_t stride = inst->n_items > 1 ? inst->stride[i] : 0;
+    if (obj.is_vector[i]) {
+      if (inst->len[i] != D) return EVOK_E_BADSIZE;
+      if (!aligned16(inst->p[i]) || stride % 4 != 0) out->vec_ok = false;
+    }
+    out->binding.p[i] = inst->p[i];
+    out->binding.item_stride[i] = stride;
+  }
+  return 0;
 }
 
 static void fill_builtin(int objective, int dev, DeviceKernels& d) {
@@ -211,11 +272,13 @@ struct KernelChoice {
 // The kernel of a call: family (EVOK_OBJ_KERNEL_*) and sym; stored samples when X is given; the vectorised variant when
 // D % 4 == 0 and every operand read or written with float4 loads / stores is 16-byte aligned with 16-byte aligned rows (mu and
 // sigma are null for the evaluation kernel, which reads X only) in every item: `item_strides` is the bitwise OR of the item
-// strides of the batched family (0 for one item), a multiple of 4 when each of them is.
+// strides of the batched family (0 for one item), a multiple of 4 when each of them is.  The data vectors of an objective are
+// such operands too (data.vec_ok): one that is not aligned sends the whole call to the scalar-column kernels.
 static KernelChoice choose_kernel(int family, bool sym, const float* X, int64_t ldx, const float* mu, const float* sigma, int64_t n_rows,
-                                  int64_t D, int64_t item_strides = 0) {
+                                  int64_t D, const LaunchData& data, int64_t item_strides = 0) {
   const bool store = X != nullptr;
-  const bool vec = (D % 4 == 0) && aligned16(mu) && aligned16(sigma) && (!store || (aligned16(X) && ldx % 4 == 0)) && item_strides % 4 == 0;
+  const bool vec = (D % 4 == 0) && aligned16(mu) && aligned16(sigma) && (!store || (aligned16(X) && ldx % 4 == 0)) && item_strides % 4 == 0 &&
+                   data.vec_ok;
   KernelChoice c;
   c.k = kernel_index(family, sym, store, vec);
   c.n_units = sym ? n_rows / 2 : n_rows;
@@ -224,7 +287,8 @@ static KernelChoice choose_kernel(int family, bool sym, const float* X, int64_t 
   return c;
 }
 
-// Launches kernel c.k of an objective on the current device with `args` in the kernel's parameter order, for `items` items
+// Launches kernel c.k of an objective on the current device with `args` in the kernel's parameter order (the last one is the
+// data binding, which a kernel without data terms takes as an empty struct), for `items` items
 // (grid y, at most kMaxGridY), on as many CTAs per item as stay resident when the items share the device, but no more than the
 // units need, and at least one (the push sampler with no rows still raises this rank's flag).  A built-in kernel goes through
 // the runtime, a registered one through the driver.
@@ -272,10 +336,12 @@ static int check_sample(int objective, const float* X, int64_t ldx, const float*
 static int sample(int objective, int family, float* X, int64_t ldx, const float* mu, const float* sigma, int64_t row0, int64_t n_rows,
                   int64_t D, bool sym, uint64_t seed, uint64_t stream_id, const uint32_t* stream_off, float* f, float* q, PushArgs push,
                   cudaStream_t st) {
-  KernelChoice c = choose_kernel(family, sym, X, ldx, mu, sigma, n_rows, D);
+  LaunchData data;
+  if (const int rc = bind_data(objective, D, 0, &data)) return rc;
+  KernelChoice c = choose_kernel(family, sym, X, ldx, mu, sigma, n_rows, D, data);
   PhiloxKey key = make_philox_key(seed, stream_id);
-  void* args[] = {&X, &ldx, &mu, &sigma, &row0, &c.n_units, &D, &key, &stream_off, &f, &push.sink, &push.epoch, &push.done, &q};
-  return launch(objective, c, args, st);
+  void* args[] = {&X, &ldx, &mu, &sigma, &row0, &c.n_units, &D, &key, &stream_off, &f, &push.sink, &push.epoch, &push.done, &q, &data.binding};
+  return launch(data.base, c, args, st);
 }
 
 }  // namespace evok
@@ -301,6 +367,7 @@ extern "C" EVOK_API int evok_objective_register(const void* cubin, size_t bytes,
 }
 
 extern "C" EVOK_API int evok_objective_load(int objective) {
+  objective = base_of(objective);
   if (!is_user(objective)) return EVOK_E_BADENUM;
   const DeviceKernels* d = nullptr;
   return device_kernels(objective, 0, &d);
@@ -320,10 +387,62 @@ extern "C" EVOK_API int evok_objective_register_batched(int objective, const voi
   return 0;
 }
 
+extern "C" EVOK_API int evok_objective_declare_data(int objective, int n_data, const int* is_vector_host) {
+  if (!is_vector_host) return EVOK_E_NULLPTR;
+  if (!is_user(objective)) return EVOK_E_BADENUM;
+  if (n_data < 1 || n_data > EVOK_MAX_DATA) return EVOK_E_BADSIZE;
+  std::lock_guard<std::mutex> lock(g_objective_mutex);
+  Objective& obj = *g_user[objective - EVOK_OBJ_USER_BASE];
+  if (obj.n_data != 0) return EVOK_E_BADSIZE;
+  obj.n_data = n_data;
+  for (int i = 0; i < n_data; ++i) obj.is_vector[i] = is_vector_host[i] != 0;
+  return 0;
+}
+
+extern "C" EVOK_API int evok_objective_instance(int base, const float* const* ptrs_host, const int64_t* lens_host, const int64_t* item_strides_host,
+                                                int64_t n_items, int n_data, int* id_out_host) {
+  if (!ptrs_host || !lens_host || !item_strides_host || !id_out_host) return EVOK_E_NULLPTR;
+  if (!is_user(base)) return EVOK_E_BADENUM;
+  std::lock_guard<std::mutex> lock(g_objective_mutex);
+  const Objective& obj = *g_user[base - EVOK_OBJ_USER_BASE];
+  if (obj.n_data == 0) return EVOK_E_NODATA;
+  if (n_data != obj.n_data || n_items < 1) return EVOK_E_BADSIZE;
+  Instance inst;
+  for (int i = 0; i < n_data; ++i) {
+    if (!ptrs_host[i]) return EVOK_E_NULLPTR;
+    if (lens_host[i] < 1 || (lens_host[i] == 1) == obj.is_vector[i] || item_strides_host[i] < 0) return EVOK_E_BADSIZE;
+    inst.p[i] = ptrs_host[i];
+    inst.len[i] = lens_host[i];
+    inst.stride[i] = item_strides_host[i];
+  }
+  inst.base = base;
+  inst.n_items = n_items;
+  int slot;
+  if (!g_free_instances.empty()) {
+    slot = g_free_instances.back();
+    g_free_instances.pop_back();
+  } else {
+    if (g_instances.size() >= EVOK_OBJ_INSTANCE_CAPACITY) return EVOK_E_BADSIZE;
+    slot = (int)g_instances.size();
+    g_instances.emplace_back();
+  }
+  g_instances[slot] = inst;
+  *id_out_host = EVOK_OBJ_INSTANCE_BASE + slot;
+  return 0;
+}
+
+extern "C" EVOK_API int evok_objective_release(int id) {
+  std::lock_guard<std::mutex> lock(g_objective_mutex);
+  if (!instance_of(id)) return EVOK_E_BADENUM;
+  g_instances[id - EVOK_OBJ_INSTANCE_BASE] = Instance{};
+  g_free_instances.push_back(id - EVOK_OBJ_INSTANCE_BASE);
+  return 0;
+}
+
 extern "C" EVOK_API int evok_sample_eval(int objective, float* X, int64_t ldx, const float* mu, const float* sigma, int64_t row0,
                                 int64_t n_rows, int64_t D, int symmetric, uint64_t seed, uint64_t stream_id,
                                 const uint32_t* stream_offset_dev, float* f, void* stream) {
-  const int rc = check_sample(objective, X, ldx, mu, sigma, row0, n_rows, D, symmetric != 0, f, nullptr);
+  const int rc = check_sample(base_of(objective), X, ldx, mu, sigma, row0, n_rows, D, symmetric != 0, f, nullptr);
   if (rc != 0 || n_rows == 0) return rc;
   return sample(objective, EVOK_OBJ_KERNEL_SAMPLE, X, ldx, mu, sigma, row0, n_rows, D, symmetric != 0, seed, stream_id, stream_offset_dev, f,
                 nullptr, PushArgs{}, (cudaStream_t)stream);
@@ -333,7 +452,7 @@ extern "C" EVOK_API int evok_sample_eval_sq(int objective, float* X, int64_t ldx
                                             int64_t D, uint64_t seed, uint64_t stream_id, const uint32_t* stream_offset_dev, float* f, float* q,
                                             void* stream) {
   if (!q) return EVOK_E_NULLPTR;
-  const int rc = check_sample(objective, X, ldx, mu, sigma, row0, n_rows, D, false, f, nullptr);
+  const int rc = check_sample(base_of(objective), X, ldx, mu, sigma, row0, n_rows, D, false, f, nullptr);
   if (rc != 0 || n_rows == 0) return rc;
   return sample(objective, EVOK_OBJ_KERNEL_SQ, X, ldx, mu, sigma, row0, n_rows, D, false, seed, stream_id, stream_offset_dev, f, q, PushArgs{},
                 (cudaStream_t)stream);
@@ -349,7 +468,7 @@ extern "C" EVOK_API int evok_sample_eval_push(int objective, float* X, int64_t l
   push.sink.rank = rank;
   push.epoch = reinterpret_cast<const unsigned long long*>(epoch_dev);
   push.done = done_dev;
-  const int rc = check_sample(objective, X, ldx, mu, sigma, row0, n_rows, D, symmetric != 0, nullptr, &push);
+  const int rc = check_sample(base_of(objective), X, ldx, mu, sigma, row0, n_rows, D, symmetric != 0, nullptr, &push);
   if (rc != 0) return rc;
   for (int p = 0; p < world; ++p) {
     if (!peer_f[p] || !peer_flags[p]) return EVOK_E_NULLPTR;
@@ -363,20 +482,26 @@ extern "C" EVOK_API int evok_sample_eval_push(int objective, float* X, int64_t l
 
 extern "C" EVOK_API int evok_eval(int objective, const float* X, int64_t ldx, int64_t n_rows, int64_t D, float* f, void* stream) {
   if (!X || !f) return EVOK_E_NULLPTR;
-  if ((objective <= EVOK_OBJ_NONE || objective >= EVOK_OBJ_COUNT) && !is_user(objective)) return EVOK_E_BADENUM;
+  const int base = base_of(objective);
+  if ((base <= EVOK_OBJ_NONE || base >= EVOK_OBJ_COUNT) && !is_user(base)) return EVOK_E_BADENUM;
   if (n_rows < 0 || D <= 0 || ldx < D) return EVOK_E_BADSIZE;
   if (n_rows == 0) return 0;
-  const KernelChoice c = choose_kernel(EVOK_OBJ_KERNEL_EVAL, false, X, ldx, nullptr, nullptr, n_rows, D);
-  void* args[] = {&X, &ldx, &n_rows, &D, &f};
-  return launch(objective, c, args, (cudaStream_t)stream);
+  LaunchData data;
+  if (const int rc = bind_data(objective, D, 0, &data)) return rc;
+  const KernelChoice c = choose_kernel(EVOK_OBJ_KERNEL_EVAL, false, X, ldx, nullptr, nullptr, n_rows, D, data);
+  void* args[] = {&X, &ldx, &n_rows, &D, &f, &data.binding};
+  return launch(data.base, c, args, (cudaStream_t)stream);
 }
 
 // One launch per item chunk of the batched family: item b of the batch samples with stream word (stream_id0 + b), chunk b0 of
-// at most kMaxGridY items (grid y) starting at stream word stream_lo + b0; f (null for EVOK_OBJ_NONE) is [items][n_rows].
+// at most kMaxGridY items (grid y) starting at stream word stream_lo + b0 and at item b0 of X, mu, sigma and the objective's
+// data; f (null for EVOK_OBJ_NONE) is [items][n_rows].
 static int sample_items(int objective, float* X, int64_t item_stride_x, int64_t ldx, const float* mu, int64_t item_stride_mu, const float* sigma,
                         int64_t item_stride_sigma, int64_t n_items, int64_t n_rows, int64_t D, bool sym, uint64_t seed, uint64_t stream_id0, float* f,
                         cudaStream_t st) {
-  KernelChoice c = choose_kernel(EVOK_OBJ_KERNEL_BATCHED, sym, X, ldx, mu, sigma, n_rows, D,
+  LaunchData data;
+  if (const int rc = bind_data(objective, D, n_items, &data)) return rc;
+  KernelChoice c = choose_kernel(EVOK_OBJ_KERNEL_BATCHED, sym, X, ldx, mu, sigma, n_rows, D, data,
                                  (X ? item_stride_x : 0) | item_stride_mu | item_stride_sigma);
   const PhiloxKey key = make_philox_key(seed, stream_id0);
   return for_item_chunks(n_items, kMaxGridY, [&](int64_t b0, int64_t nb) {
@@ -386,8 +511,10 @@ static int sample_items(int objective, float* X, int64_t item_stride_x, int64_t 
     const float* muc = mu + b0 * item_stride_mu;
     const float* sgc = sigma + b0 * item_stride_sigma;
     float* fc = f ? f + b0 * n_rows : nullptr;
-    void* args[] = {&Xc, &item_stride_x, &ldx, &muc, &item_stride_mu, &sgc, &item_stride_sigma, &c.n_units, &D, &kc, &fc};
-    return launch(objective, c, args, st, nb);
+    DataBinding dc = data.binding;
+    for (int i = 0; i < EVOK_MAX_DATA; ++i) dc.p[i] += b0 * dc.item_stride[i];
+    void* args[] = {&Xc, &item_stride_x, &ldx, &muc, &item_stride_mu, &sgc, &item_stride_sigma, &c.n_units, &D, &kc, &fc, &dc};
+    return launch(data.base, c, args, st, nb);
   });
 }
 
@@ -421,7 +548,7 @@ static int check_sample_batched(int objective, const float* X, int64_t item_stri
 extern "C" EVOK_API int evok_sample_eval_batched(int objective, float* X, int64_t item_stride_x, int64_t ldx, const float* mu, int64_t item_stride_mu,
                                                  const float* sigma, int64_t item_stride_sigma, int64_t n_items, int64_t n_rows, int64_t D,
                                                  int symmetric, uint64_t seed, uint64_t stream_id0, float* f, void* stream) {
-  const int rc = check_sample_batched(objective, X, item_stride_x, ldx, mu, item_stride_mu, sigma, item_stride_sigma, n_items, n_rows, D,
+  const int rc = check_sample_batched(base_of(objective), X, item_stride_x, ldx, mu, item_stride_mu, sigma, item_stride_sigma, n_items, n_rows, D,
                                       symmetric != 0, f);
   if (rc != 0 || n_items == 0 || n_rows == 0) return rc;
   return sample_items(objective, X, item_stride_x, ldx, mu, item_stride_mu, sigma, item_stride_sigma, n_items, n_rows, D, symmetric != 0, seed,

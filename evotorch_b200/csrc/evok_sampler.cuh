@@ -169,6 +169,12 @@ __device__ __forceinline__ void st_stream1(float* p, float a) {
 // A generated accumulator may also have pair terms (`static constexpr bool kPairs = true`, see PairTerms below):
 //   add_pair(x, xn, j) : fold the neighbour pair (x_j, x_{j+1}); it is called exactly once for every j in [0, D-2] of a row,
 //                        by the lane that holds column j+1, also in no fixed order across lanes (fold_pairs).
+// A generated accumulator may also refer to data (`static constexpr bool kData = true`, see DataTerms below): float32
+// vectors of the row length and scalars, bound per launch.  It is then constructed as Acc(D, binding), declares
+// `static constexpr int kVectors` and `const float* vec[]` (the vectors of this launch's item), loads its scalars once in the
+// constructor, and takes the vectors' entries with every fold:
+//   add(x, j, d)                  : d[i] = vec[i][j];
+//   add_pair(x, xn, j, d, dn)     : d[i] = vec[i][j], dn[i] = vec[i][j + 1].
 // The built-in ones are ObjAcc<EVOK_OBJ_*>; a user-defined one is generated by evotorch_b200/jit.py.
 // ------------------------------------------------------------------------------------------------
 template <int OBJ>
@@ -236,22 +242,111 @@ struct PairTerms<Acc, decltype(void(Acc::kPairs))> {
   static constexpr bool value = Acc::kPairs;
 };
 
+// The data of one launch of an objective with data terms: p[i] is data name i of the launch's first item and item_stride[i]
+// the distance in floats to the next item's (0: shared by all items; only the batched sampler has more than one item).  It is
+// a kernel argument, so two objectives of one source in flight on two streams, or captured in two graphs, never share it.
+struct DataBinding {
+  const float* p[EVOK_MAX_DATA];
+  int64_t item_stride[EVOK_MAX_DATA];
+};
+struct NoData {};
+
+// true for an accumulator that declares `static constexpr bool kData = true`; Arg is the last argument of its kernels (an
+// empty struct for every other accumulator, whose kernels are otherwise untouched: all data code is under `if constexpr`)
+template <typename Acc, typename = void>
+struct DataTerms {
+  static constexpr bool value = false;
+  using Arg = NoData;
+};
+template <typename Acc>
+struct DataTerms<Acc, decltype(void(Acc::kData))> {
+  static constexpr bool value = Acc::kData;
+  using Arg = DataBinding;
+};
+
+template <typename Acc, typename Arg>
+__device__ __forceinline__ Acc make_acc(int64_t D, const Arg& data) {
+  if constexpr (DataTerms<Acc>::value) return Acc(D, data);
+  else return Acc(D);
+}
+
+__device__ __forceinline__ NoData item_data(const NoData& d, int64_t) { return d; }
+__device__ __forceinline__ DataBinding item_data(DataBinding d, int64_t item) {
+#pragma unroll
+  for (int i = 0; i < EVOK_MAX_DATA; ++i) d.p[i] += item * d.item_stride[i];
+  return d;
+}
+
+// The data vectors' entries at the N columns a lane holds in one step: v[c][i] = vec[i][column c of the step], read through
+// the read-only cache (a D-vector is re-read by every row, so it stays in L1 / L2).  One load serves the + and the - row of a
+// symmetric pair.  `left` is the entry at the column before the first (the left neighbour of a pair fold across lanes).
+template <typename Acc, int N>
+struct DataCols {
+  static constexpr int kSlots = Acc::kVectors > 0 ? Acc::kVectors : 1;
+  float v[N][kSlots], left[kSlots];
+  // columns j .. j + 3 with one 16-byte load per vector: the vectorised kernels, which the host picks only when every vector is
+  // 16-byte aligned (choose_kernel)
+  __device__ __forceinline__ void load4(const Acc& acc, int64_t j) {
+    static_assert(N == 4, "a column group is 4 columns");
+#pragma unroll
+    for (int i = 0; i < Acc::kVectors; ++i) {
+      const float4 t = __ldg(reinterpret_cast<const float4*>(acc.vec[i] + j));
+      v[0][i] = t.x; v[1][i] = t.y; v[2][i] = t.z; v[3][i] = t.w;
+    }
+  }
+  __device__ __forceinline__ void load1(const Acc& acc, int64_t j, int c) {  // column j into slot c
+#pragma unroll
+    for (int i = 0; i < Acc::kVectors; ++i) v[c][i] = __ldg(acc.vec[i] + j);
+  }
+  __device__ __forceinline__ void load_left(const Acc& acc, int64_t j) {  // column j - 1, j > 0
+#pragma unroll
+    for (int i = 0; i < Acc::kVectors; ++i) left[i] = __ldg(acc.vec[i] + j - 1);
+  }
+};
+struct NoCols {
+  template <typename Acc> __device__ __forceinline__ void load4(const Acc&, int64_t) {}
+  template <typename Acc> __device__ __forceinline__ void load1(const Acc&, int64_t, int) {}
+  template <typename Acc> __device__ __forceinline__ void load_left(const Acc&, int64_t) {}
+};
+template <typename Acc, int N, bool = DataTerms<Acc>::value>
+struct ColsOf {
+  using type = NoCols;
+};
+template <typename Acc, int N>
+struct ColsOf<Acc, N, true> {
+  using type = DataCols<Acc, N>;
+};
+
+// acc.add of element x of column j, which is slot c of dc
+template <typename Acc, typename Cols>
+__device__ __forceinline__ void fold(Acc& acc, float x, int64_t j, const Cols& dc, int c) {
+  if constexpr (DataTerms<Acc>::value) acc.add(x, j, dc.v[c]);
+  else acc.add(x, j);
+}
+
 // One warp step of pair folds: this lane holds the N consecutive columns j .. j+N-1 of a row (v[]), of which the first
 // n_valid exist (0 for a lane past the row's end).  The lane holding column c + 1 folds (x_c, x_{c+1}): inside v[] from
 // registers, and for its first column with x_{j-1} = the last column of lane - 1, or for lane 0 the last column lane 31
 // held in the previous step of the same row (`carry`, zero-initialised per row and advanced here).  Every lane of the warp
 // must call it on every step, in the same order (it shuffles); a column's left neighbour is always in the previous lane
 // or the previous step because each step covers 32 * N consecutive columns.
-template <int N, typename Acc>
-__device__ __forceinline__ void fold_pairs(Acc& acc, const float (&v)[N], int64_t j, int n_valid, float& carry) {
+// dc: the data of the same columns (with `left` loaded when j > 0) for an accumulator with data terms.
+template <int N, typename Acc, typename Cols>
+__device__ __forceinline__ void fold_pairs(Acc& acc, const float (&v)[N], int64_t j, int n_valid, float& carry, const Cols& dc) {
   const int lane = threadIdx.x & 31;
   const float rot = __shfl_sync(0xffffffffu, v[N - 1], (lane + 31) & 31);  // lane 0 receives lane 31's: next step's carry
   const float left = lane == 0 ? carry : rot;
   carry = rot;
-  if (n_valid > 0 && j > 0) acc.add_pair(left, v[0], j - 1);
+  if (n_valid > 0 && j > 0) {
+    if constexpr (DataTerms<Acc>::value) acc.add_pair(left, v[0], j - 1, dc.left, dc.v[0]);
+    else acc.add_pair(left, v[0], j - 1);
+  }
 #pragma unroll
   for (int c = 1; c < N; ++c)
-    if (c < n_valid) acc.add_pair(v[c - 1], v[c], j + c - 1);
+    if (c < n_valid) {
+      if constexpr (DataTerms<Acc>::value) acc.add_pair(v[c - 1], v[c], j + c - 1, dc.v[c - 1], dc.v[c]);
+      else acc.add_pair(v[c - 1], v[c], j + c - 1);
+    }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -294,6 +389,7 @@ __device__ __forceinline__ void sample_group(const PhiloxKey& key, uint32_t sw, 
   float z[4];
   normals4(key, sw, unit, q, z);
   const int64_t j = (int64_t)q << 2;
+  typename ColsOf<Acc, 4>::type dc;
   if (VEC) {
     if (SQ) {
       *zsq = fmaf(z[0], z[0], *zsq); *zsq = fmaf(z[1], z[1], *zsq); *zsq = fmaf(z[2], z[2], *zsq); *zsq = fmaf(z[3], z[3], *zsq);
@@ -302,11 +398,12 @@ __device__ __forceinline__ void sample_group(const PhiloxKey& key, uint32_t sw, 
     const float4 s = __ldg(reinterpret_cast<const float4*>(sigma + j));
     const float p0 = fmaf(s.x, z[0], m.x), p1 = fmaf(s.y, z[1], m.y), p2 = fmaf(s.z, z[2], m.z), p3 = fmaf(s.w, z[3], m.w);
     if (STORE) st_stream4(xp + j, p0, p1, p2, p3);
-    accp.add(p0, j); accp.add(p1, j + 1); accp.add(p2, j + 2); accp.add(p3, j + 3);
+    dc.load4(accp, j);
+    fold(accp, p0, j, dc, 0); fold(accp, p1, j + 1, dc, 1); fold(accp, p2, j + 2, dc, 2); fold(accp, p3, j + 3, dc, 3);
     if (SYM) {
       const float n0 = fmaf(-s.x, z[0], m.x), n1 = fmaf(-s.y, z[1], m.y), n2 = fmaf(-s.z, z[2], m.z), n3 = fmaf(-s.w, z[3], m.w);
       if (STORE) st_stream4(xm + j, n0, n1, n2, n3);
-      accm.add(n0, j); accm.add(n1, j + 1); accm.add(n2, j + 2); accm.add(n3, j + 3);
+      fold(accm, n0, j, dc, 0); fold(accm, n1, j + 1, dc, 1); fold(accm, n2, j + 2, dc, 2); fold(accm, n3, j + 3, dc, 3);
     }
   } else {
 #pragma unroll
@@ -316,11 +413,12 @@ __device__ __forceinline__ void sample_group(const PhiloxKey& key, uint32_t sw, 
         const float m = __ldg(mu + j + c), s = __ldg(sigma + j + c);
         const float p = fmaf(s, z[c], m);
         if (STORE) st_stream1(xp + j + c, p);
-        accp.add(p, j + c);
+        dc.load1(accp, j + c, c);
+        fold(accp, p, j + c, dc, c);
         if (SYM) {
           const float n = fmaf(-s, z[c], m);
           if (STORE) st_stream1(xm + j + c, n);
-          accm.add(n, j + c);
+          fold(accm, n, j + c, dc, c);
         }
       }
     }
@@ -337,6 +435,7 @@ __device__ __forceinline__ void sample_group_pairs(const PhiloxKey& key, uint32_
   float p[4] = {0.f, 0.f, 0.f, 0.f}, n[4] = {0.f, 0.f, 0.f, 0.f};
   const int64_t j = (int64_t)q << 2;
   int n_valid = 0;
+  typename ColsOf<Acc, 4>::type dc;
   if (active) {
     float z[4];
     normals4(key, sw, unit, q, z);
@@ -348,11 +447,12 @@ __device__ __forceinline__ void sample_group_pairs(const PhiloxKey& key, uint32_
       const float4 s = __ldg(reinterpret_cast<const float4*>(sigma + j));
       p[0] = fmaf(s.x, z[0], m.x); p[1] = fmaf(s.y, z[1], m.y); p[2] = fmaf(s.z, z[2], m.z); p[3] = fmaf(s.w, z[3], m.w);
       if (STORE) st_stream4(xp + j, p[0], p[1], p[2], p[3]);
-      accp.add(p[0], j); accp.add(p[1], j + 1); accp.add(p[2], j + 2); accp.add(p[3], j + 3);
+      dc.load4(accp, j);
+      fold(accp, p[0], j, dc, 0); fold(accp, p[1], j + 1, dc, 1); fold(accp, p[2], j + 2, dc, 2); fold(accp, p[3], j + 3, dc, 3);
       if (SYM) {
         n[0] = fmaf(-s.x, z[0], m.x); n[1] = fmaf(-s.y, z[1], m.y); n[2] = fmaf(-s.z, z[2], m.z); n[3] = fmaf(-s.w, z[3], m.w);
         if (STORE) st_stream4(xm + j, n[0], n[1], n[2], n[3]);
-        accm.add(n[0], j); accm.add(n[1], j + 1); accm.add(n[2], j + 2); accm.add(n[3], j + 3);
+        fold(accm, n[0], j, dc, 0); fold(accm, n[1], j + 1, dc, 1); fold(accm, n[2], j + 2, dc, 2); fold(accm, n[3], j + 3, dc, 3);
       }
       n_valid = 4;
     } else {
@@ -363,30 +463,33 @@ __device__ __forceinline__ void sample_group_pairs(const PhiloxKey& key, uint32_
           const float m = __ldg(mu + j + c), s = __ldg(sigma + j + c);
           p[c] = fmaf(s, z[c], m);
           if (STORE) st_stream1(xp + j + c, p[c]);
-          accp.add(p[c], j + c);
+          dc.load1(accp, j + c, c);
+          fold(accp, p[c], j + c, dc, c);
           if (SYM) {
             n[c] = fmaf(-s, z[c], m);
             if (STORE) st_stream1(xm + j + c, n[c]);
-            accm.add(n[c], j + c);
+            fold(accm, n[c], j + c, dc, c);
           }
         }
       }
       n_valid = D - j < 4 ? (int)(D - j) : 4;  // the partial last group: a pair is folded only where column j + 1 < D
     }
   }
-  fold_pairs<4>(accp, p, j, n_valid, carry_p);
-  if (SYM) fold_pairs<4>(accm, n, j, n_valid, carry_m);
+  if (n_valid > 0 && j > 0) dc.load_left(accp, j);
+  fold_pairs<4>(accp, p, j, n_valid, carry_p, dc);
+  if (SYM) fold_pairs<4>(accm, n, j, n_valid, carry_m, dc);
 }
 
 // One unit u (a direction of symmetric sampling, else a row) of the warp of lane `lane`: sample its row(s) from (key, stream word sw, unit
 // unit0 + u), store them at row r = (SYM ? 2u : u) of X when STORE, fold them into the objective and store the fitness at f[r]
-// (or, PUSH, at row0 + r of every peer's vector); SQ: q_out[r] = sum of z^2.  The body of sample_eval_kernel and of
+// (or, PUSH, at row0 + r of every peer's vector); SQ: q_out[r] = sum of z^2; data: the binding of an accumulator with data terms.  The body of sample_eval_kernel and of
 // sample_eval_batched_kernel, so both give the same bits for the same operands and counters.
 template <typename Acc, bool SYM, bool STORE, bool VEC, bool PUSH, bool SQ>
 __device__ __forceinline__ void sample_eval_unit(int lane, float* __restrict__ X, int64_t ldx, const float* __restrict__ mu,
                                                  const float* __restrict__ sigma, int64_t row0, int64_t u, int64_t D, const PhiloxKey& key, uint32_t sw,
-                                                 uint32_t nq, uint64_t unit0, float* __restrict__ f, const PeerSink& sink, float* __restrict__ q_out) {
-  Acc accp(D), accm(D);
+                                                 uint32_t nq, uint64_t unit0, float* __restrict__ f, const PeerSink& sink, float* __restrict__ q_out,
+                                                 const typename DataTerms<Acc>::Arg& data) {
+  Acc accp = make_acc<Acc>(D, data), accm = make_acc<Acc>(D, data);
   const int64_t r = SYM ? 2 * u : u;
   float* xp = STORE ? X + r * ldx : nullptr;
   float* xm = STORE ? xp + ldx : nullptr;
@@ -450,7 +553,7 @@ __global__ void __launch_bounds__(kSampleThreads, SampleTune<Acc>::kMinBlocks)
     sample_eval_kernel(float* __restrict__ X, int64_t ldx, const float* __restrict__ mu, const float* __restrict__ sigma,
                        int64_t row0, int64_t n_units, int64_t D, const __grid_constant__ PhiloxKey key, const uint32_t* __restrict__ stream_off,
                        float* __restrict__ f, const __grid_constant__ PeerSink sink, const unsigned long long* epoch, unsigned int* done,
-                       float* __restrict__ q_out) {
+                       float* __restrict__ q_out, const typename DataTerms<Acc>::Arg data) {
   static_assert(!(SQ && (SYM || PUSH)), "the squared norms are produced by the plain non-symmetric sampler only");
   const int lane = threadIdx.x & 31;
   const uint32_t sw = key.stream_lo + (stream_off ? __ldg(stream_off) : 0u);
@@ -460,19 +563,20 @@ __global__ void __launch_bounds__(kSampleThreads, SampleTune<Acc>::kMinBlocks)
   const uint64_t unit0 = (uint64_t)(SYM ? (row0 >> 1) : row0);
 
   for (int64_t u = gw; u < n_units; u += warps_total)
-    sample_eval_unit<Acc, SYM, STORE, VEC, PUSH, SQ>(lane, X, ldx, mu, sigma, row0, u, D, key, sw, nq, unit0, f, sink, q_out);
+    sample_eval_unit<Acc, SYM, STORE, VEC, PUSH, SQ>(lane, X, ldx, mu, sigma, row0, u, D, key, sw, nq, unit0, f, sink, q_out, data);
   if (PUSH) peer_signal_tail(sink, epoch, done);
 }
 
 // Batched searches (the functional ask / tell API with leading batch dimensions): blockIdx.y = item b of the launch.  Every
 // item has its own X, mu and sigma at an item stride (0 = the operand is shared by all items), its fitnesses at row b of
 // f [items][n_rows], and its own Philox stream word key.stream_lo + b, so one launch samples and evaluates the populations of
-// all items, bit-identical to one sample_eval_kernel launch per item with stream id (stream id of the key) + b.
+// all items, bit-identical to one sample_eval_kernel launch per item with stream id (stream id of the key) + b.  The data of
+// an accumulator with data terms is per item too, at the item strides of its binding.
 template <typename Acc, bool SYM, bool STORE, bool VEC>
 __global__ void __launch_bounds__(kSampleThreads, SampleTune<Acc>::kMinBlocks)
     sample_eval_batched_kernel(float* __restrict__ X, int64_t item_stride_x, int64_t ldx, const float* __restrict__ mu, int64_t item_stride_mu,
                                const float* __restrict__ sigma, int64_t item_stride_sigma, int64_t n_units, int64_t D,
-                               const __grid_constant__ PhiloxKey key, float* __restrict__ f) {
+                               const __grid_constant__ PhiloxKey key, float* __restrict__ f, const typename DataTerms<Acc>::Arg data) {
   const int lane = threadIdx.x & 31;
   const int64_t item = blockIdx.y;
   if (STORE) X += item * item_stride_x;
@@ -484,20 +588,24 @@ __global__ void __launch_bounds__(kSampleThreads, SampleTune<Acc>::kMinBlocks)
   const int64_t gw = (int64_t)blockIdx.x * (kSampleThreads / 32) + (threadIdx.x >> 5);
   const uint32_t nq = (uint32_t)((D + 3) >> 2);
   const PeerSink no_sink{};
+  const typename DataTerms<Acc>::Arg my_data = item_data(data, item);
   for (int64_t u = gw; u < n_units; u += warps_total)
-    sample_eval_unit<Acc, SYM, STORE, VEC, false, false>(lane, X, ldx, mu, sigma, 0, u, D, key, sw, nq, 0, f, no_sink, nullptr);
+    sample_eval_unit<Acc, SYM, STORE, VEC, false, false>(lane, X, ldx, mu, sigma, 0, u, D, key, sw, nq, 0, f, no_sink, nullptr, my_data);
 }
 
 constexpr int kEvalThreads = 256;
 
 template <typename Acc, bool VEC>
 __global__ void __launch_bounds__(kEvalThreads)
-    eval_kernel(const float* __restrict__ X, int64_t ldx, int64_t n_rows, int64_t D, float* __restrict__ f) {
+    eval_kernel(const float* __restrict__ X, int64_t ldx, int64_t n_rows, int64_t D, float* __restrict__ f,
+                const typename DataTerms<Acc>::Arg data) {
   const int lane = threadIdx.x & 31;
   const int64_t warps_total = (int64_t)gridDim.x * (kEvalThreads / 32);
   const int64_t gw = (int64_t)blockIdx.x * (kEvalThreads / 32) + (threadIdx.x >> 5);
+  using Cols4 = typename ColsOf<Acc, 4>::type;
+  using Cols1 = typename ColsOf<Acc, 1>::type;
   for (int64_t r = gw; r < n_rows; r += warps_total) {
-    Acc acc(D);
+    Acc acc = make_acc<Acc>(D, data);
     const float* x = X + r * ldx;
     if constexpr (PairTerms<Acc>::value) {
       // warp-uniform steps (fold_pairs shuffles); per lane the groups, element adds and pair folds of sample_eval_kernel's
@@ -515,8 +623,11 @@ __global__ void __launch_bounds__(kEvalThreads)
           for (int k = 0; k < 4; ++k) {
             const int64_t jk = 4 * (q + 32 * k);
             const float v[4] = {g[k].x, g[k].y, g[k].z, g[k].w};
-            acc.add(v[0], jk); acc.add(v[1], jk + 1); acc.add(v[2], jk + 2); acc.add(v[3], jk + 3);
-            fold_pairs<4>(acc, v, jk, 4, carry);
+            Cols4 dc;
+            dc.load4(acc, jk);
+            if (jk > 0) dc.load_left(acc, jk);
+            fold(acc, v[0], jk, dc, 0); fold(acc, v[1], jk + 1, dc, 1); fold(acc, v[2], jk + 2, dc, 2); fold(acc, v[3], jk + 3, dc, 3);
+            fold_pairs<4>(acc, v, jk, 4, carry, dc);
           }
         }
         for (; b < nq; b += 32) {
@@ -525,18 +636,26 @@ __global__ void __launch_bounds__(kEvalThreads)
           const float4 a = active ? ld_stream4(x + 4 * q) : make_float4(0.f, 0.f, 0.f, 0.f);
           const float v[4] = {a.x, a.y, a.z, a.w};
           const int64_t ja = 4 * q;
+          Cols4 dc;
           if (active) {
-            acc.add(v[0], ja); acc.add(v[1], ja + 1); acc.add(v[2], ja + 2); acc.add(v[3], ja + 3);
+            dc.load4(acc, ja);
+            if (ja > 0) dc.load_left(acc, ja);
+            fold(acc, v[0], ja, dc, 0); fold(acc, v[1], ja + 1, dc, 1); fold(acc, v[2], ja + 2, dc, 2); fold(acc, v[3], ja + 3, dc, 3);
           }
-          fold_pairs<4>(acc, v, ja, active ? 4 : 0, carry);
+          fold_pairs<4>(acc, v, ja, active ? 4 : 0, carry, dc);
         }
       } else {
         for (int64_t b = 0; b < D; b += 32) {
           const int64_t j = b + lane;
           const bool active = j < D;
           const float v[1] = {active ? ld_stream1(x + j) : 0.f};
-          if (active) acc.add(v[0], j);
-          fold_pairs<1>(acc, v, j, active ? 1 : 0, carry);
+          Cols1 dc;
+          if (active) {
+            dc.load1(acc, j, 0);
+            if (j > 0) dc.load_left(acc, j);
+            fold(acc, v[0], j, dc, 0);
+          }
+          fold_pairs<1>(acc, v, j, active ? 1 : 0, carry, dc);
         }
       }
     } else if (VEC) {
@@ -547,18 +666,26 @@ __global__ void __launch_bounds__(kEvalThreads)
         const float4 a = ld_stream4(x + 4 * q), b = ld_stream4(x + 4 * (q + 32)), c = ld_stream4(x + 4 * (q + 64)),
                      d = ld_stream4(x + 4 * (q + 96));
         const int64_t ja = 4 * q, jb = 4 * (q + 32), jc = 4 * (q + 64), jd = 4 * (q + 96);
-        acc.add(a.x, ja); acc.add(a.y, ja + 1); acc.add(a.z, ja + 2); acc.add(a.w, ja + 3);
-        acc.add(b.x, jb); acc.add(b.y, jb + 1); acc.add(b.z, jb + 2); acc.add(b.w, jb + 3);
-        acc.add(c.x, jc); acc.add(c.y, jc + 1); acc.add(c.z, jc + 2); acc.add(c.w, jc + 3);
-        acc.add(d.x, jd); acc.add(d.y, jd + 1); acc.add(d.z, jd + 2); acc.add(d.w, jd + 3);
+        Cols4 da, db, dc, dd;
+        da.load4(acc, ja); db.load4(acc, jb); dc.load4(acc, jc); dd.load4(acc, jd);
+        fold(acc, a.x, ja, da, 0); fold(acc, a.y, ja + 1, da, 1); fold(acc, a.z, ja + 2, da, 2); fold(acc, a.w, ja + 3, da, 3);
+        fold(acc, b.x, jb, db, 0); fold(acc, b.y, jb + 1, db, 1); fold(acc, b.z, jb + 2, db, 2); fold(acc, b.w, jb + 3, db, 3);
+        fold(acc, c.x, jc, dc, 0); fold(acc, c.y, jc + 1, dc, 1); fold(acc, c.z, jc + 2, dc, 2); fold(acc, c.w, jc + 3, dc, 3);
+        fold(acc, d.x, jd, dd, 0); fold(acc, d.y, jd + 1, dd, 1); fold(acc, d.z, jd + 2, dd, 2); fold(acc, d.w, jd + 3, dd, 3);
       }
       for (; q < nq; q += 32) {
         const float4 a = ld_stream4(x + 4 * q);
         const int64_t ja = 4 * q;
-        acc.add(a.x, ja); acc.add(a.y, ja + 1); acc.add(a.z, ja + 2); acc.add(a.w, ja + 3);
+        Cols4 da;
+        da.load4(acc, ja);
+        fold(acc, a.x, ja, da, 0); fold(acc, a.y, ja + 1, da, 1); fold(acc, a.z, ja + 2, da, 2); fold(acc, a.w, ja + 3, da, 3);
       }
     } else {
-      for (int64_t j = lane; j < D; j += 32) acc.add(ld_stream1(x + j), j);
+      for (int64_t j = lane; j < D; j += 32) {
+        Cols1 dc;
+        dc.load1(acc, j, 0);
+        fold(acc, ld_stream1(x + j), j, dc, 0);
+      }
     }
     const float v = acc.finish(D);
     if (lane == 0) f[r] = v;

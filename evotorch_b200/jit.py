@@ -19,8 +19,15 @@ The expression language (anything else raises ValueError):
   - constants  pi, e, numeric literals;
   - names      x (the element), xn (the next element x_{j+1}), j (the 0-based column of x) and D (the row length) in a
     term; the sum names and D in `value`.
+  - data       up to 4 more names, each bound to a float32 tensor (`data={"t": t, "lam": lam}`).  Last dimension 1 makes a
+    scalar, usable in the terms and in `value`; any other last dimension makes a vector, which must have the row length D and is
+    usable in the terms only: `t` is its entry at column j and, in a pair term, `t_n` its entry at column j + 1 (as x and xn).
+    Leading dimensions are batch dimensions: one data set per item of a batched search.
 The CUDA side evaluates in float32 with the precise libdevice functions (no fast math) and contracts a * b + c into fma.
-The source of an objective without pair terms is exactly that of the element-only language (no pair code in it).
+The source of an objective without pair terms is exactly that of the element-only language (no pair code in it), and the source
+of one without data is exactly that of the language without data.  Which data name is a scalar and which a vector is part of
+the source; the tensors are not: they are bound to an instance of the compiled objective (`bind_instance`) and reach the
+kernels as a launch argument, so objectives with the same expressions and kinds share one compilation whatever their data.
 """
 
 from __future__ import annotations
@@ -44,6 +51,7 @@ CSRC = os.path.join(_PKG, "csrc")
 INCLUDE = os.path.join(os.path.dirname(_PKG), "include")
 
 MAX_SUMS = 4
+MAX_DATA = 4  # EVOK_MAX_DATA
 MAX_INT_POWER = 16
 
 FUNCTIONS = {
@@ -159,13 +167,39 @@ def _parse(text: str, names: Dict[str, str], where: str) -> _Expr:
 
 
 _RESERVED = {"x", "j", "D"} | set(CONSTANTS) | set(FUNCTIONS)
+_RESERVED_DATA = _RESERVED | {"xn"}
+
+
+def data_kinds(data: dict) -> Dict[str, bool]:
+    """{name: is a vector} of a `data` dict of tensors, after the checks on the names and tensors (ValueError)."""
+    if not isinstance(data, dict) or len(data) > MAX_DATA:
+        raise ValueError(f"data: expected a dict of at most {MAX_DATA} named float32 tensors")
+    kinds = {}
+    for name, t in data.items():
+        if not (isinstance(name, str) and name.isidentifier()) or name in _RESERVED_DATA or name.endswith("_n"):
+            raise ValueError(f"data: {name!r} cannot name data (a data name is an identifier that does not end in '_n', other than "
+                             f"{sorted(_RESERVED_DATA)})")
+        if not (isinstance(t, torch.Tensor) and t.dtype == torch.float32 and t.ndim >= 1 and t.shape[-1] >= 1):
+            what = f"{tuple(t.shape)} {t.dtype}" if isinstance(t, torch.Tensor) else type(t).__name__
+            raise ValueError(f"data[{name!r}]: expected a float32 tensor with at least one dimension, got {what}")
+        kinds[name] = t.shape[-1] != 1
+    return kinds
+
+
+def _names_used(text) -> set:
+    try:
+        return {n.id for n in ast.walk(ast.parse(text, mode="eval")) if isinstance(n, ast.Name)}
+    except (SyntaxError, TypeError):
+        return set()  # _parse reports it
 
 
 class ObjectiveSpec:
     """The parsed form of an objective: `source` is the CUDA translation unit, `torch_fn(X)` the torch function.  `pairs` names
     the sums whose term uses xn (summed over the neighbour pairs of a row); the others are summed over its elements."""
 
-    def __init__(self, sums: Dict[str, str], value: str):
+    def __init__(self, sums: Dict[str, str], value: str, kinds: Optional[Dict[str, bool]] = None):
+        """kinds: {data name: is a vector} in binding order (`data_kinds`), None or empty for an objective without data."""
+        self.kinds = dict(kinds or {})
         if not isinstance(sums, dict) or not 1 <= len(sums) <= MAX_SUMS:
             raise ValueError(f"sums: expected a dict of 1 to {MAX_SUMS} named term expressions")
         for s in sums:
@@ -173,33 +207,83 @@ class ObjectiveSpec:
                 raise ValueError(f"sums: {s!r} cannot name a sum (a sum name is an identifier other than {sorted(_RESERVED)})")
         self.sums, self.value = dict(sums), value
         term_names = {"x": "x", "xn": "xn", "j": "jf", "D": "Df"}
-        self.terms = {s: _parse(t, term_names, f"sums[{s!r}]") for s, t in sums.items()}
-        self.pairs = frozenset(s for s, e in self.terms.items() if re.search(r"\bxn\b", e.cuda))
         value_names = {s: f"S_{s}" for s in sums}
         value_names["D"] = "Df"
+        for name, vector in self.kinds.items():
+            if name in sums:
+                raise ValueError(f"data: {name!r} is the name of a sum")
+            # a vector's entries at columns j and j + 1, handed to add / add_pair; a scalar is a member of the accumulator
+            term_names.update({name: f"v_{name}", f"{name}_n": f"vn_{name}"} if vector else {name: f"c_{name}"})
+            if not vector:
+                value_names[name] = f"c_{name}"
+        for s, t in sums.items():
+            self._check_data_names(_names_used(t), f"sums[{s!r}]", term=True)
+        self._check_data_names(_names_used(value), "value", term=False)
+        self.terms = {s: _parse(t, term_names, f"sums[{s!r}]") for s, t in sums.items()}
+        self.pairs = frozenset(s for s, e in self.terms.items() if re.search(r"\bxn\b", e.cuda))
+        for s, e in self.terms.items():
+            m = re.search(r"\bvn_(\w+)\b", e.cuda)
+            if m and s not in self.pairs:
+                raise ValueError(f"sums[{s!r}]: {m.group(1)}_n is the entry of {m.group(1)!r} at column j + 1, which only a pair term (one "
+                                 f"that uses xn) has; an element term uses {m.group(1)!r}")
         self.value_expr = _parse(value, value_names, "value")
         self.source = self._cuda_source()
+
+    def _check_data_names(self, used: set, where: str, term: bool) -> None:
+        for name, vector in self.kinds.items():
+            if not vector and f"{name}_n" in used:
+                raise ValueError(f"{where}: {name}_n: {name!r} is a scalar (its last dimension is 1) and has no next entry; use {name!r}")
+            if vector and not term and (name in used or f"{name}_n" in used):
+                raise ValueError(f"{where}: {name!r} is a vector with one entry per column; it can be used in the terms of `sums` only")
 
     def _cuda_source(self) -> str:
         k = range(len(self.terms))
         uses_j = lambda es: any(re.search(r"\bjf\b", e.cuda) for e in es)  # noqa: E731
         element = [(i, e) for i, (s, e) in zip(k, self.terms.items()) if s not in self.pairs]
         pair = [(i, e) for i, (s, e) in zip(k, self.terms.items()) if s in self.pairs]
+        # data: slot i of the binding is data name i; the vectors are numbered among themselves in the same order
+        vectors = [n for n, v in self.kinds.items() if v]
+        nv = max(len(vectors), 1)
+
+        def entries(es, prefix, array):  # the locals of the vector entries that the terms `es` use
+            return [f"    const float {prefix}_{n} = {array}[{i}];" for i, n in enumerate(vectors)
+                    if any(re.search(rf"\b{prefix}_{n}\b", e.cuda) for _, e in es)]
+
         lines = ['#include "evok_sampler.cuh"', "", "namespace evok_user {", "struct Acc {"]
         if pair:
             lines.append("  static constexpr bool kPairs = true;")
+        if self.kinds:
+            lines.append("  static constexpr bool kData = true;")
+            lines.append(f"  static constexpr int kVectors = {len(vectors)};")
         lines.append("  float Df;")
         lines.append("  float " + ", ".join(f"s{i} = 0.f" for i in k) + ";")
-        lines.append("  __device__ __forceinline__ explicit Acc(int64_t D) : Df((float)D) {}")
-        lines.append("  __device__ __forceinline__ void add(float x, int64_t j) {")
+        if self.kinds:
+            slot = {n: i for i, n in enumerate(self.kinds)}
+            lines.append(f"  const float* vec[{nv}];")
+            scalars = [n for n, v in self.kinds.items() if not v]
+            if scalars:
+                lines.append("  float " + ", ".join(f"c_{n}" for n in scalars) + ";")
+            init = ["Df((float)D)", "vec{" + ", ".join(f"b.p[{slot[n]}]" for n in vectors) + "}"]
+            init += [f"c_{n}(__ldg(b.p[{slot[n]}]))" for n in scalars]
+            lines.append("  __device__ __forceinline__ Acc(int64_t D, const evok::DataBinding& b) : " + ", ".join(init) + " {}")
+            lines.append(f"  __device__ __forceinline__ void add(float x, int64_t j, const float (&d)[{nv}]) {{")
+        else:
+            lines.append("  __device__ __forceinline__ explicit Acc(int64_t D) : Df((float)D) {}")
+            lines.append("  __device__ __forceinline__ void add(float x, int64_t j) {")
         if uses_j(e for _, e in element):
             lines.append("    const float jf = (float)j;")
+        lines += entries(element, "v", "d")
         lines += [f"    s{i} += {e.cuda};" for i, e in element]
         lines.append("  }")
         if pair:
-            lines.append("  __device__ __forceinline__ void add_pair(float x, float xn, int64_t j) {")
+            if self.kinds:
+                lines.append(f"  __device__ __forceinline__ void add_pair(float x, float xn, int64_t j, const float (&d)[{nv}], "
+                             f"const float (&dn)[{nv}]) {{")
+            else:
+                lines.append("  __device__ __forceinline__ void add_pair(float x, float xn, int64_t j) {")
             if uses_j(e for _, e in pair):
                 lines.append("    const float jf = (float)j;")
+            lines += entries(pair, "v", "d") + entries(pair, "vn", "dn")
             lines += [f"    s{i} += {e.cuda};" for i, e in pair]
             lines.append("  }")
         lines.append("  __device__ __forceinline__ float finish(int64_t) {")
@@ -208,7 +292,9 @@ class ObjectiveSpec:
         lines += ["  }", "};", "}  // namespace evok_user", ""]
         return "\n".join(lines)
 
-    def torch_fn(self, X: torch.Tensor) -> torch.Tensor:
+    def torch_fn(self, X: torch.Tensor, data: Optional[Dict[str, torch.Tensor]] = None) -> torch.Tensor:
+        """The fitnesses of the rows of X (..., N, D).  data: the tensors of the data names, cast to X's dtype and device; their
+        leading (batch) dimensions broadcast against the batch dimensions of X, and the result has the broadcast shape."""
         D = X.shape[-1]
         Dt = torch.tensor(float(D), dtype=X.dtype, device=X.device)
         env = {"x": X, "j": torch.arange(D, dtype=X.dtype, device=X.device), "D": Dt, "_dtype": X.dtype, "_device": X.device}
@@ -216,11 +302,37 @@ class ObjectiveSpec:
         penv = {"x": X[..., :-1], "xn": X[..., 1:], "j": torch.arange(max(D - 1, 0), dtype=X.dtype, device=X.device), "D": Dt,
                 "_dtype": X.dtype, "_device": X.device}
         venv = {}
+        rows = X.shape[:-1]  # the shape of the result
+        if self.kinds:
+            check_data(self.kinds, data, D)
+            for name, vector in self.kinds.items():
+                t = data[name].to(dtype=X.dtype, device=X.device)
+                rows = torch.broadcast_shapes(rows, tuple(t.shape[:-1]) + (1,))
+                t = t.unsqueeze(-2)  # (*batch, 1, D or 1) against the rows (*batch, N, D)
+                env[name] = t
+                penv[name] = t[..., :-1] if vector else t
+                if vector:
+                    penv[f"{name}_n"] = t[..., 1:]
+                else:
+                    venv[name] = t[..., 0]
         for s, e in self.terms.items():
             en = penv if s in self.pairs else env
-            venv[s] = torch.broadcast_to(_as_tensor(e.torch(en), en), en["x"].shape).sum(dim=-1)
+            shape = rows + (en["x"].shape[-1],)
+            venv[s] = torch.broadcast_to(_as_tensor(e.torch(en), en), shape).sum(dim=-1)
         venv.update(D=Dt, _dtype=X.dtype, _device=X.device)
-        return torch.broadcast_to(_as_tensor(self.value_expr.torch(venv), venv), X.shape[:-1])
+        return torch.broadcast_to(_as_tensor(self.value_expr.torch(venv), venv), rows)
+
+
+def check_data(kinds: Dict[str, bool], data: Optional[Dict[str, torch.Tensor]], D: int) -> None:
+    """ValueError unless `data` holds a tensor of the declared kind for every name, with every vector of length D."""
+    if data is None or list(data) != list(kinds):
+        raise ValueError(f"data: expected tensors for the names {list(kinds)}, got {None if data is None else list(data)}")
+    for name, vector in kinds.items():
+        n = data[name].shape[-1]
+        if (n != 1) != vector:
+            raise ValueError(f"data[{name!r}]: a {'vector' if vector else 'scalar'} in the expressions, but its last dimension is {n}")
+        if vector and n != D:
+            raise ValueError(f"data[{name!r}]: the vector has length {n}, the rows have length {D}")
 
 
 # ------------------------------------------------------------------------------------------------ NVRTC
@@ -383,6 +495,26 @@ def register(cubin: bytes, names: list) -> int:
     return out.value
 
 
+def declare_data(objective_id: int, kinds: Dict[str, bool]) -> None:
+    """evok_objective_declare_data: the registered id has these data names (True: a vector) and launches through instances only."""
+    arr = (c_int * len(kinds))(*[int(v) for v in kinds.values()])
+    nat.check(nat.lib().evok_objective_declare_data(objective_id, len(kinds), arr), "evok_objective_declare_data")
+
+
+def bind_instance(base_id: int, ptrs: list, lens: list, item_strides: list, n_items: int) -> int:
+    """evok_objective_instance: a new id with the kernels of `base_id` and this data binding (release it with `release_instance`)."""
+    n = len(ptrs)
+    out = c_int()
+    rc = nat.lib().evok_objective_instance(base_id, (c_void_p * n)(*ptrs), (ctypes.c_int64 * n)(*lens), (ctypes.c_int64 * n)(*item_strides),
+                                           n_items, n, ctypes.byref(out))
+    nat.check(rc, "evok_objective_instance")
+    return out.value
+
+
+def release_instance(instance_id: int) -> None:
+    nat.check(nat.lib().evok_objective_release(instance_id), "evok_objective_release")
+
+
 def register_batched(objective_id: int, cubin: bytes, names: list) -> None:
     """evok_objective_register_batched: attach the batched kernels (in `batched_kernel_expressions` order) to a registered id."""
     arr = (c_char_p * len(names))(*[n.encode() for n in names])
@@ -401,6 +533,8 @@ def compile_objective(spec: ObjectiveSpec) -> CompiledObjective:
         if c is None:
             c = compile_source(spec.source)
             c.objective_id = register(c.cubin, c.names)
+            if spec.kinds:
+                declare_data(c.objective_id, spec.kinds)
             _cache[spec.source] = c
         return c
 

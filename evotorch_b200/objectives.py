@@ -16,7 +16,8 @@ pairs (x_j, x_{j+1}) of a row (Rosenbrock, Trid, Dixon-Price): its expressions a
 from __future__ import annotations
 
 import math
-from typing import Callable
+import weakref
+from typing import Callable, Optional
 
 import torch
 
@@ -71,21 +72,88 @@ class FusedObjective(BuiltinObjective):
     spills of every kernel.  The same source compiles once per process.  A FusedObjective pickles as its expressions.
 
     The batched samplers of the functional API (`pgpe_ask_and_evaluate`, `cem_ask_and_evaluate`) are 8 more kernels of the same
-    source, compiled on the first batched use (`compile_batched`); `batched_kernel_info` then holds their registers and spills."""
+    source, compiled on the first batched use (`compile_batched`); `batched_kernel_info` then holds their registers and spills.
 
-    def __init__(self, name: str, sums: dict, value: str):
+    `data` gives the expressions up to 4 more names, each bound to a float32 tensor:
+
+        lsq = FusedObjective("lsq", sums={"s": "w * (x - t)**2"}, value="s + lam * D", data={"t": t, "w": w, "lam": lam})
+        shifted_rosenbrock = FusedObjective("shifted_rosenbrock", value="s", data={"o": o},
+                                            sums={"s": "100*((xn - o_n) - (x - o)**2)**2 + (1 - (x - o))**2"})
+
+    A tensor whose last dimension is 1 is a scalar (usable in the terms and in `value`); any other is a vector of the row length
+    D (usable in the terms: `o` is its entry at column j, and `o_n`, in a pair term, its entry at column j + 1).  The kernels
+    read the tensors themselves, which therefore must stay where they are: `obj.data["t"].copy_(new)` changes the values from
+    the next generation on (also of a captured CUDA graph) without a recompile, and `with_data(**tensors)` gives a twin on
+    other tensors that shares the compiled kernels, as every objective with the same expressions and kinds does.  On the kernels
+    the data must be on the device of the population (ValueError).  Leading dimensions of a data tensor are batch dimensions:
+    in a batched search (`pgpe_ask_and_evaluate`, `cem_ask_and_evaluate`) every item then has its own data.  All data tensors
+    with batch dimensions have the same batch shape, which is the batch shape of the search (the centre and stdev are broadcast
+    to it); a tensor without batch dimensions is shared by all items.  A FusedObjective with data pickles with its tensors.  In a
+    multi-GPU run every rank builds its own objective: the tensors must hold the same values on every rank."""
+
+    def __init__(self, name: str, sums: dict, value: str, data: Optional[dict] = None):
         from . import jit
 
-        spec = jit.ObjectiveSpec(sums, value)
+        spec = jit.ObjectiveSpec(sums, value, jit.data_kinds(data) if data else None)
         if name in ops.OBJECTIVE_IDS and ops.OBJECTIVE_IDS[name] < ops.OBJ_USER_BASE:
             raise ValueError(f"{name!r} is the name of a built-in objective")
+        self.data = dict(data) if data else {}
+        self.data_batch_shape = self._data_batch_shape()
         compiled = jit.compile_objective(spec)
-        super().__init__(name, compiled.objective_id, spec.torch_fn)
+        super().__init__(name, compiled.objective_id, (lambda X: spec.torch_fn(X, self.data)) if self.data else spec.torch_fn)
         self.sums, self.value, self.source = dict(spec.sums), spec.value, spec.source
         self.kernel_info = compiled.kernel_info
         self.batched_kernel_info = None
         self._spec = spec
-        ops.OBJECTIVE_IDS[name] = compiled.objective_id
+        if self.data:
+            self._bind(compiled.objective_id)
+        else:
+            ops.OBJECTIVE_IDS[name] = compiled.objective_id
+
+    def _data_batch_shape(self) -> torch.Size:
+        """The one batch shape of the data tensors that have batch dimensions (ValueError if they differ), () if none has."""
+        shapes = {n: t.shape[:-1] for n, t in self.data.items() if t.ndim > 1}
+        if len(set(shapes.values())) > 1:
+            raise ValueError(f"data: the tensors with batch dimensions must have one batch shape, got "
+                             f"{ {n: tuple(s) for n, s in shapes.items()} }")
+        return next(iter(shapes.values()), torch.Size())
+
+    def _bind(self, base_id: int) -> None:
+        """With the data on a CUDA device: an instance of the compiled objective bound to the tensors, which becomes this
+        objective's id until the object is collected.  With the data elsewhere the objective has no fused kernel (torch_fn)."""
+        from . import jit
+
+        tensors = list(self.data.values())
+        if not all(t.is_cuda for t in tensors):
+            self.evok_objective_id = None
+            return
+        if len({t.device for t in tensors}) > 1:
+            raise ValueError(f"data: the tensors are on different devices: { {n: str(t.device) for n, t in self.data.items()} }")
+        strides = []
+        for n, t in self.data.items():
+            # items at one stride: the batch dimensions collapse into one, and the entries of an item are contiguous
+            batch = t.shape[:-1]
+            flat = all(t.stride(k) == t.stride(k + 1) * t.shape[k + 1] for k in range(len(batch) - 1))
+            if not (flat and (t.shape[-1] == 1 or t.stride(-1) == 1)):
+                raise ValueError(f"data[{n!r}]: expected contiguous entries and batch items at one stride, got shape {tuple(t.shape)} "
+                                 f"strides {t.stride()}")
+            strides.append(t.stride(-2) if batch else 0)
+        self.evok_objective_id = jit.bind_instance(base_id, [t.data_ptr() for t in tensors], [t.shape[-1] for t in tensors], strides,
+                                                   max(math.prod(self.data_batch_shape), 1))
+        ops.DATA_DEVICES[self.evok_objective_id] = tensors[0].device
+        weakref.finalize(self, _release, self.evok_objective_id)
+
+    def __call__(self, x: torch.Tensor) -> torch.Tensor:
+        # the evaluation kernel takes one data set: per-item data, and data that is not on a CUDA device, go through torch_fn
+        if self.data and (self.evok_objective_id is None or self.data_batch_shape):
+            return self._torch_fn(x.unsqueeze(0))[..., 0] if x.ndim == 1 else self._torch_fn(x)
+        return super().__call__(x)
+
+    def with_data(self, **tensors) -> "FusedObjective":
+        """A twin of this objective on other tensors (all of its data names, of the same kinds): no recompile."""
+        if set(tensors) != set(self.data):
+            raise ValueError(f"with_data: expected the data names {list(self.data)}, got {list(tensors)}")
+        return FusedObjective(self.name, self.sums, self.value, {n: tensors[n] for n in self.data})
 
     def compile_batched(self) -> None:
         """Compile and attach the batched samplers (once per process for one source); fills `batched_kernel_info`."""
@@ -95,10 +163,18 @@ class FusedObjective(BuiltinObjective):
             self.batched_kernel_info = jit.compile_batched(self._spec).kernel_info
 
     def __reduce__(self):
-        return (FusedObjective, (self.name, self.sums, self.value))
+        return (FusedObjective, (self.name, self.sums, self.value) + ((self.data,) if self.data else ()))
 
     def __repr__(self) -> str:
-        return f"FusedObjective({self.name!r}, sums={self.sums!r}, value={self.value!r})"
+        data = ", data={" + ", ".join(f"{n!r}: {tuple(t.shape)}" for n, t in self.data.items()) + "}" if self.data else ""
+        return f"FusedObjective({self.name!r}, sums={self.sums!r}, value={self.value!r}{data})"
+
+
+def _release(instance_id: int) -> None:
+    from . import jit
+
+    ops.DATA_DEVICES.pop(instance_id, None)
+    jit.release_instance(instance_id)
 
 
 sphere = BuiltinObjective("sphere", ops.OBJ_SPHERE, _sphere)

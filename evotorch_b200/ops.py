@@ -141,12 +141,21 @@ def _host_floats(values, n: int):
 
 # ------------------------------------------------------------------------------------------------ K1 / K2
 _loaded_objectives: set = set()
+# the id of an objective with data (an instance of a registered objective) -> the device its data tensors are on
+DATA_DEVICES: dict = {}
+
+
+def _check_data_device(objective: int, t: torch.Tensor) -> None:
+    if DATA_DEVICES.get(objective, t.device) != t.device:
+        raise ValueError(f"the data of the objective is on {DATA_DEVICES[objective]}, the population on {t.device}")
 
 
 def _load_objective(objective: int, t: torch.Tensor) -> None:
-    """Load a registered objective's module on the device of `t` before its first launch there (evok_objective_load)."""
+    """Load a registered objective's module on the device of `t` before its first launch there (evok_objective_load).  An
+    objective with data evaluates only populations on the device of its data (ValueError)."""
     if objective < OBJ_USER_BASE:
         return
+    _check_data_device(objective, t)
     key = (objective, t.device.index)
     if key not in _loaded_objectives:
         with torch.cuda.device(t.device):
@@ -563,6 +572,7 @@ def sample_eval_batched(objective: int, X: Optional[torch.Tensor], mu: torch.Ten
     for cnt in (bm, bs):
         if cnt is not None and cnt != B:
             raise ValueError("mu / sigma: number of items differs from f")
+    _check_data_device(objective, f)
     if symmetric and n % 2:
         raise ValueError(f"Symmetric sampling cannot be done if the number of solutions is odd: {n}")
     with _timed("sample_eval"):

@@ -44,6 +44,7 @@ extern "C" {
 #define EVOK_E_ODDROWS (-5) /* symmetric sampling / gradients need an even number of rows */
 #define EVOK_E_ALIGN (-6)
 #define EVOK_E_NOKERNEL (-7) /* the cubin of a registered objective lacks one of its EVOK_OBJ_KERNELS kernels */
+#define EVOK_E_NODATA (-8)   /* a registered objective that declares data was launched by its own id, not by an instance's */
 
 #define EVOK_MAX_PEERS 16 /* GPUs of one NVLink domain that can take part in a peer exchange */
 
@@ -57,6 +58,11 @@ extern "C" {
  * in registration order, at most EVOK_OBJ_USER_CAPACITY of them per process; every id in between is EVOK_E_BADENUM */
 #define EVOK_OBJ_USER_BASE 64
 #define EVOK_OBJ_USER_CAPACITY 256
+/* instances of registered objectives that declare data (evok_objective_instance) take ids from EVOK_OBJ_INSTANCE_BASE; a
+ * released id is reused, and at most EVOK_OBJ_INSTANCE_CAPACITY are alive at a time */
+#define EVOK_OBJ_INSTANCE_BASE 1024
+#define EVOK_OBJ_INSTANCE_CAPACITY 65536
+#define EVOK_MAX_DATA 4 /* data names (float32 vectors of the row length and scalars) of one objective */
 
 /* ranking methods (tools/ranking.py:186) */
 #define EVOK_RANK_CENTERED 0
@@ -115,7 +121,7 @@ int evok_eval(int objective, const float* X, int64_t ldx, int64_t n_rows, int64_
  * device), which a caller about to capture a CUDA graph uses to keep the loading out of the capture.  A cubin without one
  * of the kernels yields EVOK_E_NOKERNEL from every call on that device, and nothing is launched.
  * Errors: EVOK_E_NULLPTR, EVOK_E_BADSIZE (bytes == 0, n_kernels != EVOK_OBJ_KERNELS, registry full), EVOK_E_BADENUM
- * (evok_objective_load of an id that is not registered).
+ * (evok_objective_load of an id that is neither registered nor a live instance; an instance id loads its base).
  * --------------------------------------------------------------------------------------------- */
 #define EVOK_OBJ_KERNEL_SAMPLE 0
 #define EVOK_OBJ_KERNEL_PUSH 8
@@ -138,6 +144,33 @@ int evok_objective_load(int objective);
 #define EVOK_OBJ_KERNEL_BATCHED 22
 #define EVOK_OBJ_BATCHED_KERNELS 8
 int evok_objective_register_batched(int objective, const void* cubin, size_t bytes, const char* const* kernel_names_host, int n_kernels);
+
+/* Objectives with data.  The accumulator of a registered objective may read up to EVOK_MAX_DATA float32 device arrays (kData in
+ * csrc/evok_sampler.cuh): vectors with one entry per column of a row, and scalars.  Which name is which is part of its source;
+ * the arrays are not.  evok_objective_declare_data tells the library so, right after evok_objective_register and before the id
+ * is used: is_vector_host[i] != 0 makes data name i a vector.  From then on the id itself launches nothing (EVOK_E_NODATA):
+ * evok_objective_instance makes an id that shares the kernel images and per-device kernel tables of `base` and carries its own
+ * binding, and every entry point that takes an objective id takes it, with its signature unchanged.  The binding reaches the
+ * kernel as a launch argument (captured by value in a CUDA graph), so instances of one base never interfere, on any streams.
+ *   ptrs_host[i]         device array of data name i of the first item; the library keeps the pointer, the caller keeps the
+ *                        array alive and in place until evok_objective_release.  Writing new values into it on a stream takes
+ *                        effect on the launches (and graph replays) that follow on that stream.
+ *   lens_host[i]         1 for a scalar; for a vector its length, which must equal D of every call (EVOK_E_BADSIZE there)
+ *   n_items              1: every call, batched or not, uses the one binding.  > 1: item b of evok_sample_eval_batched reads
+ *                        ptrs_host[i] + b * item_strides_host[i] (a stride may be 0: that name is shared); n_items must then be
+ *                        the n_items of the call, and every non-batched entry refuses the id (EVOK_E_BADSIZE).
+ * The vectorised kernels read a vector with 16-byte loads: they are chosen only if every vector's ptrs_host[i] is 16-byte
+ * aligned and, with n_items > 1, its item stride is a multiple of 4; else the call runs the scalar-column kernels.
+ * The data checks of a launch come after the entry point's own, and nothing is launched when one fails.
+ * evok_objective_release frees an instance id (kernels already enqueued keep their copy of the binding).
+ * Errors: EVOK_E_NULLPTR; EVOK_E_BADENUM (`objective` / `base` is not a registered id, `id` is not a live instance);
+ * EVOK_E_BADSIZE (n_data outside 1 .. EVOK_MAX_DATA or, for an instance, not the declared count; data declared twice; a length
+ * < 1, or 1 for a declared vector, or > 1 for a declared scalar; n_items < 1; a negative stride; EVOK_OBJ_INSTANCE_CAPACITY
+ * instances alive); EVOK_E_NODATA (`base` declares no data). */
+int evok_objective_declare_data(int objective, int n_data, const int* is_vector_host);
+int evok_objective_instance(int base, const float* const* ptrs_host, const int64_t* lens_host, const int64_t* item_strides_host,
+                            int64_t n_items, int n_data, int* id_out_host);
+int evok_objective_release(int id);
 
 /* ---------------------------------------------------------------------------------------------
  * K3: fitness -> utilities.  Replaces tools/ranking.py:24-183 (`rank` :189).
