@@ -17,17 +17,10 @@
 
 namespace evok {
 
-#ifndef EVOK_GRAD_UNROLL
-#define EVOK_GRAD_UNROLL 4
-#endif
-#ifndef EVOK_GRAD_MINB
-#define EVOK_GRAD_MINB 4
-#endif
-#ifndef EVOK_GRAD_CTAS_PER_SM
-#define EVOK_GRAD_CTAS_PER_SM 4
-#endif
 constexpr int kGradThreads = 256;
-constexpr int kGradUnroll = EVOK_GRAD_UNROLL;
+constexpr int kGradUnroll = 4;
+constexpr int kGradMinBlocks = 4;  // __launch_bounds__ of grad_partial_kernel
+constexpr int kGradCtasPerSm = 4;  // the LDG plan's wave of resident CTAs
 constexpr int kMaxResidentCtas = kNumSMs * 8;
 
 template <int VEC>
@@ -72,10 +65,61 @@ struct SepWeights {
 // eps = x - mu, bit-identical to kEpsRead over the stored rows, with item b of a batch (blockIdx.z) on stream word stream_lo + b.
 constexpr int kEpsRead = 0, kEpsRegen = 1, kEpsRebuild = 2;
 
+// The arithmetic both partial kernels share.  (c1, c0) of column sigma s for `form`:
+__device__ __forceinline__ void grad_coeffs(int form, float s, float& c1, float& c0) {
+  if (form == EVOK_GRAD_EXP) {
+    c1 = __fdiv_rn(1.0f, s * s);
+    c0 = 1.0f;
+  } else if (form == EVOK_GRAD_MOMENTS) {
+    c1 = 1.0f;
+    c0 = 0.0f;
+  } else {
+    c1 = __fdiv_rn(1.0f, s);
+    c0 = s;
+  }
+}
+
+// (a, b) of unit r: the SEPW weights above, the half difference and half sum of a direction's two rows, or w[r] twice
+template <bool SYM, bool SEPW = false>
+__device__ __forceinline__ void row_weights(const float* __restrict__ w, int64_t r, float& a, float& b, int64_t D = 0,
+                                            const SepWeights* sepw = nullptr) {
+  if (SEPW) {
+    const float aw = __ldg(w + r);
+    a = fmaxf(aw, 0.0f);
+    // q is read only for the negative weights: a zero-weight row is never regenerated and never looks at its norm
+    b = (sepw->active && aw < 0.0f) ? __fdiv_rn((float)D * aw, __ldg(sepw->q + r)) : aw;
+  } else if (SYM) {
+    const float wp = __ldg(w + 2 * r), wm = __ldg(w + 2 * r + 1);
+    a = 0.5f * (wp - wm);
+    b = 0.5f * (wp + wm);
+  } else {
+    a = b = __ldg(w + r);
+  }
+}
+
+__device__ __forceinline__ void accumulate(float a, float b, float e, float c1, float c0, float& s1, float& s2) {
+  s1 = fmaf(a, e, s1);
+  s2 = fmaf(b, fmaf(e * e, c1, -c0), s2);
+}
+
+// (S1, S2) of this thread's VEC columns into row chunk `chunk` of the [chunk][2][D] workspace; TAIL: a column may lie past D
+template <int VEC, bool TAIL = true>
+__device__ __forceinline__ void store_partial(float* partial, int64_t chunk, int64_t D, int64_t col, const float* s1, const float* s2) {
+  float* p1 = partial + (chunk * 2 + 0) * D + col;
+  float* p2 = partial + (chunk * 2 + 1) * D + col;
+#pragma unroll
+  for (int c = 0; c < VEC; ++c) {
+    if (!TAIL || col + c < D) {
+      p1[c] = s1[c];
+      p2[c] = s2[c];
+    }
+  }
+}
+
 // SYM: unit r = direction (rows 2r, 2r+1), else unit r = row r.
 // SEPW (with kEpsRegen, non-symmetric, form MOMENTS, mu = sigma = NULL): the weights above, eps = z.
 template <int VEC, int TX, bool SYM, int EPS, bool SEPW = false>
-__global__ void __launch_bounds__(kGradThreads, EVOK_GRAD_MINB)
+__global__ void __launch_bounds__(kGradThreads, kGradMinBlocks)
     grad_partial_kernel(int form, const float* __restrict__ X, int64_t ldx, const float* __restrict__ w, const float* __restrict__ mu,
                         const float* __restrict__ sigma, int64_t n_units, int64_t D, int64_t units_per_chunk, uint64_t unit0,
                         const __grid_constant__ PhiloxKey key, const uint32_t* __restrict__ stream_off, float* __restrict__ partial,
@@ -102,16 +146,7 @@ __global__ void __launch_bounds__(kGradThreads, EVOK_GRAD_MINB)
     const float s = ok ? __ldg(sigma + col + c) : 1.0f;
     m[c] = ok ? __ldg(mu + col + c) : 0.0f;
     sg[c] = s;
-    if (form == EVOK_GRAD_EXP) {
-      c1[c] = __fdiv_rn(1.0f, s * s);
-      c0[c] = 1.0f;
-    } else if (form == EVOK_GRAD_MOMENTS) {
-      c1[c] = 1.0f;
-      c0[c] = 0.0f;
-    } else {
-      c1[c] = __fdiv_rn(1.0f, s);
-      c0[c] = s;
-    }
+    grad_coeffs(form, s, c1[c], c0[c]);
   }
 
   float s1[VEC], s2[VEC];
@@ -131,19 +166,8 @@ __global__ void __launch_bounds__(kGradThreads, EVOK_GRAD_MINB)
       const int64_t r = r0 + (int64_t)u * TY;
       a[u] = b[u] = 0.0f;
       if (r < r_end) {
-        if (SEPW) {
-          const float aw = __ldg(w + r);
-          a[u] = fmaxf(aw, 0.0f);
-          // q is read only for the negative weights: a zero-weight row is never regenerated and never looks at its norm
-          b[u] = (sepw.active && aw < 0.0f) ? __fdiv_rn((float)D * aw, __ldg(sepw.q + r)) : aw;
-          wb += b[u];
-        } else if (SYM) {
-          const float wp = __ldg(w + 2 * r), wm = __ldg(w + 2 * r + 1);
-          a[u] = 0.5f * (wp - wm);
-          b[u] = 0.5f * (wp + wm);
-        } else {
-          a[u] = b[u] = __ldg(w + r);
-        }
+        row_weights<SYM, SEPW>(w, r, a[u], b[u], D, &sepw);
+        if (SEPW) wb += b[u];
       }
       need[u] = active && (a[u] != 0.0f || b[u] != 0.0f);
     }
@@ -170,8 +194,7 @@ __global__ void __launch_bounds__(kGradThreads, EVOK_GRAD_MINB)
 #pragma unroll
         for (int c = 0; c < VEC; ++c) {
           const float e = EPS == kEpsRegen ? sg[c] * x[u].v[c] : EPS == kEpsRebuild ? fmaf(sg[c], x[u].v[c], m[c]) - m[c] : x[u].v[c] - m[c];
-          s1[c] = fmaf(a[u], e, s1[c]);
-          s2[c] = fmaf(b[u], fmaf(e * e, c1[c], -c0[c]), s2[c]);
+          accumulate(a[u], b[u], e, c1[c], c0[c], s1[c], s2[c]);
         }
       }
     }
@@ -199,17 +222,7 @@ __global__ void __launch_bounds__(kGradThreads, EVOK_GRAD_MINB)
       }
     }
   }
-  if (ty == 0 && active) {
-    float* p1 = partial + ((int64_t)blockIdx.y * 2 + 0) * D + col;
-    float* p2 = partial + ((int64_t)blockIdx.y * 2 + 1) * D + col;
-#pragma unroll
-    for (int c = 0; c < VEC; ++c) {
-      if (col + c < D) {
-        p1[c] = s1[c];
-        p2[c] = s2[c];
-      }
-    }
-  }
+  if (ty == 0 && active) store_partial<VEC>(partial, blockIdx.y, D, col, s1, s2);
   if (SEPW && blockIdx.x == 0) {  // uniform per CTA: every tile's row threads see the same rows, tile 0 reports their b sum
     __shared__ float wred[TY];
     if (tx == 0) wred[ty] = wb;
@@ -219,6 +232,16 @@ __global__ void __launch_bounds__(kGradThreads, EVOK_GRAD_MINB)
       for (int y = 1; y < TY; ++y) t += wred[y];
       sepw.wsum_partial[blockIdx.y] = t;
     }
+  }
+}
+
+// (S1, S2) of column j over the n_chunks row chunks, in chunk order: the fixed order that makes the result deterministic
+__device__ __forceinline__ void sum_chunks(const float* __restrict__ partial, int n_chunks, int64_t D, int64_t j, float& t1, float& t2) {
+  t1 = 0.0f;
+  t2 = 0.0f;
+  for (int c = 0; c < n_chunks; ++c) {
+    t1 += partial[((int64_t)c * 2 + 0) * D + j];
+    t2 += partial[((int64_t)c * 2 + 1) * D + j];
   }
 }
 
@@ -238,11 +261,8 @@ __global__ void __launch_bounds__(256) grad_finalize_kernel(const float* __restr
   partial += (int64_t)blockIdx.y * item_stride_partial;  // batched: blockIdx.y = item, outputs contiguous [items][D]
   out_mu += (int64_t)blockIdx.y * D;
   out_sigma += (int64_t)blockIdx.y * D;
-  float t1 = 0.0f, t2 = 0.0f;
-  for (int c = 0; c < n_chunks; ++c) {
-    t1 += partial[((int64_t)c * 2 + 0) * D + j];
-    t2 += partial[((int64_t)c * 2 + 1) * D + j];
-  }
+  float t1, t2;
+  sum_chunks(partial, n_chunks, D, j, t1, t2);
   out_mu[j] = t1 * scale_mu;
   out_sigma[j] = t2 * scale_sigma;
 }
@@ -261,11 +281,8 @@ __global__ void __launch_bounds__(256) grad_finalize_push_kernel(const float* __
                                                                  const unsigned long long* epoch, unsigned int* done) {
   const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (j < D) {
-    float t1 = 0.0f, t2 = 0.0f;
-    for (int c = 0; c < n_chunks; ++c) {
-      t1 += partial[((int64_t)c * 2 + 0) * D + j];
-      t2 += partial[((int64_t)c * 2 + 1) * D + j];
-    }
+    float t1, t2;
+    sum_chunks(partial, n_chunks, D, j, t1, t2);
     t1 *= scale_mu;
     t2 *= scale_sigma;
     for (int p = 0; p < sink.world; ++p) {
@@ -275,15 +292,6 @@ __global__ void __launch_bounds__(256) grad_finalize_push_kernel(const float* __
     }
   }
   peer_signal_tail(sink, epoch, done);
-}
-
-static int launch_finalize(const float* partial, int n_chunks, int64_t D, float scale_mu, float scale_sigma, float* out_mu, float* out_sigma,
-                           const GradPush* push, cudaStream_t st) {
-  const unsigned grid = (unsigned)((D + 255) / 256);
-  if (push) grad_finalize_push_kernel<<<grid, 256, 0, st>>>(partial, n_chunks, D, scale_mu, scale_sigma, push->sink, push->epoch, push->done);
-  else grad_finalize_kernel<<<grid, 256, 0, st>>>(partial, n_chunks, D, scale_mu, scale_sigma, out_mu, out_sigma);
-  EVOK_CHECK_LAUNCH();
-  return 0;
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -412,16 +420,7 @@ __global__ void __launch_bounds__(kTmaThreads, EVOK_GRAD_TMA_CTAS_PER_SM)
   for (int c = 0; c < 4; ++c) {
     sg[c] = active ? __ldg(sigma + col + c) : 1.0f;
     m[c] = active ? __ldg(mu + col + c) : 0.0f;
-    if (frm == EVOK_GRAD_EXP) {
-      c1[c] = __fdiv_rn(1.0f, sg[c] * sg[c]);
-      c0[c] = 1.0f;
-    } else if (frm == EVOK_GRAD_MOMENTS) {
-      c1[c] = 1.0f;
-      c0[c] = 0.0f;
-    } else {
-      c1[c] = __fdiv_rn(1.0f, sg[c]);
-      c0[c] = sg[c];
-    }
+    grad_coeffs(frm, sg[c], c1[c], c0[c]);
   }
   float s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
 
@@ -434,15 +433,7 @@ __global__ void __launch_bounds__(kTmaThreads, EVOK_GRAD_TMA_CTAS_PER_SM)
 #pragma unroll
     for (int i = 0; i < kTmaRows; ++i) {
       a[i] = b[i] = 0.0f;
-      if (i < rows) {
-        if (SYM) {
-          const float wp = __ldg(w + 2 * (r0 + i)), wm = __ldg(w + 2 * (r0 + i) + 1);
-          a[i] = 0.5f * (wp - wm);
-          b[i] = 0.5f * (wp + wm);
-        } else {
-          a[i] = b[i] = __ldg(w + r0 + i);
-        }
-      }
+      if (i < rows) row_weights<SYM>(w, r0 + i, a[i], b[i]);
       need[i] = a[i] != 0.0f || b[i] != 0.0f;
     }
     if (group_rebuilt(mask, g)) {
@@ -461,11 +452,7 @@ __global__ void __launch_bounds__(kTmaThreads, EVOK_GRAD_TMA_CTAS_PER_SM)
         for (int i = 0; i < kTmaRows; ++i) {
           if (need[i]) {
 #pragma unroll
-            for (int c = 0; c < 4; ++c) {
-              const float e = x[i][c] - m[c];
-              s1[c] = fmaf(a[i], e, s1[c]);
-              s2[c] = fmaf(b[i], fmaf(e * e, c1[c], -c0[c]), s2[c]);
-            }
+            for (int c = 0; c < 4; ++c) accumulate(a[i], b[i], x[i][c] - m[c], c1[c], c0[c], s1[c], s2[c]);
           }
         }
       }
@@ -486,71 +473,14 @@ __global__ void __launch_bounds__(kTmaThreads, EVOK_GRAD_TMA_CTAS_PER_SM)
           const float4 v = v4[i];
           const float x[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            const float e = x[c] - m[c];
-            s1[c] = fmaf(a[i], e, s1[c]);
-            s2[c] = fmaf(b[i], fmaf(e * e, c1[c], -c0[c]), s2[c]);
-          }
+          for (int c = 0; c < 4; ++c) accumulate(a[i], b[i], x[c] - m[c], c1[c], c0[c], s1[c], s2[c]);
         }
       }
     }
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[s]);
   }
-  if (active) {
-    float* p1 = partial + ((int64_t)blockIdx.y * 2 + 0) * D + col;
-    float* p2 = partial + ((int64_t)blockIdx.y * 2 + 1) * D + col;
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      p1[c] = s1[c];
-      p2[c] = s2[c];
-    }
-  }
-}
-
-struct GradPlan {
-  int vec, tx, n_coltiles, n_chunks;
-  int64_t units_per_chunk;
-};
-
-static GradPlan plan_grad(int64_t n_units, int64_t D, bool vec_ok) {
-  GradPlan p;
-  p.vec = vec_ok ? 4 : 1;
-  const int64_t col_threads = (D + p.vec - 1) / p.vec;
-  p.tx = 32;
-  while (p.tx < kGradThreads && p.tx < col_threads) p.tx <<= 1;
-  p.n_coltiles = (int)((col_threads + p.tx - 1) / p.tx);
-  const int ty = kGradThreads / p.tx;
-  int64_t chunks = (int64_t)kNumSMs * EVOK_GRAD_CTAS_PER_SM / p.n_coltiles;  // one wave of resident CTAs
-  // at least 16 unrolled iterations per CTA: fewer, fatter chunks keep the fixed-order finalisation short for small populations
-  const int64_t max_useful = (n_units + (int64_t)ty * kGradUnroll * 16 - 1) / ((int64_t)ty * kGradUnroll * 16);
-  if (chunks > max_useful) chunks = max_useful;
-  if (chunks < 1) chunks = 1;
-  if (chunks > 65535) chunks = 65535;
-  p.units_per_chunk = (n_units + chunks - 1) / chunks;
-  p.n_chunks = (int)((n_units + p.units_per_chunk - 1) / p.units_per_chunk);
-  if (p.n_chunks < 1) p.n_chunks = 1;
-  return p;
-}
-
-template <int VEC, bool SYM, int EPS, bool SEPW = false>
-static void launch_partial(const GradPlan& p, int form, const float* X, int64_t ldx, const float* w, const float* mu, const float* sigma,
-                           int64_t n_units, int64_t D, uint64_t unit0, uint64_t seed, uint64_t stream_id, const uint32_t* stream_off, float* partial,
-                           cudaStream_t st, int64_t n_items = 1, const GradItems* items = nullptr, const SepWeights* sep = nullptr) {
-  dim3 grid(p.n_coltiles, p.n_chunks, (unsigned)n_items);
-  const PhiloxKey key = make_philox_key(seed, stream_id);
-  const GradItems it = items ? *items : GradItems{0, 0, 0, 0, 0};
-  const SepWeights sw = sep ? *sep : SepWeights{nullptr, 0, nullptr};
-#define EVOK_LAUNCH_TX(TXV)                                                                                                               \
-  grad_partial_kernel<VEC, TXV, SYM, EPS, SEPW><<<grid, kGradThreads, 0, st>>>(form, X, ldx, w, mu, sigma, n_units, D, p.units_per_chunk, \
-                                                                                 unit0, key, stream_off, partial, it, sw)
-  switch (p.tx) {
-    case 32: EVOK_LAUNCH_TX(32); break;
-    case 64: EVOK_LAUNCH_TX(64); break;
-    case 128: EVOK_LAUNCH_TX(128); break;
-    default: EVOK_LAUNCH_TX(256); break;
-  }
-#undef EVOK_LAUNCH_TX
+  if (active) store_partial<4, false>(partial, blockIdx.y, D, col, s1, s2);
 }
 
 // Rebuilt groups per kSplitPeriod when the caller leaves the choice to the library, by the card's enforced power limit
@@ -614,62 +544,209 @@ static int device_auto_split() {
   return s - 1;
 }
 
-// split: rebuilt groups per kSplitPeriod in the TMA kernel (0 = stream every row, -1 = device_auto_split()); rows are rebuilt from
-// (seed, stream_id, *stream_off, row0), which must be the counters that sampled X from this mu and sigma.
-static int grad_impl(int form, const float* X, int64_t ldx, const float* w, const float* mu, const float* sigma, int64_t row0, int64_t n_rows,
-                     int64_t D, bool regen, uint64_t seed, uint64_t stream_id, const uint32_t* stream_off, float scale_mu, float scale_sigma, float* out_mu,
-                     float* out_sigma, void* ws, size_t ws_bytes, void* stream, const GradPush* push = nullptr, int split = 0) {
-  // an empty shard has no weights to point at (an empty CUDA tensor's data pointer is NULL)
-  if ((!w && n_rows != 0) || !mu || !sigma || !ws || (!regen && !X) || (!push && (!out_mu || !out_sigma))) return EVOK_E_NULLPTR;
-  if (form < EVOK_GRAD_SEPARABLE || form > EVOK_GRAD_MOMENTS) return EVOK_E_BADENUM;
-  if (n_rows < 0 || D <= 0 || row0 < 0 || (!regen && ldx < D) || split < -1 || split > kSplitPeriod) return EVOK_E_BADSIZE;
-  const bool sym = form == EVOK_GRAD_SYMMETRIC;
-  if (sym && ((n_rows & 1) || (row0 & 1))) return EVOK_E_ODDROWS;
-  if (ws_bytes < evok_grad_workspace_bytes(n_rows, D)) return EVOK_E_WORKSPACE;
-  cudaStream_t st = (cudaStream_t)stream;
-  const int64_t n_units = sym ? n_rows / 2 : n_rows;
-  const bool vec_ok = regen ? true : ((D % 4 == 0) && (ldx % 4 == 0) && aligned16(X));
+// ------------------------------------------------------------------------------------------------------------
+// Host side.  Every entry point describes its call as one GradCall and hands it to run_grad: one plan (plan_grad), one
+// partial launch per item chunk (launch_partial) and one finalisation (launch_finalize).  A single search runs as a batch of
+// one item: with zero item strides and grid z = 1 it takes the LDG plan a one-item batch takes, unless it qualifies for the
+// TMA kernel, which only single searches use.
+// ------------------------------------------------------------------------------------------------------------
+
+// One call of the gradient pass.  The constructor takes what every entry point gives; the other fields keep the defaults of a
+// single search without Philox counters, peers or separable CMA-ES weights.
+struct GradCall {
+  GradCall(int form, int eps, const float* w, const float* mu, const float* sigma, int64_t n_rows, int64_t D, float scale_mu, float scale_sigma,
+           float* out_mu, float* out_sigma, void* ws, size_t ws_bytes, void* stream)
+      : form(form), eps(eps), w(w), mu(mu), sigma(sigma), n_rows(n_rows), D(D), scale_mu(scale_mu), scale_sigma(scale_sigma), out_mu(out_mu),
+        out_sigma(out_sigma), ws(ws), ws_bytes(ws_bytes), st((cudaStream_t)stream) {}
+  int form;
+  int eps;                            // where eps comes from: X, or the Philox counters (kEpsRegen / kEpsRebuild)
+  const float* w;                     // [items][n_rows]
+  const float* mu;                    // NULL with sepw
+  const float* sigma;
+  int64_t n_rows, D;                  // rows per item, as the caller counts them (the symmetric form pairs them)
+  float scale_mu, scale_sigma;
+  float* out_mu;                      // [items][D]
+  float* out_sigma;
+  void* ws;
+  size_t ws_bytes;
+  cudaStream_t st;
+  const float* X = nullptr;           // kEpsRead: [items][n_rows][ldx]
+  int64_t ldx = 0;
+  int64_t row0 = 0;
+  PhiloxKey key{};                    // item b draws on stream word key.stream_lo + b
+  const uint32_t* stream_off = nullptr;
+  bool batched = false;               // evok_grad_batched / _batched_regen: the LDG plan of a batch, whatever the item count
+  int64_t n_items = 1;
+  GradItems items{0, 0, 0, 0, 0};     // element strides between the items' operands; run_grad sets .partial from the plan
+  int split = 0;                      // rebuilt groups per kSplitPeriod of the TMA kernel (-1 = device_auto_split())
+  SepWeights sepw{nullptr, 0, nullptr};  // the separable CMA-ES weight mode, with its weight sum into *wsum
+  float* wsum = nullptr;
+  const GradPush* push = nullptr;     // instead of out_mu / out_sigma: into every peer's slot
+};
+
+static bool is_sym(const GradCall& c) { return c.form == EVOK_GRAD_SYMMETRIC; }
+
+// The plan fixes the summation order, and with it the bits: the kernel, the column tiles, and the row chunks of every item.
+struct GradPlan {
+  bool tma;
+  int vec, tx, n_coltiles, n_chunks;  // vec, tx: the LDG kernel's columns per thread and column threads per CTA
+  int64_t n_units, units_per_chunk;
+};
+
+static void set_chunks(GradPlan& p, int64_t chunks) {
+  if (chunks < 1) chunks = 1;
+  if (chunks > 65535) chunks = 65535;
+  p.units_per_chunk = (p.n_units + chunks - 1) / chunks;
+  p.n_chunks = (int)((p.n_units + p.units_per_chunk - 1) / p.units_per_chunk);
+}
+
+// EVOK_GRAD_TMA=0 / 1 picks the LDG or TMA kernel, read per call (a getenv is ~100 ns): the parity tests run both in one process
+static bool tma_enabled() {
+  const char* env = getenv("EVOK_GRAD_TMA");
+  return env ? atoi(env) != 0 : EVOK_GRAD_TMA_DEFAULT != 0;
+}
+
+// For n_units > 0.
+static GradPlan plan_grad(const GradCall& c) {
+  GradPlan p{};
+  p.n_units = is_sym(c) ? c.n_rows / 2 : c.n_rows;
+  // 16-byte columns: always for regenerated rows, else when every item's X, mu and sigma allow them
+  const bool vec_ok = c.eps == kEpsRegen || (c.D % 4 == 0 && (c.eps == kEpsRebuild || (c.ldx % 4 == 0 && aligned16(c.X) && c.items.x % 4 == 0)) &&
+                                             c.items.mu % 4 == 0 && c.items.sigma % 4 == 0);
+  p.vec = vec_ok ? 4 : 1;
+  // the TMA kernel: a single search (not a batch, even of one item) over wide stored rows with enough of them to fill its ring
+  p.tma = !c.batched && c.eps == kEpsRead && vec_ok && c.form != EVOK_GRAD_MOMENTS && c.D >= 512 && p.n_units >= 4096 && tma_enabled();
+  if (p.tma) {
+    p.n_coltiles = (int)((c.D + kTmaCols - 1) / kTmaCols);
+    set_chunks(p, (int64_t)kNumSMs * EVOK_GRAD_TMA_CTAS_PER_SM / p.n_coltiles);
+    return p;
+  }
+  const int64_t col_threads = (c.D + p.vec - 1) / p.vec;
+  p.tx = 32;
+  while (p.tx < kGradThreads && p.tx < col_threads) p.tx <<= 1;
+  p.n_coltiles = (int)((col_threads + p.tx - 1) / p.tx);
+  const int ty = kGradThreads / p.tx;
+  int64_t chunks = (int64_t)kNumSMs * kGradCtasPerSm / p.n_coltiles;  // one wave of resident CTAs
+  // at least 16 unrolled iterations per CTA: fewer, fatter chunks keep the fixed-order finalisation short for small populations
+  const int64_t max_useful = (p.n_units + (int64_t)ty * kGradUnroll * 16 - 1) / ((int64_t)ty * kGradUnroll * 16);
+  set_chunks(p, chunks < max_useful ? chunks : max_useful);
+  // a batch fills the GPU: fewer row chunks per item keep the fixed-order finalisation short (one item never gets fewer)
+  chunks = ((int64_t)kNumSMs * kGradCtasPerSm + (int64_t)p.n_coltiles * c.n_items - 1) / ((int64_t)p.n_coltiles * c.n_items);
+  if (chunks < p.n_chunks) set_chunks(p, chunks);
+  // The rebuild always runs 4 columns per thread: one Philox group gives all 4 (a thread per column would draw each group 4
+  // times).  A column's sum depends only on the row threads per CTA (kGradThreads / tx) and the row chunks, so for the scalar
+  // plan it keeps that plan's tx and chunks, with a quarter of its column tiles, and gives the scalar read path's bits.
+  if (c.eps == kEpsRebuild && !vec_ok) {
+    p.vec = 4;
+    p.n_coltiles = (int)(((c.D + 3) / 4 + p.tx - 1) / p.tx);
+  }
+  return p;
+}
+
+// Every instantiation of grad_partial_kernel, by [row][tx]: row partial_row(...), tx 32, 64, 128, 256
+using PartialKernel = void (*)(int, const float*, int64_t, const float*, const float*, const float*, int64_t, int64_t, int64_t, uint64_t,
+                               PhiloxKey, const uint32_t*, float*, GradItems, SepWeights);
+#define EVOK_GRAD_TXS(VEC, SYM, EPS, SEPW)                                                                             \
+  {                                                                                                                    \
+    grad_partial_kernel<VEC, 32, SYM, EPS, SEPW>, grad_partial_kernel<VEC, 64, SYM, EPS, SEPW>,                        \
+        grad_partial_kernel<VEC, 128, SYM, EPS, SEPW>, grad_partial_kernel<VEC, 256, SYM, EPS, SEPW>                   \
+  }
+static const PartialKernel kPartialKernels[9][4] = {
+    EVOK_GRAD_TXS(1, false, kEpsRead, false),    EVOK_GRAD_TXS(1, true, kEpsRead, false),  EVOK_GRAD_TXS(4, false, kEpsRead, false),
+    EVOK_GRAD_TXS(4, true, kEpsRead, false),     EVOK_GRAD_TXS(4, false, kEpsRegen, false), EVOK_GRAD_TXS(4, true, kEpsRegen, false),
+    EVOK_GRAD_TXS(4, false, kEpsRebuild, false), EVOK_GRAD_TXS(4, true, kEpsRebuild, false), EVOK_GRAD_TXS(4, false, kEpsRegen, true)};
+#undef EVOK_GRAD_TXS
+
+// the SEPW mode, else (eps, vec, sym): the read kernels by vec, then one pair of rows per Philox mode
+static int partial_row(int eps, int vec, bool sym, bool sepw) { return sepw ? 8 : 2 * (eps == kEpsRead ? vec / 4 : 1 + eps) + (sym ? 1 : 0); }
+static int tx_index(int tx) { return tx == 32 ? 0 : tx == 64 ? 1 : tx == 128 ? 2 : 3; }
+
+// The partial sums of item chunk [b0, b0 + nb) into partial[item - b0][chunk][2][D]
+static void launch_partial(const GradCall& c, const GradPlan& p, int64_t b0, int64_t nb, float* partial) {
+  PhiloxKey key = c.key;
+  key.stream_lo += (uint32_t)b0;  // item b0 + z on stream word stream_lo + b0 + z, as the batched sampler draws it
+  const float* X = c.X + b0 * c.items.x;
+  const float* w = c.w + b0 * c.items.w;
+  const float* mu = c.mu + b0 * c.items.mu;
+  const float* sigma = c.sigma + b0 * c.items.sigma;
   // symmetric sampling keys its counters by direction; the regenerating kernel must use the same unit index
-  const uint64_t unit0 = (uint64_t)(sym ? row0 / 2 : row0);
-  float* partial = (float*)ws;
-  if (n_units == 0 && push) return launch_finalize(partial, 0, D, scale_mu, scale_sigma, nullptr, nullptr, push, st);  // zeros + this rank's flag
-  if (n_units == 0) {
-    cudaMemsetAsync(out_mu, 0, (size_t)D * 4, st);
-    cudaMemsetAsync(out_sigma, 0, (size_t)D * 4, st);
-    return 0;
-  }
-  const GradPlan p = plan_grad(n_units, D, vec_ok);  // after the empty case: plan_grad divides by the units per chunk
-  // read per call (a getenv is ~100 ns): the parity tests run both implementations in one process
-  const char* tma_env = getenv("EVOK_GRAD_TMA");
-  const int use_tma = tma_env ? atoi(tma_env) : EVOK_GRAD_TMA_DEFAULT;
-  if (use_tma && !regen && vec_ok && form != EVOK_GRAD_MOMENTS && D >= 512 && n_units >= 4096) {
-    const int n_coltiles = (int)((D + kTmaCols - 1) / kTmaCols);
-    int64_t chunks = (int64_t)kNumSMs * EVOK_GRAD_TMA_CTAS_PER_SM / n_coltiles;
-    if (chunks < 1) chunks = 1;
-    if (chunks > 65535) chunks = 65535;
-    const int64_t upc = (n_units + chunks - 1) / chunks;
-    const int n_chunks = (int)((n_units + upc - 1) / upc);
-    dim3 grid(n_coltiles, n_chunks);
-    const int rebuilt = split < 0 ? device_auto_split() : split;
-    const PhiloxKey key = make_philox_key(seed, stream_id);
-    auto kernel = sym ? grad_partial_tma_kernel<true> : grad_partial_tma_kernel<false>;
+  const uint64_t unit0 = (uint64_t)(is_sym(c) ? c.row0 / 2 : c.row0);
+  if (p.tma) {
+    const int rebuilt = c.split < 0 ? device_auto_split() : c.split;
+    auto kernel = is_sym(c) ? grad_partial_tma_kernel<true> : grad_partial_tma_kernel<false>;
     cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTmaSmemBytes);
-    kernel<<<grid, kTmaThreads, kTmaSmemBytes, st>>>(form, X, ldx, w, mu, sigma, n_units, D, upc, rebuilt, unit0, key, stream_off, partial);
-    EVOK_CHECK_LAUNCH();
-    return launch_finalize(partial, n_chunks, D, scale_mu, scale_sigma, out_mu, out_sigma, push, st);
+    kernel<<<dim3(p.n_coltiles, p.n_chunks), kTmaThreads, kTmaSmemBytes, c.st>>>(c.form, X, c.ldx, w, mu, sigma, p.n_units, c.D, p.units_per_chunk,
+                                                                                  rebuilt, unit0, key, c.stream_off, partial);
+    return;
   }
-  if (regen) {
-    if (sym) launch_partial<4, true, kEpsRegen>(p, form, X, ldx, w, mu, sigma, n_units, D, unit0, seed, stream_id, stream_off, partial, st);
-    else launch_partial<4, false, kEpsRegen>(p, form, X, ldx, w, mu, sigma, n_units, D, unit0, seed, stream_id, stream_off, partial, st);
-  } else if (vec_ok) {
-    if (sym) launch_partial<4, true, kEpsRead>(p, form, X, ldx, w, mu, sigma, n_units, D, unit0, seed, stream_id, stream_off, partial, st);
-    else launch_partial<4, false, kEpsRead>(p, form, X, ldx, w, mu, sigma, n_units, D, unit0, seed, stream_id, stream_off, partial, st);
+  const PartialKernel kernel = kPartialKernels[partial_row(c.eps, p.vec, is_sym(c), c.wsum != nullptr)][tx_index(p.tx)];
+  kernel<<<dim3(p.n_coltiles, p.n_chunks, (unsigned)nb), kGradThreads, 0, c.st>>>(c.form, X, c.ldx, w, mu, sigma, p.n_units, c.D,
+                                                                                    p.units_per_chunk, unit0, key, c.stream_off, partial, c.items, c.sepw);
+}
+
+// Adds the n_chunks row chunks of item chunk [b0, b0 + nb) in order into the outputs: out_mu / out_sigma (with the SEPW weight
+// sum into *wsum), or this rank's slot of every peer (push)
+static int launch_finalize(const GradCall& c, int n_chunks, int64_t b0, int64_t nb, const float* partial) {
+  const unsigned grid = (unsigned)((c.D + 255) / 256);
+  if (c.push) {
+    grad_finalize_push_kernel<<<grid, 256, 0, c.st>>>(partial, n_chunks, c.D, c.scale_mu, c.scale_sigma, c.push->sink, c.push->epoch, c.push->done);
+  } else if (c.wsum) {
+    grad_finalize_kernel<true><<<grid, 256, 0, c.st>>>(partial, n_chunks, c.D, c.scale_mu, c.scale_sigma, c.out_mu, c.out_sigma, 0, c.sepw.wsum_partial,
+                                                       c.wsum);
   } else {
-    if (sym) launch_partial<1, true, kEpsRead>(p, form, X, ldx, w, mu, sigma, n_units, D, unit0, seed, stream_id, stream_off, partial, st);
-    else launch_partial<1, false, kEpsRead>(p, form, X, ldx, w, mu, sigma, n_units, D, unit0, seed, stream_id, stream_off, partial, st);
+    grad_finalize_kernel<<<dim3(grid, (unsigned)nb), 256, 0, c.st>>>(partial, n_chunks, c.D, c.scale_mu, c.scale_sigma, c.out_mu + b0 * c.D,
+                                                                     c.out_sigma + b0 * c.D, c.items.partial);
   }
   EVOK_CHECK_LAUNCH();
-  return launch_finalize(partial, p.n_chunks, D, scale_mu, scale_sigma, out_mu, out_sigma, push, st);
+  return 0;
+}
+
+// A checked call: the empty case, the plan, then the partial and final kernels of every item chunk
+static int run_grad(GradCall c) {
+  if (c.n_items == 0) return 0;
+  float* partial = (float*)c.ws;
+  if ((is_sym(c) ? c.n_rows / 2 : c.n_rows) == 0) {
+    if (c.push) return launch_finalize(c, 0, 0, 1, partial);  // zeros + this rank's flag
+    cudaMemsetAsync(c.out_mu, 0, (size_t)c.n_items * c.D * 4, c.st);
+    cudaMemsetAsync(c.out_sigma, 0, (size_t)c.n_items * c.D * 4, c.st);
+    return 0;
+  }
+  const GradPlan p = plan_grad(c);  // after the empty case: the plan divides by the units per chunk
+  c.items.partial = (int64_t)p.n_chunks * 2 * c.D;
+  // grid z / y hold at most kMaxGridY items: larger batches run as item chunks with the plan above, in order on the stream, each
+  // reusing the partial sums of the previous one
+  const int64_t chunk = c.n_items < kMaxGridY ? c.n_items : kMaxGridY;
+  if (c.ws_bytes < (size_t)chunk * c.items.partial * sizeof(float)) return EVOK_E_WORKSPACE;
+  return for_item_chunks(c.n_items, kMaxGridY, [&](int64_t b0, int64_t nb) {
+    launch_partial(c, p, b0, nb, partial);
+    EVOK_CHECK_LAUNCH();
+    return launch_finalize(c, p.n_chunks, b0, nb, partial);
+  });
+}
+
+static bool bad_form(int form) { return form < EVOK_GRAD_SEPARABLE || form > EVOK_GRAD_MOMENTS; }
+
+// The checks of evok_grad, _regen, _hybrid and _push (after the push's own), in this order, then the pass
+static int grad_single(const GradCall& c) {
+  const bool read = c.eps == kEpsRead;
+  // an empty shard has no weights to point at (an empty CUDA tensor's data pointer is NULL)
+  if ((!c.w && c.n_rows != 0) || !c.mu || !c.sigma || !c.ws || (read && !c.X) || (!c.push && (!c.out_mu || !c.out_sigma))) return EVOK_E_NULLPTR;
+  if (bad_form(c.form)) return EVOK_E_BADENUM;
+  if (c.n_rows < 0 || c.D <= 0 || c.row0 < 0 || (read && c.ldx < c.D) || c.split < -1 || c.split > kSplitPeriod) return EVOK_E_BADSIZE;
+  if (is_sym(c) && ((c.n_rows & 1) || (c.row0 & 1))) return EVOK_E_ODDROWS;
+  if (c.ws_bytes < evok_grad_workspace_bytes(c.n_rows, c.D)) return EVOK_E_WORKSPACE;
+  return run_grad(c);
+}
+
+// The checks of evok_grad_batched and evok_grad_batched_regen, in this order, then the pass
+static int grad_batched(const GradCall& c) {
+  const bool read = c.eps == kEpsRead;
+  if ((read && !c.X) || !c.w || !c.mu || !c.sigma || !c.out_mu || !c.out_sigma || !c.ws) return EVOK_E_NULLPTR;
+  if (bad_form(c.form)) return EVOK_E_BADENUM;
+  if (c.n_items < 0 || c.n_rows < 0 || c.D <= 0 || (read && c.ldx < c.D) || c.items.x < 0 || c.items.mu < 0 || c.items.sigma < 0)
+    return EVOK_E_BADSIZE;
+  if (is_sym(c) && (c.n_rows & 1)) return EVOK_E_ODDROWS;
+  return run_grad(c);
 }
 
 }  // namespace evok
@@ -686,21 +763,35 @@ extern "C" EVOK_API size_t evok_grad_workspace_bytes(int64_t n_rows, int64_t D) 
 extern "C" EVOK_API int evok_grad(int form, const float* X, int64_t ldx, const float* w, const float* mu, const float* sigma, int64_t n_rows,
                          int64_t D, float scale_mu, float scale_sigma, float* out_mu, float* out_sigma, void* ws, size_t ws_bytes,
                          void* stream) {
-  return grad_impl(form, X, ldx, w, mu, sigma, 0, n_rows, D, false, 0, 0, nullptr, scale_mu, scale_sigma, out_mu, out_sigma, ws, ws_bytes, stream);
+  GradCall c(form, kEpsRead, w, mu, sigma, n_rows, D, scale_mu, scale_sigma, out_mu, out_sigma, ws, ws_bytes, stream);
+  c.X = X;
+  c.ldx = ldx;
+  return grad_single(c);
 }
 
 extern "C" EVOK_API int evok_grad_regen(int form, const float* w, const float* mu, const float* sigma, int64_t row0, int64_t n_rows, int64_t D,
                                uint64_t seed, uint64_t stream_id, const uint32_t* stream_offset_dev, float scale_mu, float scale_sigma,
                                float* out_mu, float* out_sigma, void* ws, size_t ws_bytes, void* stream) {
-  return grad_impl(form, nullptr, 0, w, mu, sigma, row0, n_rows, D, true, seed, stream_id, stream_offset_dev, scale_mu, scale_sigma, out_mu, out_sigma, ws,
-                   ws_bytes, stream);
+  GradCall c(form, kEpsRegen, w, mu, sigma, n_rows, D, scale_mu, scale_sigma, out_mu, out_sigma, ws, ws_bytes, stream);
+  c.row0 = row0;
+  c.key = make_philox_key(seed, stream_id);
+  c.stream_off = stream_offset_dev;
+  return grad_single(c);
 }
 
+// split: rebuilt groups per kSplitPeriod in the TMA kernel (0 = stream every row, -1 = device_auto_split()); rows are rebuilt from
+// (seed, stream_id, *stream_off, row0), which must be the counters that sampled X from this mu and sigma.
 extern "C" EVOK_API int evok_grad_hybrid(int form, const float* X, int64_t ldx, const float* w, const float* mu, const float* sigma, int64_t row0,
                                          int64_t n_rows, int64_t D, uint64_t seed, uint64_t stream_id, const uint32_t* stream_offset_dev, int split,
                                          float scale_mu, float scale_sigma, float* out_mu, float* out_sigma, void* ws, size_t ws_bytes, void* stream) {
-  return grad_impl(form, X, ldx, w, mu, sigma, row0, n_rows, D, false, seed, stream_id, stream_offset_dev, scale_mu, scale_sigma, out_mu, out_sigma, ws,
-                   ws_bytes, stream, nullptr, split);
+  GradCall c(form, kEpsRead, w, mu, sigma, n_rows, D, scale_mu, scale_sigma, out_mu, out_sigma, ws, ws_bytes, stream);
+  c.X = X;
+  c.ldx = ldx;
+  c.row0 = row0;
+  c.key = make_philox_key(seed, stream_id);
+  c.stream_off = stream_offset_dev;
+  c.split = split;
+  return grad_single(c);
 }
 
 extern "C" EVOK_API int evok_grad_auto_split(int64_t power_limit_mw) { return auto_split_for_power(power_limit_mw); }
@@ -708,7 +799,7 @@ extern "C" EVOK_API int evok_grad_auto_split(int64_t power_limit_mw) { return au
 extern "C" EVOK_API int64_t evok_grad_power_limit_mw(int device) { return enforced_power_limit_mw(device); }
 
 extern "C" EVOK_API size_t evok_sepcma_workspace_bytes(int64_t n_rows, int64_t D) {
-  // the gradient partials, then one float per row chunk (plan_grad: at most kNumSMs * EVOK_GRAD_CTAS_PER_SM chunks)
+  // the gradient partials, then one float per row chunk (plan_grad: at most kNumSMs * kGradCtasPerSm chunks)
   return evok_grad_workspace_bytes(n_rows, D) + (size_t)kMaxResidentCtas * sizeof(float);
 }
 
@@ -718,16 +809,13 @@ extern "C" EVOK_API int evok_sepcma_moments(const float* aw, const float* q, int
   if (!aw || (active && !q) || !local || !S2 || !wsum || !ws) return EVOK_E_NULLPTR;
   if (n_rows <= 0 || D <= 0 || row0 < 0) return EVOK_E_BADSIZE;
   if (ws_bytes < evok_sepcma_workspace_bytes(n_rows, D)) return EVOK_E_WORKSPACE;
-  cudaStream_t st = (cudaStream_t)stream;
-  const GradPlan p = plan_grad(n_rows, D, true);
-  float* partial = (float*)ws;
-  const SepWeights sep{q, active, partial + evok_grad_workspace_bytes(n_rows, D) / sizeof(float)};
-  launch_partial<4, false, kEpsRegen, true>(p, EVOK_GRAD_MOMENTS, nullptr, 0, aw, nullptr, nullptr, n_rows, D, (uint64_t)row0, seed, stream_id,
-                                       stream_offset_dev, partial, st, 1, nullptr, &sep);
-  EVOK_CHECK_LAUNCH();
-  grad_finalize_kernel<true><<<(unsigned)((D + 255) / 256), 256, 0, st>>>(partial, p.n_chunks, D, 1.0f, 1.0f, local, S2, 0, sep.wsum_partial, wsum);
-  EVOK_CHECK_LAUNCH();
-  return 0;
+  GradCall c(EVOK_GRAD_MOMENTS, kEpsRegen, aw, nullptr, nullptr, n_rows, D, 1.0f, 1.0f, local, S2, ws, ws_bytes, stream);
+  c.row0 = row0;
+  c.key = make_philox_key(seed, stream_id);
+  c.stream_off = stream_offset_dev;
+  c.sepw = SepWeights{q, active, (float*)ws + evok_grad_workspace_bytes(n_rows, D) / sizeof(float)};
+  c.wsum = wsum;
+  return run_grad(c);
 }
 
 extern "C" EVOK_API int evok_grad_push(int form, const float* X, int64_t ldx, const float* w, const float* mu, const float* sigma, int64_t row0,
@@ -746,8 +834,14 @@ extern "C" EVOK_API int evok_grad_push(int form, const float* X, int64_t ldx, co
   }
   push.epoch = reinterpret_cast<const unsigned long long*>(epoch_dev);
   push.done = done_dev;
-  return grad_impl(form, X, X ? ldx : 0, w, mu, sigma, row0, n_rows, D, X == nullptr, seed, stream_id, stream_offset_dev, scale_mu, scale_sigma, nullptr,
-                   nullptr, ws, ws_bytes, stream, &push);
+  GradCall c(form, X ? kEpsRead : kEpsRegen, w, mu, sigma, n_rows, D, scale_mu, scale_sigma, nullptr, nullptr, ws, ws_bytes, stream);
+  c.X = X;
+  c.ldx = X ? ldx : 0;
+  c.row0 = row0;
+  c.key = make_philox_key(seed, stream_id);
+  c.stream_off = stream_offset_dev;
+  c.push = &push;
+  return grad_single(c);
 }
 
 // Batched searches: n_items independent weighted column reductions in ONE launch chain (blockIdx.z = item).  X: [items][n_rows][D]
@@ -760,93 +854,29 @@ extern "C" EVOK_API size_t evok_grad_batched_workspace_bytes(int64_t n_items, in
   return ((size_t)kMaxResidentCtas * 1024 + 4 * (size_t)n_items * (size_t)D + 64) * sizeof(float);
 }
 
-// evok_grad_batched (X given) and evok_grad_batched_regen (X null: every needed row rebuilt from (seed, stream_id0 + item) as
-// the batched sampler stored it) after their argument checks: one plan, one workspace layout, one launch chain per item chunk.
-// The rebuilt rows take the plan of a contiguous, 16-byte aligned X [items][n_rows][D], so both give the same bits.
-static int grad_batched_impl(int form, const float* X, int64_t item_stride_x, int64_t ldx, const float* w, const float* mu, int64_t item_stride_mu,
-                             const float* sigma, int64_t item_stride_sigma, int64_t n_items, int64_t n_rows, int64_t D, uint64_t seed, uint64_t stream_id0,
-                             float scale_mu, float scale_sigma, float* out_mu, float* out_sigma, void* ws, size_t ws_bytes, cudaStream_t st) {
-  const bool sym = form == EVOK_GRAD_SYMMETRIC;
-  const int64_t n_units = sym ? n_rows / 2 : n_rows;
-  if (n_units == 0) {
-    cudaMemsetAsync(out_mu, 0, (size_t)n_items * D * 4, st);
-    cudaMemsetAsync(out_sigma, 0, (size_t)n_items * D * 4, st);
-    return 0;
-  }
-  const bool rebuild = X == nullptr;
-  const bool x_vec = rebuild || ((ldx % 4 == 0) && aligned16(X) && item_stride_x % 4 == 0);
-  const bool vec_ok = (D % 4 == 0) && x_vec && item_stride_mu % 4 == 0 && item_stride_sigma % 4 == 0;
-  GradPlan p = plan_grad(n_units, D, vec_ok);
-  // the batch fills the GPU: fewer row chunks per item keep the fixed-order finalisation short
-  int64_t chunks = ((int64_t)kNumSMs * EVOK_GRAD_CTAS_PER_SM + (int64_t)p.n_coltiles * n_items - 1) / ((int64_t)p.n_coltiles * n_items);
-  if (chunks < p.n_chunks) {
-    if (chunks < 1) chunks = 1;
-    p.units_per_chunk = (n_units + chunks - 1) / chunks;
-    p.n_chunks = (int)((n_units + p.units_per_chunk - 1) / p.units_per_chunk);
-  }
-  GradItems items;
-  items.x = rebuild ? 0 : item_stride_x;
-  items.w = n_rows;
-  items.mu = item_stride_mu;
-  items.sigma = item_stride_sigma;
-  items.partial = (int64_t)p.n_chunks * 2 * D;
-  // grid z / y hold at most kMaxGridY items: larger batches run as item chunks with the plan above, in order on the stream, each
-  // reusing the partial sums of the previous one
-  const int64_t chunk = n_items < kMaxGridY ? n_items : kMaxGridY;
-  if (ws_bytes < (size_t)chunk * items.partial * sizeof(float)) return EVOK_E_WORKSPACE;
-  float* partial = (float*)ws;
-  // The rebuild always runs 4 columns per thread: one Philox group gives all 4 (a thread per column would draw each group 4
-  // times).  A column's sum depends only on the row threads per CTA (kGradThreads / tx) and the row chunks, so for the scalar
-  // plan it keeps that plan's tx and chunks, with a quarter of its column tiles, and gives the scalar read path's bits.
-  GradPlan rp = p;
-  if (rebuild && !vec_ok) rp.n_coltiles = (int)(((D + 3) / 4 + p.tx - 1) / p.tx);
-  return for_item_chunks(n_items, kMaxGridY, [&](int64_t b0, int64_t nb) {
-    const float* Xc = rebuild ? nullptr : X + b0 * item_stride_x;
-    const float* wc = w + b0 * n_rows;
-    const float* muc = mu + b0 * item_stride_mu;
-    const float* sgc = sigma + b0 * item_stride_sigma;
-    // item b0 + z rebuilds on stream word (stream_lo of stream_id0) + b0 + z, as the batched sampler draws it
-    const uint64_t sid = (stream_id0 & ~0xffffffffull) | (uint32_t)(stream_id0 + (uint64_t)b0);
-    if (rebuild) {
-      if (sym) launch_partial<4, true, kEpsRebuild>(rp, form, Xc, ldx, wc, muc, sgc, n_units, D, 0, seed, sid, nullptr, partial, st, nb, &items);
-      else launch_partial<4, false, kEpsRebuild>(rp, form, Xc, ldx, wc, muc, sgc, n_units, D, 0, seed, sid, nullptr, partial, st, nb, &items);
-    } else if (vec_ok) {
-      if (sym) launch_partial<4, true, kEpsRead>(p, form, Xc, ldx, wc, muc, sgc, n_units, D, 0, 0, 0, nullptr, partial, st, nb, &items);
-      else launch_partial<4, false, kEpsRead>(p, form, Xc, ldx, wc, muc, sgc, n_units, D, 0, 0, 0, nullptr, partial, st, nb, &items);
-    } else {
-      if (sym) launch_partial<1, true, kEpsRead>(p, form, Xc, ldx, wc, muc, sgc, n_units, D, 0, 0, 0, nullptr, partial, st, nb, &items);
-      else launch_partial<1, false, kEpsRead>(p, form, Xc, ldx, wc, muc, sgc, n_units, D, 0, 0, 0, nullptr, partial, st, nb, &items);
-    }
-    EVOK_CHECK_LAUNCH();
-    grad_finalize_kernel<<<dim3((unsigned)((D + 255) / 256), (unsigned)nb), 256, 0, st>>>(partial, p.n_chunks, D, scale_mu, scale_sigma,
-                                                                                          out_mu + b0 * D, out_sigma + b0 * D, items.partial);
-    EVOK_CHECK_LAUNCH();
-    return 0;
-  });
-}
-
 extern "C" EVOK_API int evok_grad_batched(int form, const float* X, int64_t item_stride_x, int64_t ldx, const float* w, const float* mu,
                                           int64_t item_stride_mu, const float* sigma, int64_t item_stride_sigma, int64_t n_items, int64_t n_rows,
                                           int64_t D, float scale_mu, float scale_sigma, float* out_mu, float* out_sigma, void* ws, size_t ws_bytes,
                                           void* stream) {
-  if (!X || !w || !mu || !sigma || !out_mu || !out_sigma || !ws) return EVOK_E_NULLPTR;
-  if (form < EVOK_GRAD_SEPARABLE || form > EVOK_GRAD_MOMENTS) return EVOK_E_BADENUM;
-  if (n_items < 0 || n_rows < 0 || D <= 0 || ldx < D) return EVOK_E_BADSIZE;
-  if (form == EVOK_GRAD_SYMMETRIC && (n_rows & 1)) return EVOK_E_ODDROWS;
-  if (n_items == 0) return 0;
-  return grad_batched_impl(form, X, item_stride_x, ldx, w, mu, item_stride_mu, sigma, item_stride_sigma, n_items, n_rows, D, 0, 0, scale_mu,
-                           scale_sigma, out_mu, out_sigma, ws, ws_bytes, (cudaStream_t)stream);
+  GradCall c(form, kEpsRead, w, mu, sigma, n_rows, D, scale_mu, scale_sigma, out_mu, out_sigma, ws, ws_bytes, stream);
+  c.X = X;
+  c.ldx = ldx;
+  c.batched = true;
+  c.n_items = n_items;
+  c.items = GradItems{item_stride_x, n_rows, item_stride_mu, item_stride_sigma, 0};
+  return grad_batched(c);
 }
 
+// Every needed row rebuilt from (seed, stream_id0 + item) as the batched sampler stored it.  The rebuilt rows take the plan of a
+// contiguous, 16-byte aligned X [items][n_rows][D], so both entry points give the same bits.
 extern "C" EVOK_API int evok_grad_batched_regen(int form, const float* w, const float* mu, int64_t item_stride_mu, const float* sigma,
                                                 int64_t item_stride_sigma, int64_t n_items, int64_t n_rows, int64_t D, uint64_t seed,
                                                 uint64_t stream_id0, float scale_mu, float scale_sigma, float* out_mu, float* out_sigma, void* ws,
                                                 size_t ws_bytes, void* stream) {
-  if (!w || !mu || !sigma || !out_mu || !out_sigma || !ws) return EVOK_E_NULLPTR;
-  if (form < EVOK_GRAD_SEPARABLE || form > EVOK_GRAD_MOMENTS) return EVOK_E_BADENUM;
-  if (n_items < 0 || n_rows < 0 || D <= 0 || item_stride_mu < 0 || item_stride_sigma < 0) return EVOK_E_BADSIZE;
-  if (form == EVOK_GRAD_SYMMETRIC && (n_rows & 1)) return EVOK_E_ODDROWS;
-  if (n_items == 0) return 0;
-  return grad_batched_impl(form, nullptr, 0, D, w, mu, item_stride_mu, sigma, item_stride_sigma, n_items, n_rows, D, seed, stream_id0, scale_mu,
-                           scale_sigma, out_mu, out_sigma, ws, ws_bytes, (cudaStream_t)stream);
+  GradCall c(form, kEpsRebuild, w, mu, sigma, n_rows, D, scale_mu, scale_sigma, out_mu, out_sigma, ws, ws_bytes, stream);
+  c.key = make_philox_key(seed, stream_id0);
+  c.batched = true;
+  c.n_items = n_items;
+  c.items = GradItems{0, n_rows, item_stride_mu, item_stride_sigma, 0};
+  return grad_batched(c);
 }

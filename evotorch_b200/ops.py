@@ -222,15 +222,9 @@ def grad_push(form: int, X: Optional[torch.Tensor], w: torch.Tensor, mu: torch.T
               scale_sigma: float, peer, seed: int = 0, stream_id: int = 0, row0: int = 0, stream_offset: Optional[torch.Tensor] = None) -> None:
     """K4 with the send half of the gradient all-reduce fused in (X = None: regenerate the rows from the Philox counters).
     Follow with `peer.reduce_gradients()`."""
-    n, D = w.numel(), mu.numel()
-    _vec(w, "weights"); _vec(mu, "mu"); _vec(sigma, "sigma", D)
-    ldx = _ldx(X, n, D)
-    ws = nat.workspace(mu.device, nat.lib().evok_grad_workspace_bytes(n, D), "grad")
-    with _timed("grad" if X is not None else "grad_regen"):
-        rc = nat.lib().evok_grad_push(form, nat.ptr(X), ldx, w.data_ptr(), mu.data_ptr(), sigma.data_ptr(), row0, n, D, seed, stream_id,
-                                      _offset_ptr(stream_offset), scale_mu, scale_sigma, peer.world, peer.rank, peer.peer_slots,
-                                      peer.peer_flags_g, peer.epoch_g, peer._counter(1), ws.data_ptr(), ws.numel(), nat.stream_of(mu))
-    nat.check(rc, "evok_grad_push")
+    _grad_call("evok_grad_push", "grad" if X is not None else "grad_regen", X, w, mu, sigma, None, lambda ldx, n, D, _: (
+        form, nat.ptr(X), ldx, w.data_ptr(), mu.data_ptr(), sigma.data_ptr(), row0, n, D, seed, stream_id, _offset_ptr(stream_offset), scale_mu,
+        scale_sigma, peer.world, peer.rank, peer.peer_slots, peer.peer_flags_g, peer.epoch_g, peer._counter(1)))
 
 
 def evaluate(objective: int, X: torch.Tensor, f: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -389,33 +383,38 @@ def elite_mask(w: torch.Tensor, num_elites: int) -> torch.Tensor:
 
 
 # ------------------------------------------------------------------------------------------------ K4
+def _grad_call(entry: str, group: str, X: Optional[torch.Tensor], w: torch.Tensor, mu: torch.Tensor, sigma: torch.Tensor, outs, args):
+    """The part of `grad`, `grad_regen`, `grad_hybrid` and `grad_push` they share: the checks of the samples X (n x D) when given,
+    else n = len(w) and D = len(mu), then of w, mu and sigma against them; the outputs of `_out_pair(mu, *outs)` (`outs` None: the
+    push writes none); then `entry`(*args(ldx, n, D, outputs), workspace, its size, stream) on X's device and stream (mu's without
+    X), timed as `group`.  Returns the outputs."""
+    if X is not None:
+        _mat(X, "samples")
+        n, D = X.shape
+    else:
+        n, D = w.numel(), mu.numel()
+    _vec(w, "weights", n); _vec(mu, "mu", D); _vec(sigma, "sigma", D)
+    on = mu if X is None else X
+    out = None if outs is None else _out_pair(mu, *outs)
+    ws = nat.workspace(on.device, nat.lib().evok_grad_workspace_bytes(n, D), "grad")
+    with _timed(group):
+        rc = getattr(nat.lib(), entry)(*args(0 if X is None else X.stride(0), n, D, out), ws.data_ptr(), ws.numel(), nat.stream_of(on))
+    nat.check(rc, entry)
+    return out
+
+
 def grad(form: int, X: torch.Tensor, w: torch.Tensor, mu: torch.Tensor, sigma: torch.Tensor, scale_mu: float, scale_sigma: float,
          out_mu: Optional[torch.Tensor] = None, out_sigma: Optional[torch.Tensor] = None) -> tuple:
-    _mat(X, "samples")
-    n, D = X.shape
-    _vec(w, "weights", n); _vec(mu, "mu", D); _vec(sigma, "sigma", D)
-    out_mu, out_sigma = _out_pair(mu, out_mu, out_sigma)
-    ws = nat.workspace(X.device, nat.lib().evok_grad_workspace_bytes(n, D), "grad")
-    with _timed("grad"):
-        rc = nat.lib().evok_grad(form, X.data_ptr(), X.stride(0), w.data_ptr(), mu.data_ptr(), sigma.data_ptr(), n, D, scale_mu,
-                                 scale_sigma, out_mu.data_ptr(), out_sigma.data_ptr(), ws.data_ptr(), ws.numel(), nat.stream_of(X))
-    nat.check(rc, "evok_grad")
-    return out_mu, out_sigma
+    return _grad_call("evok_grad", "grad", X, w, mu, sigma, (out_mu, out_sigma), lambda ldx, n, D, out: (
+        form, X.data_ptr(), ldx, w.data_ptr(), mu.data_ptr(), sigma.data_ptr(), n, D, scale_mu, scale_sigma, out[0].data_ptr(), out[1].data_ptr()))
 
 
 def grad_regen(form: int, w: torch.Tensor, mu: torch.Tensor, sigma: torch.Tensor, *, seed: int, stream_id: int, row0: int,
                scale_mu: float, scale_sigma: float, out_mu: Optional[torch.Tensor] = None,
                out_sigma: Optional[torch.Tensor] = None, stream_offset: Optional[torch.Tensor] = None) -> tuple:
-    n, D = w.numel(), mu.numel()
-    _vec(w, "weights"); _vec(mu, "mu"); _vec(sigma, "sigma", D)
-    out_mu, out_sigma = _out_pair(mu, out_mu, out_sigma)
-    ws = nat.workspace(mu.device, nat.lib().evok_grad_workspace_bytes(n, D), "grad")
-    with _timed("grad_regen"):
-        rc = nat.lib().evok_grad_regen(form, w.data_ptr(), mu.data_ptr(), sigma.data_ptr(), row0, n, D, seed, stream_id,
-                                       _offset_ptr(stream_offset), scale_mu, scale_sigma, out_mu.data_ptr(), out_sigma.data_ptr(),
-                                       ws.data_ptr(), ws.numel(), nat.stream_of(mu))
-    nat.check(rc, "evok_grad_regen")
-    return out_mu, out_sigma
+    return _grad_call("evok_grad_regen", "grad_regen", None, w, mu, sigma, (out_mu, out_sigma), lambda ldx, n, D, out: (
+        form, w.data_ptr(), mu.data_ptr(), sigma.data_ptr(), row0, n, D, seed, stream_id, _offset_ptr(stream_offset), scale_mu, scale_sigma,
+        out[0].data_ptr(), out[1].data_ptr()))
 
 
 GRAD_SPLIT_PERIOD = 16  # `split` of grad_hybrid counts rebuilt row groups per this many
@@ -427,19 +426,11 @@ def grad_hybrid(form: int, X: torch.Tensor, w: torch.Tensor, mu: torch.Tensor, s
     """`grad` over an X that `sample_eval` wrote from this very `mu` / `sigma` with the same seed, stream_id, row0 and
     stream_offset: `split` of every GRAD_SPLIT_PERIOD row groups are rebuilt from their Philox counters instead of being read
     (-1 = the library's choice).  Bit-identical to `grad(form, X, ...)` for every split."""
-    _mat(X, "samples")
-    n, D = X.shape
-    _vec(w, "weights", n); _vec(mu, "mu", D); _vec(sigma, "sigma", D)
     if not -1 <= split <= GRAD_SPLIT_PERIOD:
         raise ValueError(f"split: expected -1 .. {GRAD_SPLIT_PERIOD}, got {split}")
-    out_mu, out_sigma = _out_pair(mu, out_mu, out_sigma)
-    ws = nat.workspace(X.device, nat.lib().evok_grad_workspace_bytes(n, D), "grad")
-    with _timed("grad_hybrid"):
-        rc = nat.lib().evok_grad_hybrid(form, X.data_ptr(), X.stride(0), w.data_ptr(), mu.data_ptr(), sigma.data_ptr(), row0, n, D,
-                                        seed, stream_id, _offset_ptr(stream_offset), int(split), scale_mu, scale_sigma,
-                                        out_mu.data_ptr(), out_sigma.data_ptr(), ws.data_ptr(), ws.numel(), nat.stream_of(X))
-    nat.check(rc, "evok_grad_hybrid")
-    return out_mu, out_sigma
+    return _grad_call("evok_grad_hybrid", "grad_hybrid", X, w, mu, sigma, (out_mu, out_sigma), lambda ldx, n, D, out: (
+        form, X.data_ptr(), ldx, w.data_ptr(), mu.data_ptr(), sigma.data_ptr(), row0, n, D, seed, stream_id, _offset_ptr(stream_offset),
+        int(split), scale_mu, scale_sigma, out[0].data_ptr(), out[1].data_ptr()))
 
 
 # ------------------------------------------------------------------------------------------------ K5
@@ -613,26 +604,33 @@ def weights_adjust_batched_(w: torch.Tensor, mode: int) -> torch.Tensor:
     return w
 
 
+def _grad_batched_call(entry: str, group: str, w: torch.Tensor, mu: torch.Tensor, sigma: torch.Tensor, B: int, n: int, d: int, args) -> tuple:
+    """The checks of `grad_batched` and `grad_batched_regen` (w: (B, n), mu / sigma: (d,) or (B, d)), then
+    `entry`(*args(mu, item stride of mu, sigma, item stride of sigma), outputs, workspace, its size, stream) timed as `group`."""
+    w = _rows(w, "w", (B, n))
+    mu, bm, sm = _items(mu, (d,), "mu")
+    sigma, bs, ss = _items(sigma, (d,), "sigma")
+    for cnt in (bm, bs):
+        if cnt is not None and cnt != B:
+            raise ValueError("mu / sigma: number of items differs from w")
+    out_mu = torch.empty(B, d, dtype=torch.float32, device=w.device)
+    out_sigma = torch.empty_like(out_mu)
+    lib = nat.lib()
+    ws = nat.workspace(w.device, lib.evok_grad_batched_workspace_bytes(B, n, d), "grad_batched")
+    with _timed(group):
+        rc = getattr(lib, entry)(*args(mu, sm, sigma, ss), out_mu.data_ptr(), out_sigma.data_ptr(), ws.data_ptr(), ws.numel(), nat.stream_of(w))
+    nat.check(rc, entry)
+    return out_mu, out_sigma
+
+
 def grad_batched(form: int, X: torch.Tensor, w: torch.Tensor, mu: torch.Tensor, sigma: torch.Tensor, scale_mu: float, scale_sigma: float) -> tuple:
     """K4 for `items` independent searches in one launch chain.  X: (items, N, D), w: (items, N), mu / sigma: (D,) or (items, D)."""
     if not (X.is_cuda and X.dtype == torch.float32 and X.ndim == 3):
         raise ValueError("X: expected a float32 CUDA tensor of shape (items, N, D)")
     X = as_plain_tensor(X).contiguous()
     B, n, d = X.shape
-    w = as_plain_tensor(w).contiguous()
-    if tuple(w.shape) != (B, n):
-        raise ValueError(f"w: expected shape {(B, n)}, got {tuple(w.shape)}")
-    mu, bm, sm = _items(mu, (d,), "mu")
-    sigma, bs, ss = _items(sigma, (d,), "sigma")
-    out_mu = torch.empty(B, d, dtype=torch.float32, device=X.device)
-    out_sigma = torch.empty_like(out_mu)
-    lib = nat.lib()
-    ws = nat.workspace(X.device, lib.evok_grad_batched_workspace_bytes(B, n, d), "grad_batched")
-    with _timed("grad"):
-        rc = lib.evok_grad_batched(form, X.data_ptr(), n * d, d, w.data_ptr(), mu.data_ptr(), sm, sigma.data_ptr(), ss, B, n, d, scale_mu, scale_sigma,
-                                   out_mu.data_ptr(), out_sigma.data_ptr(), ws.data_ptr(), ws.numel(), nat.stream_of(X))
-    nat.check(rc, "evok_grad_batched")
-    return out_mu, out_sigma
+    return _grad_batched_call("evok_grad_batched", "grad", w, mu, sigma, B, n, d, lambda mu, sm, sigma, ss: (
+        form, X.data_ptr(), n * d, d, w.data_ptr(), mu.data_ptr(), sm, sigma.data_ptr(), ss, B, n, d, scale_mu, scale_sigma))
 
 
 def grad_batched_regen(form: int, w: torch.Tensor, mu: torch.Tensor, sigma: torch.Tensor, scale_mu: float, scale_sigma: float, *, seed: int,
@@ -643,22 +641,9 @@ def grad_batched_regen(form: int, w: torch.Tensor, mu: torch.Tensor, sigma: torc
     if not (w.is_cuda and w.dtype == torch.float32 and w.ndim == 2):
         raise ValueError("w: expected a float32 CUDA tensor of shape (items, N)")
     B, n = w.shape
-    w = _rows(w, "w", (B, n))
     d = mu.shape[-1]
-    mu, bm, sm = _items(mu, (d,), "mu")
-    sigma, bs, ss = _items(sigma, (d,), "sigma")
-    for cnt in (bm, bs):
-        if cnt is not None and cnt != B:
-            raise ValueError("mu / sigma: number of items differs from w")
-    out_mu = torch.empty(B, d, dtype=torch.float32, device=w.device)
-    out_sigma = torch.empty_like(out_mu)
-    lib = nat.lib()
-    ws = nat.workspace(w.device, lib.evok_grad_batched_workspace_bytes(B, n, d), "grad_batched")
-    with _timed("grad_regen"):
-        rc = lib.evok_grad_batched_regen(form, w.data_ptr(), mu.data_ptr(), sm, sigma.data_ptr(), ss, B, n, d, seed, stream_id0, scale_mu,
-                                         scale_sigma, out_mu.data_ptr(), out_sigma.data_ptr(), ws.data_ptr(), ws.numel(), nat.stream_of(w))
-    nat.check(rc, "evok_grad_batched_regen")
-    return out_mu, out_sigma
+    return _grad_batched_call("evok_grad_batched_regen", "grad_regen", w, mu, sigma, B, n, d, lambda mu, sm, sigma, ss: (
+        form, w.data_ptr(), mu.data_ptr(), sm, sigma.data_ptr(), ss, B, n, d, seed, stream_id0, scale_mu, scale_sigma))
 
 
 def clipup_batched_(g: torch.Tensor, velocity: torch.Tensor, center: torch.Tensor, stepsizes, momenta, max_speeds) -> None:

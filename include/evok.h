@@ -381,7 +381,9 @@ int evok_rank_batched(int method, const float* f, int64_t N, int64_t n_items, in
                       void* stream);
 int evok_elite_mask_batched(const float* w, int64_t N, int64_t n_items, int64_t num_elites, float* mask, void* ws, size_t ws_bytes, void* stream);
 int evok_weights_adjust_batched(float* w, int64_t N, int64_t n_items, int mode, void* stream);
-/* K4: X [items][n_rows][D] (item stride / row pitch given), w [items][n_rows], out_mu / out_sigma [items][D] */
+/* K4: X [items][n_rows][D] (item stride / row pitch given), w [items][n_rows], out_mu / out_sigma [items][D].  Errors in this order:
+ * EVOK_E_NULLPTR, EVOK_E_BADENUM, EVOK_E_BADSIZE (negative counts or item strides, D <= 0, ldx < D), EVOK_E_ODDROWS,
+ * EVOK_E_WORKSPACE. */
 size_t evok_grad_batched_workspace_bytes(int64_t n_items, int64_t n_rows, int64_t D);
 int evok_grad_batched(int form, const float* X, int64_t item_stride_x, int64_t ldx, const float* w, const float* mu, int64_t item_stride_mu,
                       const float* sigma, int64_t item_stride_sigma, int64_t n_items, int64_t n_rows, int64_t D, float scale_mu, float scale_sigma,
@@ -390,7 +392,7 @@ int evok_grad_batched(int form, const float* X, int64_t item_stride_x, int64_t l
  * stream_id0), without reading it: every row with a non-zero weight is rebuilt from its Philox counters as
  * x = fmaf(sigma, z, mu) (item b on stream stream_id0 + b) and eps = x - mu, with the plan and workspace of evok_grad_batched.
  * The result is bit-identical to evok_grad_batched over the contiguous, 16-byte aligned X [items][n_rows][D] that the sampler
- * would have written.  Errors as evok_grad_batched, and EVOK_E_BADSIZE for a negative item stride. */
+ * would have written.  Errors as evok_grad_batched. */
 int evok_grad_batched_regen(int form, const float* w, const float* mu, int64_t item_stride_mu, const float* sigma, int64_t item_stride_sigma,
                             int64_t n_items, int64_t n_rows, int64_t D, uint64_t seed, uint64_t stream_id0, float scale_mu, float scale_sigma,
                             float* out_mu, float* out_sigma, void* ws, size_t ws_bytes, void* stream);

@@ -195,6 +195,14 @@ def test_grad_batched_regen_equals_grad_batched(form, D, shared, B, n):
         FB._check(f"s2 item {b}", r[1][b].cpu().numpy(), 1.9 * ref["s2"], FB.C_ROUND * FB.EPS32 * k_eff * 1.9 * ref["s2_mag"] + 1e-30)
 
 
+@pytest.mark.parametrize("form", [0, 1, 2, 3])
+@pytest.mark.parametrize("shared", [True, False])
+def test_grad_batched_regen_equals_grad_batched_one_wide_item(form, shared):
+    """One item at a shape where a single search would take the TMA kernel (D >= 512, at least 4096 row units): the batch keeps
+    the LDG plan, so the stored and rebuilt populations still give the same bits."""
+    test_grad_batched_regen_equals_grad_batched(form, 1024, shared, 1, 8192)
+
+
 # ------------------------------------------------------------------------------------------------ whole runs
 def _pgpe_state(batch, layout, opt, ranking, symmetric, D):
     g = torch.Generator().manual_seed(len(batch) * 7 + D)

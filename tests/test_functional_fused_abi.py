@@ -124,6 +124,27 @@ def test_grad_batched_regen_codes(lib, changes, code):
     assert lib.evok_launch_count() == before
 
 
+# evok_grad_batched takes the same checks, and X with its item stride and row pitch
+GRAD_BATCHED_CASES = GRAD_CASES + [
+    (dict(X=None), NULLPTR),
+    (dict(X=None, ldx=7), NULLPTR),
+    (dict(ldx=7), BADSIZE),
+    (dict(sx=-32), BADSIZE),
+    (dict(sx=-32, items=0), BADSIZE),
+    (dict(ldx=7, n_rows=3), BADSIZE),
+]
+
+
+@pytest.mark.parametrize("changes,code", GRAD_BATCHED_CASES)
+def test_grad_batched_codes(lib, changes, code):
+    a = {**GRAD_BASE, "X": P, "sx": 32, "ldx": 8, **changes}
+    before = lib.evok_launch_count()
+    rc = lib.evok_grad_batched(a["form"], a["X"], a["sx"], a["ldx"], a["w"], a["mu"], a["sm"], a["sigma"], a["ss"], a["items"], a["n_rows"], a["D"],
+                               1.0, 1.0, a["out_mu"], a["out_sigma"], a["ws"], a["ws_bytes"], None)
+    assert rc == code
+    assert lib.evok_launch_count() == before
+
+
 def test_register_batched_codes(lib, registered):
     img = b"\x7fELF" + bytes(60)
     ok = names(BATCHED_KERNELS)
