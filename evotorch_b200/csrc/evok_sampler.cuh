@@ -142,6 +142,36 @@ __device__ __forceinline__ double warp_sum(double v) {
   return v;
 }
 
+// The other reductions of a generated accumulator (products, maxima, minima): the butterfly of warp_sum with another combine,
+// in the same xor order, so every lane ends with the same, reproducible bits.  max / min propagate NaN (max.NaN / min.NaN: a
+// NaN operand gives NaN, as torch.amax / amin do; fmaxf / fminf would drop it).
+__device__ __forceinline__ float inf() { return __int_as_float(0x7f800000); }
+__device__ __forceinline__ float max_nan(float a, float b) {
+  float r;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+__device__ __forceinline__ float min_nan(float a, float b) {
+  float r;
+  asm("min.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+__device__ __forceinline__ float warp_prod(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v *= __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = max_nan(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+__device__ __forceinline__ float warp_min(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = min_nan(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
 // streaming 128-bit accesses: the population is touched once per kernel, keep it out of L1
 __device__ __forceinline__ float4 ld_stream4(const float* p) {
   float4 v;
@@ -165,7 +195,9 @@ __device__ __forceinline__ void st_stream1(float* p, float a) {
 //   Acc(D)      : a fresh accumulator for one row of D columns (one per row and lane);
 //   add(x, j)   : fold element x of column j (0-based, global) into this lane's partial sums;
 //   finish(D)   : warp-reduce the partials and return the fitness of the row (every lane gets it; lane 0 stores it).
-// A row's elements reach add() in no fixed column order (strided over the lanes of a warp), so an accumulator holds sums.
+// A row's elements reach add() in no fixed column order (strided over the lanes of a warp), so an accumulator holds
+// reductions with an associative combine: sums, and in a generated one also products, maxima and minima (warp_prod / _max /
+// _min), each slot starting from its combine's identity.
 // A generated accumulator may also have pair terms (`static constexpr bool kPairs = true`, see PairTerms below):
 //   add_pair(x, xn, j) : fold the neighbour pair (x_j, x_{j+1}); it is called exactly once for every j in [0, D-2] of a row,
 //                        by the lane that holds column j+1, also in no fixed order across lanes (fold_pairs).
@@ -175,6 +207,11 @@ __device__ __forceinline__ void st_stream1(float* p, float a) {
 // constructor, and takes the vectors' entries with every fold:
 //   add(x, j, d)                  : d[i] = vec[i][j];
 //   add_pair(x, xn, j, d, dn)     : d[i] = vec[i][j], dn[i] = vec[i][j + 1].
+// A generated accumulator may also have running sums c_j = sum_{k<=j} h(x_k, k) (`static constexpr bool kRunning = true` and
+// `static constexpr int kRunningSums` = R <= 2, see RunningTerms below).  Its element terms then see the running sums at their
+// column, so add() takes them, after the data entries of an accumulator with data:
+//   running(x, j[, d], h)  : h[i] = the increment of running sum i at column j;
+//   add(x, j[, d], r)      : fold element x of column j, where r[i] = c_j of running sum i (fold_running computes it).
 // The built-in ones are ObjAcc<EVOK_OBJ_*>; a user-defined one is generated by evotorch_b200/jit.py.
 // ------------------------------------------------------------------------------------------------
 template <int OBJ>
@@ -240,6 +277,33 @@ struct PairTerms {
 template <typename Acc>
 struct PairTerms<Acc, decltype(void(Acc::kPairs))> {
   static constexpr bool value = Acc::kPairs;
+};
+
+// true for an accumulator that declares `static constexpr bool kRunning = true` (a generated one with running sums; kSums of
+// them); all running-sum code is under `if constexpr` on it
+template <typename Acc, typename = void>
+struct RunningTerms {
+  static constexpr bool value = false;
+  static constexpr int kSums = 1;
+};
+template <typename Acc>
+struct RunningTerms<Acc, decltype(void(Acc::kRunning))> {
+  static constexpr bool value = Acc::kRunning;
+  static constexpr int kSums = Acc::kRunningSums;
+};
+
+// an accumulator whose kernels take warp-uniform steps of 32 lanes (pair folds and running sums shuffle across lanes)
+template <typename Acc>
+struct WarpSteps {
+  static constexpr bool value = PairTerms<Acc>::value || RunningTerms<Acc>::value;
+};
+
+// the carries of one row along warp-uniform steps: the last column of the previous step (pair terms) and the running sums of
+// all columns of the previous steps
+template <typename Acc>
+struct StepCarry {
+  float pair = 0.f;
+  float run[RunningTerms<Acc>::kSums] = {};
 };
 
 // The data of one launch of an objective with data terms: p[i] is data name i of the launch's first item and item_stride[i]
@@ -349,6 +413,61 @@ __device__ __forceinline__ void fold_pairs(Acc& acc, const float (&v)[N], int64_
     }
 }
 
+// One warp step of the element folds of an accumulator with running sums, in the layout of fold_pairs (this lane holds the
+// columns j .. j+N-1, of which the first n_valid exist; every lane calls it on every step, in increasing column order).  For
+// each running sum: the lane evaluates the increments h of its columns (0 past the row's end), forms their inclusive prefix
+// p_c, and takes the exclusive scan e of the lane totals p_{N-1} across the warp (a Kogge-Stone scan with __shfl_up_sync, five
+// rounds, then one shift); then c_{j+c} = p_c + (e + carry), where carry is the sum of all earlier steps of the row, and the
+// carry advances by the step total, the inclusive scan of lane 31.  Then each column's element terms are folded with its c.
+template <int N, typename Acc, typename Cols>
+__device__ __forceinline__ void fold_running(Acc& acc, const float (&v)[N], int64_t j, int n_valid, float (&carry)[RunningTerms<Acc>::kSums],
+                                             const Cols& dc) {
+  constexpr int R = RunningTerms<Acc>::kSums;
+  const int lane = threadIdx.x & 31;
+  float p[N][R];
+#pragma unroll
+  for (int c = 0; c < N; ++c) {
+    float h[R];
+#pragma unroll
+    for (int i = 0; i < R; ++i) h[i] = 0.f;
+    if (c < n_valid) {
+      if constexpr (DataTerms<Acc>::value) acc.running(v[c], j + c, dc.v[c], h);
+      else acc.running(v[c], j + c, h);
+    }
+#pragma unroll
+    for (int i = 0; i < R; ++i) p[c][i] = c == 0 ? h[i] : p[c - 1][i] + h[i];
+  }
+#pragma unroll
+  for (int i = 0; i < R; ++i) {
+    float incl = p[N - 1][i];
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const float t = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl += t;
+    }
+    const float excl = __shfl_up_sync(0xffffffffu, incl, 1);
+    const float total = __shfl_sync(0xffffffffu, incl, 31);
+    const float base = lane == 0 ? carry[i] : excl + carry[i];
+#pragma unroll
+    for (int c = 0; c < N; ++c) p[c][i] += base;
+    carry[i] += total;
+  }
+#pragma unroll
+  for (int c = 0; c < N; ++c)
+    if (c < n_valid) {
+      if constexpr (DataTerms<Acc>::value) acc.add(v[c], j + c, dc.v[c], p[c]);
+      else acc.add(v[c], j + c, p[c]);
+    }
+}
+
+// the element folds and pair folds of one warp step (see fold_pairs and fold_running): the element folds of an accumulator
+// without running sums have been made by the caller already
+template <int N, typename Acc, typename Cols>
+__device__ __forceinline__ void fold_step(Acc& acc, const float (&v)[N], int64_t j, int n_valid, StepCarry<Acc>& carry, const Cols& dc) {
+  if constexpr (RunningTerms<Acc>::value) fold_running<N>(acc, v, j, n_valid, carry.run, dc);
+  if constexpr (PairTerms<Acc>::value) fold_pairs<N>(acc, v, j, n_valid, carry.pair, dc);
+}
+
 // ------------------------------------------------------------------------------------------------
 // K1 / K2 kernels.  HBM-bound design: one warp owns one direction (a +/- row pair) or one row; every lane produces 4
 // consecutive columns per step from ONE Philox4x32-10 call, writes them with 128-bit streaming stores (512 contiguous bytes
@@ -376,7 +495,7 @@ constexpr int kSampleThreads = EVOK_SAMPLE_THREADS;
 // bound and prefers occupancy
 template <typename Acc>
 struct SampleTune {
-  static constexpr int kUnroll = SampleOnly<Acc>::value ? EVOK_SAMPLEONLY_UNR : EVOK_SAMPLE_UNR;
+  static constexpr int kUnroll = SampleOnly<Acc>::value ? EVOK_SAMPLEONLY_UNR : RunningTerms<Acc>::value ? 1 : EVOK_SAMPLE_UNR;
   static constexpr int kMinBlocks = SampleOnly<Acc>::value ? EVOK_SAMPLEONLY_MINB : EVOK_SAMPLE_MINB;
 };
 
@@ -425,13 +544,16 @@ __device__ __forceinline__ void sample_group(const PhiloxKey& key, uint32_t sw, 
   }
 }
 
-// sample_group for an accumulator with pair terms, called by EVERY lane of the warp on every step (fold_pairs shuffles): a
-// lane whose group lies past the row's end (!active) draws, loads and stores nothing and folds nothing.  The samples and the
-// element adds are those of sample_group, in the same order; the + and - rows have their own neighbours and carries.
+// sample_group for an accumulator with pair terms or running sums, called by EVERY lane of the warp on every step (fold_step
+// shuffles): a lane whose group lies past the row's end (!active) draws, loads and stores nothing and folds nothing.  The
+// samples and the element adds are those of sample_group, in the same order (with running sums the element adds come after the
+// scan, in fold_running); the + and - rows have their own neighbours and carries.
 template <typename Acc, bool SYM, bool STORE, bool VEC, bool SQ>
 __device__ __forceinline__ void sample_group_pairs(const PhiloxKey& key, uint32_t sw, uint64_t unit, uint32_t q, int64_t D,
                                                    const float* __restrict__ mu, const float* __restrict__ sigma, float* xp, float* xm,
-                                                   Acc& accp, Acc& accm, float* zsq, bool active, float& carry_p, float& carry_m) {
+                                                   Acc& accp, Acc& accm, float* zsq, bool active, StepCarry<Acc>& carry_p,
+                                                   StepCarry<Acc>& carry_m) {
+  constexpr bool kFoldNow = !RunningTerms<Acc>::value;  // element terms without running sums fold as they are sampled
   float p[4] = {0.f, 0.f, 0.f, 0.f}, n[4] = {0.f, 0.f, 0.f, 0.f};
   const int64_t j = (int64_t)q << 2;
   int n_valid = 0;
@@ -448,11 +570,15 @@ __device__ __forceinline__ void sample_group_pairs(const PhiloxKey& key, uint32_
       p[0] = fmaf(s.x, z[0], m.x); p[1] = fmaf(s.y, z[1], m.y); p[2] = fmaf(s.z, z[2], m.z); p[3] = fmaf(s.w, z[3], m.w);
       if (STORE) st_stream4(xp + j, p[0], p[1], p[2], p[3]);
       dc.load4(accp, j);
-      fold(accp, p[0], j, dc, 0); fold(accp, p[1], j + 1, dc, 1); fold(accp, p[2], j + 2, dc, 2); fold(accp, p[3], j + 3, dc, 3);
+      if constexpr (kFoldNow) {
+        fold(accp, p[0], j, dc, 0); fold(accp, p[1], j + 1, dc, 1); fold(accp, p[2], j + 2, dc, 2); fold(accp, p[3], j + 3, dc, 3);
+      }
       if (SYM) {
         n[0] = fmaf(-s.x, z[0], m.x); n[1] = fmaf(-s.y, z[1], m.y); n[2] = fmaf(-s.z, z[2], m.z); n[3] = fmaf(-s.w, z[3], m.w);
         if (STORE) st_stream4(xm + j, n[0], n[1], n[2], n[3]);
-        fold(accm, n[0], j, dc, 0); fold(accm, n[1], j + 1, dc, 1); fold(accm, n[2], j + 2, dc, 2); fold(accm, n[3], j + 3, dc, 3);
+        if constexpr (kFoldNow) {
+          fold(accm, n[0], j, dc, 0); fold(accm, n[1], j + 1, dc, 1); fold(accm, n[2], j + 2, dc, 2); fold(accm, n[3], j + 3, dc, 3);
+        }
       }
       n_valid = 4;
     } else {
@@ -464,20 +590,21 @@ __device__ __forceinline__ void sample_group_pairs(const PhiloxKey& key, uint32_
           p[c] = fmaf(s, z[c], m);
           if (STORE) st_stream1(xp + j + c, p[c]);
           dc.load1(accp, j + c, c);
-          fold(accp, p[c], j + c, dc, c);
+          if constexpr (kFoldNow) fold(accp, p[c], j + c, dc, c);
           if (SYM) {
             n[c] = fmaf(-s, z[c], m);
             if (STORE) st_stream1(xm + j + c, n[c]);
-            fold(accm, n[c], j + c, dc, c);
+            if constexpr (kFoldNow) fold(accm, n[c], j + c, dc, c);
           }
         }
       }
       n_valid = D - j < 4 ? (int)(D - j) : 4;  // the partial last group: a pair is folded only where column j + 1 < D
     }
   }
-  if (n_valid > 0 && j > 0) dc.load_left(accp, j);
-  fold_pairs<4>(accp, p, j, n_valid, carry_p, dc);
-  if (SYM) fold_pairs<4>(accm, n, j, n_valid, carry_m, dc);
+  if constexpr (PairTerms<Acc>::value)
+    if (n_valid > 0 && j > 0) dc.load_left(accp, j);
+  fold_step<4>(accp, p, j, n_valid, carry_p, dc);
+  if (SYM) fold_step<4>(accm, n, j, n_valid, carry_m, dc);
 }
 
 // One unit u (a direction of symmetric sampling, else a row) of the warp of lane `lane`: sample its row(s) from (key, stream word sw, unit
@@ -496,10 +623,10 @@ __device__ __forceinline__ void sample_eval_unit(int lane, float* __restrict__ X
   const uint64_t unit = unit0 + (uint64_t)u;
   constexpr int kSampleUnroll = SampleTune<Acc>::kUnroll;
   float zsq = 0.f;
-  if constexpr (PairTerms<Acc>::value) {
-    // warp-uniform steps of 32 groups (fold_pairs shuffles); each lane still visits its groups lane, lane + 32, ... in
-    // increasing order, the order of the loops below and of eval_kernel
-    float carry_p = 0.f, carry_m = 0.f;
+  if constexpr (WarpSteps<Acc>::value) {
+    // warp-uniform steps of 32 groups in increasing column order (fold_step shuffles and carries from step to step); each lane
+    // still visits its groups lane, lane + 32, ... in increasing order, the order of the loops below and of eval_kernel
+    StepCarry<Acc> carry_p, carry_m;
     uint32_t b = 0;
     for (; b + 32u * kSampleUnroll <= nq; b += 32u * kSampleUnroll) {
 #pragma unroll
@@ -607,10 +734,11 @@ __global__ void __launch_bounds__(kEvalThreads)
   for (int64_t r = gw; r < n_rows; r += warps_total) {
     Acc acc = make_acc<Acc>(D, data);
     const float* x = X + r * ldx;
-    if constexpr (PairTerms<Acc>::value) {
-      // warp-uniform steps (fold_pairs shuffles); per lane the groups, element adds and pair folds of sample_eval_kernel's
-      // VEC path in the same order, so both kernels give the same fitness bit for bit on the same X
-      float carry = 0.f;
+    if constexpr (WarpSteps<Acc>::value) {
+      // warp-uniform steps (fold_step shuffles); per lane the groups, element adds, running sums and pair folds of
+      // sample_eval_kernel's VEC path in the same order, so both kernels give the same fitness bit for bit on the same X
+      constexpr bool kFoldNow = !RunningTerms<Acc>::value;
+      StepCarry<Acc> carry;
       if (VEC) {
         const int64_t nq = D >> 2;
         int64_t b = 0;
@@ -625,9 +753,12 @@ __global__ void __launch_bounds__(kEvalThreads)
             const float v[4] = {g[k].x, g[k].y, g[k].z, g[k].w};
             Cols4 dc;
             dc.load4(acc, jk);
-            if (jk > 0) dc.load_left(acc, jk);
-            fold(acc, v[0], jk, dc, 0); fold(acc, v[1], jk + 1, dc, 1); fold(acc, v[2], jk + 2, dc, 2); fold(acc, v[3], jk + 3, dc, 3);
-            fold_pairs<4>(acc, v, jk, 4, carry, dc);
+            if constexpr (PairTerms<Acc>::value)
+              if (jk > 0) dc.load_left(acc, jk);
+            if constexpr (kFoldNow) {
+              fold(acc, v[0], jk, dc, 0); fold(acc, v[1], jk + 1, dc, 1); fold(acc, v[2], jk + 2, dc, 2); fold(acc, v[3], jk + 3, dc, 3);
+            }
+            fold_step<4>(acc, v, jk, 4, carry, dc);
           }
         }
         for (; b < nq; b += 32) {
@@ -639,10 +770,13 @@ __global__ void __launch_bounds__(kEvalThreads)
           Cols4 dc;
           if (active) {
             dc.load4(acc, ja);
-            if (ja > 0) dc.load_left(acc, ja);
-            fold(acc, v[0], ja, dc, 0); fold(acc, v[1], ja + 1, dc, 1); fold(acc, v[2], ja + 2, dc, 2); fold(acc, v[3], ja + 3, dc, 3);
+            if constexpr (PairTerms<Acc>::value)
+              if (ja > 0) dc.load_left(acc, ja);
+            if constexpr (kFoldNow) {
+              fold(acc, v[0], ja, dc, 0); fold(acc, v[1], ja + 1, dc, 1); fold(acc, v[2], ja + 2, dc, 2); fold(acc, v[3], ja + 3, dc, 3);
+            }
           }
-          fold_pairs<4>(acc, v, ja, active ? 4 : 0, carry, dc);
+          fold_step<4>(acc, v, ja, active ? 4 : 0, carry, dc);
         }
       } else {
         for (int64_t b = 0; b < D; b += 32) {
@@ -652,10 +786,11 @@ __global__ void __launch_bounds__(kEvalThreads)
           Cols1 dc;
           if (active) {
             dc.load1(acc, j, 0);
-            if (j > 0) dc.load_left(acc, j);
-            fold(acc, v[0], j, dc, 0);
+            if constexpr (PairTerms<Acc>::value)
+              if (j > 0) dc.load_left(acc, j);
+            if constexpr (kFoldNow) fold(acc, v[0], j, dc, 0);
           }
-          fold_pairs<1>(acc, v, j, active ? 1 : 0, carry, dc);
+          fold_step<1>(acc, v, j, active ? 1 : 0, carry, dc);
         }
       }
     } else if (VEC) {

@@ -1,13 +1,23 @@
-"""Run-time compiled objectives: a function of sums over the elements or neighbour pairs of a row, given as Python
+"""Run-time compiled objectives: a function of reductions over the elements or neighbour pairs of a row, given as Python
 expressions, becomes an accumulator of the fused sampler (csrc/evok_sampler.cuh), compiled with NVRTC for sm_90a and
 registered with libevok.so.
 
     f(x) = value(S_1, ..., S_k, D),    k <= 4,
-    S_i = sum_{j=0}^{D-1} term_i(x_j, j, D)              (an element term), or
-    S_i = sum_{j=0}^{D-2} term_i(x_j, x_{j+1}, j, D)     (a pair term: one that uses xn; 0 when D = 1)
+    S_i = R_{j=0}^{D-1} term_i(x_j, j, D)              (an element term), or
+    S_i = R_{j=0}^{D-2} term_i(x_j, x_{j+1}, j, D)     (a pair term: one that uses xn; empty when D = 1)
+
+where the reduction R is a sum (`sums`), a product (`prods`), a maximum (`maxs`) or a minimum (`mins`); the k reductions share
+one namespace.  An empty reduction is 0, 1, -inf or +inf respectively.  A NaN term makes its product, maximum or minimum NaN, as
+torch.prod / amax / amin do (the kernels' max / min propagate NaN; fmaxf / fminf would not); +-inf pass through.
 
 Pair terms give the chained test functions, e.g. Rosenbrock: {"s": "100*(xn - x**2)**2 + (1 - x)**2"}, value "s".  One
 objective may mix both kinds.
+
+`running` defines up to 2 running sums c_j = sum_{k<=j} h(x_k, k, D), inclusive of column j, with h an element term (x, j, D and
+data; no xn, no running or reduction name).  A running name is usable in the element terms of every reduction, and nowhere
+else (pair terms, running terms, `value`): Schwefel 1.2 is running {"c": "x"}, sums {"s": "c**2"}, value "s".  The kernels
+compute c_j with one warp scan per step of 128 columns and a carry per row (fold_running in csrc/evok_sampler.cuh); the torch
+function with cumsum.
 
 One parse of the expressions gives both the CUDA accumulator and a torch function of the same formula (the evaluation of
 CPU problems, other dtypes, rng="torch" and before-eval hooks; the float64 reference of the tests).
@@ -16,16 +26,20 @@ The expression language (anything else raises ValueError):
   - operators  + - * /, unary -, ** (an integer literal exponent expands to products, any other exponent is powf / torch.pow);
   - functions  abs sqrt exp log sin cos tan tanh floor minimum maximum  (minimum / maximum return the other operand when
     one is NaN, like fminf / fmaxf and torch.fmin / torch.fmax);
+  - where(cond, a, b)  a conditional, CUDA (cond) ? a : b and torch.where; cond is one comparison < <= > >= == != of two
+    expressions, and comparisons are allowed nowhere else.  As in IEEE arithmetic a comparison with NaN is false, except !=,
+    which is true (CUDA and torch agree);
   - constants  pi, e, numeric literals;
   - names      x (the element), xn (the next element x_{j+1}), j (the 0-based column of x) and D (the row length) in a
-    term; the sum names and D in `value`.
+    term, and the running names in an element term of a reduction; the reduction names and D in `value`.
   - data       up to 4 more names, each bound to a float32 tensor (`data={"t": t, "lam": lam}`).  Last dimension 1 makes a
     scalar, usable in the terms and in `value`; any other last dimension makes a vector, which must have the row length D and is
     usable in the terms only: `t` is its entry at column j and, in a pair term, `t_n` its entry at column j + 1 (as x and xn).
     Leading dimensions are batch dimensions: one data set per item of a batched search.
 The CUDA side evaluates in float32 with the precise libdevice functions (no fast math) and contracts a * b + c into fma.
-The source of an objective without pair terms is exactly that of the element-only language (no pair code in it), and the source
-of one without data is exactly that of the language without data.  Which data name is a scalar and which a vector is part of
+The source of an objective without pair terms is exactly that of the element-only language (no pair code in it), the source
+of one without data is exactly that of the language without data, and the source of one of sums without running sums is exactly
+that of the language before products, maxima, minima and running sums.  Which data name is a scalar and which a vector is part of
 the source; the tensors are not: they are bound to an instance of the compiled objective (`bind_instance`) and reach the
 kernels as a launch argument, so objectives with the same expressions and kinds share one compilation whatever their data.
 """
@@ -50,7 +64,8 @@ _PKG = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_PKG, "csrc")
 INCLUDE = os.path.join(os.path.dirname(_PKG), "include")
 
-MAX_SUMS = 4
+MAX_SUMS = 4  # reductions of all kinds together
+MAX_RUNNING = 2
 MAX_DATA = 4  # EVOK_MAX_DATA
 MAX_INT_POWER = 16
 
@@ -62,8 +77,10 @@ FUNCTIONS = {
 CONSTANTS = {"pi": math.pi, "e": math.e}
 _ARITY = {"minimum": 2, "maximum": 2}
 _BINOPS = {ast.Add: "+", ast.Sub: "-", ast.Mult: "*", ast.Div: "/"}
-_ALLOWED_TEXT = ("allowed: + - * / ** and unary -, the functions " + " ".join(FUNCTIONS) + ", the constants pi and e, numeric "
-                 "literals and the names {names}")
+_COMPARE = {ast.Lt: ("<", torch.lt), ast.LtE: ("<=", torch.le), ast.Gt: (">", torch.gt), ast.GtE: (">=", torch.ge),
+            ast.Eq: ("==", torch.eq), ast.NotEq: ("!=", torch.ne)}
+_ALLOWED_TEXT = ("allowed: + - * / ** and unary -, the functions " + " ".join(FUNCTIONS) + ", where(cond, a, b) with one comparison "
+                 "< <= > >= == != as cond, the constants pi and e, numeric literals and the names {names}")
 
 
 def _float_literal(v: float) -> str:
@@ -139,6 +156,25 @@ def _translate(node, names: Dict[str, str], where: str) -> _Expr:
         fn = {"+": lambda env: a.torch(env) + b.torch(env), "-": lambda env: a.torch(env) - b.torch(env),
               "*": lambda env: a.torch(env) * b.torch(env), "/": lambda env: a.torch(env) / b.torch(env)}[op]
         return _Expr(f"({a.cuda} {op} {b.cuda})", fn)
+    if isinstance(node, ast.Call) and isinstance(node.func, ast.Name) and node.func.id == "where":
+        if node.keywords or len(node.args) != 3:
+            raise ValueError(f"{where}: where takes 3 positional arguments (cond, a, b), got {ast.unparse(node)!r}")
+        cond = node.args[0]
+        if not (isinstance(cond, ast.Compare) and len(cond.ops) == 1 and type(cond.ops[0]) in _COMPARE):
+            raise ValueError(f"{where}: the condition of where must be one comparison < <= > >= == != of two expressions, got "
+                             f"{ast.unparse(cond)!r}")
+        op, top = _COMPARE[type(cond.ops[0])]
+        l, r = _translate(cond.left, names, where), _translate(cond.comparators[0], names, where)
+        a, b = _translate(node.args[1], names, where), _translate(node.args[2], names, where)
+
+        def where_fn(env):
+            lv, rv = _as_tensor(l.torch(env), env), _as_tensor(r.torch(env), env)
+            return torch.where(top(lv, rv), _as_tensor(a.torch(env), env), _as_tensor(b.torch(env), env))
+
+        return _Expr(f"(({l.cuda} {op} {r.cuda}) ? {a.cuda} : {b.cuda})", where_fn)
+    if isinstance(node, ast.Compare):
+        raise ValueError(f"{where}: Compare ({ast.unparse(node)!r}) is not supported outside where: a comparison is allowed only as "
+                         f"the condition of where(cond, a, b); {allowed}")
     if isinstance(node, ast.Call):
         if not isinstance(node.func, ast.Name) or node.func.id not in FUNCTIONS:
             what = node.func.id if isinstance(node.func, ast.Name) else ast.unparse(node.func)
@@ -165,6 +201,12 @@ def _parse(text: str, names: Dict[str, str], where: str) -> _Expr:
         raise ValueError(f"{where}: not a Python expression: {text!r} ({e.msg})") from None
     return _translate(tree, names, where)
 
+
+# the reductions in slot order, with their keyword, the identity their slot starts from and their warp butterfly
+REDUCTIONS = ("sum", "prod", "max", "min")
+GROUP_OF = {"sum": "sums", "prod": "prods", "max": "maxs", "min": "mins"}
+IDENTITY = {"sum": "0.f", "prod": "1.f", "max": "-evok::inf()", "min": "evok::inf()"}
+WARP_REDUCE = {"sum": "warp_sum", "prod": "warp_prod", "max": "warp_max", "min": "warp_min"}
 
 _RESERVED = {"x", "j", "D"} | set(CONSTANTS) | set(FUNCTIONS)
 _RESERVED_DATA = _RESERVED | {"xn"}
@@ -194,38 +236,91 @@ def _names_used(text) -> set:
 
 
 class ObjectiveSpec:
-    """The parsed form of an objective: `source` is the CUDA translation unit, `torch_fn(X)` the torch function.  `pairs` names
-    the sums whose term uses xn (summed over the neighbour pairs of a row); the others are summed over its elements."""
+    """The parsed form of an objective: `source` is the CUDA translation unit, `torch_fn(X)` the torch function.  `reductions`
+    maps every reduction name to its combine operation ("sum", "prod", "max" or "min") in slot order, `pairs` names the
+    reductions whose term uses xn (reduced over the neighbour pairs of a row; the others over its elements) and `running` the
+    running-sum terms."""
 
-    def __init__(self, sums: Dict[str, str], value: str, kinds: Optional[Dict[str, bool]] = None):
+    def __init__(self, sums: Optional[Dict[str, str]], value: str, kinds: Optional[Dict[str, bool]] = None, *,
+                 prods: Optional[Dict[str, str]] = None, maxs: Optional[Dict[str, str]] = None, mins: Optional[Dict[str, str]] = None,
+                 running: Optional[Dict[str, str]] = None):
         """kinds: {data name: is a vector} in binding order (`data_kinds`), None or empty for an objective without data."""
         self.kinds = dict(kinds or {})
-        if not isinstance(sums, dict) or not 1 <= len(sums) <= MAX_SUMS:
-            raise ValueError(f"sums: expected a dict of 1 to {MAX_SUMS} named term expressions")
-        for s in sums:
-            if not (isinstance(s, str) and s.isidentifier()) or s in _RESERVED:
-                raise ValueError(f"sums: {s!r} cannot name a sum (a sum name is an identifier other than {sorted(_RESERVED)})")
-        self.sums, self.value = dict(sums), value
+        if value is None:
+            raise ValueError("value: an objective needs a `value` expression of its reductions")
+        groups = {"sums": sums, "prods": prods, "maxs": maxs, "mins": mins}
+        for what, g in groups.items():
+            if g is not None and not isinstance(g, dict):
+                raise ValueError(f"{what}: expected a dict of named term expressions, got {type(g).__name__}")
+        if prods is None and maxs is None and mins is None:
+            if not isinstance(sums, dict) or not 1 <= len(sums) <= MAX_SUMS:
+                raise ValueError(f"sums: expected a dict of 1 to {MAX_SUMS} named term expressions")
+        elif not 1 <= sum(len(g or {}) for g in groups.values()) <= MAX_SUMS:
+            raise ValueError(f"sums, prods, maxs, mins: expected 1 to {MAX_SUMS} reductions in all, got "
+                             f"{sum(len(g or {}) for g in groups.values())}")
+        self.reductions, texts = {}, {}
+        for (what, g), op in zip(groups.items(), REDUCTIONS):
+            for s, t in (g or {}).items():
+                if not (isinstance(s, str) and s.isidentifier()) or s in _RESERVED:
+                    raise ValueError(f"{what}: {s!r} cannot name a {op} (a reduction name is an identifier other than {sorted(_RESERVED)})")
+                if s in self.reductions:
+                    raise ValueError(f"{what}: {s!r} names two reductions; sums, prods, maxs and mins share one namespace")
+                self.reductions[s], texts[s] = op, t
+        if running is not None and not isinstance(running, dict) or len(running or {}) > MAX_RUNNING:
+            raise ValueError(f"running: expected a dict of at most {MAX_RUNNING} named running-sum terms")
+        running = dict(running or {})
+        for c in running:
+            if not (isinstance(c, str) and c.isidentifier()) or c in _RESERVED_DATA:
+                raise ValueError(f"running: {c!r} cannot name a running sum (an identifier other than {sorted(_RESERVED_DATA)})")
+            if c in self.reductions:
+                raise ValueError(f"running: {c!r} is also the name of a reduction")
+        self.sums, self.value = dict(sums or {}), value
+        self.prods, self.maxs, self.mins, self.running = dict(prods or {}), dict(maxs or {}), dict(mins or {}), running
         term_names = {"x": "x", "xn": "xn", "j": "jf", "D": "Df"}
-        value_names = {s: f"S_{s}" for s in sums}
+        value_names = {s: f"S_{s}" for s in self.reductions}
         value_names["D"] = "Df"
         for name, vector in self.kinds.items():
-            if name in sums:
-                raise ValueError(f"data: {name!r} is the name of a sum")
+            if name in self.reductions:
+                raise ValueError(f"data: {name!r} is the name of a {self.reductions[name]}")
+            if name in running:
+                raise ValueError(f"data: {name!r} is the name of a running sum")
             # a vector's entries at columns j and j + 1, handed to add / add_pair; a scalar is a member of the accumulator
             term_names.update({name: f"v_{name}", f"{name}_n": f"vn_{name}"} if vector else {name: f"c_{name}"})
             if not vector:
                 value_names[name] = f"c_{name}"
-        for s, t in sums.items():
-            self._check_data_names(_names_used(t), f"sums[{s!r}]", term=True)
-        self._check_data_names(_names_used(value), "value", term=False)
-        self.terms = {s: _parse(t, term_names, f"sums[{s!r}]") for s, t in sums.items()}
+        allowed_where = ("a running sum is usable in the element terms of sums, prods, maxs and mins only (not in a pair term, a "
+                         "running term or `value`)")
+        for c, t in running.items():
+            used = _names_used(t)
+            self._check_data_names(used, f"running[{c!r}]", term=True)
+            bad = used & (set(running) | set(self.reductions))
+            if bad:
+                raise ValueError(f"running[{c!r}]: {sorted(bad)[0]!r}: a running term is an element term of x, j, D and data; "
+                                 f"{allowed_where}")
+        self.running_terms = {c: _parse(t, {k: v for k, v in term_names.items() if k != "xn"}, f"running[{c!r}]")
+                              for c, t in running.items()}
+        for c, e in self.running_terms.items():
+            m = re.search(r"\bvn_(\w+)\b", e.cuda)
+            if m:
+                raise ValueError(f"running[{c!r}]: {m.group(1)}_n is the entry at column j + 1, which only a pair term has")
+        run_names = dict(term_names, **{c: f"r[{i}]" for i, c in enumerate(running)})
+        for s, t in texts.items():
+            used = _names_used(t)
+            self._check_data_names(used, f"{GROUP_OF[self.reductions[s]]}[{s!r}]", term=True)
+            if used & set(running) and "xn" in used:
+                raise ValueError(f"{GROUP_OF[self.reductions[s]]}[{s!r}]: {sorted(used & set(running))[0]!r} in a pair term; "
+                                 f"{allowed_where}")
+        used = _names_used(value)
+        self._check_data_names(used, "value", term=False)
+        if used & set(running):
+            raise ValueError(f"value: {sorted(used & set(running))[0]!r} is a running sum; {allowed_where}")
+        self.terms = {s: _parse(t, run_names, f"{GROUP_OF[self.reductions[s]]}[{s!r}]") for s, t in texts.items()}
         self.pairs = frozenset(s for s, e in self.terms.items() if re.search(r"\bxn\b", e.cuda))
         for s, e in self.terms.items():
             m = re.search(r"\bvn_(\w+)\b", e.cuda)
             if m and s not in self.pairs:
-                raise ValueError(f"sums[{s!r}]: {m.group(1)}_n is the entry of {m.group(1)!r} at column j + 1, which only a pair term (one "
-                                 f"that uses xn) has; an element term uses {m.group(1)!r}")
+                raise ValueError(f"{GROUP_OF[self.reductions[s]]}[{s!r}]: {m.group(1)}_n is the entry of {m.group(1)!r} at column j + 1, "
+                                 f"which only a pair term (one that uses xn) has; an element term uses {m.group(1)!r}")
         self.value_expr = _parse(value, value_names, "value")
         self.source = self._cuda_source()
 
@@ -241,6 +336,8 @@ class ObjectiveSpec:
         uses_j = lambda es: any(re.search(r"\bjf\b", e.cuda) for e in es)  # noqa: E731
         element = [(i, e) for i, (s, e) in zip(k, self.terms.items()) if s not in self.pairs]
         pair = [(i, e) for i, (s, e) in zip(k, self.terms.items()) if s in self.pairs]
+        ops = [self.reductions[s] for s in self.terms]
+        nr = len(self.running_terms)
         # data: slot i of the binding is data name i; the vectors are numbered among themselves in the same order
         vectors = [n for n, v in self.kinds.items() if v]
         nv = max(len(vectors), 1)
@@ -249,14 +346,22 @@ class ObjectiveSpec:
             return [f"    const float {prefix}_{n} = {array}[{i}];" for i, n in enumerate(vectors)
                     if any(re.search(rf"\b{prefix}_{n}\b", e.cuda) for _, e in es)]
 
+        def combine(i, e):  # slot i folds the term e with its reduction's operation
+            return {"sum": f"    s{i} += {e};", "prod": f"    s{i} *= {e};", "max": f"    s{i} = evok::max_nan(s{i}, {e});",
+                    "min": f"    s{i} = evok::min_nan(s{i}, {e});"}[ops[i]]
+
         lines = ['#include "evok_sampler.cuh"', "", "namespace evok_user {", "struct Acc {"]
         if pair:
             lines.append("  static constexpr bool kPairs = true;")
+        if nr:
+            lines.append("  static constexpr bool kRunning = true;")
+            lines.append(f"  static constexpr int kRunningSums = {nr};")
         if self.kinds:
             lines.append("  static constexpr bool kData = true;")
             lines.append(f"  static constexpr int kVectors = {len(vectors)};")
         lines.append("  float Df;")
-        lines.append("  float " + ", ".join(f"s{i} = 0.f" for i in k) + ";")
+        lines.append("  float " + ", ".join(f"s{i} = {IDENTITY[ops[i]]}" for i in k) + ";")
+        data_arg = f"const float (&d)[{nv}], " if self.kinds else ""
         if self.kinds:
             slot = {n: i for i, n in enumerate(self.kinds)}
             lines.append(f"  const float* vec[{nv}];")
@@ -266,14 +371,25 @@ class ObjectiveSpec:
             init = ["Df((float)D)", "vec{" + ", ".join(f"b.p[{slot[n]}]" for n in vectors) + "}"]
             init += [f"c_{n}(__ldg(b.p[{slot[n]}]))" for n in scalars]
             lines.append("  __device__ __forceinline__ Acc(int64_t D, const evok::DataBinding& b) : " + ", ".join(init) + " {}")
-            lines.append(f"  __device__ __forceinline__ void add(float x, int64_t j, const float (&d)[{nv}]) {{")
         else:
             lines.append("  __device__ __forceinline__ explicit Acc(int64_t D) : Df((float)D) {}")
+        if nr:
+            run = [(i, e) for i, e in enumerate(self.running_terms.values())]
+            lines.append(f"  __device__ __forceinline__ void running(float x, int64_t j, {data_arg}float (&h)[{nr}]) {{")
+            if uses_j(e for _, e in run):
+                lines.append("    const float jf = (float)j;")
+            lines += entries(run, "v", "d")
+            lines += [f"    h[{i}] = {e.cuda};" for i, e in run]
+            lines.append("  }")
+            lines.append(f"  __device__ __forceinline__ void add(float x, int64_t j, {data_arg}const float (&r)[{nr}]) {{")
+        elif self.kinds:
+            lines.append(f"  __device__ __forceinline__ void add(float x, int64_t j, const float (&d)[{nv}]) {{")
+        else:
             lines.append("  __device__ __forceinline__ void add(float x, int64_t j) {")
         if uses_j(e for _, e in element):
             lines.append("    const float jf = (float)j;")
         lines += entries(element, "v", "d")
-        lines += [f"    s{i} += {e.cuda};" for i, e in element]
+        lines += [combine(i, e.cuda) for i, e in element]
         lines.append("  }")
         if pair:
             if self.kinds:
@@ -284,10 +400,10 @@ class ObjectiveSpec:
             if uses_j(e for _, e in pair):
                 lines.append("    const float jf = (float)j;")
             lines += entries(pair, "v", "d") + entries(pair, "vn", "dn")
-            lines += [f"    s{i} += {e.cuda};" for i, e in pair]
+            lines += [combine(i, e.cuda) for i, e in pair]
             lines.append("  }")
         lines.append("  __device__ __forceinline__ float finish(int64_t) {")
-        lines += [f"    const float S_{s} = evok::warp_sum(s{i});" for i, s in zip(k, self.terms)]
+        lines += [f"    const float S_{s} = evok::{WARP_REDUCE[ops[i]]}(s{i});" for i, s in zip(k, self.terms)]
         lines.append(f"    return {self.value_expr.cuda};")
         lines += ["  }", "};", "}  // namespace evok_user", ""]
         return "\n".join(lines)
@@ -298,7 +414,7 @@ class ObjectiveSpec:
         D = X.shape[-1]
         Dt = torch.tensor(float(D), dtype=X.dtype, device=X.device)
         env = {"x": X, "j": torch.arange(D, dtype=X.dtype, device=X.device), "D": Dt, "_dtype": X.dtype, "_device": X.device}
-        # a pair term on (x_j, x_{j+1}) for j = 0 .. D-2: an empty sum when D = 1
+        # a pair term on (x_j, x_{j+1}) for j = 0 .. D-2: an empty reduction when D = 1
         penv = {"x": X[..., :-1], "xn": X[..., 1:], "j": torch.arange(max(D - 1, 0), dtype=X.dtype, device=X.device), "D": Dt,
                 "_dtype": X.dtype, "_device": X.device}
         venv = {}
@@ -315,10 +431,21 @@ class ObjectiveSpec:
                     penv[f"{name}_n"] = t[..., 1:]
                 else:
                     venv[name] = t[..., 0]
+        for c, e in self.running_terms.items():  # c_j = sum_{k <= j} h(x_k, k, D)
+            env[c] = torch.broadcast_to(_as_tensor(e.torch(env), env), rows + (D,)).cumsum(dim=-1)
         for s, e in self.terms.items():
             en = penv if s in self.pairs else env
             shape = rows + (en["x"].shape[-1],)
-            venv[s] = torch.broadcast_to(_as_tensor(e.torch(en), en), shape).sum(dim=-1)
+            t = torch.broadcast_to(_as_tensor(e.torch(en), en), shape)
+            op = self.reductions[s]
+            if op == "sum":
+                venv[s] = t.sum(dim=-1)
+            elif op == "prod":
+                venv[s] = t.prod(dim=-1)
+            elif shape[-1] == 0:  # torch.amax / amin refuse an empty dimension: the identity
+                venv[s] = torch.full(rows, -math.inf if op == "max" else math.inf, dtype=t.dtype, device=t.device)
+            else:
+                venv[s] = t.amax(dim=-1) if op == "max" else t.amin(dim=-1)
         venv.update(D=Dt, _dtype=X.dtype, _device=X.device)
         return torch.broadcast_to(_as_tensor(self.value_expr.torch(venv), venv), rows)
 

@@ -8,9 +8,10 @@ written once and never re-read for evaluation.  Called directly on a CUDA fp32 p
 row-reduction kernel (K2); on any other tensor the plain torch expression (same formula as the reference's README
 example, README.md:86-89).
 
-`FusedObjective` is the same for a user-defined function of sums over the elements (sum-separable) or over the neighbour
-pairs (x_j, x_{j+1}) of a row (Rosenbrock, Trid, Dixon-Price): its expressions are compiled at run time into the same kernels
-(evotorch_b200/jit.py), so every fused path of the package takes it.
+`FusedObjective` is the same for a user-defined function of sums, products, maxima and minima over the elements or over the
+neighbour pairs (x_j, x_{j+1}) of a row (Rosenbrock, Griewank, Schwefel 2.21), whose element terms may also see running sums
+along the row (Schwefel 1.2): its expressions are compiled at run time into the same kernels (evotorch_b200/jit.py), so every
+fused path of the package takes it.
 """
 
 from __future__ import annotations
@@ -61,7 +62,8 @@ def _ackley(x: torch.Tensor) -> torch.Tensor:
 
 class FusedObjective(BuiltinObjective):
     """A user-defined objective f(x) = value(S_1, ..., S_k, D), k <= 4, fused into the sampler, where S_i is either
-    sum_{j<D} term_i(x_j, j, D) or, for a term that uses xn = x_{j+1}, the pair sum sum_{j<D-1} term_i(x_j, x_{j+1}, j, D).
+    sum_{j<D} term_i(x_j, j, D) or, for a term that uses xn = x_{j+1}, the pair sum sum_{j<D-1} term_i(x_j, x_{j+1}, j, D); or
+    the same with a product, a maximum or a minimum in place of the sum.
 
         styblinski_tang = FusedObjective("styblinski_tang", sums={"s": "x**4 - 16*x**2 + 5*x"}, value="0.5 * s")
         rosenbrock = FusedObjective("rosenbrock", sums={"s": "100*(xn - x**2)**2 + (1 - x)**2"}, value="s")
@@ -73,6 +75,16 @@ class FusedObjective(BuiltinObjective):
 
     The batched samplers of the functional API (`pgpe_ask_and_evaluate`, `cem_ask_and_evaluate`) are 8 more kernels of the same
     source, compiled on the first batched use (`compile_batched`); `batched_kernel_info` then holds their registers and spills.
+
+    `prods`, `maxs` and `mins` are reductions of terms like those of `sums`, by product, maximum and minimum; with `sums` they
+    are at most 4 in all and share one namespace.  An empty reduction (a pair term at D = 1) is 0, 1, -inf or +inf, and a NaN
+    term makes its product, maximum or minimum NaN (as torch.prod / amax / amin).  `running` defines at most 2 running sums
+    c_j = sum_{k<=j} h(x_k, k, D), whose names the element terms of the reductions can use; `where(cond, a, b)` with one
+    comparison as cond is a conditional:
+
+        griewank = FusedObjective("griewank", sums={"s": "x**2"}, prods={"p": "cos(x / sqrt(j + 1))"}, value="1 + s / 4000 - p")
+        schwefel_1_2 = FusedObjective("schwefel_1_2", running={"c": "x"}, sums={"s": "c**2"}, value="s")
+        schwefel_2_21 = FusedObjective("schwefel_2_21", maxs={"m": "abs(x)"}, value="m")
 
     `data` gives the expressions up to 4 more names, each bound to a float32 tensor:
 
@@ -91,10 +103,12 @@ class FusedObjective(BuiltinObjective):
     to it); a tensor without batch dimensions is shared by all items.  A FusedObjective with data pickles with its tensors.  In a
     multi-GPU run every rank builds its own objective: the tensors must hold the same values on every rank."""
 
-    def __init__(self, name: str, sums: dict, value: str, data: Optional[dict] = None):
+    def __init__(self, name: str, sums: Optional[dict] = None, value: Optional[str] = None, data: Optional[dict] = None, *,
+                 prods: Optional[dict] = None, maxs: Optional[dict] = None, mins: Optional[dict] = None, running: Optional[dict] = None):
         from . import jit
 
-        spec = jit.ObjectiveSpec(sums, value, jit.data_kinds(data) if data else None)
+        spec = jit.ObjectiveSpec(sums, value, jit.data_kinds(data) if data else None, prods=prods, maxs=maxs, mins=mins,
+                                 running=running)
         if name in ops.OBJECTIVE_IDS and ops.OBJECTIVE_IDS[name] < ops.OBJ_USER_BASE:
             raise ValueError(f"{name!r} is the name of a built-in objective")
         self.data = dict(data) if data else {}
@@ -102,6 +116,7 @@ class FusedObjective(BuiltinObjective):
         compiled = jit.compile_objective(spec)
         super().__init__(name, compiled.objective_id, (lambda X: spec.torch_fn(X, self.data)) if self.data else spec.torch_fn)
         self.sums, self.value, self.source = dict(spec.sums), spec.value, spec.source
+        self.prods, self.maxs, self.mins, self.running = dict(spec.prods), dict(spec.maxs), dict(spec.mins), dict(spec.running)
         self.kernel_info = compiled.kernel_info
         self.batched_kernel_info = None
         self._spec = spec
@@ -153,7 +168,11 @@ class FusedObjective(BuiltinObjective):
         """A twin of this objective on other tensors (all of its data names, of the same kinds): no recompile."""
         if set(tensors) != set(self.data):
             raise ValueError(f"with_data: expected the data names {list(self.data)}, got {list(tensors)}")
-        return FusedObjective(self.name, self.sums, self.value, {n: tensors[n] for n in self.data})
+        return FusedObjective(self.name, self.sums, self.value, {n: tensors[n] for n in self.data}, **self._keywords())
+
+    def _keywords(self) -> dict:
+        """The non-empty ones of prods, maxs, mins and running (an objective of sums only has none)."""
+        return {k: v for k, v in (("prods", self.prods), ("maxs", self.maxs), ("mins", self.mins), ("running", self.running)) if v}
 
     def compile_batched(self) -> None:
         """Compile and attach the batched samplers (once per process for one source); fills `batched_kernel_info`."""
@@ -163,11 +182,21 @@ class FusedObjective(BuiltinObjective):
             self.batched_kernel_info = jit.compile_batched(self._spec).kernel_info
 
     def __reduce__(self):
-        return (FusedObjective, (self.name, self.sums, self.value) + ((self.data,) if self.data else ()))
+        args = (self.name, self.sums, self.value) + ((self.data,) if self.data else ())
+        kw = self._keywords()
+        if not kw:
+            return (FusedObjective, args)
+        return (_make_fused, (args, kw))
 
     def __repr__(self) -> str:
         data = ", data={" + ", ".join(f"{n!r}: {tuple(t.shape)}" for n, t in self.data.items()) + "}" if self.data else ""
-        return f"FusedObjective({self.name!r}, sums={self.sums!r}, value={self.value!r}{data})"
+        more = "".join(f", {k}={v!r}" for k, v in self._keywords().items())
+        return f"FusedObjective({self.name!r}, sums={self.sums!r}, value={self.value!r}{data}{more})"
+
+
+def _make_fused(args: tuple, keywords: dict) -> FusedObjective:
+    """Unpickle a FusedObjective with keyword reductions or running sums."""
+    return FusedObjective(*args, **keywords)
 
 
 def _release(instance_id: int) -> None:
