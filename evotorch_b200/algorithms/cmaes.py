@@ -165,9 +165,13 @@ class CMAES(SearchAlgorithm, SinglePopulationAlgorithmMixin, CUDAGraphMixin):
         # persistent buffers of the fused generation (the separable one draws inside its own sampler and keeps no zs)
         fs = self.__dict__.get("_fused") if n == self.popsize and not self.separable else None
         zs = problem.make_empty(num_solutions=n) if fs is None else fs["zs"]
+        self.__dict__.pop("_z_draw", None)
         if ops.uses_kernels(zs) and problem.rng == "philox":
             zero, one = (problem.make_zeros(d), problem.make_ones(d)) if fs is None else (fs["zero"], fs["one"])
-            ops.sample_eval(ops.OBJ_NONE, zs, zero, one, n_rows=n, symmetric=False, **problem.next_philox_draw().kwargs)
+            draw = problem.next_philox_draw()
+            ops.sample_eval(ops.OBJ_NONE, zs, zero, one, n_rows=n, symmetric=False, **draw.kwargs)
+            # row i of xs is m + sigma A z_i of this draw: an objective with noise evaluates it with the same draw (_rows_draw)
+            self._z_draw = draw
         else:
             problem.make_gaussian(out=zs)
         if self.separable:
@@ -184,10 +188,19 @@ class CMAES(SearchAlgorithm, SinglePopulationAlgorithmMixin, CUDAGraphMixin):
         xs = self.m.unsqueeze(0) + self.sigma * ys
         return zs, ys, xs
 
+    def _take_z_draw(self):
+        """The z draw of the population about to be evaluated (taken once), or None: rows that a before-eval hook may edit, or that
+        an overriding `sample_distribution` produced, have no draw of their own."""
+        draw = self.__dict__.pop("_z_draw", None)
+        if len(self._problem.before_eval_hook) or "sample_distribution" in self.__dict__ or type(self).sample_distribution is not CMAES.sample_distribution:
+            return None
+        return draw
+
     def get_population_weights(self, xs: torch.Tensor) -> torch.Tensor:
         """Evaluate, sort best-first, weight of each solution = weights[rank] (cmaes.py:432-452)."""
         self._population.set_values(xs)
-        self._problem.evaluate(self._population)
+        with self._problem._rows_drawn_by(self._take_z_draw()):
+            self._problem.evaluate(self._population)
         indices = self._population.argsort(obj_index=self.obj_index)
         ranks = torch.empty_like(indices)
         ranks[indices] = torch.arange(self.popsize, dtype=indices.dtype, device=indices.device)
@@ -325,7 +338,8 @@ class CMAES(SearchAlgorithm, SinglePopulationAlgorithmMixin, CUDAGraphMixin):
             pop._evdata.fill_(float("nan"))
         else:  # an overriding `sample_distribution` (e.g. recorded draws in the tests) returns its own tensors
             pop.set_values(xs)
-        self._problem.evaluate(pop)
+        with self._problem._rows_drawn_by(self._take_z_draw()):
+            self._problem.evaluate(pop)
         f = pop._evdata.view(-1)
         ops.rank_table(f, self._problem.senses[self._obj_index] == "max", self.weights, out=fs["aw"])
         ops.cmaes_row_weights(fs["aw"], zs, self.active, fs["w_pos"], fs["w_act"])

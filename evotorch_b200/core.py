@@ -12,6 +12,7 @@ multi-objective pareto utilities.  Population sharding across GPUs is done with 
 
 from __future__ import annotations
 
+import contextlib
 import math
 from dataclasses import dataclass, replace
 from typing import Any, Callable, Iterable, Optional, Union
@@ -472,7 +473,13 @@ class Problem(Clonable):
     def _evaluate_batch(self, batch: "SolutionBatch"):
         """Override point (core.py:2602-2611).  Built-in objectives run the K2 row-reduction kernel."""
         if self._vectorized and self._objective_func is not None:
-            result = self._objective_func(batch.values)
+            fn, values = self._objective_func, batch.values
+            if getattr(fn, "takes_key", None) is not None and fn.takes_key(values):
+                # a fused objective with noise: the rows' own draw (`_rows_drawn_by`), else a fresh one of this problem
+                draw = getattr(self, "_rows_draw", None)
+                result = fn.evaluate_keyed(values, draw if draw is not None else self.next_philox_draw())
+            else:
+                result = fn(values)
             if isinstance(result, tuple):
                 batch.set_evals(*result)
             else:
@@ -480,6 +487,16 @@ class Problem(Clonable):
         else:
             for sln in batch:
                 self._evaluate(sln)
+
+    @contextlib.contextmanager
+    def _rows_drawn_by(self, draw: Optional["PhiloxDraw"]):
+        """Inside, the rows evaluated are those that `draw` sampled (full-covariance CMA-ES: X = m + sigma A z of its z draw), so
+        an objective with noise evaluates them with that draw rather than a fresh one; None: no draw of their own."""
+        self._rows_draw = draw
+        try:
+            yield
+        finally:
+            self.__dict__.pop("_rows_draw", None)
 
     def _evaluate(self, solution: "Solution"):
         if self._objective_func is None:

@@ -101,6 +101,8 @@ struct Objective {
   // evok_objective_declare_data: the data names of its accumulator (0: none) and which of them are vectors of the row length
   int n_data = 0;
   bool is_vector[EVOK_MAX_DATA] = {};
+  // evok_objective_declare_noise: its accumulator draws noise, and its EVOK_OBJ_KERNEL_EVAL entries take the key
+  bool noisy = false;
   DeviceKernels dev[kMaxDevices];
 };
 
@@ -199,6 +201,13 @@ static int bind_data(int objective, int64_t D, int64_t items, LaunchData* out) {
     out->binding.item_stride[i] = stride;
   }
   return 0;
+}
+
+// true for a registered id (a base, not an instance) that declares noise
+static bool is_noisy(int base) {
+  if (!is_user(base)) return false;
+  std::lock_guard<std::mutex> lock(g_objective_mutex);
+  return g_user[base - EVOK_OBJ_USER_BASE]->noisy;
 }
 
 static void fill_builtin(int objective, int dev, DeviceKernels& d) {
@@ -399,6 +408,13 @@ extern "C" EVOK_API int evok_objective_declare_data(int objective, int n_data, c
   return 0;
 }
 
+extern "C" EVOK_API int evok_objective_declare_noise(int objective) {
+  if (!is_user(objective)) return EVOK_E_BADENUM;
+  std::lock_guard<std::mutex> lock(g_objective_mutex);
+  g_user[objective - EVOK_OBJ_USER_BASE]->noisy = true;
+  return 0;
+}
+
 extern "C" EVOK_API int evok_objective_instance(int base, const float* const* ptrs_host, const int64_t* lens_host, const int64_t* item_strides_host,
                                                 int64_t n_items, int n_data, int* id_out_host) {
   if (!ptrs_host || !lens_host || !item_strides_host || !id_out_host) return EVOK_E_NULLPTR;
@@ -480,17 +496,32 @@ extern "C" EVOK_API int evok_sample_eval_push(int objective, float* X, int64_t l
                 nullptr, nullptr, push, (cudaStream_t)stream);
 }
 
-extern "C" EVOK_API int evok_eval(int objective, const float* X, int64_t ldx, int64_t n_rows, int64_t D, float* f, void* stream) {
+// evok_eval (keyed = false) and evok_eval_keyed.  The evaluation kernel's last argument is the draw of the rows (EvalKey) for
+// an objective with noise, an empty struct (which takes its one byte from `noise`) for every other.
+static int eval_call(int objective, const float* X, int64_t ldx, int64_t row0, int64_t n_rows, int64_t D, bool keyed, uint64_t seed,
+                     uint64_t stream_id, const uint32_t* stream_off, float* f, cudaStream_t st) {
   if (!X || !f) return EVOK_E_NULLPTR;
   const int base = base_of(objective);
   if ((base <= EVOK_OBJ_NONE || base >= EVOK_OBJ_COUNT) && !is_user(base)) return EVOK_E_BADENUM;
-  if (n_rows < 0 || D <= 0 || ldx < D) return EVOK_E_BADSIZE;
+  if (n_rows < 0 || D <= 0 || ldx < D || row0 < 0) return EVOK_E_BADSIZE;
+  const bool noisy = is_noisy(base);
+  if (noisy && !keyed) return EVOK_E_NOISEKEY;
   if (n_rows == 0) return 0;
   LaunchData data;
   if (const int rc = bind_data(objective, D, 0, &data)) return rc;
   const KernelChoice c = choose_kernel(EVOK_OBJ_KERNEL_EVAL, false, X, ldx, nullptr, nullptr, n_rows, D, data);
-  void* args[] = {&X, &ldx, &n_rows, &D, &f, &data.binding};
-  return launch(data.base, c, args, (cudaStream_t)stream);
+  EvalKey noise{noisy ? make_philox_key(seed, stream_id) : PhiloxKey{}, stream_off, row0};
+  void* args[] = {&X, &ldx, &n_rows, &D, &f, &data.binding, &noise};
+  return launch(data.base, c, args, st);
+}
+
+extern "C" EVOK_API int evok_eval(int objective, const float* X, int64_t ldx, int64_t n_rows, int64_t D, float* f, void* stream) {
+  return eval_call(objective, X, ldx, 0, n_rows, D, false, 0, 0, nullptr, f, (cudaStream_t)stream);
+}
+
+extern "C" EVOK_API int evok_eval_keyed(int objective, const float* X, int64_t ldx, int64_t row0, int64_t n_rows, int64_t D, uint64_t seed,
+                                        uint64_t stream_id, const uint32_t* stream_offset_dev, float* f, void* stream) {
+  return eval_call(objective, X, ldx, row0, n_rows, D, true, seed, stream_id, stream_offset_dev, f, (cudaStream_t)stream);
 }
 
 // One launch per item chunk of the batched family: item b of the batch samples with stream word (stream_id0 + b), chunk b0 of

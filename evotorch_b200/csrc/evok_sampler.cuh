@@ -129,6 +129,57 @@ __device__ __forceinline__ void normals4(const PhiloxKey& key, uint32_t stream_w
 }
 
 // ------------------------------------------------------------------------------------------------
+// Noise: the draws of rand() / randn() in a generated accumulator, on the key and stream word of the population's own draw.
+// Occurrence k of the source (0 .. 3 in the element terms, 4 .. 7 in `value`) at global row `row` takes Philox counter
+//   c = (x, (uint32)row, 0x80000000 | k << 24 | (row >> 32) & 0xFFFFFF, stream word),
+// x = the column group q = j >> 2 of an element occurrence at column j, 0xFFFFFFFF for one in `value`.  A sample counter
+// (normals4) has c.z = unit >> 32 < 2^31, so no noise counter equals a sample counter, on any path.
+// rand() is (word >> 8) * 2^-24 in [0, 1), exact in float32; randn() is box_muller of the sampler.
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ U4 noise_bits(const PhiloxKey& key, uint32_t stream_word, uint64_t row, uint32_t x, int k) {
+  U4 c;
+  c.x = x;
+  c.y = (uint32_t)row;
+  c.z = 0x80000000u | ((uint32_t)k << 24) | ((uint32_t)(row >> 32) & 0xFFFFFFu);
+  c.w = stream_word;
+  return philox4x32_10(c, key);
+}
+__device__ __forceinline__ float uniform24(uint32_t w) { return (float)(w >> 8) * 5.9604644775390625e-08f; }
+
+// element occurrence k at the 4 columns of group q: rand() takes word c for column 4q + c; randn() the normals4 layout
+// (columns 4q, 4q + 1 from (x, y), 4q + 2, 4q + 3 from (z, w))
+__device__ __forceinline__ void noise4(const PhiloxKey& key, uint32_t stream_word, uint64_t row, uint32_t q, int k, bool normal, float u[4]) {
+  const U4 r = noise_bits(key, stream_word, row, q, k);
+  if (normal) {
+    box_muller(r.x, r.y, u[0], u[1]);
+    box_muller(r.z, r.w, u[2], u[3]);
+  } else {
+    u[0] = uniform24(r.x); u[1] = uniform24(r.y); u[2] = uniform24(r.z); u[3] = uniform24(r.w);
+  }
+}
+// the same draw for column j alone (one call, one word or one word pair): entry j & 3 of noise4 for group j >> 2
+__device__ __forceinline__ float noise1(const PhiloxKey& key, uint32_t stream_word, uint64_t row, int64_t j, int k, bool normal) {
+  const U4 r = noise_bits(key, stream_word, row, (uint32_t)(j >> 2), k);
+  const int c = (int)(j & 3);
+  if (normal) {
+    float z0, z1;
+    box_muller(c < 2 ? r.x : r.z, c < 2 ? r.y : r.w, z0, z1);
+    return (c & 1) ? z1 : z0;
+  }
+  return uniform24(c == 0 ? r.x : c == 1 ? r.y : c == 2 ? r.z : r.w);
+}
+// occurrence k of `value`: rand() takes word x, randn() z0 of box_muller(x, y)
+__device__ __forceinline__ float value_rand(const PhiloxKey& key, uint32_t stream_word, uint64_t row, int k) {
+  return uniform24(noise_bits(key, stream_word, row, 0xFFFFFFFFu, k).x);
+}
+__device__ __forceinline__ float value_randn(const PhiloxKey& key, uint32_t stream_word, uint64_t row, int k) {
+  const U4 r = noise_bits(key, stream_word, row, 0xFFFFFFFFu, k);
+  float z0, z1;
+  box_muller(r.x, r.y, z0, z1);
+  return z0;
+}
+
+// ------------------------------------------------------------------------------------------------
 // Warp reductions
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ float warp_sum(float v) {
@@ -212,6 +263,11 @@ __device__ __forceinline__ void st_stream1(float* p, float a) {
 // column, so add() takes them, after the data entries of an accumulator with data:
 //   running(x, j[, d], h)  : h[i] = the increment of running sum i at column j;
 //   add(x, j[, d], r)      : fold element x of column j, where r[i] = c_j of running sum i (fold_running computes it).
+// A generated accumulator may also draw noise (`static constexpr bool kNoise = true`, see NoiseTerms below): kDraws <= 4
+// occurrences of rand() / randn() in its element terms (bit k of kNormalDraws: occurrence k is randn()) and up to 4 in `value`.
+// Its element draws at column j reach add() (and running() / add_pair(), which do not use them) as the entries d[kVectors + k]
+// after the data entries, loaded next to them (DataCols::draw4 / draw1), and its finish takes the draw of its row:
+//   finish(D, key, stream_word, row) : row = the global row index; `value` draws with value_rand / value_randn.
 // The built-in ones are ObjAcc<EVOK_OBJ_*>; a user-defined one is generated by evotorch_b200/jit.py.
 // ------------------------------------------------------------------------------------------------
 template <int OBJ>
@@ -328,6 +384,59 @@ struct DataTerms<Acc, decltype(void(Acc::kData))> {
   using Arg = DataBinding;
 };
 
+// The draw of the rows that eval_kernel evaluates, its last argument for an accumulator with noise: row r of X is global row
+// row0 + r, on stream word key.stream_lo + *stream_off (stream_off may be null)
+struct EvalKey {
+  PhiloxKey key;
+  const uint32_t* stream_off;
+  int64_t row0;
+};
+
+// true for an accumulator that declares `static constexpr bool kNoise = true` (a generated one with rand() / randn()); kDraws
+// of its occurrences are in the element terms, kNormal has bit k set for a randn() among them.  All noise code is under
+// `if constexpr` on it.
+template <typename Acc, typename = void>
+struct NoiseTerms {
+  static constexpr bool value = false;
+  static constexpr int kDraws = 0;
+  static constexpr unsigned kNormal = 0;
+  using EvalArg = NoData;
+  static constexpr int kEvalMinBlocks = 0;  // eval_kernel's launch bounds: none beyond the block size
+};
+template <typename Acc>
+struct NoiseTerms<Acc, decltype(void(Acc::kNoise))> {
+  static constexpr bool value = Acc::kNoise;
+  static constexpr int kDraws = Acc::kDraws;
+  static constexpr unsigned kNormal = Acc::kNormalDraws;
+  using EvalArg = EvalKey;
+  // 2 CTAs per SM: without a bound ptxas fits the kernel of a `value` draw with few element terms into 32 registers and spills
+  static constexpr int kEvalMinBlocks = 2;
+};
+
+// the data vectors of an accumulator (0 without data terms)
+template <typename Acc, bool = DataTerms<Acc>::value>
+struct DataVectors {
+  static constexpr int value = 0;
+};
+template <typename Acc>
+struct DataVectors<Acc, true> {
+  static constexpr int value = Acc::kVectors;
+};
+
+// an accumulator whose folds take per-column entries (data vectors, element draws): add / add_pair / running get the d arrays
+template <typename Acc>
+struct ColTerms {
+  static constexpr bool value = DataTerms<Acc>::value || NoiseTerms<Acc>::kDraws > 0;
+  static constexpr int kVectors = DataVectors<Acc>::value;
+};
+
+// acc.finish of the row with global index `row`: an accumulator with noise draws its `value` occurrences from (key, sw, row)
+template <typename Acc>
+__device__ __forceinline__ float finish_row(Acc& acc, int64_t D, const PhiloxKey& key, uint32_t sw, uint64_t row) {
+  if constexpr (NoiseTerms<Acc>::value) return acc.finish(D, key, sw, row);
+  else return acc.finish(D);
+}
+
 template <typename Acc, typename Arg>
 __device__ __forceinline__ Acc make_acc(int64_t D, const Arg& data) {
   if constexpr (DataTerms<Acc>::value) return Acc(D, data);
@@ -346,25 +455,43 @@ __device__ __forceinline__ DataBinding item_data(DataBinding d, int64_t item) {
 // symmetric pair.  `left` is the entry at the column before the first (the left neighbour of a pair fold across lanes).
 template <typename Acc, int N>
 struct DataCols {
-  static constexpr int kSlots = Acc::kVectors > 0 ? Acc::kVectors : 1;
+  static constexpr int kVectors = ColTerms<Acc>::kVectors, kDraws = NoiseTerms<Acc>::kDraws;
+  static constexpr int kSlots = kVectors + kDraws > 0 ? kVectors + kDraws : 1;
   float v[N][kSlots], left[kSlots];
   // columns j .. j + 3 with one 16-byte load per vector: the vectorised kernels, which the host picks only when every vector is
   // 16-byte aligned (choose_kernel)
   __device__ __forceinline__ void load4(const Acc& acc, int64_t j) {
     static_assert(N == 4, "a column group is 4 columns");
+    if constexpr (kVectors > 0)  // an accumulator with element draws and no data has no `vec`
 #pragma unroll
-    for (int i = 0; i < Acc::kVectors; ++i) {
+    for (int i = 0; i < kVectors; ++i) {
       const float4 t = __ldg(reinterpret_cast<const float4*>(acc.vec[i] + j));
       v[0][i] = t.x; v[1][i] = t.y; v[2][i] = t.z; v[3][i] = t.w;
     }
   }
   __device__ __forceinline__ void load1(const Acc& acc, int64_t j, int c) {  // column j into slot c
+    if constexpr (kVectors > 0)
 #pragma unroll
-    for (int i = 0; i < Acc::kVectors; ++i) v[c][i] = __ldg(acc.vec[i] + j);
+    for (int i = 0; i < kVectors; ++i) v[c][i] = __ldg(acc.vec[i] + j);
   }
   __device__ __forceinline__ void load_left(const Acc& acc, int64_t j) {  // column j - 1, j > 0
+    if constexpr (kVectors > 0)
 #pragma unroll
-    for (int i = 0; i < Acc::kVectors; ++i) left[i] = __ldg(acc.vec[i] + j - 1);
+    for (int i = 0; i < kVectors; ++i) left[i] = __ldg(acc.vec[i] + j - 1);
+  }
+  // the element draws of global row `row` at the columns of group q (one Philox call per occurrence), after the data entries
+  __device__ __forceinline__ void draw4(const PhiloxKey& key, uint32_t sw, uint64_t row, uint32_t q) {
+    static_assert(N == 4, "a column group is 4 columns");
+#pragma unroll
+    for (int k = 0; k < kDraws; ++k) {
+      float u[4];
+      noise4(key, sw, row, q, k, (NoiseTerms<Acc>::kNormal >> k) & 1u, u);
+      v[0][kVectors + k] = u[0]; v[1][kVectors + k] = u[1]; v[2][kVectors + k] = u[2]; v[3][kVectors + k] = u[3];
+    }
+  }
+  __device__ __forceinline__ void draw1(const PhiloxKey& key, uint32_t sw, uint64_t row, int64_t j, int c) {  // column j into slot c
+#pragma unroll
+    for (int k = 0; k < kDraws; ++k) v[c][kVectors + k] = noise1(key, sw, row, j, k, (NoiseTerms<Acc>::kNormal >> k) & 1u);
   }
 };
 struct NoCols {
@@ -372,7 +499,12 @@ struct NoCols {
   template <typename Acc> __device__ __forceinline__ void load1(const Acc&, int64_t, int) {}
   template <typename Acc> __device__ __forceinline__ void load_left(const Acc&, int64_t) {}
 };
-template <typename Acc, int N, bool = DataTerms<Acc>::value>
+// true when the element terms draw noise: the + and - rows of a direction then fold with their own column entries
+template <typename Acc>
+struct ElementDraws {
+  static constexpr bool value = NoiseTerms<Acc>::kDraws > 0;
+};
+template <typename Acc, int N, bool = ColTerms<Acc>::value>
 struct ColsOf {
   using type = NoCols;
 };
@@ -384,7 +516,7 @@ struct ColsOf<Acc, N, true> {
 // acc.add of element x of column j, which is slot c of dc
 template <typename Acc, typename Cols>
 __device__ __forceinline__ void fold(Acc& acc, float x, int64_t j, const Cols& dc, int c) {
-  if constexpr (DataTerms<Acc>::value) acc.add(x, j, dc.v[c]);
+  if constexpr (ColTerms<Acc>::value) acc.add(x, j, dc.v[c]);
   else acc.add(x, j);
 }
 
@@ -402,13 +534,13 @@ __device__ __forceinline__ void fold_pairs(Acc& acc, const float (&v)[N], int64_
   const float left = lane == 0 ? carry : rot;
   carry = rot;
   if (n_valid > 0 && j > 0) {
-    if constexpr (DataTerms<Acc>::value) acc.add_pair(left, v[0], j - 1, dc.left, dc.v[0]);
+    if constexpr (ColTerms<Acc>::value) acc.add_pair(left, v[0], j - 1, dc.left, dc.v[0]);
     else acc.add_pair(left, v[0], j - 1);
   }
 #pragma unroll
   for (int c = 1; c < N; ++c)
     if (c < n_valid) {
-      if constexpr (DataTerms<Acc>::value) acc.add_pair(v[c - 1], v[c], j + c - 1, dc.v[c - 1], dc.v[c]);
+      if constexpr (ColTerms<Acc>::value) acc.add_pair(v[c - 1], v[c], j + c - 1, dc.v[c - 1], dc.v[c]);
       else acc.add_pair(v[c - 1], v[c], j + c - 1);
     }
 }
@@ -431,7 +563,7 @@ __device__ __forceinline__ void fold_running(Acc& acc, const float (&v)[N], int6
 #pragma unroll
     for (int i = 0; i < R; ++i) h[i] = 0.f;
     if (c < n_valid) {
-      if constexpr (DataTerms<Acc>::value) acc.running(v[c], j + c, dc.v[c], h);
+      if constexpr (ColTerms<Acc>::value) acc.running(v[c], j + c, dc.v[c], h);
       else acc.running(v[c], j + c, h);
     }
 #pragma unroll
@@ -455,7 +587,7 @@ __device__ __forceinline__ void fold_running(Acc& acc, const float (&v)[N], int6
 #pragma unroll
   for (int c = 0; c < N; ++c)
     if (c < n_valid) {
-      if constexpr (DataTerms<Acc>::value) acc.add(v[c], j + c, dc.v[c], p[c]);
+      if constexpr (ColTerms<Acc>::value) acc.add(v[c], j + c, dc.v[c], p[c]);
       else acc.add(v[c], j + c, p[c]);
     }
 }
@@ -493,11 +625,34 @@ __device__ __forceinline__ void fold_step(Acc& acc, const float (&v)[N], int64_t
 constexpr int kSampleThreads = EVOK_SAMPLE_THREADS;
 // the fused kernels are issue/XU bound (two independent Philox chains per lane help); the sample-only kernel is store
 // bound and prefers occupancy
+// (more than one element draw per column: one Philox chain per lane and 2 CTAs per SM, so that no kernel spills)
 template <typename Acc>
 struct SampleTune {
-  static constexpr int kUnroll = SampleOnly<Acc>::value ? EVOK_SAMPLEONLY_UNR : RunningTerms<Acc>::value ? 1 : EVOK_SAMPLE_UNR;
-  static constexpr int kMinBlocks = SampleOnly<Acc>::value ? EVOK_SAMPLEONLY_MINB : EVOK_SAMPLE_MINB;
+  static constexpr bool kManyDraws = NoiseTerms<Acc>::kDraws > 1;
+  static constexpr int kUnroll = SampleOnly<Acc>::value ? EVOK_SAMPLEONLY_UNR : RunningTerms<Acc>::value || kManyDraws ? 1 : EVOK_SAMPLE_UNR;
+  static constexpr int kMinBlocks = SampleOnly<Acc>::value ? EVOK_SAMPLEONLY_MINB : kManyDraws ? 2 : EVOK_SAMPLE_MINB;
 };
+
+// the column entries the - row of a direction folds with: its own (dm) when the element terms draw noise, else the + row's
+template <typename Acc, typename Cols>
+__device__ __forceinline__ const Cols& minus_cols(const Cols& dp, const Cols& dm) {
+  if constexpr (ElementDraws<Acc>::value) return dm;
+  else return dp;
+}
+
+// the element draws of unit `unit` at column group q: its row (the + row, global row 2 unit, of a direction) into dp, and the
+// - row's (2 unit + 1) into dm, which takes dp's data entries first
+template <typename Acc, bool SYM, typename Cols>
+__device__ __forceinline__ void draw_rows(Cols& dp, Cols& dm, const PhiloxKey& key, uint32_t sw, uint64_t unit, uint32_t q) {
+  if constexpr (ElementDraws<Acc>::value) {
+    const uint64_t row = SYM ? 2 * unit : unit;
+    if (SYM) {
+      dm = dp;
+      dm.draw4(key, sw, row + 1, q);
+    }
+    dp.draw4(key, sw, row, q);
+  }
+}
 
 // one column group (4 columns) of one unit: sample, store, accumulate.  SQ: also *zsq += z^2 (the unscaled normals; the
 // squared norm that separable CMA-ES's active reweighting needs), in column order
@@ -508,7 +663,8 @@ __device__ __forceinline__ void sample_group(const PhiloxKey& key, uint32_t sw, 
   float z[4];
   normals4(key, sw, unit, q, z);
   const int64_t j = (int64_t)q << 2;
-  typename ColsOf<Acc, 4>::type dc;
+  typename ColsOf<Acc, 4>::type dc, dm;  // dm: the - row's entries, with its own draws (element noise only)
+  const auto& dcm = minus_cols<Acc>(dc, dm);
   if (VEC) {
     if (SQ) {
       *zsq = fmaf(z[0], z[0], *zsq); *zsq = fmaf(z[1], z[1], *zsq); *zsq = fmaf(z[2], z[2], *zsq); *zsq = fmaf(z[3], z[3], *zsq);
@@ -518,13 +674,15 @@ __device__ __forceinline__ void sample_group(const PhiloxKey& key, uint32_t sw, 
     const float p0 = fmaf(s.x, z[0], m.x), p1 = fmaf(s.y, z[1], m.y), p2 = fmaf(s.z, z[2], m.z), p3 = fmaf(s.w, z[3], m.w);
     if (STORE) st_stream4(xp + j, p0, p1, p2, p3);
     dc.load4(accp, j);
+    draw_rows<Acc, SYM>(dc, dm, key, sw, unit, q);
     fold(accp, p0, j, dc, 0); fold(accp, p1, j + 1, dc, 1); fold(accp, p2, j + 2, dc, 2); fold(accp, p3, j + 3, dc, 3);
     if (SYM) {
       const float n0 = fmaf(-s.x, z[0], m.x), n1 = fmaf(-s.y, z[1], m.y), n2 = fmaf(-s.z, z[2], m.z), n3 = fmaf(-s.w, z[3], m.w);
       if (STORE) st_stream4(xm + j, n0, n1, n2, n3);
-      fold(accm, n0, j, dc, 0); fold(accm, n1, j + 1, dc, 1); fold(accm, n2, j + 2, dc, 2); fold(accm, n3, j + 3, dc, 3);
+      fold(accm, n0, j, dcm, 0); fold(accm, n1, j + 1, dcm, 1); fold(accm, n2, j + 2, dcm, 2); fold(accm, n3, j + 3, dcm, 3);
     }
   } else {
+    draw_rows<Acc, SYM>(dc, dm, key, sw, unit, q);
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
       if (j + c < D) {
@@ -537,7 +695,8 @@ __device__ __forceinline__ void sample_group(const PhiloxKey& key, uint32_t sw, 
         if (SYM) {
           const float n = fmaf(-s, z[c], m);
           if (STORE) st_stream1(xm + j + c, n);
-          fold(accm, n, j + c, dc, c);
+          if constexpr (ElementDraws<Acc>::value) dm.load1(accp, j + c, c);
+          fold(accm, n, j + c, dcm, c);
         }
       }
     }
@@ -557,7 +716,8 @@ __device__ __forceinline__ void sample_group_pairs(const PhiloxKey& key, uint32_
   float p[4] = {0.f, 0.f, 0.f, 0.f}, n[4] = {0.f, 0.f, 0.f, 0.f};
   const int64_t j = (int64_t)q << 2;
   int n_valid = 0;
-  typename ColsOf<Acc, 4>::type dc;
+  typename ColsOf<Acc, 4>::type dc, dm;  // dm: the - row's entries, with its own draws (element noise only)
+  const auto& dcm = minus_cols<Acc>(dc, dm);
   if (active) {
     float z[4];
     normals4(key, sw, unit, q, z);
@@ -570,6 +730,7 @@ __device__ __forceinline__ void sample_group_pairs(const PhiloxKey& key, uint32_
       p[0] = fmaf(s.x, z[0], m.x); p[1] = fmaf(s.y, z[1], m.y); p[2] = fmaf(s.z, z[2], m.z); p[3] = fmaf(s.w, z[3], m.w);
       if (STORE) st_stream4(xp + j, p[0], p[1], p[2], p[3]);
       dc.load4(accp, j);
+      draw_rows<Acc, SYM>(dc, dm, key, sw, unit, q);
       if constexpr (kFoldNow) {
         fold(accp, p[0], j, dc, 0); fold(accp, p[1], j + 1, dc, 1); fold(accp, p[2], j + 2, dc, 2); fold(accp, p[3], j + 3, dc, 3);
       }
@@ -577,11 +738,12 @@ __device__ __forceinline__ void sample_group_pairs(const PhiloxKey& key, uint32_
         n[0] = fmaf(-s.x, z[0], m.x); n[1] = fmaf(-s.y, z[1], m.y); n[2] = fmaf(-s.z, z[2], m.z); n[3] = fmaf(-s.w, z[3], m.w);
         if (STORE) st_stream4(xm + j, n[0], n[1], n[2], n[3]);
         if constexpr (kFoldNow) {
-          fold(accm, n[0], j, dc, 0); fold(accm, n[1], j + 1, dc, 1); fold(accm, n[2], j + 2, dc, 2); fold(accm, n[3], j + 3, dc, 3);
+          fold(accm, n[0], j, dcm, 0); fold(accm, n[1], j + 1, dcm, 1); fold(accm, n[2], j + 2, dcm, 2); fold(accm, n[3], j + 3, dcm, 3);
         }
       }
       n_valid = 4;
     } else {
+      draw_rows<Acc, SYM>(dc, dm, key, sw, unit, q);
 #pragma unroll
       for (int c = 0; c < 4; ++c) {
         if (j + c < D) {
@@ -594,7 +756,8 @@ __device__ __forceinline__ void sample_group_pairs(const PhiloxKey& key, uint32_
           if (SYM) {
             n[c] = fmaf(-s, z[c], m);
             if (STORE) st_stream1(xm + j + c, n[c]);
-            if constexpr (kFoldNow) fold(accm, n[c], j + c, dc, c);
+            if constexpr (ElementDraws<Acc>::value) dm.load1(accp, j + c, c);
+            if constexpr (kFoldNow) fold(accm, n[c], j + c, dcm, c);
           }
         }
       }
@@ -602,9 +765,12 @@ __device__ __forceinline__ void sample_group_pairs(const PhiloxKey& key, uint32_
     }
   }
   if constexpr (PairTerms<Acc>::value)
-    if (n_valid > 0 && j > 0) dc.load_left(accp, j);
+    if (n_valid > 0 && j > 0) {
+      dc.load_left(accp, j);
+      if constexpr (ElementDraws<Acc>::value) dm.load_left(accp, j);
+    }
   fold_step<4>(accp, p, j, n_valid, carry_p, dc);
-  if (SYM) fold_step<4>(accm, n, j, n_valid, carry_m, dc);
+  if (SYM) fold_step<4>(accm, n, j, n_valid, carry_m, dcm);
 }
 
 // One unit u (a direction of symmetric sampling, else a row) of the warp of lane `lane`: sample its row(s) from (key, stream word sw, unit
@@ -654,9 +820,10 @@ __device__ __forceinline__ void sample_eval_unit(int lane, float* __restrict__ X
     if (lane == 0) q_out[r] = zsq;
   }
   if (!SampleOnly<Acc>::value) {
-    const float fp = accp.finish(D);
+    const uint64_t row = SYM ? 2 * unit : unit;  // the global row of the + row (or the row)
+    const float fp = finish_row(accp, D, key, sw, row);
     float fm = 0.f;
-    if (SYM) fm = accm.finish(D);
+    if (SYM) fm = finish_row(accm, D, key, sw, row + 1);
     if (lane == 0) {
       if (PUSH) {
         for (int p = 0; p < sink.world; ++p) {
@@ -722,11 +889,27 @@ __global__ void __launch_bounds__(kSampleThreads, SampleTune<Acc>::kMinBlocks)
 
 constexpr int kEvalThreads = 256;
 
+// the stream word of eval_kernel's draw, and the fitness of its row r (an accumulator with noise draws from global row row0 + r)
+template <typename Acc>
+__device__ __forceinline__ uint32_t eval_stream_word(const typename NoiseTerms<Acc>::EvalArg& noise) {
+  if constexpr (NoiseTerms<Acc>::value) return noise.key.stream_lo + (noise.stream_off ? __ldg(noise.stream_off) : 0u);
+  else return 0u;
+}
+template <typename Acc>
+__device__ __forceinline__ float eval_finish(Acc& acc, int64_t D, const typename NoiseTerms<Acc>::EvalArg& noise, uint32_t sw, int64_t r) {
+  if constexpr (NoiseTerms<Acc>::value) return acc.finish(D, noise.key, sw, (uint64_t)(noise.row0 + r));
+  else return acc.finish(D);
+}
+
+// The evaluation kernel.  Row r of X is global row noise.row0 + r of the draw (noise.key, stream word noise.key.stream_lo +
+// *noise.stream_off) for an accumulator with noise (evok_eval_keyed), which then gets the noise the sampler gave the row;
+// `noise` is an empty struct for every other accumulator.
 template <typename Acc, bool VEC>
-__global__ void __launch_bounds__(kEvalThreads)
+__global__ void __launch_bounds__(kEvalThreads, NoiseTerms<Acc>::kEvalMinBlocks)
     eval_kernel(const float* __restrict__ X, int64_t ldx, int64_t n_rows, int64_t D, float* __restrict__ f,
-                const typename DataTerms<Acc>::Arg data) {
+                const typename DataTerms<Acc>::Arg data, const typename NoiseTerms<Acc>::EvalArg noise) {
   const int lane = threadIdx.x & 31;
+  const uint32_t sw = eval_stream_word<Acc>(noise);
   const int64_t warps_total = (int64_t)gridDim.x * (kEvalThreads / 32);
   const int64_t gw = (int64_t)blockIdx.x * (kEvalThreads / 32) + (threadIdx.x >> 5);
   using Cols4 = typename ColsOf<Acc, 4>::type;
@@ -753,6 +936,7 @@ __global__ void __launch_bounds__(kEvalThreads)
             const float v[4] = {g[k].x, g[k].y, g[k].z, g[k].w};
             Cols4 dc;
             dc.load4(acc, jk);
+            if constexpr (ElementDraws<Acc>::value) dc.draw4(noise.key, sw, noise.row0 + r, (uint32_t)(q + 32 * k));
             if constexpr (PairTerms<Acc>::value)
               if (jk > 0) dc.load_left(acc, jk);
             if constexpr (kFoldNow) {
@@ -770,6 +954,7 @@ __global__ void __launch_bounds__(kEvalThreads)
           Cols4 dc;
           if (active) {
             dc.load4(acc, ja);
+            if constexpr (ElementDraws<Acc>::value) dc.draw4(noise.key, sw, noise.row0 + r, (uint32_t)q);
             if constexpr (PairTerms<Acc>::value)
               if (ja > 0) dc.load_left(acc, ja);
             if constexpr (kFoldNow) {
@@ -786,6 +971,7 @@ __global__ void __launch_bounds__(kEvalThreads)
           Cols1 dc;
           if (active) {
             dc.load1(acc, j, 0);
+            if constexpr (ElementDraws<Acc>::value) dc.draw1(noise.key, sw, noise.row0 + r, j, 0);
             if constexpr (PairTerms<Acc>::value)
               if (j > 0) dc.load_left(acc, j);
             if constexpr (kFoldNow) fold(acc, v[0], j, dc, 0);
@@ -803,6 +989,11 @@ __global__ void __launch_bounds__(kEvalThreads)
         const int64_t ja = 4 * q, jb = 4 * (q + 32), jc = 4 * (q + 64), jd = 4 * (q + 96);
         Cols4 da, db, dc, dd;
         da.load4(acc, ja); db.load4(acc, jb); dc.load4(acc, jc); dd.load4(acc, jd);
+        if constexpr (ElementDraws<Acc>::value) {
+          const uint64_t row = noise.row0 + r;
+          da.draw4(noise.key, sw, row, (uint32_t)q); db.draw4(noise.key, sw, row, (uint32_t)(q + 32));
+          dc.draw4(noise.key, sw, row, (uint32_t)(q + 64)); dd.draw4(noise.key, sw, row, (uint32_t)(q + 96));
+        }
         fold(acc, a.x, ja, da, 0); fold(acc, a.y, ja + 1, da, 1); fold(acc, a.z, ja + 2, da, 2); fold(acc, a.w, ja + 3, da, 3);
         fold(acc, b.x, jb, db, 0); fold(acc, b.y, jb + 1, db, 1); fold(acc, b.z, jb + 2, db, 2); fold(acc, b.w, jb + 3, db, 3);
         fold(acc, c.x, jc, dc, 0); fold(acc, c.y, jc + 1, dc, 1); fold(acc, c.z, jc + 2, dc, 2); fold(acc, c.w, jc + 3, dc, 3);
@@ -813,16 +1004,18 @@ __global__ void __launch_bounds__(kEvalThreads)
         const int64_t ja = 4 * q;
         Cols4 da;
         da.load4(acc, ja);
+        if constexpr (ElementDraws<Acc>::value) da.draw4(noise.key, sw, noise.row0 + r, (uint32_t)q);
         fold(acc, a.x, ja, da, 0); fold(acc, a.y, ja + 1, da, 1); fold(acc, a.z, ja + 2, da, 2); fold(acc, a.w, ja + 3, da, 3);
       }
     } else {
       for (int64_t j = lane; j < D; j += 32) {
         Cols1 dc;
         dc.load1(acc, j, 0);
+        if constexpr (ElementDraws<Acc>::value) dc.draw1(noise.key, sw, noise.row0 + r, j, 0);
         fold(acc, ld_stream1(x + j), j, dc, 0);
       }
     }
-    const float v = acc.finish(D);
+    const float v = eval_finish(acc, D, noise, sw, r);
     if (lane == 0) f[r] = v;
   }
 }

@@ -268,6 +268,7 @@ extern "C" EVOK_API const char* evok_error_string(int code) {
     case EVOK_E_ALIGN: return "misaligned pointer";
     case EVOK_E_NOKERNEL: return "the cubin of the registered objective lacks one of its kernels";
     case EVOK_E_NODATA: return "the objective declares data: launch an instance of it (evok_objective_instance)";
+    case EVOK_E_NOISEKEY: return "the objective draws noise: evaluate it with the key of its rows (evok_eval_keyed)";
     default: return code > 0 ? cudaGetErrorString((cudaError_t)code) : "unknown error";
   }
 }

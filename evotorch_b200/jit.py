@@ -29,6 +29,13 @@ The expression language (anything else raises ValueError):
   - where(cond, a, b)  a conditional, CUDA (cond) ? a : b and torch.where; cond is one comparison < <= > >= == != of two
     expressions, and comparisons are allowed nowhere else.  As in IEEE arithmetic a comparison with NaN is false, except !=,
     which is true (CUDA and torch agree);
+  - noise      rand() (uniform on [0, 1)) and randn() (standard normal), each occurrence its own independent draw: one per
+    row and column in the element terms of sums, prods, maxs and mins, one per row in `value`, also inside where(...); not in a
+    pair term or a running term, and without arguments.  At most 4 occurrences in the element terms and 4 in `value`; each
+    element occurrence costs one Philox4x32-10 call per 4 columns and row.  The kernels draw from the Philox key of the
+    population's own draw (csrc/evok_sampler.cuh: noise_bits), the torch function with torch.rand / torch.randn: the same
+    distributions, not the same bits (as rng="torch").  Only a call draws: `rand` and `randn` remain usable as the names of
+    reductions, running sums and data;
   - constants  pi, e, numeric literals;
   - names      x (the element), xn (the next element x_{j+1}), j (the 0-based column of x) and D (the row length) in a
     term, and the running names in an element term of a reduction; the reduction names and D in `value`.
@@ -75,6 +82,8 @@ FUNCTIONS = {
     "floor": ("floorf", torch.floor), "minimum": ("fminf", torch.fmin), "maximum": ("fmaxf", torch.fmax),
 }
 CONSTANTS = {"pi": math.pi, "e": math.e}
+NOISE = {"rand": torch.rand, "randn": torch.randn}  # zero-argument functions: one independent draw per occurrence
+MAX_DRAWS = 4  # occurrences of rand() / randn() in the element terms, and again in `value`
 _ARITY = {"minimum": 2, "maximum": 2}
 _BINOPS = {ast.Add: "+", ast.Sub: "-", ast.Mult: "*", ast.Div: "/"}
 _COMPARE = {ast.Lt: ("<", torch.lt), ast.LtE: ("<=", torch.le), ast.Gt: (">", torch.gt), ast.GtE: (">=", torch.ge),
@@ -114,11 +123,12 @@ def _int_exponent(node) -> Optional[int]:
     return None
 
 
-def _translate(node, names: Dict[str, str], where: str) -> _Expr:
-    """names: the Python names allowed here -> their CUDA identifiers."""
+def _translate(node, names: Dict[str, str], where: str, draws: Optional["_Draws"] = None) -> _Expr:
+    """names: the Python names allowed here -> their CUDA identifiers; draws: where rand() / randn() here draw from (None: they
+    are refused here)."""
     allowed = _ALLOWED_TEXT.format(names=", ".join(names))
     if isinstance(node, ast.Expression):
-        return _translate(node.body, names, where)
+        return _translate(node.body, names, where, draws)
     if isinstance(node, ast.Constant):
         if type(node.value) not in (int, float):
             raise ValueError(f"{where}: the literal {node.value!r} is not a number; {allowed}")
@@ -132,14 +142,14 @@ def _translate(node, names: Dict[str, str], where: str) -> _Expr:
             return _Expr(_float_literal(v), lambda env, v=v: v)
         raise ValueError(f"{where}: unknown name {node.id!r}; {allowed}")
     if isinstance(node, ast.UnaryOp):
-        a = _translate(node.operand, names, where)
+        a = _translate(node.operand, names, where, draws)
         if isinstance(node.op, ast.USub):
             return _Expr(f"(-{a.cuda})", lambda env: -a.torch(env))
         if isinstance(node.op, ast.UAdd):
             return a
         raise ValueError(f"{where}: the operator {type(node.op).__name__} is not supported; {allowed}")
     if isinstance(node, ast.BinOp):
-        a = _translate(node.left, names, where)
+        a = _translate(node.left, names, where, draws)
         if isinstance(node.op, ast.Pow):
             n = _int_exponent(node.right)
             if n is not None:
@@ -147,15 +157,22 @@ def _translate(node, names: Dict[str, str], where: str) -> _Expr:
                     return _Expr("1.0f", lambda env: 1.0)
                 prod = "(" + " * ".join([a.cuda] * abs(n)) + ")"
                 return _Expr(prod if n > 0 else f"(1.0f / {prod})", lambda env: a.torch(env) ** n)
-            b = _translate(node.right, names, where)
+            b = _translate(node.right, names, where, draws)
             return _Expr(f"powf({a.cuda}, {b.cuda})", lambda env: torch.pow(_as_tensor(a.torch(env), env), b.torch(env)))
         if type(node.op) not in _BINOPS:
             raise ValueError(f"{where}: the operator {type(node.op).__name__} is not supported; {allowed}")
-        b = _translate(node.right, names, where)
+        b = _translate(node.right, names, where, draws)
         op = _BINOPS[type(node.op)]
         fn = {"+": lambda env: a.torch(env) + b.torch(env), "-": lambda env: a.torch(env) - b.torch(env),
               "*": lambda env: a.torch(env) * b.torch(env), "/": lambda env: a.torch(env) / b.torch(env)}[op]
         return _Expr(f"({a.cuda} {op} {b.cuda})", fn)
+    if isinstance(node, ast.Call) and isinstance(node.func, ast.Name) and node.func.id in NOISE:
+        if node.args or node.keywords:
+            raise ValueError(f"{where}: {node.func.id}() takes no arguments, got {ast.unparse(node)!r}")
+        if draws is None:
+            raise ValueError(f"{where}: {node.func.id}() draws noise, which is allowed in the element terms of sums, prods, maxs and mins "
+                             f"and in `value` only (not in a pair term or a running term)")
+        return draws.take(node.func.id, where)
     if isinstance(node, ast.Call) and isinstance(node.func, ast.Name) and node.func.id == "where":
         if node.keywords or len(node.args) != 3:
             raise ValueError(f"{where}: where takes 3 positional arguments (cond, a, b), got {ast.unparse(node)!r}")
@@ -164,8 +181,8 @@ def _translate(node, names: Dict[str, str], where: str) -> _Expr:
             raise ValueError(f"{where}: the condition of where must be one comparison < <= > >= == != of two expressions, got "
                              f"{ast.unparse(cond)!r}")
         op, top = _COMPARE[type(cond.ops[0])]
-        l, r = _translate(cond.left, names, where), _translate(cond.comparators[0], names, where)
-        a, b = _translate(node.args[1], names, where), _translate(node.args[2], names, where)
+        l, r = _translate(cond.left, names, where, draws), _translate(cond.comparators[0], names, where, draws)
+        a, b = _translate(node.args[1], names, where, draws), _translate(node.args[2], names, where, draws)
 
         def where_fn(env):
             lv, rv = _as_tensor(l.torch(env), env), _as_tensor(r.torch(env), env)
@@ -185,21 +202,41 @@ def _translate(node, names: Dict[str, str], where: str) -> _Expr:
         arity = _ARITY.get(name, 1)
         if len(node.args) != arity:
             raise ValueError(f"{where}: {name} takes {arity} argument(s), got {len(node.args)}")
-        args = [_translate(a, names, where) for a in node.args]
+        args = [_translate(a, names, where, draws) for a in node.args]
         cname, tfn = FUNCTIONS[name]
         return _Expr(f"{cname}(" + ", ".join(a.cuda for a in args) + ")",
                      lambda env: tfn(*[_as_tensor(a.torch(env), env) for a in args]))
     raise ValueError(f"{where}: {type(node).__name__} ({ast.unparse(node)!r}) is not supported; {allowed}")
 
 
-def _parse(text: str, names: Dict[str, str], where: str) -> _Expr:
+def _parse(text: str, names: Dict[str, str], where: str, draws: Optional["_Draws"] = None) -> _Expr:
     if not isinstance(text, str):
         raise ValueError(f"{where}: expected an expression string, got {type(text).__name__}")
     try:
         tree = ast.parse(text, mode="eval")
     except SyntaxError as e:
         raise ValueError(f"{where}: not a Python expression: {text!r} ({e.msg})") from None
-    return _translate(tree, names, where)
+    return _translate(tree, names, where, draws)
+
+
+class _Draws:
+    """The occurrences of rand() / randn() in one context (the element terms, or `value`), in source order: occurrence k is
+    `cuda(k, name)` in the CUDA source and a fresh torch.rand / torch.randn of the context's shape (env["_shape"]) in torch."""
+
+    def __init__(self, context: str, cuda: Callable[[int, str], str]):
+        self.context, self.cuda, self.normal = context, cuda, []
+
+    def take(self, name: str, where: str) -> _Expr:
+        if len(self.normal) >= MAX_DRAWS:
+            raise ValueError(f"{where}: at most {MAX_DRAWS} occurrences of rand() / randn() in {self.context}, got more")
+        k = len(self.normal)
+        self.normal.append(name == "randn")
+        fn = NOISE[name]
+        return _Expr(self.cuda(k, name), lambda env: fn(env["_shape"], dtype=env["_dtype"], device=env["_device"]))
+
+    @property
+    def normal_mask(self) -> int:
+        return sum(1 << k for k, n in enumerate(self.normal) if n)
 
 
 # the reductions in slot order, with their keyword, the identity their slot starts from and their warp butterfly
@@ -229,10 +266,13 @@ def data_kinds(data: dict) -> Dict[str, bool]:
 
 
 def _names_used(text) -> set:
+    """The names an expression reads (not the functions it calls: a reduction, running sum or data name may be `rand`)."""
     try:
-        return {n.id for n in ast.walk(ast.parse(text, mode="eval")) if isinstance(n, ast.Name)}
+        tree = ast.parse(text, mode="eval")
     except (SyntaxError, TypeError):
         return set()  # _parse reports it
+    called = {id(n.func) for n in ast.walk(tree) if isinstance(n, ast.Call)}
+    return {n.id for n in ast.walk(tree) if isinstance(n, ast.Name) and id(n) not in called}
 
 
 class ObjectiveSpec:
@@ -297,6 +337,11 @@ class ObjectiveSpec:
             if bad:
                 raise ValueError(f"running[{c!r}]: {sorted(bad)[0]!r}: a running term is an element term of x, j, D and data; "
                                  f"{allowed_where}")
+        # noise: element occurrences are the column entries d[kVectors + k] (after the data vectors'), occurrences in `value` the
+        # row's draws in finish (evok_sampler.cuh: DataCols::draw4, value_rand / value_randn)
+        n_vectors = sum(1 for v in self.kinds.values() if v)
+        self.element_draws = _Draws("the element terms", lambda k, name: f"d[{n_vectors + k}]")
+        self.value_draws = _Draws("`value`", lambda k, name: f"evok::value_{name}(key, sw, row, {MAX_DRAWS + k})")
         self.running_terms = {c: _parse(t, {k: v for k, v in term_names.items() if k != "xn"}, f"running[{c!r}]")
                               for c, t in running.items()}
         for c, e in self.running_terms.items():
@@ -314,14 +359,16 @@ class ObjectiveSpec:
         self._check_data_names(used, "value", term=False)
         if used & set(running):
             raise ValueError(f"value: {sorted(used & set(running))[0]!r} is a running sum; {allowed_where}")
-        self.terms = {s: _parse(t, run_names, f"{GROUP_OF[self.reductions[s]]}[{s!r}]") for s, t in texts.items()}
+        self.terms = {s: _parse(t, run_names, f"{GROUP_OF[self.reductions[s]]}[{s!r}]", None if "xn" in _names_used(t) else self.element_draws)
+                      for s, t in texts.items()}
         self.pairs = frozenset(s for s, e in self.terms.items() if re.search(r"\bxn\b", e.cuda))
         for s, e in self.terms.items():
             m = re.search(r"\bvn_(\w+)\b", e.cuda)
             if m and s not in self.pairs:
                 raise ValueError(f"{GROUP_OF[self.reductions[s]]}[{s!r}]: {m.group(1)}_n is the entry of {m.group(1)!r} at column j + 1, "
                                  f"which only a pair term (one that uses xn) has; an element term uses {m.group(1)!r}")
-        self.value_expr = _parse(value, value_names, "value")
+        self.value_expr = _parse(value, value_names, "value", self.value_draws)
+        self.noisy = bool(self.element_draws.normal or self.value_draws.normal)
         self.source = self._cuda_source()
 
     def _check_data_names(self, used: set, where: str, term: bool) -> None:
@@ -340,7 +387,8 @@ class ObjectiveSpec:
         nr = len(self.running_terms)
         # data: slot i of the binding is data name i; the vectors are numbered among themselves in the same order
         vectors = [n for n, v in self.kinds.items() if v]
-        nv = max(len(vectors), 1)
+        nd = len(self.element_draws.normal)
+        nv = max(len(vectors) + nd, 1)  # the column entries of a fold: data vectors, then element draws
 
         def entries(es, prefix, array):  # the locals of the vector entries that the terms `es` use
             return [f"    const float {prefix}_{n} = {array}[{i}];" for i, n in enumerate(vectors)
@@ -359,9 +407,13 @@ class ObjectiveSpec:
         if self.kinds:
             lines.append("  static constexpr bool kData = true;")
             lines.append(f"  static constexpr int kVectors = {len(vectors)};")
+        if self.noisy:
+            lines.append("  static constexpr bool kNoise = true;")
+            lines.append(f"  static constexpr int kDraws = {nd};")
+            lines.append(f"  static constexpr unsigned kNormalDraws = {self.element_draws.normal_mask}u;")
         lines.append("  float Df;")
         lines.append("  float " + ", ".join(f"s{i} = {IDENTITY[ops[i]]}" for i in k) + ";")
-        data_arg = f"const float (&d)[{nv}], " if self.kinds else ""
+        data_arg = f"const float (&d)[{nv}], " if self.kinds or nd else ""
         if self.kinds:
             slot = {n: i for i, n in enumerate(self.kinds)}
             lines.append(f"  const float* vec[{nv}];")
@@ -382,7 +434,7 @@ class ObjectiveSpec:
             lines += [f"    h[{i}] = {e.cuda};" for i, e in run]
             lines.append("  }")
             lines.append(f"  __device__ __forceinline__ void add(float x, int64_t j, {data_arg}const float (&r)[{nr}]) {{")
-        elif self.kinds:
+        elif data_arg:
             lines.append(f"  __device__ __forceinline__ void add(float x, int64_t j, const float (&d)[{nv}]) {{")
         else:
             lines.append("  __device__ __forceinline__ void add(float x, int64_t j) {")
@@ -392,7 +444,7 @@ class ObjectiveSpec:
         lines += [combine(i, e.cuda) for i, e in element]
         lines.append("  }")
         if pair:
-            if self.kinds:
+            if data_arg:
                 lines.append(f"  __device__ __forceinline__ void add_pair(float x, float xn, int64_t j, const float (&d)[{nv}], "
                              f"const float (&dn)[{nv}]) {{")
             else:
@@ -402,7 +454,10 @@ class ObjectiveSpec:
             lines += entries(pair, "v", "d") + entries(pair, "vn", "dn")
             lines += [combine(i, e.cuda) for i, e in pair]
             lines.append("  }")
-        lines.append("  __device__ __forceinline__ float finish(int64_t) {")
+        if self.noisy:
+            lines.append("  __device__ __forceinline__ float finish(int64_t, const evok::PhiloxKey& key, uint32_t sw, uint64_t row) {")
+        else:
+            lines.append("  __device__ __forceinline__ float finish(int64_t) {")
         lines += [f"    const float S_{s} = evok::{WARP_REDUCE[ops[i]]}(s{i});" for i, s in zip(k, self.terms)]
         lines.append(f"    return {self.value_expr.cuda};")
         lines += ["  }", "};", "}  // namespace evok_user", ""]
@@ -431,6 +486,7 @@ class ObjectiveSpec:
                     penv[f"{name}_n"] = t[..., 1:]
                 else:
                     venv[name] = t[..., 0]
+        env["_shape"] = rows + (D,)  # of an element draw (rand() / randn() in an element term): one per row and column
         for c, e in self.running_terms.items():  # c_j = sum_{k <= j} h(x_k, k, D)
             env[c] = torch.broadcast_to(_as_tensor(e.torch(env), env), rows + (D,)).cumsum(dim=-1)
         for s, e in self.terms.items():
@@ -446,7 +502,7 @@ class ObjectiveSpec:
                 venv[s] = torch.full(rows, -math.inf if op == "max" else math.inf, dtype=t.dtype, device=t.device)
             else:
                 venv[s] = t.amax(dim=-1) if op == "max" else t.amin(dim=-1)
-        venv.update(D=Dt, _dtype=X.dtype, _device=X.device)
+        venv.update(D=Dt, _dtype=X.dtype, _device=X.device, _shape=rows)
         return torch.broadcast_to(_as_tensor(self.value_expr.torch(venv), venv), rows)
 
 
@@ -662,6 +718,8 @@ def compile_objective(spec: ObjectiveSpec) -> CompiledObjective:
             c.objective_id = register(c.cubin, c.names)
             if spec.kinds:
                 declare_data(c.objective_id, spec.kinds)
+            if spec.noisy:
+                nat.check(nat.lib().evok_objective_declare_noise(c.objective_id), "evok_objective_declare_noise")
             _cache[spec.source] = c
         return c
 

@@ -101,7 +101,18 @@ class FusedObjective(BuiltinObjective):
     in a batched search (`pgpe_ask_and_evaluate`, `cem_ask_and_evaluate`) every item then has its own data.  All data tensors
     with batch dimensions have the same batch shape, which is the batch shape of the search (the centre and stdev are broadcast
     to it); a tensor without batch dimensions is shared by all items.  A FusedObjective with data pickles with its tensors.  In a
-    multi-GPU run every rank builds its own objective: the tensors must hold the same values on every rank."""
+    multi-GPU run every rank builds its own objective: the tensors must hold the same values on every rank.
+
+    `rand()` and `randn()` draw noise (`noisy` is then True): at most 4 occurrences in the element terms (one draw per row and
+    column each) and 4 in `value` (one per row), not in pair or running terms:
+
+        f7 = FusedObjective("f7", sums={"s": "(j + 1) * x**4"}, value="s + rand()")
+        input_noise_sphere = FusedObjective("ins", sums={"s": "(x + 0.1 * randn())**2"}, value="s")
+
+    The noise comes from the Philox key of the population's draw, so it is the same whether the population is stored or lazy,
+    stepped or replayed from a CUDA graph, sharded or batched.  Rows without a draw of their own (`obj(X)`, user-set values)
+    take a fresh key; on CPU tensors and other dtypes the torch function draws with torch.rand / torch.randn (the same
+    distributions, not the same bits)."""
 
     def __init__(self, name: str, sums: Optional[dict] = None, value: Optional[str] = None, data: Optional[dict] = None, *,
                  prods: Optional[dict] = None, maxs: Optional[dict] = None, mins: Optional[dict] = None, running: Optional[dict] = None):
@@ -119,6 +130,7 @@ class FusedObjective(BuiltinObjective):
         self.prods, self.maxs, self.mins, self.running = dict(spec.prods), dict(spec.maxs), dict(spec.mins), dict(spec.running)
         self.kernel_info = compiled.kernel_info
         self.batched_kernel_info = None
+        self.noisy = spec.noisy
         self._spec = spec
         if self.data:
             self._bind(compiled.objective_id)
@@ -162,7 +174,21 @@ class FusedObjective(BuiltinObjective):
         # the evaluation kernel takes one data set: per-item data, and data that is not on a CUDA device, go through torch_fn
         if self.data and (self.evok_objective_id is None or self.data_batch_shape):
             return self._torch_fn(x.unsqueeze(0))[..., 0] if x.ndim == 1 else self._torch_fn(x)
+        if self.takes_key(x):  # rows without a draw of their own: a fresh key from torch's generator
+            from .algorithms.functional.misc import draw_philox_seed
+
+            return ops.evaluate_keyed(self.evok_objective_id, x, seed=draw_philox_seed(), stream_id=0)
         return super().__call__(x)
+
+    def takes_key(self, x: torch.Tensor) -> bool:
+        """True when the kernels evaluate the rows of x and the objective draws noise: then `evaluate_keyed` applies."""
+        return (self.noisy and self.evok_objective_id is not None and not self.data_batch_shape and ops.uses_kernels(x) and x.ndim == 2
+                and x.stride(1) == 1)
+
+    def evaluate_keyed(self, x: torch.Tensor, draw) -> torch.Tensor:
+        """The fitnesses of the rows of x (CUDA float32, `takes_key`), whose noise comes from `draw` (a `PhiloxDraw`): row i is
+        global row draw.row0 + i of it, so a row the fused sampler drew with `draw` gets the fitness the sampler gave it."""
+        return ops.evaluate_keyed(self.evok_objective_id, x, **draw.kwargs)
 
     def with_data(self, **tensors) -> "FusedObjective":
         """A twin of this objective on other tensors (all of its data names, of the same kinds): no recompile."""

@@ -240,6 +240,24 @@ def evaluate(objective: int, X: torch.Tensor, f: Optional[torch.Tensor] = None) 
     return f
 
 
+def evaluate_keyed(objective: int, X: torch.Tensor, *, seed: int, stream_id: int, row0: int = 0,
+                   stream_offset: Optional[torch.Tensor] = None, f: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """`evaluate` with the Philox draw of the rows (the keyword arguments of a `PhiloxDraw`): row i of X is global row row0 + i
+    of the draw, so an objective with noise gives each row the noise the fused sampler gives it with the same draw.  For an
+    objective without noise it is `evaluate`."""
+    _mat(X, "X")
+    n, D = X.shape
+    if f is None:
+        f = torch.empty(n, dtype=torch.float32, device=X.device)
+    _vec(f, "f", n)
+    _load_objective(objective, X)
+    with _timed("eval"):
+        rc = nat.lib().evok_eval_keyed(objective, X.data_ptr(), X.stride(0), row0, n, D, seed, stream_id, _offset_ptr(stream_offset),
+                                       f.data_ptr(), nat.stream_of(X))
+    nat.check(rc, "evok_eval_keyed")
+    return f
+
+
 # ------------------------------------------------------------------------------------------------ K3
 def _rank_ws(device: torch.device, n: int) -> torch.Tensor:
     return nat.workspace(device, nat.lib().evok_rank_workspace_bytes(n), "rank")

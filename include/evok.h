@@ -45,6 +45,7 @@ extern "C" {
 #define EVOK_E_ALIGN (-6)
 #define EVOK_E_NOKERNEL (-7) /* the cubin of a registered objective lacks one of its EVOK_OBJ_KERNELS kernels */
 #define EVOK_E_NODATA (-8)   /* a registered objective that declares data was launched by its own id, not by an instance's */
+#define EVOK_E_NOISEKEY (-9) /* evok_eval of an objective that draws noise: evaluate it with a key (evok_eval_keyed) */
 
 #define EVOK_MAX_PEERS 16 /* GPUs of one NVLink domain that can take part in a peer exchange */
 
@@ -105,6 +106,15 @@ int evok_sample_eval(int objective, float* X, int64_t ldx, const float* mu, cons
  * CMA-ES / XNES populations).  Replaces the user's vectorised torch objective at core.py:2604. */
 int evok_eval(int objective, const float* X, int64_t ldx, int64_t n_rows, int64_t D, float* f, void* stream);
 
+/* K2 with the Philox draw of the rows: row i of X is global row (row0 + i) of the draw (seed, stream_id, stream_offset_dev as in
+ * evok_sample_eval).  An objective whose expressions draw noise (evok_objective_declare_noise) takes its rand() / randn() from
+ * that draw, so a row that evok_sample_eval sampled with the same arguments gets the same fitness bit for bit on the vectorised
+ * path; evok_eval refuses such an objective (EVOK_E_NOISEKEY) and launches nothing, rather than evaluate it with a fixed key.
+ * For an objective without noise it is evok_eval: the same kernel and the same bits.  Errors: those of evok_eval, and
+ * EVOK_E_BADSIZE for row0 < 0. */
+int evok_eval_keyed(int objective, const float* X, int64_t ldx, int64_t row0, int64_t n_rows, int64_t D, uint64_t seed, uint64_t stream_id,
+                    const uint32_t* stream_offset_dev, float* f, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Objectives defined at run time (evotorch_b200/jit.py compiles them with NVRTC from csrc/evok_sampler.cuh).
  * evok_objective_register takes an sm_90a cubin and the lowered names of its EVOK_OBJ_KERNELS kernels, in this order:
@@ -144,6 +154,14 @@ int evok_objective_load(int objective);
 #define EVOK_OBJ_KERNEL_BATCHED 22
 #define EVOK_OBJ_BATCHED_KERNELS 8
 int evok_objective_register_batched(int objective, const void* cubin, size_t bytes, const char* const* kernel_names_host, int n_kernels);
+
+/* Objectives with noise.  The accumulator of a registered objective may draw uniform and normal noise from the Philox key of
+ * the population it evaluates (kNoise in csrc/evok_sampler.cuh); its eval_kernel<Acc, vec> then takes the draw of the rows as
+ * its last argument.  evok_objective_declare_noise tells the library so, right after
+ * evok_objective_register: from then on evok_eval refuses the id (and its instances) with EVOK_E_NOISEKEY and evok_eval_keyed
+ * passes the key.  The samplers need nothing more: they draw the noise from the key they sample with.
+ * Errors: EVOK_E_BADENUM (`objective` is not a registered id). */
+int evok_objective_declare_noise(int objective);
 
 /* Objectives with data.  The accumulator of a registered objective may read up to EVOK_MAX_DATA float32 device arrays (kData in
  * csrc/evok_sampler.cuh): vectors with one entry per column of a row, and scalars.  Which name is which is part of its source;
