@@ -249,26 +249,25 @@ __device__ __forceinline__ void st_stream1(float* p, float a) {
 // A row's elements reach add() in no fixed column order (strided over the lanes of a warp), so an accumulator holds
 // reductions with an associative combine: sums, and in a generated one also products, maxima and minima (warp_prod / _max /
 // _min), each slot starting from its combine's identity.
-// A generated accumulator may also have pair terms (`static constexpr bool kPairs = true`, see PairTerms below):
-//   add_pair(x, xn, j) : fold the neighbour pair (x_j, x_{j+1}); it is called exactly once for every j in [0, D-2] of a row,
-//                        by the lane that holds column j+1, also in no fixed order across lanes (fold_pairs).
-// A generated accumulator may also refer to data (`static constexpr bool kData = true`, see DataTerms below): float32
-// vectors of the row length and scalars, bound per launch.  It is then constructed as Acc(D, binding), declares
-// `static constexpr int kVectors` and `const float* vec[]` (the vectors of this launch's item), loads its scalars once in the
-// constructor, and takes the vectors' entries with every fold:
-//   add(x, j, d)                  : d[i] = vec[i][j];
-//   add_pair(x, xn, j, d, dn)     : d[i] = vec[i][j], dn[i] = vec[i][j + 1].
-// A generated accumulator may also have running sums c_j = sum_{k<=j} h(x_k, k) (`static constexpr bool kRunning = true` and
-// `static constexpr int kRunningSums` = R <= 2, see RunningTerms below).  Its element terms then see the running sums at their
-// column, so add() takes them, after the data entries of an accumulator with data:
-//   running(x, j[, d], h)  : h[i] = the increment of running sum i at column j;
-//   add(x, j[, d], r)      : fold element x of column j, where r[i] = c_j of running sum i (fold_running computes it).
-// A generated accumulator may also draw noise (`static constexpr bool kNoise = true`, see NoiseTerms below): kDraws <= 4
-// occurrences of rand() / randn() in its element terms (bit k of kNormalDraws: occurrence k is randn()) and up to 4 in `value`.
-// Its element draws at column j reach add() (and running() / add_pair(), which do not use them) as the entries d[kVectors + k]
-// after the data entries, loaded next to them (DataCols::draw4 / draw1), and its finish takes the draw of its row:
-//   finish(D, key, stream_word, row) : row = the global row index; `value` draws with value_rand / value_randn.
-// The built-in ones are ObjAcc<EVOK_OBJ_*>; a user-defined one is generated by evotorch_b200/jit.py.
+// The built-in ones are ObjAcc<EVOK_OBJ_*>; a user-defined one is generated by evotorch_b200/jit.py and may declare optional
+// markers, each of which adds calls or arguments:
+//   kPairs = true (pair terms):
+//     add_pair(x, xn, j)  : fold the neighbour pair (x_j, x_{j+1}); it is called exactly once for every j in [0, D-2] of a
+//                           row, by the lane that holds column j+1, also in no fixed order across lanes (fold_pairs).
+//   kRunning = true, kRunningSums = R <= 2 (running sums c_j = sum_{k<=j} h(x_k, k)):
+//     running(x, j, h)    : h[i] = the increment of running sum i at column j;
+//     add(x, j, r)        : the element fold takes r last, r[i] = c_j of running sum i (fold_running computes it).
+//   kData = true, kVectors (data: float32 vectors of the row length and scalars, bound per launch):
+//     Acc(D, binding)     : the constructor takes the DataBinding of the launch's item, keeps `const float* vec[]` (the vectors)
+//                           and loads the scalars.
+//   kNoise = true, kDraws <= 4, kNormalDraws (rand() / randn(): kDraws occurrences in the element terms, bit k of kNormalDraws
+//   set where occurrence k is randn(), and up to 4 in `value`):
+//     finish(D, key, stream_word, row) : row = the global row index; `value` draws with value_rand / value_randn.
+// An accumulator with data vectors or element draws takes the column entries of a fold after j (DataCols: d[i] = vec[i][j],
+// then d[kVectors + k] = element draw k at column j), in every fold, whether its terms use them or not:
+//   add(x, j, d[, r]),  running(x, j, d, h),  add_pair(x, xn, j, d, dn)  with dn the entries at column j + 1.
+// AccTraits reads the markers, and the acc_* functions below are the only calls into an accumulator: the kernels hand every
+// fold the column entries, every finish the row's draw, and never depend on which of these signatures an accumulator has.
 // ------------------------------------------------------------------------------------------------
 template <int OBJ>
 struct ObjAcc;
@@ -314,54 +313,6 @@ struct ObjAcc<EVOK_OBJ_ACKLEY> {
   }
 };
 
-// true only for ObjAcc<EVOK_OBJ_NONE> (sample without evaluating)
-template <typename Acc>
-struct SampleOnly {
-  static constexpr bool value = false;
-};
-template <>
-struct SampleOnly<ObjAcc<EVOK_OBJ_NONE>> {
-  static constexpr bool value = true;
-};
-
-// true for an accumulator that declares `static constexpr bool kPairs = true` (a generated one whose terms use x_{j+1});
-// false for every ObjAcc<> and every accumulator without the marker.  All pair code is under `if constexpr` on it.
-template <typename Acc, typename = void>
-struct PairTerms {
-  static constexpr bool value = false;
-};
-template <typename Acc>
-struct PairTerms<Acc, decltype(void(Acc::kPairs))> {
-  static constexpr bool value = Acc::kPairs;
-};
-
-// true for an accumulator that declares `static constexpr bool kRunning = true` (a generated one with running sums; kSums of
-// them); all running-sum code is under `if constexpr` on it
-template <typename Acc, typename = void>
-struct RunningTerms {
-  static constexpr bool value = false;
-  static constexpr int kSums = 1;
-};
-template <typename Acc>
-struct RunningTerms<Acc, decltype(void(Acc::kRunning))> {
-  static constexpr bool value = Acc::kRunning;
-  static constexpr int kSums = Acc::kRunningSums;
-};
-
-// an accumulator whose kernels take warp-uniform steps of 32 lanes (pair folds and running sums shuffle across lanes)
-template <typename Acc>
-struct WarpSteps {
-  static constexpr bool value = PairTerms<Acc>::value || RunningTerms<Acc>::value;
-};
-
-// the carries of one row along warp-uniform steps: the last column of the previous step (pair terms) and the running sums of
-// all columns of the previous steps
-template <typename Acc>
-struct StepCarry {
-  float pair = 0.f;
-  float run[RunningTerms<Acc>::kSums] = {};
-};
-
 // The data of one launch of an objective with data terms: p[i] is data name i of the launch's first item and item_stride[i]
 // the distance in floats to the next item's (0: shared by all items; only the batched sampler has more than one item).  It is
 // a kernel argument, so two objectives of one source in flight on two streams, or captured in two graphs, never share it.
@@ -371,19 +322,6 @@ struct DataBinding {
 };
 struct NoData {};
 
-// true for an accumulator that declares `static constexpr bool kData = true`; Arg is the last argument of its kernels (an
-// empty struct for every other accumulator, whose kernels are otherwise untouched: all data code is under `if constexpr`)
-template <typename Acc, typename = void>
-struct DataTerms {
-  static constexpr bool value = false;
-  using Arg = NoData;
-};
-template <typename Acc>
-struct DataTerms<Acc, decltype(void(Acc::kData))> {
-  static constexpr bool value = Acc::kData;
-  using Arg = DataBinding;
-};
-
 // The draw of the rows that eval_kernel evaluates, its last argument for an accumulator with noise: row r of X is global row
 // row0 + r, on stream word key.stream_lo + *stream_off (stream_off may be null)
 struct EvalKey {
@@ -392,56 +330,123 @@ struct EvalKey {
   int64_t row0;
 };
 
-// true for an accumulator that declares `static constexpr bool kNoise = true` (a generated one with rand() / randn()); kDraws
-// of its occurrences are in the element terms, kNormal has bit k set for a randn() among them.  All noise code is under
-// `if constexpr` on it.
-template <typename Acc, typename = void>
-struct NoiseTerms {
-  static constexpr bool value = false;
-  static constexpr int kDraws = 0;
-  static constexpr unsigned kNormal = 0;
-  using EvalArg = NoData;
-  static constexpr int kEvalMinBlocks = 0;  // eval_kernel's launch bounds: none beyond the block size
+// tunables (build-time, for measurement builds: scripts/build_variants.py, scripts/kbench.py)
+#ifndef EVOK_SAMPLE_THREADS
+#define EVOK_SAMPLE_THREADS 256
+#endif
+#ifndef EVOK_SAMPLE_MINB
+#define EVOK_SAMPLE_MINB 3
+#endif
+#ifndef EVOK_SAMPLE_UNR
+#define EVOK_SAMPLE_UNR 2
+#endif
+#ifndef EVOK_SAMPLEONLY_MINB
+#define EVOK_SAMPLEONLY_MINB 5
+#endif
+#ifndef EVOK_SAMPLEONLY_UNR
+#define EVOK_SAMPLEONLY_UNR 1
+#endif
+
+// One optional marker of an accumulator: whether it is declared (and true), and the counts declared with it.  Every marker is
+// read with one idiom: the first overload exists only when Acc declares the marker, and the argument 0 prefers its int
+// parameter to the second overload's long.
+struct Marker {
+  bool on = false;
+  int n = 0;
+  unsigned mask = 0u;
 };
-template <typename Acc>
-struct NoiseTerms<Acc, decltype(void(Acc::kNoise))> {
-  static constexpr bool value = Acc::kNoise;
-  static constexpr int kDraws = Acc::kDraws;
-  static constexpr unsigned kNormal = Acc::kNormalDraws;
-  using EvalArg = EvalKey;
-  // 2 CTAs per SM: without a bound ptxas fits the kernel of a `value` draw with few element terms into 32 registers and spills
-  static constexpr int kEvalMinBlocks = 2;
+template <typename A> constexpr auto pairs_marker(int) -> decltype(Marker{A::kPairs}) { return {A::kPairs}; }
+template <typename A> constexpr Marker pairs_marker(long) { return {}; }
+template <typename A> constexpr auto running_marker(int) -> decltype(Marker{A::kRunning}) { return {A::kRunning, A::kRunningSums}; }
+template <typename A> constexpr Marker running_marker(long) { return {}; }
+template <typename A> constexpr auto data_marker(int) -> decltype(Marker{A::kData}) { return {A::kData, A::kVectors}; }
+template <typename A> constexpr Marker data_marker(long) { return {}; }
+template <typename A> constexpr auto noise_marker(int) -> decltype(Marker{A::kNoise}) { return {A::kNoise, A::kDraws, A::kNormalDraws}; }
+template <typename A> constexpr Marker noise_marker(long) { return {}; }
+// ObjAcc<EVOK_OBJ_NONE> samples without evaluating
+template <typename A> constexpr bool sample_only(const A*) { return false; }
+constexpr bool sample_only(const ObjAcc<EVOK_OBJ_NONE>*) { return true; }
+
+template <bool B, typename T, typename F>
+struct Pick {
+  using type = F;
+};
+template <typename T, typename F>
+struct Pick<true, T, F> {
+  using type = T;
 };
 
-// the data vectors of an accumulator (0 without data terms)
-template <typename Acc, bool = DataTerms<Acc>::value>
-struct DataVectors {
-  static constexpr int value = 0;
-};
+// Every compile-time fact about an accumulator that the kernels use.  Each feature's code is under `if constexpr` on its
+// fact, so the kernels of an accumulator without it are those of one written without the feature.
 template <typename Acc>
-struct DataVectors<Acc, true> {
-  static constexpr int value = Acc::kVectors;
+struct AccTraits {
+  static constexpr Marker kPairMark = pairs_marker<Acc>(0), kRunMark = running_marker<Acc>(0), kDataMark = data_marker<Acc>(0),
+                          kNoiseMark = noise_marker<Acc>(0);
+  static constexpr bool kSampleOnly = sample_only(static_cast<const Acc*>(nullptr));
+  static constexpr bool kPairs = kPairMark.on;
+  static constexpr bool kRunning = kRunMark.on;
+  static constexpr int kRunningSums = kRunning ? kRunMark.n : 0;
+  static constexpr bool kData = kDataMark.on;
+  static constexpr int kVectors = kData ? kDataMark.n : 0;
+  static constexpr bool kNoise = kNoiseMark.on;
+  static constexpr int kDraws = kNoise ? kNoiseMark.n : 0;  // element draws (those of `value` are the accumulator's own)
+  static constexpr unsigned kNormal = kNoise ? kNoiseMark.mask : 0u;
+  // element draws: the + and - rows of a direction fold with their own column entries
+  static constexpr bool kElementDraws = kDraws > 0;
+  // the folds take column entries (data vectors, then element draws), kSlots of them per column
+  static constexpr bool kCols = kData || kElementDraws;
+  static constexpr int kSlots = kVectors + kDraws > 0 ? kVectors + kDraws : 1;
+  // the kernels take warp-uniform steps of 32 lanes (pair folds and running sums shuffle across lanes)
+  static constexpr bool kWarpSteps = kPairs || kRunning;
+  // Launch bounds.  The fused samplers are issue/XU bound (two independent Philox chains per lane help); the sample-only kernel
+  // is store bound and prefers occupancy.  Running sums, and more than one element draw per column, run one Philox chain per
+  // lane, the latter at 2 CTAs per SM, so that no kernel spills.  eval_kernel of an accumulator with noise has 2 CTAs per SM:
+  // without a bound ptxas fits the kernel of a `value` draw with few element terms into 32 registers and spills.
+  static constexpr int kSampleUnroll = kSampleOnly ? EVOK_SAMPLEONLY_UNR : kRunning || kDraws > 1 ? 1 : EVOK_SAMPLE_UNR;
+  static constexpr int kSampleMinBlocks = kSampleOnly ? EVOK_SAMPLEONLY_MINB : kDraws > 1 ? 2 : EVOK_SAMPLE_MINB;
+  static constexpr int kEvalMinBlocks = kNoise ? 2 : 0;
+  // the last argument of the sampling kernels, and of eval_kernel (empty structs for an accumulator without data / noise)
+  using DataArg = typename Pick<kData, DataBinding, NoData>::type;
+  using EvalArg = typename Pick<kNoise, EvalKey, NoData>::type;
 };
 
-// an accumulator whose folds take per-column entries (data vectors, element draws): add / add_pair / running get the d arrays
+// The accumulator calls.  d / dn are the column entries of a fold (a row of DataCols), r / h the running sums and their
+// increments, (key, sw, row) the draw of the row; each function passes on what the accumulator's signature takes.
+template <typename Acc, typename Arg>
+__device__ __forceinline__ Acc acc_make(int64_t D, const Arg& data) {
+  if constexpr (AccTraits<Acc>::kData) return Acc(D, data);
+  else return Acc(D);
+}
+template <typename Acc, typename... Run>
+__device__ __forceinline__ void acc_add(Acc& acc, float x, int64_t j, const float (&d)[AccTraits<Acc>::kSlots], const Run&... r) {
+  if constexpr (AccTraits<Acc>::kCols) acc.add(x, j, d, r...);
+  else acc.add(x, j, r...);
+}
 template <typename Acc>
-struct ColTerms {
-  static constexpr bool value = DataTerms<Acc>::value || NoiseTerms<Acc>::kDraws > 0;
-  static constexpr int kVectors = DataVectors<Acc>::value;
-};
-
-// acc.finish of the row with global index `row`: an accumulator with noise draws its `value` occurrences from (key, sw, row)
+__device__ __forceinline__ void acc_pair(Acc& acc, float x, float xn, int64_t j, const float (&d)[AccTraits<Acc>::kSlots],
+                                         const float (&dn)[AccTraits<Acc>::kSlots]) {
+  if constexpr (AccTraits<Acc>::kCols) acc.add_pair(x, xn, j, d, dn);
+  else acc.add_pair(x, xn, j);
+}
+template <typename Acc, int R>
+__device__ __forceinline__ void acc_running(Acc& acc, float x, int64_t j, const float (&d)[AccTraits<Acc>::kSlots], float (&h)[R]) {
+  if constexpr (AccTraits<Acc>::kCols) acc.running(x, j, d, h);
+  else acc.running(x, j, h);
+}
+// key: null for an accumulator without noise (eval_kernel has no draw then)
 template <typename Acc>
-__device__ __forceinline__ float finish_row(Acc& acc, int64_t D, const PhiloxKey& key, uint32_t sw, uint64_t row) {
-  if constexpr (NoiseTerms<Acc>::value) return acc.finish(D, key, sw, row);
+__device__ __forceinline__ float acc_finish(Acc& acc, int64_t D, const PhiloxKey* key, uint32_t sw, uint64_t row) {
+  if constexpr (AccTraits<Acc>::kNoise) return acc.finish(D, *key, sw, row);
   else return acc.finish(D);
 }
 
-template <typename Acc, typename Arg>
-__device__ __forceinline__ Acc make_acc(int64_t D, const Arg& data) {
-  if constexpr (DataTerms<Acc>::value) return Acc(D, data);
-  else return Acc(D);
-}
+// the carries of one row along warp-uniform steps: the last column of the previous step (pair terms) and the running sums of
+// all columns of the previous steps
+template <typename Acc>
+struct StepCarry {
+  float pair = 0.f;
+  float run[AccTraits<Acc>::kRunningSums > 0 ? AccTraits<Acc>::kRunningSums : 1] = {};
+};
 
 __device__ __forceinline__ NoData item_data(const NoData& d, int64_t) { return d; }
 __device__ __forceinline__ DataBinding item_data(DataBinding d, int64_t item) {
@@ -450,19 +455,19 @@ __device__ __forceinline__ DataBinding item_data(DataBinding d, int64_t item) {
   return d;
 }
 
-// The data vectors' entries at the N columns a lane holds in one step: v[c][i] = vec[i][column c of the step], read through
-// the read-only cache (a D-vector is re-read by every row, so it stays in L1 / L2).  One load serves the + and the - row of a
-// symmetric pair.  `left` is the entry at the column before the first (the left neighbour of a pair fold across lanes).
+// The column entries of the N columns a lane holds in one step: v[c] = the entries of column c of the step, the data vectors'
+// vec[i][column] read through the read-only cache (a D-vector is re-read by every row, so it stays in L1 / L2), then the element
+// draws.  One load serves the + and the - row of a symmetric pair.  `left` holds the data entries at the column before the
+// first (the left neighbour of a pair fold across lanes).  Without data vectors and element draws nothing is loaded or drawn.
 template <typename Acc, int N>
 struct DataCols {
-  static constexpr int kVectors = ColTerms<Acc>::kVectors, kDraws = NoiseTerms<Acc>::kDraws;
-  static constexpr int kSlots = kVectors + kDraws > 0 ? kVectors + kDraws : 1;
-  float v[N][kSlots], left[kSlots];
+  static constexpr int kVectors = AccTraits<Acc>::kVectors, kDraws = AccTraits<Acc>::kDraws;
+  float v[N][AccTraits<Acc>::kSlots], left[AccTraits<Acc>::kSlots];
   // columns j .. j + 3 with one 16-byte load per vector: the vectorised kernels, which the host picks only when every vector is
   // 16-byte aligned (choose_kernel)
   __device__ __forceinline__ void load4(const Acc& acc, int64_t j) {
     static_assert(N == 4, "a column group is 4 columns");
-    if constexpr (kVectors > 0)  // an accumulator with element draws and no data has no `vec`
+    if constexpr (kVectors > 0)  // an accumulator without data vectors has no `vec`
 #pragma unroll
     for (int i = 0; i < kVectors; ++i) {
       const float4 t = __ldg(reinterpret_cast<const float4*>(acc.vec[i] + j));
@@ -485,40 +490,15 @@ struct DataCols {
 #pragma unroll
     for (int k = 0; k < kDraws; ++k) {
       float u[4];
-      noise4(key, sw, row, q, k, (NoiseTerms<Acc>::kNormal >> k) & 1u, u);
+      noise4(key, sw, row, q, k, (AccTraits<Acc>::kNormal >> k) & 1u, u);
       v[0][kVectors + k] = u[0]; v[1][kVectors + k] = u[1]; v[2][kVectors + k] = u[2]; v[3][kVectors + k] = u[3];
     }
   }
   __device__ __forceinline__ void draw1(const PhiloxKey& key, uint32_t sw, uint64_t row, int64_t j, int c) {  // column j into slot c
 #pragma unroll
-    for (int k = 0; k < kDraws; ++k) v[c][kVectors + k] = noise1(key, sw, row, j, k, (NoiseTerms<Acc>::kNormal >> k) & 1u);
+    for (int k = 0; k < kDraws; ++k) v[c][kVectors + k] = noise1(key, sw, row, j, k, (AccTraits<Acc>::kNormal >> k) & 1u);
   }
 };
-struct NoCols {
-  template <typename Acc> __device__ __forceinline__ void load4(const Acc&, int64_t) {}
-  template <typename Acc> __device__ __forceinline__ void load1(const Acc&, int64_t, int) {}
-  template <typename Acc> __device__ __forceinline__ void load_left(const Acc&, int64_t) {}
-};
-// true when the element terms draw noise: the + and - rows of a direction then fold with their own column entries
-template <typename Acc>
-struct ElementDraws {
-  static constexpr bool value = NoiseTerms<Acc>::kDraws > 0;
-};
-template <typename Acc, int N, bool = ColTerms<Acc>::value>
-struct ColsOf {
-  using type = NoCols;
-};
-template <typename Acc, int N>
-struct ColsOf<Acc, N, true> {
-  using type = DataCols<Acc, N>;
-};
-
-// acc.add of element x of column j, which is slot c of dc
-template <typename Acc, typename Cols>
-__device__ __forceinline__ void fold(Acc& acc, float x, int64_t j, const Cols& dc, int c) {
-  if constexpr (ColTerms<Acc>::value) acc.add(x, j, dc.v[c]);
-  else acc.add(x, j);
-}
 
 // One warp step of pair folds: this lane holds the N consecutive columns j .. j+N-1 of a row (v[]), of which the first
 // n_valid exist (0 for a lane past the row's end).  The lane holding column c + 1 folds (x_c, x_{c+1}): inside v[] from
@@ -526,23 +506,17 @@ __device__ __forceinline__ void fold(Acc& acc, float x, int64_t j, const Cols& d
 // held in the previous step of the same row (`carry`, zero-initialised per row and advanced here).  Every lane of the warp
 // must call it on every step, in the same order (it shuffles); a column's left neighbour is always in the previous lane
 // or the previous step because each step covers 32 * N consecutive columns.
-// dc: the data of the same columns (with `left` loaded when j > 0) for an accumulator with data terms.
-template <int N, typename Acc, typename Cols>
-__device__ __forceinline__ void fold_pairs(Acc& acc, const float (&v)[N], int64_t j, int n_valid, float& carry, const Cols& dc) {
+// dc: the column entries of the same columns (with `left` loaded when j > 0).
+template <int N, typename Acc>
+__device__ __forceinline__ void fold_pairs(Acc& acc, const float (&v)[N], int64_t j, int n_valid, float& carry, const DataCols<Acc, N>& dc) {
   const int lane = threadIdx.x & 31;
   const float rot = __shfl_sync(0xffffffffu, v[N - 1], (lane + 31) & 31);  // lane 0 receives lane 31's: next step's carry
   const float left = lane == 0 ? carry : rot;
   carry = rot;
-  if (n_valid > 0 && j > 0) {
-    if constexpr (ColTerms<Acc>::value) acc.add_pair(left, v[0], j - 1, dc.left, dc.v[0]);
-    else acc.add_pair(left, v[0], j - 1);
-  }
+  if (n_valid > 0 && j > 0) acc_pair(acc, left, v[0], j - 1, dc.left, dc.v[0]);
 #pragma unroll
   for (int c = 1; c < N; ++c)
-    if (c < n_valid) {
-      if constexpr (ColTerms<Acc>::value) acc.add_pair(v[c - 1], v[c], j + c - 1, dc.v[c - 1], dc.v[c]);
-      else acc.add_pair(v[c - 1], v[c], j + c - 1);
-    }
+    if (c < n_valid) acc_pair(acc, v[c - 1], v[c], j + c - 1, dc.v[c - 1], dc.v[c]);
 }
 
 // One warp step of the element folds of an accumulator with running sums, in the layout of fold_pairs (this lane holds the
@@ -551,10 +525,8 @@ __device__ __forceinline__ void fold_pairs(Acc& acc, const float (&v)[N], int64_
 // p_c, and takes the exclusive scan e of the lane totals p_{N-1} across the warp (a Kogge-Stone scan with __shfl_up_sync, five
 // rounds, then one shift); then c_{j+c} = p_c + (e + carry), where carry is the sum of all earlier steps of the row, and the
 // carry advances by the step total, the inclusive scan of lane 31.  Then each column's element terms are folded with its c.
-template <int N, typename Acc, typename Cols>
-__device__ __forceinline__ void fold_running(Acc& acc, const float (&v)[N], int64_t j, int n_valid, float (&carry)[RunningTerms<Acc>::kSums],
-                                             const Cols& dc) {
-  constexpr int R = RunningTerms<Acc>::kSums;
+template <int N, typename Acc, int R>
+__device__ __forceinline__ void fold_running(Acc& acc, const float (&v)[N], int64_t j, int n_valid, float (&carry)[R], const DataCols<Acc, N>& dc) {
   const int lane = threadIdx.x & 31;
   float p[N][R];
 #pragma unroll
@@ -562,10 +534,7 @@ __device__ __forceinline__ void fold_running(Acc& acc, const float (&v)[N], int6
     float h[R];
 #pragma unroll
     for (int i = 0; i < R; ++i) h[i] = 0.f;
-    if (c < n_valid) {
-      if constexpr (ColTerms<Acc>::value) acc.running(v[c], j + c, dc.v[c], h);
-      else acc.running(v[c], j + c, h);
-    }
+    if (c < n_valid) acc_running(acc, v[c], j + c, dc.v[c], h);
 #pragma unroll
     for (int i = 0; i < R; ++i) p[c][i] = c == 0 ? h[i] : p[c - 1][i] + h[i];
   }
@@ -586,18 +555,15 @@ __device__ __forceinline__ void fold_running(Acc& acc, const float (&v)[N], int6
   }
 #pragma unroll
   for (int c = 0; c < N; ++c)
-    if (c < n_valid) {
-      if constexpr (ColTerms<Acc>::value) acc.add(v[c], j + c, dc.v[c], p[c]);
-      else acc.add(v[c], j + c, p[c]);
-    }
+    if (c < n_valid) acc_add(acc, v[c], j + c, dc.v[c], p[c]);
 }
 
 // the element folds and pair folds of one warp step (see fold_pairs and fold_running): the element folds of an accumulator
 // without running sums have been made by the caller already
-template <int N, typename Acc, typename Cols>
-__device__ __forceinline__ void fold_step(Acc& acc, const float (&v)[N], int64_t j, int n_valid, StepCarry<Acc>& carry, const Cols& dc) {
-  if constexpr (RunningTerms<Acc>::value) fold_running<N>(acc, v, j, n_valid, carry.run, dc);
-  if constexpr (PairTerms<Acc>::value) fold_pairs<N>(acc, v, j, n_valid, carry.pair, dc);
+template <int N, typename Acc>
+__device__ __forceinline__ void fold_step(Acc& acc, const float (&v)[N], int64_t j, int n_valid, StepCarry<Acc>& carry, const DataCols<Acc, N>& dc) {
+  if constexpr (AccTraits<Acc>::kRunning) fold_running<N>(acc, v, j, n_valid, carry.run, dc);
+  if constexpr (AccTraits<Acc>::kPairs) fold_pairs<N>(acc, v, j, n_valid, carry.pair, dc);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -606,37 +572,12 @@ __device__ __forceinline__ void fold_step(Acc& acc, const float (&v)[N], int64_t
 // per warp-row) and folds them into the objective accumulators while they are still in registers, so the population is
 // written once and never re-read for evaluation.
 // ------------------------------------------------------------------------------------------------
-// tunables (build-time, for measurement builds: scripts/build_variants.py, scripts/kbench.py)
-#ifndef EVOK_SAMPLE_THREADS
-#define EVOK_SAMPLE_THREADS 256
-#endif
-#ifndef EVOK_SAMPLE_MINB
-#define EVOK_SAMPLE_MINB 3
-#endif
-#ifndef EVOK_SAMPLE_UNR
-#define EVOK_SAMPLE_UNR 2
-#endif
-#ifndef EVOK_SAMPLEONLY_MINB
-#define EVOK_SAMPLEONLY_MINB 5
-#endif
-#ifndef EVOK_SAMPLEONLY_UNR
-#define EVOK_SAMPLEONLY_UNR 1
-#endif
 constexpr int kSampleThreads = EVOK_SAMPLE_THREADS;
-// the fused kernels are issue/XU bound (two independent Philox chains per lane help); the sample-only kernel is store
-// bound and prefers occupancy
-// (more than one element draw per column: one Philox chain per lane and 2 CTAs per SM, so that no kernel spills)
-template <typename Acc>
-struct SampleTune {
-  static constexpr bool kManyDraws = NoiseTerms<Acc>::kDraws > 1;
-  static constexpr int kUnroll = SampleOnly<Acc>::value ? EVOK_SAMPLEONLY_UNR : RunningTerms<Acc>::value || kManyDraws ? 1 : EVOK_SAMPLE_UNR;
-  static constexpr int kMinBlocks = SampleOnly<Acc>::value ? EVOK_SAMPLEONLY_MINB : kManyDraws ? 2 : EVOK_SAMPLE_MINB;
-};
 
 // the column entries the - row of a direction folds with: its own (dm) when the element terms draw noise, else the + row's
 template <typename Acc, typename Cols>
 __device__ __forceinline__ const Cols& minus_cols(const Cols& dp, const Cols& dm) {
-  if constexpr (ElementDraws<Acc>::value) return dm;
+  if constexpr (AccTraits<Acc>::kElementDraws) return dm;
   else return dp;
 }
 
@@ -644,7 +585,7 @@ __device__ __forceinline__ const Cols& minus_cols(const Cols& dp, const Cols& dm
 // - row's (2 unit + 1) into dm, which takes dp's data entries first
 template <typename Acc, bool SYM, typename Cols>
 __device__ __forceinline__ void draw_rows(Cols& dp, Cols& dm, const PhiloxKey& key, uint32_t sw, uint64_t unit, uint32_t q) {
-  if constexpr (ElementDraws<Acc>::value) {
+  if constexpr (AccTraits<Acc>::kElementDraws) {
     const uint64_t row = SYM ? 2 * unit : unit;
     if (SYM) {
       dm = dp;
@@ -654,71 +595,26 @@ __device__ __forceinline__ void draw_rows(Cols& dp, Cols& dm, const PhiloxKey& k
   }
 }
 
-// one column group (4 columns) of one unit: sample, store, accumulate.  SQ: also *zsq += z^2 (the unscaled normals; the
-// squared norm that separable CMA-ES's active reweighting needs), in column order
-template <typename Acc, bool SYM, bool STORE, bool VEC, bool SQ = false>
+// One column group (4 columns) of one unit: sample, store, fold.  SQ: also *zsq += z^2 (the unscaled normals; the squared norm
+// that separable CMA-ES's active reweighting needs), in column order.
+// An accumulator without warp steps folds each element as it is sampled; `active` and the carries are not used.  One with warp
+// steps is called by EVERY lane of the warp on every step (fold_step shuffles): a lane whose group lies past the row's end
+// (!active) draws, loads and stores nothing and folds nothing.  Its samples and element folds are the same, in the same order
+// (with running sums the element folds come after the scan, in fold_running); the + and - rows have their own neighbours and
+// carries.
+template <typename Acc, bool SYM, bool STORE, bool VEC, bool SQ>
 __device__ __forceinline__ void sample_group(const PhiloxKey& key, uint32_t sw, uint64_t unit, uint32_t q, int64_t D,
                                              const float* __restrict__ mu, const float* __restrict__ sigma, float* xp, float* xm,
-                                             Acc& accp, Acc& accm, float* zsq = nullptr) {
-  float z[4];
-  normals4(key, sw, unit, q, z);
-  const int64_t j = (int64_t)q << 2;
-  typename ColsOf<Acc, 4>::type dc, dm;  // dm: the - row's entries, with its own draws (element noise only)
-  const auto& dcm = minus_cols<Acc>(dc, dm);
-  if (VEC) {
-    if (SQ) {
-      *zsq = fmaf(z[0], z[0], *zsq); *zsq = fmaf(z[1], z[1], *zsq); *zsq = fmaf(z[2], z[2], *zsq); *zsq = fmaf(z[3], z[3], *zsq);
-    }
-    const float4 m = __ldg(reinterpret_cast<const float4*>(mu + j));
-    const float4 s = __ldg(reinterpret_cast<const float4*>(sigma + j));
-    const float p0 = fmaf(s.x, z[0], m.x), p1 = fmaf(s.y, z[1], m.y), p2 = fmaf(s.z, z[2], m.z), p3 = fmaf(s.w, z[3], m.w);
-    if (STORE) st_stream4(xp + j, p0, p1, p2, p3);
-    dc.load4(accp, j);
-    draw_rows<Acc, SYM>(dc, dm, key, sw, unit, q);
-    fold(accp, p0, j, dc, 0); fold(accp, p1, j + 1, dc, 1); fold(accp, p2, j + 2, dc, 2); fold(accp, p3, j + 3, dc, 3);
-    if (SYM) {
-      const float n0 = fmaf(-s.x, z[0], m.x), n1 = fmaf(-s.y, z[1], m.y), n2 = fmaf(-s.z, z[2], m.z), n3 = fmaf(-s.w, z[3], m.w);
-      if (STORE) st_stream4(xm + j, n0, n1, n2, n3);
-      fold(accm, n0, j, dcm, 0); fold(accm, n1, j + 1, dcm, 1); fold(accm, n2, j + 2, dcm, 2); fold(accm, n3, j + 3, dcm, 3);
-    }
-  } else {
-    draw_rows<Acc, SYM>(dc, dm, key, sw, unit, q);
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      if (j + c < D) {
-        if (SQ) *zsq = fmaf(z[c], z[c], *zsq);
-        const float m = __ldg(mu + j + c), s = __ldg(sigma + j + c);
-        const float p = fmaf(s, z[c], m);
-        if (STORE) st_stream1(xp + j + c, p);
-        dc.load1(accp, j + c, c);
-        fold(accp, p, j + c, dc, c);
-        if (SYM) {
-          const float n = fmaf(-s, z[c], m);
-          if (STORE) st_stream1(xm + j + c, n);
-          if constexpr (ElementDraws<Acc>::value) dm.load1(accp, j + c, c);
-          fold(accm, n, j + c, dcm, c);
-        }
-      }
-    }
-  }
-}
-
-// sample_group for an accumulator with pair terms or running sums, called by EVERY lane of the warp on every step (fold_step
-// shuffles): a lane whose group lies past the row's end (!active) draws, loads and stores nothing and folds nothing.  The
-// samples and the element adds are those of sample_group, in the same order (with running sums the element adds come after the
-// scan, in fold_running); the + and - rows have their own neighbours and carries.
-template <typename Acc, bool SYM, bool STORE, bool VEC, bool SQ>
-__device__ __forceinline__ void sample_group_pairs(const PhiloxKey& key, uint32_t sw, uint64_t unit, uint32_t q, int64_t D,
-                                                   const float* __restrict__ mu, const float* __restrict__ sigma, float* xp, float* xm,
-                                                   Acc& accp, Acc& accm, float* zsq, bool active, StepCarry<Acc>& carry_p,
-                                                   StepCarry<Acc>& carry_m) {
-  constexpr bool kFoldNow = !RunningTerms<Acc>::value;  // element terms without running sums fold as they are sampled
+                                             Acc& accp, Acc& accm, float* zsq, bool active, StepCarry<Acc>& carry_p,
+                                             StepCarry<Acc>& carry_m) {
+  using T = AccTraits<Acc>;
+  constexpr bool kFoldNow = !T::kRunning;  // element terms without running sums fold as they are sampled
   float p[4] = {0.f, 0.f, 0.f, 0.f}, n[4] = {0.f, 0.f, 0.f, 0.f};
   const int64_t j = (int64_t)q << 2;
   int n_valid = 0;
-  typename ColsOf<Acc, 4>::type dc, dm;  // dm: the - row's entries, with its own draws (element noise only)
+  DataCols<Acc, 4> dc, dm;  // dm: the - row's entries, with its own draws (element noise only)
   const auto& dcm = minus_cols<Acc>(dc, dm);
-  if (active) {
+  if (!T::kWarpSteps || active) {  // a compile-time true without warp steps
     float z[4];
     normals4(key, sw, unit, q, z);
     if (VEC) {
@@ -732,13 +628,13 @@ __device__ __forceinline__ void sample_group_pairs(const PhiloxKey& key, uint32_
       dc.load4(accp, j);
       draw_rows<Acc, SYM>(dc, dm, key, sw, unit, q);
       if constexpr (kFoldNow) {
-        fold(accp, p[0], j, dc, 0); fold(accp, p[1], j + 1, dc, 1); fold(accp, p[2], j + 2, dc, 2); fold(accp, p[3], j + 3, dc, 3);
+        acc_add(accp, p[0], j, dc.v[0]); acc_add(accp, p[1], j + 1, dc.v[1]); acc_add(accp, p[2], j + 2, dc.v[2]); acc_add(accp, p[3], j + 3, dc.v[3]);
       }
       if (SYM) {
         n[0] = fmaf(-s.x, z[0], m.x); n[1] = fmaf(-s.y, z[1], m.y); n[2] = fmaf(-s.z, z[2], m.z); n[3] = fmaf(-s.w, z[3], m.w);
         if (STORE) st_stream4(xm + j, n[0], n[1], n[2], n[3]);
         if constexpr (kFoldNow) {
-          fold(accm, n[0], j, dcm, 0); fold(accm, n[1], j + 1, dcm, 1); fold(accm, n[2], j + 2, dcm, 2); fold(accm, n[3], j + 3, dcm, 3);
+          acc_add(accm, n[0], j, dcm.v[0]); acc_add(accm, n[1], j + 1, dcm.v[1]); acc_add(accm, n[2], j + 2, dcm.v[2]); acc_add(accm, n[3], j + 3, dcm.v[3]);
         }
       }
       n_valid = 4;
@@ -752,25 +648,27 @@ __device__ __forceinline__ void sample_group_pairs(const PhiloxKey& key, uint32_
           p[c] = fmaf(s, z[c], m);
           if (STORE) st_stream1(xp + j + c, p[c]);
           dc.load1(accp, j + c, c);
-          if constexpr (kFoldNow) fold(accp, p[c], j + c, dc, c);
+          if constexpr (kFoldNow) acc_add(accp, p[c], j + c, dc.v[c]);
           if (SYM) {
             n[c] = fmaf(-s, z[c], m);
             if (STORE) st_stream1(xm + j + c, n[c]);
-            if constexpr (ElementDraws<Acc>::value) dm.load1(accp, j + c, c);
-            if constexpr (kFoldNow) fold(accm, n[c], j + c, dcm, c);
+            if constexpr (T::kElementDraws) dm.load1(accp, j + c, c);
+            if constexpr (kFoldNow) acc_add(accm, n[c], j + c, dcm.v[c]);
           }
         }
       }
       n_valid = D - j < 4 ? (int)(D - j) : 4;  // the partial last group: a pair is folded only where column j + 1 < D
     }
   }
-  if constexpr (PairTerms<Acc>::value)
-    if (n_valid > 0 && j > 0) {
-      dc.load_left(accp, j);
-      if constexpr (ElementDraws<Acc>::value) dm.load_left(accp, j);
-    }
-  fold_step<4>(accp, p, j, n_valid, carry_p, dc);
-  if (SYM) fold_step<4>(accm, n, j, n_valid, carry_m, dcm);
+  if constexpr (T::kWarpSteps) {
+    if constexpr (T::kPairs)
+      if (n_valid > 0 && j > 0) {
+        dc.load_left(accp, j);
+        if constexpr (T::kElementDraws) dm.load_left(accp, j);
+      }
+    fold_step<4>(accp, p, j, n_valid, carry_p, dc);
+    if (SYM) fold_step<4>(accm, n, j, n_valid, carry_m, dcm);
+  }
 }
 
 // One unit u (a direction of symmetric sampling, else a row) of the warp of lane `lane`: sample its row(s) from (key, stream word sw, unit
@@ -781,28 +679,28 @@ template <typename Acc, bool SYM, bool STORE, bool VEC, bool PUSH, bool SQ>
 __device__ __forceinline__ void sample_eval_unit(int lane, float* __restrict__ X, int64_t ldx, const float* __restrict__ mu,
                                                  const float* __restrict__ sigma, int64_t row0, int64_t u, int64_t D, const PhiloxKey& key, uint32_t sw,
                                                  uint32_t nq, uint64_t unit0, float* __restrict__ f, const PeerSink& sink, float* __restrict__ q_out,
-                                                 const typename DataTerms<Acc>::Arg& data) {
-  Acc accp = make_acc<Acc>(D, data), accm = make_acc<Acc>(D, data);
+                                                 const typename AccTraits<Acc>::DataArg& data) {
+  Acc accp = acc_make<Acc>(D, data), accm = acc_make<Acc>(D, data);
   const int64_t r = SYM ? 2 * u : u;
   float* xp = STORE ? X + r * ldx : nullptr;
   float* xm = STORE ? xp + ldx : nullptr;
   const uint64_t unit = unit0 + (uint64_t)u;
-  constexpr int kSampleUnroll = SampleTune<Acc>::kUnroll;
+  constexpr int kSampleUnroll = AccTraits<Acc>::kSampleUnroll;
   float zsq = 0.f;
-  if constexpr (WarpSteps<Acc>::value) {
+  StepCarry<Acc> carry_p, carry_m;
+  if constexpr (AccTraits<Acc>::kWarpSteps) {
     // warp-uniform steps of 32 groups in increasing column order (fold_step shuffles and carries from step to step); each lane
     // still visits its groups lane, lane + 32, ... in increasing order, the order of the loops below and of eval_kernel
-    StepCarry<Acc> carry_p, carry_m;
     uint32_t b = 0;
     for (; b + 32u * kSampleUnroll <= nq; b += 32u * kSampleUnroll) {
 #pragma unroll
       for (int uu = 0; uu < kSampleUnroll; ++uu)
-        sample_group_pairs<Acc, SYM, STORE, VEC, SQ>(key, sw, unit, b + 32u * uu + lane, D, mu, sigma, xp, xm, accp, accm, &zsq, true,
-                                                     carry_p, carry_m);
+        sample_group<Acc, SYM, STORE, VEC, SQ>(key, sw, unit, b + 32u * uu + lane, D, mu, sigma, xp, xm, accp, accm, &zsq, true,
+                                               carry_p, carry_m);
     }
     for (; b < nq; b += 32)
-      sample_group_pairs<Acc, SYM, STORE, VEC, SQ>(key, sw, unit, b + lane, D, mu, sigma, xp, xm, accp, accm, &zsq, b + lane < nq,
-                                                   carry_p, carry_m);
+      sample_group<Acc, SYM, STORE, VEC, SQ>(key, sw, unit, b + lane, D, mu, sigma, xp, xm, accp, accm, &zsq, b + lane < nq,
+                                             carry_p, carry_m);
   } else {
     uint32_t q = lane;
     if (kSampleUnroll > 1) {
@@ -810,20 +708,22 @@ __device__ __forceinline__ void sample_eval_unit(int lane, float* __restrict__ X
       for (; q + 32u * (kSampleUnroll - 1) < nq; q += 32u * kSampleUnroll) {
 #pragma unroll
         for (int uu = 0; uu < kSampleUnroll; ++uu)
-          sample_group<Acc, SYM, STORE, VEC, SQ>(key, sw, unit, q + 32u * uu, D, mu, sigma, xp, xm, accp, accm, &zsq);
+          sample_group<Acc, SYM, STORE, VEC, SQ>(key, sw, unit, q + 32u * uu, D, mu, sigma, xp, xm, accp, accm, &zsq, true, carry_p,
+                                                 carry_m);
       }
     }
-    for (; q < nq; q += 32) sample_group<Acc, SYM, STORE, VEC, SQ>(key, sw, unit, q, D, mu, sigma, xp, xm, accp, accm, &zsq);
+    for (; q < nq; q += 32)
+      sample_group<Acc, SYM, STORE, VEC, SQ>(key, sw, unit, q, D, mu, sigma, xp, xm, accp, accm, &zsq, true, carry_p, carry_m);
   }
   if (SQ) {
     zsq = warp_sum(zsq);
     if (lane == 0) q_out[r] = zsq;
   }
-  if (!SampleOnly<Acc>::value) {
+  if (!AccTraits<Acc>::kSampleOnly) {
     const uint64_t row = SYM ? 2 * unit : unit;  // the global row of the + row (or the row)
-    const float fp = finish_row(accp, D, key, sw, row);
+    const float fp = acc_finish(accp, D, &key, sw, row);
     float fm = 0.f;
-    if (SYM) fm = finish_row(accm, D, key, sw, row + 1);
+    if (SYM) fm = acc_finish(accm, D, &key, sw, row + 1);
     if (lane == 0) {
       if (PUSH) {
         for (int p = 0; p < sink.world; ++p) {
@@ -843,11 +743,11 @@ __device__ __forceinline__ void sample_eval_unit(int lane, float* __restrict__ X
 // generation, fused into the producer) and the last CTA raises this rank's flag on every peer.
 // SQ (non-symmetric only): q[r] = sum_j z_rj^2 of the unscaled normals, accumulated in registers next to the objective.
 template <typename Acc, bool SYM, bool STORE, bool VEC, bool PUSH, bool SQ = false>
-__global__ void __launch_bounds__(kSampleThreads, SampleTune<Acc>::kMinBlocks)
+__global__ void __launch_bounds__(kSampleThreads, AccTraits<Acc>::kSampleMinBlocks)
     sample_eval_kernel(float* __restrict__ X, int64_t ldx, const float* __restrict__ mu, const float* __restrict__ sigma,
                        int64_t row0, int64_t n_units, int64_t D, const __grid_constant__ PhiloxKey key, const uint32_t* __restrict__ stream_off,
                        float* __restrict__ f, const __grid_constant__ PeerSink sink, const unsigned long long* epoch, unsigned int* done,
-                       float* __restrict__ q_out, const typename DataTerms<Acc>::Arg data) {
+                       float* __restrict__ q_out, const typename AccTraits<Acc>::DataArg data) {
   static_assert(!(SQ && (SYM || PUSH)), "the squared norms are produced by the plain non-symmetric sampler only");
   const int lane = threadIdx.x & 31;
   const uint32_t sw = key.stream_lo + (stream_off ? __ldg(stream_off) : 0u);
@@ -867,60 +767,54 @@ __global__ void __launch_bounds__(kSampleThreads, SampleTune<Acc>::kMinBlocks)
 // all items, bit-identical to one sample_eval_kernel launch per item with stream id (stream id of the key) + b.  The data of
 // an accumulator with data terms is per item too, at the item strides of its binding.
 template <typename Acc, bool SYM, bool STORE, bool VEC>
-__global__ void __launch_bounds__(kSampleThreads, SampleTune<Acc>::kMinBlocks)
+__global__ void __launch_bounds__(kSampleThreads, AccTraits<Acc>::kSampleMinBlocks)
     sample_eval_batched_kernel(float* __restrict__ X, int64_t item_stride_x, int64_t ldx, const float* __restrict__ mu, int64_t item_stride_mu,
                                const float* __restrict__ sigma, int64_t item_stride_sigma, int64_t n_units, int64_t D,
-                               const __grid_constant__ PhiloxKey key, float* __restrict__ f, const typename DataTerms<Acc>::Arg data) {
+                               const __grid_constant__ PhiloxKey key, float* __restrict__ f, const typename AccTraits<Acc>::DataArg data) {
   const int lane = threadIdx.x & 31;
   const int64_t item = blockIdx.y;
   if (STORE) X += item * item_stride_x;
   mu += item * item_stride_mu;
   sigma += item * item_stride_sigma;
-  if (!SampleOnly<Acc>::value) f += item * (SYM ? 2 * n_units : n_units);
+  if (!AccTraits<Acc>::kSampleOnly) f += item * (SYM ? 2 * n_units : n_units);
   const uint32_t sw = key.stream_lo + (uint32_t)item;
   const int64_t warps_total = (int64_t)gridDim.x * (kSampleThreads / 32);
   const int64_t gw = (int64_t)blockIdx.x * (kSampleThreads / 32) + (threadIdx.x >> 5);
   const uint32_t nq = (uint32_t)((D + 3) >> 2);
   const PeerSink no_sink{};
-  const typename DataTerms<Acc>::Arg my_data = item_data(data, item);
+  const typename AccTraits<Acc>::DataArg my_data = item_data(data, item);
   for (int64_t u = gw; u < n_units; u += warps_total)
     sample_eval_unit<Acc, SYM, STORE, VEC, false, false>(lane, X, ldx, mu, sigma, 0, u, D, key, sw, nq, 0, f, no_sink, nullptr, my_data);
 }
 
 constexpr int kEvalThreads = 256;
 
-// the stream word of eval_kernel's draw, and the fitness of its row r (an accumulator with noise draws from global row row0 + r)
-template <typename Acc>
-__device__ __forceinline__ uint32_t eval_stream_word(const typename NoiseTerms<Acc>::EvalArg& noise) {
-  if constexpr (NoiseTerms<Acc>::value) return noise.key.stream_lo + (noise.stream_off ? __ldg(noise.stream_off) : 0u);
-  else return 0u;
-}
-template <typename Acc>
-__device__ __forceinline__ float eval_finish(Acc& acc, int64_t D, const typename NoiseTerms<Acc>::EvalArg& noise, uint32_t sw, int64_t r) {
-  if constexpr (NoiseTerms<Acc>::value) return acc.finish(D, noise.key, sw, (uint64_t)(noise.row0 + r));
-  else return acc.finish(D);
-}
-
 // The evaluation kernel.  Row r of X is global row noise.row0 + r of the draw (noise.key, stream word noise.key.stream_lo +
 // *noise.stream_off) for an accumulator with noise (evok_eval_keyed), which then gets the noise the sampler gave the row;
 // `noise` is an empty struct for every other accumulator.
 template <typename Acc, bool VEC>
-__global__ void __launch_bounds__(kEvalThreads, NoiseTerms<Acc>::kEvalMinBlocks)
+__global__ void __launch_bounds__(kEvalThreads, AccTraits<Acc>::kEvalMinBlocks)
     eval_kernel(const float* __restrict__ X, int64_t ldx, int64_t n_rows, int64_t D, float* __restrict__ f,
-                const typename DataTerms<Acc>::Arg data, const typename NoiseTerms<Acc>::EvalArg noise) {
+                const typename AccTraits<Acc>::DataArg data, const typename AccTraits<Acc>::EvalArg noise) {
+  using T = AccTraits<Acc>;
   const int lane = threadIdx.x & 31;
-  const uint32_t sw = eval_stream_word<Acc>(noise);
+  const PhiloxKey* key = nullptr;  // the rows' draw: none without noise
+  uint32_t sw = 0u;
+  int64_t row0 = 0;
+  if constexpr (T::kNoise) {
+    key = &noise.key;
+    sw = noise.key.stream_lo + (noise.stream_off ? __ldg(noise.stream_off) : 0u);
+    row0 = noise.row0;
+  }
   const int64_t warps_total = (int64_t)gridDim.x * (kEvalThreads / 32);
   const int64_t gw = (int64_t)blockIdx.x * (kEvalThreads / 32) + (threadIdx.x >> 5);
-  using Cols4 = typename ColsOf<Acc, 4>::type;
-  using Cols1 = typename ColsOf<Acc, 1>::type;
   for (int64_t r = gw; r < n_rows; r += warps_total) {
-    Acc acc = make_acc<Acc>(D, data);
+    Acc acc = acc_make<Acc>(D, data);
     const float* x = X + r * ldx;
-    if constexpr (WarpSteps<Acc>::value) {
+    if constexpr (T::kWarpSteps) {
       // warp-uniform steps (fold_step shuffles); per lane the groups, element adds, running sums and pair folds of
       // sample_eval_kernel's VEC path in the same order, so both kernels give the same fitness bit for bit on the same X
-      constexpr bool kFoldNow = !RunningTerms<Acc>::value;
+      constexpr bool kFoldNow = !T::kRunning;
       StepCarry<Acc> carry;
       if (VEC) {
         const int64_t nq = D >> 2;
@@ -934,13 +828,13 @@ __global__ void __launch_bounds__(kEvalThreads, NoiseTerms<Acc>::kEvalMinBlocks)
           for (int k = 0; k < 4; ++k) {
             const int64_t jk = 4 * (q + 32 * k);
             const float v[4] = {g[k].x, g[k].y, g[k].z, g[k].w};
-            Cols4 dc;
+            DataCols<Acc, 4> dc;
             dc.load4(acc, jk);
-            if constexpr (ElementDraws<Acc>::value) dc.draw4(noise.key, sw, noise.row0 + r, (uint32_t)(q + 32 * k));
-            if constexpr (PairTerms<Acc>::value)
+            if constexpr (T::kElementDraws) dc.draw4(*key, sw, row0 + r, (uint32_t)(q + 32 * k));
+            if constexpr (T::kPairs)
               if (jk > 0) dc.load_left(acc, jk);
             if constexpr (kFoldNow) {
-              fold(acc, v[0], jk, dc, 0); fold(acc, v[1], jk + 1, dc, 1); fold(acc, v[2], jk + 2, dc, 2); fold(acc, v[3], jk + 3, dc, 3);
+              acc_add(acc, v[0], jk, dc.v[0]); acc_add(acc, v[1], jk + 1, dc.v[1]); acc_add(acc, v[2], jk + 2, dc.v[2]); acc_add(acc, v[3], jk + 3, dc.v[3]);
             }
             fold_step<4>(acc, v, jk, 4, carry, dc);
           }
@@ -951,14 +845,14 @@ __global__ void __launch_bounds__(kEvalThreads, NoiseTerms<Acc>::kEvalMinBlocks)
           const float4 a = active ? ld_stream4(x + 4 * q) : make_float4(0.f, 0.f, 0.f, 0.f);
           const float v[4] = {a.x, a.y, a.z, a.w};
           const int64_t ja = 4 * q;
-          Cols4 dc;
+          DataCols<Acc, 4> dc;
           if (active) {
             dc.load4(acc, ja);
-            if constexpr (ElementDraws<Acc>::value) dc.draw4(noise.key, sw, noise.row0 + r, (uint32_t)q);
-            if constexpr (PairTerms<Acc>::value)
+            if constexpr (T::kElementDraws) dc.draw4(*key, sw, row0 + r, (uint32_t)q);
+            if constexpr (T::kPairs)
               if (ja > 0) dc.load_left(acc, ja);
             if constexpr (kFoldNow) {
-              fold(acc, v[0], ja, dc, 0); fold(acc, v[1], ja + 1, dc, 1); fold(acc, v[2], ja + 2, dc, 2); fold(acc, v[3], ja + 3, dc, 3);
+              acc_add(acc, v[0], ja, dc.v[0]); acc_add(acc, v[1], ja + 1, dc.v[1]); acc_add(acc, v[2], ja + 2, dc.v[2]); acc_add(acc, v[3], ja + 3, dc.v[3]);
             }
           }
           fold_step<4>(acc, v, ja, active ? 4 : 0, carry, dc);
@@ -968,13 +862,13 @@ __global__ void __launch_bounds__(kEvalThreads, NoiseTerms<Acc>::kEvalMinBlocks)
           const int64_t j = b + lane;
           const bool active = j < D;
           const float v[1] = {active ? ld_stream1(x + j) : 0.f};
-          Cols1 dc;
+          DataCols<Acc, 1> dc;
           if (active) {
             dc.load1(acc, j, 0);
-            if constexpr (ElementDraws<Acc>::value) dc.draw1(noise.key, sw, noise.row0 + r, j, 0);
-            if constexpr (PairTerms<Acc>::value)
+            if constexpr (T::kElementDraws) dc.draw1(*key, sw, row0 + r, j, 0);
+            if constexpr (T::kPairs)
               if (j > 0) dc.load_left(acc, j);
-            if constexpr (kFoldNow) fold(acc, v[0], j, dc, 0);
+            if constexpr (kFoldNow) acc_add(acc, v[0], j, dc.v[0]);
           }
           fold_step<1>(acc, v, j, active ? 1 : 0, carry, dc);
         }
@@ -987,35 +881,35 @@ __global__ void __launch_bounds__(kEvalThreads, NoiseTerms<Acc>::kEvalMinBlocks)
         const float4 a = ld_stream4(x + 4 * q), b = ld_stream4(x + 4 * (q + 32)), c = ld_stream4(x + 4 * (q + 64)),
                      d = ld_stream4(x + 4 * (q + 96));
         const int64_t ja = 4 * q, jb = 4 * (q + 32), jc = 4 * (q + 64), jd = 4 * (q + 96);
-        Cols4 da, db, dc, dd;
+        DataCols<Acc, 4> da, db, dc, dd;
         da.load4(acc, ja); db.load4(acc, jb); dc.load4(acc, jc); dd.load4(acc, jd);
-        if constexpr (ElementDraws<Acc>::value) {
-          const uint64_t row = noise.row0 + r;
-          da.draw4(noise.key, sw, row, (uint32_t)q); db.draw4(noise.key, sw, row, (uint32_t)(q + 32));
-          dc.draw4(noise.key, sw, row, (uint32_t)(q + 64)); dd.draw4(noise.key, sw, row, (uint32_t)(q + 96));
+        if constexpr (T::kElementDraws) {
+          const uint64_t row = row0 + r;
+          da.draw4(*key, sw, row, (uint32_t)q); db.draw4(*key, sw, row, (uint32_t)(q + 32));
+          dc.draw4(*key, sw, row, (uint32_t)(q + 64)); dd.draw4(*key, sw, row, (uint32_t)(q + 96));
         }
-        fold(acc, a.x, ja, da, 0); fold(acc, a.y, ja + 1, da, 1); fold(acc, a.z, ja + 2, da, 2); fold(acc, a.w, ja + 3, da, 3);
-        fold(acc, b.x, jb, db, 0); fold(acc, b.y, jb + 1, db, 1); fold(acc, b.z, jb + 2, db, 2); fold(acc, b.w, jb + 3, db, 3);
-        fold(acc, c.x, jc, dc, 0); fold(acc, c.y, jc + 1, dc, 1); fold(acc, c.z, jc + 2, dc, 2); fold(acc, c.w, jc + 3, dc, 3);
-        fold(acc, d.x, jd, dd, 0); fold(acc, d.y, jd + 1, dd, 1); fold(acc, d.z, jd + 2, dd, 2); fold(acc, d.w, jd + 3, dd, 3);
+        acc_add(acc, a.x, ja, da.v[0]); acc_add(acc, a.y, ja + 1, da.v[1]); acc_add(acc, a.z, ja + 2, da.v[2]); acc_add(acc, a.w, ja + 3, da.v[3]);
+        acc_add(acc, b.x, jb, db.v[0]); acc_add(acc, b.y, jb + 1, db.v[1]); acc_add(acc, b.z, jb + 2, db.v[2]); acc_add(acc, b.w, jb + 3, db.v[3]);
+        acc_add(acc, c.x, jc, dc.v[0]); acc_add(acc, c.y, jc + 1, dc.v[1]); acc_add(acc, c.z, jc + 2, dc.v[2]); acc_add(acc, c.w, jc + 3, dc.v[3]);
+        acc_add(acc, d.x, jd, dd.v[0]); acc_add(acc, d.y, jd + 1, dd.v[1]); acc_add(acc, d.z, jd + 2, dd.v[2]); acc_add(acc, d.w, jd + 3, dd.v[3]);
       }
       for (; q < nq; q += 32) {
         const float4 a = ld_stream4(x + 4 * q);
         const int64_t ja = 4 * q;
-        Cols4 da;
+        DataCols<Acc, 4> da;
         da.load4(acc, ja);
-        if constexpr (ElementDraws<Acc>::value) da.draw4(noise.key, sw, noise.row0 + r, (uint32_t)q);
-        fold(acc, a.x, ja, da, 0); fold(acc, a.y, ja + 1, da, 1); fold(acc, a.z, ja + 2, da, 2); fold(acc, a.w, ja + 3, da, 3);
+        if constexpr (T::kElementDraws) da.draw4(*key, sw, row0 + r, (uint32_t)q);
+        acc_add(acc, a.x, ja, da.v[0]); acc_add(acc, a.y, ja + 1, da.v[1]); acc_add(acc, a.z, ja + 2, da.v[2]); acc_add(acc, a.w, ja + 3, da.v[3]);
       }
     } else {
       for (int64_t j = lane; j < D; j += 32) {
-        Cols1 dc;
+        DataCols<Acc, 1> dc;
         dc.load1(acc, j, 0);
-        if constexpr (ElementDraws<Acc>::value) dc.draw1(noise.key, sw, noise.row0 + r, j, 0);
-        fold(acc, ld_stream1(x + j), j, dc, 0);
+        if constexpr (T::kElementDraws) dc.draw1(*key, sw, row0 + r, j, 0);
+        acc_add(acc, ld_stream1(x + j), j, dc.v[0]);
       }
     }
-    const float v = eval_finish(acc, D, noise, sw, r);
+    const float v = acc_finish(acc, D, key, sw, (uint64_t)(row0 + r));
     if (lane == 0) f[r] = v;
   }
 }

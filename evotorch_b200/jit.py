@@ -101,10 +101,11 @@ def _float_literal(v: float) -> str:
 
 
 class _Expr:
-    """One parsed expression: `cuda` is its CUDA text over the given identifiers, `torch(env)` evaluates it on tensors."""
+    """One translated expression: `cuda` is its CUDA text over the given identifiers, `torch(env)` evaluates it on tensors and
+    `names` holds the Python names whose identifiers `cuda` contains."""
 
-    def __init__(self, cuda: str, fn: Callable):
-        self.cuda, self.torch = cuda, fn
+    def __init__(self, cuda: str, fn: Callable, names: frozenset = frozenset()):
+        self.cuda, self.torch, self.names = cuda, fn, names
 
 
 def _as_tensor(v, env):
@@ -124,8 +125,8 @@ def _int_exponent(node) -> Optional[int]:
 
 
 def _translate(node, names: Dict[str, str], where: str, draws: Optional["_Draws"] = None) -> _Expr:
-    """names: the Python names allowed here -> their CUDA identifiers; draws: where rand() / randn() here draw from (None: they
-    are refused here)."""
+    """node: a tree of `_parse`; names: the Python names allowed here -> their CUDA identifiers; draws: where rand() / randn() here
+    draw from (None: they are refused here)."""
     allowed = _ALLOWED_TEXT.format(names=", ".join(names))
     if isinstance(node, ast.Expression):
         return _translate(node.body, names, where, draws)
@@ -136,7 +137,7 @@ def _translate(node, names: Dict[str, str], where: str, draws: Optional["_Draws"
         return _Expr(_float_literal(v), lambda env, v=v: v)
     if isinstance(node, ast.Name):
         if node.id in names:
-            return _Expr(names[node.id], lambda env, n=node.id: env[n])
+            return _Expr(names[node.id], lambda env, n=node.id: env[n], frozenset((node.id,)))
         if node.id in CONSTANTS:
             v = CONSTANTS[node.id]
             return _Expr(_float_literal(v), lambda env, v=v: v)
@@ -144,7 +145,7 @@ def _translate(node, names: Dict[str, str], where: str, draws: Optional["_Draws"
     if isinstance(node, ast.UnaryOp):
         a = _translate(node.operand, names, where, draws)
         if isinstance(node.op, ast.USub):
-            return _Expr(f"(-{a.cuda})", lambda env: -a.torch(env))
+            return _Expr(f"(-{a.cuda})", lambda env: -a.torch(env), a.names)
         if isinstance(node.op, ast.UAdd):
             return a
         raise ValueError(f"{where}: the operator {type(node.op).__name__} is not supported; {allowed}")
@@ -156,16 +157,16 @@ def _translate(node, names: Dict[str, str], where: str, draws: Optional["_Draws"
                 if n == 0:
                     return _Expr("1.0f", lambda env: 1.0)
                 prod = "(" + " * ".join([a.cuda] * abs(n)) + ")"
-                return _Expr(prod if n > 0 else f"(1.0f / {prod})", lambda env: a.torch(env) ** n)
+                return _Expr(prod if n > 0 else f"(1.0f / {prod})", lambda env: a.torch(env) ** n, a.names)
             b = _translate(node.right, names, where, draws)
-            return _Expr(f"powf({a.cuda}, {b.cuda})", lambda env: torch.pow(_as_tensor(a.torch(env), env), b.torch(env)))
+            return _Expr(f"powf({a.cuda}, {b.cuda})", lambda env: torch.pow(_as_tensor(a.torch(env), env), b.torch(env)), a.names | b.names)
         if type(node.op) not in _BINOPS:
             raise ValueError(f"{where}: the operator {type(node.op).__name__} is not supported; {allowed}")
         b = _translate(node.right, names, where, draws)
         op = _BINOPS[type(node.op)]
         fn = {"+": lambda env: a.torch(env) + b.torch(env), "-": lambda env: a.torch(env) - b.torch(env),
               "*": lambda env: a.torch(env) * b.torch(env), "/": lambda env: a.torch(env) / b.torch(env)}[op]
-        return _Expr(f"({a.cuda} {op} {b.cuda})", fn)
+        return _Expr(f"({a.cuda} {op} {b.cuda})", fn, a.names | b.names)
     if isinstance(node, ast.Call) and isinstance(node.func, ast.Name) and node.func.id in NOISE:
         if node.args or node.keywords:
             raise ValueError(f"{where}: {node.func.id}() takes no arguments, got {ast.unparse(node)!r}")
@@ -188,7 +189,7 @@ def _translate(node, names: Dict[str, str], where: str, draws: Optional["_Draws"
             lv, rv = _as_tensor(l.torch(env), env), _as_tensor(r.torch(env), env)
             return torch.where(top(lv, rv), _as_tensor(a.torch(env), env), _as_tensor(b.torch(env), env))
 
-        return _Expr(f"(({l.cuda} {op} {r.cuda}) ? {a.cuda} : {b.cuda})", where_fn)
+        return _Expr(f"(({l.cuda} {op} {r.cuda}) ? {a.cuda} : {b.cuda})", where_fn, l.names | r.names | a.names | b.names)
     if isinstance(node, ast.Compare):
         raise ValueError(f"{where}: Compare ({ast.unparse(node)!r}) is not supported outside where: a comparison is allowed only as "
                          f"the condition of where(cond, a, b); {allowed}")
@@ -205,18 +206,26 @@ def _translate(node, names: Dict[str, str], where: str, draws: Optional["_Draws"
         args = [_translate(a, names, where, draws) for a in node.args]
         cname, tfn = FUNCTIONS[name]
         return _Expr(f"{cname}(" + ", ".join(a.cuda for a in args) + ")",
-                     lambda env: tfn(*[_as_tensor(a.torch(env), env) for a in args]))
+                     lambda env: tfn(*[_as_tensor(a.torch(env), env) for a in args]), frozenset().union(*(a.names for a in args)))
     raise ValueError(f"{where}: {type(node).__name__} ({ast.unparse(node)!r}) is not supported; {allowed}")
 
 
-def _parse(text: str, names: Dict[str, str], where: str, draws: Optional["_Draws"] = None) -> _Expr:
+def _parse(text: str, where: str):
+    """The tree of an expression, for `_translate`, and the names it reads (not the functions it calls: a reduction, running sum
+    or data name may be `rand`)."""
     if not isinstance(text, str):
         raise ValueError(f"{where}: expected an expression string, got {type(text).__name__}")
     try:
         tree = ast.parse(text, mode="eval")
     except SyntaxError as e:
         raise ValueError(f"{where}: not a Python expression: {text!r} ({e.msg})") from None
-    return _translate(tree, names, where, draws)
+    called, reads = set(), set()
+    for n in ast.walk(tree):  # breadth first: a call comes before the name it calls
+        if isinstance(n, ast.Call):
+            called.add(id(n.func))
+        elif isinstance(n, ast.Name) and id(n) not in called:
+            reads.add(n.id)
+    return tree, reads
 
 
 class _Draws:
@@ -263,16 +272,6 @@ def data_kinds(data: dict) -> Dict[str, bool]:
             raise ValueError(f"data[{name!r}]: expected a float32 tensor with at least one dimension, got {what}")
         kinds[name] = t.shape[-1] != 1
     return kinds
-
-
-def _names_used(text) -> set:
-    """The names an expression reads (not the functions it calls: a reduction, running sum or data name may be `rand`)."""
-    try:
-        tree = ast.parse(text, mode="eval")
-    except (SyntaxError, TypeError):
-        return set()  # _parse reports it
-    called = {id(n.func) for n in ast.walk(tree) if isinstance(n, ast.Call)}
-    return {n.id for n in ast.walk(tree) if isinstance(n, ast.Name) and id(n) not in called}
 
 
 class ObjectiveSpec:
@@ -330,8 +329,13 @@ class ObjectiveSpec:
                 value_names[name] = f"c_{name}"
         allowed_where = ("a running sum is usable in the element terms of sums, prods, maxs and mins only (not in a pair term, a "
                          "running term or `value`)")
-        for c, t in running.items():
-            used = _names_used(t)
+        vectors = [n for n, v in self.kinds.items() if v]
+
+        def next_entry(e: _Expr) -> Optional[str]:  # a vector whose entry at column j + 1 (name_n) the expression reads
+            return next((n for n in vectors if f"{n}_n" in e.names), None)
+
+        running_trees = {c: _parse(t, f"running[{c!r}]") for c, t in running.items()}
+        for c, (_, used) in running_trees.items():
             self._check_data_names(used, f"running[{c!r}]", term=True)
             bad = used & (set(running) | set(self.reductions))
             if bad:
@@ -339,35 +343,35 @@ class ObjectiveSpec:
                                  f"{allowed_where}")
         # noise: element occurrences are the column entries d[kVectors + k] (after the data vectors'), occurrences in `value` the
         # row's draws in finish (evok_sampler.cuh: DataCols::draw4, value_rand / value_randn)
-        n_vectors = sum(1 for v in self.kinds.values() if v)
-        self.element_draws = _Draws("the element terms", lambda k, name: f"d[{n_vectors + k}]")
+        self.element_draws = _Draws("the element terms", lambda k, name: f"d[{len(vectors) + k}]")
         self.value_draws = _Draws("`value`", lambda k, name: f"evok::value_{name}(key, sw, row, {MAX_DRAWS + k})")
-        self.running_terms = {c: _parse(t, {k: v for k, v in term_names.items() if k != "xn"}, f"running[{c!r}]")
-                              for c, t in running.items()}
+        self.running_terms = {c: _translate(tree, {k: v for k, v in term_names.items() if k != "xn"}, f"running[{c!r}]")
+                              for c, (tree, _) in running_trees.items()}
         for c, e in self.running_terms.items():
-            m = re.search(r"\bvn_(\w+)\b", e.cuda)
-            if m:
-                raise ValueError(f"running[{c!r}]: {m.group(1)}_n is the entry at column j + 1, which only a pair term has")
+            n = next_entry(e)
+            if n:
+                raise ValueError(f"running[{c!r}]: {n}_n is the entry at column j + 1, which only a pair term has")
         run_names = dict(term_names, **{c: f"r[{i}]" for i, c in enumerate(running)})
-        for s, t in texts.items():
-            used = _names_used(t)
+        term_trees = {s: _parse(t, f"{GROUP_OF[self.reductions[s]]}[{s!r}]") for s, t in texts.items()}
+        for s, (_, used) in term_trees.items():
             self._check_data_names(used, f"{GROUP_OF[self.reductions[s]]}[{s!r}]", term=True)
             if used & set(running) and "xn" in used:
                 raise ValueError(f"{GROUP_OF[self.reductions[s]]}[{s!r}]: {sorted(used & set(running))[0]!r} in a pair term; "
                                  f"{allowed_where}")
-        used = _names_used(value)
+        value_tree, used = _parse(value, "value")
         self._check_data_names(used, "value", term=False)
         if used & set(running):
             raise ValueError(f"value: {sorted(used & set(running))[0]!r} is a running sum; {allowed_where}")
-        self.terms = {s: _parse(t, run_names, f"{GROUP_OF[self.reductions[s]]}[{s!r}]", None if "xn" in _names_used(t) else self.element_draws)
-                      for s, t in texts.items()}
-        self.pairs = frozenset(s for s, e in self.terms.items() if re.search(r"\bxn\b", e.cuda))
+        # a term that reads xn is a pair term, where rand() / randn() are refused
+        self.terms = {s: _translate(tree, run_names, f"{GROUP_OF[self.reductions[s]]}[{s!r}]", None if "xn" in used else self.element_draws)
+                      for s, (tree, used) in term_trees.items()}
+        self.pairs = frozenset(s for s, e in self.terms.items() if "xn" in e.names)
         for s, e in self.terms.items():
-            m = re.search(r"\bvn_(\w+)\b", e.cuda)
-            if m and s not in self.pairs:
-                raise ValueError(f"{GROUP_OF[self.reductions[s]]}[{s!r}]: {m.group(1)}_n is the entry of {m.group(1)!r} at column j + 1, "
-                                 f"which only a pair term (one that uses xn) has; an element term uses {m.group(1)!r}")
-        self.value_expr = _parse(value, value_names, "value", self.value_draws)
+            n = next_entry(e)
+            if n and s not in self.pairs:
+                raise ValueError(f"{GROUP_OF[self.reductions[s]]}[{s!r}]: {n}_n is the entry of {n!r} at column j + 1, "
+                                 f"which only a pair term (one that uses xn) has; an element term uses {n!r}")
+        self.value_expr = _translate(value_tree, value_names, "value", self.value_draws)
         self.noisy = bool(self.element_draws.normal or self.value_draws.normal)
         self.source = self._cuda_source()
 
@@ -380,7 +384,7 @@ class ObjectiveSpec:
 
     def _cuda_source(self) -> str:
         k = range(len(self.terms))
-        uses_j = lambda es: any(re.search(r"\bjf\b", e.cuda) for e in es)  # noqa: E731
+        uses_j = lambda es: any("j" in e.names for e in es)  # noqa: E731
         element = [(i, e) for i, (s, e) in zip(k, self.terms.items()) if s not in self.pairs]
         pair = [(i, e) for i, (s, e) in zip(k, self.terms.items()) if s in self.pairs]
         ops = [self.reductions[s] for s in self.terms]
@@ -390,9 +394,8 @@ class ObjectiveSpec:
         nd = len(self.element_draws.normal)
         nv = max(len(vectors) + nd, 1)  # the column entries of a fold: data vectors, then element draws
 
-        def entries(es, prefix, array):  # the locals of the vector entries that the terms `es` use
-            return [f"    const float {prefix}_{n} = {array}[{i}];" for i, n in enumerate(vectors)
-                    if any(re.search(rf"\b{prefix}_{n}\b", e.cuda) for _, e in es)]
+        def entries(es, prefix, array, suffix=""):  # the locals of the vector entries that the terms `es` read (name + suffix)
+            return [f"    const float {prefix}_{n} = {array}[{i}];" for i, n in enumerate(vectors) if any(n + suffix in e.names for _, e in es)]
 
         def combine(i, e):  # slot i folds the term e with its reduction's operation
             return {"sum": f"    s{i} += {e};", "prod": f"    s{i} *= {e};", "max": f"    s{i} = evok::max_nan(s{i}, {e});",
@@ -451,7 +454,7 @@ class ObjectiveSpec:
                 lines.append("  __device__ __forceinline__ void add_pair(float x, float xn, int64_t j) {")
             if uses_j(e for _, e in pair):
                 lines.append("    const float jf = (float)j;")
-            lines += entries(pair, "v", "d") + entries(pair, "vn", "dn")
+            lines += entries(pair, "v", "d") + entries(pair, "vn", "dn", "_n")
             lines += [combine(i, e.cuda) for i, e in pair]
             lines.append("  }")
         if self.noisy:
