@@ -90,6 +90,15 @@ _SIGNATURES = {
     "evok_gemm_nt_affine": (c_int, [_P, c_int64, _P, c_int64, c_int64, c_int64, c_int64, _P, c_int64, _P, _P, c_int64, _P, _P, c_size_t, _P]),
     "evok_transpose_pair": (c_int, [_P, c_int64, c_int64, c_int64, _P, _P, _P, c_int64, _P]),
     "evok_transpose_scale": (c_int, [_P, c_int64, c_int64, c_int64, _P, _P, c_int64, _P]),
+    "evok_gemm_nt_batched_workspace_bytes": (c_size_t, [_P, c_int64, c_int64, _P, c_int64, c_int64, c_int64, c_int64, c_int64, c_int64]),
+    "evok_gemm_nt_batched": (c_int, [_P, c_int64, c_int64, _P, c_int64, c_int64, c_int64, c_int64, c_int64, c_int64, _P, c_int64, c_int64, _P, c_int64,
+                                     c_int64, _P, c_int64, _P, c_int64, _P, c_size_t, _P]),
+    "evok_gemm_nt_affine_batched": (c_int, [_P, c_int64, c_int64, _P, c_int64, c_int64, c_int64, c_int64, c_int64, c_int64, _P, c_int64, c_int64, _P,
+                                            c_int64, _P, c_int64, c_int64, _P, c_int64, _P, c_size_t, _P]),
+    "evok_transpose_pair_batched": (c_int, [_P, c_int64, c_int64, c_int64, c_int64, _P, c_int64, _P, _P, c_int64, c_int64, c_int64, _P]),
+    "evok_rank_table_batched": (c_int, [_P, c_int64, c_int64, c_int, _P, _P, _P, c_size_t, _P]),
+    "evok_cmaes_row_weights_batched": (c_int, [_P, _P, c_int64, c_int64, c_int64, c_int64, c_int64, c_int, _P, _P, _P]),
+    "evok_cmaes_vector_update_batched": (c_int, [_P, _P, c_int64, c_int64, _P, _P, _P, _P, c_int64, _P, c_int, _P, _P]),
     "evok_peer_alloc": (c_int, [c_size_t, _P, _P]),
     "evok_peer_open": (c_int, [_P, _P]),
     "evok_peer_close": (c_int, [_P]),

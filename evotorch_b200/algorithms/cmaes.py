@@ -24,7 +24,7 @@ from __future__ import annotations
 
 import math
 import os
-from typing import Optional, Tuple
+from typing import NamedTuple, Optional, Tuple
 
 import numpy as np
 import torch
@@ -42,6 +42,84 @@ def _safe_divide(a, b):
     return a / b
 
 
+class CMAESHyperparameters(NamedTuple):
+    """The recombination weights and learning rates of a CMA-ES search (see `cmaes_hyperparameters`)."""
+
+    popsize: int
+    mu: int
+    weights: torch.Tensor
+    weights_sum: float
+    mu_eff: float
+    c_m: float
+    c_sigma: float
+    damp_sigma: float
+    c_c: float
+    c_1: float
+    c_mu: float
+    variance_discount_sigma: float
+    variance_discount_c: float
+    unbiased_expectation: float
+    decompose_C_freq: int
+
+
+def cmaes_hyperparameters(d: int, popsize: Optional[int], *, dtype: torch.dtype, device, c_m: float = 1.0, c_sigma: Optional[float] = None,
+                          c_sigma_ratio: float = 1.0, damp_sigma: Optional[float] = None, damp_sigma_ratio: float = 1.0, c_c: Optional[float] = None,
+                          c_c_ratio: float = 1.0, c_1: Optional[float] = None, c_1_ratio: float = 1.0, c_mu: Optional[float] = None,
+                          c_mu_ratio: float = 1.0, active: bool = True, separable: bool = False,
+                          limit_C_decomposition: bool = True) -> CMAESHyperparameters:
+    """Default population size, recombination weights and learning rates of CMA-ES for solution length `d` (cmaes.py:270-385 of the
+    reference): host scalars in float64, the weight vector in `dtype` on `device`.  `CMAES` and the functional `cmaes` both take them
+    from here."""
+    if not popsize:
+        popsize = 4 + int(np.floor(3 * np.log(d)))  # cmaes.py:270-272
+    popsize = int(popsize)
+    mu = int(np.floor(popsize / 2))
+    raw_weights = torch.as_tensor(np.log((popsize + 1) / 2) - torch.log(torch.arange(popsize) + 1), dtype=dtype, device=device)
+    positive, negative = raw_weights[:mu], raw_weights[mu:]
+    mu_eff = float(torch.sum(positive).pow(2.0) / torch.sum(positive.pow(2.0)))
+    if c_sigma is None:
+        c_sigma = (mu_eff + 2.0) / (d + mu_eff + 3)
+    c_sigma = c_sigma_ratio * c_sigma
+    if damp_sigma is None:
+        damp_sigma = 1 + 2 * max(0.0, math.sqrt((mu_eff - 1) / (d + 1)) - 1) + c_sigma
+    damp_sigma = damp_sigma_ratio * damp_sigma
+    if c_c is None:
+        if separable:
+            c_c = (1 + (1 / d) + (mu_eff / d)) / (d**0.5 + (1 / d) + 2 * (mu_eff / d))
+        else:
+            c_c = (4 + mu_eff / d) / (d + (4 + 2 * mu_eff / d))
+    c_c = c_c_ratio * c_c
+    if c_1 is None:
+        if separable:
+            c_1 = 1.0 / (d + 2.0 * np.sqrt(d) + mu_eff / d)
+        else:
+            c_1 = min(1, popsize / 6) * 2 / ((d + 1.3) ** 2.0 + mu_eff)
+    c_1 = float(c_1_ratio * c_1)
+    if c_mu is None:
+        if separable:
+            c_mu = (0.25 + mu_eff + (1.0 / mu_eff) - 2) / (d + 4 * np.sqrt(d) + (mu_eff / 2.0))
+        else:
+            c_mu = min(1 - c_1, 2 * ((0.25 + mu_eff - 2 + (1 / mu_eff)) / ((d + 2) ** 2.0 + mu_eff)))
+    c_mu = float(c_mu_ratio * c_mu)
+    positive = positive / torch.sum(positive)
+    if active:
+        mu_eff_neg = float(torch.sum(negative).pow(2.0) / torch.sum(negative.pow(2.0)))
+        alpha = min(1 + c_1 / c_mu, 1 + 2 * mu_eff_neg / (mu_eff + 2), (1 - c_mu - c_1) / (d * c_mu))
+        negative = alpha * negative / torch.sum(torch.abs(negative))
+    else:
+        negative = torch.zeros_like(negative)
+    weights = torch.cat([positive, negative], dim=-1)
+    if limit_C_decomposition:
+        decompose_C_freq = max(1, int(np.floor(_safe_divide(1, 10 * d * (c_1 + c_mu)))))
+    else:
+        decompose_C_freq = 1
+    return CMAESHyperparameters(popsize=popsize, mu=mu, weights=weights, weights_sum=float(torch.sum(weights)), mu_eff=mu_eff, c_m=c_m,
+                                c_sigma=c_sigma, damp_sigma=damp_sigma, c_c=c_c, c_1=c_1, c_mu=c_mu,
+                                variance_discount_sigma=math.sqrt(c_sigma * (2 - c_sigma) * mu_eff),
+                                variance_discount_c=math.sqrt(c_c * (2 - c_c) * mu_eff),
+                                unbiased_expectation=np.sqrt(d) * (1 - (1 / (4 * d)) + 1 / (21 * d**2)), decompose_C_freq=decompose_C_freq)
+
+
 class CMAES(SearchAlgorithm, SinglePopulationAlgorithmMixin, CUDAGraphMixin):
     def __init__(self, problem: Problem, *, stdev_init, popsize: Optional[int] = None, center_init=None, c_m: float = 1.0,
                  c_sigma: Optional[float] = None, c_sigma_ratio: float = 1.0, damp_sigma: Optional[float] = None,
@@ -54,10 +132,13 @@ class CMAES(SearchAlgorithm, SinglePopulationAlgorithmMixin, CUDAGraphMixin):
         problem.ensure_unbounded()
         self._obj_index = problem.normalize_obj_index(obj_index)
         d = problem.solution_length
-        if not popsize:
-            popsize = 4 + int(np.floor(3 * np.log(d)))  # cmaes.py:270-272
-        self.popsize = int(popsize)
-        self.mu = int(np.floor(popsize / 2))
+        # weights and learning rates (cmaes.py:270-385)
+        hp = cmaes_hyperparameters(d, popsize, dtype=problem.dtype, device=problem.device, c_m=c_m, c_sigma=c_sigma, c_sigma_ratio=c_sigma_ratio,
+                                   damp_sigma=damp_sigma, damp_sigma_ratio=damp_sigma_ratio, c_c=c_c, c_c_ratio=c_c_ratio, c_1=c_1,
+                                   c_1_ratio=c_1_ratio, c_mu=c_mu, c_mu_ratio=c_mu_ratio, active=active, separable=separable,
+                                   limit_C_decomposition=limit_C_decomposition)
+        popsize = self.popsize = hp.popsize
+        self.mu = hp.mu
         self.separable = bool(separable)
         if self.separable and problem.lazy_population:
             # the fused separable generation never reads the population back, so it can stay a function of the Philox counters.
@@ -87,57 +168,13 @@ class CMAES(SearchAlgorithm, SinglePopulationAlgorithmMixin, CUDAGraphMixin):
             self.C = problem.make_I(d)
             self.A = self.C.clone()
 
-        # weights and learning rates (cmaes.py:300-385); host scalars in float64, the weight vector in the problem dtype
-        raw_weights = problem.make_tensor(np.log((popsize + 1) / 2) - torch.log(torch.arange(popsize) + 1))
-        positive, negative = raw_weights[: self.mu], raw_weights[self.mu:]
-        self.mu_eff = float(torch.sum(positive).pow(2.0) / torch.sum(positive.pow(2.0)))
-        self.c_m, self.active, self.csa_squared = c_m, bool(active), bool(csa_squared)
+        self.mu_eff, self.c_m, self.c_sigma, self.damp_sigma, self.c_c = hp.mu_eff, hp.c_m, hp.c_sigma, hp.damp_sigma, hp.c_c
+        self.c_1, self.c_mu, self.variance_discount_sigma, self.variance_discount_c = hp.c_1, hp.c_mu, hp.variance_discount_sigma, hp.variance_discount_c
+        self.weights, self._weights_sum, self.unbiased_expectation, self.decompose_C_freq = hp.weights, hp.weights_sum, hp.unbiased_expectation, hp.decompose_C_freq
+        self.active, self.csa_squared = bool(active), bool(csa_squared)
         self.stdev_min, self.stdev_max = stdev_min, stdev_max
-        mu_eff = self.mu_eff
-        if c_sigma is None:
-            c_sigma = (mu_eff + 2.0) / (d + mu_eff + 3)
-        self.c_sigma = c_sigma_ratio * c_sigma
-        if damp_sigma is None:
-            damp_sigma = 1 + 2 * max(0.0, math.sqrt((mu_eff - 1) / (d + 1)) - 1) + self.c_sigma
-        self.damp_sigma = damp_sigma_ratio * damp_sigma
-        if c_c is None:
-            if separable:
-                c_c = (1 + (1 / d) + (mu_eff / d)) / (d**0.5 + (1 / d) + 2 * (mu_eff / d))
-            else:
-                c_c = (4 + mu_eff / d) / (d + (4 + 2 * mu_eff / d))
-        self.c_c = c_c_ratio * c_c
-        if c_1 is None:
-            if separable:
-                c_1 = 1.0 / (d + 2.0 * np.sqrt(d) + mu_eff / d)
-            else:
-                c_1 = min(1, popsize / 6) * 2 / ((d + 1.3) ** 2.0 + mu_eff)
-        self.c_1 = float(c_1_ratio * c_1)
-        if c_mu is None:
-            if separable:
-                c_mu = (0.25 + mu_eff + (1.0 / mu_eff) - 2) / (d + 4 * np.sqrt(d) + (mu_eff / 2.0))
-            else:
-                c_mu = min(1 - self.c_1, 2 * ((0.25 + mu_eff - 2 + (1 / mu_eff)) / ((d + 2) ** 2.0 + mu_eff)))
-        self.c_mu = float(c_mu_ratio * c_mu)
-        self.variance_discount_sigma = math.sqrt(self.c_sigma * (2 - self.c_sigma) * mu_eff)
-        self.variance_discount_c = math.sqrt(self.c_c * (2 - self.c_c) * mu_eff)
-
-        positive = positive / torch.sum(positive)
-        if self.active:
-            mu_eff_neg = float(torch.sum(negative).pow(2.0) / torch.sum(negative.pow(2.0)))
-            alpha = min(1 + self.c_1 / self.c_mu, 1 + 2 * mu_eff_neg / (mu_eff + 2), (1 - self.c_mu - self.c_1) / (d * self.c_mu))
-            negative = alpha * negative / torch.sum(torch.abs(negative))
-        else:
-            negative = torch.zeros_like(negative)
-        self.weights = torch.cat([positive, negative], dim=-1)
-        self._weights_sum = float(torch.sum(self.weights))
-
         self.p_sigma = problem.make_zeros(d)
         self.p_c = problem.make_zeros(d)
-        self.unbiased_expectation = np.sqrt(d) * (1 - (1 / (4 * d)) + 1 / (21 * d**2))
-        if limit_C_decomposition:
-            self.decompose_C_freq = max(1, int(np.floor(_safe_divide(1, 10 * d * (self.c_1 + self.c_mu)))))
-        else:
-            self.decompose_C_freq = 1
         CUDAGraphMixin.__init__(self)
         SinglePopulationAlgorithmMixin.__init__(self)
 

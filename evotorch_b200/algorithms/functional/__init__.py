@@ -7,6 +7,13 @@
         state = pgpe_tell(state, population, f(population))
     best_guess = state.optimizer_state.center
 
+Full-covariance CMA-ES over a batch of independent searches (one launch per stage for all of them on CUDA float32):
+
+    state = cmaes(center_init=torch.randn(1024, 32, device="cuda"), stdev_init=1.0, objective_sense="min")
+    for _ in range(generations):
+        population = cmaes_ask(state)                        # (1024, popsize, 32)
+        state = cmaes_tell(state, population, f(population))
+
 With an objective that has a fused kernel, `pgpe_ask_and_evaluate` / `cem_ask_and_evaluate` sample and evaluate all batch items
 in one launch, and with `lazy=True` never store the population:
 
@@ -17,11 +24,12 @@ in one launch, and with `lazy=True` never store the population:
 from .funcadam import AdamState, adam, adam_ask, adam_tell
 from .funccem import CEMState, cem, cem_ask, cem_ask_and_evaluate, cem_tell
 from .funcclipup import ClipUpState, clipup, clipup_ask, clipup_tell
+from .funccmaes import CMAESState, cmaes, cmaes_ask, cmaes_tell
 from .funcpgpe import PGPEState, pgpe, pgpe_ask, pgpe_ask_and_evaluate, pgpe_tell
 from .fused import LazyPopulation
 from .funcsgd import SGDState, sgd, sgd_ask, sgd_tell
 from .misc import OptimizerFunctions, get_functional_optimizer
 
 __all__ = ["AdamState", "adam", "adam_ask", "adam_tell", "CEMState", "cem", "cem_ask", "cem_ask_and_evaluate", "cem_tell", "ClipUpState",
-           "clipup", "clipup_ask", "clipup_tell", "LazyPopulation", "PGPEState", "pgpe", "pgpe_ask", "pgpe_ask_and_evaluate", "pgpe_tell",
+           "clipup", "clipup_ask", "clipup_tell", "CMAESState", "cmaes", "cmaes_ask", "cmaes_tell", "LazyPopulation", "PGPEState", "pgpe", "pgpe_ask", "pgpe_ask_and_evaluate", "pgpe_tell",
            "SGDState", "sgd", "sgd_ask", "sgd_tell", "OptimizerFunctions", "get_functional_optimizer"]

@@ -6,16 +6,23 @@
 //                            reweighting  w_i > 0 ? w_i : d * w_i / ||z_i||^2   (cmaes.py:468-475, :531-535); one pass over Z
 //   evok_cmaes_vector_update D-vectors + scalars, one CTA: m, p_sigma, sigma, h_sig, p_c and the three coefficients of the
 //                            covariance update consumed by evok_gemm_nt_affine (cmaes.py:454-517, :31-46, :537-545)
+// The *_batched entry points run the same kernels for a batch of independent searches: grid y (row weights) or grid x (vector
+// update) is the item, so every item gets the bits of the single call on its operands.
 #include "evok_common.cuh"
 
 namespace evok {
 
-// one warp per row: ||z_i||^2, then the two weight vectors
+// one warp per row: ||z_i||^2, then the two weight vectors.  grid y = item: Z at item stride item_stride_z, aw / w_pos / w_act at N
 __global__ void __launch_bounds__(256) cmaes_row_weights_kernel(const float* __restrict__ aw, const float* __restrict__ Z, int64_t ldz, int64_t N,
-                                                                int64_t D, int active, float* __restrict__ w_pos, float* __restrict__ w_act) {
+                                                                int64_t D, int active, float* __restrict__ w_pos, float* __restrict__ w_act,
+                                                                int64_t item_stride_z) {
   const int lane = threadIdx.x & 31;
   const int64_t row = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
   if (row >= N) return;
+  Z += blockIdx.y * item_stride_z;
+  aw += blockIdx.y * N;
+  w_pos += blockIdx.y * N;
+  w_act += blockIdx.y * N;
   const float a = aw[row];
   float out_act = a;
   if (active && !(a > 0.0f)) {  // only the non-positive weights need the row norm (cmaes.py:532)
@@ -88,11 +95,20 @@ __device__ __forceinline__ CmaVectorStep cma_vector_step(const float* __restrict
   return CmaVectorStep{new_sigma, h, steps};
 }
 
+// one CTA per item (grid x): the D-vectors of item b at b * D, its sigma at b, its k_out at 3 b (steps_dev / h_sig_out: single call only)
 __global__ void __launch_bounds__(kCmaThreads)
     cmaes_vector_update_kernel(const float* __restrict__ local_disp, const float* __restrict__ shaped_disp, int64_t D, float* __restrict__ m,
                                float* __restrict__ p_sigma, float* __restrict__ p_c, float* __restrict__ sigma, long long* steps_dev,
                                long long steps_host, const __grid_constant__ CmaesConsts c, float* __restrict__ k_out, float* __restrict__ h_sig_out) {
   __shared__ double sm[33];
+  const int64_t off = (int64_t)blockIdx.x * D;
+  local_disp += off;
+  shaped_disp += off;
+  m += off;
+  p_sigma += off;
+  p_c += off;
+  sigma += blockIdx.x;
+  k_out += 3 * (int64_t)blockIdx.x;
   const CmaVectorStep v = cma_vector_step<false>(local_disp, shaped_disp, nullptr, D, m, p_sigma, p_c, sigma, steps_dev, steps_host, c, sm, nullptr);
   const float new_sigma = v.new_sigma, h = v.h;
   const long long steps = v.steps;
@@ -159,9 +175,21 @@ extern "C" EVOK_API int evok_cmaes_row_weights(const float* assigned_weights, co
                                                float* w_positive, float* w_active, void* stream) {
   if (!assigned_weights || !Z || !w_positive || !w_active) return EVOK_E_NULLPTR;
   if (N <= 0 || D <= 0 || ldz < D) return EVOK_E_BADSIZE;
-  cmaes_row_weights_kernel<<<(unsigned)((N + 7) / 8), 256, 0, (cudaStream_t)stream>>>(assigned_weights, Z, ldz, N, D, active, w_positive, w_active);
+  cmaes_row_weights_kernel<<<(unsigned)((N + 7) / 8), 256, 0, (cudaStream_t)stream>>>(assigned_weights, Z, ldz, N, D, active, w_positive, w_active, 0);
   EVOK_CHECK_LAUNCH();
   return 0;
+}
+
+extern "C" EVOK_API int evok_cmaes_row_weights_batched(const float* assigned_weights, const float* Z, int64_t item_stride_z, int64_t ldz, int64_t n_items,
+                                                       int64_t N, int64_t D, int active, float* w_positive, float* w_active, void* stream) {
+  if (!assigned_weights || !Z || !w_positive || !w_active) return EVOK_E_NULLPTR;
+  if (n_items < 0 || N <= 0 || D <= 0 || ldz < D || item_stride_z < 0) return EVOK_E_BADSIZE;
+  return for_item_chunks(n_items, kMaxGridY, [&](int64_t b0, int64_t nb) {
+    cmaes_row_weights_kernel<<<dim3((unsigned)((N + 7) / 8), (unsigned)nb), 256, 0, (cudaStream_t)stream>>>(
+        assigned_weights + b0 * N, Z + b0 * item_stride_z, ldz, N, D, active, w_positive + b0 * N, w_active + b0 * N, item_stride_z);
+    EVOK_CHECK_LAUNCH();
+    return 0;
+  });
 }
 
 static CmaesConsts cmaes_consts(const float* consts_host, int csa_squared) {
@@ -184,6 +212,22 @@ extern "C" EVOK_API int evok_cmaes_vector_update(const float* local_disp, const 
                                                                          h_sig_out);
   EVOK_CHECK_LAUNCH();
   return 0;
+}
+
+extern "C" EVOK_API int evok_cmaes_vector_update_batched(const float* local_disp, const float* shaped_disp, int64_t n_items, int64_t D, float* m,
+                                                         float* p_sigma, float* p_c, float* sigma_dev, int64_t steps_host, const float* consts_host,
+                                                         int csa_squared, float* k_out, void* stream) {
+  if (!local_disp || !shaped_disp || !m || !p_sigma || !p_c || !sigma_dev || !consts_host || !k_out) return EVOK_E_NULLPTR;
+  if (n_items < 0 || D <= 0) return EVOK_E_BADSIZE;
+  const CmaesConsts c = cmaes_consts(consts_host, csa_squared);
+  return for_item_chunks(n_items, (int64_t)INT32_MAX, [&](int64_t b0, int64_t nb) {
+    const int64_t off = b0 * D;
+    cmaes_vector_update_kernel<<<(unsigned)nb, kCmaThreads, 0, (cudaStream_t)stream>>>(local_disp + off, shaped_disp + off, D, m + off, p_sigma + off,
+                                                                                      p_c + off, sigma_dev + b0, nullptr, (long long)steps_host, c,
+                                                                                      k_out + 3 * b0, nullptr);
+    EVOK_CHECK_LAUNCH();
+    return 0;
+  });
 }
 
 extern "C" EVOK_API int evok_sepcma_update(const float* local_disp, const float* S2, const float* wsum, int64_t D, float* m, float* p_sigma, float* p_c,

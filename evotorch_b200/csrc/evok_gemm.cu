@@ -66,6 +66,12 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, i
                "l"(reinterpret_cast<uint64_t>(map)), "r"(x), "r"(y), "r"(s32(bar))
                : "memory");
 }
+// rank-3 map [items][rows][K] (batched GEMM): box depth 1, so a tile never reads the next item's rows
+__device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, int x, int y, int z, uint64_t* bar) {
+  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];" ::"r"(s32(dst)),
+               "l"(reinterpret_cast<uint64_t>(map)), "r"(x), "r"(y), "r"(z), "r"(s32(bar))
+               : "memory");
+}
 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -174,6 +180,10 @@ struct GemmParams {
   int row_act;
   int b_lo_tma;  // CONVERT: the lo tile of B comes from a pre-split copy (map_b_lo) instead of being derived by the converter warps
   int c_unit_fastest;  // persistent gather kernel: C[(batch * N + col) * rows_per_batch + row_in_batch]
+  // BATCHED: grid z = item (never a K split); split_stride is then C's item stride.  map_item_a / _b: 1 = the operand's map has one
+  // plane per item, 0 = one plane shared by all items.  The epilogue operands sit at these item strides (0 = shared).
+  int map_item_a, map_item_b;
+  int64_t c2_item_stride, alpha_item_stride, bias_item_stride, k_item_stride, e_item_stride, u_item_stride;
 };
 
 // The tensor core does not round its fp32 accumulation to nearest; over hundreds of MMAs that is a systematic drift of the
@@ -193,10 +203,11 @@ __device__ __noinline__ float gemm_act(float v, int act) {
 // GATHER (implies CONVERT): the A operand is not TMA-addressable (rows only 4-byte aligned, non-uniform pitch: the stacked first-layer
 // weights of a population of flat parameter vectors); the two converter warps fetch its tile with coalesced 128-byte row loads and
 // write BOTH the raw and the lo tile in the 128-byte-swizzled layout the tensor core expects, so the weights are read from HBM once.
-template <bool CONVERT, bool GATHER = false>
-__global__ void __launch_bounds__(kGemmThreads, 1)
-    gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
-                       const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo, const GemmParams p) {
+// BATCHED: independent products C_b = A_b B_b^T, item b = blockIdx.z, through rank-3 maps [items][rows][K] (rows past M / N zero-filled
+// per item); each item walks the whole K range in the order of a one-split single call, so it gets that call's bits.
+template <bool CONVERT, bool GATHER, bool BATCHED>
+__device__ __forceinline__ void gemm_tf32x3_body(const CUtensorMap& map_a_hi, const CUtensorMap& map_a_lo, const CUtensorMap& map_b_hi,
+                                                 const CUtensorMap& map_b_lo, const GemmParams p) {
   extern __shared__ unsigned char gemm_smem_raw[];
   // tiles need 1024-byte alignment (swizzle atom)
   unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(gemm_smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -207,9 +218,10 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
   const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;  // (uniform: keeps the wgmma path non-divergent)
   const int m0 = blockIdx.x * kGemmBM, n0 = blockIdx.y * kGemmBN;
   const int total_kb = (p.K + kGemmBK - 1) / kGemmBK;
-  const int kb_begin = blockIdx.z * p.kblocks_per_split;
+  const int kb_begin = BATCHED ? 0 : blockIdx.z * p.kblocks_per_split;
   const int kb_end = min(total_kb, kb_begin + p.kblocks_per_split);
   const int num_kb = max(kb_end - kb_begin, 0);
+  const int64_t item = BATCHED ? blockIdx.z : 0;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < kGemmStages; ++s) {
@@ -230,6 +242,14 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
         unsigned char* st = base + (size_t)s * kStageBytes;
         bar_expect_tx(&full[s], (GATHER ? kTileBBytes : (CONVERT ? kTileABytes + kTileBBytes : kStageBytes)) + ((CONVERT && p.b_lo_tma) ? kTileBBytes : 0u));
         const int kx = (kb_begin + i) * kGemmBK;
+        if (BATCHED) {
+          const int za = (int)item * p.map_item_a, zb = (int)item * p.map_item_b;
+          tma_load_3d(st, &map_a_hi, kx, m0, za, &full[s]);
+          if (!CONVERT) tma_load_3d(st + kTileABytes, &map_a_lo, kx, m0, za, &full[s]);
+          tma_load_3d(st + 2 * kTileABytes, &map_b_hi, kx, n0, zb, &full[s]);
+          if (!CONVERT) tma_load_3d(st + 2 * kTileABytes + kTileBBytes, &map_b_lo, kx, n0, zb, &full[s]);
+          continue;
+        }
         if (!GATHER) tma_load_2d(st, &map_a_hi, kx, m0, &full[s]);
         if (!CONVERT) tma_load_2d(st + kTileABytes, &map_a_lo, kx, m0, &full[s]);
         tma_load_2d(st + 2 * kTileABytes, &map_b_hi, kx, n0, &full[s]);
@@ -345,9 +365,14 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
       }
     }
     asm volatile("bar.sync 2, 256;" ::: "memory");
-    const float alpha = (p.C2 && p.alpha_dev) ? *p.alpha_dev : 1.0f;
-    const bool affine = p.affine_k != nullptr && gridDim.z == 1;
-    const float k0 = affine ? p.affine_k[0] : 1.0f, k1 = affine ? p.affine_k[1] : 0.0f, k2 = affine ? p.affine_k[2] : 0.0f;
+    const float alpha = (p.C2 && p.alpha_dev) ? p.alpha_dev[item * p.alpha_item_stride] : 1.0f;
+    const bool affine = p.affine_k != nullptr && (BATCHED || gridDim.z == 1);
+    const float* kk = p.affine_k + item * p.k_item_stride;
+    const float k0 = affine ? kk[0] : 1.0f, k1 = affine ? kk[1] : 0.0f, k2 = affine ? kk[2] : 0.0f;
+    const float* affine_E = p.affine_E ? p.affine_E + item * p.e_item_stride : nullptr;
+    const float* affine_u = p.affine_u ? p.affine_u + item * p.u_item_stride : nullptr;
+    const float* bias = p.bias ? p.bias + item * p.bias_item_stride : nullptr;
+    float* c2base = p.C2 ? p.C2 + item * p.c2_item_stride : nullptr;
     float* cbase = p.C + (int64_t)blockIdx.z * p.split_stride;
     const bool vec_ok = ((reinterpret_cast<uintptr_t>(cbase) & 15) == 0) && (p.ldc % 4 == 0);
     const int col = n0 + lane * 4;
@@ -364,11 +389,11 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
         for (int t = 0; t < 4; ++t) e[t] = p.row_act == EVOK_ACT_NONE ? e[t] + b : gemm_act(e[t] + b, p.row_act);
       }
       if (affine) {
-        const float ur = p.affine_u ? __ldg(p.affine_u + row) : 0.0f;
+        const float ur = affine_u ? __ldg(affine_u + row) : 0.0f;
         for (int t = 0; t < 4; ++t)
           if (col + t < p.N)
-            e[t] = fmaf(k0, e[t], fmaf(k1, p.affine_E ? p.affine_E[(int64_t)row * p.lde + col + t] : 0.0f,
-                                      k2 * ur * (p.affine_u ? __ldg(p.affine_u + col + t) : 0.0f)));
+            e[t] = fmaf(k0, e[t], fmaf(k1, affine_E ? affine_E[(int64_t)row * p.lde + col + t] : 0.0f,
+                                      k2 * ur * (affine_u ? __ldg(affine_u + col + t) : 0.0f)));
       }
       float* cp = cbase + (int64_t)row * p.ldc + col;
       if (vec_ok && col + 4 <= p.N) {
@@ -377,13 +402,27 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
         for (int t = 0; t < 4; ++t)
           if (col + t < p.N) cp[t] = e[t];
       }
-      if (p.C2) {
-        float* c2 = p.C2 + (int64_t)row * p.ldc2 + col;
+      if (c2base) {
+        float* c2 = c2base + (int64_t)row * p.ldc2 + col;
         for (int t = 0; t < 4; ++t)
-          if (col + t < p.N) c2[t] = fmaf(alpha, e[t], p.bias ? __ldg(p.bias + col + t) : 0.0f);
+          if (col + t < p.N) c2[t] = fmaf(alpha, e[t], bias ? __ldg(bias + col + t) : 0.0f);
       }
     }
   }
+}
+
+template <bool CONVERT, bool GATHER = false>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+    gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
+                       const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo, const GemmParams p) {
+  gemm_tf32x3_body<CONVERT, GATHER, false>(map_a_hi, map_a_lo, map_b_hi, map_b_lo, p);
+}
+
+template <bool CONVERT>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+    gemm_tf32x3_batched_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
+                               const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo, const GemmParams p) {
+  gemm_tf32x3_body<CONVERT, false, true>(map_a_hi, map_a_lo, map_b_hi, map_b_lo, p);
 }
 
 // ---- persistent gather GEMM (batched policy forward on ONE shared minibatch) ------------------------------------------------
@@ -758,13 +797,31 @@ __global__ void __launch_bounds__(256) reduce_splits_kernel(const float* __restr
   C[r * ldc + c] = acc;
 }
 
+// hi / lo split copies of a batch of operands: item b's rows x cols at x + b * item_stride (pitch ldx) -> [b][r][c] at pitch ldo
+__global__ void __launch_bounds__(256) split_tf32_items_kernel(const float* __restrict__ x, int64_t item_stride, int64_t ldx, int64_t rows,
+                                                               int64_t cols, float* __restrict__ hi, float* __restrict__ lo, int64_t ldo) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t b = blockIdx.y;
+  if (i >= rows * cols) return;
+  const int64_t r = i / cols, c = i % cols;
+  const float v = x[b * item_stride + r * ldx + c];
+  const float h = __uint_as_float(__float_as_uint(v) & 0xFFFFE000u);
+  hi[(b * rows + r) * ldo + c] = h;
+  lo[(b * rows + r) * ldo + c] = v - h;
+}
+
 // Operands of the weighted SYRK  S = Y^T diag(w) Y  as K-major matrices (K = the population axis), built in ONE pass over Y:
 //   out_w[c, r] = w[r] * Y[r, c]      out_p[c, r] = Y[r, c]          (32 x 32 tiles through shared memory)
+// grid z = item of a batch (strides in elements; 0 for a single operand)
 __global__ void __launch_bounds__(256) transpose_pair_kernel(const float* __restrict__ in, int64_t ldi, int64_t rows, int64_t cols,
                                                              const float* __restrict__ w, float* __restrict__ out_w, float* __restrict__ out_p,
-                                                             int64_t ldo) {
+                                                             int64_t ldo, int64_t item_stride_in, int64_t item_stride_w, int64_t item_stride_out) {
   __shared__ float tile[32][33];
   __shared__ float wrow[32];
+  in += blockIdx.z * item_stride_in;
+  w += blockIdx.z * item_stride_w;
+  out_w += blockIdx.z * item_stride_out;
+  out_p += blockIdx.z * item_stride_out;
   const int64_t r0 = (int64_t)blockIdx.y * 32, c0 = (int64_t)blockIdx.x * 32;
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;  // 32 x 8
   if (ty == 0) wrow[tx] = (r0 + tx < rows) ? w[r0 + tx] : 0.0f;
@@ -807,6 +864,19 @@ static int make_map(CUtensorMap* map, const float* ptr, int64_t rows, int64_t K,
   const cuuint32_t box[2] = {(cuuint32_t)kGemmBK, (cuuint32_t)box_rows};
   const cuuint32_t estr[2] = {1, 1};
   const CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? 0 : (int)cudaErrorInvalidValue;
+}
+
+// 3-D fp32 tensor [items][rows][K] (row pitch ld, item pitch item_ld floats); box = 32 floats x box_rows x 1 item; 128-byte swizzle
+static int make_map3(CUtensorMap* map, const float* ptr, int64_t items, int64_t rows, int64_t K, int64_t ld, int64_t item_ld, int box_rows) {
+  EncodeTiledFn enc = get_encode_fn();
+  if (!enc) return (int)cudaErrorNotSupported;
+  const cuuint64_t dims[3] = {(cuuint64_t)K, (cuuint64_t)rows, (cuuint64_t)items};
+  const cuuint64_t strides[2] = {(cuuint64_t)ld * sizeof(float), (cuuint64_t)item_ld * sizeof(float)};
+  const cuuint32_t box[3] = {(cuuint32_t)kGemmBK, (cuuint32_t)box_rows, 1};
+  const cuuint32_t estr[3] = {1, 1, 1};
+  const CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                          CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : (int)cudaErrorInvalidValue;
 }
@@ -908,7 +978,7 @@ static int gemm_impl(const float* A, int64_t lda, const float* B, int64_t ldb, i
     if ((rc = make_map(&mb_hi, b_hi, N, K, g.ldk, kGemmBN))) return rc;
     if ((rc = make_map(&mb_lo, b_lo, N, K, g.ldk, kGemmBN))) return rc;
   }
-  GemmParams p;
+  GemmParams p{};
   p.M = (int)M; p.N = (int)N; p.K = (int)K;
   p.kblocks_per_split = g.kblocks_per_split;
   const bool split = g.splits > 1;
@@ -960,6 +1030,157 @@ extern "C" EVOK_API int evok_gemm_nt_affine(const float* A, int64_t lda, const f
   if (!k_dev) return EVOK_E_NULLPTR;
   const GemmAffine aff{k_dev, E, lde, u};
   return gemm_impl(A, lda, B, ldb, M, N, K, C, ldc, nullptr, 0, nullptr, nullptr, &aff, ws, ws_bytes, stream);
+}
+
+// ---- batched products: C_b = A_b B_b^T for n_items items, item b = grid z ------------------------------------------------
+struct ItemOperand {
+  const float* ptr;
+  int64_t ld, item_stride;  // item_stride 0: one matrix shared by every item
+};
+
+// read by the GEMM itself through a rank-3 map (16-byte aligned base, row and item pitch, items that do not overlap), or not
+static bool tma_ok_items(const ItemOperand& o, int64_t rows) {
+  return tma_ok(o.ptr, o.ld) && (o.item_stride == 0 || (o.item_stride % 4 == 0 && o.item_stride >= rows * o.ld));
+}
+
+struct BatchedPlan {
+  bool convert;  // both operands by TMA straight from their own memory; else both from split copies in the workspace
+  int64_t ldk;
+  size_t off_a_lo, off_b_hi, off_b_lo, total;
+};
+
+static BatchedPlan plan_batched(const ItemOperand& a, const ItemOperand& b, int64_t n_items, int64_t M, int64_t N, int64_t K) {
+  BatchedPlan g{};
+  g.convert = tma_ok_items(a, M) && tma_ok_items(b, N);
+  g.ldk = round_up(K, 4);
+  if (g.convert) return g;
+  const int64_t chunk = n_items < kMaxGridY ? n_items : kMaxGridY;  // one chunk at a time reuses the copies
+  auto al = [](size_t x) { return (x + 1023) & ~(size_t)1023; };
+  const size_t a_bytes = al((size_t)(a.item_stride ? chunk : 1) * M * g.ldk * 4), b_bytes = al((size_t)(b.item_stride ? chunk : 1) * N * g.ldk * 4);
+  g.off_a_lo = a_bytes;
+  g.off_b_hi = 2 * a_bytes;
+  g.off_b_lo = 2 * a_bytes + b_bytes;
+  g.total = 2 * a_bytes + 2 * b_bytes;
+  return g;
+}
+
+// per-item epilogue operands and their item strides (0 = shared)
+struct ItemEpilogue {
+  float* C2;
+  int64_t ldc2, item_stride_c2;
+  const float* alpha;
+  int64_t item_stride_alpha;
+  const float* bias;
+  int64_t item_stride_bias;
+  const GemmAffine* aff;
+  int64_t item_stride_k, item_stride_e, item_stride_u;
+};
+
+static int gemm_batched_impl(const ItemOperand& a, const ItemOperand& b, int64_t n_items, int64_t M, int64_t N, int64_t K, float* C, int64_t ldc,
+                             int64_t item_stride_c, const ItemEpilogue& ep, void* ws, size_t ws_bytes, void* stream) {
+  const GemmAffine* aff = ep.aff;
+  if (!a.ptr || !b.ptr || !C || !ws) return EVOK_E_NULLPTR;
+  if (n_items < 0 || M <= 0 || N <= 0 || K <= 0 || a.ld < K || b.ld < K || ldc < N || (ep.C2 && ep.ldc2 < N)) return EVOK_E_BADSIZE;
+  if (M >= (1ll << 31) || N >= (1ll << 31) || K >= (1ll << 31)) return EVOK_E_BADSIZE;
+  if (a.item_stride < 0 || b.item_stride < 0 || ep.item_stride_alpha < 0 || ep.item_stride_bias < 0 || ep.item_stride_k < 0 || ep.item_stride_e < 0 ||
+      ep.item_stride_u < 0)
+    return EVOK_E_BADSIZE;
+  // the outputs belong to one item each
+  if (n_items > 1 && (item_stride_c < (M - 1) * ldc + N || (ep.C2 && ep.item_stride_c2 < (M - 1) * ep.ldc2 + N))) return EVOK_E_BADSIZE;
+  if (aff && (!aff->k || (aff->u && M != N) || (aff->E && aff->lde < N))) return EVOK_E_BADSIZE;
+  if (n_items == 0) return 0;
+  const BatchedPlan g = plan_batched(a, b, n_items, M, N, K);
+  char* w8 = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(ws) + 1023) & ~(uintptr_t)1023);
+  if (ws_bytes < g.total + (size_t)(w8 - (char*)ws)) return EVOK_E_WORKSPACE;
+  static bool attr_set = false;
+  if (!attr_set) {
+    if (cudaFuncSetAttribute(gemm_tf32x3_batched_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kGemmSmemBytes) != cudaSuccess ||
+        cudaFuncSetAttribute(gemm_tf32x3_batched_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kGemmSmemBytes) != cudaSuccess)
+      return (int)cudaGetLastError();
+    attr_set = true;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  return for_item_chunks(n_items, kMaxGridY, [&](int64_t b0, int64_t nb) {
+    const float* pa = a.ptr + b0 * a.item_stride;
+    const float* pb = b.ptr + b0 * b.item_stride;
+    const int64_t ia = a.item_stride ? nb : 1, ib = b.item_stride ? nb : 1;
+    CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
+    int rc;
+    if (g.convert) {
+      if ((rc = make_map3(&ma_hi, pa, ia, M, K, a.ld, a.item_stride ? a.item_stride : M * a.ld, kGemmBM))) return rc;
+      if ((rc = make_map3(&mb_hi, pb, ib, N, K, b.ld, b.item_stride ? b.item_stride : N * b.ld, kGemmBN))) return rc;
+      ma_lo = ma_hi;
+      mb_lo = mb_hi;
+    } else {
+      float* a_hi = (float*)w8;
+      float* a_lo = (float*)(w8 + g.off_a_lo);
+      float* b_hi = (float*)(w8 + g.off_b_hi);
+      float* b_lo = (float*)(w8 + g.off_b_lo);
+      split_tf32_items_kernel<<<dim3((unsigned)((M * K + 255) / 256), (unsigned)ia), 256, 0, st>>>(pa, a.item_stride, a.ld, M, K, a_hi, a_lo, g.ldk);
+      split_tf32_items_kernel<<<dim3((unsigned)((N * K + 255) / 256), (unsigned)ib), 256, 0, st>>>(pb, b.item_stride, b.ld, N, K, b_hi, b_lo, g.ldk);
+      EVOK_CHECK_LAUNCH_N(2);
+      if ((rc = make_map3(&ma_hi, a_hi, ia, M, K, g.ldk, M * g.ldk, kGemmBM))) return rc;
+      if ((rc = make_map3(&ma_lo, a_lo, ia, M, K, g.ldk, M * g.ldk, kGemmBM))) return rc;
+      if ((rc = make_map3(&mb_hi, b_hi, ib, N, K, g.ldk, N * g.ldk, kGemmBN))) return rc;
+      if ((rc = make_map3(&mb_lo, b_lo, ib, N, K, g.ldk, N * g.ldk, kGemmBN))) return rc;
+    }
+    GemmParams p{};
+    p.M = (int)M; p.N = (int)N; p.K = (int)K;
+    p.kblocks_per_split = (int)((K + kGemmBK - 1) / kGemmBK);  // never split K: the items fill the grid
+    p.C = C + b0 * item_stride_c;
+    p.ldc = ldc;
+    p.split_stride = item_stride_c;
+    p.C2 = ep.C2 ? ep.C2 + b0 * ep.item_stride_c2 : nullptr;
+    p.ldc2 = ep.ldc2;
+    p.c2_item_stride = ep.item_stride_c2;
+    p.alpha_dev = ep.alpha ? ep.alpha + b0 * ep.item_stride_alpha : nullptr;
+    p.alpha_item_stride = ep.item_stride_alpha;
+    p.bias = ep.bias ? ep.bias + b0 * ep.item_stride_bias : nullptr;
+    p.bias_item_stride = ep.item_stride_bias;
+    if (aff) {
+      p.affine_k = aff->k + b0 * ep.item_stride_k;
+      p.k_item_stride = ep.item_stride_k;
+      p.affine_E = aff->E ? aff->E + b0 * ep.item_stride_e : nullptr;
+      p.lde = aff->lde;
+      p.e_item_stride = ep.item_stride_e;
+      p.affine_u = aff->u ? aff->u + b0 * ep.item_stride_u : nullptr;
+      p.u_item_stride = ep.item_stride_u;
+    }
+    p.map_item_a = a.item_stride ? 1 : 0;
+    p.map_item_b = b.item_stride ? 1 : 0;
+    const dim3 grid((unsigned)((M + kGemmBM - 1) / kGemmBM), (unsigned)((N + kGemmBN - 1) / kGemmBN), (unsigned)nb);
+    if (g.convert) gemm_tf32x3_batched_kernel<true><<<grid, kGemmThreads, kGemmSmemBytes, st>>>(ma_hi, ma_lo, mb_hi, mb_lo, p);
+    else gemm_tf32x3_batched_kernel<false><<<grid, kGemmThreads, kGemmSmemBytes, st>>>(ma_hi, ma_lo, mb_hi, mb_lo, p);
+    EVOK_CHECK_LAUNCH();
+    return 0;
+  });
+}
+
+extern "C" EVOK_API size_t evok_gemm_nt_batched_workspace_bytes(const float* A, int64_t lda, int64_t item_stride_a, const float* B, int64_t ldb,
+                                                                int64_t item_stride_b, int64_t n_items, int64_t M, int64_t N, int64_t K) {
+  if (n_items <= 0 || M <= 0 || N <= 0 || K <= 0) return 1024;
+  return plan_batched(ItemOperand{A, lda, item_stride_a}, ItemOperand{B, ldb, item_stride_b}, n_items, M, N, K).total + 1024;
+}
+
+extern "C" EVOK_API int evok_gemm_nt_batched(const float* A, int64_t lda, int64_t item_stride_a, const float* B, int64_t ldb, int64_t item_stride_b,
+                                             int64_t n_items, int64_t M, int64_t N, int64_t K, float* C, int64_t ldc, int64_t item_stride_c, float* C2,
+                                             int64_t ldc2, int64_t item_stride_c2, const float* alpha_dev, int64_t item_stride_alpha, const float* bias,
+                                             int64_t item_stride_bias, void* ws, size_t ws_bytes, void* stream) {
+  const ItemEpilogue ep{C2, ldc2, item_stride_c2, alpha_dev, item_stride_alpha, bias, item_stride_bias, nullptr, 0, 0, 0};
+  return gemm_batched_impl(ItemOperand{A, lda, item_stride_a}, ItemOperand{B, ldb, item_stride_b}, n_items, M, N, K, C, ldc, item_stride_c, ep, ws,
+                           ws_bytes, stream);
+}
+
+extern "C" EVOK_API int evok_gemm_nt_affine_batched(const float* A, int64_t lda, int64_t item_stride_a, const float* B, int64_t ldb,
+                                                    int64_t item_stride_b, int64_t n_items, int64_t M, int64_t N, int64_t K, float* C, int64_t ldc,
+                                                    int64_t item_stride_c, const float* k_dev, int64_t item_stride_k, const float* E, int64_t lde,
+                                                    int64_t item_stride_e, const float* u, int64_t item_stride_u, void* ws, size_t ws_bytes,
+                                                    void* stream) {
+  if (!k_dev) return EVOK_E_NULLPTR;
+  const GemmAffine aff{k_dev, E, lde, u};
+  const ItemEpilogue ep{nullptr, 0, 0, nullptr, 0, nullptr, 0, &aff, item_stride_k, item_stride_e, item_stride_u};
+  return gemm_batched_impl(ItemOperand{A, lda, item_stride_a}, ItemOperand{B, ldb, item_stride_b}, n_items, M, N, K, C, ldc, item_stride_c, ep, ws,
+                           ws_bytes, stream);
 }
 
 // Stacked-rows GEMM of the batched policy forward:  C[(i, h), b] = act( sum_k W_i[h, k] * X[b, k] + bias_i[h] )
@@ -1069,9 +1290,26 @@ extern "C" EVOK_API int evok_transpose_pair(const float* in, int64_t ldi, int64_
   if (!in || !w || !out_w || !out_p) return EVOK_E_NULLPTR;
   if (rows <= 0 || cols <= 0 || ldi < cols || ldo < rows) return EVOK_E_BADSIZE;
   dim3 grid((unsigned)((cols + 31) / 32), (unsigned)((rows + 31) / 32));
-  transpose_pair_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(in, ldi, rows, cols, w, out_w, out_p, ldo);
+  transpose_pair_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(in, ldi, rows, cols, w, out_w, out_p, ldo, 0, 0, 0);
   EVOK_CHECK_LAUNCH();
   return 0;
+}
+
+extern "C" EVOK_API int evok_transpose_pair_batched(const float* in, int64_t ldi, int64_t item_stride_in, int64_t rows, int64_t cols, const float* w,
+                                                    int64_t item_stride_w, float* out_w, float* out_p, int64_t ldo, int64_t item_stride_out,
+                                                    int64_t n_items, void* stream) {
+  if (!in || !w || !out_w || !out_p) return EVOK_E_NULLPTR;
+  if (rows <= 0 || cols <= 0 || n_items < 0 || ldi < cols || ldo < rows || item_stride_in < 0 || item_stride_w < 0) return EVOK_E_BADSIZE;
+  if (n_items > 1 && item_stride_out < cols * ldo) return EVOK_E_BADSIZE;  // the outputs are per item
+  if ((rows + 31) / 32 > kMaxGridY) return EVOK_E_BADSIZE;
+  const dim3 tiles((unsigned)((cols + 31) / 32), (unsigned)((rows + 31) / 32));
+  return for_item_chunks(n_items, kMaxGridY, [&](int64_t b0, int64_t nb) {
+    transpose_pair_kernel<<<dim3(tiles.x, tiles.y, (unsigned)nb), 256, 0, (cudaStream_t)stream>>>(
+        in + b0 * item_stride_in, ldi, rows, cols, w + b0 * item_stride_w, out_w + b0 * item_stride_out, out_p + b0 * item_stride_out, ldo,
+        item_stride_in, item_stride_w, item_stride_out);
+    EVOK_CHECK_LAUNCH();
+    return 0;
+  });
 }
 
 extern "C" EVOK_API int evok_transpose_scale(const float* in, int64_t ldi, int64_t rows, int64_t cols, const float* w, float* out, int64_t ldo,

@@ -715,6 +715,15 @@ extern "C" EVOK_API int evok_rank_batched(int method, const float* f, int64_t N,
   return rank_rows(f, N, n_items, !higher_is_better, utilities(method, w, nullptr), ws, ws_bytes, st);
 }
 
+// n_items rank-table lookups (keys, out: [items][N]) with one shared table
+extern "C" EVOK_API int evok_rank_table_batched(const float* keys, int64_t N, int64_t n_items, int descending, const float* table, float* out, void* ws,
+                                                size_t ws_bytes, void* stream) {
+  if (!keys || !table || !out || !ws) return EVOK_E_NULLPTR;
+  if (N < 0 || N >= (int64_t)1 << 32 || n_items < 0) return EVOK_E_BADSIZE;
+  if (N == 0 || n_items == 0) return 0;
+  return rank_rows(keys, N, n_items, descending, table_entries(table, out), ws, ws_bytes, (cudaStream_t)stream);
+}
+
 extern "C" EVOK_API int evok_elite_mask_batched(const float* w, int64_t N, int64_t n_items, int64_t num_elites, float* mask, void* ws,
                                                 size_t ws_bytes, void* stream) {
   if (!w || !mask || !ws) return EVOK_E_NULLPTR;

@@ -854,3 +854,158 @@ def transpose_scale(X: torch.Tensor, w: Optional[torch.Tensor] = None) -> torch.
     nat.check(nat.lib().evok_transpose_scale(X.data_ptr(), X.stride(0), rows, cols, nat.ptr(w), out.data_ptr(), out.stride(0),
                                              nat.stream_of(X)), "evok_transpose_scale")
     return out
+
+
+# ------------------------------------------------------------------------------------------------ batched K6 / K7 and CMA-ES glue
+def _item_mat(t: torch.Tensor, name: str, core: tuple) -> tuple:
+    """(tensor, n_items or None, item stride, row pitch) of a row-major matrix operand of a batched product: shape `core` (shared
+    by every item: stride 0) or (items, *core) at any item stride."""
+    if not (t.is_cuda and t.dtype == torch.float32 and t.ndim in (2, 3) and tuple(t.shape[-2:]) == tuple(core)):
+        raise ValueError(f"{name}: expected a float32 CUDA tensor of shape {core} or (items, {core[0]}, {core[1]}), got {tuple(t.shape)} {t.dtype}")
+    if not (t.stride(-1) == 1 and t.stride(-2) >= core[1]):
+        raise ValueError(f"{name}: expected row-major rows (strides {t.stride()})")
+    t = as_plain_tensor(t)
+    if t.ndim == 2:
+        return t, None, 0, t.stride(0)
+    if t.shape[0] > 1 and t.stride(0) < 0:
+        raise ValueError(f"{name}: negative item stride")
+    return t, t.shape[0], t.stride(0) if t.shape[0] > 1 else 0, t.stride(1)
+
+
+def _item_vec(t: Optional[torch.Tensor], name: str, n: int, n_items: int) -> int:
+    """Item stride of a contiguous per-item vector operand: (n,) shared -> 0, (items, n) -> n (n = 1 also takes shape (items,))."""
+    if t is None:
+        return 0
+    if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()):
+        raise ValueError(f"{name}: expected a contiguous float32 CUDA tensor")
+    if t.numel() == n and (t.ndim <= 1 or t.shape[0] == 1):
+        return 0
+    if t.numel() == n * n_items and t.shape[0] == n_items:
+        return n
+    raise ValueError(f"{name}: expected {n} values shared by the items or {n_items} x {n}, got shape {tuple(t.shape)}")
+
+
+def _batch_count(*counts) -> int:
+    given = {c for c in counts if c is not None}
+    if len(given) > 1:
+        raise ValueError(f"operands disagree on the number of items: {sorted(given)}")
+    return given.pop() if given else 1
+
+
+def gemm_nt_batched(A: torch.Tensor, B: torch.Tensor, out: Optional[torch.Tensor] = None, *, out2: Optional[torch.Tensor] = None,
+                    alpha: Optional[torch.Tensor] = None, bias: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out[b] = A[b] @ B[b].T for every item in one launch per 65535 items (`gemm_nt`'s 3xTF32 kernel, item = grid z; per item the
+    bits of `gemm_nt` wherever its plan has one K split); optionally out2[b] = alpha[b] * out[b] + bias[b] (broadcast over rows).
+    A: (M, K) or (items, M, K), B: (N, K) or (items, N, K) -- a 2-D operand is shared by every item; alpha: 1 or (items,) values,
+    bias: (N,) or (items, N)."""
+    A, na, sa, lda = _item_mat(A, "A", tuple(A.shape[-2:]))
+    B, nb, sb, ldb = _item_mat(B, "B", tuple(B.shape[-2:]))
+    M, K = A.shape[-2:]
+    N, K2 = B.shape[-2:]
+    if K != K2:
+        raise ValueError(f"inner dimensions differ: {K} vs {K2}")
+    n_items = _batch_count(na, nb, None if out is None or out.ndim < 3 else out.shape[0], None if out2 is None or out2.ndim < 3 else out2.shape[0])
+    if out is None:
+        out = torch.empty(n_items, M, N, dtype=torch.float32, device=A.device)
+    out, _, sc, ldc = _item_mat(out, "out", (M, N))
+    sc2, ldc2 = 0, 0
+    if out2 is not None:
+        out2, _, sc2, ldc2 = _item_mat(out2, "out2", (M, N))
+    s_alpha = _item_vec(alpha, "alpha", 1, n_items)
+    s_bias = _item_vec(bias, "bias", N, n_items)
+    lib = nat.lib()
+    ws = nat.workspace(A.device, lib.evok_gemm_nt_batched_workspace_bytes(A.data_ptr(), lda, sa, B.data_ptr(), ldb, sb, n_items, M, N, K), "gemm_batched")
+    with _timed("gemm"):
+        rc = lib.evok_gemm_nt_batched(A.data_ptr(), lda, sa, B.data_ptr(), ldb, sb, n_items, M, N, K, out.data_ptr(), ldc, sc, nat.ptr(out2), ldc2, sc2,
+                                      nat.ptr(alpha), s_alpha, nat.ptr(bias), s_bias, ws.data_ptr(), ws.numel(), nat.stream_of(A))
+    nat.check(rc, "evok_gemm_nt_batched")
+    return out
+
+
+def gemm_nt_affine_batched(A: torch.Tensor, B: torch.Tensor, k: torch.Tensor, out: torch.Tensor, *, E: Optional[torch.Tensor] = None,
+                           u: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out[b] = k[b, 0] * A[b] @ B[b].T + k[b, 1] * E[b] + k[b, 2] * outer(u[b], u[b]) for every item (`E` may be `out`).
+    A / B as in `gemm_nt_batched`; k: (3,) or (items, 3); E: (M, N) or (items, M, N); u: (M,) or (items, M), needs M == N."""
+    A, na, sa, lda = _item_mat(A, "A", tuple(A.shape[-2:]))
+    B, nb, sb, ldb = _item_mat(B, "B", tuple(B.shape[-2:]))
+    M, K = A.shape[-2:]
+    N = B.shape[-2]
+    if B.shape[-1] != K:
+        raise ValueError(f"inner dimensions differ: {K} vs {B.shape[-1]}")
+    n_items = _batch_count(na, nb, out.shape[0] if out.ndim == 3 else None)
+    out, _, sc, ldc = _item_mat(out, "out", (M, N))
+    se, lde = 0, 0
+    if E is not None:
+        E, ne, se, lde = _item_mat(E, "E", (M, N))
+        _batch_count(n_items, ne)
+    sk = _item_vec(k, "k", 3, n_items)
+    su = _item_vec(u, "u", M, n_items)
+    lib = nat.lib()
+    ws = nat.workspace(A.device, lib.evok_gemm_nt_batched_workspace_bytes(A.data_ptr(), lda, sa, B.data_ptr(), ldb, sb, n_items, M, N, K), "gemm_batched")
+    with _timed("gemm"):
+        rc = lib.evok_gemm_nt_affine_batched(A.data_ptr(), lda, sa, B.data_ptr(), ldb, sb, n_items, M, N, K, out.data_ptr(), ldc, sc, k.data_ptr(), sk,
+                                             nat.ptr(E), lde, se, nat.ptr(u), su, ws.data_ptr(), ws.numel(), nat.stream_of(A))
+    nat.check(rc, "evok_gemm_nt_affine_batched")
+    return out
+
+
+def weighted_syrk_update_batched(Y: torch.Tensor, w: torch.Tensor, k: torch.Tensor, C: torch.Tensor, u: Optional[torch.Tensor] = None,
+                                 out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """`weighted_syrk_update` for every item: out[b] = k[b, 0] Y[b]^T diag(w[b]) Y[b] + k[b, 1] C[b] + k[b, 2] u[b] u[b]^T, as one
+    transposing pass over all Y[b] and one batched GEMM whose epilogue applies the update.  Y: (items, n, d), w: (items, n),
+    k: (items, 3), C: (items, d, d), u: (items, d).  `out` may be `C` (in place)."""
+    if not (Y.is_cuda and Y.dtype == torch.float32 and Y.ndim == 3):
+        raise ValueError("Y: expected a float32 CUDA tensor of shape (items, n, d)")
+    Y = as_plain_tensor(Y).contiguous()
+    B, n, d = Y.shape
+    w = _rows(w, "w", (B, n))
+    k = _rows(k, "k", (B, 3))
+    C, nc, _, _ = _item_mat(C, "C", (d, d))
+    _batch_count(B, nc)
+    if u is not None:
+        u = _rows(u, "u", (B, d))
+    out = torch.empty(B, d, d, dtype=torch.float32, device=Y.device) if out is None else out
+    ldo = (n + 3) // 4 * 4
+    lib = nat.lib()
+    a_w, a_p = torch.empty(2, B, d, ldo, dtype=torch.float32, device=Y.device)  # K-major operands, 16-byte aligned rows
+    nat.check(lib.evok_transpose_pair_batched(Y.data_ptr(), d, n * d, n, d, w.data_ptr(), n, a_w.data_ptr(), a_p.data_ptr(), ldo, d * ldo, B,
+                                              nat.stream_of(Y)), "evok_transpose_pair_batched")
+    return gemm_nt_affine_batched(a_w[:, :, :n], a_p[:, :, :n], k, out, E=C, u=u)
+
+
+def rank_table_batched(keys: torch.Tensor, descending: bool, table: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """`rank_table` for every row of keys (items, N) with one shared table (N,)."""
+    if not (keys.is_cuda and keys.dtype == torch.float32 and keys.ndim == 2):
+        raise ValueError("keys: expected a float32 CUDA tensor of shape (items, N)")
+    keys = as_plain_tensor(keys).contiguous()
+    B, n = keys.shape
+    _vec(table, "table", n)
+    out = torch.empty_like(keys) if out is None else _rows(out, "out", (B, n))
+    _rank_call("evok_rank_table_batched", keys, keys.data_ptr(), n, B, int(bool(descending)), table.data_ptr(), out.data_ptr())
+    return out
+
+
+def cmaes_row_weights_batched(assigned: torch.Tensor, Z: torch.Tensor, active: bool, w_pos: torch.Tensor, w_act: torch.Tensor) -> None:
+    """`cmaes_row_weights` for every item: assigned, w_pos, w_act (items, N); Z (items, N, D) with row-major rows."""
+    Z, nz, sz, ldz = _item_mat(Z, "Z", tuple(Z.shape[-2:]))
+    if nz is None:
+        raise ValueError("Z: expected shape (items, N, D)")
+    B, n, d = Z.shape
+    for t, name in ((assigned, "assigned"), (w_pos, "w_pos"), (w_act, "w_act")):
+        _rows(t, name, (B, n))
+    nat.check(nat.lib().evok_cmaes_row_weights_batched(assigned.data_ptr(), Z.data_ptr(), sz, ldz, B, n, d, int(bool(active)), w_pos.data_ptr(),
+                                                       w_act.data_ptr(), nat.stream_of(Z)), "evok_cmaes_row_weights_batched")
+
+
+def cmaes_vector_update_batched(local_disp: torch.Tensor, shaped_disp: torch.Tensor, m: torch.Tensor, p_sigma: torch.Tensor, p_c: torch.Tensor,
+                                sigma: torch.Tensor, consts, csa_squared: bool, k_out: torch.Tensor, *, steps: int) -> None:
+    """`cmaes_vector_update` for every item, one CTA each, in place: m, p_sigma, p_c, local / shaped (items, D), sigma (items,),
+    k_out (items, 3).  The 10 constants and the generation counter `steps` are shared."""
+    B, d = m.shape
+    for t, name in ((local_disp, "local_disp"), (shaped_disp, "shaped_disp"), (m, "m"), (p_sigma, "p_sigma"), (p_c, "p_c")):
+        _rows(t, name, (B, d))
+    _rows(sigma.view(B, 1) if sigma.numel() == B and sigma.is_contiguous() else sigma, "sigma", (B, 1))
+    _rows(k_out, "k_out", (B, 3))
+    nat.check(nat.lib().evok_cmaes_vector_update_batched(local_disp.data_ptr(), shaped_disp.data_ptr(), B, d, m.data_ptr(), p_sigma.data_ptr(),
+                                                         p_c.data_ptr(), sigma.data_ptr(), int(steps), _host_floats(consts, 10), int(bool(csa_squared)),
+                                                         k_out.data_ptr(), nat.stream_of(m)), "evok_cmaes_vector_update_batched")

@@ -370,6 +370,32 @@ int evok_transpose_scale(const float* in, int64_t ldi, int64_t rows, int64_t col
 int evok_transpose_pair(const float* in, int64_t ldi, int64_t rows, int64_t cols, const float* w, float* out_w, float* out_p, int64_t ldo,
                         void* stream);
 
+/* Batched K6 / K7: n_items independent products C_b = A_b B_b^T (M x N x K each) in one launch per 65535 items (grid z = item).
+ * Operand b of A is at A + b * item_stride_a (item_stride_a = 0: one A shared by every item), likewise B; C_b at C + b * item_stride_c
+ * (outputs are per item: item_stride_c >= (M - 1) ldc + N when n_items > 1).  A batched product never splits K, so every item is
+ * summed in the order of evok_gemm_nt with a one-split plan and gets its bits.  Operands with a 16-byte aligned base, row pitch and
+ * item pitch (and items that do not overlap) are read once by the GEMM through rank-3 tensor maps [items][rows][K] (rows past M / N
+ * read as zeros per item); otherwise both are first split into hi / lo copies in `ws`
+ * (evok_gemm_nt_batched_workspace_bytes, which takes the same operands).
+ *   evok_gemm_nt_batched        : optional C2_b = alpha_b * C_b + bias_b[col] with alpha at alpha_dev + b * item_stride_alpha and bias at
+ *                                 bias + b * item_stride_bias (0 = shared).  CMA-ES sampling x = m_b + sigma_b z A_b^T.
+ *   evok_gemm_nt_affine_batched : C_b = k_b[0] A_b B_b^T + k_b[1] E_b + k_b[2] u_b u_b^T with k_b, E_b, u_b at their item strides (E may
+ *                                 be C).  The CMA-ES covariance update of a batch of searches.
+ *   evok_transpose_pair_batched : evok_transpose_pair per item (in, w, out_w / out_p at their item strides; one launch per 65535 items). */
+size_t evok_gemm_nt_batched_workspace_bytes(const float* A, int64_t lda, int64_t item_stride_a, const float* B, int64_t ldb, int64_t item_stride_b,
+                                            int64_t n_items, int64_t M, int64_t N, int64_t K);
+int evok_gemm_nt_batched(const float* A, int64_t lda, int64_t item_stride_a, const float* B, int64_t ldb, int64_t item_stride_b, int64_t n_items,
+                         int64_t M, int64_t N, int64_t K, float* C, int64_t ldc, int64_t item_stride_c, float* C2, int64_t ldc2, int64_t item_stride_c2,
+                         const float* alpha_dev, int64_t item_stride_alpha, const float* bias, int64_t item_stride_bias, void* ws, size_t ws_bytes,
+                         void* stream);
+int evok_gemm_nt_affine_batched(const float* A, int64_t lda, int64_t item_stride_a, const float* B, int64_t ldb, int64_t item_stride_b,
+                                int64_t n_items, int64_t M, int64_t N, int64_t K, float* C, int64_t ldc, int64_t item_stride_c, const float* k_dev,
+                                int64_t item_stride_k, const float* E, int64_t lde, int64_t item_stride_e, const float* u, int64_t item_stride_u,
+                                void* ws, size_t ws_bytes, void* stream);
+int evok_transpose_pair_batched(const float* in, int64_t ldi, int64_t item_stride_in, int64_t rows, int64_t cols, const float* w,
+                                int64_t item_stride_w, float* out_w, float* out_p, int64_t ldo, int64_t item_stride_out, int64_t n_items,
+                                void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Batched searches: the functional ask / tell API with leading batch dimensions (algorithms/functional/funcpgpe.py:67, :301, :330,
  * funccem.py, funcclipup.py:95-108; `expects_ndim`, decorators.py:613).  n_items independent searches of the same shape run in ONE
@@ -435,6 +461,18 @@ int evok_cmaes_row_weights(const float* assigned_weights, const float* Z, int64_
 int evok_cmaes_vector_update(const float* local_disp, const float* shaped_disp, int64_t D, float* m, float* p_sigma, float* p_c, float* sigma_dev,
                              int64_t* steps_dev, int64_t steps_host, const float* consts_host, int csa_squared, float* k_out, float* h_sig_out,
                              void* stream);
+/* The same two stages for n_items independent searches (functional CMA-ES), per item the bits of the single call:
+ *   evok_rank_table_batched        : keys, out [items][N], one shared table; the workspace of evok_rank_table.
+ *   evok_cmaes_row_weights_batched : Z_b at Z + b * item_stride_z (pitch ldz); assigned_weights, w_positive, w_active [items][N].
+ *   evok_cmaes_vector_update_batched: one CTA per item; local_disp, shaped_disp, m, p_sigma, p_c [items][D], sigma_dev [items],
+ *       k_out [items][3]; the constants and the generation counter steps_host are shared. */
+int evok_rank_table_batched(const float* keys, int64_t N, int64_t n_items, int descending, const float* table, float* out, void* ws, size_t ws_bytes,
+                            void* stream);
+int evok_cmaes_row_weights_batched(const float* assigned_weights, const float* Z, int64_t item_stride_z, int64_t ldz, int64_t n_items, int64_t N,
+                                   int64_t D, int active, float* w_positive, float* w_active, void* stream);
+int evok_cmaes_vector_update_batched(const float* local_disp, const float* shaped_disp, int64_t n_items, int64_t D, float* m, float* p_sigma,
+                                     float* p_c, float* sigma_dev, int64_t steps_host, const float* consts_host, int csa_squared, float* k_out,
+                                     void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Separable CMA-ES (diagonal C, algorithms/cmaes.py with separable=True) as three kernels plus evok_rank_table, with no host
