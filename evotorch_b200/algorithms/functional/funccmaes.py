@@ -189,11 +189,17 @@ def _tell_kernels(state, hp, B, n, d, m, sigma, C, y, z, f) -> tuple:
     return m, p_sigma, p_c, sigma, C_new
 
 
+def _assigned_weights(f: torch.Tensor, maximize: bool, weights: torch.Tensor) -> torch.Tensor:
+    """weights[rank of f[b, i] in row b], best first: a stable sort, NaN the largest value (the order of rank_table_batched)."""
+    B, n = f.shape
+    order = torch.argsort(f, dim=-1, descending=maximize, stable=True)
+    ranks = torch.empty_like(order).scatter_(-1, order, torch.arange(n, device=f.device).expand(B, n).contiguous())
+    return weights.to(f.device)[ranks]
+
+
 def _tell_torch(state, hp, B, n, d, m, sigma, C, y, z, f) -> tuple:
     """The same stages as batched torch ops (CMAES's op-by-op generation: update_m ... update_C, cmaes.py:454-553)."""
-    order = torch.argsort(f, dim=-1, descending=state.maximize, stable=True)  # best first
-    ranks = torch.empty_like(order).scatter_(-1, order, torch.arange(n, device=f.device).expand(B, n).contiguous())
-    aw = hp.weights.to(m.device)[ranks]
+    aw = _assigned_weights(f, state.maximize, hp.weights)
     w_pos = torch.clamp_min(aw, 0.0)
     local = torch.einsum("bn,bnd->bd", w_pos, z)
     shaped = torch.einsum("bn,bnd->bd", w_pos, y)

@@ -862,14 +862,17 @@ def _item_mat(t: torch.Tensor, name: str, core: tuple) -> tuple:
     by every item: stride 0) or (items, *core) at any item stride."""
     if not (t.is_cuda and t.dtype == torch.float32 and t.ndim in (2, 3) and tuple(t.shape[-2:]) == tuple(core)):
         raise ValueError(f"{name}: expected a float32 CUDA tensor of shape {core} or (items, {core[0]}, {core[1]}), got {tuple(t.shape)} {t.dtype}")
-    if not (t.stride(-1) == 1 and t.stride(-2) >= core[1]):
+    rows, cols = core
+    # the stride of a dimension of size 1 is never stepped (torch leaves it arbitrary, even in a contiguous tensor of shape (n, 1))
+    if not ((t.stride(-1) == 1 or cols == 1) and (t.stride(-2) >= cols or rows == 1)):
         raise ValueError(f"{name}: expected row-major rows (strides {t.stride()})")
     t = as_plain_tensor(t)
+    ld = t.stride(-2) if rows > 1 else cols
     if t.ndim == 2:
-        return t, None, 0, t.stride(0)
+        return t, None, 0, ld
     if t.shape[0] > 1 and t.stride(0) < 0:
         raise ValueError(f"{name}: negative item stride")
-    return t, t.shape[0], t.stride(0) if t.shape[0] > 1 else 0, t.stride(1)
+    return t, t.shape[0], t.stride(0) if t.shape[0] > 1 else 0, ld
 
 
 def _item_vec(t: Optional[torch.Tensor], name: str, n: int, n_items: int) -> int:

@@ -150,5 +150,42 @@ st = cem(center_init=torch.randn(3, 21, device=dev), parenthood_ratio=0.5, objec
 for _ in range(2):
     pop = cem_ask(st, popsize=10)
     st = cem_tell(st, pop, (pop * pop).sum(-1))
+# functional CMA-ES stages: batched GEMM (aligned, split copies, shared operands, affine epilogue in place), transposing pass,
+# rank table (merge and radix paths), row weights (float4 / scalar items), vector update (more than one element per thread)
+from evotorch_b200 import _native as nat  # noqa: E402
+from evotorch_b200.algorithms.functional import cmaes, cmaes_ask, cmaes_tell  # noqa: E402
+
+for items, M, K in ((3, 5, 7), (2, 33, 130), (4, 8, 16)):
+    A = torch.randn(items * (M * (K + 1) + 1) + 4, device=dev).as_strided((items, M, K), (M * (K + 1) + 1, K + 1, 1), 1)
+    Bs = torch.randn(M, K, device=dev)
+    y, x = torch.empty(items, M, M, device=dev), torch.empty(items, M, M, device=dev)
+    ops.gemm_nt_batched(A, Bs, y, out2=x, alpha=torch.rand(items, device=dev), bias=torch.randn(M, device=dev))
+    ops.gemm_nt_batched(A.contiguous(), A.contiguous(), y)
+    ops.gemm_nt_affine_batched(A, A.contiguous(), torch.rand(3, device=dev), y, E=y, u=torch.randn(items, M, device=dev))
+    ops.gemm_nt_affine_batched(A.contiguous(), Bs, torch.rand(items, 3, device=dev), x)
+    ops.weighted_syrk_update_batched(torch.randn(items, K, M, device=dev), torch.randn(items, K, device=dev), torch.rand(items, 3, device=dev), y,
+                                     u=torch.randn(items, M, device=dev), out=y)
+    rows, cols = K, M
+    inp = torch.randn(items * (rows * (cols + 1) + 3), device=dev)
+    ldo = rows + 5
+    ow, op = torch.empty(items * (cols * ldo + 7), device=dev), torch.empty(items * (cols * ldo + 7), device=dev)
+    w = torch.randn(rows, device=dev)
+    nat.check(nat.lib().evok_transpose_pair_batched(inp.data_ptr(), cols + 1, rows * (cols + 1) + 3, rows, cols, w.data_ptr(), 0, ow.data_ptr(),
+                                                    op.data_ptr(), ldo, cols * ldo + 7, items, nat.stream_of(inp)), "evok_transpose_pair_batched")
+for items, n in ((3, 7), (2, 1025), (2, 8193)):
+    f = torch.randn(items, n, device=dev)
+    ops.rank_table_batched(f, True, torch.randn(n, device=dev))
+for items, n, D in ((3, 9, 4), (3, 7, 37), (2, 5, 1025)):
+    stride = n * D + 2
+    Z = torch.randn(items * stride, device=dev).as_strided((items, n, D), (stride, D, 1))
+    ops.cmaes_row_weights_batched(torch.randn(items, n, device=dev), Z, True, torch.empty(items, n, device=dev), torch.empty(items, n, device=dev))
+for items, D in ((3, 1), (2, 31), (2, 1025)):
+    v = lambda: torch.randn(items, D, device=dev)  # noqa: E731
+    ops.cmaes_vector_update_batched(v(), v(), v(), v(), v(), torch.rand(items, device=dev) + 0.5, (1.0, 0.3, 1.3, 0.2, 0.01, 0.02, 0.7, 0.6, 1.0, 1.0),
+                                    False, torch.empty(items, 3, device=dev), steps=2)
+fst = cmaes(center_init=torch.randn(3, 7, device=dev), stdev_init=1.0, objective_sense="min")
+for _ in range(2):
+    xs = cmaes_ask(fst)
+    fst = cmaes_tell(fst, xs, (xs * xs).sum(-1))
 torch.cuda.synchronize()
 print("SANITIZE_RUN_COMPLETE")

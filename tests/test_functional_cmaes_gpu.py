@@ -4,14 +4,13 @@ convergence next to the CMAES class."""
 
 import math
 
-import numpy as np
 import pytest
 import torch
 
 from evotorch_b200 import Problem, ops
 from evotorch_b200.algorithms import CMAES
 from evotorch_b200.algorithms.functional import cmaes, cmaes_ask, cmaes_tell
-from oracle import es_oracle as O
+from oracle.functional_cmaes_oracle import tell_bound
 
 pytestmark = pytest.mark.gpu
 
@@ -134,73 +133,8 @@ def ellipsoid(x):
 
 
 def _tell_bound(state, x, f, new):
-    """Per item: (max over the state tensors of |kernel - oracle| / first-order bound).  The oracle (float64 sums, fp32 state) gets
-    the tell's own y = (x - m) / sigma and z = A^-1 y solved in float64.  The kernel's z comes from a backward-stable TRSM:
-    |z^ - z| <= gamma_D |A^-1| |A| |z^|, carried to the sums, the vector update and the covariance update to first order, with the
-    K7 bound for the SYRK."""
-    hp = state.hyperparameters
-    B, n, d = x.shape
-    m, sig, A, C = state.center, state.sigma, state.A, state.C
-    y = (x - m[:, None, :]) / sig[:, None, None]
-    A64 = A.double()
-    z64 = torch.linalg.solve_triangular(A64.mT, y.double(), upper=True, left=False)
-    gD = d * EPS / (1 - d * EPS)
-    dz = gD * (z64.abs() @ (torch.linalg.inv(A64).abs() @ A64.abs()).mT) + EPS * z64.abs()
-    aw = torch.stack([torch.as_tensor(O.cmaes_assign_weights(_oracle_state(state, b), f[b].cpu().numpy(), "max" if state.maximize else "min"))
-                      for b in range(B)]).to(DEV).double()
-    wp = aw.clamp_min(0)
-    gn = n * EPS
-    e_local = (wp[:, :, None] * dz).sum(1) + gn * (wp[:, :, None] * z64.abs()).sum(1)
-    shaped = (wp[:, :, None] * y.double()).sum(1)
-    e_shaped = gn * (wp[:, :, None] * y.double().abs()).sum(1)
-    s = sig.double()[:, None]
-    e_m = hp.c_m * s * e_shaped + 4 * EPS * (m.double().abs() + hp.c_m * s * shaped.abs())
-    ps_new = new.p_sigma.double()
-    e_ps = hp.variance_discount_sigma * e_local + 4 * EPS * ((1 - hp.c_sigma) * state.p_sigma.double().abs() + ps_new.abs())
-    e_pn = e_ps.norm(dim=-1)
-    pn = ps_new.norm(dim=-1)
-    slope = (pn / d) if state.csa_squared else torch.full_like(pn, 1 / hp.unbiased_expectation)
-    e_sigma = new.sigma.double() * ((hp.c_sigma / hp.damp_sigma) * slope * e_pn + 8 * EPS)
-    e_pc = hp.variance_discount_c * e_shaped + 4 * EPS * ((1 - hp.c_c) * state.p_c.double().abs() + new.p_c.double().abs())
-    # active weights: w = D aw / ||z||^2 for aw <= 0, so |dw| <= |w| 2 sum|z||dz| / ||z||^2
-    zn2 = (z64 * z64).sum(-1)
-    w_act = torch.where(aw > 0, aw, d * aw / zn2) if state.active else aw
-    e_w = torch.where(aw > 0, torch.zeros_like(aw), w_act.abs() * 2 * (z64.abs() * dz).sum(-1) / zn2) if state.active else torch.zeros_like(aw)
-    Y = y.double()
-    S_abs = (Y.abs().mT * w_act.abs()[:, None, :]) @ Y.abs()
-    e_S = gamma(n) * S_abs + (Y.abs().mT * e_w[:, None, :]) @ Y.abs()
-    pc = new.p_c.double()
-    k2 = hp.c_1 * (hp.c_1 / (hp.c_1 + 1e-23))  # c1a * weighted_pc^2 <= c_1 (h = 1)
-    e_C = (hp.c_mu * e_S + 2 * k2 * pc.abs()[:, :, None] * e_pc[:, None, :]
-           + 8 * EPS * (hp.c_mu * S_abs + C.double().abs() + k2 * pc.abs()[:, :, None] * pc.abs()[:, None, :] + new.C.double().abs()))
-    ratios = []
-    for b in range(B):
-        o = _oracle_state(state, b)
-        O.cmaes_update(o, z64[b].cpu().numpy(), y[b].cpu().numpy(), aw[b].cpu().numpy().astype(np.float32))
-        r = 0.0
-        for got, ref, e in ((new.center[b], o.m, e_m[b]), (new.p_sigma[b], o.p_sigma, e_ps[b]), (new.p_c[b], o.p_c, e_pc[b]),
-                            (new.sigma[b], o.sigma, e_sigma[b]), (new.C[b], o.C, e_C[b])):
-            err = (got.double().cpu() - torch.as_tensor(np.asarray(ref, dtype=np.float64))).abs()
-            r = max(r, worst(err, 2 * e.cpu() + 1e-30))
-        ratios.append(r)
-    return ratios
-
-
-def _oracle_state(state, b):
-    hp = state.hyperparameters
-    d = state.center.shape[-1]
-    o = O.CMAESState(d, hp.popsize, float(state.sigma[b]), state.center[b].cpu().numpy(), active=state.active, csa_squared=state.csa_squared,
-                     stdev_min=state.stdev_min, stdev_max=state.stdev_max)
-    # the learning rates and weights of the state under test (bit for bit those of CMAES); the oracle's own differ in the last bits
-    o.c_m, o.c_sigma, o.damp_sigma, o.c_c, o.c_1, o.c_mu = hp.c_m, hp.c_sigma, hp.damp_sigma, hp.c_c, hp.c_1, hp.c_mu
-    o.variance_discount_sigma, o.variance_discount_c, o.unbiased_expectation = hp.variance_discount_sigma, hp.variance_discount_c, hp.unbiased_expectation
-    o.weights = hp.weights.cpu().numpy().astype(np.float32)
-    o.decompose_C_freq = hp.decompose_C_freq
-    for name in ("p_sigma", "p_c", "C", "A"):
-        setattr(o, name, getattr(state, name)[b].cpu().numpy().astype(np.float32))
-    o.sigma = np.float32(state.sigma[b].item())
-    o.steps = state.generation
-    return o
+    """Per item: (max over the state tensors of |kernel - oracle| / first-order bound), `oracle.functional_cmaes_oracle.tell_bound`."""
+    return tell_bound(state, x, f, new)
 
 
 @pytest.mark.parametrize("d,items", [(8, 6), (33, 4), (130, 3)])
