@@ -59,6 +59,11 @@ _SIGNATURES = {
     "evok_sepcma_moments": (c_int, [_P, _P, c_int, c_int64, c_int64, c_int64, c_uint64, c_uint64, _P, _P, _P, _P, _P, c_size_t, _P]),
     "evok_sepcma_update": (c_int, [_P, _P, _P, c_int64, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int64, _P, c_int, c_int64, c_float, c_float, _P,
                                    _P]),
+    "evok_sepcma_moments_batched_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int64]),
+    "evok_sepcma_moments_batched": (c_int, [_P, c_int64, c_int64, _P, _P, _P, c_int, c_int64, c_int64, c_int64, c_uint64, c_uint64, _P, _P, _P, _P,
+                                            c_size_t, _P]),
+    "evok_sepcma_update_batched": (c_int, [_P, _P, _P, c_int64, c_int64, _P, _P, _P, _P, _P, _P, _P, c_int64, _P, c_int, c_int64, c_float, c_float,
+                                           _P]),
     "evok_weights_adjust": (c_int, [_P, c_int64, c_int, _P]),
     "evok_elite_mask": (c_int, [_P, c_int64, c_int64, _P, _P, c_size_t, _P]),
     "evok_grad_workspace_bytes": (c_size_t, [c_int64, c_int64]),

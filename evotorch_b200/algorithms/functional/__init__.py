@@ -27,9 +27,11 @@ from .funcclipup import ClipUpState, clipup, clipup_ask, clipup_tell
 from .funccmaes import CMAESState, cmaes, cmaes_ask, cmaes_tell
 from .funcpgpe import PGPEState, pgpe, pgpe_ask, pgpe_ask_and_evaluate, pgpe_tell
 from .fused import LazyPopulation
+from .funcsepcmaes import SepCMAESState, sepcmaes, sepcmaes_ask, sepcmaes_ask_and_evaluate, sepcmaes_tell
 from .funcsgd import SGDState, sgd, sgd_ask, sgd_tell
 from .misc import OptimizerFunctions, get_functional_optimizer
 
 __all__ = ["AdamState", "adam", "adam_ask", "adam_tell", "CEMState", "cem", "cem_ask", "cem_ask_and_evaluate", "cem_tell", "ClipUpState",
            "clipup", "clipup_ask", "clipup_tell", "CMAESState", "cmaes", "cmaes_ask", "cmaes_tell", "LazyPopulation", "PGPEState", "pgpe", "pgpe_ask", "pgpe_ask_and_evaluate", "pgpe_tell",
+           "SepCMAESState", "sepcmaes", "sepcmaes_ask", "sepcmaes_ask_and_evaluate", "sepcmaes_tell",
            "SGDState", "sgd", "sgd_ask", "sgd_tell", "OptimizerFunctions", "get_functional_optimizer"]

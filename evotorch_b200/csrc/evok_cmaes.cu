@@ -130,7 +130,8 @@ __global__ void __launch_bounds__(kCmaThreads)
 //   C <- C + c1a (p_c^2 - C) + c_mu (A^2 S2 - wsum C)              (S2 = sum_i b_i z_i^2, so A^2 S2 = sum_i b_i y_i^2)
 //   stdev bounds with the new sigma: C <- (clamp(sigma' sqrt(C), lo, hi) / sigma')^2
 //   A <- sqrt(C) on the generations where (steps + 1) % decompose_freq == 0;   s <- sigma' A  (the sampler's per-column stdev)
-// s_prev (nullable) receives s before the update.  lo / hi: NaN = no bound.
+// s_prev (nullable) receives s before the update.  lo / hi: NaN = no bound.  Grid x = item: the D-vectors of item b at b * D, its sigma
+// and wsum at b (m_prev / s_prev / steps_dev / h_sig_out: single call only).
 __global__ void __launch_bounds__(kCmaThreads)
     sepcma_update_kernel(const float* __restrict__ local_disp, const float* __restrict__ S2, const float* __restrict__ wsum, int64_t D,
                          float* __restrict__ m, float* __restrict__ p_sigma, float* __restrict__ p_c, float* __restrict__ sigma, float* __restrict__ C,
@@ -138,6 +139,17 @@ __global__ void __launch_bounds__(kCmaThreads)
                          long long steps_host, const __grid_constant__ CmaesConsts c, long long decompose_freq, float lo, float hi,
                          float* __restrict__ h_sig_out) {
   __shared__ double sm[33];
+  const int64_t off = (int64_t)blockIdx.x * D;
+  local_disp += off;
+  S2 += off;
+  m += off;
+  p_sigma += off;
+  p_c += off;
+  C += off;
+  A += off;
+  s += off;
+  sigma += blockIdx.x;
+  wsum += blockIdx.x;
   const CmaVectorStep v = cma_vector_step<true>(local_disp, nullptr, A, D, m, p_sigma, p_c, sigma, steps_dev, steps_host, c, sm, m_prev);
   const float sg = v.new_sigma, h = v.h;
   const float c1a = c.c_1 * (1.0f - (1.0f - h * h) * c.c_c * (2.0f - c.c_c));
@@ -242,4 +254,22 @@ extern "C" EVOK_API int evok_sepcma_update(const float* local_disp, const float*
                                                                    (long long)decompose_C_freq, stdev_min, stdev_max, h_sig_out);
   EVOK_CHECK_LAUNCH();
   return 0;
+}
+
+extern "C" EVOK_API int evok_sepcma_update_batched(const float* local_disp, const float* S2, const float* wsum, int64_t n_items, int64_t D, float* m,
+                                                   float* p_sigma, float* p_c, float* sigma_dev, float* C, float* A, float* s, int64_t steps_host,
+                                                   const float* consts_host, int csa_squared, int64_t decompose_C_freq, float stdev_min, float stdev_max,
+                                                   void* stream) {
+  if (!local_disp || !S2 || !wsum || !m || !p_sigma || !p_c || !sigma_dev || !C || !A || !s || !consts_host) return EVOK_E_NULLPTR;
+  if (n_items < 0 || D <= 0 || decompose_C_freq < 1) return EVOK_E_BADSIZE;
+  const CmaesConsts c = cmaes_consts(consts_host, csa_squared);
+  return for_item_chunks(n_items, (int64_t)INT32_MAX, [&](int64_t b0, int64_t nb) {
+    const int64_t off = b0 * D;
+    sepcma_update_kernel<<<(unsigned)nb, kCmaThreads, 0, (cudaStream_t)stream>>>(local_disp + off, S2 + off, wsum + b0, D, m + off, p_sigma + off,
+                                                                                p_c + off, sigma_dev + b0, C + off, A + off, s + off, nullptr, nullptr,
+                                                                                nullptr, (long long)steps_host, c, (long long)decompose_C_freq,
+                                                                                stdev_min, stdev_max, nullptr);
+    EVOK_CHECK_LAUNCH();
+    return 0;
+  });
 }

@@ -53,7 +53,8 @@ struct GradItems {
 
 // Separable CMA-ES row weights (SEPW mode): w holds the rank-assigned weights aw; row r contributes a = max(aw, 0) to S1
 // (recombination) and b = aw, or with active weights b = aw > 0 ? aw : D * aw / q[r] (q = ||z_r||^2, cmaes.py:531-535 of the
-// reference), to S2; the CTAs of column tile 0 also add up b per row chunk into wsum_partial[chunk].
+// reference), to S2; the CTAs of column tile 0 also add up b per row chunk into wsum_partial[chunk].  In a batch q is [items][n_rows]
+// (the layout of w) and wsum_partial [items][n_chunks].
 struct SepWeights {
   const float* q;
   int active;
@@ -82,12 +83,12 @@ __device__ __forceinline__ void grad_coeffs(int form, float s, float& c1, float&
 // (a, b) of unit r: the SEPW weights above, the half difference and half sum of a direction's two rows, or w[r] twice
 template <bool SYM, bool SEPW = false>
 __device__ __forceinline__ void row_weights(const float* __restrict__ w, int64_t r, float& a, float& b, int64_t D = 0,
-                                            const SepWeights* sepw = nullptr) {
+                                            const float* __restrict__ q = nullptr, int active = 0) {
   if (SEPW) {
     const float aw = __ldg(w + r);
     a = fmaxf(aw, 0.0f);
     // q is read only for the negative weights: a zero-weight row is never regenerated and never looks at its norm
-    b = (sepw->active && aw < 0.0f) ? __fdiv_rn((float)D * aw, __ldg(sepw->q + r)) : aw;
+    b = (active && aw < 0.0f) ? __fdiv_rn((float)D * aw, __ldg(q + r)) : aw;
   } else if (SYM) {
     const float wp = __ldg(w + 2 * r), wm = __ldg(w + 2 * r + 1);
     a = 0.5f * (wp - wm);
@@ -117,15 +118,19 @@ __device__ __forceinline__ void store_partial(float* partial, int64_t chunk, int
 }
 
 // SYM: unit r = direction (rows 2r, 2r+1), else unit r = row r.
-// SEPW (with kEpsRegen, non-symmetric, form MOMENTS, mu = sigma = NULL): the weights above, eps = z.
+// SEPW (non-symmetric, form MOMENTS): the weights above, over the steps z.  With kEpsRegen (mu = sigma = NULL) z is the Philox
+// normal itself; with kEpsRead / kEpsRebuild it is the step recovered from the row as the functional tell recovers it,
+// z = (x - m) / s correctly rounded, with (mu, sigma) = (m, s), the centre and per-column stdev the rows were drawn from.
 template <int VEC, int TX, bool SYM, int EPS, bool SEPW = false>
 __global__ void __launch_bounds__(kGradThreads, kGradMinBlocks)
     grad_partial_kernel(int form, const float* __restrict__ X, int64_t ldx, const float* __restrict__ w, const float* __restrict__ mu,
                         const float* __restrict__ sigma, int64_t n_units, int64_t D, int64_t units_per_chunk, uint64_t unit0,
                         const __grid_constant__ PhiloxKey key, const uint32_t* __restrict__ stream_off, float* __restrict__ partial,
                         const __grid_constant__ GradItems items, const __grid_constant__ SepWeights sepw) {
-  static_assert(!SEPW || (EPS == kEpsRegen && !SYM), "the CMA-ES weight mode regenerates non-symmetric rows");
+  static_assert(!SEPW || !SYM, "the CMA-ES weight mode reduces non-symmetric rows");
   constexpr int TY = kGradThreads / TX;
+  const float* q = sepw.q;
+  float* wsum_partial = sepw.wsum_partial;
   if (gridDim.z > 1) {
     const int64_t item = blockIdx.z;
     X += item * items.x;
@@ -133,6 +138,10 @@ __global__ void __launch_bounds__(kGradThreads, kGradMinBlocks)
     mu += item * items.mu;
     sigma += item * items.sigma;
     partial += item * items.partial;
+    if (SEPW) {
+      q += item * items.w;
+      wsum_partial += item * gridDim.y;
+    }
   }
   const uint32_t sw = key.stream_lo + ((EPS != kEpsRead && stream_off) ? __ldg(stream_off) : 0u) + (EPS == kEpsRebuild ? (uint32_t)blockIdx.z : 0u);
   const int tx = threadIdx.x % TX, ty = threadIdx.x / TX;
@@ -142,7 +151,7 @@ __global__ void __launch_bounds__(kGradThreads, kGradMinBlocks)
   float m[VEC], c1[VEC], c0[VEC], sg[VEC];
 #pragma unroll
   for (int c = 0; c < VEC; ++c) {
-    const bool ok = active && (col + c < D) && !SEPW;
+    const bool ok = active && (col + c < D) && !(SEPW && EPS == kEpsRegen);
     const float s = ok ? __ldg(sigma + col + c) : 1.0f;
     m[c] = ok ? __ldg(mu + col + c) : 0.0f;
     sg[c] = s;
@@ -166,7 +175,7 @@ __global__ void __launch_bounds__(kGradThreads, kGradMinBlocks)
       const int64_t r = r0 + (int64_t)u * TY;
       a[u] = b[u] = 0.0f;
       if (r < r_end) {
-        row_weights<SYM, SEPW>(w, r, a[u], b[u], D, &sepw);
+        row_weights<SYM, SEPW>(w, r, a[u], b[u], D, q, sepw.active);
         if (SEPW) wb += b[u];
       }
       need[u] = active && (a[u] != 0.0f || b[u] != 0.0f);
@@ -193,7 +202,8 @@ __global__ void __launch_bounds__(kGradThreads, kGradMinBlocks)
       if (need[u]) {
 #pragma unroll
         for (int c = 0; c < VEC; ++c) {
-          const float e = EPS == kEpsRegen ? sg[c] * x[u].v[c] : EPS == kEpsRebuild ? fmaf(sg[c], x[u].v[c], m[c]) - m[c] : x[u].v[c] - m[c];
+          float e = EPS == kEpsRegen ? sg[c] * x[u].v[c] : EPS == kEpsRebuild ? fmaf(sg[c], x[u].v[c], m[c]) - m[c] : x[u].v[c] - m[c];
+          if (SEPW && EPS != kEpsRegen) e = __fdiv_rn(e, sg[c]);  // the recovered step
           accumulate(a[u], b[u], e, c1[c], c0[c], s1[c], s2[c]);
         }
       }
@@ -230,7 +240,7 @@ __global__ void __launch_bounds__(kGradThreads, kGradMinBlocks)
     if (threadIdx.x == 0) {
       float t = wred[0];
       for (int y = 1; y < TY; ++y) t += wred[y];
-      sepw.wsum_partial[blockIdx.y] = t;
+      wsum_partial[blockIdx.y] = t;
     }
   }
 }
@@ -245,7 +255,7 @@ __device__ __forceinline__ void sum_chunks(const float* __restrict__ partial, in
   }
 }
 
-// WSUM: block 0 also adds the per-chunk sums of the separable CMA-ES weight mode, in chunk order, into *wsum_out
+// WSUM: block x 0 of item y also adds the item's per-chunk sums of the separable CMA-ES weight mode, in chunk order, into wsum_out[y]
 template <bool WSUM = false>
 __global__ void __launch_bounds__(256) grad_finalize_kernel(const float* __restrict__ partial, int n_chunks, int64_t D, float scale_mu,
                                                             float scale_sigma, float* __restrict__ out_mu, float* __restrict__ out_sigma,
@@ -253,9 +263,10 @@ __global__ void __launch_bounds__(256) grad_finalize_kernel(const float* __restr
                                                             float* __restrict__ wsum_out = nullptr) {
   const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (WSUM && j == 0) {
+    wsum_partial += (int64_t)blockIdx.y * n_chunks;
     float t = 0.0f;
     for (int c = 0; c < n_chunks; ++c) t += wsum_partial[c];
-    *wsum_out = t;
+    wsum_out[blockIdx.y] = t;
   }
   if (j >= D) return;
   partial += (int64_t)blockIdx.y * item_stride_partial;  // batched: blockIdx.y = item, outputs contiguous [items][D]
@@ -265,6 +276,55 @@ __global__ void __launch_bounds__(256) grad_finalize_kernel(const float* __restr
   sum_chunks(partial, n_chunks, D, j, t1, t2);
   out_mu[j] = t1 * scale_mu;
   out_sigma[j] = t2 * scale_sigma;
+}
+
+// The row pass of the separable CMA-ES moments over recovered steps: q_i = ||z_i||^2 with z_ij = (x_ij - m_j) / s_j correctly
+// rounded, the z of the column pass.  One warp per row, only for the rows whose norm the column pass reads (aw_i < 0).  Lane l
+// takes the column groups l, l + 32, ... of 4 columns in order and the warp adds the lanes in a fixed order.  x is the stored row
+// (kEpsRead) or the row rebuilt as the batched sampler stored it (kEpsRebuild: x = fmaf(s, z, m), item b on stream word
+// key.stream_lo + b); both give the same bits.  grid y = item: X at item_stride_x, m / s [items][D], aw / q [items][n_rows].
+template <int EPS>
+__global__ void __launch_bounds__(256) sepcma_sqnorm_kernel(const float* __restrict__ X, int64_t item_stride_x, int64_t ldx, const float* __restrict__ m,
+                                                            const float* __restrict__ s, const float* __restrict__ aw, int64_t n_rows, int64_t D,
+                                                            const __grid_constant__ PhiloxKey key, float* __restrict__ q) {
+  const int lane = threadIdx.x & 31;
+  const int64_t row = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (row >= n_rows) return;
+  const int64_t item = blockIdx.y;
+  aw += item * n_rows;
+  q += item * n_rows;
+  if (!(__ldg(aw + row) < 0.0f)) return;  // warp-uniform
+  m += item * D;
+  s += item * D;
+  const float* x_row = EPS == kEpsRead ? X + item * item_stride_x + row * ldx : nullptr;
+  const bool vec = EPS == kEpsRead && (D & 3) == 0 && aligned16_dev(x_row);
+  const uint32_t sw = key.stream_lo + (uint32_t)item;
+  float acc = 0.0f;
+  for (int64_t g = lane; 4 * g < D; g += 32) {
+    const int64_t col = 4 * g;
+    float x[4];
+    if (EPS == kEpsRebuild) {
+      float z[4];
+      normals4(key, sw, (uint64_t)row, (uint32_t)g, z);
+#pragma unroll
+      for (int c = 0; c < 4; ++c) x[c] = col + c < D ? fmaf(__ldg(s + col + c), z[c], __ldg(m + col + c)) : 0.0f;
+    } else if (vec) {
+      const float4 v = ld_stream4(x_row + col);
+      x[0] = v.x; x[1] = v.y; x[2] = v.z; x[3] = v.w;
+    } else {
+#pragma unroll
+      for (int c = 0; c < 4; ++c) x[c] = col + c < D ? ld_stream1(x_row + col + c) : 0.0f;
+    }
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      if (col + c < D) {
+        const float z = __fdiv_rn(x[c] - __ldg(m + col + c), __ldg(s + col + c));
+        acc = fmaf(z, z, acc);
+      }
+    }
+  }
+  acc = warp_sum(acc);
+  if (lane == 0) q[row] = acc;
 }
 
 // The same finalisation for the sharded generation: this rank's (grad_mu | grad_sigma) goes into slot `rank` of EVERY peer's
@@ -579,7 +639,7 @@ struct GradCall {
   int64_t n_items = 1;
   GradItems items{0, 0, 0, 0, 0};     // element strides between the items' operands; run_grad sets .partial from the plan
   int split = 0;                      // rebuilt groups per kSplitPeriod of the TMA kernel (-1 = device_auto_split())
-  SepWeights sepw{nullptr, 0, nullptr};  // the separable CMA-ES weight mode, with its weight sum into *wsum
+  SepWeights sepw{nullptr, 0, nullptr};  // the separable CMA-ES weight mode, with its weight sums into wsum [items]
   float* wsum = nullptr;
   const GradPush* push = nullptr;     // instead of out_mu / out_sigma: into every peer's slot
 };
@@ -630,9 +690,10 @@ static GradPlan plan_grad(const GradCall& c) {
   // at least 16 unrolled iterations per CTA: fewer, fatter chunks keep the fixed-order finalisation short for small populations
   const int64_t max_useful = (p.n_units + (int64_t)ty * kGradUnroll * 16 - 1) / ((int64_t)ty * kGradUnroll * 16);
   set_chunks(p, chunks < max_useful ? chunks : max_useful);
-  // a batch fills the GPU: fewer row chunks per item keep the fixed-order finalisation short (one item never gets fewer)
+  // a batch fills the GPU: fewer row chunks per item keep the fixed-order finalisation short (one item never gets fewer).  The
+  // separable CMA-ES moments keep the plan of one item for every item, so that item b has the bits of a one-item call.
   chunks = ((int64_t)kNumSMs * kGradCtasPerSm + (int64_t)p.n_coltiles * c.n_items - 1) / ((int64_t)p.n_coltiles * c.n_items);
-  if (chunks < p.n_chunks) set_chunks(p, chunks);
+  if (chunks < p.n_chunks && !c.wsum) set_chunks(p, chunks);
   // The rebuild always runs 4 columns per thread: one Philox group gives all 4 (a thread per column would draw each group 4
   // times).  A column's sum depends only on the row threads per CTA (kGradThreads / tx) and the row chunks, so for the scalar
   // plan it keeps that plan's tx and chunks, with a quarter of its column tiles, and gives the scalar read path's bits.
@@ -651,14 +712,18 @@ using PartialKernel = void (*)(int, const float*, int64_t, const float*, const f
     grad_partial_kernel<VEC, 32, SYM, EPS, SEPW>, grad_partial_kernel<VEC, 64, SYM, EPS, SEPW>,                        \
         grad_partial_kernel<VEC, 128, SYM, EPS, SEPW>, grad_partial_kernel<VEC, 256, SYM, EPS, SEPW>                   \
   }
-static const PartialKernel kPartialKernels[9][4] = {
+static const PartialKernel kPartialKernels[12][4] = {
     EVOK_GRAD_TXS(1, false, kEpsRead, false),    EVOK_GRAD_TXS(1, true, kEpsRead, false),  EVOK_GRAD_TXS(4, false, kEpsRead, false),
     EVOK_GRAD_TXS(4, true, kEpsRead, false),     EVOK_GRAD_TXS(4, false, kEpsRegen, false), EVOK_GRAD_TXS(4, true, kEpsRegen, false),
-    EVOK_GRAD_TXS(4, false, kEpsRebuild, false), EVOK_GRAD_TXS(4, true, kEpsRebuild, false), EVOK_GRAD_TXS(4, false, kEpsRegen, true)};
+    EVOK_GRAD_TXS(4, false, kEpsRebuild, false), EVOK_GRAD_TXS(4, true, kEpsRebuild, false), EVOK_GRAD_TXS(4, false, kEpsRegen, true),
+    EVOK_GRAD_TXS(1, false, kEpsRead, true),     EVOK_GRAD_TXS(4, false, kEpsRead, true),  EVOK_GRAD_TXS(4, false, kEpsRebuild, true)};
 #undef EVOK_GRAD_TXS
 
-// the SEPW mode, else (eps, vec, sym): the read kernels by vec, then one pair of rows per Philox mode
-static int partial_row(int eps, int vec, bool sym, bool sepw) { return sepw ? 8 : 2 * (eps == kEpsRead ? vec / 4 : 1 + eps) + (sym ? 1 : 0); }
+// (eps, vec, sym): the read kernels by vec, then one pair of rows per Philox mode; the SEPW mode: regenerated, read by vec, rebuilt
+static int partial_row(int eps, int vec, bool sym, bool sepw) {
+  if (sepw) return eps == kEpsRegen ? 8 : eps == kEpsRead ? 9 + vec / 4 : 11;
+  return 2 * (eps == kEpsRead ? vec / 4 : 1 + eps) + (sym ? 1 : 0);
+}
 static int tx_index(int tx) { return tx == 32 ? 0 : tx == 64 ? 1 : tx == 128 ? 2 : 3; }
 
 // The partial sums of item chunk [b0, b0 + nb) into partial[item - b0][chunk][2][D]
@@ -679,9 +744,11 @@ static void launch_partial(const GradCall& c, const GradPlan& p, int64_t b0, int
                                                                                   rebuilt, unit0, key, c.stream_off, partial);
     return;
   }
+  SepWeights sepw = c.sepw;
+  if (sepw.q) sepw.q += b0 * c.items.w;  // the squared norms have the layout of w
   const PartialKernel kernel = kPartialKernels[partial_row(c.eps, p.vec, is_sym(c), c.wsum != nullptr)][tx_index(p.tx)];
   kernel<<<dim3(p.n_coltiles, p.n_chunks, (unsigned)nb), kGradThreads, 0, c.st>>>(c.form, X, c.ldx, w, mu, sigma, p.n_units, c.D,
-                                                                                    p.units_per_chunk, unit0, key, c.stream_off, partial, c.items, c.sepw);
+                                                                                    p.units_per_chunk, unit0, key, c.stream_off, partial, c.items, sepw);
 }
 
 // Adds the n_chunks row chunks of item chunk [b0, b0 + nb) in order into the outputs: out_mu / out_sigma (with the SEPW weight
@@ -691,8 +758,8 @@ static int launch_finalize(const GradCall& c, int n_chunks, int64_t b0, int64_t 
   if (c.push) {
     grad_finalize_push_kernel<<<grid, 256, 0, c.st>>>(partial, n_chunks, c.D, c.scale_mu, c.scale_sigma, c.push->sink, c.push->epoch, c.push->done);
   } else if (c.wsum) {
-    grad_finalize_kernel<true><<<grid, 256, 0, c.st>>>(partial, n_chunks, c.D, c.scale_mu, c.scale_sigma, c.out_mu, c.out_sigma, 0, c.sepw.wsum_partial,
-                                                       c.wsum);
+    grad_finalize_kernel<true><<<dim3(grid, (unsigned)nb), 256, 0, c.st>>>(partial, n_chunks, c.D, c.scale_mu, c.scale_sigma, c.out_mu + b0 * c.D,
+                                                                           c.out_sigma + b0 * c.D, c.items.partial, c.sepw.wsum_partial, c.wsum + b0);
   } else {
     grad_finalize_kernel<<<dim3(grid, (unsigned)nb), 256, 0, c.st>>>(partial, n_chunks, c.D, c.scale_mu, c.scale_sigma, c.out_mu + b0 * c.D,
                                                                      c.out_sigma + b0 * c.D, c.items.partial);
@@ -879,4 +946,75 @@ extern "C" EVOK_API int evok_grad_batched_regen(int form, const float* w, const 
   c.n_items = n_items;
   c.items = GradItems{0, n_rows, item_stride_mu, item_stride_sigma, 0};
   return grad_batched(c);
+}
+
+// Separable CMA-ES moments of a batch of searches over the steps recovered from their rows.  Every item has the plan of one item,
+// whose row chunks depend only on the columns per thread: the most chunks of either width (16-byte rows, or the scalar plan that
+// unaligned stored rows and rebuilt rows with D % 4 != 0 take).  The workspace holds the partial sums of the column pass and the
+// per-chunk weight sums of at most kMaxGridY items, then q [items][n_rows].
+static size_t round256(size_t b) { return (b + 255) / 256 * 256; }
+static int64_t sepcma_max_chunks(int64_t n_rows, int64_t D) {
+  int64_t most = 1;
+  for (int scalar = 0; scalar < 2; ++scalar) {
+    GradCall c(EVOK_GRAD_MOMENTS, scalar ? kEpsRead : kEpsRebuild, nullptr, nullptr, nullptr, n_rows, D, 1.0f, 1.0f, nullptr, nullptr, nullptr, 0,
+               nullptr);
+    c.ldx = D + 1;  // rows whose pitch rules out 16-byte loads
+    c.batched = true;
+    const GradPlan p = plan_grad(c);
+    if (p.n_chunks > most) most = p.n_chunks;
+  }
+  return most;
+}
+static int64_t item_chunk(int64_t n_items) { return n_items < kMaxGridY ? n_items : kMaxGridY; }
+static size_t sepcma_batched_grad_bytes(int64_t n_items, int64_t n_rows, int64_t D) {
+  return round256((size_t)item_chunk(n_items) * (size_t)sepcma_max_chunks(n_rows, D) * 2 * (size_t)D * sizeof(float));
+}
+static size_t sepcma_batched_wsum_bytes(int64_t n_items, int64_t n_rows, int64_t D) {
+  return round256((size_t)item_chunk(n_items) * (size_t)sepcma_max_chunks(n_rows, D) * sizeof(float));
+}
+
+extern "C" EVOK_API size_t evok_sepcma_moments_batched_workspace_bytes(int64_t n_items, int64_t n_rows, int64_t D) {
+  if (n_items <= 0 || n_rows <= 0 || D <= 0) return 256;
+  return sepcma_batched_grad_bytes(n_items, n_rows, D) + sepcma_batched_wsum_bytes(n_items, n_rows, D) + (size_t)n_items * (size_t)n_rows * sizeof(float);
+}
+
+extern "C" EVOK_API int evok_sepcma_moments_batched(const float* X, int64_t item_stride_x, int64_t ldx, const float* m, const float* s, const float* aw,
+                                                    int active, int64_t n_items, int64_t n_rows, int64_t D, uint64_t seed, uint64_t stream_id0,
+                                                    float* local, float* S2, float* wsum, void* ws, size_t ws_bytes, void* stream) {
+  if (!m || !s || !aw || !local || !S2 || !wsum || !ws) return EVOK_E_NULLPTR;
+  if (n_items < 0 || n_rows <= 0 || D <= 0 || (X && (ldx < D || item_stride_x < 0))) return EVOK_E_BADSIZE;
+  if (n_items == 0) return 0;
+  if (ws_bytes < evok_sepcma_moments_batched_workspace_bytes(n_items, n_rows, D)) return EVOK_E_WORKSPACE;
+  const size_t grad_bytes = sepcma_batched_grad_bytes(n_items, n_rows, D);
+  float* wsum_partial = (float*)((char*)ws + grad_bytes);
+  float* q = active ? (float*)((char*)ws + grad_bytes + sepcma_batched_wsum_bytes(n_items, n_rows, D)) : nullptr;
+  const cudaStream_t st = (cudaStream_t)stream;
+  const PhiloxKey key = make_philox_key(seed, stream_id0);
+  if (active) {  // the row pass: q of the rows with a negative weight, before the column pass reads it
+    const int rc = for_item_chunks(n_items, kMaxGridY, [&](int64_t b0, int64_t nb) {
+      PhiloxKey kc = key;
+      kc.stream_lo += (uint32_t)b0;
+      const dim3 grid((unsigned)((n_rows + 7) / 8), (unsigned)nb);
+      const float* Xc = X ? X + b0 * item_stride_x : nullptr;
+      if (X)
+        sepcma_sqnorm_kernel<kEpsRead><<<grid, 256, 0, st>>>(Xc, item_stride_x, ldx, m + b0 * D, s + b0 * D, aw + b0 * n_rows, n_rows, D, kc,
+                                                             q + b0 * n_rows);
+      else
+        sepcma_sqnorm_kernel<kEpsRebuild><<<grid, 256, 0, st>>>(nullptr, 0, 0, m + b0 * D, s + b0 * D, aw + b0 * n_rows, n_rows, D, kc,
+                                                                q + b0 * n_rows);
+      EVOK_CHECK_LAUNCH();
+      return 0;
+    });
+    if (rc) return rc;
+  }
+  GradCall c(EVOK_GRAD_MOMENTS, X ? kEpsRead : kEpsRebuild, aw, m, s, n_rows, D, 1.0f, 1.0f, local, S2, ws, grad_bytes, stream);
+  c.X = X;
+  c.ldx = X ? ldx : 0;
+  c.key = key;
+  c.batched = true;
+  c.n_items = n_items;
+  c.items = GradItems{X ? item_stride_x : 0, n_rows, D, D, 0};
+  c.sepw = SepWeights{q, active, wsum_partial};
+  c.wsum = wsum;
+  return run_grad(c);
 }

@@ -1000,6 +1000,55 @@ def cmaes_row_weights_batched(assigned: torch.Tensor, Z: torch.Tensor, active: b
                                                        w_act.data_ptr(), nat.stream_of(Z)), "evok_cmaes_row_weights_batched")
 
 
+def sepcma_moments_batched(X: Optional[torch.Tensor], m: torch.Tensor, s: torch.Tensor, aw: torch.Tensor, active: bool, *, seed: int = 0,
+                           stream_id0: int = 0) -> tuple:
+    """Separable CMA-ES moments of every item over the steps recovered from its rows, z = (x - m) / s (correctly rounded):
+    local = sum_i a_i z_i, S2 = sum_i b_i z_i^2 (items, D) and wsum = sum_i b_i (items,), with the weights of `sepcma_moments` and
+    q_i = ||z_i||^2 of that z.  X: (items, N, D), or None for the population that `sample_eval_batched` drew from these m and s with
+    this seed and stream_id0, whose rows are rebuilt bit for bit instead of read.  m, s: (items, D); aw: (items, N)."""
+    if not (aw.is_cuda and aw.dtype == torch.float32 and aw.ndim == 2):
+        raise ValueError("aw: expected a float32 CUDA tensor of shape (items, N)")
+    B, n = aw.shape
+    d = m.shape[-1]
+    aw = _rows(aw, "aw", (B, n))
+    m, s = _rows(m, "m", (B, d)), _rows(s, "s", (B, d))
+    if X is not None:
+        if not (X.is_cuda and X.dtype == torch.float32 and X.is_contiguous() and tuple(X.shape) == (B, n, d)):
+            raise ValueError(f"X: expected a contiguous float32 CUDA tensor of shape {(B, n, d)}")
+        X = as_plain_tensor(X)
+    local, S2 = torch.empty(B, d, dtype=torch.float32, device=aw.device), torch.empty(B, d, dtype=torch.float32, device=aw.device)
+    wsum = torch.empty(B, dtype=torch.float32, device=aw.device)
+    lib = nat.lib()
+    ws = nat.workspace(aw.device, lib.evok_sepcma_moments_batched_workspace_bytes(B, n, d), "grad_batched")
+    with _timed("sepcma_moments"):
+        rc = lib.evok_sepcma_moments_batched(nat.ptr(X), n * d, d, m.data_ptr(), s.data_ptr(), aw.data_ptr(), int(bool(active)), B, n, d, seed,
+                                             stream_id0, local.data_ptr(), S2.data_ptr(), wsum.data_ptr(), ws.data_ptr(), ws.numel(),
+                                             nat.stream_of(aw))
+    nat.check(rc, "evok_sepcma_moments_batched")
+    return local, S2, wsum
+
+
+def sepcma_update_batched(local: torch.Tensor, S2: torch.Tensor, wsum: torch.Tensor, m: torch.Tensor, p_sigma: torch.Tensor, p_c: torch.Tensor,
+                          sigma: torch.Tensor, C: torch.Tensor, A: torch.Tensor, s: torch.Tensor, consts, csa_squared: bool, *, steps: int,
+                          decompose_C_freq: int, stdev_min: Optional[float] = None, stdev_max: Optional[float] = None) -> None:
+    """`sepcma_update` for every item, one CTA each, in place: m, p_sigma, p_c, C, A, s, local, S2 (items, D), sigma, wsum (items,).
+    The 10 constants, the generation counter `steps`, `decompose_C_freq` and the stdev bounds are shared."""
+    B, d = m.shape
+    for t, name in ((local, "local"), (S2, "S2"), (m, "m"), (p_sigma, "p_sigma"), (p_c, "p_c"), (C, "C"), (A, "A"), (s, "s")):
+        _rows(t, name, (B, d))
+    for t, name in ((sigma, "sigma"), (wsum, "wsum")):
+        _rows(t, name, (B,))
+    if int(decompose_C_freq) < 1:
+        raise ValueError("decompose_C_freq: expected a positive integer")
+    lo = NAN if stdev_min is None else float(stdev_min)
+    hi = NAN if stdev_max is None else float(stdev_max)
+    with _timed("sepcma_update"):
+        rc = nat.lib().evok_sepcma_update_batched(local.data_ptr(), S2.data_ptr(), wsum.data_ptr(), B, d, m.data_ptr(), p_sigma.data_ptr(),
+                                                  p_c.data_ptr(), sigma.data_ptr(), C.data_ptr(), A.data_ptr(), s.data_ptr(), int(steps),
+                                                  _host_floats(consts, 10), int(bool(csa_squared)), int(decompose_C_freq), lo, hi, nat.stream_of(m))
+    nat.check(rc, "evok_sepcma_update_batched")
+
+
 def cmaes_vector_update_batched(local_disp: torch.Tensor, shaped_disp: torch.Tensor, m: torch.Tensor, p_sigma: torch.Tensor, p_c: torch.Tensor,
                                 sigma: torch.Tensor, consts, csa_squared: bool, k_out: torch.Tensor, *, steps: int) -> None:
     """`cmaes_vector_update` for every item, one CTA each, in place: m, p_sigma, p_c, local / shaped (items, D), sigma (items,),

@@ -500,6 +500,27 @@ int evok_sepcma_moments(const float* aw, const float* q, int active, int64_t row
 int evok_sepcma_update(const float* local, const float* S2, const float* wsum, int64_t D, float* m, float* p_sigma, float* p_c, float* sigma_dev,
                        float* C, float* A, float* s, float* m_prev, float* s_prev, int64_t* steps_dev, int64_t steps_host, const float* consts_host,
                        int csa_squared, int64_t decompose_C_freq, float stdev_min, float stdev_max, float* h_sig_out, void* stream);
+/* The same two stages for n_items independent separable searches (functional separable CMA-ES), whose populations may have been
+ * repaired or replaced after the ask, so the steps are recovered from the rows: z_ij = (x_ij - m_j) / s_j (correctly rounded) and
+ * q_i = ||z_i||^2 of that z.
+ *   evok_sepcma_moments_batched: local = sum_i a_i z_i, S2 = sum_i b_i z_i^2, wsum = sum_i b_i per item, with the weights of
+ *       evok_sepcma_moments (b_i = D aw_i / q_i for the negative weights when active).  X: [items][n_rows][D] at item stride
+ *       item_stride_x and row pitch ldx; NULL: the rows with a non-zero weight are rebuilt as the batched sampler stored them from
+ *       (seed, stream_id0 + b), x = fmaf(s, z, m), with the same bits as the stored rows.  m, s, local, S2 [items][D]; aw [items][n_rows];
+ *       wsum [items].  A row pass writes q of the rows with a negative weight to the workspace (active only), then the column pass
+ *       reduces: the population is read (or rebuilt) at most twice, rows of zero weight not at all.  Fixed summation order, no
+ *       atomics; item b gives the bits of a one-item call on its operands with stream_id0 + b.  Errors in this order:
+ *       EVOK_E_NULLPTR, EVOK_E_BADSIZE (n_items < 0, n_rows <= 0, D <= 0, with X: ldx < D or a negative item stride),
+ *       EVOK_E_WORKSPACE (none with n_items == 0).
+ *   evok_sepcma_update_batched: evok_sepcma_update with one CTA per item, per item the bits of the single call; local, S2, m, p_sigma,
+ *       p_c, C, A, s [items][D], wsum, sigma_dev [items].  The constants, the generation counter and the stdev bounds are shared. */
+size_t evok_sepcma_moments_batched_workspace_bytes(int64_t n_items, int64_t n_rows, int64_t D);
+int evok_sepcma_moments_batched(const float* X, int64_t item_stride_x, int64_t ldx, const float* m, const float* s, const float* aw, int active,
+                                int64_t n_items, int64_t n_rows, int64_t D, uint64_t seed, uint64_t stream_id0, float* local, float* S2, float* wsum,
+                                void* ws, size_t ws_bytes, void* stream);
+int evok_sepcma_update_batched(const float* local, const float* S2, const float* wsum, int64_t n_items, int64_t D, float* m, float* p_sigma, float* p_c,
+                               float* sigma_dev, float* C, float* A, float* s, int64_t steps_host, const float* consts_host, int csa_squared,
+                               int64_t decompose_C_freq, float stdev_min, float stdev_max, void* stream);
 
 /* Cholesky factorisation A = L L^T (fp32, lower; the strictly upper part of L is zeroed, like torch.linalg.cholesky).  Replaces
  * CMAES.decompose_C (cmaes.py:555-565, torch.linalg.cholesky -> cuSOLVER potrf).  ONE persistent kernel: 64 x 64 tiles, left-looking
