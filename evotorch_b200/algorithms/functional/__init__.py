@@ -19,12 +19,18 @@ in one launch, and with `lazy=True` never store the population:
 
     population, evals = pgpe_ask_and_evaluate(state, popsize=1000, objective=rastrigin, lazy=True)
     state = pgpe_tell(state, population, evals)
+
+`cmaes_ask_and_evaluate` evaluates the full-covariance asks of all items in one launch of the batched evaluation kernel, keyed
+with the ask's Philox draw, so per-item data and noise reach CMA-ES too:
+
+    population, evals = cmaes_ask_and_evaluate(state, objective=shifted_sphere)   # data of batch shape (1024,)
+    state = cmaes_tell(state, population, evals)
 """
 
 from .funcadam import AdamState, adam, adam_ask, adam_tell
 from .funccem import CEMState, cem, cem_ask, cem_ask_and_evaluate, cem_tell
 from .funcclipup import ClipUpState, clipup, clipup_ask, clipup_tell
-from .funccmaes import CMAESState, cmaes, cmaes_ask, cmaes_tell
+from .funccmaes import CMAESState, cmaes, cmaes_ask, cmaes_ask_and_evaluate, cmaes_tell
 from .funcpgpe import PGPEState, pgpe, pgpe_ask, pgpe_ask_and_evaluate, pgpe_tell
 from .fused import LazyPopulation
 from .funcsepcmaes import SepCMAESState, sepcmaes, sepcmaes_ask, sepcmaes_ask_and_evaluate, sepcmaes_tell
@@ -32,6 +38,6 @@ from .funcsgd import SGDState, sgd, sgd_ask, sgd_tell
 from .misc import OptimizerFunctions, get_functional_optimizer
 
 __all__ = ["AdamState", "adam", "adam_ask", "adam_tell", "CEMState", "cem", "cem_ask", "cem_ask_and_evaluate", "cem_tell", "ClipUpState",
-           "clipup", "clipup_ask", "clipup_tell", "CMAESState", "cmaes", "cmaes_ask", "cmaes_tell", "LazyPopulation", "PGPEState", "pgpe", "pgpe_ask", "pgpe_ask_and_evaluate", "pgpe_tell",
+           "clipup", "clipup_ask", "clipup_tell", "CMAESState", "cmaes", "cmaes_ask", "cmaes_ask_and_evaluate", "cmaes_tell", "LazyPopulation", "PGPEState", "pgpe", "pgpe_ask", "pgpe_ask_and_evaluate", "pgpe_tell",
            "SepCMAESState", "sepcmaes", "sepcmaes_ask", "sepcmaes_ask_and_evaluate", "sepcmaes_tell",
            "SGDState", "sgd", "sgd_ask", "sgd_tell", "OptimizerFunctions", "get_functional_optimizer"]

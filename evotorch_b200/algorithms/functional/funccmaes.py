@@ -12,6 +12,9 @@ On CUDA float32 a generation of ALL items is one launch per stage:
 Nothing is read back to the host: the generation counter that drives h_sig and the schedule is a Python int in the state.
 Anywhere else the same algorithm runs as batched torch ops.
 
+`cmaes_ask_and_evaluate(state, objective=...)` asks and evaluates: with an objective that has a fused kernel, the fitnesses of all
+items come from one launch of the batched evaluation kernel, keyed with the ask's Philox draw (per-item data, noise of the draw).
+
 `cmaes_tell` takes any `values` of the asked shape, so repaired or injected solutions are legal (as in pycma's `tell`): the
 steps z are recovered from the values, not remembered from the ask.
 """
@@ -19,7 +22,7 @@ steps z are recovered from the values, not remembered from the ask.
 from __future__ import annotations
 
 import math
-from typing import NamedTuple, Optional
+from typing import Callable, NamedTuple, Optional
 
 import torch
 
@@ -108,21 +111,50 @@ def _items(state: CMAESState) -> tuple:
     return batch, B, d
 
 
-def cmaes_ask(state: CMAESState) -> torch.Tensor:
-    """A population per item: a tensor of shape (..., popsize, D), row i of item b = m_b + sigma_b A_b z_i."""
+def _ask(state: CMAESState) -> tuple:
+    """(`cmaes_ask`'s population, the Philox seed of its z on the kernels (item b on stream b), None elsewhere)."""
     batch, B, d = _items(state)
     n = state.popsize
     m, sigma, A = state.center.reshape(B, d), state.sigma.reshape(B), state.A.reshape(B, d, d)
+    seed = None
     if on_kernels(m, sigma, A):
         z = torch.empty(B, n, d, dtype=torch.float32, device=m.device)
         zero = torch.zeros(d, dtype=torch.float32, device=m.device)
-        ops.sample_batched(z, zero, zero + 1.0, symmetric=False, seed=draw_philox_seed())
+        seed = draw_philox_seed()
+        ops.sample_batched(z, zero, zero + 1.0, symmetric=False, seed=seed)
         x = torch.empty_like(z)
         ops.gemm_nt_batched(z, A.contiguous(), torch.empty_like(z), out2=x, alpha=sigma.contiguous(), bias=m.contiguous())
     else:
         z = torch.randn(B, n, d, dtype=m.dtype, device=m.device)
         x = m[:, None, :] + sigma[:, None, None] * (z @ A.mT)
-    return x.view(batch + (n, d))
+    return x.view(batch + (n, d)), seed
+
+
+def cmaes_ask(state: CMAESState) -> torch.Tensor:
+    """A population per item: a tensor of shape (..., popsize, D), row i of item b = m_b + sigma_b A_b z_i."""
+    return _ask(state)[0]
+
+
+def cmaes_ask_and_evaluate(state: CMAESState, *, objective: Callable) -> tuple:
+    """`cmaes_ask` and the fitnesses of the population: (values (..., popsize, D), evals (..., popsize)).
+
+    With the state on the kernels (float32 CUDA) and an objective with a fused kernel (`evok_objective_id`: the objectives of
+    evotorch_b200.objectives and every FusedObjective), the ask runs as `cmaes_ask` does (under the same torch.manual_seed the
+    values are bit-identical) and one launch of the batched evaluation kernel evaluates every item, keyed with the Philox draw of
+    the z: an objective with noise gives row i of item b the noise the batched sampler would give it, and an objective with
+    per-item data gives item b its own data.  Otherwise this is `cmaes_ask` followed by `objective(values)`.  An objective whose
+    data has a batch shape must have the state's batch shape.  There is no lazy form: `cmaes_tell` recovers its steps from the
+    values."""
+    batch, _, _ = _items(state)
+    per_item = tuple(getattr(objective, "data_batch_shape", ()))
+    if per_item and per_item != batch:
+        raise ValueError(f"the data of {objective!r} has batch shape {per_item}, the CMA-ES state {batch}: each item of the data needs "
+                         "its own search (build the state with that batch shape)")
+    values, seed = _ask(state)
+    oid = getattr(objective, "evok_objective_id", None)
+    if seed is not None and oid is not None and oid != ops.OBJ_NONE and hasattr(objective, "evaluate_batched"):
+        return values, objective.evaluate_batched(values, seed=seed)
+    return values, objective(values)
 
 
 def _limit_stdev(C: torch.Tensor, sigma: torch.Tensor, lo: Optional[float], hi: Optional[float]) -> None:

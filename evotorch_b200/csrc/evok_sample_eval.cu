@@ -25,22 +25,34 @@ struct PushArgs {
 // kernel of a call (choose_kernel) and one function launches it (launch).
 // ------------------------------------------------------------------------------------------------
 
-// The position of a kernel in the EVOK_OBJ_KERNEL_* order: its family (EVOK_OBJ_KERNEL_SAMPLE, _PUSH, _SQ, _EVAL or
-// _BATCHED), then + 4 sym (SAMPLE, PUSH and BATCHED), + 2 store (all but EVAL), + vec.  jit.kernel_expressions() lists a
-// registered objective's first EVOK_OBJ_KERNELS kernels in the same order, jit.batched_kernel_expressions() its batched ones.
+// The position of a kernel in the EVOK_OBJ_KERNEL_* order: its family (EVOK_OBJ_KERNEL_SAMPLE, _PUSH, _SQ, _EVAL, _BATCHED or
+// _EVAL_BATCHED), then + 4 sym (SAMPLE, PUSH and BATCHED), + 2 store (all but the evaluation families), + vec.
+// jit.kernel_expressions() lists a registered objective's first EVOK_OBJ_KERNELS kernels in the same order,
+// jit.batched_kernel_expressions() its batched samplers and jit.eval_batched_kernel_expressions() its batched evaluation.
+constexpr bool is_eval_family(int family) { return family == EVOK_OBJ_KERNEL_EVAL || family == EVOK_OBJ_KERNEL_EVAL_BATCHED; }
 constexpr int kernel_index(int family, bool sym, bool store, bool vec) {
   return family + (sym && (family < EVOK_OBJ_KERNEL_SQ || family == EVOK_OBJ_KERNEL_BATCHED) ? 4 : 0) +
-         (store && family != EVOK_OBJ_KERNEL_EVAL ? 2 : 0) + (vec ? 1 : 0);
+         (store && !is_eval_family(family) ? 2 : 0) + (vec ? 1 : 0);
 }
 
-// every kernel of an objective's table: the EVOK_OBJ_KERNELS of its first image, then the batched family of its second
-constexpr int kTableKernels = EVOK_OBJ_KERNEL_BATCHED + EVOK_OBJ_BATCHED_KERNELS;
+// every kernel of an objective's table: the EVOK_OBJ_KERNELS of its first image, the batched samplers of its second, the
+// batched evaluation of its third
+constexpr int kImages = 3;
+constexpr int kTableKernels = EVOK_OBJ_KERNEL_EVAL_BATCHED + EVOK_OBJ_EVAL_BATCHED_KERNELS;
 static_assert(EVOK_OBJ_KERNEL_BATCHED == EVOK_OBJ_KERNELS, "the batched family follows the first image's kernels");
+static_assert(EVOK_OBJ_KERNEL_EVAL_BATCHED == EVOK_OBJ_KERNEL_BATCHED + EVOK_OBJ_BATCHED_KERNELS, "the batched evaluation follows the batched samplers");
 
-static int kernel_threads(int k) { return k >= EVOK_OBJ_KERNEL_EVAL && k < EVOK_OBJ_KERNEL_BATCHED ? kEvalThreads : kSampleThreads; }
+// the first table position and the number of kernels of each image
+constexpr int kImageFirst[kImages] = {0, EVOK_OBJ_KERNEL_BATCHED, EVOK_OBJ_KERNEL_EVAL_BATCHED};
+constexpr int kImageKernels[kImages] = {EVOK_OBJ_KERNELS, EVOK_OBJ_BATCHED_KERNELS, EVOK_OBJ_EVAL_BATCHED_KERNELS};
 
-// the image of a registered objective that holds kernel k: 0 = the one of evok_objective_register, 1 = the batched one
-static int image_of(int k) { return k >= EVOK_OBJ_KERNEL_BATCHED ? 1 : 0; }
+static int kernel_threads(int k) {
+  return (k >= EVOK_OBJ_KERNEL_EVAL && k < EVOK_OBJ_KERNEL_BATCHED) || k >= EVOK_OBJ_KERNEL_EVAL_BATCHED ? kEvalThreads : kSampleThreads;
+}
+
+// the image of a registered objective that holds kernel k: 0 = the one of evok_objective_register, 1 = the batched samplers,
+// 2 = the batched evaluation
+static int image_of(int k) { return k >= EVOK_OBJ_KERNEL_EVAL_BATCHED ? 2 : k >= EVOK_OBJ_KERNEL_BATCHED ? 1 : 0; }
 
 // The sampler of built-in objective OBJ with the variant bits V = sym | store << 1 | vec << 2 | push << 3 | sq << 4, if it
 // exists (the SQ sampler is plain and non-symmetric) and can be reached: EVOK_OBJ_NONE only stores samples, since
@@ -65,9 +77,11 @@ template <int OBJ, int... V>
 static void put_builtin_kernels(void** fn, std::integer_sequence<int, V...>) {
   (put_builtin_sampler<OBJ, V>(fn), ...);
   (put_builtin_batched<OBJ, V>(fn), ...);
-  if constexpr (OBJ != EVOK_OBJ_NONE) {  // evok_eval refuses EVOK_OBJ_NONE
+  if constexpr (OBJ != EVOK_OBJ_NONE) {  // evok_eval and evok_eval_batched refuse EVOK_OBJ_NONE
     fn[kernel_index(EVOK_OBJ_KERNEL_EVAL, false, true, false)] = reinterpret_cast<void*>(eval_kernel<ObjAcc<OBJ>, false>);
     fn[kernel_index(EVOK_OBJ_KERNEL_EVAL, false, true, true)] = reinterpret_cast<void*>(eval_kernel<ObjAcc<OBJ>, true>);
+    fn[kernel_index(EVOK_OBJ_KERNEL_EVAL_BATCHED, false, true, false)] = reinterpret_cast<void*>(eval_batched_kernel<ObjAcc<OBJ>, false>);
+    fn[kernel_index(EVOK_OBJ_KERNEL_EVAL_BATCHED, false, true, true)] = reinterpret_cast<void*>(eval_batched_kernel<ObjAcc<OBJ>, true>);
   }
 }
 
@@ -84,10 +98,10 @@ constexpr int kMaxDevices = 64;
 // The kernels of one objective on one device, filled on the first use there and kept until the process ends.  A built-in
 // objective's entries are its nvcc-compiled kernels (null where no entry point reaches them); a registered objective's are the
 // functions of its modules, loaded into the device's primary context: the first image's on the first use of the id, the
-// batched image's on the first batched use.
+// batched samplers' on the first batched sampling, the batched evaluation's on the first batched evaluation.
 struct DeviceKernels {
-  int state[2] = {};             // per image: 0: not filled; 1: filled; EVOK_E_NOKERNEL: the cubin lacks a kernel (a permanent failure)
-  CUmodule module[2] = {};       // set for a registered objective: fn holds CUfunctions, launched through the driver
+  int state[kImages] = {};        // per image: 0: not filled; 1: filled; EVOK_E_NOKERNEL: the cubin lacks a kernel (a permanent failure)
+  CUmodule module[kImages] = {};  // set for a registered objective: fn holds CUfunctions, launched through the driver
   void* fn[kTableKernels] = {};
   int per_sm[kTableKernels] = {};  // resident CTAs per SM
   int sms = 0;
@@ -95,9 +109,10 @@ struct DeviceKernels {
 
 struct Objective {
   // a registered objective's cubins and the lowered names of their kernels (in the EVOK_OBJ_KERNEL_* order): [0] from
-  // evok_objective_register, [1] (the batched family, empty until attached) from evok_objective_register_batched
-  std::vector<char> image[2];
-  std::vector<std::string> names[2];
+  // evok_objective_register, [1] (the batched samplers, empty until attached) from evok_objective_register_batched, [2] (the
+  // batched evaluation, empty until attached) from evok_objective_register_eval_batched
+  std::vector<char> image[kImages];
+  std::vector<std::string> names[kImages];
   // evok_objective_declare_data: the data names of its accumulator (0: none) and which of them are vectors of the row length
   int n_data = 0;
   bool is_vector[EVOK_MAX_DATA] = {};
@@ -216,11 +231,11 @@ static void fill_builtin(int objective, int dev, DeviceKernels& d) {
     if (d.fn[k] && (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&d.per_sm[k], d.fn[k], kernel_threads(k), 0) != cudaSuccess || d.per_sm[k] <= 0))
       d.per_sm[k] = 4;
   if (cudaDeviceGetAttribute(&d.sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || d.sms <= 0) d.sms = kNumSMs;
-  d.state[0] = d.state[1] = 1;
+  for (int part = 0; part < kImages; ++part) d.state[part] = 1;
 }
 
-// Loads image `part` of a registered objective on device `dev` into its table positions (EVOK_OBJ_KERNELS kernels from 0 for
-// part 0, EVOK_OBJ_BATCHED_KERNELS from EVOK_OBJ_KERNEL_BATCHED for part 1).
+// Loads image `part` of a registered objective on device `dev` into its table positions (kImageKernels[part] kernels from
+// kImageFirst[part]).
 static int load_module(const Objective& obj, int part, int dev, DeviceKernels& d) {
   cudaError_t ce = cudaSetDevice(dev);  // makes the device's primary context (the runtime's) current, creating it if needed
   if (ce != cudaSuccess) return (int)ce;
@@ -231,8 +246,8 @@ static int load_module(const Objective& obj, int part, int dev, DeviceKernels& d
   if (r == CUDA_SUCCESS) r = api.device_attribute(&d.sms, CU_DEVICE_ATTRIBUTE_MULTIPROCESSOR_COUNT, cu_dev);
   if (r == CUDA_SUCCESS) r = api.module_load(&d.module[part], obj.image[part].data());
   if (r != CUDA_SUCCESS) return (int)r;  // CUresult and cudaError_t share their codes
-  const int k0 = part ? EVOK_OBJ_KERNEL_BATCHED : 0;
-  const int n = part ? EVOK_OBJ_BATCHED_KERNELS : EVOK_OBJ_KERNELS;
+  const int k0 = kImageFirst[part];
+  const int n = kImageKernels[part];
   for (int i = 0; i < n; ++i) {
     const int k = k0 + i;
     CUfunction fn = nullptr;
@@ -251,8 +266,8 @@ static int load_module(const Objective& obj, int part, int dev, DeviceKernels& d
 }
 
 // The kernel table of an objective (a built-in id or a registered one) on the current device, with the kernels of image `part`
-// (image_of) filled here on the first call that needs them on that device.  A registered id without a batched image gives
-// EVOK_E_NOKERNEL for part 1 (not kept: the image may be attached later).
+// (image_of) filled here on the first call that needs them on that device.  A registered id without image `part` (1 or 2) gives
+// EVOK_E_NOKERNEL (not kept: the image may be attached later).
 static int device_kernels(int objective, int part, const DeviceKernels** out) {
   int dev = 0;
   const cudaError_t ce = cudaGetDevice(&dev);
@@ -382,18 +397,28 @@ extern "C" EVOK_API int evok_objective_load(int objective) {
   return device_kernels(objective, 0, &d);
 }
 
-extern "C" EVOK_API int evok_objective_register_batched(int objective, const void* cubin, size_t bytes, const char* const* kernel_names_host,
-                                                        int n_kernels) {
+// evok_objective_register_batched (part 1) and evok_objective_register_eval_batched (part 2): attach image `part` of a registered id
+static int attach_image(int objective, int part, const void* cubin, size_t bytes, const char* const* kernel_names_host, int n_kernels) {
   if (!cubin || !kernel_names_host) return EVOK_E_NULLPTR;
-  if (bytes == 0 || n_kernels != EVOK_OBJ_BATCHED_KERNELS) return EVOK_E_BADSIZE;
+  if (bytes == 0 || n_kernels != kImageKernels[part]) return EVOK_E_BADSIZE;
   for (int k = 0; k < n_kernels; ++k)
     if (!kernel_names_host[k]) return EVOK_E_NULLPTR;
   if (!is_user(objective)) return EVOK_E_BADENUM;
   std::lock_guard<std::mutex> lock(g_objective_mutex);
   Objective& obj = *g_user[objective - EVOK_OBJ_USER_BASE];
-  obj.image[1].assign(static_cast<const char*>(cubin), static_cast<const char*>(cubin) + bytes);
-  obj.names[1].assign(kernel_names_host, kernel_names_host + n_kernels);
+  obj.image[part].assign(static_cast<const char*>(cubin), static_cast<const char*>(cubin) + bytes);
+  obj.names[part].assign(kernel_names_host, kernel_names_host + n_kernels);
   return 0;
+}
+
+extern "C" EVOK_API int evok_objective_register_batched(int objective, const void* cubin, size_t bytes, const char* const* kernel_names_host,
+                                                        int n_kernels) {
+  return attach_image(objective, 1, cubin, bytes, kernel_names_host, n_kernels);
+}
+
+extern "C" EVOK_API int evok_objective_register_eval_batched(int objective, const void* cubin, size_t bytes, const char* const* kernel_names_host,
+                                                             int n_kernels) {
+  return attach_image(objective, 2, cubin, bytes, kernel_names_host, n_kernels);
 }
 
 extern "C" EVOK_API int evok_objective_declare_data(int objective, int n_data, const int* is_vector_host) {
@@ -584,4 +609,44 @@ extern "C" EVOK_API int evok_sample_eval_batched(int objective, float* X, int64_
   if (rc != 0 || n_items == 0 || n_rows == 0) return rc;
   return sample_items(objective, X, item_stride_x, ldx, mu, item_stride_mu, sigma, item_stride_sigma, n_items, n_rows, D, symmetric != 0, seed,
                       stream_id0, f, (cudaStream_t)stream);
+}
+
+// true for a registered id (a base) without image `part`: its calls of that family launch nothing (EVOK_E_NOKERNEL)
+static bool lacks_image(int base, int part) {
+  if (!is_user(base)) return false;
+  std::lock_guard<std::mutex> lock(g_objective_mutex);
+  return g_user[base - EVOK_OBJ_USER_BASE]->image[part].empty();
+}
+
+// true for an instance id whose binding has per-item data for another number of items than n_items
+static bool items_differ(int objective, int64_t n_items) {
+  if (objective < EVOK_OBJ_INSTANCE_BASE) return false;
+  std::lock_guard<std::mutex> lock(g_objective_mutex);
+  const Instance* inst = instance_of(objective);
+  return inst && inst->n_items > 1 && inst->n_items != n_items;
+}
+
+extern "C" EVOK_API int evok_eval_batched(int objective, const float* X, int64_t item_stride_x, int64_t ldx, int64_t n_items, int64_t n_rows,
+                                          int64_t D, uint64_t seed, uint64_t stream_id0, float* f, void* stream) {
+  if (!X || !f) return EVOK_E_NULLPTR;
+  const int base = base_of(objective);
+  if ((base <= EVOK_OBJ_NONE || base >= EVOK_OBJ_COUNT) && !is_user(base)) return EVOK_E_BADENUM;
+  if (n_items < 0 || n_rows < 0 || item_stride_x < 0 || D <= 0 || ldx < D || items_differ(objective, n_items)) return EVOK_E_BADSIZE;
+  if (lacks_image(base, 2)) return EVOK_E_NOKERNEL;
+  LaunchData data;
+  if (const int rc = bind_data(objective, D, n_items, &data)) return rc;
+  if (n_items == 0 || n_rows == 0) return 0;
+  const KernelChoice c = choose_kernel(EVOK_OBJ_KERNEL_EVAL_BATCHED, false, X, ldx, nullptr, nullptr, n_rows, D, data, item_stride_x);
+  // one key for all items: item b draws its noise on stream word (stream_id0 + b), chunk b0 from stream_lo + b0
+  const EvalKey noise{is_noisy(base) ? make_philox_key(seed, stream_id0) : PhiloxKey{}, nullptr, 0};
+  return for_item_chunks(n_items, kMaxGridY, [&](int64_t b0, int64_t nb) {
+    EvalKey kc = noise;
+    kc.key.stream_lo += (uint32_t)b0;
+    const float* Xc = X + b0 * item_stride_x;
+    float* fc = f + b0 * n_rows;
+    DataBinding dc = data.binding;
+    for (int i = 0; i < EVOK_MAX_DATA; ++i) dc.p[i] += b0 * dc.item_stride[i];
+    void* args[] = {&Xc, &item_stride_x, &ldx, &n_rows, &D, &fc, &dc, &kc};
+    return launch(data.base, c, args, (cudaStream_t)stream, nb);
+  });
 }

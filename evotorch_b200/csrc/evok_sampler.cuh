@@ -789,6 +789,117 @@ __global__ void __launch_bounds__(kSampleThreads, AccTraits<Acc>::kSampleMinBloc
 
 constexpr int kEvalThreads = 256;
 
+// One row of the evaluation kernels: the fitness of row r of X (row pitch ldx, D columns; every lane gets it), with the data
+// binding `data` and, for an accumulator with noise, global row row0 + r of the draw (key, stream word sw); key is null for every
+// other accumulator.  The body of eval_kernel and of eval_batched_kernel, so both give the same bits for the same row, draw and
+// path.
+template <typename Acc, bool VEC>
+__device__ __forceinline__ float eval_row(int lane, const float* __restrict__ X, int64_t ldx, int64_t r, int64_t D,
+                                          const typename AccTraits<Acc>::DataArg& data, const PhiloxKey* key, uint32_t sw, int64_t row0) {
+  using T = AccTraits<Acc>;
+  Acc acc = acc_make<Acc>(D, data);
+  const float* x = X + r * ldx;
+  if constexpr (T::kWarpSteps) {
+    // warp-uniform steps (fold_step shuffles); per lane the groups, element adds, running sums and pair folds of
+    // sample_eval_kernel's VEC path in the same order, so both kernels give the same fitness bit for bit on the same X
+    constexpr bool kFoldNow = !T::kRunning;
+    StepCarry<Acc> carry;
+    if (VEC) {
+      const int64_t nq = D >> 2;
+      int64_t b = 0;
+      for (; b + 128 <= nq; b += 128) {
+        const int64_t q = b + lane;
+        float4 g[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) g[k] = ld_stream4(x + 4 * (q + 32 * k));
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const int64_t jk = 4 * (q + 32 * k);
+          const float v[4] = {g[k].x, g[k].y, g[k].z, g[k].w};
+          DataCols<Acc, 4> dc;
+          dc.load4(acc, jk);
+          if constexpr (T::kElementDraws) dc.draw4(*key, sw, row0 + r, (uint32_t)(q + 32 * k));
+          if constexpr (T::kPairs)
+            if (jk > 0) dc.load_left(acc, jk);
+          if constexpr (kFoldNow) {
+            acc_add(acc, v[0], jk, dc.v[0]); acc_add(acc, v[1], jk + 1, dc.v[1]); acc_add(acc, v[2], jk + 2, dc.v[2]); acc_add(acc, v[3], jk + 3, dc.v[3]);
+          }
+          fold_step<4>(acc, v, jk, 4, carry, dc);
+        }
+      }
+      for (; b < nq; b += 32) {
+        const int64_t q = b + lane;
+        const bool active = q < nq;
+        const float4 a = active ? ld_stream4(x + 4 * q) : make_float4(0.f, 0.f, 0.f, 0.f);
+        const float v[4] = {a.x, a.y, a.z, a.w};
+        const int64_t ja = 4 * q;
+        DataCols<Acc, 4> dc;
+        if (active) {
+          dc.load4(acc, ja);
+          if constexpr (T::kElementDraws) dc.draw4(*key, sw, row0 + r, (uint32_t)q);
+          if constexpr (T::kPairs)
+            if (ja > 0) dc.load_left(acc, ja);
+          if constexpr (kFoldNow) {
+            acc_add(acc, v[0], ja, dc.v[0]); acc_add(acc, v[1], ja + 1, dc.v[1]); acc_add(acc, v[2], ja + 2, dc.v[2]); acc_add(acc, v[3], ja + 3, dc.v[3]);
+          }
+        }
+        fold_step<4>(acc, v, ja, active ? 4 : 0, carry, dc);
+      }
+    } else {
+      for (int64_t b = 0; b < D; b += 32) {
+        const int64_t j = b + lane;
+        const bool active = j < D;
+        const float v[1] = {active ? ld_stream1(x + j) : 0.f};
+        DataCols<Acc, 1> dc;
+        if (active) {
+          dc.load1(acc, j, 0);
+          if constexpr (T::kElementDraws) dc.draw1(*key, sw, row0 + r, j, 0);
+          if constexpr (T::kPairs)
+            if (j > 0) dc.load_left(acc, j);
+          if constexpr (kFoldNow) acc_add(acc, v[0], j, dc.v[0]);
+        }
+        fold_step<1>(acc, v, j, active ? 1 : 0, carry, dc);
+      }
+    }
+  } else if (VEC) {
+    const int64_t nq = D >> 2;
+    int64_t q = lane;
+    // 4 independent 128-bit loads in flight per lane
+    for (; q + 96 < nq; q += 128) {
+      const float4 a = ld_stream4(x + 4 * q), b = ld_stream4(x + 4 * (q + 32)), c = ld_stream4(x + 4 * (q + 64)),
+                   d = ld_stream4(x + 4 * (q + 96));
+      const int64_t ja = 4 * q, jb = 4 * (q + 32), jc = 4 * (q + 64), jd = 4 * (q + 96);
+      DataCols<Acc, 4> da, db, dc, dd;
+      da.load4(acc, ja); db.load4(acc, jb); dc.load4(acc, jc); dd.load4(acc, jd);
+      if constexpr (T::kElementDraws) {
+        const uint64_t row = row0 + r;
+        da.draw4(*key, sw, row, (uint32_t)q); db.draw4(*key, sw, row, (uint32_t)(q + 32));
+        dc.draw4(*key, sw, row, (uint32_t)(q + 64)); dd.draw4(*key, sw, row, (uint32_t)(q + 96));
+      }
+      acc_add(acc, a.x, ja, da.v[0]); acc_add(acc, a.y, ja + 1, da.v[1]); acc_add(acc, a.z, ja + 2, da.v[2]); acc_add(acc, a.w, ja + 3, da.v[3]);
+      acc_add(acc, b.x, jb, db.v[0]); acc_add(acc, b.y, jb + 1, db.v[1]); acc_add(acc, b.z, jb + 2, db.v[2]); acc_add(acc, b.w, jb + 3, db.v[3]);
+      acc_add(acc, c.x, jc, dc.v[0]); acc_add(acc, c.y, jc + 1, dc.v[1]); acc_add(acc, c.z, jc + 2, dc.v[2]); acc_add(acc, c.w, jc + 3, dc.v[3]);
+      acc_add(acc, d.x, jd, dd.v[0]); acc_add(acc, d.y, jd + 1, dd.v[1]); acc_add(acc, d.z, jd + 2, dd.v[2]); acc_add(acc, d.w, jd + 3, dd.v[3]);
+    }
+    for (; q < nq; q += 32) {
+      const float4 a = ld_stream4(x + 4 * q);
+      const int64_t ja = 4 * q;
+      DataCols<Acc, 4> da;
+      da.load4(acc, ja);
+      if constexpr (T::kElementDraws) da.draw4(*key, sw, row0 + r, (uint32_t)q);
+      acc_add(acc, a.x, ja, da.v[0]); acc_add(acc, a.y, ja + 1, da.v[1]); acc_add(acc, a.z, ja + 2, da.v[2]); acc_add(acc, a.w, ja + 3, da.v[3]);
+    }
+  } else {
+    for (int64_t j = lane; j < D; j += 32) {
+      DataCols<Acc, 1> dc;
+      dc.load1(acc, j, 0);
+      if constexpr (T::kElementDraws) dc.draw1(*key, sw, row0 + r, j, 0);
+      acc_add(acc, ld_stream1(x + j), j, dc.v[0]);
+    }
+  }
+  return acc_finish(acc, D, key, sw, (uint64_t)(row0 + r));
+}
+
 // The evaluation kernel.  Row r of X is global row noise.row0 + r of the draw (noise.key, stream word noise.key.stream_lo +
 // *noise.stream_off) for an accumulator with noise (evok_eval_keyed), which then gets the noise the sampler gave the row;
 // `noise` is an empty struct for every other accumulator.
@@ -809,107 +920,36 @@ __global__ void __launch_bounds__(kEvalThreads, AccTraits<Acc>::kEvalMinBlocks)
   const int64_t warps_total = (int64_t)gridDim.x * (kEvalThreads / 32);
   const int64_t gw = (int64_t)blockIdx.x * (kEvalThreads / 32) + (threadIdx.x >> 5);
   for (int64_t r = gw; r < n_rows; r += warps_total) {
-    Acc acc = acc_make<Acc>(D, data);
-    const float* x = X + r * ldx;
-    if constexpr (T::kWarpSteps) {
-      // warp-uniform steps (fold_step shuffles); per lane the groups, element adds, running sums and pair folds of
-      // sample_eval_kernel's VEC path in the same order, so both kernels give the same fitness bit for bit on the same X
-      constexpr bool kFoldNow = !T::kRunning;
-      StepCarry<Acc> carry;
-      if (VEC) {
-        const int64_t nq = D >> 2;
-        int64_t b = 0;
-        for (; b + 128 <= nq; b += 128) {
-          const int64_t q = b + lane;
-          float4 g[4];
-#pragma unroll
-          for (int k = 0; k < 4; ++k) g[k] = ld_stream4(x + 4 * (q + 32 * k));
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const int64_t jk = 4 * (q + 32 * k);
-            const float v[4] = {g[k].x, g[k].y, g[k].z, g[k].w};
-            DataCols<Acc, 4> dc;
-            dc.load4(acc, jk);
-            if constexpr (T::kElementDraws) dc.draw4(*key, sw, row0 + r, (uint32_t)(q + 32 * k));
-            if constexpr (T::kPairs)
-              if (jk > 0) dc.load_left(acc, jk);
-            if constexpr (kFoldNow) {
-              acc_add(acc, v[0], jk, dc.v[0]); acc_add(acc, v[1], jk + 1, dc.v[1]); acc_add(acc, v[2], jk + 2, dc.v[2]); acc_add(acc, v[3], jk + 3, dc.v[3]);
-            }
-            fold_step<4>(acc, v, jk, 4, carry, dc);
-          }
-        }
-        for (; b < nq; b += 32) {
-          const int64_t q = b + lane;
-          const bool active = q < nq;
-          const float4 a = active ? ld_stream4(x + 4 * q) : make_float4(0.f, 0.f, 0.f, 0.f);
-          const float v[4] = {a.x, a.y, a.z, a.w};
-          const int64_t ja = 4 * q;
-          DataCols<Acc, 4> dc;
-          if (active) {
-            dc.load4(acc, ja);
-            if constexpr (T::kElementDraws) dc.draw4(*key, sw, row0 + r, (uint32_t)q);
-            if constexpr (T::kPairs)
-              if (ja > 0) dc.load_left(acc, ja);
-            if constexpr (kFoldNow) {
-              acc_add(acc, v[0], ja, dc.v[0]); acc_add(acc, v[1], ja + 1, dc.v[1]); acc_add(acc, v[2], ja + 2, dc.v[2]); acc_add(acc, v[3], ja + 3, dc.v[3]);
-            }
-          }
-          fold_step<4>(acc, v, ja, active ? 4 : 0, carry, dc);
-        }
-      } else {
-        for (int64_t b = 0; b < D; b += 32) {
-          const int64_t j = b + lane;
-          const bool active = j < D;
-          const float v[1] = {active ? ld_stream1(x + j) : 0.f};
-          DataCols<Acc, 1> dc;
-          if (active) {
-            dc.load1(acc, j, 0);
-            if constexpr (T::kElementDraws) dc.draw1(*key, sw, row0 + r, j, 0);
-            if constexpr (T::kPairs)
-              if (j > 0) dc.load_left(acc, j);
-            if constexpr (kFoldNow) acc_add(acc, v[0], j, dc.v[0]);
-          }
-          fold_step<1>(acc, v, j, active ? 1 : 0, carry, dc);
-        }
-      }
-    } else if (VEC) {
-      const int64_t nq = D >> 2;
-      int64_t q = lane;
-      // 4 independent 128-bit loads in flight per lane
-      for (; q + 96 < nq; q += 128) {
-        const float4 a = ld_stream4(x + 4 * q), b = ld_stream4(x + 4 * (q + 32)), c = ld_stream4(x + 4 * (q + 64)),
-                     d = ld_stream4(x + 4 * (q + 96));
-        const int64_t ja = 4 * q, jb = 4 * (q + 32), jc = 4 * (q + 64), jd = 4 * (q + 96);
-        DataCols<Acc, 4> da, db, dc, dd;
-        da.load4(acc, ja); db.load4(acc, jb); dc.load4(acc, jc); dd.load4(acc, jd);
-        if constexpr (T::kElementDraws) {
-          const uint64_t row = row0 + r;
-          da.draw4(*key, sw, row, (uint32_t)q); db.draw4(*key, sw, row, (uint32_t)(q + 32));
-          dc.draw4(*key, sw, row, (uint32_t)(q + 64)); dd.draw4(*key, sw, row, (uint32_t)(q + 96));
-        }
-        acc_add(acc, a.x, ja, da.v[0]); acc_add(acc, a.y, ja + 1, da.v[1]); acc_add(acc, a.z, ja + 2, da.v[2]); acc_add(acc, a.w, ja + 3, da.v[3]);
-        acc_add(acc, b.x, jb, db.v[0]); acc_add(acc, b.y, jb + 1, db.v[1]); acc_add(acc, b.z, jb + 2, db.v[2]); acc_add(acc, b.w, jb + 3, db.v[3]);
-        acc_add(acc, c.x, jc, dc.v[0]); acc_add(acc, c.y, jc + 1, dc.v[1]); acc_add(acc, c.z, jc + 2, dc.v[2]); acc_add(acc, c.w, jc + 3, dc.v[3]);
-        acc_add(acc, d.x, jd, dd.v[0]); acc_add(acc, d.y, jd + 1, dd.v[1]); acc_add(acc, d.z, jd + 2, dd.v[2]); acc_add(acc, d.w, jd + 3, dd.v[3]);
-      }
-      for (; q < nq; q += 32) {
-        const float4 a = ld_stream4(x + 4 * q);
-        const int64_t ja = 4 * q;
-        DataCols<Acc, 4> da;
-        da.load4(acc, ja);
-        if constexpr (T::kElementDraws) da.draw4(*key, sw, row0 + r, (uint32_t)q);
-        acc_add(acc, a.x, ja, da.v[0]); acc_add(acc, a.y, ja + 1, da.v[1]); acc_add(acc, a.z, ja + 2, da.v[2]); acc_add(acc, a.w, ja + 3, da.v[3]);
-      }
-    } else {
-      for (int64_t j = lane; j < D; j += 32) {
-        DataCols<Acc, 1> dc;
-        dc.load1(acc, j, 0);
-        if constexpr (T::kElementDraws) dc.draw1(*key, sw, row0 + r, j, 0);
-        acc_add(acc, ld_stream1(x + j), j, dc.v[0]);
-      }
-    }
-    const float v = acc_finish(acc, D, key, sw, (uint64_t)(row0 + r));
+    const float v = eval_row<Acc, VEC>(lane, X, ldx, r, D, data, key, sw, row0);
+    if (lane == 0) f[r] = v;
+  }
+}
+
+// The evaluation of a batch of populations (evok_eval_batched): blockIdx.y = item b of the launch, whose rows are those of
+// X + b * item_stride_x (row pitch ldx; item stride 0 = every item evaluates the same rows), whose data is item b of the binding
+// (item_data) and whose fitnesses go to f[b * n_rows + r].  For an accumulator with noise, row r of item b is row r of the draw
+// (noise.key, stream word noise.key.stream_lo + b): the noise the batched sampler gives row r of item b with that key, so a
+// population it stored gets its fitnesses again.  noise.stream_off and noise.row0 are not read (null and 0).  Every item gets
+// the bits of one eval_kernel launch on its rows with stream id (stream id of the key) + b, on the same path.
+template <typename Acc, bool VEC>
+__global__ void __launch_bounds__(kEvalThreads, AccTraits<Acc>::kEvalMinBlocks)
+    eval_batched_kernel(const float* __restrict__ X, int64_t item_stride_x, int64_t ldx, int64_t n_rows, int64_t D, float* __restrict__ f,
+                        const typename AccTraits<Acc>::DataArg data, const typename AccTraits<Acc>::EvalArg noise) {
+  const int lane = threadIdx.x & 31;
+  const int64_t item = blockIdx.y;
+  X += item * item_stride_x;
+  f += item * n_rows;
+  const PhiloxKey* key = nullptr;
+  uint32_t sw = 0u;
+  if constexpr (AccTraits<Acc>::kNoise) {
+    key = &noise.key;
+    sw = noise.key.stream_lo + (uint32_t)item;
+  }
+  const typename AccTraits<Acc>::DataArg my_data = item_data(data, item);
+  const int64_t warps_total = (int64_t)gridDim.x * (kEvalThreads / 32);
+  const int64_t gw = (int64_t)blockIdx.x * (kEvalThreads / 32) + (threadIdx.x >> 5);
+  for (int64_t r = gw; r < n_rows; r += warps_total) {
+    const float v = eval_row<Acc, VEC>(lane, X, ldx, r, D, my_data, key, sw, 0);
     if (lane == 0) f[r] = v;
   }
 }

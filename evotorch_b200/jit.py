@@ -549,8 +549,16 @@ def batched_kernel_expressions() -> list:
             for sym in (False, True) for store in (False, True) for vec in (False, True)]
 
 
+def eval_batched_kernel_expressions() -> list:
+    """The 2 batched evaluation kernels of a registered objective, in the order of EVOK_OBJ_KERNEL_EVAL_BATCHED + vec of
+    include/evok.h.  They are compiled from the same source as `kernel_expressions`, as a third image, on the first batched
+    evaluation (`compile_eval_batched`)."""
+    return [f"evok::eval_batched_kernel<evok_user::Acc, {'true' if vec else 'false'}>" for vec in (False, True)]
+
+
 N_KERNELS = 22
 N_BATCHED_KERNELS = 8
+N_EVAL_BATCHED_KERNELS = 2
 # -default-device: the declarations of the C ABI in include/evok.h (reached through evok_sampler.cuh) are unannotated
 NVRTC_OPTIONS = ("--gpu-architecture=sm_90a", "-std=c++17", "--fmad=true", "--ptxas-options=-v", "-default-device", f"-I{CSRC}",
                  f"-I{INCLUDE}")
@@ -707,8 +715,17 @@ def register_batched(objective_id: int, cubin: bytes, names: list) -> None:
     nat.check(nat.lib().evok_objective_register_batched(objective_id, cubin, len(cubin), arr, len(names)), "evok_objective_register_batched")
 
 
+def register_eval_batched(objective_id: int, cubin: bytes, names: list) -> None:
+    """evok_objective_register_eval_batched: attach the batched evaluation kernels (in `eval_batched_kernel_expressions` order)
+    to a registered id."""
+    arr = (c_char_p * len(names))(*[n.encode() for n in names])
+    nat.check(nat.lib().evok_objective_register_eval_batched(objective_id, cubin, len(cubin), arr, len(names)),
+              "evok_objective_register_eval_batched")
+
+
 _cache: Dict[str, CompiledObjective] = {}
 _batched_cache: Dict[str, CompiledObjective] = {}
+_eval_batched_cache: Dict[str, CompiledObjective] = {}
 _cache_lock = threading.Lock()
 
 
@@ -737,4 +754,18 @@ def compile_batched(spec: ObjectiveSpec) -> CompiledObjective:
             register_batched(base.objective_id, c.cubin, c.names)
             c.objective_id = base.objective_id
             _batched_cache[spec.source] = c
+        return c
+
+
+def compile_eval_batched(spec: ObjectiveSpec) -> CompiledObjective:
+    """Compile the batched evaluation kernels of `spec` and attach them to its registered id, once per process for one generated
+    source."""
+    base = compile_objective(spec)
+    with _cache_lock:
+        c = _eval_batched_cache.get(spec.source)
+        if c is None:
+            c = compile_source(spec.source, eval_batched_kernel_expressions())
+            register_eval_batched(base.objective_id, c.cubin, c.names)
+            c.objective_id = base.objective_id
+            _eval_batched_cache[spec.source] = c
         return c

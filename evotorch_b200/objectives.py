@@ -41,6 +41,34 @@ class BuiltinObjective:
             return ops.evaluate(self.evok_objective_id, x)
         return self._torch_fn(x)
 
+    def evaluate_batched(self, values: torch.Tensor, *, seed: Optional[int] = None) -> torch.Tensor:
+        """The fitnesses (..., n) of a batch of populations `values` (..., n, D), for example the asks of a batched full-covariance
+        CMA-ES.  On CUDA float32 values, with a fused kernel, one launch evaluates every item: item b (in row-major order of the
+        batch dimensions) draws the noise of an objective with noise from Philox key `seed` on stream b, so row i of item b gets
+        the noise the batched sampler gives row i of item b with that seed (no seed: a fresh one from torch's generator).
+        Anywhere else this is the torch function.  An objective with per-item data needs values of its `data_batch_shape`
+        (ValueError naming both shapes otherwise)."""
+        if values.ndim < 2:
+            raise ValueError(f"values: expected a batch of populations of shape (..., n, D), got {tuple(values.shape)}")
+        batch, (n, d) = tuple(values.shape[:-2]), tuple(values.shape[-2:])
+        per_item = tuple(getattr(self, "data_batch_shape", ()))
+        if per_item and per_item != batch:
+            raise ValueError(f"the data of {self!r} has batch shape {per_item}, the values {batch}: every item of the data evaluates "
+                             "the population of its own item")
+        oid = self.evok_objective_id
+        if oid is None or not ops.uses_kernels(values):
+            return self._torch_fn(values)
+        if hasattr(self, "compile_eval_batched"):  # a FusedObjective: its batched evaluation is compiled on the first use
+            self.compile_eval_batched()
+        if seed is None:
+            from .algorithms.functional.misc import draw_philox_seed
+
+            seed = draw_philox_seed()
+        X = values.reshape(math.prod(batch), n, d)
+        if d > 1 and X.stride(2) != 1:
+            X = X.contiguous()
+        return ops.evaluate_batched(oid, X, seed=seed).view(batch + (n,))
+
     def __repr__(self) -> str:
         return f"<evotorch_b200.objectives.{self.name}>"
 
@@ -75,6 +103,8 @@ class FusedObjective(BuiltinObjective):
 
     The batched samplers of the functional API (`pgpe_ask_and_evaluate`, `cem_ask_and_evaluate`) are 8 more kernels of the same
     source, compiled on the first batched use (`compile_batched`); `batched_kernel_info` then holds their registers and spills.
+    The batched evaluation (`evaluate_batched`, `cmaes_ask_and_evaluate`) is 2 more, compiled on its first use
+    (`compile_eval_batched`), with `eval_batched_kernel_info`.
 
     `prods`, `maxs` and `mins` are reductions of terms like those of `sums`, by product, maximum and minimum; with `sums` they
     are at most 4 in all and share one namespace.  An empty reduction (a pair term at D = 1) is 0, 1, -inf or +inf, and a NaN
@@ -130,6 +160,7 @@ class FusedObjective(BuiltinObjective):
         self.prods, self.maxs, self.mins, self.running = dict(spec.prods), dict(spec.maxs), dict(spec.mins), dict(spec.running)
         self.kernel_info = compiled.kernel_info
         self.batched_kernel_info = None
+        self.eval_batched_kernel_info = None
         self.noisy = spec.noisy
         self._spec = spec
         if self.data:
@@ -206,6 +237,13 @@ class FusedObjective(BuiltinObjective):
             from . import jit
 
             self.batched_kernel_info = jit.compile_batched(self._spec).kernel_info
+
+    def compile_eval_batched(self) -> None:
+        """Compile and attach the batched evaluation kernels (once per process for one source); fills `eval_batched_kernel_info`."""
+        if self.eval_batched_kernel_info is None:
+            from . import jit
+
+            self.eval_batched_kernel_info = jit.compile_eval_batched(self._spec).kernel_info
 
     def __reduce__(self):
         args = (self.name, self.sums, self.value) + ((self.data,) if self.data else ())

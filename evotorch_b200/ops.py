@@ -258,6 +258,31 @@ def evaluate_keyed(objective: int, X: torch.Tensor, *, seed: int, stream_id: int
     return f
 
 
+def evaluate_batched(objective: int, X: torch.Tensor, *, seed: int, stream_id0: int = 0, f: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """K2 for a batch of populations in one launch: f[b, i] = objective(X[b, i]) for X (items, N, D) float32 CUDA with unit
+    column stride (any item stride and row pitch), f (items, N).  Item b is evaluated as `evaluate_keyed(..., stream_id=stream_id0
+    + b)` on its rows: an objective with noise draws row i of item b's noise from the draw (seed, stream_id0 + b), the noise the
+    batched sampler gave row i of item b.  Per-item data of an instance is item b's.  A registered objective needs its batched
+    evaluation kernels (`FusedObjective.compile_eval_batched`)."""
+    if not (X.is_cuda and X.dtype == torch.float32 and X.ndim == 3 and (X.shape[2] <= 1 or X.stride(2) == 1)):
+        raise ValueError(f"X: expected a float32 CUDA tensor of shape (items, N, D) with unit column stride, got {tuple(X.shape)} "
+                         f"strides {X.stride()} {X.dtype} {X.device}")
+    B, n, D = X.shape
+    # the stride of a dimension of size 1 is arbitrary in torch: an item or row that has no successor needs none
+    item_stride = X.stride(0) if B > 1 else 0
+    ldx = X.stride(1) if n > 1 else D
+    if f is None:
+        f = torch.empty(B, n, dtype=torch.float32, device=X.device)
+    f = _rows(f, "f", (B, n))
+    _check_data_device(objective, X)
+    if B == 0 or n == 0:  # nothing to evaluate (and an empty tensor may have no storage to point at)
+        return f
+    with _timed("eval"):
+        rc = nat.lib().evok_eval_batched(objective, X.data_ptr(), item_stride, ldx, B, n, D, seed, stream_id0, f.data_ptr(), nat.stream_of(X))
+    nat.check(rc, "evok_eval_batched")
+    return f
+
+
 # ------------------------------------------------------------------------------------------------ K3
 def _rank_ws(device: torch.device, n: int) -> torch.Tensor:
     return nat.workspace(device, nat.lib().evok_rank_workspace_bytes(n), "rank")

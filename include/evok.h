@@ -155,6 +155,19 @@ int evok_objective_load(int objective);
 #define EVOK_OBJ_BATCHED_KERNELS 8
 int evok_objective_register_batched(int objective, const void* cubin, size_t bytes, const char* const* kernel_names_host, int n_kernels);
 
+/* The batched evaluation of an objective (evok_eval_batched) is a third family, in a third image, so that a registered objective
+ * that never evaluates batched populations compiles and loads neither it nor the batched samplers:
+ *   EVOK_OBJ_KERNEL_EVAL_BATCHED + vec : eval_batched_kernel<Acc, vec>
+ * evok_objective_register_eval_batched attaches the sm_90a cubin of these EVOK_OBJ_EVAL_BATCHED_KERNELS kernels (lowered names in
+ * this order, positions counted from EVOK_OBJ_KERNEL_EVAL_BATCHED) to the registered id `objective`, as
+ * evok_objective_register_batched does for the batched samplers; the module is loaded on a device by the first
+ * evok_eval_batched there.  A registered id without this image yields EVOK_E_NOKERNEL from evok_eval_batched.
+ * Errors: EVOK_E_NULLPTR, EVOK_E_BADSIZE (bytes == 0, n_kernels != EVOK_OBJ_EVAL_BATCHED_KERNELS), EVOK_E_BADENUM (`objective`
+ * is a built-in id or is not registered). */
+#define EVOK_OBJ_KERNEL_EVAL_BATCHED 30
+#define EVOK_OBJ_EVAL_BATCHED_KERNELS 2
+int evok_objective_register_eval_batched(int objective, const void* cubin, size_t bytes, const char* const* kernel_names_host, int n_kernels);
+
 /* Objectives with noise.  The accumulator of a registered objective may draw uniform and normal noise from the Philox key of
  * the population it evaluates (kNoise in csrc/evok_sampler.cuh); its eval_kernel<Acc, vec> then takes the draw of the rows as
  * its last argument.  evok_objective_declare_noise tells the library so, right after
@@ -420,6 +433,23 @@ int evok_sample_batched(float* X, int64_t item_stride_x, int64_t ldx, const floa
 int evok_sample_eval_batched(int objective, float* X, int64_t item_stride_x, int64_t ldx, const float* mu, int64_t item_stride_mu,
                              const float* sigma, int64_t item_stride_sigma, int64_t n_items, int64_t n_rows, int64_t D, int symmetric,
                              uint64_t seed, uint64_t stream_id0, float* f, void* stream);
+/* K2 for a batch of populations in one launch per 65535 items (the populations of a full-covariance CMA-ES, or values a caller
+ * asked, repaired or injected): item b evaluates the n_rows rows of X + b * item_stride_x (row pitch ldx; item_stride_x = 0: every
+ * item evaluates the same rows) with item b of the objective's data and writes f[b * n_rows ...] (f: [items][n_rows],
+ * contiguous).  Per item, f is bit-identical to evok_eval_keyed(objective, X + b * item_stride_x, ldx, row0 = 0, n_rows, D, seed,
+ * stream_id0 + b, NULL, ...) on the same path (the vectorised one needs D % 4 == 0, a 16-byte aligned X, ldx and item_stride_x
+ * multiples of 4 and the data vectors' alignment of evok_objective_instance).  Only an objective with noise uses the key: row r of
+ * item b then gets the noise that evok_sample_eval_batched(..., seed, stream_id0) gives row r of item b, so a population it stored
+ * gets its fitnesses again.  An instance with per-item data (n_items > 1) gives item b its item b.
+ * objective: a built-in id other than EVOK_OBJ_NONE, or a registered id with its batched evaluation image
+ * (evok_objective_register_eval_batched), or an instance of one.  Grid: y = item, x = the resident CTAs of the kernel shared over
+ * the items of a launch, at least 1 and at most what the rows need; zero items or zero rows launch nothing.
+ * Errors in this order: EVOK_E_NULLPTR (X, f), EVOK_E_BADENUM (EVOK_OBJ_NONE, an id out of range or not registered),
+ * EVOK_E_BADSIZE (negative n_items, n_rows or item_stride_x, D <= 0, ldx < D, an instance whose n_items is neither 1 nor the
+ * call's), EVOK_E_NOKERNEL, EVOK_E_NODATA (a registered id that declares data, not launched through an instance), EVOK_E_BADSIZE
+ * (a data vector whose length is not D). */
+int evok_eval_batched(int objective, const float* X, int64_t item_stride_x, int64_t ldx, int64_t n_items, int64_t n_rows, int64_t D,
+                      uint64_t seed, uint64_t stream_id0, float* f, void* stream);
 /* K3: f, w: [items][N].  ws: max(evok_rank_workspace_bytes(N), 8 * min(n_items, 65535) + 256) bytes */
 int evok_rank_batched(int method, const float* f, int64_t N, int64_t n_items, int higher_is_better, float* w, void* ws, size_t ws_bytes,
                       void* stream);
