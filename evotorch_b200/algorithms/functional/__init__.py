@@ -25,6 +25,13 @@ with the ask's Philox draw, so per-item data and noise reach CMA-ES too:
 
     population, evals = cmaes_ask_and_evaluate(state, objective=shifted_sphere)   # data of batch shape (1024,)
     state = cmaes_tell(state, population, evals)
+
+`restarts` wraps a `cmaes` or `sepcmaes` state for multi-start search: per item, best-ever tracking, termination criteria and
+re-initialisation on the device, each item with its own generation counter:
+
+    rs = restarts(state, lb=-5.0, ub=5.0)
+    values, evals = cmaes_ask_and_evaluate(rs.search, objective=rastrigin)
+    rs = restarts_tell(rs, values, evals)                # rs.best_values, rs.best_evals, rs.num_restarts, rs.stop_flags
 """
 
 from .funcadam import AdamState, adam, adam_ask, adam_tell
@@ -32,6 +39,7 @@ from .funccem import CEMState, cem, cem_ask, cem_ask_and_evaluate, cem_tell
 from .funcclipup import ClipUpState, clipup, clipup_ask, clipup_tell
 from .funccmaes import CMAESState, cmaes, cmaes_ask, cmaes_ask_and_evaluate, cmaes_tell
 from .funcpgpe import PGPEState, pgpe, pgpe_ask, pgpe_ask_and_evaluate, pgpe_tell
+from .funcrestarts import RestartState, restarts, restarts_tell
 from .fused import LazyPopulation
 from .funcsepcmaes import SepCMAESState, sepcmaes, sepcmaes_ask, sepcmaes_ask_and_evaluate, sepcmaes_tell
 from .funcsgd import SGDState, sgd, sgd_ask, sgd_tell
@@ -39,5 +47,6 @@ from .misc import OptimizerFunctions, get_functional_optimizer
 
 __all__ = ["AdamState", "adam", "adam_ask", "adam_tell", "CEMState", "cem", "cem_ask", "cem_ask_and_evaluate", "cem_tell", "ClipUpState",
            "clipup", "clipup_ask", "clipup_tell", "CMAESState", "cmaes", "cmaes_ask", "cmaes_ask_and_evaluate", "cmaes_tell", "LazyPopulation", "PGPEState", "pgpe", "pgpe_ask", "pgpe_ask_and_evaluate", "pgpe_tell",
+           "RestartState", "restarts", "restarts_tell",
            "SepCMAESState", "sepcmaes", "sepcmaes_ask", "sepcmaes_ask_and_evaluate", "sepcmaes_tell",
            "SGDState", "sgd", "sgd_ask", "sgd_tell", "OptimizerFunctions", "get_functional_optimizer"]

@@ -169,6 +169,13 @@ def _limit_stdev(C: torch.Tensor, sigma: torch.Tensor, lo: Optional[float], hi: 
 def cmaes_tell(state: CMAESState, values: torch.Tensor, evals: torch.Tensor) -> CMAESState:
     """The next state, given a population `values` (..., popsize, D) and its fitnesses `evals` (..., popsize).  The state passed
     in is left unchanged."""
+    return _tell(state, values, evals, state.generation)[0]
+
+
+def _tell(state: CMAESState, values: torch.Tensor, evals: torch.Tensor, steps) -> tuple:
+    """(`cmaes_tell`'s next state, the generation counters after it).  `steps` drives h_sig and the decomposition schedule: the
+    int `state.generation`, or a (B,) int64 tensor of per-item counters (then every item is factored and keeps its old A unless
+    (steps + 1) % decompose_C_freq == 0 for it)."""
     if isinstance(values, LazyPopulation):
         raise ValueError("The functional CMA-ES recovers its steps from the values: a lazy population cannot be told; ask for the values")
     batch, B, d = _items(state)
@@ -185,16 +192,25 @@ def cmaes_tell(state: CMAESState, values: torch.Tensor, evals: torch.Tensor) -> 
     x, f = values.reshape(B, n, d), evals.reshape(B, n)
     y = (x - m[:, None, :]) / sigma[:, None, None]
     z = torch.linalg.solve_triangular(A.mT, y, upper=True, left=False).contiguous()  # z A^T = y
+    per_item = isinstance(steps, torch.Tensor)
     if on_kernels(m, x, f):
-        m, p_sigma, p_c, sigma, C_new = _tell_kernels(state, hp, B, n, d, m, sigma, C, y, z, f)
+        counters = steps.clone() if per_item else steps  # the kernel increments per-item counters in place
+        m, p_sigma, p_c, sigma, C_new = _tell_kernels(state, hp, B, n, d, m, sigma, C, y, z, f, counters)
+        steps_next = counters if per_item else steps + 1
     else:
-        m, p_sigma, p_c, sigma, C_new = _tell_torch(state, hp, B, n, d, m, sigma, C, y, z, f)
+        m, p_sigma, p_c, sigma, C_new = _tell_torch(state, hp, B, n, d, m, sigma, C, y, z, f, steps)
+        steps_next = steps + 1
     _limit_stdev(C_new, sigma, state.stdev_min, state.stdev_max)
     A_new = A
-    if (state.generation + 1) % hp.decompose_C_freq == 0:
+    if per_item:
         A_new, _ = torch.linalg.cholesky_ex(C_new, check_errors=False)
-    return state._replace(center=m.view(batch + (d,)), sigma=sigma.view(batch), C=C_new.view(batch + (d, d)), A=A_new.view(batch + (d, d)),
-                          p_sigma=p_sigma.view(batch + (d,)), p_c=p_c.view(batch + (d,)), generation=state.generation + 1)
+        if hp.decompose_C_freq > 1:
+            A_new = torch.where((steps_next % hp.decompose_C_freq == 0)[:, None, None], A_new, A)
+    elif (state.generation + 1) % hp.decompose_C_freq == 0:
+        A_new, _ = torch.linalg.cholesky_ex(C_new, check_errors=False)
+    new = state._replace(center=m.view(batch + (d,)), sigma=sigma.view(batch), C=C_new.view(batch + (d, d)), A=A_new.view(batch + (d, d)),
+                         p_sigma=p_sigma.view(batch + (d,)), p_c=p_c.view(batch + (d,)), generation=state.generation + 1)
+    return new, steps_next
 
 
 def _consts(hp: CMAESHyperparameters) -> tuple:
@@ -202,8 +218,9 @@ def _consts(hp: CMAESHyperparameters) -> tuple:
             float(hp.unbiased_expectation), hp.weights_sum)
 
 
-def _tell_kernels(state, hp, B, n, d, m, sigma, C, y, z, f) -> tuple:
-    """The stages of CMAES._step_fused for all items at once, one launch each; every output is a new tensor."""
+def _tell_kernels(state, hp, B, n, d, m, sigma, C, y, z, f, steps) -> tuple:
+    """The stages of CMAES._step_fused for all items at once, one launch each; every output is a new tensor.  `steps`: the shared
+    int counter, or the per-item int64 counters, which the vector update increments."""
     dev = m.device
     new = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=dev)  # noqa: E731
     aw, w_pos, w_act = new(B, n), new(B, n), new(B, n)
@@ -216,7 +233,7 @@ def _tell_kernels(state, hp, B, n, d, m, sigma, C, y, z, f) -> tuple:
     m, sigma = m.clone(), sigma.clone()
     p_sigma, p_c = state.p_sigma.reshape(B, d).clone(), state.p_c.reshape(B, d).clone()
     k = new(B, 3)
-    ops.cmaes_vector_update_batched(local, shaped, m, p_sigma, p_c, sigma, _consts(hp), state.csa_squared, k, steps=state.generation)
+    ops.cmaes_vector_update_batched(local, shaped, m, p_sigma, p_c, sigma, _consts(hp), state.csa_squared, k, steps=steps)
     C_new = ops.weighted_syrk_update_batched(y, w_act, k, C.contiguous(), u=p_c, out=new(B, d, d))
     return m, p_sigma, p_c, sigma, C_new
 
@@ -229,8 +246,19 @@ def _assigned_weights(f: torch.Tensor, maximize: bool, weights: torch.Tensor) ->
     return weights.to(f.device)[ranks]
 
 
-def _tell_torch(state, hp, B, n, d, m, sigma, C, y, z, f) -> tuple:
-    """The same stages as batched torch ops (CMAES's op-by-op generation: update_m ... update_C, cmaes.py:454-553)."""
+def _h_sig(hp: CMAESHyperparameters, pnorm: torch.Tensor, d: int, steps) -> torch.Tensor:
+    """CMAES._h_sig per item, with the generation counter `steps` (an int, or a tensor of per-item counters) before its increment."""
+    if isinstance(steps, torch.Tensor):
+        decay = 1 - torch.full_like(pnorm, 1 - hp.c_sigma).pow((2 * steps + 1).to(pnorm.dtype))
+    else:
+        decay = 1 - (1 - hp.c_sigma) ** (2 * steps + 1)
+    squared_sum = pnorm.pow(2.0) / decay
+    return ((squared_sum / d) - 1 < 1 + 4.0 / (d + 1)).to(pnorm.dtype)
+
+
+def _tell_torch(state, hp, B, n, d, m, sigma, C, y, z, f, steps) -> tuple:
+    """The same stages as batched torch ops (CMAES's op-by-op generation: update_m ... update_C, cmaes.py:454-553), with the
+    generation counter `steps` (an int, or per-item counters)."""
     aw = _assigned_weights(f, state.maximize, hp.weights)
     w_pos = torch.clamp_min(aw, 0.0)
     local = torch.einsum("bn,bnd->bd", w_pos, z)
@@ -243,8 +271,7 @@ def _tell_torch(state, hp, B, n, d, m, sigma, C, y, z, f) -> tuple:
     else:
         expo = pnorm / hp.unbiased_expectation - 1
     sigma = sigma * torch.exp((hp.c_sigma / hp.damp_sigma) * expo)
-    squared_sum = pnorm.pow(2.0) / (1 - (1 - hp.c_sigma) ** (2 * state.generation + 1))
-    h_sig = ((squared_sum / d) - 1 < 1 + 4.0 / (d + 1)).to(m.dtype)
+    h_sig = _h_sig(hp, pnorm, d, steps)
     p_c = (1 - hp.c_c) * state.p_c.reshape(B, d) + (h_sig * hp.variance_discount_c)[:, None] * shaped
     w = torch.where(aw > 0, aw, d * aw / torch.sum(z * z, dim=-1)) if state.active else aw
     c1a = hp.c_1 * (1 - (1 - h_sig**2) * hp.c_c * (2 - hp.c_c))

@@ -1,0 +1,196 @@
+"""Restarts for the functional CMA-ES families: `restarts(state, ...) -> RestartState`, `restarts_tell(rs, values, evals)`.
+
+A batch of `cmaes` or `sepcmaes` searches used as a multi-start global optimiser: every item keeps its best solution ever, checks
+the termination criteria of Hansen's tutorial (The CMA Evolution Strategy: A Tutorial, appendix B.3) after each of its updates,
+and starts again from a uniform centre in [lb, ub] with its initial step size when one fires.  Each item has its own generation
+counter, which drives its h_sig and its decomposition schedule, so a restarted item runs exactly as a fresh search would.
+
+    state = cmaes(center_init=torch.empty(1024, 10, device="cuda").uniform_(-5, 5), stdev_init=2.0, objective_sense="min")
+    rs = restarts(state, lb=-5.0, ub=5.0)
+    for _ in range(generations):
+        values, evals = cmaes_ask_and_evaluate(rs.search, objective=rastrigin)
+        rs = restarts_tell(rs, values, evals)
+    rs.best_values, rs.best_evals, rs.num_restarts
+
+On CUDA float32 a generation is the family's stages, with per-item counters in the update, and one restart stage (one launch;
+two for the full family, whose second launch resets C and A of the restarted items): nothing is read back to the host.  With
+decompose_C_freq > 1 the full family then factors C of every item in every generation and keeps the old factor where the item
+is not due, since which items are due is only known on the device.  Anywhere else the same algorithm runs as batched torch ops.
+
+`stop_flags` bits (ops.RESTART_CRITERIA): 0 tol_fun, 1 tol_x, 2 tol_x_up, 3 max_condition, 4 min_fitness_stdev, 5 max_generations,
+6 non-finite state (always on).
+"""
+
+from __future__ import annotations
+
+import math
+from typing import NamedTuple, Optional, Union
+
+import torch
+
+from ... import ops
+from . import funccmaes, funcsepcmaes
+from .funccmaes import CMAESState, _host_float
+from .funcsepcmaes import SepCMAESState
+from .fused import LazyPopulation
+from .misc import draw_philox_seed, on_kernels
+
+
+class RestartState(NamedTuple):
+    search: Union[CMAESState, SepCMAESState]  # the state to ask from
+    best_values: torch.Tensor  # (..., D): the best solution ever per item, over all of its restarts (NaN until one was finite)
+    best_evals: torch.Tensor  # (...): its fitness (+inf for "min", -inf for "max" until then)
+    num_restarts: torch.Tensor  # (...) int64
+    item_generation: torch.Tensor  # (...) int64: generations since the item's (re)start
+    history: torch.Tensor  # (..., H): ring of the best fitness of the item's last H generations, slot (g - 1) % H for generation g
+    stop_flags: torch.Tensor  # (...) int32: the criteria that fired in the last tell
+    stdev_init: torch.Tensor  # (...): the step size an item restarts with
+    lb: torch.Tensor  # (..., D)
+    ub: torch.Tensor  # (..., D)
+    tol_fun: Optional[float]
+    tol_x: Optional[float]
+    tol_x_up: Optional[float]
+    max_condition: Optional[float]
+    min_fitness_stdev: Optional[float]
+    max_generations: Optional[float]
+
+    @property
+    def thresholds(self) -> tuple:
+        """The thresholds in the order of ops.RESTART_CRITERIA (None = off)."""
+        return tuple(getattr(self, name) for name in ops.RESTART_CRITERIA)
+
+
+def history_length(d: int, popsize: int) -> int:
+    """H = 10 + ceil(30 D / popsize): the generations the tol_fun criterion looks back over."""
+    return 10 + math.ceil(30 * d / popsize)
+
+
+def restarts(state: Union[CMAESState, SepCMAESState], *, lb, ub, tol_fun: Optional[float] = 1e-12, tol_x: Optional[float] = 1e-12,
+             tol_x_up: Optional[float] = 1e4, max_condition: Optional[float] = 1e14, min_fitness_stdev: Optional[float] = None,
+             max_generations: Optional[int] = None) -> RestartState:
+    """A restart state around `state` (a `CMAESState` or `SepCMAESState`).  `lb`, `ub`: the box the restarted centres are drawn
+    from, scalars, (D,) or (..., D), finite with lb < ub.  A threshold of None turns its criterion off.  Every item's generation
+    counter starts at `state.generation` and its restart step size is its current sigma."""
+    if not isinstance(state, (CMAESState, SepCMAESState)):
+        raise TypeError(f"`restarts` takes a CMAESState or a SepCMAESState, got {type(state).__name__}")
+    center = state.center
+    batch, d = tuple(center.shape[:-1]), center.shape[-1]
+    bounds = []
+    for name, v in (("lb", lb), ("ub", ub)):
+        t = torch.as_tensor(v, dtype=center.dtype, device=center.device)
+        try:
+            t = t.expand(batch + (d,))
+        except RuntimeError:
+            raise ValueError(f"`{name}` of shape {tuple(t.shape)} does not broadcast to the search's {batch + (d,)}") from None
+        bounds.append(t.contiguous().clone())
+    lb_t, ub_t = bounds
+    if not bool(torch.isfinite(lb_t).all() & torch.isfinite(ub_t).all() & (lb_t < ub_t).all()):
+        raise ValueError("`lb` and `ub` must be finite with lb < ub")
+    th = {}
+    for name, v in (("tol_fun", tol_fun), ("tol_x", tol_x), ("tol_x_up", tol_x_up), ("max_condition", max_condition),
+                    ("min_fitness_stdev", min_fitness_stdev), ("max_generations", max_generations)):
+        th[name] = None if v is None else _host_float(v, name)
+    maximize = state.maximize
+    H = history_length(d, state.popsize)
+    opts = dict(dtype=center.dtype, device=center.device)
+    return RestartState(
+        search=state,
+        best_values=torch.full(batch + (d,), math.nan, **opts),
+        best_evals=torch.full(batch, -math.inf if maximize else math.inf, **opts),
+        num_restarts=torch.zeros(batch, dtype=torch.int64, device=center.device),
+        item_generation=torch.full(batch, state.generation, dtype=torch.int64, device=center.device),
+        history=torch.full(batch + (H,), math.nan, **opts),
+        stop_flags=torch.zeros(batch, dtype=torch.int32, device=center.device),
+        stdev_init=state.sigma.clone(),
+        lb=lb_t,
+        ub=ub_t,
+        **th,
+    )
+
+
+def restarts_tell(rs: RestartState, values: Union[torch.Tensor, LazyPopulation], evals: torch.Tensor) -> RestartState:
+    """The family's tell with per-item generation counters, then per item: best ever, history, the criteria, and the re-initialisation
+    of the items that met one.  `values` as the family's tell takes it (a separable search also takes the LazyPopulation that
+    `sepcmaes_ask_and_evaluate(..., lazy=True)` returned).  `rs` is left unchanged."""
+    search = rs.search
+    sep = isinstance(search, SepCMAESState)
+    center = search.center
+    batch, d = tuple(center.shape[:-1]), center.shape[-1]
+    B, n = math.prod(batch), search.popsize
+    family = funcsepcmaes if sep else funccmaes
+    new, steps = family._tell(search, values, evals, rs.item_generation.reshape(B))
+    f = torch.as_tensor(evals, dtype=center.dtype, device=center.device).reshape(B, n)
+    lazy = isinstance(values, LazyPopulation)
+    x = None if lazy else torch.as_tensor(values, dtype=center.dtype, device=center.device).reshape(B, n, d)
+    mat = (B, d) if sep else (B, d, d)
+    st = dict(m=new.center.reshape(B, d), sigma=new.sigma.reshape(B), p_sigma=new.p_sigma.reshape(B, d), p_c=new.p_c.reshape(B, d),
+              C=new.C.reshape(mat), A=new.A.reshape(mat), s=new.s.reshape(B, d) if sep else None)
+    r = dict(history=rs.history.reshape(B, -1).clone(), best_x=rs.best_values.reshape(B, d).clone(), best_f=rs.best_evals.reshape(B).clone(),
+             num_restarts=rs.num_restarts.reshape(B).clone())
+    sigma0, lb, ub = rs.stdev_init.reshape(B), rs.lb.reshape(B, d), rs.ub.reshape(B, d)
+    if lazy or on_kernels(center):
+        # in place on the tell's fresh tensors and on the clones above
+        flags = torch.empty(B, dtype=torch.int32, device=center.device)
+        draw = dict(m_draw=search.center.reshape(B, d), s_draw=search.s.reshape(B, d), draw_seed=values.seed) if lazy else {}
+        ops.cma_restart_batched(sep, f.contiguous(), None if lazy else x.contiguous(), search.maximize, steps, st["m"], st["sigma"], st["p_sigma"],
+                                st["p_c"], st["C"], st["A"], st["s"], r["history"], r["best_x"], r["best_f"], r["num_restarts"], flags,
+                                sigma0.contiguous(), lb, ub, rs.thresholds, seed=draw_philox_seed(), **draw)
+    else:
+        st, r, steps, flags = _restart_torch(rs.thresholds, sep, search.maximize, f, x, steps, st, r, sigma0, lb, ub)
+    vec = batch + (d,)
+    new = new._replace(center=st["m"].view(vec), sigma=st["sigma"].view(batch), p_sigma=st["p_sigma"].view(vec), p_c=st["p_c"].view(vec),
+                       C=st["C"].view(vec if sep else vec + (d,)), A=st["A"].view(vec if sep else vec + (d,)),
+                       **({"s": st["s"].view(vec)} if sep else {}))
+    return rs._replace(search=new, best_values=r["best_x"].view(vec), best_evals=r["best_f"].view(batch), num_restarts=r["num_restarts"].view(batch),
+                       item_generation=steps.view(batch), history=r["history"].view(batch + (-1,)), stop_flags=flags.view(batch))
+
+
+def _restart_torch(thresholds, sep, maximize, f, x, gen, st, r, sigma0, lb, ub) -> tuple:
+    """The restart stage as batched torch ops (the semantics of evok_cma_restart_batched; the new centres from torch.rand(B, D))."""
+    B, n = f.shape
+    d = lb.shape[-1]
+    H = r["history"].shape[-1]
+    nan = torch.tensor(math.nan, dtype=f.dtype, device=f.device)
+    fin = torch.isfinite(f)
+    key = torch.where(fin, f, -math.inf if maximize else math.inf)
+    idx = key.argmax(-1) if maximize else key.argmin(-1)  # the first of equal values: the lower row wins ties
+    g_best = key.gather(-1, idx[:, None])[:, 0]
+    has = fin.any(-1)
+    improved = has & (g_best > r["best_f"] if maximize else g_best < r["best_f"])
+    best_x = torch.where(improved[:, None], x[torch.arange(B), idx], r["best_x"])
+    best_f = torch.where(improved, g_best, r["best_f"])
+    slot = torch.remainder(gen - 1, H)
+    written = r["history"].scatter(1, slot[:, None], torch.where(has, g_best, nan)[:, None])
+    history = torch.where((gen >= 1)[:, None], written, r["history"])
+
+    sig, m, p_sigma, p_c, C, A = st["sigma"], st["m"], st["p_sigma"], st["p_c"], st["C"], st["A"]
+    c_diag = C if sep else torch.diagonal(C, dim1=-2, dim2=-1)
+    r_diag = C if sep else torch.diagonal(A, dim1=-2, dim2=-1)
+    nan_to = lambda t, v: torch.where(torch.isnan(t), v, t)  # noqa: E731 -- maxima and minima ignore NaN (fmaxf / fminf)
+    max_pc = nan_to(p_c.abs(), 0.0).amax(-1).clamp_min(0.0)
+    max_sd = nan_to(c_diag.sqrt(), 0.0).amax(-1).clamp_min(0.0)
+    ratio = nan_to(r_diag, -math.inf).amax(-1) / nan_to(r_diag, math.inf).amin(-1)
+    zero = torch.zeros(B, dtype=torch.bool, device=f.device)
+    th = dict(zip(ops.RESTART_CRITERIA, thresholds))
+    bits = [
+        zero if th["tol_fun"] is None else ((gen >= H) & fin.all(-1) & torch.isfinite(history).all(-1)
+                                            & (torch.maximum(f.amax(-1), history.amax(-1)) - torch.minimum(f.amin(-1), history.amin(-1)) < th["tol_fun"])),
+        zero if th["tol_x"] is None else sig * torch.maximum(max_pc, max_sd) < th["tol_x"] * sigma0,
+        zero if th["tol_x_up"] is None else sig * max_sd > th["tol_x_up"] * sigma0,
+        zero if th["max_condition"] is None else (ratio if sep else ratio * ratio) > th["max_condition"],
+        zero if th["min_fitness_stdev"] is None or n < 2 else f.std(-1) < th["min_fitness_stdev"],
+        zero if th["max_generations"] is None else gen >= th["max_generations"],
+        ~(sig > 0) | ~torch.isfinite(sig) | ~torch.isfinite(torch.cat([m, p_sigma, p_c, c_diag], -1)).all(-1),
+    ]
+    flags = sum(b.to(torch.int32) << k for k, b in enumerate(bits))
+    go = flags != 0
+    centre = lb + (ub - lb) * torch.rand(B, d, dtype=f.dtype, device=f.device)
+    col = go[:, None]
+    out = dict(m=torch.where(col, centre, m), sigma=torch.where(go, sigma0, sig), p_sigma=torch.where(col, 0.0, p_sigma), p_c=torch.where(col, 0.0, p_c))
+    if sep:
+        out.update(C=torch.where(col, 1.0, C), A=torch.where(col, 1.0, A), s=torch.where(col, sigma0[:, None].expand(B, d), st["s"]))
+    else:
+        eye = torch.eye(d, dtype=f.dtype, device=f.device)
+        out.update(C=torch.where(go[:, None, None], eye, C), A=torch.where(go[:, None, None], eye, A), s=None)
+    r = dict(history=torch.where(col, nan, history), best_x=best_x, best_f=best_f, num_restarts=r["num_restarts"] + go.to(torch.int64))
+    return out, r, torch.where(go, 0, gen), flags

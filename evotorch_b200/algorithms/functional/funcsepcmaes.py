@@ -29,7 +29,7 @@ import torch
 
 from ... import ops
 from ..cmaes import CMAESHyperparameters, cmaes_hyperparameters
-from .funccmaes import _assigned_weights, _consts, _host_float
+from .funccmaes import _assigned_weights, _consts, _h_sig, _host_float
 from .fused import LazyPopulation, ask_and_evaluate
 from .misc import draw_philox_seed, on_kernels
 
@@ -139,6 +139,12 @@ def sepcmaes_ask_and_evaluate(state: SepCMAESState, *, objective: Callable, lazy
 def sepcmaes_tell(state: SepCMAESState, values: Union[torch.Tensor, LazyPopulation], evals: torch.Tensor) -> SepCMAESState:
     """The next state, given a population `values` (..., popsize, D) -- or the LazyPopulation that `sepcmaes_ask_and_evaluate`
     returned for this very state -- and its fitnesses `evals` (..., popsize).  The state passed in is left unchanged."""
+    return _tell(state, values, evals, state.generation)[0]
+
+
+def _tell(state: SepCMAESState, values: Union[torch.Tensor, LazyPopulation], evals: torch.Tensor, steps) -> tuple:
+    """(`sepcmaes_tell`'s next state, the generation counters after it).  `steps` drives h_sig and the decomposition schedule: the
+    int `state.generation`, or a (B,) int64 tensor of per-item counters."""
     batch, B, d = _items(state)
     n = state.popsize
     m0 = state.center
@@ -153,18 +159,24 @@ def sepcmaes_tell(state: SepCMAESState, values: Union[torch.Tensor, LazyPopulati
     if tuple(evals.shape) != batch + (n,):
         raise ValueError(f"`evals` was expected with shape {batch + (n,)}, got {tuple(evals.shape)}")
     f = evals.reshape(B, n)
+    per_item = isinstance(steps, torch.Tensor)
     if lazy or on_kernels(m0, values, f):
-        new = _tell_kernels(state, B, n, d, values, f)
+        counters = steps.clone() if per_item else steps  # the kernel increments per-item counters in place
+        new = _tell_kernels(state, B, n, d, values, f, counters)
+        steps_next = counters if per_item else steps + 1
     else:
-        new = _tell_torch(state, B, n, d, values.reshape(B, n, d), f)
+        new = _tell_torch(state, B, n, d, values.reshape(B, n, d), f, steps)
+        steps_next = steps + 1
     m, sigma, C, A, s, p_sigma, p_c = new
     vec = batch + (d,)
-    return state._replace(center=m.view(vec), sigma=sigma.view(batch), C=C.view(vec), A=A.view(vec), s=s.view(vec), p_sigma=p_sigma.view(vec),
-                          p_c=p_c.view(vec), generation=state.generation + 1)
+    new_state = state._replace(center=m.view(vec), sigma=sigma.view(batch), C=C.view(vec), A=A.view(vec), s=s.view(vec), p_sigma=p_sigma.view(vec),
+                               p_c=p_c.view(vec), generation=state.generation + 1)
+    return new_state, steps_next
 
 
-def _tell_kernels(state, B, n, d, values, f) -> tuple:
-    """Rank table, moments (row pass + column pass) and update, one launch each for all items; every output is a new tensor."""
+def _tell_kernels(state, B, n, d, values, f, steps) -> tuple:
+    """Rank table, moments (row pass + column pass) and update, one launch each for all items; every output is a new tensor.
+    `steps`: the shared int counter, or the per-item int64 counters, which the update increments."""
     hp = state.hyperparameters
     lazy = isinstance(values, LazyPopulation)
     m, s = state.center.reshape(B, d).contiguous(), state.s.reshape(B, d).contiguous()
@@ -174,13 +186,14 @@ def _tell_kernels(state, B, n, d, values, f) -> tuple:
     out = [t.reshape(B, d).clone() for t in (state.center, state.C, state.A, state.s, state.p_sigma, state.p_c)]
     m_new, C, A, s_new, p_sigma, p_c = out
     sigma = state.sigma.reshape(B).clone()
-    ops.sepcma_update_batched(local, S2, wsum, m_new, p_sigma, p_c, sigma, C, A, s_new, _consts(hp), state.csa_squared, steps=state.generation,
+    ops.sepcma_update_batched(local, S2, wsum, m_new, p_sigma, p_c, sigma, C, A, s_new, _consts(hp), state.csa_squared, steps=steps,
                               decompose_C_freq=hp.decompose_C_freq, stdev_min=state.stdev_min, stdev_max=state.stdev_max)
     return m_new, sigma, C, A, s_new, p_sigma, p_c
 
 
-def _tell_torch(state, B, n, d, x, f) -> tuple:
-    """The same generation as batched torch ops (CMAES's op-by-op generation with separable=True, cmaes.py:454-565)."""
+def _tell_torch(state, B, n, d, x, f, steps) -> tuple:
+    """The same generation as batched torch ops (CMAES's op-by-op generation with separable=True, cmaes.py:454-565), with the
+    generation counter `steps` (an int, or per-item counters)."""
     hp = state.hyperparameters
     m, sigma, C, A, s = state.center.reshape(B, d), state.sigma.reshape(B), state.C.reshape(B, d), state.A.reshape(B, d), state.s.reshape(B, d)
     z = (x - m[:, None, :]) / s[:, None, :]
@@ -200,14 +213,15 @@ def _tell_torch(state, B, n, d, x, f) -> tuple:
     else:
         expo = pnorm / hp.unbiased_expectation - 1
     sigma = sigma * torch.exp((hp.c_sigma / hp.damp_sigma) * expo)
-    squared_sum = pnorm.pow(2.0) / (1 - (1 - hp.c_sigma) ** (2 * state.generation + 1))
-    h_sig = ((squared_sum / d) - 1 < 1 + 4.0 / (d + 1)).to(m.dtype)
+    h_sig = _h_sig(hp, pnorm, d, steps)
     p_c = (1 - hp.c_c) * state.p_c.reshape(B, d) + (h_sig * hp.variance_discount_c)[:, None] * shaped
     c1a = hp.c_1 * (1 - (1 - h_sig**2) * hp.c_c * (2 - hp.c_c))
     C = C + c1a[:, None] * (p_c.pow(2.0) - C) + hp.c_mu * (A.pow(2.0) * S2 - wsum[:, None] * C)
     if state.stdev_min is not None or state.stdev_max is not None:  # CMAES._limit_stdev, with the new sigma
         stdevs = torch.clamp(sigma[:, None] * torch.sqrt(C), min=state.stdev_min, max=state.stdev_max)
         C = (stdevs / sigma[:, None]).pow(2.0)
-    if (state.generation + 1) % hp.decompose_C_freq == 0:
+    if isinstance(steps, torch.Tensor):
+        A = torch.where(((steps + 1) % hp.decompose_C_freq == 0)[:, None], C.pow(0.5), A)
+    elif (steps + 1) % hp.decompose_C_freq == 0:
         A = C.pow(0.5)
     return m, sigma, C, A, sigma[:, None] * A, p_sigma, p_c

@@ -95,7 +95,8 @@ __device__ __forceinline__ CmaVectorStep cma_vector_step(const float* __restrict
   return CmaVectorStep{new_sigma, h, steps};
 }
 
-// one CTA per item (grid x): the D-vectors of item b at b * D, its sigma at b, its k_out at 3 b (steps_dev / h_sig_out: single call only)
+// one CTA per item (grid x): the D-vectors of item b at b * D, its sigma at b, its k_out at 3 b, its step counter (nullable) at
+// steps_dev[b] (h_sig_out: single call only)
 __global__ void __launch_bounds__(kCmaThreads)
     cmaes_vector_update_kernel(const float* __restrict__ local_disp, const float* __restrict__ shaped_disp, int64_t D, float* __restrict__ m,
                                float* __restrict__ p_sigma, float* __restrict__ p_c, float* __restrict__ sigma, long long* steps_dev,
@@ -109,6 +110,7 @@ __global__ void __launch_bounds__(kCmaThreads)
   p_c += off;
   sigma += blockIdx.x;
   k_out += 3 * (int64_t)blockIdx.x;
+  if (steps_dev) steps_dev += blockIdx.x;
   const CmaVectorStep v = cma_vector_step<false>(local_disp, shaped_disp, nullptr, D, m, p_sigma, p_c, sigma, steps_dev, steps_host, c, sm, nullptr);
   const float new_sigma = v.new_sigma, h = v.h;
   const long long steps = v.steps;
@@ -131,7 +133,7 @@ __global__ void __launch_bounds__(kCmaThreads)
 //   stdev bounds with the new sigma: C <- (clamp(sigma' sqrt(C), lo, hi) / sigma')^2
 //   A <- sqrt(C) on the generations where (steps + 1) % decompose_freq == 0;   s <- sigma' A  (the sampler's per-column stdev)
 // s_prev (nullable) receives s before the update.  lo / hi: NaN = no bound.  Grid x = item: the D-vectors of item b at b * D, its sigma
-// and wsum at b (m_prev / s_prev / steps_dev / h_sig_out: single call only).
+// and wsum at b, its step counter (nullable) at steps_dev[b] (m_prev / s_prev / h_sig_out: single call only).
 __global__ void __launch_bounds__(kCmaThreads)
     sepcma_update_kernel(const float* __restrict__ local_disp, const float* __restrict__ S2, const float* __restrict__ wsum, int64_t D,
                          float* __restrict__ m, float* __restrict__ p_sigma, float* __restrict__ p_c, float* __restrict__ sigma, float* __restrict__ C,
@@ -150,6 +152,7 @@ __global__ void __launch_bounds__(kCmaThreads)
   s += off;
   sigma += blockIdx.x;
   wsum += blockIdx.x;
+  if (steps_dev) steps_dev += blockIdx.x;
   const CmaVectorStep v = cma_vector_step<true>(local_disp, nullptr, A, D, m, p_sigma, p_c, sigma, steps_dev, steps_host, c, sm, m_prev);
   const float sg = v.new_sigma, h = v.h;
   const float c1a = c.c_1 * (1.0f - (1.0f - h * h) * c.c_c * (2.0f - c.c_c));
@@ -226,20 +229,36 @@ extern "C" EVOK_API int evok_cmaes_vector_update(const float* local_disp, const 
   return 0;
 }
 
-extern "C" EVOK_API int evok_cmaes_vector_update_batched(const float* local_disp, const float* shaped_disp, int64_t n_items, int64_t D, float* m,
-                                                         float* p_sigma, float* p_c, float* sigma_dev, int64_t steps_host, const float* consts_host,
-                                                         int csa_squared, float* k_out, void* stream) {
+// the batched vector update with a shared step counter (steps_dev == NULL) or one per item (steps_dev[b])
+static int cmaes_vector_update_items(const float* local_disp, const float* shaped_disp, int64_t n_items, int64_t D, float* m, float* p_sigma,
+                                     float* p_c, float* sigma_dev, int64_t* steps_dev, int64_t steps_host, const float* consts_host, int csa_squared,
+                                     float* k_out, void* stream) {
   if (!local_disp || !shaped_disp || !m || !p_sigma || !p_c || !sigma_dev || !consts_host || !k_out) return EVOK_E_NULLPTR;
   if (n_items < 0 || D <= 0) return EVOK_E_BADSIZE;
   const CmaesConsts c = cmaes_consts(consts_host, csa_squared);
   return for_item_chunks(n_items, (int64_t)INT32_MAX, [&](int64_t b0, int64_t nb) {
     const int64_t off = b0 * D;
-    cmaes_vector_update_kernel<<<(unsigned)nb, kCmaThreads, 0, (cudaStream_t)stream>>>(local_disp + off, shaped_disp + off, D, m + off, p_sigma + off,
-                                                                                      p_c + off, sigma_dev + b0, nullptr, (long long)steps_host, c,
-                                                                                      k_out + 3 * b0, nullptr);
+    cmaes_vector_update_kernel<<<(unsigned)nb, kCmaThreads, 0, (cudaStream_t)stream>>>(
+        local_disp + off, shaped_disp + off, D, m + off, p_sigma + off, p_c + off, sigma_dev + b0,
+        steps_dev ? reinterpret_cast<long long*>(steps_dev + b0) : nullptr, (long long)steps_host, c, k_out + 3 * b0, nullptr);
     EVOK_CHECK_LAUNCH();
     return 0;
   });
+}
+
+extern "C" EVOK_API int evok_cmaes_vector_update_batched(const float* local_disp, const float* shaped_disp, int64_t n_items, int64_t D, float* m,
+                                                         float* p_sigma, float* p_c, float* sigma_dev, int64_t steps_host, const float* consts_host,
+                                                         int csa_squared, float* k_out, void* stream) {
+  return cmaes_vector_update_items(local_disp, shaped_disp, n_items, D, m, p_sigma, p_c, sigma_dev, nullptr, steps_host, consts_host, csa_squared,
+                                   k_out, stream);
+}
+
+extern "C" EVOK_API int evok_cmaes_vector_update_batched_steps(const float* local_disp, const float* shaped_disp, int64_t n_items, int64_t D,
+                                                               float* m, float* p_sigma, float* p_c, float* sigma_dev, int64_t* steps_dev,
+                                                               const float* consts_host, int csa_squared, float* k_out, void* stream) {
+  if (!steps_dev) return EVOK_E_NULLPTR;
+  return cmaes_vector_update_items(local_disp, shaped_disp, n_items, D, m, p_sigma, p_c, sigma_dev, steps_dev, 0, consts_host, csa_squared, k_out,
+                                   stream);
 }
 
 extern "C" EVOK_API int evok_sepcma_update(const float* local_disp, const float* S2, const float* wsum, int64_t D, float* m, float* p_sigma, float* p_c,
@@ -256,20 +275,37 @@ extern "C" EVOK_API int evok_sepcma_update(const float* local_disp, const float*
   return 0;
 }
 
-extern "C" EVOK_API int evok_sepcma_update_batched(const float* local_disp, const float* S2, const float* wsum, int64_t n_items, int64_t D, float* m,
-                                                   float* p_sigma, float* p_c, float* sigma_dev, float* C, float* A, float* s, int64_t steps_host,
-                                                   const float* consts_host, int csa_squared, int64_t decompose_C_freq, float stdev_min, float stdev_max,
-                                                   void* stream) {
+// the batched separable update with a shared step counter (steps_dev == NULL) or one per item (steps_dev[b])
+static int sepcma_update_items(const float* local_disp, const float* S2, const float* wsum, int64_t n_items, int64_t D, float* m, float* p_sigma,
+                               float* p_c, float* sigma_dev, float* C, float* A, float* s, int64_t* steps_dev, int64_t steps_host,
+                               const float* consts_host, int csa_squared, int64_t decompose_C_freq, float stdev_min, float stdev_max, void* stream) {
   if (!local_disp || !S2 || !wsum || !m || !p_sigma || !p_c || !sigma_dev || !C || !A || !s || !consts_host) return EVOK_E_NULLPTR;
   if (n_items < 0 || D <= 0 || decompose_C_freq < 1) return EVOK_E_BADSIZE;
   const CmaesConsts c = cmaes_consts(consts_host, csa_squared);
   return for_item_chunks(n_items, (int64_t)INT32_MAX, [&](int64_t b0, int64_t nb) {
     const int64_t off = b0 * D;
-    sepcma_update_kernel<<<(unsigned)nb, kCmaThreads, 0, (cudaStream_t)stream>>>(local_disp + off, S2 + off, wsum + b0, D, m + off, p_sigma + off,
-                                                                                p_c + off, sigma_dev + b0, C + off, A + off, s + off, nullptr, nullptr,
-                                                                                nullptr, (long long)steps_host, c, (long long)decompose_C_freq,
-                                                                                stdev_min, stdev_max, nullptr);
+    sepcma_update_kernel<<<(unsigned)nb, kCmaThreads, 0, (cudaStream_t)stream>>>(
+        local_disp + off, S2 + off, wsum + b0, D, m + off, p_sigma + off, p_c + off, sigma_dev + b0, C + off, A + off, s + off, nullptr, nullptr,
+        steps_dev ? reinterpret_cast<long long*>(steps_dev + b0) : nullptr, (long long)steps_host, c, (long long)decompose_C_freq, stdev_min,
+        stdev_max, nullptr);
     EVOK_CHECK_LAUNCH();
     return 0;
   });
+}
+
+extern "C" EVOK_API int evok_sepcma_update_batched(const float* local_disp, const float* S2, const float* wsum, int64_t n_items, int64_t D, float* m,
+                                                   float* p_sigma, float* p_c, float* sigma_dev, float* C, float* A, float* s, int64_t steps_host,
+                                                   const float* consts_host, int csa_squared, int64_t decompose_C_freq, float stdev_min, float stdev_max,
+                                                   void* stream) {
+  return sepcma_update_items(local_disp, S2, wsum, n_items, D, m, p_sigma, p_c, sigma_dev, C, A, s, nullptr, steps_host, consts_host, csa_squared,
+                             decompose_C_freq, stdev_min, stdev_max, stream);
+}
+
+extern "C" EVOK_API int evok_sepcma_update_batched_steps(const float* local_disp, const float* S2, const float* wsum, int64_t n_items, int64_t D,
+                                                         float* m, float* p_sigma, float* p_c, float* sigma_dev, float* C, float* A, float* s,
+                                                         int64_t* steps_dev, const float* consts_host, int csa_squared, int64_t decompose_C_freq,
+                                                         float stdev_min, float stdev_max, void* stream) {
+  if (!steps_dev) return EVOK_E_NULLPTR;
+  return sepcma_update_items(local_disp, S2, wsum, n_items, D, m, p_sigma, p_c, sigma_dev, C, A, s, steps_dev, 0, consts_host, csa_squared,
+                             decompose_C_freq, stdev_min, stdev_max, stream);
 }

@@ -1053,11 +1053,22 @@ def sepcma_moments_batched(X: Optional[torch.Tensor], m: torch.Tensor, s: torch.
     return local, S2, wsum
 
 
+def _item_steps(steps, B: int) -> Optional[torch.Tensor]:
+    """None for a shared host counter (an int), else `steps` checked as one int64 CUDA counter per item, (items,) contiguous."""
+    if not isinstance(steps, torch.Tensor):
+        return None
+    if not (steps.is_cuda and steps.dtype == torch.int64 and steps.is_contiguous() and tuple(steps.shape) == (B,)):
+        raise ValueError(f"steps: expected an int or a contiguous int64 CUDA tensor of shape ({B},), got {tuple(steps.shape)} {steps.dtype}")
+    return steps
+
+
 def sepcma_update_batched(local: torch.Tensor, S2: torch.Tensor, wsum: torch.Tensor, m: torch.Tensor, p_sigma: torch.Tensor, p_c: torch.Tensor,
-                          sigma: torch.Tensor, C: torch.Tensor, A: torch.Tensor, s: torch.Tensor, consts, csa_squared: bool, *, steps: int,
+                          sigma: torch.Tensor, C: torch.Tensor, A: torch.Tensor, s: torch.Tensor, consts, csa_squared: bool, *, steps,
                           decompose_C_freq: int, stdev_min: Optional[float] = None, stdev_max: Optional[float] = None) -> None:
     """`sepcma_update` for every item, one CTA each, in place: m, p_sigma, p_c, C, A, s, local, S2 (items, D), sigma, wsum (items,).
-    The 10 constants, the generation counter `steps`, `decompose_C_freq` and the stdev bounds are shared."""
+    The 10 constants, `decompose_C_freq` and the stdev bounds are shared.  `steps`: the generation counter, an int shared by every
+    item, or an int64 CUDA tensor (items,) of per-item counters that drive each item's h_sig and decomposition schedule and are
+    incremented in place."""
     B, d = m.shape
     for t, name in ((local, "local"), (S2, "S2"), (m, "m"), (p_sigma, "p_sigma"), (p_c, "p_c"), (C, "C"), (A, "A"), (s, "s")):
         _rows(t, name, (B, d))
@@ -1065,24 +1076,87 @@ def sepcma_update_batched(local: torch.Tensor, S2: torch.Tensor, wsum: torch.Ten
         _rows(t, name, (B,))
     if int(decompose_C_freq) < 1:
         raise ValueError("decompose_C_freq: expected a positive integer")
+    steps_dev = _item_steps(steps, B)
     lo = NAN if stdev_min is None else float(stdev_min)
     hi = NAN if stdev_max is None else float(stdev_max)
+    lib = nat.lib()
+    head = (local.data_ptr(), S2.data_ptr(), wsum.data_ptr(), B, d, m.data_ptr(), p_sigma.data_ptr(), p_c.data_ptr(), sigma.data_ptr(), C.data_ptr(),
+            A.data_ptr(), s.data_ptr())
+    tail = (_host_floats(consts, 10), int(bool(csa_squared)), int(decompose_C_freq), lo, hi, nat.stream_of(m))
     with _timed("sepcma_update"):
-        rc = nat.lib().evok_sepcma_update_batched(local.data_ptr(), S2.data_ptr(), wsum.data_ptr(), B, d, m.data_ptr(), p_sigma.data_ptr(),
-                                                  p_c.data_ptr(), sigma.data_ptr(), C.data_ptr(), A.data_ptr(), s.data_ptr(), int(steps),
-                                                  _host_floats(consts, 10), int(bool(csa_squared)), int(decompose_C_freq), lo, hi, nat.stream_of(m))
-    nat.check(rc, "evok_sepcma_update_batched")
+        if steps_dev is None:
+            rc, entry = lib.evok_sepcma_update_batched(*head, int(steps), *tail), "evok_sepcma_update_batched"
+        else:
+            rc, entry = lib.evok_sepcma_update_batched_steps(*head, steps_dev.data_ptr(), *tail), "evok_sepcma_update_batched_steps"
+    nat.check(rc, entry)
 
 
 def cmaes_vector_update_batched(local_disp: torch.Tensor, shaped_disp: torch.Tensor, m: torch.Tensor, p_sigma: torch.Tensor, p_c: torch.Tensor,
-                                sigma: torch.Tensor, consts, csa_squared: bool, k_out: torch.Tensor, *, steps: int) -> None:
+                                sigma: torch.Tensor, consts, csa_squared: bool, k_out: torch.Tensor, *, steps) -> None:
     """`cmaes_vector_update` for every item, one CTA each, in place: m, p_sigma, p_c, local / shaped (items, D), sigma (items,),
-    k_out (items, 3).  The 10 constants and the generation counter `steps` are shared."""
+    k_out (items, 3).  The 10 constants are shared.  `steps`: the generation counter, an int shared by every item, or an int64
+    CUDA tensor (items,) of per-item counters that drive each item's h_sig and are incremented in place."""
     B, d = m.shape
     for t, name in ((local_disp, "local_disp"), (shaped_disp, "shaped_disp"), (m, "m"), (p_sigma, "p_sigma"), (p_c, "p_c")):
         _rows(t, name, (B, d))
     _rows(sigma.view(B, 1) if sigma.numel() == B and sigma.is_contiguous() else sigma, "sigma", (B, 1))
     _rows(k_out, "k_out", (B, 3))
-    nat.check(nat.lib().evok_cmaes_vector_update_batched(local_disp.data_ptr(), shaped_disp.data_ptr(), B, d, m.data_ptr(), p_sigma.data_ptr(),
-                                                         p_c.data_ptr(), sigma.data_ptr(), int(steps), _host_floats(consts, 10), int(bool(csa_squared)),
-                                                         k_out.data_ptr(), nat.stream_of(m)), "evok_cmaes_vector_update_batched")
+    steps_dev = _item_steps(steps, B)
+    lib = nat.lib()
+    head = (local_disp.data_ptr(), shaped_disp.data_ptr(), B, d, m.data_ptr(), p_sigma.data_ptr(), p_c.data_ptr(), sigma.data_ptr())
+    tail = (_host_floats(consts, 10), int(bool(csa_squared)), k_out.data_ptr(), nat.stream_of(m))
+    if steps_dev is None:
+        nat.check(lib.evok_cmaes_vector_update_batched(*head, int(steps), *tail), "evok_cmaes_vector_update_batched")
+    else:
+        nat.check(lib.evok_cmaes_vector_update_batched_steps(*head, steps_dev.data_ptr(), *tail), "evok_cmaes_vector_update_batched_steps")
+
+
+RESTART_CRITERIA = ("tol_fun", "tol_x", "tol_x_up", "max_condition", "min_fitness_stdev", "max_generations")  # bits 0-5; bit 6: non-finite
+
+
+def cma_restart_batched(separable: bool, f: torch.Tensor, X: Optional[torch.Tensor], maximize: bool, item_steps: torch.Tensor, m: torch.Tensor,
+                        sigma: torch.Tensor, p_sigma: torch.Tensor, p_c: torch.Tensor, C: torch.Tensor, A: torch.Tensor, s: Optional[torch.Tensor],
+                        history: torch.Tensor, best_x: torch.Tensor, best_f: torch.Tensor, num_restarts: torch.Tensor, stop_flags: torch.Tensor,
+                        sigma0: torch.Tensor, lb: torch.Tensor, ub: torch.Tensor, thresholds, *, seed: int, m_draw: Optional[torch.Tensor] = None,
+                        s_draw: Optional[torch.Tensor] = None, draw_seed: int = 0) -> None:
+    """The restart stage of every item after its update, in place (include/evok.h, evok_cma_restart_batched): best ever, history,
+    stop flags and the re-initialisation of the items that met a criterion.  f (items, N); X (items, N, D), or None for a separable
+    population rebuilt from (draw_seed, stream b) with m_draw / s_draw (items, D); item_steps, num_restarts int64 (items,); m, p_sigma,
+    p_c, best_x, lb, ub (items, D); C, A (items, D, D), separable (items, D) with s; sigma, sigma0, best_f (items,); history
+    (items, H); stop_flags int32 (items,); `thresholds` the 6 criteria of RESTART_CRITERIA, None = off; `seed` the Philox key of
+    the new centres."""
+    B, n = f.shape
+    d = m.shape[-1]
+    f = _rows(f, "f", (B, n))
+    for t, name in ((m, "m"), (p_sigma, "p_sigma"), (p_c, "p_c"), (best_x, "best_x"), (lb, "lb"), (ub, "ub")):
+        _rows(t, name, (B, d))
+    for t, name in ((sigma, "sigma"), (sigma0, "sigma0"), (best_f, "best_f")):
+        _rows(t, name, (B,))
+    for t, name in ((C, "C"), (A, "A")):
+        # the stage reads the diagonals and writes I: a matrix may be row- or column-major (torch's batched Cholesky is the latter)
+        if not (t.is_cuda and t.dtype == torch.float32 and (t.is_contiguous() or (not separable and t.mT.is_contiguous()))
+                and tuple(t.shape) == ((B, d) if separable else (B, d, d))):
+            raise ValueError(f"{name}: expected a float32 CUDA tensor of shape {(B, d) if separable else (B, d, d)}, contiguous (or its "
+                             "transposes contiguous)")
+    if separable:
+        _rows(s, "s", (B, d))
+    if not (history.is_cuda and history.dtype == torch.float32 and history.is_contiguous() and history.ndim == 2 and history.shape[0] == B):
+        raise ValueError(f"history: expected a contiguous float32 CUDA tensor of shape ({B}, H)")
+    for t, name, dt in ((item_steps, "item_steps", torch.int64), (num_restarts, "num_restarts", torch.int64), (stop_flags, "stop_flags", torch.int32)):
+        if not (t.is_cuda and t.dtype == dt and t.is_contiguous() and tuple(t.shape) == (B,)):
+            raise ValueError(f"{name}: expected a contiguous {dt} CUDA tensor of shape ({B},)")
+    if X is not None:
+        if not (X.is_cuda and X.dtype == torch.float32 and X.is_contiguous() and tuple(X.shape) == (B, n, d)):
+            raise ValueError(f"X: expected a contiguous float32 CUDA tensor of shape {(B, n, d)}")
+    elif not separable or m_draw is None or s_draw is None:
+        raise ValueError("X: the population is needed, except for a separable one rebuilt from m_draw and s_draw")
+    else:
+        m_draw, s_draw = _rows(m_draw, "m_draw", (B, d)), _rows(s_draw, "s_draw", (B, d))
+    th = [NAN if t is None else float(t) for t in thresholds]
+    with _timed("cma_restart"):
+        rc = nat.lib().evok_cma_restart_batched(int(bool(separable)), f.data_ptr(), nat.ptr(X), n * d, d, nat.ptr(m_draw), nat.ptr(s_draw), int(draw_seed),
+                                                B, n, d, int(bool(maximize)), item_steps.data_ptr(), m.data_ptr(), sigma.data_ptr(), p_sigma.data_ptr(),
+                                                p_c.data_ptr(), C.data_ptr(), A.data_ptr(), nat.ptr(s), history.data_ptr(), history.shape[1],
+                                                best_x.data_ptr(), best_f.data_ptr(), num_restarts.data_ptr(), stop_flags.data_ptr(), sigma0.data_ptr(),
+                                                lb.data_ptr(), ub.data_ptr(), d, _host_floats(th, 6), int(seed), nat.stream_of(f))
+    nat.check(rc, "evok_cma_restart_batched")

@@ -495,7 +495,10 @@ int evok_cmaes_vector_update(const float* local_disp, const float* shaped_disp, 
  *   evok_rank_table_batched        : keys, out [items][N], one shared table; the workspace of evok_rank_table.
  *   evok_cmaes_row_weights_batched : Z_b at Z + b * item_stride_z (pitch ldz); assigned_weights, w_positive, w_active [items][N].
  *   evok_cmaes_vector_update_batched: one CTA per item; local_disp, shaped_disp, m, p_sigma, p_c [items][D], sigma_dev [items],
- *       k_out [items][3]; the constants and the generation counter steps_host are shared. */
+ *       k_out [items][3]; the constants and the generation counter steps_host are shared.
+ *   evok_cmaes_vector_update_batched_steps: the same with one generation counter per item: item b's _h_sig reads steps_dev[b]
+ *       (int64, device) and the kernel increments it, as the single call does with its steps_dev.  Errors: those of
+ *       evok_cmaes_vector_update_batched, and EVOK_E_NULLPTR for steps_dev. */
 int evok_rank_table_batched(const float* keys, int64_t N, int64_t n_items, int descending, const float* table, float* out, void* ws, size_t ws_bytes,
                             void* stream);
 int evok_cmaes_row_weights_batched(const float* assigned_weights, const float* Z, int64_t item_stride_z, int64_t ldz, int64_t n_items, int64_t N,
@@ -503,6 +506,9 @@ int evok_cmaes_row_weights_batched(const float* assigned_weights, const float* Z
 int evok_cmaes_vector_update_batched(const float* local_disp, const float* shaped_disp, int64_t n_items, int64_t D, float* m, float* p_sigma,
                                      float* p_c, float* sigma_dev, int64_t steps_host, const float* consts_host, int csa_squared, float* k_out,
                                      void* stream);
+int evok_cmaes_vector_update_batched_steps(const float* local_disp, const float* shaped_disp, int64_t n_items, int64_t D, float* m,
+                                           float* p_sigma, float* p_c, float* sigma_dev, int64_t* steps_dev, const float* consts_host,
+                                           int csa_squared, float* k_out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Separable CMA-ES (diagonal C, algorithms/cmaes.py with separable=True) as three kernels plus evok_rank_table, with no host
@@ -543,7 +549,10 @@ int evok_sepcma_update(const float* local, const float* S2, const float* wsum, i
  *       EVOK_E_NULLPTR, EVOK_E_BADSIZE (n_items < 0, n_rows <= 0, D <= 0, with X: ldx < D or a negative item stride),
  *       EVOK_E_WORKSPACE (none with n_items == 0).
  *   evok_sepcma_update_batched: evok_sepcma_update with one CTA per item, per item the bits of the single call; local, S2, m, p_sigma,
- *       p_c, C, A, s [items][D], wsum, sigma_dev [items].  The constants, the generation counter and the stdev bounds are shared. */
+ *       p_c, C, A, s [items][D], wsum, sigma_dev [items].  The constants, the generation counter and the stdev bounds are shared.
+ *   evok_sepcma_update_batched_steps: the same with one generation counter per item, steps_dev[b] (int64, device, incremented by
+ *       the kernel): item b's _h_sig and its decomposition schedule, (steps_dev[b] + 1) % decompose_C_freq == 0, follow its own
+ *       counter.  Errors: those of evok_sepcma_update_batched, and EVOK_E_NULLPTR for steps_dev. */
 size_t evok_sepcma_moments_batched_workspace_bytes(int64_t n_items, int64_t n_rows, int64_t D);
 int evok_sepcma_moments_batched(const float* X, int64_t item_stride_x, int64_t ldx, const float* m, const float* s, const float* aw, int active,
                                 int64_t n_items, int64_t n_rows, int64_t D, uint64_t seed, uint64_t stream_id0, float* local, float* S2, float* wsum,
@@ -551,6 +560,44 @@ int evok_sepcma_moments_batched(const float* X, int64_t item_stride_x, int64_t l
 int evok_sepcma_update_batched(const float* local, const float* S2, const float* wsum, int64_t n_items, int64_t D, float* m, float* p_sigma, float* p_c,
                                float* sigma_dev, float* C, float* A, float* s, int64_t steps_host, const float* consts_host, int csa_squared,
                                int64_t decompose_C_freq, float stdev_min, float stdev_max, void* stream);
+int evok_sepcma_update_batched_steps(const float* local, const float* S2, const float* wsum, int64_t n_items, int64_t D, float* m, float* p_sigma,
+                                     float* p_c, float* sigma_dev, float* C, float* A, float* s, int64_t* steps_dev, const float* consts_host,
+                                     int csa_squared, int64_t decompose_C_freq, float stdev_min, float stdev_max, void* stream);
+
+/* Restarts of the functional CMA-ES families: the stage after a batched update (evok_cmaes_vector_update_batched_steps + the
+ * covariance update + Cholesky, or evok_sepcma_update_batched_steps), one CTA per item, no host reads.
+ *   evok_cma_restart_batched: per item b, with N = n_rows and g = item_steps[b] (the generations since the item's (re)start, the
+ *       update already counted),
+ *       - best ever: the best finite f of this generation (under `maximize`; the lower row on ties), if strictly better than
+ *         best_f[b], goes to best_f[b] and its row to best_x[b] (D floats): row i of X, or with X == NULL (separable only) the
+ *         row the batched sampler stored for (draw_seed, stream b, row i), x = fmaf(s_draw, z, m_draw), the same bits;
+ *       - history [items][H]: slot (g - 1) % H <- that best value (NaN when no f was finite);
+ *       - stop_flags[b] (int32) <- the criteria that fire, thresholds_host[0..5] (6 host floats, NaN = off):
+ *           bit 0 tol_fun    g >= H and max - min over the H history slots and the N values of f < thresholds[0] (all finite)
+ *           bit 1 tol_x      sigma max_j max(|p_c,j|, sqrt(C_jj)) < thresholds[1] sigma0[b]
+ *           bit 2 tol_x_up   sigma max_j sqrt(C_jj) > thresholds[2] sigma0[b]
+ *           bit 3 max_cond   full: (max_j A_jj / min_j A_jj)^2 > thresholds[3]; every Cholesky pivot A_jj^2 lies in
+ *                            [lambda_min(C), lambda_max(C)], so this is a lower bound of cond(C) and never fires early;
+ *                            separable: max_j C_j / min_j C_j > thresholds[3]
+ *           bit 4 min_fitness_stdev  the unbiased standard deviation of the N values (N > 1, finite) < thresholds[4]
+ *           bit 5 max_generations    g >= thresholds[5]
+ *           bit 6 non-finite (always on)  sigma <= 0, or sigma, an entry of m, p_sigma, p_c or diag C is not finite
+ *       - an item with a flag restarts: m_j = lb_j + (ub_j - lb_j) u_j (float32, unfused) with u_j = uniform24 of word j & 3 of
+ *         Philox4x32-10(counter (j >> 2, 0, 0xFF000000, stream word b), key (seed, stream 0)) -- no sample counter (third word
+ *         below 2^31) or noise counter (0x80.. to 0x87..) has this third word; sigma <- sigma0[b], p_sigma = p_c = 0,
+ *         item_steps[b] = 0, history row NaN, num_restarts[b] (int64) += 1; C = A = I (full: a second, grid-wide launch masked by
+ *         the flags), separable: C = A = 1 and s = sigma0[b].
+ *       separable != 0: C, A, s [items][D]; else C, A [items][D][D] (s unused, nullable).  m, p_sigma, p_c, best_x, m_draw,
+ *       s_draw [items][D]; f [items][N]; X at item_stride_x / ldx; sigma, sigma0, best_f [items]; lb, ub at item_stride_bounds
+ *       (0: shared, or D).  One launch (separable) or two (full).  Errors in this order: EVOK_E_NULLPTR (any state pointer,
+ *       thresholds_host, X for the full family, s for the separable one, m_draw / s_draw without X), EVOK_E_BADSIZE (n_items < 0,
+ *       n_rows <= 0, D <= 0, H <= 0, with X: ldx < D or a negative item stride, item_stride_bounds not 0 or D).  Nothing is
+ *       launched for n_items == 0. */
+int evok_cma_restart_batched(int separable, const float* f, const float* X, int64_t item_stride_x, int64_t ldx, const float* m_draw,
+                             const float* s_draw, uint64_t draw_seed, int64_t n_items, int64_t n_rows, int64_t D, int maximize, int64_t* item_steps,
+                             float* m, float* sigma, float* p_sigma, float* p_c, float* C, float* A, float* s, float* history, int64_t H,
+                             float* best_x, float* best_f, int64_t* num_restarts, int32_t* stop_flags, const float* sigma0, const float* lb,
+                             const float* ub, int64_t item_stride_bounds, const float* thresholds_host, uint64_t seed, void* stream);
 
 /* Cholesky factorisation A = L L^T (fp32, lower; the strictly upper part of L is zeroed, like torch.linalg.cholesky).  Replaces
  * CMAES.decompose_C (cmaes.py:555-565, torch.linalg.cholesky -> cuSOLVER potrf).  ONE persistent kernel: 64 x 64 tiles, left-looking
