@@ -111,6 +111,14 @@ _SIGNATURES = {
                                                  _P]),
     "evok_cma_restart_batched": (c_int, [c_int, _P, _P, c_int64, c_int64, _P, _P, c_uint64, c_int64, c_int64, c_int64, c_int, _P, _P, _P, _P, _P, _P,
                                          _P, _P, _P, c_int64, _P, _P, _P, _P, _P, _P, _P, c_int64, _P, c_uint64, _P]),
+    "evok_rank_table_batched_tiered": (c_int, [_P, c_int64, c_int64, c_int, _P, _P, _P, _P, _P]),
+    "evok_cmaes_row_weights_batched_tiered": (c_int, [_P, _P, c_int64, c_int64, c_int64, c_int64, c_int64, c_int, _P, _P, _P, _P, _P]),
+    "evok_cmaes_vector_update_batched_tiered": (c_int, [_P, _P, c_int64, c_int64, _P, _P, _P, _P, _P, _P, _P, c_int, _P, _P]),
+    "evok_sepcma_update_batched_tiered": (c_int, [_P, _P, _P, c_int64, c_int64, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_float, c_float,
+                                                  _P]),
+    "evok_cma_restart_batched_tiered": (c_int, [c_int, _P, _P, c_int64, c_int64, _P, _P, c_uint64, c_int64, c_int64, c_int64, c_int, _P, _P, _P, _P,
+                                                _P, _P, _P, _P, _P, c_int64, _P, _P, _P, _P, _P, _P, _P, c_int64, _P, c_uint64, _P, _P, _P, c_int64,
+                                                _P, _P]),
     "evok_peer_alloc": (c_int, [c_size_t, _P, _P]),
     "evok_peer_open": (c_int, [_P, _P]),
     "evok_peer_close": (c_int, [_P]),

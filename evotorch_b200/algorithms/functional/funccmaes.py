@@ -22,6 +22,7 @@ steps z are recovered from the values, not remembered from the ask.
 from __future__ import annotations
 
 import math
+from types import SimpleNamespace
 from typing import Callable, NamedTuple, Optional
 
 import torch
@@ -172,10 +173,12 @@ def cmaes_tell(state: CMAESState, values: torch.Tensor, evals: torch.Tensor) -> 
     return _tell(state, values, evals, state.generation)[0]
 
 
-def _tell(state: CMAESState, values: torch.Tensor, evals: torch.Tensor, steps) -> tuple:
+def _tell(state: CMAESState, values: torch.Tensor, evals: torch.Tensor, steps, tiers=None) -> tuple:
     """(`cmaes_tell`'s next state, the generation counters after it).  `steps` drives h_sig and the decomposition schedule: the
     int `state.generation`, or a (B,) int64 tensor of per-item counters (then every item is factored and keeps its old A unless
-    (steps + 1) % decompose_C_freq == 0 for it)."""
+    (steps + 1) % decompose_C_freq == 0 for it).  `tiers` (with per-item counters): None, or (ladder, tier) of a padded
+    population (funcrestarts.IPOPLadder, int32 (B,)): item b is told its first ladder.popsizes[tier[b]] rows with the constants of
+    its tier, and its pad rows reach nothing."""
     if isinstance(values, LazyPopulation):
         raise ValueError("The functional CMA-ES recovers its steps from the values: a lazy population cannot be told; ask for the values")
     batch, B, d = _items(state)
@@ -190,22 +193,25 @@ def _tell(state: CMAESState, values: torch.Tensor, evals: torch.Tensor, steps) -
     hp = state.hyperparameters
     m, sigma, C, A = m0.reshape(B, d), state.sigma.reshape(B), state.C.reshape(B, d, d), state.A.reshape(B, d, d)
     x, f = values.reshape(B, n, d), evals.reshape(B, n)
+    if tiers is not None:  # pad rows at the centre: their y and z are exactly 0, whatever they held
+        x = torch.where(_real_rows(tiers, n)[:, :, None], x, m[:, None, :])
     y = (x - m[:, None, :]) / sigma[:, None, None]
     z = torch.linalg.solve_triangular(A.mT, y, upper=True, left=False).contiguous()  # z A^T = y
     per_item = isinstance(steps, torch.Tensor)
     if on_kernels(m, x, f):
         counters = steps.clone() if per_item else steps  # the kernel increments per-item counters in place
-        m, p_sigma, p_c, sigma, C_new = _tell_kernels(state, hp, B, n, d, m, sigma, C, y, z, f, counters)
+        m, p_sigma, p_c, sigma, C_new = _tell_kernels(state, hp, B, n, d, m, sigma, C, y, z, f, counters, tiers)
         steps_next = counters if per_item else steps + 1
     else:
-        m, p_sigma, p_c, sigma, C_new = _tell_torch(state, hp, B, n, d, m, sigma, C, y, z, f, steps)
+        m, p_sigma, p_c, sigma, C_new = _tell_torch(state, hp, B, n, d, m, sigma, C, y, z, f, steps, tiers)
         steps_next = steps + 1
     _limit_stdev(C_new, sigma, state.stdev_min, state.stdev_max)
     A_new = A
     if per_item:
         A_new, _ = torch.linalg.cholesky_ex(C_new, check_errors=False)
-        if hp.decompose_C_freq > 1:
-            A_new = torch.where((steps_next % hp.decompose_C_freq == 0)[:, None, None], A_new, A)
+        freq = hp.decompose_C_freq if tiers is None else tiers[0].decompose_C_freq[tiers[1].long()]
+        if tiers is not None or hp.decompose_C_freq > 1:
+            A_new = torch.where((steps_next % freq == 0)[:, None, None], A_new, A)
     elif (state.generation + 1) % hp.decompose_C_freq == 0:
         A_new, _ = torch.linalg.cholesky_ex(C_new, check_errors=False)
     new = state._replace(center=m.view(batch + (d,)), sigma=sigma.view(batch), C=C_new.view(batch + (d, d)), A=A_new.view(batch + (d, d)),
@@ -213,19 +219,46 @@ def _tell(state: CMAESState, values: torch.Tensor, evals: torch.Tensor, steps) -
     return new, steps_next
 
 
+CONST_NAMES = ("c_m", "c_sigma", "damp_sigma", "c_c", "c_1", "c_mu", "variance_discount_sigma", "variance_discount_c", "unbiased_expectation",
+               "weights_sum")  # the order of the 10 constants the update kernels take
+
+
 def _consts(hp: CMAESHyperparameters) -> tuple:
     return (hp.c_m, hp.c_sigma, hp.damp_sigma, hp.c_c, hp.c_1, hp.c_mu, hp.variance_discount_sigma, hp.variance_discount_c,
             float(hp.unbiased_expectation), hp.weights_sum)
 
 
-def _tell_kernels(state, hp, B, n, d, m, sigma, C, y, z, f, steps) -> tuple:
+def _real_rows(tiers, n: int) -> torch.Tensor:
+    """(B, n) bool: the rows each item of a padded population uses, its first ladder.popsizes[tier] of the n drawn."""
+    ladder, tier = tiers
+    return torch.arange(n, device=tier.device) < ladder.counts.long()[tier.long()][:, None]
+
+
+def _tier_items(tiers, n: int) -> tuple:
+    """(per-item constants: the names of CONST_NAMES and decompose_C_freq as (B,) tensors, per-item weight rows (B, n), the real
+    rows (B, n)) of the items of a padded population at their tiers."""
+    ladder, tier = tiers
+    t = tier.long()
+    c = ladder.consts[t]
+    hp = SimpleNamespace(decompose_C_freq=ladder.decompose_C_freq[t], **{name: c[:, k] for k, name in enumerate(CONST_NAMES)})
+    return hp, ladder.weights[t], _real_rows(tiers, n)
+
+
+def _col(v, dims: int = 1):
+    """A per-item constant, a (B,) tensor, with `dims` trailing dimensions to meet (B, D) or (B, D, D) operands; a float as is."""
+    return v[(slice(None),) + (None,) * dims] if isinstance(v, torch.Tensor) else v
+
+
+def _tell_kernels(state, hp, B, n, d, m, sigma, C, y, z, f, steps, tiers=None) -> tuple:
     """The stages of CMAES._step_fused for all items at once, one launch each; every output is a new tensor.  `steps`: the shared
-    int counter, or the per-item int64 counters, which the vector update increments."""
+    int counter, or the per-item int64 counters, which the vector update increments.  `tiers`: as in `_tell`."""
     dev = m.device
     new = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=dev)  # noqa: E731
     aw, w_pos, w_act = new(B, n), new(B, n), new(B, n)
-    ops.rank_table_batched(f, state.maximize, hp.weights, out=aw)
-    ops.cmaes_row_weights_batched(aw, z, state.active, w_pos, w_act)
+    ladder, tier = tiers if tiers is not None else (None, None)
+    tiered = {} if tiers is None else dict(tier=tier, counts=ladder.counts)
+    ops.rank_table_batched(f, state.maximize, hp.weights if tiers is None else ladder.weights, out=aw, **tiered)
+    ops.cmaes_row_weights_batched(aw, z, state.active, w_pos, w_act, **tiered)
     zero = torch.zeros(d, dtype=torch.float32, device=dev)
     one = zero + 1.0
     local, _ = ops.grad_batched(ops.GRAD_MOMENTS, z, w_pos, zero, one, 1.0, 1.0)
@@ -233,22 +266,31 @@ def _tell_kernels(state, hp, B, n, d, m, sigma, C, y, z, f, steps) -> tuple:
     m, sigma = m.clone(), sigma.clone()
     p_sigma, p_c = state.p_sigma.reshape(B, d).clone(), state.p_c.reshape(B, d).clone()
     k = new(B, 3)
-    ops.cmaes_vector_update_batched(local, shaped, m, p_sigma, p_c, sigma, _consts(hp), state.csa_squared, k, steps=steps)
+    ops.cmaes_vector_update_batched(local, shaped, m, p_sigma, p_c, sigma, _consts(hp) if tiers is None else ladder.consts, state.csa_squared, k,
+                                    steps=steps, tier=tier)
     C_new = ops.weighted_syrk_update_batched(y, w_act, k, C.contiguous(), u=p_c, out=new(B, d, d))
     return m, p_sigma, p_c, sigma, C_new
 
 
-def _assigned_weights(f: torch.Tensor, maximize: bool, weights: torch.Tensor) -> torch.Tensor:
-    """weights[rank of f[b, i] in row b], best first: a stable sort, NaN the largest value (the order of rank_table_batched)."""
+def _assigned_weights(f: torch.Tensor, maximize: bool, weights: torch.Tensor, real: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """weights[rank of f[b, i] in row b], best first: a stable sort, NaN the largest value (the order of rank_table_batched).
+    With `real` (B, n) (a padded population), row b ranks only its real rows, in the same order, with its own weights[b] (B, n);
+    its pad rows come after them, at zero weight."""
     B, n = f.shape
     order = torch.argsort(f, dim=-1, descending=maximize, stable=True)
+    if real is not None:
+        order = order.gather(-1, torch.argsort((~real).gather(-1, order).to(torch.int32), dim=-1, stable=True))
     ranks = torch.empty_like(order).scatter_(-1, order, torch.arange(n, device=f.device).expand(B, n).contiguous())
+    if real is not None:
+        return torch.where(real, weights.gather(-1, ranks), 0.0)
     return weights.to(f.device)[ranks]
 
 
 def _h_sig(hp: CMAESHyperparameters, pnorm: torch.Tensor, d: int, steps) -> torch.Tensor:
     """CMAES._h_sig per item, with the generation counter `steps` (an int, or a tensor of per-item counters) before its increment."""
-    if isinstance(steps, torch.Tensor):
+    if isinstance(hp.c_sigma, torch.Tensor):
+        decay = 1 - (1 - hp.c_sigma).pow((2 * steps + 1).to(pnorm.dtype))
+    elif isinstance(steps, torch.Tensor):
         decay = 1 - torch.full_like(pnorm, 1 - hp.c_sigma).pow((2 * steps + 1).to(pnorm.dtype))
     else:
         decay = 1 - (1 - hp.c_sigma) ** (2 * steps + 1)
@@ -256,15 +298,20 @@ def _h_sig(hp: CMAESHyperparameters, pnorm: torch.Tensor, d: int, steps) -> torc
     return ((squared_sum / d) - 1 < 1 + 4.0 / (d + 1)).to(pnorm.dtype)
 
 
-def _tell_torch(state, hp, B, n, d, m, sigma, C, y, z, f, steps) -> tuple:
+def _tell_torch(state, hp, B, n, d, m, sigma, C, y, z, f, steps, tiers=None) -> tuple:
     """The same stages as batched torch ops (CMAES's op-by-op generation: update_m ... update_C, cmaes.py:454-553), with the
-    generation counter `steps` (an int, or per-item counters)."""
-    aw = _assigned_weights(f, state.maximize, hp.weights)
+    generation counter `steps` (an int, or per-item counters).  `tiers`: as in `_tell` (the constants become per-item tensors)."""
+    real = None
+    if tiers is None:
+        aw = _assigned_weights(f, state.maximize, hp.weights)
+    else:
+        hp, weights, real = _tier_items(tiers, n)
+        aw = _assigned_weights(f, state.maximize, weights, real)
     w_pos = torch.clamp_min(aw, 0.0)
     local = torch.einsum("bn,bnd->bd", w_pos, z)
     shaped = torch.einsum("bn,bnd->bd", w_pos, y)
-    m = m + hp.c_m * sigma[:, None] * shaped
-    p_sigma = (1 - hp.c_sigma) * state.p_sigma.reshape(B, d) + hp.variance_discount_sigma * local
+    m = m + _col(hp.c_m) * sigma[:, None] * shaped
+    p_sigma = _col(1 - hp.c_sigma) * state.p_sigma.reshape(B, d) + _col(hp.variance_discount_sigma) * local
     pnorm = torch.linalg.vector_norm(p_sigma, dim=-1)
     if state.csa_squared:
         expo = (pnorm.pow(2.0) / d - 1) / 2
@@ -272,10 +319,12 @@ def _tell_torch(state, hp, B, n, d, m, sigma, C, y, z, f, steps) -> tuple:
         expo = pnorm / hp.unbiased_expectation - 1
     sigma = sigma * torch.exp((hp.c_sigma / hp.damp_sigma) * expo)
     h_sig = _h_sig(hp, pnorm, d, steps)
-    p_c = (1 - hp.c_c) * state.p_c.reshape(B, d) + (h_sig * hp.variance_discount_c)[:, None] * shaped
+    p_c = _col(1 - hp.c_c) * state.p_c.reshape(B, d) + (h_sig * hp.variance_discount_c)[:, None] * shaped
     w = torch.where(aw > 0, aw, d * aw / torch.sum(z * z, dim=-1)) if state.active else aw
+    if real is not None:  # a pad row's 0 / ||0||^2
+        w = torch.where(real, w, 0.0)
     c1a = hp.c_1 * (1 - (1 - h_sig**2) * hp.c_c * (2 - hp.c_c))
     pc = ((hp.c_1 / (c1a + 1e-23)) ** 0.5)[:, None] * p_c
     r1 = c1a[:, None, None] * (pc[:, :, None] * pc[:, None, :] - C)
-    rmu = hp.c_mu * ((y.mT * w[:, None, :]) @ y - hp.weights_sum * C)
+    rmu = _col(hp.c_mu, 2) * ((y.mT * w[:, None, :]) @ y - _col(hp.weights_sum, 2) * C)
     return m, p_sigma, p_c, sigma, C + r1 + rmu

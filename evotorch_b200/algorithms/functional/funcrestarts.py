@@ -19,6 +19,14 @@ is not due, since which items are due is only known on the device.  Anywhere els
 
 `stop_flags` bits (ops.RESTART_CRITERIA): 0 tol_fun, 1 tol_x, 2 tol_x_up, 3 max_condition, 4 min_fitness_stdev, 5 max_generations,
 6 non-finite state (always on).
+
+IPOP (Auger & Hansen, "A Restart CMA Evolution Strategy With Increasing Population Size", CEC 2005):
+`restarts(state, ..., popsize_multiplier=2, max_popsize=640)` multiplies an item's population size at each of its restarts, along
+the ladder lambda_0 = state.popsize, lambda_{k+1} = min(int(multiplier * lambda_k), max_popsize), with the default learning rates
+of each size.  Items restart at different times, so the populations are padded: the ask draws max_popsize rows for every item
+(`rs.search` has the top tier's popsize) and item b uses only its first `rs.popsize[b]` rows.  Its other rows are pad rows: their
+values and evals may hold anything, NaN and inf included, and never reach the state, the best ever, the history or the criteria.
+On the kernels the stages that depend on the population size read the item's tier from device tables: still no host reads.
 """
 
 from __future__ import annotations
@@ -29,11 +37,27 @@ from typing import NamedTuple, Optional, Union
 import torch
 
 from ... import ops
+from ..cmaes import CMAESHyperparameters, cmaes_hyperparameters
 from . import funccmaes, funcsepcmaes
 from .funccmaes import CMAESState, _host_float
 from .funcsepcmaes import SepCMAESState
 from .fused import LazyPopulation
 from .misc import draw_philox_seed, on_kernels
+
+MAX_TIERED_POPSIZE = 8192  # on the kernels: the largest padded population the one-launch counting rank takes
+
+
+class IPOPLadder(NamedTuple):
+    """The population sizes of an IPOP restart state and their constants: host values per tier k, and the device tables the
+    tiered stages read at an item's tier."""
+    popsizes: tuple  # lambda_k (host ints), increasing; the last is max_popsize
+    history_lengths: tuple  # H_k = 10 + ceil(30 D / lambda_k) (host ints), decreasing
+    hyperparameters: tuple  # CMAESHyperparameters of each tier
+    counts: torch.Tensor  # (K,) int32: lambda_k
+    history: torch.Tensor  # (K,) int64: H_k
+    weights: torch.Tensor  # (K, max_popsize): the weights of tier k, zero past lambda_k
+    consts: torch.Tensor  # (K, 10): the update constants of tier k (funccmaes.CONST_NAMES)
+    decompose_C_freq: torch.Tensor  # (K,) int64
 
 
 class RestartState(NamedTuple):
@@ -53,11 +77,22 @@ class RestartState(NamedTuple):
     max_condition: Optional[float]
     min_fitness_stdev: Optional[float]
     max_generations: Optional[float]
+    # IPOP only (None otherwise); the history ring has H_0 slots, of which an item at tier k uses the first H_k
+    tier: Optional[torch.Tensor] = None  # (...) int32: the item's rung of the ladder
+    num_evaluations: Optional[torch.Tensor] = None  # (...) int64: the rows told to the item so far, lambda of its tier per tell
+    ladder: Optional[IPOPLadder] = None
 
     @property
     def thresholds(self) -> tuple:
         """The thresholds in the order of ops.RESTART_CRITERIA (None = off)."""
         return tuple(getattr(self, name) for name in ops.RESTART_CRITERIA)
+
+    @property
+    def popsize(self) -> torch.Tensor:
+        """(...) the number of rows each item uses: lambda of its tier (a device gather), or the search's popsize."""
+        if self.ladder is None:
+            return torch.full(self.best_evals.shape, self.search.popsize, dtype=torch.int64, device=self.best_evals.device)
+        return self.ladder.counts.long()[self.tier.long()]
 
 
 def history_length(d: int, popsize: int) -> int:
@@ -65,12 +100,64 @@ def history_length(d: int, popsize: int) -> int:
     return 10 + math.ceil(30 * d / popsize)
 
 
+def _same_hyperparameters(a: CMAESHyperparameters, b: CMAESHyperparameters) -> bool:
+    return all(torch.equal(x, y) if isinstance(x, torch.Tensor) else x == y for x, y in zip(a, b))
+
+
+def ipop_ladder(state: Union[CMAESState, SepCMAESState], popsize_multiplier, max_popsize) -> IPOPLadder:
+    """The IPOP ladder of `state` (see `restarts`).  Raises ValueError for a multiplier <= 1, a max_popsize below state.popsize, a
+    step that does not grow, max_popsize > MAX_TIERED_POPSIZE on the kernels, and a state whose constants are not the defaults of
+    its population size."""
+    if max_popsize is None:
+        raise ValueError("IPOP restarts need `max_popsize`, the population size the ladder stops at")
+    mult = _host_float(popsize_multiplier, "popsize_multiplier")
+    if not mult > 1.0:
+        raise ValueError(f"`popsize_multiplier` must be > 1, got {mult}")
+    lam0, cap = state.popsize, int(max_popsize)
+    if cap < lam0:
+        raise ValueError(f"`max_popsize` ({cap}) is below the search's popsize ({lam0})")
+    sizes = [lam0]
+    while sizes[-1] < cap:
+        nxt = int(mult * sizes[-1])
+        if nxt <= sizes[-1]:
+            raise ValueError(f"popsize_multiplier {mult} does not grow the population size {sizes[-1]} (int({mult} * {sizes[-1]}) = {nxt})")
+        sizes.append(min(nxt, cap))
+    center = state.center
+    if on_kernels(center) and cap > MAX_TIERED_POPSIZE:
+        raise ValueError(f"`max_popsize` {cap} is above {MAX_TIERED_POPSIZE}, the largest padded population the kernels rank")
+    sep, d = isinstance(state, SepCMAESState), center.shape[-1]
+    make = lambda lam, limit: cmaes_hyperparameters(d, lam, dtype=center.dtype, device=center.device, active=state.active,  # noqa: E731
+                                                    separable=sep, limit_C_decomposition=limit)
+    limit = next((lim for lim in (True, False) if _same_hyperparameters(make(lam0, lim), state.hyperparameters)), None)
+    if limit is None:
+        raise ValueError("IPOP uses the default learning rates of each population size: build the search with the default c_m and "
+                         "learning-rate ratios")
+    hps = tuple(make(lam, limit) for lam in sizes)
+    K = len(sizes)
+    weights = torch.zeros(K, cap, dtype=center.dtype, device=center.device)
+    for k, hp in enumerate(hps):
+        weights[k, :hp.popsize] = hp.weights
+    hist = tuple(history_length(d, lam) for lam in sizes)
+    dev = center.device
+    return IPOPLadder(popsizes=tuple(sizes), history_lengths=hist, hyperparameters=hps, counts=torch.tensor(sizes, dtype=torch.int32, device=dev),
+                      history=torch.tensor(hist, dtype=torch.int64, device=dev), weights=weights,
+                      consts=torch.tensor([funccmaes._consts(hp) for hp in hps], dtype=center.dtype, device=dev),
+                      decompose_C_freq=torch.tensor([hp.decompose_C_freq for hp in hps], dtype=torch.int64, device=dev))
+
+
 def restarts(state: Union[CMAESState, SepCMAESState], *, lb, ub, tol_fun: Optional[float] = 1e-12, tol_x: Optional[float] = 1e-12,
              tol_x_up: Optional[float] = 1e4, max_condition: Optional[float] = 1e14, min_fitness_stdev: Optional[float] = None,
-             max_generations: Optional[int] = None) -> RestartState:
+             max_generations: Optional[int] = None, popsize_multiplier: Optional[float] = None, max_popsize: Optional[int] = None) -> RestartState:
     """A restart state around `state` (a `CMAESState` or `SepCMAESState`).  `lb`, `ub`: the box the restarted centres are drawn
     from, scalars, (D,) or (..., D), finite with lb < ub.  A threshold of None turns its criterion off.  Every item's generation
-    counter starts at `state.generation` and its restart step size is its current sigma."""
+    counter starts at `state.generation` and its restart step size is its current sigma.
+
+    IPOP: with `popsize_multiplier` (> 1) and `max_popsize` (required with it), every item starts at tier 0, popsize
+    lambda_0 = state.popsize, and each of its restarts moves it one tier up the ladder lambda_{k+1} = min(int(popsize_multiplier *
+    lambda_k), max_popsize) (`ipop_ladder`), with the hyperparameters of `cmaes_hyperparameters` at that size.  `state` must have
+    the default constants of its own size.  `rs.search` then asks for max_popsize rows per item (its popsize is the top tier's);
+    item b uses the first `rs.popsize[b]` and ignores the others (pad rows, which may hold anything).  On the kernels
+    max_popsize is at most 8192."""
     if not isinstance(state, (CMAESState, SepCMAESState)):
         raise TypeError(f"`restarts` takes a CMAESState or a SepCMAESState, got {type(state).__name__}")
     center = state.center
@@ -91,10 +178,15 @@ def restarts(state: Union[CMAESState, SepCMAESState], *, lb, ub, tol_fun: Option
                     ("min_fitness_stdev", min_fitness_stdev), ("max_generations", max_generations)):
         th[name] = None if v is None else _host_float(v, name)
     maximize = state.maximize
+    ladder = None
+    if popsize_multiplier is not None or max_popsize is not None:
+        if popsize_multiplier is None:
+            raise ValueError("`max_popsize` is the cap of IPOP restarts: give `popsize_multiplier` with it")
+        ladder = ipop_ladder(state, popsize_multiplier, max_popsize)
     H = history_length(d, state.popsize)
     opts = dict(dtype=center.dtype, device=center.device)
     return RestartState(
-        search=state,
+        search=state if ladder is None else state._replace(hyperparameters=ladder.hyperparameters[-1]),
         best_values=torch.full(batch + (d,), math.nan, **opts),
         best_evals=torch.full(batch, -math.inf if maximize else math.inf, **opts),
         num_restarts=torch.zeros(batch, dtype=torch.int64, device=center.device),
@@ -105,20 +197,26 @@ def restarts(state: Union[CMAESState, SepCMAESState], *, lb, ub, tol_fun: Option
         lb=lb_t,
         ub=ub_t,
         **th,
+        **({} if ladder is None else dict(tier=torch.zeros(batch, dtype=torch.int32, device=center.device),
+                                          num_evaluations=torch.zeros(batch, dtype=torch.int64, device=center.device), ladder=ladder)),
     )
 
 
 def restarts_tell(rs: RestartState, values: Union[torch.Tensor, LazyPopulation], evals: torch.Tensor) -> RestartState:
     """The family's tell with per-item generation counters, then per item: best ever, history, the criteria, and the re-initialisation
     of the items that met one.  `values` as the family's tell takes it (a separable search also takes the LazyPopulation that
-    `sepcmaes_ask_and_evaluate(..., lazy=True)` returned).  `rs` is left unchanged."""
+    `sepcmaes_ask_and_evaluate(..., lazy=True)` returned).  `rs` is left unchanged.  IPOP: item b at tier k is told its first
+    lambda_k rows with tier k's constants; its evaluations count grows by lambda_k, and a restart moves it to tier k + 1 (the top
+    tier stays)."""
     search = rs.search
     sep = isinstance(search, SepCMAESState)
     center = search.center
     batch, d = tuple(center.shape[:-1]), center.shape[-1]
     B, n = math.prod(batch), search.popsize
     family = funcsepcmaes if sep else funccmaes
-    new, steps = family._tell(search, values, evals, rs.item_generation.reshape(B))
+    ipop = rs.ladder is not None
+    tier = rs.tier.reshape(B).clone() if ipop else None
+    new, steps = family._tell(search, values, evals, rs.item_generation.reshape(B), tiers=(rs.ladder, tier) if ipop else None)
     f = torch.as_tensor(evals, dtype=center.dtype, device=center.device).reshape(B, n)
     lazy = isinstance(values, LazyPopulation)
     x = None if lazy else torch.as_tensor(values, dtype=center.dtype, device=center.device).reshape(B, n, d)
@@ -128,30 +226,46 @@ def restarts_tell(rs: RestartState, values: Union[torch.Tensor, LazyPopulation],
     r = dict(history=rs.history.reshape(B, -1).clone(), best_x=rs.best_values.reshape(B, d).clone(), best_f=rs.best_evals.reshape(B).clone(),
              num_restarts=rs.num_restarts.reshape(B).clone())
     sigma0, lb, ub = rs.stdev_init.reshape(B), rs.lb.reshape(B, d), rs.ub.reshape(B, d)
+    n_evals = rs.num_evaluations.reshape(B).clone() if ipop else None
     if lazy or on_kernels(center):
         # in place on the tell's fresh tensors and on the clones above
         flags = torch.empty(B, dtype=torch.int32, device=center.device)
         draw = dict(m_draw=search.center.reshape(B, d), s_draw=search.s.reshape(B, d), draw_seed=values.seed) if lazy else {}
+        if ipop:
+            draw.update(tier=tier, tier_counts=rs.ladder.counts, tier_history=rs.ladder.history, num_evaluations=n_evals)
         ops.cma_restart_batched(sep, f.contiguous(), None if lazy else x.contiguous(), search.maximize, steps, st["m"], st["sigma"], st["p_sigma"],
                                 st["p_c"], st["C"], st["A"], st["s"], r["history"], r["best_x"], r["best_f"], r["num_restarts"], flags,
                                 sigma0.contiguous(), lb, ub, rs.thresholds, seed=draw_philox_seed(), **draw)
     else:
-        st, r, steps, flags = _restart_torch(rs.thresholds, sep, search.maximize, f, x, steps, st, r, sigma0, lb, ub)
+        if ipop:
+            r.update(tier=tier, num_evaluations=n_evals)
+        st, r, steps, flags = _restart_torch(rs.thresholds, sep, search.maximize, f, x, steps, st, r, sigma0, lb, ub, ladder=rs.ladder)
+        if ipop:
+            tier, n_evals = r["tier"], r["num_evaluations"]
     vec = batch + (d,)
     new = new._replace(center=st["m"].view(vec), sigma=st["sigma"].view(batch), p_sigma=st["p_sigma"].view(vec), p_c=st["p_c"].view(vec),
                        C=st["C"].view(vec if sep else vec + (d,)), A=st["A"].view(vec if sep else vec + (d,)),
                        **({"s": st["s"].view(vec)} if sep else {}))
     return rs._replace(search=new, best_values=r["best_x"].view(vec), best_evals=r["best_f"].view(batch), num_restarts=r["num_restarts"].view(batch),
-                       item_generation=steps.view(batch), history=r["history"].view(batch + (-1,)), stop_flags=flags.view(batch))
+                       item_generation=steps.view(batch), history=r["history"].view(batch + (-1,)), stop_flags=flags.view(batch),
+                       **(dict(tier=tier.view(batch), num_evaluations=n_evals.view(batch)) if ipop else {}))
 
 
-def _restart_torch(thresholds, sep, maximize, f, x, gen, st, r, sigma0, lb, ub) -> tuple:
-    """The restart stage as batched torch ops (the semantics of evok_cma_restart_batched; the new centres from torch.rand(B, D))."""
+def _restart_torch(thresholds, sep, maximize, f, x, gen, st, r, sigma0, lb, ub, ladder=None) -> tuple:
+    """The restart stage as batched torch ops (the semantics of evok_cma_restart_batched; the new centres from torch.rand(B, D)).
+    With `ladder` (IPOP; r then also holds "tier" and "num_evaluations"), N and H of each item come from its tier, and the
+    evaluation count and the tier advance follow (evok_cma_restart_batched_tiered)."""
     B, n = f.shape
     d = lb.shape[-1]
     H = r["history"].shape[-1]
     nan = torch.tensor(math.nan, dtype=f.dtype, device=f.device)
-    fin = torch.isfinite(f)
+    real = hreal = None
+    if ladder is not None:
+        t = r["tier"].long()
+        n_b, H = ladder.counts.long()[t], ladder.history[t]
+        real = torch.arange(n, device=f.device) < n_b[:, None]
+        hreal = torch.arange(r["history"].shape[-1], device=f.device) < H[:, None]
+    fin = torch.isfinite(f) if real is None else torch.isfinite(f) & real
     key = torch.where(fin, f, -math.inf if maximize else math.inf)
     idx = key.argmax(-1) if maximize else key.argmin(-1)  # the first of equal values: the lower row wins ties
     g_best = key.gather(-1, idx[:, None])[:, 0]
@@ -172,13 +286,27 @@ def _restart_torch(thresholds, sep, maximize, f, x, gen, st, r, sigma0, lb, ub) 
     ratio = nan_to(r_diag, -math.inf).amax(-1) / nan_to(r_diag, math.inf).amin(-1)
     zero = torch.zeros(B, dtype=torch.bool, device=f.device)
     th = dict(zip(ops.RESTART_CRITERIA, thresholds))
+    if real is None:
+        f_all_fin, h_all_fin = fin.all(-1), torch.isfinite(history).all(-1)
+        f_max, f_min, h_max, h_min = f.amax(-1), f.amin(-1), history.amax(-1), history.amin(-1)
+        too_flat = zero if th["min_fitness_stdev"] is None or n < 2 else f.std(-1) < th["min_fitness_stdev"]
+    else:  # only the first N_b values and H_b slots of each item
+        f_all_fin, h_all_fin = (fin | ~real).all(-1), (torch.isfinite(history) | ~hreal).all(-1)
+        f_max, f_min = torch.where(real, f, -math.inf).amax(-1), torch.where(real, f, math.inf).amin(-1)
+        h_max, h_min = torch.where(hreal, history, -math.inf).amax(-1), torch.where(hreal, history, math.inf).amin(-1)
+        too_flat = zero
+        if th["min_fitness_stdev"] is not None:
+            fr = torch.where(real, f, 0.0)
+            mean = fr.sum(-1) / n_b
+            var = torch.where(real, (fr - mean[:, None]) ** 2, 0.0).sum(-1) / (n_b - 1).clamp_min(1)
+            too_flat = (n_b > 1) & (var.sqrt() < th["min_fitness_stdev"])
     bits = [
-        zero if th["tol_fun"] is None else ((gen >= H) & fin.all(-1) & torch.isfinite(history).all(-1)
-                                            & (torch.maximum(f.amax(-1), history.amax(-1)) - torch.minimum(f.amin(-1), history.amin(-1)) < th["tol_fun"])),
+        zero if th["tol_fun"] is None else ((gen >= H) & f_all_fin & h_all_fin
+                                            & (torch.maximum(f_max, h_max) - torch.minimum(f_min, h_min) < th["tol_fun"])),
         zero if th["tol_x"] is None else sig * torch.maximum(max_pc, max_sd) < th["tol_x"] * sigma0,
         zero if th["tol_x_up"] is None else sig * max_sd > th["tol_x_up"] * sigma0,
         zero if th["max_condition"] is None else (ratio if sep else ratio * ratio) > th["max_condition"],
-        zero if th["min_fitness_stdev"] is None or n < 2 else f.std(-1) < th["min_fitness_stdev"],
+        too_flat,
         zero if th["max_generations"] is None else gen >= th["max_generations"],
         ~(sig > 0) | ~torch.isfinite(sig) | ~torch.isfinite(torch.cat([m, p_sigma, p_c, c_diag], -1)).all(-1),
     ]
@@ -192,5 +320,8 @@ def _restart_torch(thresholds, sep, maximize, f, x, gen, st, r, sigma0, lb, ub) 
     else:
         eye = torch.eye(d, dtype=f.dtype, device=f.device)
         out.update(C=torch.where(go[:, None, None], eye, C), A=torch.where(go[:, None, None], eye, A), s=None)
-    r = dict(history=torch.where(col, nan, history), best_x=best_x, best_f=best_f, num_restarts=r["num_restarts"] + go.to(torch.int64))
+    out_r = dict(history=torch.where(col, nan, history), best_x=best_x, best_f=best_f, num_restarts=r["num_restarts"] + go.to(torch.int64))
+    if ladder is not None:
+        out_r.update(num_evaluations=r["num_evaluations"] + n_b, tier=torch.where(go, torch.clamp_max(r["tier"] + 1, len(ladder.popsizes) - 1), r["tier"]))
+    r = out_r
     return out, r, torch.where(go, 0, gen), flags

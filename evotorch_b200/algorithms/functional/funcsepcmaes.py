@@ -29,7 +29,7 @@ import torch
 
 from ... import ops
 from ..cmaes import CMAESHyperparameters, cmaes_hyperparameters
-from .funccmaes import _assigned_weights, _consts, _h_sig, _host_float
+from .funccmaes import _assigned_weights, _col, _consts, _h_sig, _host_float, _tier_items
 from .fused import LazyPopulation, ask_and_evaluate
 from .misc import draw_philox_seed, on_kernels
 
@@ -142,9 +142,10 @@ def sepcmaes_tell(state: SepCMAESState, values: Union[torch.Tensor, LazyPopulati
     return _tell(state, values, evals, state.generation)[0]
 
 
-def _tell(state: SepCMAESState, values: Union[torch.Tensor, LazyPopulation], evals: torch.Tensor, steps) -> tuple:
+def _tell(state: SepCMAESState, values: Union[torch.Tensor, LazyPopulation], evals: torch.Tensor, steps, tiers=None) -> tuple:
     """(`sepcmaes_tell`'s next state, the generation counters after it).  `steps` drives h_sig and the decomposition schedule: the
-    int `state.generation`, or a (B,) int64 tensor of per-item counters."""
+    int `state.generation`, or a (B,) int64 tensor of per-item counters.  `tiers`: as in funccmaes._tell (a padded population:
+    item b is told its first ladder.popsizes[tier[b]] rows with the constants and decomposition schedule of its tier)."""
     batch, B, d = _items(state)
     n = state.popsize
     m0 = state.center
@@ -162,10 +163,10 @@ def _tell(state: SepCMAESState, values: Union[torch.Tensor, LazyPopulation], eva
     per_item = isinstance(steps, torch.Tensor)
     if lazy or on_kernels(m0, values, f):
         counters = steps.clone() if per_item else steps  # the kernel increments per-item counters in place
-        new = _tell_kernels(state, B, n, d, values, f, counters)
+        new = _tell_kernels(state, B, n, d, values, f, counters, tiers)
         steps_next = counters if per_item else steps + 1
     else:
-        new = _tell_torch(state, B, n, d, values.reshape(B, n, d), f, steps)
+        new = _tell_torch(state, B, n, d, values.reshape(B, n, d), f, steps, tiers)
         steps_next = steps + 1
     m, sigma, C, A, s, p_sigma, p_c = new
     vec = batch + (d,)
@@ -174,39 +175,49 @@ def _tell(state: SepCMAESState, values: Union[torch.Tensor, LazyPopulation], eva
     return new_state, steps_next
 
 
-def _tell_kernels(state, B, n, d, values, f, steps) -> tuple:
+def _tell_kernels(state, B, n, d, values, f, steps, tiers=None) -> tuple:
     """Rank table, moments (row pass + column pass) and update, one launch each for all items; every output is a new tensor.
-    `steps`: the shared int counter, or the per-item int64 counters, which the update increments."""
+    `steps`: the shared int counter, or the per-item int64 counters, which the update increments.  `tiers`: as in `_tell`; the
+    moments never read (or rebuild) a pad row, whose weight is 0."""
     hp = state.hyperparameters
     lazy = isinstance(values, LazyPopulation)
     m, s = state.center.reshape(B, d).contiguous(), state.s.reshape(B, d).contiguous()
-    aw = ops.rank_table_batched(f, state.maximize, hp.weights)
+    if tiers is None:
+        aw = ops.rank_table_batched(f, state.maximize, hp.weights)
+        consts, freq, tier = _consts(hp), hp.decompose_C_freq, None
+    else:
+        ladder, tier = tiers
+        aw = ops.rank_table_batched(f, state.maximize, ladder.weights, tier=tier, counts=ladder.counts)
+        consts, freq = ladder.consts, ladder.decompose_C_freq
     X = None if lazy else values.reshape(B, n, d).contiguous()
     local, S2, wsum = ops.sepcma_moments_batched(X, m, s, aw, state.active, seed=values.seed if lazy else 0)
     out = [t.reshape(B, d).clone() for t in (state.center, state.C, state.A, state.s, state.p_sigma, state.p_c)]
     m_new, C, A, s_new, p_sigma, p_c = out
     sigma = state.sigma.reshape(B).clone()
-    ops.sepcma_update_batched(local, S2, wsum, m_new, p_sigma, p_c, sigma, C, A, s_new, _consts(hp), state.csa_squared, steps=steps,
-                              decompose_C_freq=hp.decompose_C_freq, stdev_min=state.stdev_min, stdev_max=state.stdev_max)
+    ops.sepcma_update_batched(local, S2, wsum, m_new, p_sigma, p_c, sigma, C, A, s_new, consts, state.csa_squared, steps=steps,
+                              decompose_C_freq=freq, stdev_min=state.stdev_min, stdev_max=state.stdev_max, tier=tier)
     return m_new, sigma, C, A, s_new, p_sigma, p_c
 
 
-def _tell_torch(state, B, n, d, x, f, steps) -> tuple:
+def _tell_torch(state, B, n, d, x, f, steps, tiers=None) -> tuple:
     """The same generation as batched torch ops (CMAES's op-by-op generation with separable=True, cmaes.py:454-565), with the
-    generation counter `steps` (an int, or per-item counters)."""
+    generation counter `steps` (an int, or per-item counters).  `tiers`: as in `_tell` (the constants become per-item tensors)."""
     hp = state.hyperparameters
     m, sigma, C, A, s = state.center.reshape(B, d), state.sigma.reshape(B), state.C.reshape(B, d), state.A.reshape(B, d), state.s.reshape(B, d)
+    if tiers is not None:  # pad rows at the centre: their z is exactly 0, whatever they held
+        hp, weights, real = _tier_items(tiers, n)
+        x = torch.where(real[:, :, None], x, m[:, None, :])
     z = (x - m[:, None, :]) / s[:, None, :]
     zz = z * z
-    aw = _assigned_weights(f, state.maximize, hp.weights)
+    aw = _assigned_weights(f, state.maximize, hp.weights) if tiers is None else _assigned_weights(f, state.maximize, weights, real)
     a = torch.clamp_min(aw, 0.0)
     b = torch.where(aw < 0, d * aw / zz.sum(-1), aw) if state.active else aw
     local = torch.einsum("bn,bnd->bd", a, z)
     S2 = torch.einsum("bn,bnd->bd", b, zz)
     wsum = b.sum(-1)
     shaped = A * local
-    m = m + hp.c_m * sigma[:, None] * shaped
-    p_sigma = (1 - hp.c_sigma) * state.p_sigma.reshape(B, d) + hp.variance_discount_sigma * local
+    m = m + _col(hp.c_m) * sigma[:, None] * shaped
+    p_sigma = _col(1 - hp.c_sigma) * state.p_sigma.reshape(B, d) + _col(hp.variance_discount_sigma) * local
     pnorm = torch.linalg.vector_norm(p_sigma, dim=-1)
     if state.csa_squared:
         expo = (pnorm.pow(2.0) / d - 1) / 2
@@ -214,9 +225,9 @@ def _tell_torch(state, B, n, d, x, f, steps) -> tuple:
         expo = pnorm / hp.unbiased_expectation - 1
     sigma = sigma * torch.exp((hp.c_sigma / hp.damp_sigma) * expo)
     h_sig = _h_sig(hp, pnorm, d, steps)
-    p_c = (1 - hp.c_c) * state.p_c.reshape(B, d) + (h_sig * hp.variance_discount_c)[:, None] * shaped
+    p_c = _col(1 - hp.c_c) * state.p_c.reshape(B, d) + (h_sig * hp.variance_discount_c)[:, None] * shaped
     c1a = hp.c_1 * (1 - (1 - h_sig**2) * hp.c_c * (2 - hp.c_c))
-    C = C + c1a[:, None] * (p_c.pow(2.0) - C) + hp.c_mu * (A.pow(2.0) * S2 - wsum[:, None] * C)
+    C = C + c1a[:, None] * (p_c.pow(2.0) - C) + _col(hp.c_mu) * (A.pow(2.0) * S2 - wsum[:, None] * C)
     if state.stdev_min is not None or state.stdev_max is not None:  # CMAES._limit_stdev, with the new sigma
         stdevs = torch.clamp(sigma[:, None] * torch.sqrt(C), min=state.stdev_min, max=state.stdev_max)
         C = (stdevs / sigma[:, None]).pow(2.0)

@@ -13,9 +13,11 @@
 namespace evok {
 
 // one warp per row: ||z_i||^2, then the two weight vectors.  grid y = item: Z at item stride item_stride_z, aw / w_pos / w_act at N
+// TIERED (padded populations): item b uses its first counts[tier[b]] rows; w_pos = w_act = 0 on the others, whatever Z holds there
+template <bool TIERED>
 __global__ void __launch_bounds__(256) cmaes_row_weights_kernel(const float* __restrict__ aw, const float* __restrict__ Z, int64_t ldz, int64_t N,
                                                                 int64_t D, int active, float* __restrict__ w_pos, float* __restrict__ w_act,
-                                                                int64_t item_stride_z) {
+                                                                int64_t item_stride_z, const int* __restrict__ tier, const int* __restrict__ counts) {
   const int lane = threadIdx.x & 31;
   const int64_t row = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
   if (row >= N) return;
@@ -23,6 +25,10 @@ __global__ void __launch_bounds__(256) cmaes_row_weights_kernel(const float* __r
   aw += blockIdx.y * N;
   w_pos += blockIdx.y * N;
   w_act += blockIdx.y * N;
+  if (TIERED && row >= counts[tier[blockIdx.y]]) {
+    if (lane == 0) w_pos[row] = w_act[row] = 0.0f;
+    return;
+  }
   const float a = aw[row];
   float out_act = a;
   if (active && !(a > 0.0f)) {  // only the non-positive weights need the row norm (cmaes.py:532)
@@ -54,6 +60,17 @@ struct CmaesConsts {
 };
 
 constexpr int kCmaThreads = 1024;
+
+// padded populations (the *_tiered entries): the constants of tier k, row k of a device table [tiers][10] in the order of
+// cmaes_consts; csa_squared stays the shared one
+__device__ __forceinline__ CmaesConsts tier_consts(const CmaesConsts& shared, const float* __restrict__ tab, int k) {
+  const float* r = tab + (int64_t)k * 10;
+  CmaesConsts c;
+  c.c_m = r[0]; c.c_sigma = r[1]; c.damp_sigma = r[2]; c.c_c = r[3]; c.c_1 = r[4]; c.c_mu = r[5]; c.vd_sigma = r[6]; c.vd_c = r[7];
+  c.unbiased_expectation = r[8]; c.weights_sum = r[9];
+  c.csa_squared = shared.csa_squared;
+  return c;
+}
 
 struct CmaVectorStep {
   float new_sigma, h;
@@ -96,12 +113,15 @@ __device__ __forceinline__ CmaVectorStep cma_vector_step(const float* __restrict
 }
 
 // one CTA per item (grid x): the D-vectors of item b at b * D, its sigma at b, its k_out at 3 b, its step counter (nullable) at
-// steps_dev[b] (h_sig_out: single call only)
+// steps_dev[b] (h_sig_out: single call only).  TIERED: item b's constants are row tier[b] of consts_tab.
+template <bool TIERED>
 __global__ void __launch_bounds__(kCmaThreads)
     cmaes_vector_update_kernel(const float* __restrict__ local_disp, const float* __restrict__ shaped_disp, int64_t D, float* __restrict__ m,
                                float* __restrict__ p_sigma, float* __restrict__ p_c, float* __restrict__ sigma, long long* steps_dev,
-                               long long steps_host, const __grid_constant__ CmaesConsts c, float* __restrict__ k_out, float* __restrict__ h_sig_out) {
+                               long long steps_host, const __grid_constant__ CmaesConsts shared, float* __restrict__ k_out, float* __restrict__ h_sig_out,
+                               const int* __restrict__ tier, const float* __restrict__ consts_tab) {
   __shared__ double sm[33];
+  const CmaesConsts c = TIERED ? tier_consts(shared, consts_tab, tier[blockIdx.x]) : shared;
   const int64_t off = (int64_t)blockIdx.x * D;
   local_disp += off;
   shaped_disp += off;
@@ -133,14 +153,19 @@ __global__ void __launch_bounds__(kCmaThreads)
 //   stdev bounds with the new sigma: C <- (clamp(sigma' sqrt(C), lo, hi) / sigma')^2
 //   A <- sqrt(C) on the generations where (steps + 1) % decompose_freq == 0;   s <- sigma' A  (the sampler's per-column stdev)
 // s_prev (nullable) receives s before the update.  lo / hi: NaN = no bound.  Grid x = item: the D-vectors of item b at b * D, its sigma
-// and wsum at b, its step counter (nullable) at steps_dev[b] (m_prev / s_prev / h_sig_out: single call only).
+// and wsum at b, its step counter (nullable) at steps_dev[b] (m_prev / s_prev / h_sig_out: single call only).  TIERED: item b's
+// constants are row tier[b] of consts_tab and its decomposition period freq_tab[tier[b]].
+template <bool TIERED>
 __global__ void __launch_bounds__(kCmaThreads)
     sepcma_update_kernel(const float* __restrict__ local_disp, const float* __restrict__ S2, const float* __restrict__ wsum, int64_t D,
                          float* __restrict__ m, float* __restrict__ p_sigma, float* __restrict__ p_c, float* __restrict__ sigma, float* __restrict__ C,
                          float* __restrict__ A, float* __restrict__ s, float* __restrict__ m_prev, float* __restrict__ s_prev, long long* steps_dev,
-                         long long steps_host, const __grid_constant__ CmaesConsts c, long long decompose_freq, float lo, float hi,
-                         float* __restrict__ h_sig_out) {
+                         long long steps_host, const __grid_constant__ CmaesConsts shared, long long decompose_freq_shared, float lo, float hi,
+                         float* __restrict__ h_sig_out, const int* __restrict__ tier, const float* __restrict__ consts_tab,
+                         const long long* __restrict__ freq_tab) {
   __shared__ double sm[33];
+  const CmaesConsts c = TIERED ? tier_consts(shared, consts_tab, tier[blockIdx.x]) : shared;
+  const long long decompose_freq = TIERED ? freq_tab[tier[blockIdx.x]] : decompose_freq_shared;
   const int64_t off = (int64_t)blockIdx.x * D;
   local_disp += off;
   S2 += off;
@@ -190,21 +215,38 @@ extern "C" EVOK_API int evok_cmaes_row_weights(const float* assigned_weights, co
                                                float* w_positive, float* w_active, void* stream) {
   if (!assigned_weights || !Z || !w_positive || !w_active) return EVOK_E_NULLPTR;
   if (N <= 0 || D <= 0 || ldz < D) return EVOK_E_BADSIZE;
-  cmaes_row_weights_kernel<<<(unsigned)((N + 7) / 8), 256, 0, (cudaStream_t)stream>>>(assigned_weights, Z, ldz, N, D, active, w_positive, w_active, 0);
+  cmaes_row_weights_kernel<false><<<(unsigned)((N + 7) / 8), 256, 0, (cudaStream_t)stream>>>(assigned_weights, Z, ldz, N, D, active, w_positive,
+                                                                                       w_active, 0, nullptr, nullptr);
   EVOK_CHECK_LAUNCH();
   return 0;
 }
 
-extern "C" EVOK_API int evok_cmaes_row_weights_batched(const float* assigned_weights, const float* Z, int64_t item_stride_z, int64_t ldz, int64_t n_items,
-                                                       int64_t N, int64_t D, int active, float* w_positive, float* w_active, void* stream) {
+// the batched row weights, every row of every item (tier == NULL) or the first counts[tier[b]] rows of item b
+template <bool TIERED>
+static int cmaes_row_weights_items(const float* assigned_weights, const float* Z, int64_t item_stride_z, int64_t ldz, int64_t n_items, int64_t N,
+                                   int64_t D, int active, const int32_t* tier, const int32_t* counts, float* w_positive, float* w_active,
+                                   void* stream) {
   if (!assigned_weights || !Z || !w_positive || !w_active) return EVOK_E_NULLPTR;
   if (n_items < 0 || N <= 0 || D <= 0 || ldz < D || item_stride_z < 0) return EVOK_E_BADSIZE;
   return for_item_chunks(n_items, kMaxGridY, [&](int64_t b0, int64_t nb) {
-    cmaes_row_weights_kernel<<<dim3((unsigned)((N + 7) / 8), (unsigned)nb), 256, 0, (cudaStream_t)stream>>>(
-        assigned_weights + b0 * N, Z + b0 * item_stride_z, ldz, N, D, active, w_positive + b0 * N, w_active + b0 * N, item_stride_z);
+    cmaes_row_weights_kernel<TIERED><<<dim3((unsigned)((N + 7) / 8), (unsigned)nb), 256, 0, (cudaStream_t)stream>>>(
+        assigned_weights + b0 * N, Z + b0 * item_stride_z, ldz, N, D, active, w_positive + b0 * N, w_active + b0 * N, item_stride_z,
+        TIERED ? tier + b0 : nullptr, counts);
     EVOK_CHECK_LAUNCH();
     return 0;
   });
+}
+
+extern "C" EVOK_API int evok_cmaes_row_weights_batched(const float* assigned_weights, const float* Z, int64_t item_stride_z, int64_t ldz, int64_t n_items,
+                                                       int64_t N, int64_t D, int active, float* w_positive, float* w_active, void* stream) {
+  return cmaes_row_weights_items<false>(assigned_weights, Z, item_stride_z, ldz, n_items, N, D, active, nullptr, nullptr, w_positive, w_active, stream);
+}
+
+extern "C" EVOK_API int evok_cmaes_row_weights_batched_tiered(const float* assigned_weights, const float* Z, int64_t item_stride_z, int64_t ldz,
+                                                              int64_t n_items, int64_t N, int64_t D, int active, const int32_t* tier,
+                                                              const int32_t* counts, float* w_positive, float* w_active, void* stream) {
+  if (!tier || !counts) return EVOK_E_NULLPTR;
+  return cmaes_row_weights_items<true>(assigned_weights, Z, item_stride_z, ldz, n_items, N, D, active, tier, counts, w_positive, w_active, stream);
 }
 
 static CmaesConsts cmaes_consts(const float* consts_host, int csa_squared) {
@@ -222,25 +264,29 @@ extern "C" EVOK_API int evok_cmaes_vector_update(const float* local_disp, const 
   if (!local_disp || !shaped_disp || !m || !p_sigma || !p_c || !sigma_dev || !consts_host || !k_out) return EVOK_E_NULLPTR;
   if (D <= 0) return EVOK_E_BADSIZE;
   const CmaesConsts c = cmaes_consts(consts_host, csa_squared);
-  cmaes_vector_update_kernel<<<1, kCmaThreads, 0, (cudaStream_t)stream>>>(local_disp, shaped_disp, D, m, p_sigma, p_c, sigma_dev,
-                                                                         reinterpret_cast<long long*>(steps_dev), (long long)steps_host, c, k_out,
-                                                                         h_sig_out);
+  cmaes_vector_update_kernel<false><<<1, kCmaThreads, 0, (cudaStream_t)stream>>>(local_disp, shaped_disp, D, m, p_sigma, p_c, sigma_dev,
+                                                                                reinterpret_cast<long long*>(steps_dev), (long long)steps_host, c, k_out,
+                                                                                h_sig_out, nullptr, nullptr);
   EVOK_CHECK_LAUNCH();
   return 0;
 }
 
-// the batched vector update with a shared step counter (steps_dev == NULL) or one per item (steps_dev[b])
+// the batched vector update with a shared step counter (steps_dev == NULL) or one per item (steps_dev[b]), with the shared
+// constants of consts_host or (TIERED) item b's row tier[b] of the device table consts_dev
+template <bool TIERED>
 static int cmaes_vector_update_items(const float* local_disp, const float* shaped_disp, int64_t n_items, int64_t D, float* m, float* p_sigma,
                                      float* p_c, float* sigma_dev, int64_t* steps_dev, int64_t steps_host, const float* consts_host, int csa_squared,
-                                     float* k_out, void* stream) {
-  if (!local_disp || !shaped_disp || !m || !p_sigma || !p_c || !sigma_dev || !consts_host || !k_out) return EVOK_E_NULLPTR;
+                                     float* k_out, const int32_t* tier, const float* consts_dev, void* stream) {
+  if (!local_disp || !shaped_disp || !m || !p_sigma || !p_c || !sigma_dev || !(TIERED ? consts_dev : consts_host) || !k_out) return EVOK_E_NULLPTR;
   if (n_items < 0 || D <= 0) return EVOK_E_BADSIZE;
-  const CmaesConsts c = cmaes_consts(consts_host, csa_squared);
+  const float zeros[10] = {};
+  const CmaesConsts c = cmaes_consts(TIERED ? zeros : consts_host, csa_squared);
   return for_item_chunks(n_items, (int64_t)INT32_MAX, [&](int64_t b0, int64_t nb) {
     const int64_t off = b0 * D;
-    cmaes_vector_update_kernel<<<(unsigned)nb, kCmaThreads, 0, (cudaStream_t)stream>>>(
+    cmaes_vector_update_kernel<TIERED><<<(unsigned)nb, kCmaThreads, 0, (cudaStream_t)stream>>>(
         local_disp + off, shaped_disp + off, D, m + off, p_sigma + off, p_c + off, sigma_dev + b0,
-        steps_dev ? reinterpret_cast<long long*>(steps_dev + b0) : nullptr, (long long)steps_host, c, k_out + 3 * b0, nullptr);
+        steps_dev ? reinterpret_cast<long long*>(steps_dev + b0) : nullptr, (long long)steps_host, c, k_out + 3 * b0, nullptr,
+        TIERED ? tier + b0 : nullptr, consts_dev);
     EVOK_CHECK_LAUNCH();
     return 0;
   });
@@ -249,16 +295,25 @@ static int cmaes_vector_update_items(const float* local_disp, const float* shape
 extern "C" EVOK_API int evok_cmaes_vector_update_batched(const float* local_disp, const float* shaped_disp, int64_t n_items, int64_t D, float* m,
                                                          float* p_sigma, float* p_c, float* sigma_dev, int64_t steps_host, const float* consts_host,
                                                          int csa_squared, float* k_out, void* stream) {
-  return cmaes_vector_update_items(local_disp, shaped_disp, n_items, D, m, p_sigma, p_c, sigma_dev, nullptr, steps_host, consts_host, csa_squared,
-                                   k_out, stream);
+  return cmaes_vector_update_items<false>(local_disp, shaped_disp, n_items, D, m, p_sigma, p_c, sigma_dev, nullptr, steps_host, consts_host,
+                                          csa_squared, k_out, nullptr, nullptr, stream);
 }
 
 extern "C" EVOK_API int evok_cmaes_vector_update_batched_steps(const float* local_disp, const float* shaped_disp, int64_t n_items, int64_t D,
                                                                float* m, float* p_sigma, float* p_c, float* sigma_dev, int64_t* steps_dev,
                                                                const float* consts_host, int csa_squared, float* k_out, void* stream) {
   if (!steps_dev) return EVOK_E_NULLPTR;
-  return cmaes_vector_update_items(local_disp, shaped_disp, n_items, D, m, p_sigma, p_c, sigma_dev, steps_dev, 0, consts_host, csa_squared, k_out,
-                                   stream);
+  return cmaes_vector_update_items<false>(local_disp, shaped_disp, n_items, D, m, p_sigma, p_c, sigma_dev, steps_dev, 0, consts_host, csa_squared,
+                                          k_out, nullptr, nullptr, stream);
+}
+
+extern "C" EVOK_API int evok_cmaes_vector_update_batched_tiered(const float* local_disp, const float* shaped_disp, int64_t n_items, int64_t D,
+                                                                float* m, float* p_sigma, float* p_c, float* sigma_dev, int64_t* steps_dev,
+                                                                const int32_t* tier, const float* consts_dev, int csa_squared, float* k_out,
+                                                                void* stream) {
+  if (!steps_dev || !tier) return EVOK_E_NULLPTR;
+  return cmaes_vector_update_items<true>(local_disp, shaped_disp, n_items, D, m, p_sigma, p_c, sigma_dev, steps_dev, 0, nullptr, csa_squared, k_out,
+                                         tier, consts_dev, stream);
 }
 
 extern "C" EVOK_API int evok_sepcma_update(const float* local_disp, const float* S2, const float* wsum, int64_t D, float* m, float* p_sigma, float* p_c,
@@ -268,26 +323,32 @@ extern "C" EVOK_API int evok_sepcma_update(const float* local_disp, const float*
   if (!local_disp || !S2 || !wsum || !m || !p_sigma || !p_c || !sigma_dev || !C || !A || !s || !consts_host) return EVOK_E_NULLPTR;
   if (D <= 0 || decompose_C_freq < 1) return EVOK_E_BADSIZE;
   const CmaesConsts c = cmaes_consts(consts_host, csa_squared);
-  sepcma_update_kernel<<<1, kCmaThreads, 0, (cudaStream_t)stream>>>(local_disp, S2, wsum, D, m, p_sigma, p_c, sigma_dev, C, A, s, m_prev, s_prev,
-                                                                   reinterpret_cast<long long*>(steps_dev), (long long)steps_host, c,
-                                                                   (long long)decompose_C_freq, stdev_min, stdev_max, h_sig_out);
+  sepcma_update_kernel<false><<<1, kCmaThreads, 0, (cudaStream_t)stream>>>(local_disp, S2, wsum, D, m, p_sigma, p_c, sigma_dev, C, A, s, m_prev,
+                                                                          s_prev, reinterpret_cast<long long*>(steps_dev), (long long)steps_host, c,
+                                                                          (long long)decompose_C_freq, stdev_min, stdev_max, h_sig_out, nullptr, nullptr,
+                                                                          nullptr);
   EVOK_CHECK_LAUNCH();
   return 0;
 }
 
-// the batched separable update with a shared step counter (steps_dev == NULL) or one per item (steps_dev[b])
+// the batched separable update with a shared step counter (steps_dev == NULL) or one per item (steps_dev[b]), with the shared
+// constants and decomposition period or (TIERED) item b's row tier[b] of the device tables consts_dev and freq_dev
+template <bool TIERED>
 static int sepcma_update_items(const float* local_disp, const float* S2, const float* wsum, int64_t n_items, int64_t D, float* m, float* p_sigma,
                                float* p_c, float* sigma_dev, float* C, float* A, float* s, int64_t* steps_dev, int64_t steps_host,
-                               const float* consts_host, int csa_squared, int64_t decompose_C_freq, float stdev_min, float stdev_max, void* stream) {
-  if (!local_disp || !S2 || !wsum || !m || !p_sigma || !p_c || !sigma_dev || !C || !A || !s || !consts_host) return EVOK_E_NULLPTR;
+                               const float* consts_host, int csa_squared, int64_t decompose_C_freq, float stdev_min, float stdev_max,
+                               const int32_t* tier, const float* consts_dev, const int64_t* freq_dev, void* stream) {
+  if (!local_disp || !S2 || !wsum || !m || !p_sigma || !p_c || !sigma_dev || !C || !A || !s || !(TIERED ? consts_dev && freq_dev : consts_host != nullptr))
+    return EVOK_E_NULLPTR;
   if (n_items < 0 || D <= 0 || decompose_C_freq < 1) return EVOK_E_BADSIZE;
-  const CmaesConsts c = cmaes_consts(consts_host, csa_squared);
+  const float zeros[10] = {};
+  const CmaesConsts c = cmaes_consts(TIERED ? zeros : consts_host, csa_squared);
   return for_item_chunks(n_items, (int64_t)INT32_MAX, [&](int64_t b0, int64_t nb) {
     const int64_t off = b0 * D;
-    sepcma_update_kernel<<<(unsigned)nb, kCmaThreads, 0, (cudaStream_t)stream>>>(
+    sepcma_update_kernel<TIERED><<<(unsigned)nb, kCmaThreads, 0, (cudaStream_t)stream>>>(
         local_disp + off, S2 + off, wsum + b0, D, m + off, p_sigma + off, p_c + off, sigma_dev + b0, C + off, A + off, s + off, nullptr, nullptr,
         steps_dev ? reinterpret_cast<long long*>(steps_dev + b0) : nullptr, (long long)steps_host, c, (long long)decompose_C_freq, stdev_min,
-        stdev_max, nullptr);
+        stdev_max, nullptr, TIERED ? tier + b0 : nullptr, consts_dev, reinterpret_cast<const long long*>(freq_dev));
     EVOK_CHECK_LAUNCH();
     return 0;
   });
@@ -297,8 +358,8 @@ extern "C" EVOK_API int evok_sepcma_update_batched(const float* local_disp, cons
                                                    float* p_sigma, float* p_c, float* sigma_dev, float* C, float* A, float* s, int64_t steps_host,
                                                    const float* consts_host, int csa_squared, int64_t decompose_C_freq, float stdev_min, float stdev_max,
                                                    void* stream) {
-  return sepcma_update_items(local_disp, S2, wsum, n_items, D, m, p_sigma, p_c, sigma_dev, C, A, s, nullptr, steps_host, consts_host, csa_squared,
-                             decompose_C_freq, stdev_min, stdev_max, stream);
+  return sepcma_update_items<false>(local_disp, S2, wsum, n_items, D, m, p_sigma, p_c, sigma_dev, C, A, s, nullptr, steps_host, consts_host, csa_squared,
+                                    decompose_C_freq, stdev_min, stdev_max, nullptr, nullptr, nullptr, stream);
 }
 
 extern "C" EVOK_API int evok_sepcma_update_batched_steps(const float* local_disp, const float* S2, const float* wsum, int64_t n_items, int64_t D,
@@ -306,6 +367,16 @@ extern "C" EVOK_API int evok_sepcma_update_batched_steps(const float* local_disp
                                                          int64_t* steps_dev, const float* consts_host, int csa_squared, int64_t decompose_C_freq,
                                                          float stdev_min, float stdev_max, void* stream) {
   if (!steps_dev) return EVOK_E_NULLPTR;
-  return sepcma_update_items(local_disp, S2, wsum, n_items, D, m, p_sigma, p_c, sigma_dev, C, A, s, steps_dev, 0, consts_host, csa_squared,
-                             decompose_C_freq, stdev_min, stdev_max, stream);
+  return sepcma_update_items<false>(local_disp, S2, wsum, n_items, D, m, p_sigma, p_c, sigma_dev, C, A, s, steps_dev, 0, consts_host, csa_squared,
+                                    decompose_C_freq, stdev_min, stdev_max, nullptr, nullptr, nullptr, stream);
+}
+
+extern "C" EVOK_API int evok_sepcma_update_batched_tiered(const float* local_disp, const float* S2, const float* wsum, int64_t n_items, int64_t D,
+                                                          float* m, float* p_sigma, float* p_c, float* sigma_dev, float* C, float* A, float* s,
+                                                          int64_t* steps_dev, const int32_t* tier, const float* consts_dev,
+                                                          const int64_t* decompose_C_freq_dev, int csa_squared, float stdev_min, float stdev_max,
+                                                          void* stream) {
+  if (!steps_dev || !tier) return EVOK_E_NULLPTR;
+  return sepcma_update_items<true>(local_disp, S2, wsum, n_items, D, m, p_sigma, p_c, sigma_dev, C, A, s, steps_dev, 0, nullptr, csa_squared, 1,
+                                   stdev_min, stdev_max, tier, consts_dev, decompose_C_freq_dev, stream);
 }

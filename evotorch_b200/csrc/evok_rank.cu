@@ -335,16 +335,9 @@ constexpr int kSmallRankMax = 8192;
 constexpr int kSmallThreads = 256;
 constexpr int kSmallTile = 2048;
 
+// the stable position of key i among the first N keys of f (PARTS lanes per element, reduced over them)
 template <int PARTS>
-__global__ void __launch_bounds__(kSmallThreads) rank_small_kernel(const float* __restrict__ f, int N, int descending, Emit e) {
-  __shared__ uint32_t tile[kSmallTile];
-  __shared__ double red[33];
-  constexpr int kElems = kSmallThreads / PARTS;
-  // batched searches: blockIdx.y = batch item, every item ranks its own N fitnesses
-  f += (int64_t)blockIdx.y * N;
-  e = e.item((int64_t)blockIdx.y * N);
-  const int part = threadIdx.x % PARTS;
-  const int i = blockIdx.x * kElems + threadIdx.x / PARTS;
+__device__ __forceinline__ uint32_t counting_rank(const float* __restrict__ f, int N, int i, int part, int descending, uint32_t* tile) {
   const uint32_t ki = i < N ? sort_key(f[i], descending) : 0u;
   uint32_t cnt = 0;
   for (int base = 0; base < N; base += kSmallTile) {
@@ -363,6 +356,20 @@ __global__ void __launch_bounds__(kSmallThreads) rank_small_kernel(const float* 
   }
 #pragma unroll
   for (int o = 1; o < PARTS; o <<= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+  return cnt;
+}
+
+template <int PARTS>
+__global__ void __launch_bounds__(kSmallThreads) rank_small_kernel(const float* __restrict__ f, int N, int descending, Emit e) {
+  __shared__ uint32_t tile[kSmallTile];
+  __shared__ double red[33];
+  constexpr int kElems = kSmallThreads / PARTS;
+  // batched searches: blockIdx.y = batch item, every item ranks its own N fitnesses
+  f += (int64_t)blockIdx.y * N;
+  e = e.item((int64_t)blockIdx.y * N);
+  const int part = threadIdx.x % PARTS;
+  const int i = blockIdx.x * kElems + threadIdx.x / PARTS;
+  const uint32_t cnt = counting_rank<PARTS>(f, N, i, part, descending, tile);
 
   float nes_sum = 0.0f;
   if (e.mode == kUtilities && e.method == EVOK_RANK_NES)  // the table sum of nes_table_sum_kernel, once per CTA
@@ -382,6 +389,24 @@ static int rank_small(const float* f, int64_t N, int64_t n_items, int descending
   }
   EVOK_CHECK_LAUNCH();
   return 0;
+}
+
+// Tiered rank-table lookup (padded populations): item b (grid y) ranks its first n = counts[tier[b]] of N keys and writes
+// tables[tier[b]][its position] to them, 0 to its pad rows n..N-1.  The table row is read only at positions < n.
+template <int PARTS>
+__global__ void __launch_bounds__(kSmallThreads)
+    rank_table_tiered_kernel(const float* __restrict__ f, int N, int descending, const float* __restrict__ tables, const int* __restrict__ tier,
+                             const int* __restrict__ counts, float* __restrict__ out) {
+  __shared__ uint32_t tile[kSmallTile];
+  constexpr int kElems = kSmallThreads / PARTS;
+  f += (int64_t)blockIdx.y * N;
+  out += (int64_t)blockIdx.y * N;
+  const int k = tier[blockIdx.y];
+  const int n = min(counts[k], N);
+  const int part = threadIdx.x % PARTS;
+  const int i = blockIdx.x * kElems + threadIdx.x / PARTS;
+  const uint32_t cnt = counting_rank<PARTS>(f, n, i, part, descending, tile);
+  if (i < N && part == 0) out[i] = i < n ? tables[(int64_t)k * N + cnt] : 0.0f;
 }
 
 // ---- host side ------------------------------------------------------------------------------------
@@ -722,6 +747,29 @@ extern "C" EVOK_API int evok_rank_table_batched(const float* keys, int64_t N, in
   if (N < 0 || N >= (int64_t)1 << 32 || n_items < 0) return EVOK_E_BADSIZE;
   if (N == 0 || n_items == 0) return 0;
   return rank_rows(keys, N, n_items, descending, table_entries(table, out), ws, ws_bytes, (cudaStream_t)stream);
+}
+
+// n_items tiered rank-table lookups (padded populations of N rows): the counting rank of rank_small, one launch per item chunk
+extern "C" EVOK_API int evok_rank_table_batched_tiered(const float* keys, int64_t N, int64_t n_items, int descending, const float* tables,
+                                                       const int32_t* tier, const int32_t* counts, float* out, void* stream) {
+  if (!keys || !tables || !tier || !counts || !out) return EVOK_E_NULLPTR;
+  if (N < 0 || N > kSmallRankMax || n_items < 0) return EVOK_E_BADSIZE;
+  if (N == 0 || n_items == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  return for_item_chunks(n_items, kMaxGridY, [&](int64_t b0, int64_t nb) {
+    const float* f = keys + b0 * N;
+    const int* t = tier + b0;
+    float* o = out + b0 * N;
+    if (N <= 1024) {
+      rank_table_tiered_kernel<4><<<dim3((unsigned)((N + 63) / 64), (unsigned)nb), kSmallThreads, 0, st>>>(f, (int)N, descending, tables, t, counts, o);
+    } else if (N <= 4096) {
+      rank_table_tiered_kernel<8><<<dim3((unsigned)((N + 31) / 32), (unsigned)nb), kSmallThreads, 0, st>>>(f, (int)N, descending, tables, t, counts, o);
+    } else {
+      rank_table_tiered_kernel<16><<<dim3((unsigned)((N + 15) / 16), (unsigned)nb), kSmallThreads, 0, st>>>(f, (int)N, descending, tables, t, counts, o);
+    }
+    EVOK_CHECK_LAUNCH();
+    return 0;
+  });
 }
 
 extern "C" EVOK_API int evok_elite_mask_batched(const float* w, int64_t N, int64_t n_items, int64_t num_elites, float* mask, void* ws,

@@ -4,6 +4,8 @@
 //   cma_restart_kernel     one CTA per item: best of this generation, best ever, history, criteria, stop flags; for a restarted
 //                          item a uniform centre in [lb, ub], sigma0, zero paths, counter 0, empty history (separable: C = A = 1, s)
 //   cma_restart_eye_kernel full family only: C = A = I for the restarted items, grid-wide, masked by the flags
+// The tiered form (IPOP, padded populations) reads N and H of item b from its tier, moves a restarted item one tier up and
+// counts the evaluations of each item.
 #include "evok_common.cuh"
 
 namespace evok {
@@ -32,6 +34,12 @@ struct RestartArgs {
   const float *sigma0, *lb, *ub;
   int64_t item_stride_bounds;
   float tol_fun, tol_x, tol_x_up, max_condition, min_fitness_stdev, max_generations;  // NaN = off
+  // tiered only: item b uses the first tier_counts[tier[b]] of its n_rows rows and the first tier_history[tier[b]] of its H slots
+  int* tier;
+  const int* tier_counts;
+  const long long* tier_history;
+  int n_tiers;
+  long long* num_evaluations;
 };
 
 // the row that wins: finite, better under the sense, the lower index on ties; index -1 = none
@@ -63,15 +71,19 @@ struct FMax { __device__ float operator()(float a, float b) const { return fmaxf
 struct FMin { __device__ float operator()(float a, float b) const { return fminf(a, b); } };
 struct DSum { __device__ double operator()(double a, double b) const { return a + b; } };
 
+template <bool TIERED>
 __global__ void __launch_bounds__(kRestartThreads) cma_restart_kernel(const __grid_constant__ RestartArgs a) {
   __shared__ float smf[kRestartWarps + 1];
   __shared__ double smd[kRestartWarps + 1];
   __shared__ float s_best_v[kRestartWarps];
   __shared__ long long s_best_i[kRestartWarps];
   __shared__ int s_flags;
-  const int64_t b = blockIdx.x, D = a.D, N = a.n_rows, H = a.H;
+  const int64_t b = blockIdx.x, D = a.D;
+  const int tk = TIERED ? a.tier[b] : 0;
+  const int64_t N = TIERED ? min((int64_t)a.tier_counts[tk], a.n_rows) : a.n_rows;
+  const int64_t H = TIERED ? min((int64_t)a.tier_history[tk], a.H) : a.H;
   const bool maximize = a.maximize != 0;
-  const float* f = a.f + b * N;
+  const float* f = a.f + b * a.n_rows;
   const float old_best = a.best_f[b];  // read before the barriers below: thread 0 overwrites it
 
   // this generation's fitnesses: the best finite row, min, max, a non-finite one, the sum
@@ -140,7 +152,7 @@ __global__ void __launch_bounds__(kRestartThreads) cma_restart_kernel(const __gr
 
   // history: slot (g - 1) % H holds the best eval of the item's generation g (NaN: none was finite)
   const long long gen = a.item_steps[b];
-  float* hist = a.history + b * H;
+  float* hist = a.history + b * a.H;
   if (threadIdx.x == 0 && gen >= 1) hist[(gen - 1) % H] = bi >= 0 ? bv : NAN;
   __syncthreads();
   float hmn = INFINITY, hmx = -INFINITY;
@@ -196,6 +208,7 @@ __global__ void __launch_bounds__(kRestartThreads) cma_restart_kernel(const __gr
     if (nonfinite) flags |= 64;
     a.stop_flags[b] = flags;
     s_flags = flags;
+    if (TIERED) a.num_evaluations[b] += N;
   }
   __syncthreads();
   if (s_flags == 0) return;
@@ -226,8 +239,9 @@ __global__ void __launch_bounds__(kRestartThreads) cma_restart_kernel(const __gr
       a.s[b * D + j] = s0;
     }
   }
-  for (int64_t k = threadIdx.x; k < H; k += kRestartThreads) hist[k] = NAN;
+  for (int64_t k = threadIdx.x; k < a.H; k += kRestartThreads) hist[k] = NAN;
   if (threadIdx.x == 0) {
+    if (TIERED) a.tier[b] = min(tk + 1, a.n_tiers - 1);
     a.sigma[b] = s0;
     a.item_steps[b] = 0;
     a.num_restarts[b] += 1;
@@ -252,18 +266,22 @@ __global__ void __launch_bounds__(kEyeThreads) cma_restart_eye_kernel(const int*
 
 using namespace evok;
 
-extern "C" EVOK_API int evok_cma_restart_batched(int separable, const float* f, const float* X, int64_t item_stride_x, int64_t ldx, const float* m_draw,
-                                                 const float* s_draw, uint64_t draw_seed, int64_t n_items, int64_t n_rows, int64_t D, int maximize,
-                                                 int64_t* item_steps, float* m, float* sigma, float* p_sigma, float* p_c, float* C, float* A, float* s,
-                                                 float* history, int64_t H, float* best_x, float* best_f, int64_t* num_restarts, int32_t* stop_flags,
-                                                 const float* sigma0, const float* lb, const float* ub, int64_t item_stride_bounds,
-                                                 const float* thresholds_host, uint64_t seed, void* stream) {
+// the restart stage of evok_cma_restart_batched, or (TIERED) of evok_cma_restart_batched_tiered with the tier arrays
+template <bool TIERED>
+static int cma_restart_items(int separable, const float* f, const float* X, int64_t item_stride_x, int64_t ldx, const float* m_draw, const float* s_draw,
+                             uint64_t draw_seed, int64_t n_items, int64_t n_rows, int64_t D, int maximize, int64_t* item_steps, float* m, float* sigma,
+                             float* p_sigma, float* p_c, float* C, float* A, float* s, float* history, int64_t H, float* best_x, float* best_f,
+                             int64_t* num_restarts, int32_t* stop_flags, const float* sigma0, const float* lb, const float* ub,
+                             int64_t item_stride_bounds, const float* thresholds_host, uint64_t seed, int32_t* tier, const int32_t* tier_counts,
+                             const int64_t* tier_history, int64_t n_tiers, int64_t* num_evaluations, void* stream) {
   if (!f || !item_steps || !m || !sigma || !p_sigma || !p_c || !C || !A || !history || !best_x || !best_f || !num_restarts || !stop_flags || !sigma0 ||
       !lb || !ub || !thresholds_host)
     return EVOK_E_NULLPTR;
   if (separable ? (!s || (!X && (!m_draw || !s_draw))) : !X) return EVOK_E_NULLPTR;
+  if (TIERED && (!tier || !tier_counts || !tier_history || !num_evaluations)) return EVOK_E_NULLPTR;
   if (n_items < 0 || n_rows <= 0 || D <= 0 || H <= 0 || (X && (ldx < D || item_stride_x < 0)) || (item_stride_bounds != 0 && item_stride_bounds != D))
     return EVOK_E_BADSIZE;
+  if (TIERED && (n_tiers < 1 || n_tiers > INT32_MAX)) return EVOK_E_BADSIZE;
   if (n_items == 0) return 0;
   RestartArgs a;
   a.f = f; a.X = X; a.item_stride_x = item_stride_x; a.ldx = ldx; a.m_draw = m_draw; a.s_draw = s_draw;
@@ -277,6 +295,8 @@ extern "C" EVOK_API int evok_cma_restart_batched(int separable, const float* f, 
   a.sigma0 = sigma0; a.lb = lb; a.ub = ub; a.item_stride_bounds = item_stride_bounds;
   a.tol_fun = thresholds_host[0]; a.tol_x = thresholds_host[1]; a.tol_x_up = thresholds_host[2]; a.max_condition = thresholds_host[3];
   a.min_fitness_stdev = thresholds_host[4]; a.max_generations = thresholds_host[5];
+  a.tier = tier; a.tier_counts = tier_counts; a.tier_history = reinterpret_cast<const long long*>(tier_history); a.n_tiers = (int)n_tiers;
+  a.num_evaluations = reinterpret_cast<long long*>(num_evaluations);
   const int rc = for_item_chunks(n_items, (int64_t)INT32_MAX, [&](int64_t b0, int64_t nb) {
     RestartArgs c = a;
     const int64_t mat = separable ? D : D * D;
@@ -289,7 +309,8 @@ extern "C" EVOK_API int evok_cma_restart_batched(int separable, const float* f, 
     if (c.s) c.s += b0 * D;
     c.history += b0 * H; c.best_x += b0 * D; c.best_f += b0; c.num_restarts += b0; c.stop_flags += b0; c.sigma0 += b0;
     c.lb += b0 * item_stride_bounds; c.ub += b0 * item_stride_bounds;
-    cma_restart_kernel<<<(unsigned)nb, kRestartThreads, 0, (cudaStream_t)stream>>>(c);
+    if (TIERED) { c.tier += b0; c.num_evaluations += b0; }
+    cma_restart_kernel<TIERED><<<(unsigned)nb, kRestartThreads, 0, (cudaStream_t)stream>>>(c);
     EVOK_CHECK_LAUNCH();
     return 0;
   });
@@ -301,4 +322,28 @@ extern "C" EVOK_API int evok_cma_restart_batched(int separable, const float* f, 
     EVOK_CHECK_LAUNCH();
     return 0;
   });
+}
+
+extern "C" EVOK_API int evok_cma_restart_batched(int separable, const float* f, const float* X, int64_t item_stride_x, int64_t ldx, const float* m_draw,
+                                                 const float* s_draw, uint64_t draw_seed, int64_t n_items, int64_t n_rows, int64_t D, int maximize,
+                                                 int64_t* item_steps, float* m, float* sigma, float* p_sigma, float* p_c, float* C, float* A, float* s,
+                                                 float* history, int64_t H, float* best_x, float* best_f, int64_t* num_restarts, int32_t* stop_flags,
+                                                 const float* sigma0, const float* lb, const float* ub, int64_t item_stride_bounds,
+                                                 const float* thresholds_host, uint64_t seed, void* stream) {
+  return cma_restart_items<false>(separable, f, X, item_stride_x, ldx, m_draw, s_draw, draw_seed, n_items, n_rows, D, maximize, item_steps, m, sigma,
+                                  p_sigma, p_c, C, A, s, history, H, best_x, best_f, num_restarts, stop_flags, sigma0, lb, ub, item_stride_bounds,
+                                  thresholds_host, seed, nullptr, nullptr, nullptr, 0, nullptr, stream);
+}
+
+extern "C" EVOK_API int evok_cma_restart_batched_tiered(int separable, const float* f, const float* X, int64_t item_stride_x, int64_t ldx,
+                                                        const float* m_draw, const float* s_draw, uint64_t draw_seed, int64_t n_items, int64_t n_rows,
+                                                        int64_t D, int maximize, int64_t* item_steps, float* m, float* sigma, float* p_sigma, float* p_c,
+                                                        float* C, float* A, float* s, float* history, int64_t H, float* best_x, float* best_f,
+                                                        int64_t* num_restarts, int32_t* stop_flags, const float* sigma0, const float* lb, const float* ub,
+                                                        int64_t item_stride_bounds, const float* thresholds_host, uint64_t seed, int32_t* tier,
+                                                        const int32_t* tier_counts, const int64_t* tier_history, int64_t n_tiers,
+                                                        int64_t* num_evaluations, void* stream) {
+  return cma_restart_items<true>(separable, f, X, item_stride_x, ldx, m_draw, s_draw, draw_seed, n_items, n_rows, D, maximize, item_steps, m, sigma,
+                                 p_sigma, p_c, C, A, s, history, H, best_x, best_f, num_restarts, stop_flags, sigma0, lb, ub, item_stride_bounds,
+                                 thresholds_host, seed, tier, tier_counts, tier_history, n_tiers, num_evaluations, stream);
 }

@@ -1001,28 +1001,59 @@ def weighted_syrk_update_batched(Y: torch.Tensor, w: torch.Tensor, k: torch.Tens
     return gemm_nt_affine_batched(a_w[:, :, :n], a_p[:, :, :n], k, out, E=C, u=u)
 
 
-def rank_table_batched(keys: torch.Tensor, descending: bool, table: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """`rank_table` for every row of keys (items, N) with one shared table (N,)."""
+def _tiers(tier: torch.Tensor, B: int, table: Optional[torch.Tensor] = None, name: str = "", dtype=None) -> int:
+    """Checks the per-item tier indices of a padded-population stage, int32 (items,), and a device table indexed by tier (its
+    first dimension, the number of tiers, is returned)."""
+    if not (tier.is_cuda and tier.dtype == torch.int32 and tier.is_contiguous() and tuple(tier.shape) == (B,)):
+        raise ValueError(f"tier: expected a contiguous int32 CUDA tensor of shape ({B},)")
+    if table is None:
+        return 0
+    if not (table.is_cuda and table.dtype == dtype and table.is_contiguous() and table.ndim >= 1 and table.device == tier.device):
+        raise ValueError(f"{name}: expected a contiguous {dtype} CUDA tensor indexed by tier, got {tuple(table.shape)} {table.dtype}")
+    return table.shape[0]
+
+
+def rank_table_batched(keys: torch.Tensor, descending: bool, table: torch.Tensor, out: Optional[torch.Tensor] = None, *,
+                       tier: Optional[torch.Tensor] = None, counts: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """`rank_table` for every row of keys (items, N) with one shared table (N,).  With `tier` (int32 (items,)), the padded form:
+    `table` is (K, N), `counts` int32 (K,) with 1 <= counts[k] <= N, and item b ranks its first counts[tier[b]] keys with table
+    row tier[b] and gets 0 on the rest (its pad rows); counting rank only, N <= 8192."""
     if not (keys.is_cuda and keys.dtype == torch.float32 and keys.ndim == 2):
         raise ValueError("keys: expected a float32 CUDA tensor of shape (items, N)")
     keys = as_plain_tensor(keys).contiguous()
     B, n = keys.shape
-    _vec(table, "table", n)
     out = torch.empty_like(keys) if out is None else _rows(out, "out", (B, n))
-    _rank_call("evok_rank_table_batched", keys, keys.data_ptr(), n, B, int(bool(descending)), table.data_ptr(), out.data_ptr())
+    if tier is None:
+        _vec(table, "table", n)
+        _rank_call("evok_rank_table_batched", keys, keys.data_ptr(), n, B, int(bool(descending)), table.data_ptr(), out.data_ptr())
+        return out
+    K = _tiers(tier, B, counts, "counts", torch.int32)
+    if not (table.is_cuda and table.dtype == torch.float32 and table.is_contiguous() and tuple(table.shape) == (K, n)):
+        raise ValueError(f"table: expected a contiguous float32 CUDA tensor of shape {(K, n)}")
+    with _timed("rank"):
+        rc = nat.lib().evok_rank_table_batched_tiered(keys.data_ptr(), n, B, int(bool(descending)), table.data_ptr(), tier.data_ptr(), counts.data_ptr(),
+                                                      out.data_ptr(), nat.stream_of(keys))
+    nat.check(rc, "evok_rank_table_batched_tiered")
     return out
 
 
-def cmaes_row_weights_batched(assigned: torch.Tensor, Z: torch.Tensor, active: bool, w_pos: torch.Tensor, w_act: torch.Tensor) -> None:
-    """`cmaes_row_weights` for every item: assigned, w_pos, w_act (items, N); Z (items, N, D) with row-major rows."""
+def cmaes_row_weights_batched(assigned: torch.Tensor, Z: torch.Tensor, active: bool, w_pos: torch.Tensor, w_act: torch.Tensor, *,
+                              tier: Optional[torch.Tensor] = None, counts: Optional[torch.Tensor] = None) -> None:
+    """`cmaes_row_weights` for every item: assigned, w_pos, w_act (items, N); Z (items, N, D) with row-major rows.  With `tier`
+    (int32 (items,)) and `counts` (int32 (K,)), item b uses its first counts[tier[b]] rows and gets 0 weights on the rest."""
     Z, nz, sz, ldz = _item_mat(Z, "Z", tuple(Z.shape[-2:]))
     if nz is None:
         raise ValueError("Z: expected shape (items, N, D)")
     B, n, d = Z.shape
     for t, name in ((assigned, "assigned"), (w_pos, "w_pos"), (w_act, "w_act")):
         _rows(t, name, (B, n))
-    nat.check(nat.lib().evok_cmaes_row_weights_batched(assigned.data_ptr(), Z.data_ptr(), sz, ldz, B, n, d, int(bool(active)), w_pos.data_ptr(),
-                                                       w_act.data_ptr(), nat.stream_of(Z)), "evok_cmaes_row_weights_batched")
+    head = (assigned.data_ptr(), Z.data_ptr(), sz, ldz, B, n, d, int(bool(active)))
+    if tier is None:
+        nat.check(nat.lib().evok_cmaes_row_weights_batched(*head, w_pos.data_ptr(), w_act.data_ptr(), nat.stream_of(Z)), "evok_cmaes_row_weights_batched")
+        return
+    _tiers(tier, B, counts, "counts", torch.int32)
+    nat.check(nat.lib().evok_cmaes_row_weights_batched_tiered(*head, tier.data_ptr(), counts.data_ptr(), w_pos.data_ptr(), w_act.data_ptr(),
+                                                              nat.stream_of(Z)), "evok_cmaes_row_weights_batched_tiered")
 
 
 def sepcma_moments_batched(X: Optional[torch.Tensor], m: torch.Tensor, s: torch.Tensor, aw: torch.Tensor, active: bool, *, seed: int = 0,
@@ -1064,21 +1095,37 @@ def _item_steps(steps, B: int) -> Optional[torch.Tensor]:
 
 def sepcma_update_batched(local: torch.Tensor, S2: torch.Tensor, wsum: torch.Tensor, m: torch.Tensor, p_sigma: torch.Tensor, p_c: torch.Tensor,
                           sigma: torch.Tensor, C: torch.Tensor, A: torch.Tensor, s: torch.Tensor, consts, csa_squared: bool, *, steps,
-                          decompose_C_freq: int, stdev_min: Optional[float] = None, stdev_max: Optional[float] = None) -> None:
+                          decompose_C_freq, stdev_min: Optional[float] = None, stdev_max: Optional[float] = None,
+                          tier: Optional[torch.Tensor] = None) -> None:
     """`sepcma_update` for every item, one CTA each, in place: m, p_sigma, p_c, C, A, s, local, S2 (items, D), sigma, wsum (items,).
     The 10 constants, `decompose_C_freq` and the stdev bounds are shared.  `steps`: the generation counter, an int shared by every
     item, or an int64 CUDA tensor (items,) of per-item counters that drive each item's h_sig and decomposition schedule and are
-    incremented in place."""
+    incremented in place.  With `tier` (int32 (items,), per-item counters), `consts` is a float32 CUDA table (K, 10) and
+    `decompose_C_freq` an int64 CUDA table (K,), both read at row tier[b] for item b."""
     B, d = m.shape
     for t, name in ((local, "local"), (S2, "S2"), (m, "m"), (p_sigma, "p_sigma"), (p_c, "p_c"), (C, "C"), (A, "A"), (s, "s")):
         _rows(t, name, (B, d))
     for t, name in ((sigma, "sigma"), (wsum, "wsum")):
         _rows(t, name, (B,))
+    lo = NAN if stdev_min is None else float(stdev_min)
+    hi = NAN if stdev_max is None else float(stdev_max)
+    if tier is not None:
+        steps_dev = _item_steps(steps, B)
+        if steps_dev is None:
+            raise ValueError("steps: the tiered update takes per-item counters")
+        K = _tiers(tier, B, consts, "consts", torch.float32)
+        if tuple(consts.shape) != (K, 10) or _tiers(tier, B, decompose_C_freq, "decompose_C_freq", torch.int64) != K or decompose_C_freq.ndim != 1:
+            raise ValueError(f"consts, decompose_C_freq: expected tables of shapes ({K}, 10) and ({K},)")
+        with _timed("sepcma_update"):
+            rc = nat.lib().evok_sepcma_update_batched_tiered(local.data_ptr(), S2.data_ptr(), wsum.data_ptr(), B, d, m.data_ptr(), p_sigma.data_ptr(),
+                                                             p_c.data_ptr(), sigma.data_ptr(), C.data_ptr(), A.data_ptr(), s.data_ptr(), steps_dev.data_ptr(),
+                                                             tier.data_ptr(), consts.data_ptr(), decompose_C_freq.data_ptr(), int(bool(csa_squared)), lo, hi,
+                                                             nat.stream_of(m))
+        nat.check(rc, "evok_sepcma_update_batched_tiered")
+        return
     if int(decompose_C_freq) < 1:
         raise ValueError("decompose_C_freq: expected a positive integer")
     steps_dev = _item_steps(steps, B)
-    lo = NAN if stdev_min is None else float(stdev_min)
-    hi = NAN if stdev_max is None else float(stdev_max)
     lib = nat.lib()
     head = (local.data_ptr(), S2.data_ptr(), wsum.data_ptr(), B, d, m.data_ptr(), p_sigma.data_ptr(), p_c.data_ptr(), sigma.data_ptr(), C.data_ptr(),
             A.data_ptr(), s.data_ptr())
@@ -1092,10 +1139,12 @@ def sepcma_update_batched(local: torch.Tensor, S2: torch.Tensor, wsum: torch.Ten
 
 
 def cmaes_vector_update_batched(local_disp: torch.Tensor, shaped_disp: torch.Tensor, m: torch.Tensor, p_sigma: torch.Tensor, p_c: torch.Tensor,
-                                sigma: torch.Tensor, consts, csa_squared: bool, k_out: torch.Tensor, *, steps) -> None:
+                                sigma: torch.Tensor, consts, csa_squared: bool, k_out: torch.Tensor, *, steps,
+                                tier: Optional[torch.Tensor] = None) -> None:
     """`cmaes_vector_update` for every item, one CTA each, in place: m, p_sigma, p_c, local / shaped (items, D), sigma (items,),
     k_out (items, 3).  The 10 constants are shared.  `steps`: the generation counter, an int shared by every item, or an int64
-    CUDA tensor (items,) of per-item counters that drive each item's h_sig and are incremented in place."""
+    CUDA tensor (items,) of per-item counters that drive each item's h_sig and are incremented in place.  With `tier` (int32
+    (items,), per-item counters), `consts` is a float32 CUDA table (K, 10) read at row tier[b] for item b."""
     B, d = m.shape
     for t, name in ((local_disp, "local_disp"), (shaped_disp, "shaped_disp"), (m, "m"), (p_sigma, "p_sigma"), (p_c, "p_c")):
         _rows(t, name, (B, d))
@@ -1104,6 +1153,15 @@ def cmaes_vector_update_batched(local_disp: torch.Tensor, shaped_disp: torch.Ten
     steps_dev = _item_steps(steps, B)
     lib = nat.lib()
     head = (local_disp.data_ptr(), shaped_disp.data_ptr(), B, d, m.data_ptr(), p_sigma.data_ptr(), p_c.data_ptr(), sigma.data_ptr())
+    if tier is not None:
+        if steps_dev is None:
+            raise ValueError("steps: the tiered update takes per-item counters")
+        K = _tiers(tier, B, consts, "consts", torch.float32)
+        if tuple(consts.shape) != (K, 10):
+            raise ValueError(f"consts: expected a table of shape ({K}, 10)")
+        nat.check(lib.evok_cmaes_vector_update_batched_tiered(*head, steps_dev.data_ptr(), tier.data_ptr(), consts.data_ptr(), int(bool(csa_squared)),
+                                                              k_out.data_ptr(), nat.stream_of(m)), "evok_cmaes_vector_update_batched_tiered")
+        return
     tail = (_host_floats(consts, 10), int(bool(csa_squared)), k_out.data_ptr(), nat.stream_of(m))
     if steps_dev is None:
         nat.check(lib.evok_cmaes_vector_update_batched(*head, int(steps), *tail), "evok_cmaes_vector_update_batched")
@@ -1118,13 +1176,17 @@ def cma_restart_batched(separable: bool, f: torch.Tensor, X: Optional[torch.Tens
                         sigma: torch.Tensor, p_sigma: torch.Tensor, p_c: torch.Tensor, C: torch.Tensor, A: torch.Tensor, s: Optional[torch.Tensor],
                         history: torch.Tensor, best_x: torch.Tensor, best_f: torch.Tensor, num_restarts: torch.Tensor, stop_flags: torch.Tensor,
                         sigma0: torch.Tensor, lb: torch.Tensor, ub: torch.Tensor, thresholds, *, seed: int, m_draw: Optional[torch.Tensor] = None,
-                        s_draw: Optional[torch.Tensor] = None, draw_seed: int = 0) -> None:
+                        s_draw: Optional[torch.Tensor] = None, draw_seed: int = 0, tier: Optional[torch.Tensor] = None,
+                        tier_counts: Optional[torch.Tensor] = None, tier_history: Optional[torch.Tensor] = None,
+                        num_evaluations: Optional[torch.Tensor] = None) -> None:
     """The restart stage of every item after its update, in place (include/evok.h, evok_cma_restart_batched): best ever, history,
     stop flags and the re-initialisation of the items that met a criterion.  f (items, N); X (items, N, D), or None for a separable
     population rebuilt from (draw_seed, stream b) with m_draw / s_draw (items, D); item_steps, num_restarts int64 (items,); m, p_sigma,
     p_c, best_x, lb, ub (items, D); C, A (items, D, D), separable (items, D) with s; sigma, sigma0, best_f (items,); history
     (items, H); stop_flags int32 (items,); `thresholds` the 6 criteria of RESTART_CRITERIA, None = off; `seed` the Philox key of
-    the new centres."""
+    the new centres.  With `tier` (int32 (items,), in place), the padded form (evok_cma_restart_batched_tiered): item b uses its
+    first tier_counts[tier[b]] values and tier_history[tier[b]] history slots (tables int32 and int64 (K,)), num_evaluations
+    (int64 (items,)) grows by its count, and a restarted item moves one tier up."""
     B, n = f.shape
     d = m.shape[-1]
     f = _rows(f, "f", (B, n))
@@ -1153,10 +1215,22 @@ def cma_restart_batched(separable: bool, f: torch.Tensor, X: Optional[torch.Tens
     else:
         m_draw, s_draw = _rows(m_draw, "m_draw", (B, d)), _rows(s_draw, "s_draw", (B, d))
     th = [NAN if t is None else float(t) for t in thresholds]
+    if tier is not None:
+        K = _tiers(tier, B, tier_counts, "tier_counts", torch.int32)
+        if _tiers(tier, B, tier_history, "tier_history", torch.int64) != K:
+            raise ValueError("tier_counts and tier_history must have one entry per tier")
+        if not (num_evaluations is not None and num_evaluations.is_cuda and num_evaluations.dtype == torch.int64 and num_evaluations.is_contiguous()
+                and tuple(num_evaluations.shape) == (B,)):
+            raise ValueError(f"num_evaluations: expected a contiguous int64 CUDA tensor of shape ({B},)")
     with _timed("cma_restart"):
-        rc = nat.lib().evok_cma_restart_batched(int(bool(separable)), f.data_ptr(), nat.ptr(X), n * d, d, nat.ptr(m_draw), nat.ptr(s_draw), int(draw_seed),
-                                                B, n, d, int(bool(maximize)), item_steps.data_ptr(), m.data_ptr(), sigma.data_ptr(), p_sigma.data_ptr(),
-                                                p_c.data_ptr(), C.data_ptr(), A.data_ptr(), nat.ptr(s), history.data_ptr(), history.shape[1],
-                                                best_x.data_ptr(), best_f.data_ptr(), num_restarts.data_ptr(), stop_flags.data_ptr(), sigma0.data_ptr(),
-                                                lb.data_ptr(), ub.data_ptr(), d, _host_floats(th, 6), int(seed), nat.stream_of(f))
+        args = (int(bool(separable)), f.data_ptr(), nat.ptr(X), n * d, d, nat.ptr(m_draw), nat.ptr(s_draw), int(draw_seed), B, n, d, int(bool(maximize)),
+                item_steps.data_ptr(), m.data_ptr(), sigma.data_ptr(), p_sigma.data_ptr(), p_c.data_ptr(), C.data_ptr(), A.data_ptr(), nat.ptr(s),
+                history.data_ptr(), history.shape[1], best_x.data_ptr(), best_f.data_ptr(), num_restarts.data_ptr(), stop_flags.data_ptr(),
+                sigma0.data_ptr(), lb.data_ptr(), ub.data_ptr(), d, _host_floats(th, 6), int(seed))
+        if tier is not None:
+            rc = nat.lib().evok_cma_restart_batched_tiered(*args, tier.data_ptr(), tier_counts.data_ptr(), tier_history.data_ptr(), K,
+                                                           num_evaluations.data_ptr(), nat.stream_of(f))
+            nat.check(rc, "evok_cma_restart_batched_tiered")
+            return
+        rc = nat.lib().evok_cma_restart_batched(*args, nat.stream_of(f))
     nat.check(rc, "evok_cma_restart_batched")

@@ -599,6 +599,50 @@ int evok_cma_restart_batched(int separable, const float* f, const float* X, int6
                              float* best_x, float* best_f, int64_t* num_restarts, int32_t* stop_flags, const float* sigma0, const float* lb,
                              const float* ub, int64_t item_stride_bounds, const float* thresholds_host, uint64_t seed, void* stream);
 
+/* IPOP restarts (padded populations): every item draws N = max_popsize rows, and item b uses only its first n_b rows, n_b =
+ * counts[tier[b]] of a ladder of population sizes, with the constants of its tier.  tier [items] int32 and the tables (counts [K]
+ * int32 with 1 <= counts[k] <= N, tables [K][N], consts_dev [K][10], decompose_C_freq_dev [K] int64 >= 1, tier_history [K] int64
+ * with 1 <= tier_history[k] <= H) are device memory; nothing is read back.  Rows n_b..N-1 of item b are pad rows: whatever their
+ * keys, values or Z hold (NaN and inf included), they reach no output but their own zero weights.
+ *   evok_rank_table_batched_tiered: item b ranks its first n_b keys (the counting rank of evok_rank_table_batched, stable, NaN the
+ *       largest) and writes tables[tier[b]][position] to them, 0 to its pad rows; an item with n_b = N gets the bits of
+ *       evok_rank_table_batched with table row tier[b].  No workspace.  Errors: EVOK_E_NULLPTR, EVOK_E_BADSIZE (N < 0, N > 8192,
+ *       n_items < 0).  Grid y = item, chunks of 65535 items.
+ *   evok_cmaes_row_weights_batched_tiered: evok_cmaes_row_weights_batched on the first n_b rows of item b, w_positive = w_active =
+ *       0 on its pad rows.  Errors: EVOK_E_NULLPTR (tier, counts first), then those of evok_cmaes_row_weights_batched.
+ *   evok_cmaes_vector_update_batched_tiered: evok_cmaes_vector_update_batched_steps with item b's constants read from row tier[b]
+ *       of consts_dev (the 10 floats of consts_host; its weights_sum enters k_out).  Errors: EVOK_E_NULLPTR (steps_dev, tier,
+ *       consts_dev and the state), EVOK_E_BADSIZE (n_items < 0, D <= 0).
+ *   evok_sepcma_update_batched_tiered: evok_sepcma_update_batched_steps with item b's constants from row tier[b] of consts_dev and
+ *       its decomposition schedule (steps_dev[b] + 1) % decompose_C_freq_dev[tier[b]] == 0.  Errors: EVOK_E_NULLPTR (steps_dev,
+ *       tier, consts_dev, decompose_C_freq_dev and the state), EVOK_E_BADSIZE (n_items < 0, D <= 0).
+ *   evok_cma_restart_batched_tiered: evok_cma_restart_batched (n_rows = N, H the ring length of every history row) with, for
+ *       item b, N = counts[tier[b]] (tier_counts) and H = tier_history[tier[b]]: the best row, the history slot (g - 1) % H, the
+ *       tol_fun and min_fitness_stdev criteria use only the first N values or rows and the first H slots (a lazy separable row
+ *       is rebuilt only for the best of those N).  Then num_evaluations[b] (int64) += N, and a restarted item moves to tier
+ *       min(tier[b] + 1, n_tiers - 1) and has its whole history row set to NaN.  Errors: those of evok_cma_restart_batched in its
+ *       order, with EVOK_E_NULLPTR also for tier, tier_counts, tier_history and num_evaluations, and EVOK_E_BADSIZE also for
+ *       n_tiers < 1. */
+int evok_rank_table_batched_tiered(const float* keys, int64_t N, int64_t n_items, int descending, const float* tables, const int32_t* tier,
+                                   const int32_t* counts, float* out, void* stream);
+int evok_cmaes_row_weights_batched_tiered(const float* assigned_weights, const float* Z, int64_t item_stride_z, int64_t ldz, int64_t n_items,
+                                          int64_t N, int64_t D, int active, const int32_t* tier, const int32_t* counts, float* w_positive,
+                                          float* w_active, void* stream);
+int evok_cmaes_vector_update_batched_tiered(const float* local_disp, const float* shaped_disp, int64_t n_items, int64_t D, float* m,
+                                            float* p_sigma, float* p_c, float* sigma_dev, int64_t* steps_dev, const int32_t* tier,
+                                            const float* consts_dev, int csa_squared, float* k_out, void* stream);
+int evok_sepcma_update_batched_tiered(const float* local, const float* S2, const float* wsum, int64_t n_items, int64_t D, float* m, float* p_sigma,
+                                      float* p_c, float* sigma_dev, float* C, float* A, float* s, int64_t* steps_dev, const int32_t* tier,
+                                      const float* consts_dev, const int64_t* decompose_C_freq_dev, int csa_squared, float stdev_min,
+                                      float stdev_max, void* stream);
+int evok_cma_restart_batched_tiered(int separable, const float* f, const float* X, int64_t item_stride_x, int64_t ldx, const float* m_draw,
+                                    const float* s_draw, uint64_t draw_seed, int64_t n_items, int64_t n_rows, int64_t D, int maximize,
+                                    int64_t* item_steps, float* m, float* sigma, float* p_sigma, float* p_c, float* C, float* A, float* s,
+                                    float* history, int64_t H, float* best_x, float* best_f, int64_t* num_restarts, int32_t* stop_flags,
+                                    const float* sigma0, const float* lb, const float* ub, int64_t item_stride_bounds,
+                                    const float* thresholds_host, uint64_t seed, int32_t* tier, const int32_t* tier_counts,
+                                    const int64_t* tier_history, int64_t n_tiers, int64_t* num_evaluations, void* stream);
+
 /* Cholesky factorisation A = L L^T (fp32, lower; the strictly upper part of L is zeroed, like torch.linalg.cholesky).  Replaces
  * CMAES.decompose_C (cmaes.py:555-565, torch.linalg.cholesky -> cuSOLVER potrf).  ONE persistent kernel: 64 x 64 tiles, left-looking
  * tile dataflow with per-tile release / acquire flags instead of a launch (or grid barrier) per panel step.  Only the lower triangle
