@@ -119,6 +119,9 @@ _SIGNATURES = {
     "evok_cma_restart_batched_tiered": (c_int, [c_int, _P, _P, c_int64, c_int64, _P, _P, c_uint64, c_int64, c_int64, c_int64, c_int, _P, _P, _P, _P,
                                                 _P, _P, _P, _P, _P, c_int64, _P, _P, _P, _P, _P, _P, _P, c_int64, _P, c_uint64, _P, _P, _P, c_int64,
                                                 _P, _P]),
+    "evok_cma_restart_batched_bipop": (c_int, [c_int, _P, _P, c_int64, c_int64, _P, _P, c_uint64, c_int64, c_int64, c_int64, c_int, _P, _P, _P, _P,
+                                               _P, _P, _P, _P, _P, c_int64, _P, _P, _P, _P, _P, _P, _P, c_int64, _P, c_uint64, _P, _P, _P, c_int64,
+                                               _P, _P, _P, _P, _P, _P, _P, c_int64, c_int64, _P]),
     "evok_peer_alloc": (c_int, [c_size_t, _P, _P]),
     "evok_peer_open": (c_int, [_P, _P]),
     "evok_peer_close": (c_int, [_P]),

@@ -34,7 +34,8 @@ re-initialisation on the device, each item with its own generation counter:
     rs = restarts_tell(rs, values, evals)                # rs.best_values, rs.best_evals, rs.num_restarts, rs.stop_flags
 
 With `restarts(state, ..., popsize_multiplier=2, max_popsize=640)` every restart of an item doubles its population size (IPOP):
-the ask draws 640 rows per item and item b uses its first `rs.popsize[b]`.
+the ask draws 640 rows per item and item b uses its first `rs.popsize[b]`.  With `bipop=True` as well, restarts alternate between
+that ladder and small runs of random population size and step size, each regime given a similar share of the evaluations (BIPOP).
 """
 
 from .funcadam import AdamState, adam, adam_ask, adam_tell
@@ -42,7 +43,7 @@ from .funccem import CEMState, cem, cem_ask, cem_ask_and_evaluate, cem_tell
 from .funcclipup import ClipUpState, clipup, clipup_ask, clipup_tell
 from .funccmaes import CMAESState, cmaes, cmaes_ask, cmaes_ask_and_evaluate, cmaes_tell
 from .funcpgpe import PGPEState, pgpe, pgpe_ask, pgpe_ask_and_evaluate, pgpe_tell
-from .funcrestarts import IPOPLadder, RestartState, ipop_ladder, restarts, restarts_tell
+from .funcrestarts import IPOPLadder, RestartState, bipop_ladder, ipop_ladder, restarts, restarts_tell
 from .fused import LazyPopulation
 from .funcsepcmaes import SepCMAESState, sepcmaes, sepcmaes_ask, sepcmaes_ask_and_evaluate, sepcmaes_tell
 from .funcsgd import SGDState, sgd, sgd_ask, sgd_tell
@@ -50,6 +51,6 @@ from .misc import OptimizerFunctions, get_functional_optimizer
 
 __all__ = ["AdamState", "adam", "adam_ask", "adam_tell", "CEMState", "cem", "cem_ask", "cem_ask_and_evaluate", "cem_tell", "ClipUpState",
            "clipup", "clipup_ask", "clipup_tell", "CMAESState", "cmaes", "cmaes_ask", "cmaes_ask_and_evaluate", "cmaes_tell", "LazyPopulation", "PGPEState", "pgpe", "pgpe_ask", "pgpe_ask_and_evaluate", "pgpe_tell",
-           "IPOPLadder", "RestartState", "ipop_ladder", "restarts", "restarts_tell",
+           "IPOPLadder", "RestartState", "bipop_ladder", "ipop_ladder", "restarts", "restarts_tell",
            "SepCMAESState", "sepcmaes", "sepcmaes_ask", "sepcmaes_ask_and_evaluate", "sepcmaes_tell",
            "SGDState", "sgd", "sgd_ask", "sgd_tell", "OptimizerFunctions", "get_functional_optimizer"]

@@ -18,7 +18,8 @@ decompose_C_freq > 1 the full family then factors C of every item in every gener
 is not due, since which items are due is only known on the device.  Anywhere else the same algorithm runs as batched torch ops.
 
 `stop_flags` bits (ops.RESTART_CRITERIA): 0 tol_fun, 1 tol_x, 2 tol_x_up, 3 max_condition, 4 min_fitness_stdev, 5 max_generations,
-6 non-finite state (always on).
+6 non-finite state (always on), 7 small-run budget (BIPOP only, always on there: a small run has used half the evaluations of the
+item's latest large run).
 
 IPOP (Auger & Hansen, "A Restart CMA Evolution Strategy With Increasing Population Size", CEC 2005):
 `restarts(state, ..., popsize_multiplier=2, max_popsize=640)` multiplies an item's population size at each of its restarts, along
@@ -27,6 +28,14 @@ of each size.  Items restart at different times, so the populations are padded: 
 (`rs.search` has the top tier's popsize) and item b uses only its first `rs.popsize[b]` rows.  Its other rows are pad rows: their
 values and evals may hold anything, NaN and inf included, and never reach the state, the best ever, the history or the criteria.
 On the kernels the stages that depend on the population size read the item's tier from device tables: still no host reads.
+
+BIPOP (Hansen, "Benchmarking a BI-Population CMA-ES on the BBOB-2009 Function Testbed", GECCO 2009 workshops):
+`restarts(state, ..., popsize_multiplier=2, max_popsize=640, bipop=True)` interleaves two regimes per item.  Large runs climb IPOP's
+ladder with the default step size; small runs draw a population size lambda_s = floor(lambda_0 (lambda_l / (2 lambda_0))^(u1^2))
+(at least lambda_0; lambda_l the latest large run's) and a step size sigma_def 10^(-2 u2), and stop once they have used half the
+evaluations of the latest large run (bit 7).  At each restart the regime that has used fewer evaluations runs next, large on a tie
+(so the first restart is large); the first run counts in neither budget.  The tables hold the ladder's tiers and then one tier
+per population size lambda_0 .. max(lambda_0, max_popsize // 2), so the small tier of lambda is n_large + lambda - lambda_0.
 """
 
 from __future__ import annotations
@@ -58,6 +67,9 @@ class IPOPLadder(NamedTuple):
     weights: torch.Tensor  # (K, max_popsize): the weights of tier k, zero past lambda_k
     consts: torch.Tensor  # (K, 10): the update constants of tier k (funccmaes.CONST_NAMES)
     decompose_C_freq: torch.Tensor  # (K,) int64
+    # BIPOP (`bipop_ladder`): the number of ladder tiers; tiers n_large.. are the small runs' population sizes lambda_0, lambda_0 + 1,
+    # .., and `hyperparameters` holds the ladder tiers' only (the small tiers' constants are in the tables).  None for IPOP.
+    n_large: Optional[int] = None
 
 
 class RestartState(NamedTuple):
@@ -81,6 +93,13 @@ class RestartState(NamedTuple):
     tier: Optional[torch.Tensor] = None  # (...) int32: the item's rung of the ladder
     num_evaluations: Optional[torch.Tensor] = None  # (...) int64: the rows told to the item so far, lambda of its tier per tell
     ladder: Optional[IPOPLadder] = None
+    # BIPOP only (None otherwise)
+    regime: Optional[torch.Tensor] = None  # (...) int32: 0 the first run, 1 a large run, 2 a small run
+    large_tier: Optional[torch.Tensor] = None  # (...) int32: the ladder rung of the item's latest large run (0 before any)
+    large_evaluations: Optional[torch.Tensor] = None  # (...) int64: the rows told to the item in its large runs
+    small_evaluations: Optional[torch.Tensor] = None  # (...) int64: in its small runs
+    last_large_evaluations: Optional[torch.Tensor] = None  # (...) int64: in its latest large run (0 before one ended)
+    run_stdev: Optional[torch.Tensor] = None  # (...): the step size the item's current run started with
 
     @property
     def thresholds(self) -> tuple:
@@ -104,6 +123,20 @@ def _same_hyperparameters(a: CMAESHyperparameters, b: CMAESHyperparameters) -> b
     return all(torch.equal(x, y) if isinstance(x, torch.Tensor) else x == y for x, y in zip(a, b))
 
 
+def _make_hyperparameters(state: Union[CMAESState, SepCMAESState], limit: bool, device=None):
+    """lambda -> the default hyperparameters of `state`'s family at population size lambda (on `device`, by default the state's)."""
+    center = state.center
+    sep, d = isinstance(state, SepCMAESState), center.shape[-1]
+    dev = center.device if device is None else device
+    return lambda lam: cmaes_hyperparameters(d, lam, dtype=center.dtype, device=dev, active=state.active, separable=sep, limit_C_decomposition=limit)
+
+
+def _default_limit(state: Union[CMAESState, SepCMAESState]) -> Optional[bool]:
+    """The limit_C_decomposition flag under which `state` has the default constants of its population size (None: neither)."""
+    return next((lim for lim in (True, False) if _same_hyperparameters(_make_hyperparameters(state, lim)(state.popsize), state.hyperparameters)),
+                None)
+
+
 def ipop_ladder(state: Union[CMAESState, SepCMAESState], popsize_multiplier, max_popsize) -> IPOPLadder:
     """The IPOP ladder of `state` (see `restarts`).  Raises ValueError for a multiplier <= 1, a max_popsize below state.popsize, a
     step that does not grow, max_popsize > MAX_TIERED_POPSIZE on the kernels, and a state whose constants are not the defaults of
@@ -125,14 +158,13 @@ def ipop_ladder(state: Union[CMAESState, SepCMAESState], popsize_multiplier, max
     center = state.center
     if on_kernels(center) and cap > MAX_TIERED_POPSIZE:
         raise ValueError(f"`max_popsize` {cap} is above {MAX_TIERED_POPSIZE}, the largest padded population the kernels rank")
-    sep, d = isinstance(state, SepCMAESState), center.shape[-1]
-    make = lambda lam, limit: cmaes_hyperparameters(d, lam, dtype=center.dtype, device=center.device, active=state.active,  # noqa: E731
-                                                    separable=sep, limit_C_decomposition=limit)
-    limit = next((lim for lim in (True, False) if _same_hyperparameters(make(lam0, lim), state.hyperparameters)), None)
+    d = center.shape[-1]
+    limit = _default_limit(state)
     if limit is None:
         raise ValueError("IPOP uses the default learning rates of each population size: build the search with the default c_m and "
                          "learning-rate ratios")
-    hps = tuple(make(lam, limit) for lam in sizes)
+    make = _make_hyperparameters(state, limit)
+    hps = tuple(make(lam) for lam in sizes)
     K = len(sizes)
     weights = torch.zeros(K, cap, dtype=center.dtype, device=center.device)
     for k, hp in enumerate(hps):
@@ -145,9 +177,37 @@ def ipop_ladder(state: Union[CMAESState, SepCMAESState], popsize_multiplier, max
                       decompose_C_freq=torch.tensor([hp.decompose_C_freq for hp in hps], dtype=torch.int64, device=dev))
 
 
+def bipop_ladder(state: Union[CMAESState, SepCMAESState], popsize_multiplier, max_popsize) -> IPOPLadder:
+    """The tables of BIPOP restarts of `state` (see `restarts`): the IPOP ladder (`ipop_ladder`, whose checks apply), then one
+    small tier for every population size lambda_0 .. max(lambda_0, max_popsize // 2), with the default constants of that size.
+    The small tiers' constants are computed on the host and copied to the state's device once: at max_popsize 8192 from
+    lambda_0 = 10 the weight table has about 4100 x 8192 entries (134 MB in float32)."""
+    lad = ipop_ladder(state, popsize_multiplier, max_popsize)
+    lam0, cap, K = lad.popsizes[0], lad.popsizes[-1], len(lad.popsizes)
+    small = tuple(range(lam0, max(lam0, cap // 2) + 1))
+    center = state.center
+    d, dev = center.shape[-1], center.device
+    make = _make_hyperparameters(state, _default_limit(state), device="cpu")
+    weights = torch.zeros(K + len(small), cap, dtype=center.dtype)
+    weights[:K] = lad.weights.cpu()
+    consts, freq = [], []
+    for t, lam in enumerate(small):
+        hp = make(lam)
+        weights[K + t, :lam] = hp.weights
+        consts.append(funccmaes._consts(hp))
+        freq.append(hp.decompose_C_freq)
+    hist = tuple(history_length(d, lam) for lam in small)
+    return lad._replace(popsizes=lad.popsizes + small, history_lengths=lad.history_lengths + hist,
+                        counts=torch.cat([lad.counts, torch.tensor(small, dtype=torch.int32, device=dev)]),
+                        history=torch.cat([lad.history, torch.tensor(hist, dtype=torch.int64, device=dev)]), weights=weights.to(dev),
+                        consts=torch.cat([lad.consts, torch.tensor(consts, dtype=center.dtype).to(dev)]),
+                        decompose_C_freq=torch.cat([lad.decompose_C_freq, torch.tensor(freq, dtype=torch.int64, device=dev)]), n_large=K)
+
+
 def restarts(state: Union[CMAESState, SepCMAESState], *, lb, ub, tol_fun: Optional[float] = 1e-12, tol_x: Optional[float] = 1e-12,
              tol_x_up: Optional[float] = 1e4, max_condition: Optional[float] = 1e14, min_fitness_stdev: Optional[float] = None,
-             max_generations: Optional[int] = None, popsize_multiplier: Optional[float] = None, max_popsize: Optional[int] = None) -> RestartState:
+             max_generations: Optional[int] = None, popsize_multiplier: Optional[float] = None, max_popsize: Optional[int] = None,
+             bipop: bool = False) -> RestartState:
     """A restart state around `state` (a `CMAESState` or `SepCMAESState`).  `lb`, `ub`: the box the restarted centres are drawn
     from, scalars, (D,) or (..., D), finite with lb < ub.  A threshold of None turns its criterion off.  Every item's generation
     counter starts at `state.generation` and its restart step size is its current sigma.
@@ -157,7 +217,13 @@ def restarts(state: Union[CMAESState, SepCMAESState], *, lb, ub, tol_fun: Option
     lambda_k), max_popsize) (`ipop_ladder`), with the hyperparameters of `cmaes_hyperparameters` at that size.  `state` must have
     the default constants of its own size.  `rs.search` then asks for max_popsize rows per item (its popsize is the top tier's);
     item b uses the first `rs.popsize[b]` and ignores the others (pad rows, which may hold anything).  On the kernels
-    max_popsize is at most 8192."""
+    max_popsize is at most 8192.
+
+    BIPOP: with `bipop=True` as well (it needs `popsize_multiplier` and `max_popsize`, with the same checks), a restarted item runs
+    either a large run one rung up the ladder or a small run of random population size in [lambda_0, max_popsize // 2] and step
+    size in (sigma_def / 100, sigma_def] (sigma_def: the item's restart step size), whichever regime has used fewer evaluations
+    (`bipop_ladder`; the module's docstring has the rule).  tol_x and tol_x_up then compare against the step size the current run
+    started with (`rs.run_stdev`)."""
     if not isinstance(state, (CMAESState, SepCMAESState)):
         raise TypeError(f"`restarts` takes a CMAESState or a SepCMAESState, got {type(state).__name__}")
     center = state.center
@@ -179,12 +245,18 @@ def restarts(state: Union[CMAESState, SepCMAESState], *, lb, ub, tol_fun: Option
         th[name] = None if v is None else _host_float(v, name)
     maximize = state.maximize
     ladder = None
+    if bipop and (popsize_multiplier is None or max_popsize is None):
+        raise ValueError("BIPOP restarts climb an IPOP ladder in their large runs: give `popsize_multiplier` and `max_popsize` with `bipop`")
     if popsize_multiplier is not None or max_popsize is not None:
         if popsize_multiplier is None:
             raise ValueError("`max_popsize` is the cap of IPOP restarts: give `popsize_multiplier` with it")
-        ladder = ipop_ladder(state, popsize_multiplier, max_popsize)
+        ladder = (bipop_ladder if bipop else ipop_ladder)(state, popsize_multiplier, max_popsize)
     H = history_length(d, state.popsize)
     opts = dict(dtype=center.dtype, device=center.device)
+    zeros = lambda dt: torch.zeros(batch, dtype=dt, device=center.device)  # noqa: E731
+    policy = {} if not bipop else dict(regime=zeros(torch.int32), large_tier=zeros(torch.int32), large_evaluations=zeros(torch.int64),
+                                       small_evaluations=zeros(torch.int64), last_large_evaluations=zeros(torch.int64),
+                                       run_stdev=state.sigma.clone())
     return RestartState(
         search=state if ladder is None else state._replace(hyperparameters=ladder.hyperparameters[-1]),
         best_values=torch.full(batch + (d,), math.nan, **opts),
@@ -199,6 +271,7 @@ def restarts(state: Union[CMAESState, SepCMAESState], *, lb, ub, tol_fun: Option
         **th,
         **({} if ladder is None else dict(tier=torch.zeros(batch, dtype=torch.int32, device=center.device),
                                           num_evaluations=torch.zeros(batch, dtype=torch.int64, device=center.device), ladder=ladder)),
+        **policy,
     )
 
 
@@ -207,7 +280,7 @@ def restarts_tell(rs: RestartState, values: Union[torch.Tensor, LazyPopulation],
     of the items that met one.  `values` as the family's tell takes it (a separable search also takes the LazyPopulation that
     `sepcmaes_ask_and_evaluate(..., lazy=True)` returned).  `rs` is left unchanged.  IPOP: item b at tier k is told its first
     lambda_k rows with tier k's constants; its evaluations count grows by lambda_k, and a restart moves it to tier k + 1 (the top
-    tier stays)."""
+    tier stays).  BIPOP: the same, with the regime's budget growing too and the regime policy choosing a restarted item's tier."""
     search = rs.search
     sep = isinstance(search, SepCMAESState)
     center = search.center
@@ -227,34 +300,45 @@ def restarts_tell(rs: RestartState, values: Union[torch.Tensor, LazyPopulation],
              num_restarts=rs.num_restarts.reshape(B).clone())
     sigma0, lb, ub = rs.stdev_init.reshape(B), rs.lb.reshape(B, d), rs.ub.reshape(B, d)
     n_evals = rs.num_evaluations.reshape(B).clone() if ipop else None
+    bipop = rs.regime is not None
+    policy = {k: getattr(rs, k).reshape(B).clone() for k in BIPOP_FIELDS} if bipop else {}
     if lazy or on_kernels(center):
         # in place on the tell's fresh tensors and on the clones above
         flags = torch.empty(B, dtype=torch.int32, device=center.device)
         draw = dict(m_draw=search.center.reshape(B, d), s_draw=search.s.reshape(B, d), draw_seed=values.seed) if lazy else {}
         if ipop:
             draw.update(tier=tier, tier_counts=rs.ladder.counts, tier_history=rs.ladder.history, num_evaluations=n_evals)
+        if bipop:
+            draw.update(policy, n_large=rs.ladder.n_large, popsize0=rs.ladder.popsizes[0])
         ops.cma_restart_batched(sep, f.contiguous(), None if lazy else x.contiguous(), search.maximize, steps, st["m"], st["sigma"], st["p_sigma"],
                                 st["p_c"], st["C"], st["A"], st["s"], r["history"], r["best_x"], r["best_f"], r["num_restarts"], flags,
                                 sigma0.contiguous(), lb, ub, rs.thresholds, seed=draw_philox_seed(), **draw)
     else:
         if ipop:
-            r.update(tier=tier, num_evaluations=n_evals)
+            r.update(tier=tier, num_evaluations=n_evals, **policy)
         st, r, steps, flags = _restart_torch(rs.thresholds, sep, search.maximize, f, x, steps, st, r, sigma0, lb, ub, ladder=rs.ladder)
         if ipop:
             tier, n_evals = r["tier"], r["num_evaluations"]
+            policy = {k: r[k] for k in policy}
     vec = batch + (d,)
     new = new._replace(center=st["m"].view(vec), sigma=st["sigma"].view(batch), p_sigma=st["p_sigma"].view(vec), p_c=st["p_c"].view(vec),
                        C=st["C"].view(vec if sep else vec + (d,)), A=st["A"].view(vec if sep else vec + (d,)),
                        **({"s": st["s"].view(vec)} if sep else {}))
     return rs._replace(search=new, best_values=r["best_x"].view(vec), best_evals=r["best_f"].view(batch), num_restarts=r["num_restarts"].view(batch),
                        item_generation=steps.view(batch), history=r["history"].view(batch + (-1,)), stop_flags=flags.view(batch),
-                       **(dict(tier=tier.view(batch), num_evaluations=n_evals.view(batch)) if ipop else {}))
+                       **(dict(tier=tier.view(batch), num_evaluations=n_evals.view(batch)) if ipop else {}),
+                       **{k: v.view(batch) for k, v in policy.items()})
+
+
+BIPOP_FIELDS = ("regime", "large_tier", "large_evaluations", "small_evaluations", "last_large_evaluations", "run_stdev")
 
 
 def _restart_torch(thresholds, sep, maximize, f, x, gen, st, r, sigma0, lb, ub, ladder=None) -> tuple:
     """The restart stage as batched torch ops (the semantics of evok_cma_restart_batched; the new centres from torch.rand(B, D)).
     With `ladder` (IPOP; r then also holds "tier" and "num_evaluations"), N and H of each item come from its tier, and the
-    evaluation count and the tier advance follow (evok_cma_restart_batched_tiered)."""
+    evaluation count and the tier advance follow (evok_cma_restart_batched_tiered).  With a BIPOP ladder (ladder.n_large set; r then
+    also holds BIPOP_FIELDS), the regime policy of evok_cma_restart_batched_bipop replaces the tier advance; sigma0 is the default
+    step size, and u1, u2 of a small run come from torch.rand(B, 2) after the centres."""
     B, n = f.shape
     d = lb.shape[-1]
     H = r["history"].shape[-1]
@@ -265,6 +349,8 @@ def _restart_torch(thresholds, sep, maximize, f, x, gen, st, r, sigma0, lb, ub, 
         n_b, H = ladder.counts.long()[t], ladder.history[t]
         real = torch.arange(n, device=f.device) < n_b[:, None]
         hreal = torch.arange(r["history"].shape[-1], device=f.device) < H[:, None]
+    bipop = ladder is not None and ladder.n_large is not None
+    run0 = r["run_stdev"] if bipop else sigma0  # the step size tol_x and tol_x_up compare against
     fin = torch.isfinite(f) if real is None else torch.isfinite(f) & real
     key = torch.where(fin, f, -math.inf if maximize else math.inf)
     idx = key.argmax(-1) if maximize else key.argmin(-1)  # the first of equal values: the lower row wins ties
@@ -303,25 +389,57 @@ def _restart_torch(thresholds, sep, maximize, f, x, gen, st, r, sigma0, lb, ub, 
     bits = [
         zero if th["tol_fun"] is None else ((gen >= H) & f_all_fin & h_all_fin
                                             & (torch.maximum(f_max, h_max) - torch.minimum(f_min, h_min) < th["tol_fun"])),
-        zero if th["tol_x"] is None else sig * torch.maximum(max_pc, max_sd) < th["tol_x"] * sigma0,
-        zero if th["tol_x_up"] is None else sig * max_sd > th["tol_x_up"] * sigma0,
+        zero if th["tol_x"] is None else sig * torch.maximum(max_pc, max_sd) < th["tol_x"] * run0,
+        zero if th["tol_x_up"] is None else sig * max_sd > th["tol_x_up"] * run0,
         zero if th["max_condition"] is None else (ratio if sep else ratio * ratio) > th["max_condition"],
         too_flat,
         zero if th["max_generations"] is None else gen >= th["max_generations"],
         ~(sig > 0) | ~torch.isfinite(sig) | ~torch.isfinite(torch.cat([m, p_sigma, p_c, c_diag], -1)).all(-1),
     ]
+    if bipop:
+        regime = r["regime"]
+        n_large_ev = r["large_evaluations"] + torch.where(regime == 1, n_b, 0)
+        n_small_ev = r["small_evaluations"] + torch.where(regime == 2, n_b, 0)
+        bits.append((regime == 2) & (2 * gen * n_b >= r["last_large_evaluations"]))
     flags = sum(b.to(torch.int32) << k for k, b in enumerate(bits))
     go = flags != 0
     centre = lb + (ub - lb) * torch.rand(B, d, dtype=f.dtype, device=f.device)
+    s0 = sigma0
+    if bipop:
+        policy = _bipop_policy(ladder, go, regime, gen, n_b, n_large_ev, n_small_ev, r, sigma0, torch.rand(B, 2, dtype=f.dtype, device=f.device))
+        s0 = policy["run_stdev"]
     col = go[:, None]
-    out = dict(m=torch.where(col, centre, m), sigma=torch.where(go, sigma0, sig), p_sigma=torch.where(col, 0.0, p_sigma), p_c=torch.where(col, 0.0, p_c))
+    out = dict(m=torch.where(col, centre, m), sigma=torch.where(go, s0, sig), p_sigma=torch.where(col, 0.0, p_sigma), p_c=torch.where(col, 0.0, p_c))
     if sep:
-        out.update(C=torch.where(col, 1.0, C), A=torch.where(col, 1.0, A), s=torch.where(col, sigma0[:, None].expand(B, d), st["s"]))
+        out.update(C=torch.where(col, 1.0, C), A=torch.where(col, 1.0, A), s=torch.where(col, s0[:, None].expand(B, d), st["s"]))
     else:
         eye = torch.eye(d, dtype=f.dtype, device=f.device)
         out.update(C=torch.where(go[:, None, None], eye, C), A=torch.where(go[:, None, None], eye, A), s=None)
     out_r = dict(history=torch.where(col, nan, history), best_x=best_x, best_f=best_f, num_restarts=r["num_restarts"] + go.to(torch.int64))
-    if ladder is not None:
+    if bipop:
+        out_r.update(num_evaluations=r["num_evaluations"] + n_b, **policy)
+    elif ladder is not None:
         out_r.update(num_evaluations=r["num_evaluations"] + n_b, tier=torch.where(go, torch.clamp_max(r["tier"] + 1, len(ladder.popsizes) - 1), r["tier"]))
     r = out_r
     return out, r, torch.where(go, 0, gen), flags
+
+
+def _bipop_policy(ladder, go, regime, gen, n_b, n_large_ev, n_small_ev, r, sigma_def, u) -> dict:
+    """The BIPOP fields after a tell, `go` the items that restart: the next run large (one rung up) when n_large_ev <= n_small_ev,
+    else small, of population size max(lambda_0, floor(lambda_0 exp(u1^2 log(lambda_l / (2 lambda_0))))) and step size
+    sigma_def 10^(-2 u2), in float64 (u (B, 2) in [0, 1))."""
+    K, lam0 = ladder.n_large, ladder.popsizes[0]
+    lt = r["large_tier"]
+    large = n_large_ev <= n_small_ev
+    last = torch.where(go & (regime == 1), gen * n_b, r["last_large_evaluations"])
+    lt_up = torch.clamp_max(lt + 1, K - 1)
+    u1, u2 = u[:, 0].double(), u[:, 1].double()
+    lam_l = ladder.counts.long()[lt.long()].double()
+    lam_s = torch.floor(lam0 * torch.exp(u1 * u1 * torch.log(0.5 * lam_l / lam0))).clamp_min(lam0).long()
+    small_tier = torch.clamp_max(K + lam_s - lam0, len(ladder.popsizes) - 1).to(torch.int32)
+    small_stdev = (sigma_def.double() * torch.pow(10.0, -2.0 * u2)).to(sigma_def.dtype)
+    return dict(regime=torch.where(go, torch.where(large, 1, 2), regime).to(torch.int32),
+                large_tier=torch.where(go & large, lt_up, lt).to(torch.int32),
+                tier=torch.where(go, torch.where(large, lt_up, small_tier), r["tier"]).to(torch.int32),
+                large_evaluations=n_large_ev, small_evaluations=n_small_ev, last_large_evaluations=last,
+                run_stdev=torch.where(go, torch.where(large, sigma_def, small_stdev), r["run_stdev"]))

@@ -5,7 +5,9 @@
 //                          item a uniform centre in [lb, ub], sigma0, zero paths, counter 0, empty history (separable: C = A = 1, s)
 //   cma_restart_eye_kernel full family only: C = A = I for the restarted items, grid-wide, masked by the flags
 // The tiered form (IPOP, padded populations) reads N and H of item b from its tier, moves a restarted item one tier up and
-// counts the evaluations of each item.
+// counts the evaluations of each item.  The BIPOP form is the tiered one with a per-item policy at restart time instead of the
+// tier advance: a large run one rung up the ladder or a small run of random population size and step size, whichever regime has
+// used fewer evaluations, and a budget stop (bit 7) for small runs.
 #include "evok_common.cuh"
 
 namespace evok {
@@ -14,6 +16,9 @@ constexpr int kRestartThreads = 256;
 constexpr int kRestartWarps = kRestartThreads / kWarp;
 constexpr int kEyeThreads = 256;
 constexpr int64_t kEyeMaxBlocksPerItem = 64;
+
+// the forms of the stage: plain, tiered (IPOP) and BIPOP (tiered, with the regime policy at restart time)
+enum RestartMode : int { kRestartPlain = 0, kRestartTiered = 1, kRestartBipop = 2 };
 
 struct RestartArgs {
   const float* f;       // [items][n_rows]
@@ -40,6 +45,13 @@ struct RestartArgs {
   const long long* tier_history;
   int n_tiers;
   long long* num_evaluations;
+  // BIPOP only: the regime (0 first run, 1 large, 2 small), the ladder rung of the latest large run, the evaluations of each regime
+  // and of the latest large run, the step size the current run started with; tiers 0..n_large-1 are the ladder, tier
+  // n_large + (lambda - popsize0) the small run of population size lambda; sigma0 is the default step size
+  int *regime, *large_tier;
+  long long *large_evaluations, *small_evaluations, *last_large_evaluations;
+  float* run_stdev;
+  int n_large, popsize0;
 };
 
 // the row that wins: finite, better under the sense, the lower index on ties; index -1 = none
@@ -71,13 +83,45 @@ struct FMax { __device__ float operator()(float a, float b) const { return fmaxf
 struct FMin { __device__ float operator()(float a, float b) const { return fminf(a, b); } };
 struct DSum { __device__ double operator()(double a, double b) const { return a + b; } };
 
-template <bool TIERED>
+// BIPOP, thread 0 of a restarting item's CTA, after its run was accounted: the next run.  Large (one rung up the ladder, the default
+// step size) unless the large runs used more evaluations than the small ones.  Small: lambda_s = max(lambda_0, floor(lambda_0
+// (lambda_l / (2 lambda_0))^(u1^2))), step size sigma_def 10^(-2 u2), in float64, with u1, u2 = uniform24 of words x, y of Philox
+// counter (0, 1, 0xFF000000, item) under the reset key: the reset centres use (j >> 2, 0, 0xFF000000, item), so no other draw
+// has this counter.
+__device__ __forceinline__ void bipop_next_run(const RestartArgs& a, int64_t b, int regime, long long gen, int64_t N, float* s_run_stdev) {
+  if (regime == 1) a.last_large_evaluations[b] = gen * N;
+  int lt = a.large_tier[b], next;
+  float stdev = a.sigma0[b];
+  if (a.large_evaluations[b] <= a.small_evaluations[b]) {
+    lt = min(lt + 1, a.n_large - 1);
+    a.large_tier[b] = lt;
+    a.regime[b] = 1;
+    next = lt;
+  } else {
+    const U4 r = philox4x32_10(U4{0u, 1u, 0xFF000000u, a.reset_key.stream_lo + (uint32_t)b}, a.reset_key);
+    const double u1 = (double)uniform24(r.x), u2 = (double)uniform24(r.y);
+    const double lam0 = (double)a.popsize0;
+    const double lam = floor(lam0 * exp(u1 * u1 * log(0.5 * (double)a.tier_counts[lt] / lam0)));
+    const int small = lam > lam0 ? (int)lam - a.popsize0 : 0;
+    next = min(a.n_large + small, a.n_tiers - 1);
+    stdev = (float)((double)a.sigma0[b] * exp10(-2.0 * u2));
+    a.regime[b] = 2;
+  }
+  a.tier[b] = next;
+  a.run_stdev[b] = stdev;
+  *s_run_stdev = stdev;
+}
+
+template <int MODE>
 __global__ void __launch_bounds__(kRestartThreads) cma_restart_kernel(const __grid_constant__ RestartArgs a) {
+  constexpr bool TIERED = MODE != kRestartPlain;
+  constexpr bool BIPOP = MODE == kRestartBipop;
   __shared__ float smf[kRestartWarps + 1];
   __shared__ double smd[kRestartWarps + 1];
   __shared__ float s_best_v[kRestartWarps];
   __shared__ long long s_best_i[kRestartWarps];
   __shared__ int s_flags;
+  __shared__ float s_run_stdev;
   const int64_t b = blockIdx.x, D = a.D;
   const int tk = TIERED ? a.tier[b] : 0;
   const int64_t N = TIERED ? min((int64_t)a.tier_counts[tk], a.n_rows) : a.n_rows;
@@ -194,7 +238,7 @@ __global__ void __launch_bounds__(kRestartThreads) cma_restart_kernel(const __gr
   rmn = block_reduce(rmn, FMin(), smf);
 
   if (threadIdx.x == 0) {
-    const double s0 = (double)a.sigma0[b];
+    const double s0 = (double)(BIPOP ? a.run_stdev[b] : a.sigma0[b]);
     int flags = 0;
     if (!isnan(a.tol_fun) && gen >= H && !bad && !hbad && (double)fmaxf(fmx, hmx) - (double)fminf(fmn, hmn) < (double)a.tol_fun) flags |= 1;
     if (!isnan(a.tol_x) && (double)sig * (double)fmaxf(mpc, msd) < (double)a.tol_x * s0) flags |= 2;
@@ -206,6 +250,13 @@ __global__ void __launch_bounds__(kRestartThreads) cma_restart_kernel(const __gr
     if (!isnan(a.min_fitness_stdev) && N > 1 && sqrt(dev / (double)(N - 1)) < (double)a.min_fitness_stdev) flags |= 16;
     if (!isnan(a.max_generations) && (double)gen >= (double)a.max_generations) flags |= 32;
     if (nonfinite) flags |= 64;
+    if constexpr (BIPOP) {
+      const int regime = a.regime[b];
+      if (regime == 1) a.large_evaluations[b] += N;
+      if (regime == 2) a.small_evaluations[b] += N;
+      if (regime == 2 && 2 * gen * N >= a.last_large_evaluations[b]) flags |= 128;  // the run used half the latest large run
+      if (flags) bipop_next_run(a, b, regime, gen, N, &s_run_stdev);
+    }
     a.stop_flags[b] = flags;
     s_flags = flags;
     if (TIERED) a.num_evaluations[b] += N;
@@ -213,10 +264,11 @@ __global__ void __launch_bounds__(kRestartThreads) cma_restart_kernel(const __gr
   __syncthreads();
   if (s_flags == 0) return;
 
+
   // re-initialisation: x_j = lb_j + (ub_j - lb_j) u_j, u_j = uniform24 of word j & 3 of Philox counter (j >> 2, 0, 0xFF000000, item)
   const float* lb = a.lb + b * a.item_stride_bounds;
   const float* ub = a.ub + b * a.item_stride_bounds;
-  const float s0 = a.sigma0[b];
+  const float s0 = BIPOP ? s_run_stdev : a.sigma0[b];
   float* mw = a.m + b * D;
   float* psw = a.p_sigma + b * D;
   float* pcw = a.p_c + b * D;
@@ -241,7 +293,7 @@ __global__ void __launch_bounds__(kRestartThreads) cma_restart_kernel(const __gr
   }
   for (int64_t k = threadIdx.x; k < a.H; k += kRestartThreads) hist[k] = NAN;
   if (threadIdx.x == 0) {
-    if (TIERED) a.tier[b] = min(tk + 1, a.n_tiers - 1);
+    if (MODE == kRestartTiered) a.tier[b] = min(tk + 1, a.n_tiers - 1);
     a.sigma[b] = s0;
     a.item_steps[b] = 0;
     a.num_restarts[b] += 1;
@@ -266,22 +318,36 @@ __global__ void __launch_bounds__(kEyeThreads) cma_restart_eye_kernel(const int*
 
 using namespace evok;
 
-// the restart stage of evok_cma_restart_batched, or (TIERED) of evok_cma_restart_batched_tiered with the tier arrays
-template <bool TIERED>
+// BIPOP's per-item policy arrays (evok_cma_restart_batched_bipop); unused by the other forms
+struct BipopArrays {
+  int32_t *regime, *large_tier;
+  int64_t *large_evaluations, *small_evaluations, *last_large_evaluations;
+  float* run_stdev;
+  int64_t n_large, popsize0;
+};
+
+// the restart stage of evok_cma_restart_batched, of evok_cma_restart_batched_tiered with the tier arrays (kRestartTiered), or of
+// evok_cma_restart_batched_bipop with the tier and policy arrays (kRestartBipop)
+template <int MODE>
 static int cma_restart_items(int separable, const float* f, const float* X, int64_t item_stride_x, int64_t ldx, const float* m_draw, const float* s_draw,
                              uint64_t draw_seed, int64_t n_items, int64_t n_rows, int64_t D, int maximize, int64_t* item_steps, float* m, float* sigma,
                              float* p_sigma, float* p_c, float* C, float* A, float* s, float* history, int64_t H, float* best_x, float* best_f,
                              int64_t* num_restarts, int32_t* stop_flags, const float* sigma0, const float* lb, const float* ub,
                              int64_t item_stride_bounds, const float* thresholds_host, uint64_t seed, int32_t* tier, const int32_t* tier_counts,
-                             const int64_t* tier_history, int64_t n_tiers, int64_t* num_evaluations, void* stream) {
+                             const int64_t* tier_history, int64_t n_tiers, int64_t* num_evaluations, const BipopArrays& bp, void* stream) {
+  constexpr bool TIERED = MODE != kRestartPlain;
+  constexpr bool BIPOP = MODE == kRestartBipop;
   if (!f || !item_steps || !m || !sigma || !p_sigma || !p_c || !C || !A || !history || !best_x || !best_f || !num_restarts || !stop_flags || !sigma0 ||
       !lb || !ub || !thresholds_host)
     return EVOK_E_NULLPTR;
   if (separable ? (!s || (!X && (!m_draw || !s_draw))) : !X) return EVOK_E_NULLPTR;
   if (TIERED && (!tier || !tier_counts || !tier_history || !num_evaluations)) return EVOK_E_NULLPTR;
+  if (BIPOP && (!bp.regime || !bp.large_tier || !bp.large_evaluations || !bp.small_evaluations || !bp.last_large_evaluations || !bp.run_stdev))
+    return EVOK_E_NULLPTR;
   if (n_items < 0 || n_rows <= 0 || D <= 0 || H <= 0 || (X && (ldx < D || item_stride_x < 0)) || (item_stride_bounds != 0 && item_stride_bounds != D))
     return EVOK_E_BADSIZE;
   if (TIERED && (n_tiers < 1 || n_tiers > INT32_MAX)) return EVOK_E_BADSIZE;
+  if (BIPOP && (bp.n_large < 1 || bp.n_large >= n_tiers || bp.popsize0 < 1 || bp.popsize0 > INT32_MAX)) return EVOK_E_BADSIZE;
   if (n_items == 0) return 0;
   RestartArgs a;
   a.f = f; a.X = X; a.item_stride_x = item_stride_x; a.ldx = ldx; a.m_draw = m_draw; a.s_draw = s_draw;
@@ -297,6 +363,11 @@ static int cma_restart_items(int separable, const float* f, const float* X, int6
   a.min_fitness_stdev = thresholds_host[4]; a.max_generations = thresholds_host[5];
   a.tier = tier; a.tier_counts = tier_counts; a.tier_history = reinterpret_cast<const long long*>(tier_history); a.n_tiers = (int)n_tiers;
   a.num_evaluations = reinterpret_cast<long long*>(num_evaluations);
+  a.regime = bp.regime; a.large_tier = bp.large_tier;
+  a.large_evaluations = reinterpret_cast<long long*>(bp.large_evaluations);
+  a.small_evaluations = reinterpret_cast<long long*>(bp.small_evaluations);
+  a.last_large_evaluations = reinterpret_cast<long long*>(bp.last_large_evaluations);
+  a.run_stdev = bp.run_stdev; a.n_large = (int)bp.n_large; a.popsize0 = (int)bp.popsize0;
   const int rc = for_item_chunks(n_items, (int64_t)INT32_MAX, [&](int64_t b0, int64_t nb) {
     RestartArgs c = a;
     const int64_t mat = separable ? D : D * D;
@@ -310,7 +381,11 @@ static int cma_restart_items(int separable, const float* f, const float* X, int6
     c.history += b0 * H; c.best_x += b0 * D; c.best_f += b0; c.num_restarts += b0; c.stop_flags += b0; c.sigma0 += b0;
     c.lb += b0 * item_stride_bounds; c.ub += b0 * item_stride_bounds;
     if (TIERED) { c.tier += b0; c.num_evaluations += b0; }
-    cma_restart_kernel<TIERED><<<(unsigned)nb, kRestartThreads, 0, (cudaStream_t)stream>>>(c);
+    if (BIPOP) {
+      c.regime += b0; c.large_tier += b0; c.large_evaluations += b0; c.small_evaluations += b0; c.last_large_evaluations += b0;
+      c.run_stdev += b0;
+    }
+    cma_restart_kernel<MODE><<<(unsigned)nb, kRestartThreads, 0, (cudaStream_t)stream>>>(c);
     EVOK_CHECK_LAUNCH();
     return 0;
   });
@@ -330,9 +405,9 @@ extern "C" EVOK_API int evok_cma_restart_batched(int separable, const float* f, 
                                                  float* history, int64_t H, float* best_x, float* best_f, int64_t* num_restarts, int32_t* stop_flags,
                                                  const float* sigma0, const float* lb, const float* ub, int64_t item_stride_bounds,
                                                  const float* thresholds_host, uint64_t seed, void* stream) {
-  return cma_restart_items<false>(separable, f, X, item_stride_x, ldx, m_draw, s_draw, draw_seed, n_items, n_rows, D, maximize, item_steps, m, sigma,
-                                  p_sigma, p_c, C, A, s, history, H, best_x, best_f, num_restarts, stop_flags, sigma0, lb, ub, item_stride_bounds,
-                                  thresholds_host, seed, nullptr, nullptr, nullptr, 0, nullptr, stream);
+  return cma_restart_items<kRestartPlain>(separable, f, X, item_stride_x, ldx, m_draw, s_draw, draw_seed, n_items, n_rows, D, maximize, item_steps, m,
+                                          sigma, p_sigma, p_c, C, A, s, history, H, best_x, best_f, num_restarts, stop_flags, sigma0, lb, ub,
+                                          item_stride_bounds, thresholds_host, seed, nullptr, nullptr, nullptr, 0, nullptr, BipopArrays{}, stream);
 }
 
 extern "C" EVOK_API int evok_cma_restart_batched_tiered(int separable, const float* f, const float* X, int64_t item_stride_x, int64_t ldx,
@@ -343,7 +418,25 @@ extern "C" EVOK_API int evok_cma_restart_batched_tiered(int separable, const flo
                                                         int64_t item_stride_bounds, const float* thresholds_host, uint64_t seed, int32_t* tier,
                                                         const int32_t* tier_counts, const int64_t* tier_history, int64_t n_tiers,
                                                         int64_t* num_evaluations, void* stream) {
-  return cma_restart_items<true>(separable, f, X, item_stride_x, ldx, m_draw, s_draw, draw_seed, n_items, n_rows, D, maximize, item_steps, m, sigma,
-                                 p_sigma, p_c, C, A, s, history, H, best_x, best_f, num_restarts, stop_flags, sigma0, lb, ub, item_stride_bounds,
-                                 thresholds_host, seed, tier, tier_counts, tier_history, n_tiers, num_evaluations, stream);
+  return cma_restart_items<kRestartTiered>(separable, f, X, item_stride_x, ldx, m_draw, s_draw, draw_seed, n_items, n_rows, D, maximize, item_steps, m,
+                                           sigma, p_sigma, p_c, C, A, s, history, H, best_x, best_f, num_restarts, stop_flags, sigma0, lb, ub,
+                                           item_stride_bounds, thresholds_host, seed, tier, tier_counts, tier_history, n_tiers, num_evaluations,
+                                           BipopArrays{}, stream);
+}
+
+extern "C" EVOK_API int evok_cma_restart_batched_bipop(int separable, const float* f, const float* X, int64_t item_stride_x, int64_t ldx,
+                                                       const float* m_draw, const float* s_draw, uint64_t draw_seed, int64_t n_items, int64_t n_rows,
+                                                       int64_t D, int maximize, int64_t* item_steps, float* m, float* sigma, float* p_sigma, float* p_c,
+                                                       float* C, float* A, float* s, float* history, int64_t H, float* best_x, float* best_f,
+                                                       int64_t* num_restarts, int32_t* stop_flags, const float* sigma_def, const float* lb, const float* ub,
+                                                       int64_t item_stride_bounds, const float* thresholds_host, uint64_t seed, int32_t* tier,
+                                                       const int32_t* tier_counts, const int64_t* tier_history, int64_t n_tiers,
+                                                       int64_t* num_evaluations, int32_t* regime, int32_t* large_tier, int64_t* large_evaluations,
+                                                       int64_t* small_evaluations, int64_t* last_large_evaluations, float* run_stdev, int64_t n_large,
+                                                       int64_t popsize0, void* stream) {
+  const BipopArrays bp{regime, large_tier, large_evaluations, small_evaluations, last_large_evaluations, run_stdev, n_large, popsize0};
+  return cma_restart_items<kRestartBipop>(separable, f, X, item_stride_x, ldx, m_draw, s_draw, draw_seed, n_items, n_rows, D, maximize, item_steps, m,
+                                          sigma, p_sigma, p_c, C, A, s, history, H, best_x, best_f, num_restarts, stop_flags, sigma_def, lb, ub,
+                                          item_stride_bounds, thresholds_host, seed, tier, tier_counts, tier_history, n_tiers, num_evaluations, bp,
+                                          stream);
 }

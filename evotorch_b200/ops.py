@@ -1170,6 +1170,7 @@ def cmaes_vector_update_batched(local_disp: torch.Tensor, shaped_disp: torch.Ten
 
 
 RESTART_CRITERIA = ("tol_fun", "tol_x", "tol_x_up", "max_condition", "min_fitness_stdev", "max_generations")  # bits 0-5; bit 6: non-finite
+# bit 7 (BIPOP only): a small run has used half the evaluations of the item's latest large run; it has no threshold
 
 
 def cma_restart_batched(separable: bool, f: torch.Tensor, X: Optional[torch.Tensor], maximize: bool, item_steps: torch.Tensor, m: torch.Tensor,
@@ -1178,7 +1179,10 @@ def cma_restart_batched(separable: bool, f: torch.Tensor, X: Optional[torch.Tens
                         sigma0: torch.Tensor, lb: torch.Tensor, ub: torch.Tensor, thresholds, *, seed: int, m_draw: Optional[torch.Tensor] = None,
                         s_draw: Optional[torch.Tensor] = None, draw_seed: int = 0, tier: Optional[torch.Tensor] = None,
                         tier_counts: Optional[torch.Tensor] = None, tier_history: Optional[torch.Tensor] = None,
-                        num_evaluations: Optional[torch.Tensor] = None) -> None:
+                        num_evaluations: Optional[torch.Tensor] = None, regime: Optional[torch.Tensor] = None,
+                        large_tier: Optional[torch.Tensor] = None, large_evaluations: Optional[torch.Tensor] = None,
+                        small_evaluations: Optional[torch.Tensor] = None, last_large_evaluations: Optional[torch.Tensor] = None,
+                        run_stdev: Optional[torch.Tensor] = None, n_large: int = 0, popsize0: int = 0) -> None:
     """The restart stage of every item after its update, in place (include/evok.h, evok_cma_restart_batched): best ever, history,
     stop flags and the re-initialisation of the items that met a criterion.  f (items, N); X (items, N, D), or None for a separable
     population rebuilt from (draw_seed, stream b) with m_draw / s_draw (items, D); item_steps, num_restarts int64 (items,); m, p_sigma,
@@ -1186,7 +1190,10 @@ def cma_restart_batched(separable: bool, f: torch.Tensor, X: Optional[torch.Tens
     (items, H); stop_flags int32 (items,); `thresholds` the 6 criteria of RESTART_CRITERIA, None = off; `seed` the Philox key of
     the new centres.  With `tier` (int32 (items,), in place), the padded form (evok_cma_restart_batched_tiered): item b uses its
     first tier_counts[tier[b]] values and tier_history[tier[b]] history slots (tables int32 and int64 (K,)), num_evaluations
-    (int64 (items,)) grows by its count, and a restarted item moves one tier up."""
+    (int64 (items,)) grows by its count, and a restarted item moves one tier up.  With `regime` as well, the BIPOP form
+    (evok_cma_restart_batched_bipop): sigma0 is the default step size; regime, large_tier int32 (items,), large_evaluations,
+    small_evaluations, last_large_evaluations int64 (items,) and run_stdev (items,) are the per-item policy state, in place; tiers
+    0..n_large-1 of the tables are the ladder from popsize0, tier n_large + (lambda - popsize0) a small run of size lambda."""
     B, n = f.shape
     d = m.shape[-1]
     f = _rows(f, "f", (B, n))
@@ -1222,11 +1229,26 @@ def cma_restart_batched(separable: bool, f: torch.Tensor, X: Optional[torch.Tens
         if not (num_evaluations is not None and num_evaluations.is_cuda and num_evaluations.dtype == torch.int64 and num_evaluations.is_contiguous()
                 and tuple(num_evaluations.shape) == (B,)):
             raise ValueError(f"num_evaluations: expected a contiguous int64 CUDA tensor of shape ({B},)")
+    if regime is not None:
+        if tier is None:
+            raise ValueError("the BIPOP stage is the tiered one with a policy: give `tier` and its tables with `regime`")
+        for t, name, dt in ((regime, "regime", torch.int32), (large_tier, "large_tier", torch.int32), (large_evaluations, "large_evaluations", torch.int64),
+                            (small_evaluations, "small_evaluations", torch.int64), (last_large_evaluations, "last_large_evaluations", torch.int64)):
+            if not (t is not None and t.is_cuda and t.dtype == dt and t.is_contiguous() and tuple(t.shape) == (B,)):
+                raise ValueError(f"{name}: expected a contiguous {dt} CUDA tensor of shape ({B},)")
+        _rows(run_stdev, "run_stdev", (B,))
     with _timed("cma_restart"):
         args = (int(bool(separable)), f.data_ptr(), nat.ptr(X), n * d, d, nat.ptr(m_draw), nat.ptr(s_draw), int(draw_seed), B, n, d, int(bool(maximize)),
                 item_steps.data_ptr(), m.data_ptr(), sigma.data_ptr(), p_sigma.data_ptr(), p_c.data_ptr(), C.data_ptr(), A.data_ptr(), nat.ptr(s),
                 history.data_ptr(), history.shape[1], best_x.data_ptr(), best_f.data_ptr(), num_restarts.data_ptr(), stop_flags.data_ptr(),
                 sigma0.data_ptr(), lb.data_ptr(), ub.data_ptr(), d, _host_floats(th, 6), int(seed))
+        if regime is not None:
+            rc = nat.lib().evok_cma_restart_batched_bipop(*args, tier.data_ptr(), tier_counts.data_ptr(), tier_history.data_ptr(), K,
+                                                          num_evaluations.data_ptr(), regime.data_ptr(), large_tier.data_ptr(),
+                                                          large_evaluations.data_ptr(), small_evaluations.data_ptr(), last_large_evaluations.data_ptr(),
+                                                          run_stdev.data_ptr(), int(n_large), int(popsize0), nat.stream_of(f))
+            nat.check(rc, "evok_cma_restart_batched_bipop")
+            return
         if tier is not None:
             rc = nat.lib().evok_cma_restart_batched_tiered(*args, tier.data_ptr(), tier_counts.data_ptr(), tier_history.data_ptr(), K,
                                                            num_evaluations.data_ptr(), nat.stream_of(f))

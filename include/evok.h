@@ -582,6 +582,7 @@ int evok_sepcma_update_batched_steps(const float* local, const float* S2, const 
  *           bit 4 min_fitness_stdev  the unbiased standard deviation of the N values (N > 1, finite) < thresholds[4]
  *           bit 5 max_generations    g >= thresholds[5]
  *           bit 6 non-finite (always on)  sigma <= 0, or sigma, an entry of m, p_sigma, p_c or diag C is not finite
+ *           bit 7 small-run budget (BIPOP only, evok_cma_restart_batched_bipop; never set by this entry)
  *       - an item with a flag restarts: m_j = lb_j + (ub_j - lb_j) u_j (float32, unfused) with u_j = uniform24 of word j & 3 of
  *         Philox4x32-10(counter (j >> 2, 0, 0xFF000000, stream word b), key (seed, stream 0)) -- no sample counter (third word
  *         below 2^31) or noise counter (0x80.. to 0x87..) has this third word; sigma <- sigma0[b], p_sigma = p_c = 0,
@@ -642,6 +643,37 @@ int evok_cma_restart_batched_tiered(int separable, const float* f, const float* 
                                     const float* sigma0, const float* lb, const float* ub, int64_t item_stride_bounds,
                                     const float* thresholds_host, uint64_t seed, int32_t* tier, const int32_t* tier_counts,
                                     const int64_t* tier_history, int64_t n_tiers, int64_t* num_evaluations, void* stream);
+
+/* BIPOP restarts (Hansen, GECCO 2009 workshops): IPOP's padded populations with two regimes per item, large runs that climb the
+ * ladder and small runs of random population size and step size, each given a similar share of the evaluations.
+ *   evok_cma_restart_batched_bipop: evok_cma_restart_batched_tiered (sigma0 renamed sigma_def: the default step size per item)
+ *       with a per-item policy in place of the tier advance.  Tiers 0..n_large-1 of the tables are the ladder lambda_0 =
+ *       popsize0 .. lambda_{K-1}; tier n_large + (lambda - popsize0) is a small run of population size lambda, for every lambda in
+ *       [popsize0, max(popsize0, floor(lambda_{K-1} / 2))], so n_tiers is at least n_large + 1.  Per item b, device memory:
+ *       regime [items] int32 (0 the first run, 1 a large run, 2 a small run), large_tier [items] int32 (l: the rung of the latest
+ *       large run, 0 before any), large_evaluations, small_evaluations, last_large_evaluations [items] int64 (n_L, n_S, n_last),
+ *       run_stdev [items] float (the step size the current run started with).  With N = counts[tier[b]] and g = item_steps[b]:
+ *       - n_L (regime 1) or n_S (regime 2) grows by N; the first run counts in neither;
+ *       - tol_x and tol_x_up compare against run_stdev[b] instead of sigma0;
+ *           bit 7 small-run budget  regime 2 and 2 g N >= n_last (the run has used half the evaluations of the latest large run)
+ *       - an item with a flag: if its run was large, n_last <- g N.  Then the next run is large when n_L <= n_S (so the first
+ *         restart is): l <- min(l + 1, n_large - 1), tier = l, run_stdev = sigma_def.  Otherwise small: u1, u2 = uniform24 of
+ *         words x and y of Philox4x32-10(counter (0, 1, 0xFF000000, stream word b), key (seed, stream 0)) -- the reset centres
+ *         have second word 0, so no other draw has this counter; lambda_s = max(popsize0, floor(popsize0 exp(u1^2 log(0.5
+ *         counts[l] / popsize0)))) and run_stdev = (float)(sigma_def 10^(-2 u2)), both in float64; tier = n_large + lambda_s -
+ *         popsize0 (at most n_tiers - 1).  The reset is evok_cma_restart_batched's with run_stdev[b] in place of sigma0[b]
+ *         (sigma, and s for the separable family).
+ *       Errors: those of evok_cma_restart_batched_tiered in its order, with EVOK_E_NULLPTR also for regime, large_tier, the three
+ *       budgets and run_stdev, and EVOK_E_BADSIZE also for n_large < 1, n_large >= n_tiers, popsize0 < 1. */
+int evok_cma_restart_batched_bipop(int separable, const float* f, const float* X, int64_t item_stride_x, int64_t ldx, const float* m_draw,
+                                   const float* s_draw, uint64_t draw_seed, int64_t n_items, int64_t n_rows, int64_t D, int maximize,
+                                   int64_t* item_steps, float* m, float* sigma, float* p_sigma, float* p_c, float* C, float* A, float* s,
+                                   float* history, int64_t H, float* best_x, float* best_f, int64_t* num_restarts, int32_t* stop_flags,
+                                   const float* sigma_def, const float* lb, const float* ub, int64_t item_stride_bounds,
+                                   const float* thresholds_host, uint64_t seed, int32_t* tier, const int32_t* tier_counts,
+                                   const int64_t* tier_history, int64_t n_tiers, int64_t* num_evaluations, int32_t* regime, int32_t* large_tier,
+                                   int64_t* large_evaluations, int64_t* small_evaluations, int64_t* last_large_evaluations, float* run_stdev,
+                                   int64_t n_large, int64_t popsize0, void* stream);
 
 /* Cholesky factorisation A = L L^T (fp32, lower; the strictly upper part of L is zeroed, like torch.linalg.cholesky).  Replaces
  * CMAES.decompose_C (cmaes.py:555-565, torch.linalg.cholesky -> cuSOLVER potrf).  ONE persistent kernel: 64 x 64 tiles, left-looking
