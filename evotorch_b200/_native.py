@@ -37,6 +37,10 @@ _SIGNATURES = {
     "evok_sample_eval_batched": (c_int, [c_int, _P, c_int64, c_int64, _P, c_int64, _P, c_int64, c_int64, c_int64, c_int64, c_int, c_uint64, c_uint64,
                                          _P, _P]),
     "evok_eval_batched": (c_int, [c_int, _P, c_int64, c_int64, c_int64, c_int64, c_int64, c_uint64, c_uint64, _P, _P]),
+    "evok_objective_register_transform": (c_int, [_P, c_size_t, _P, c_int, _P]),
+    "evok_eval_transform_workspace_bytes": (c_size_t, [_P, c_int64, c_int64, c_int64, c_int64]),
+    "evok_eval_transform_batched": (c_int, [c_int, _P, c_int64, c_int64, _P, c_int64, _P, c_int64, c_int64, c_int64, c_int64, c_uint64, c_uint64,
+                                            _P, c_size_t, _P, _P]),
     "evok_grad_batched_regen": (c_int, [c_int, _P, _P, c_int64, _P, c_int64, c_int64, c_int64, c_int64, c_uint64, c_uint64, c_float, c_float, _P,
                                         _P, _P, c_size_t, _P]),
     "evok_rank_workspace_bytes": (c_size_t, [c_int64]),

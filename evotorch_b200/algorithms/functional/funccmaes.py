@@ -28,6 +28,7 @@ from typing import Callable, NamedTuple, Optional
 import torch
 
 from ... import ops
+from ...objectives import is_transformed
 from ..cmaes import CMAESHyperparameters, cmaes_hyperparameters
 from .fused import LazyPopulation
 from .misc import draw_philox_seed, on_kernels
@@ -154,6 +155,8 @@ def cmaes_ask_and_evaluate(state: CMAESState, *, objective: Callable) -> tuple:
     values, seed = _ask(state)
     oid = getattr(objective, "evok_objective_id", None)
     if seed is not None and oid is not None and oid != ops.OBJ_NONE and hasattr(objective, "evaluate_batched"):
+        return values, objective.evaluate_batched(values, seed=seed)
+    if seed is not None and is_transformed(objective):  # a FusedObjective of y = M (x - o): its own kernels
         return values, objective.evaluate_batched(values, seed=seed)
     return values, objective(values)
 

@@ -28,6 +28,7 @@ from typing import Callable, NamedTuple, Optional, Union
 import torch
 
 from ... import ops
+from ...objectives import is_transformed
 from ..cmaes import CMAESHyperparameters, cmaes_hyperparameters
 from .funccmaes import _assigned_weights, _col, _consts, _h_sig, _host_float, _tier_items
 from .fused import LazyPopulation, ask_and_evaluate
@@ -105,18 +106,25 @@ def _items(state: SepCMAESState) -> tuple:
     return batch, math.prod(batch), d
 
 
-def sepcmaes_ask(state: SepCMAESState) -> torch.Tensor:
-    """A population per item: a tensor of shape (..., popsize, D), row i of item b = m_b + s_b * z_i (on the kernels
-    fmaf(s_b, z_i, m_b), one launch of the batched sampler for all items, item b on Philox stream b)."""
+def _ask(state: SepCMAESState) -> tuple:
+    """(`sepcmaes_ask`'s population, the Philox seed of its draw on the kernels (item b on stream b), None elsewhere)."""
     batch, B, d = _items(state)
     n = state.popsize
     m, s = state.center.reshape(B, d), state.s.reshape(B, d)
+    seed = None
     if on_kernels(m, s):
         x = torch.empty(B, n, d, dtype=torch.float32, device=m.device)
-        ops.sample_batched(x, m, s, symmetric=False, seed=draw_philox_seed())
+        seed = draw_philox_seed()
+        ops.sample_batched(x, m, s, symmetric=False, seed=seed)
     else:
         x = m[:, None, :] + s[:, None, :] * torch.randn(B, n, d, dtype=m.dtype, device=m.device)
-    return x.view(batch + (n, d))
+    return x.view(batch + (n, d)), seed
+
+
+def sepcmaes_ask(state: SepCMAESState) -> torch.Tensor:
+    """A population per item: a tensor of shape (..., popsize, D), row i of item b = m_b + s_b * z_i (on the kernels
+    fmaf(s_b, z_i, m_b), one launch of the batched sampler for all items, item b on Philox stream b)."""
+    return _ask(state)[0]
 
 
 def sepcmaes_ask_and_evaluate(state: SepCMAESState, *, objective: Callable, lazy: bool = False) -> tuple:
@@ -127,12 +135,17 @@ def sepcmaes_ask_and_evaluate(state: SepCMAESState, *, objective: Callable, lazy
     under the same torch.manual_seed the stored population is the one `sepcmaes_ask` would return.  `lazy=True` does not store it:
     `values` is then a `LazyPopulation`, which `sepcmaes_tell` takes in place of the tensor.  Otherwise this is `sepcmaes_ask`
     followed by `objective(values)`, and `lazy=True` raises ValueError.  An objective whose data has a batch shape must have the
-    state's batch shape: a CMA-ES state is not broadcast to more items."""
+    state's batch shape: a CMA-ES state is not broadcast to more items.  A FusedObjective with a transform has no fused sampler:
+    the population is stored and its kernels evaluate it, keyed with the ask's Philox draw (so a noisy one gets the noise the
+    batched sampler would give it)."""
     batch, _, _ = _items(state)
     per_item = tuple(getattr(objective, "data_batch_shape", ()))
     if per_item and per_item != batch:
         raise ValueError(f"the data of {objective!r} has batch shape {per_item}, the separable CMA-ES state {batch}: each item of the data "
                          "needs its own search (build the state with that batch shape)")
+    if is_transformed(objective) and not lazy:
+        values, seed = _ask(state)
+        return values, (objective(values) if seed is None else objective.evaluate_batched(values, seed=seed))
     return ask_and_evaluate(lambda: sepcmaes_ask(state), state.center, state.s, state.popsize, False, objective, lazy)
 
 

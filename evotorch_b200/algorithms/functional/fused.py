@@ -17,6 +17,7 @@ from typing import Callable, Optional
 import torch
 
 from ... import ops
+from ...objectives import is_transformed
 from .misc import batch_shape_of, draw_philox_seed, flat_items, on_kernels
 
 
@@ -103,6 +104,10 @@ def ask_and_evaluate(ask: Callable, center: torch.Tensor, stdev: torch.Tensor, p
     batch = data_batch(objective, batch_shape_of((center, 1), (stdev, 1)))
     if oid is None:
         if lazy:
+            if is_transformed(objective):
+                raise ValueError(f"lazy=True: {objective!r} reads the transformed row y = M (x - o), which needs the whole row; the fused "
+                                 "sampler produces a row one column group at a time, so a transformed objective evaluates stored "
+                                 "populations only (lazy=False)")
             oid = getattr(objective, "evok_objective_id", None)
             why = (f"{objective!r} has no fused kernel (use an objective of evotorch_b200.objectives or a FusedObjective)"
                    if oid is None or oid == ops.OBJ_NONE else "the centre and stdev are not float32 CUDA tensors")

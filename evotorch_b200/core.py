@@ -20,6 +20,7 @@ from typing import Any, Callable, Iterable, Optional, Union
 import torch
 
 from . import ops
+from .objectives import is_transformed
 from .tools.cloning import Clonable
 from .tools.hook import Hook
 from .tools.readonlytensor import as_read_only_tensor
@@ -115,6 +116,10 @@ class Problem(Clonable):
         # Philox counters and the gradient kernel regenerates them, so a generation needs O(N + D) memory (BASELINE config 5,
         # 1 M x 100 k = 400 GB of samples, then runs on a single GPU).  Only for built-in objectives + the Philox sampler.
         self.lazy_population = bool(lazy_population)
+        if self.lazy_population and is_transformed(objective_func):
+            raise ValueError(f"lazy_population=True: {objective_func!r} reads the transformed row y = M (x - o), which needs the whole "
+                             "row; a lazy population exists only as the fused sampler's draw, which produces a row one column group "
+                             "at a time")
 
     # ------------------------------------------------------------------ construction helpers
     def _process_bounds(self, pair) -> tuple:

@@ -36,23 +36,26 @@ constexpr int kernel_index(int family, bool sym, bool store, bool vec) {
 }
 
 // every kernel of an objective's table: the EVOK_OBJ_KERNELS of its first image, the batched samplers of its second, the
-// batched evaluation of its third
-constexpr int kImages = 3;
-constexpr int kTableKernels = EVOK_OBJ_KERNEL_EVAL_BATCHED + EVOK_OBJ_EVAL_BATCHED_KERNELS;
+// batched evaluation of its third, the transformed evaluation of its fourth
+constexpr int kImages = 4;
+constexpr int kTableKernels = EVOK_OBJ_KERNEL_TRANSFORM + EVOK_OBJ_TRANSFORM_KERNELS;
 static_assert(EVOK_OBJ_KERNEL_BATCHED == EVOK_OBJ_KERNELS, "the batched family follows the first image's kernels");
 static_assert(EVOK_OBJ_KERNEL_EVAL_BATCHED == EVOK_OBJ_KERNEL_BATCHED + EVOK_OBJ_BATCHED_KERNELS, "the batched evaluation follows the batched samplers");
+static_assert(EVOK_OBJ_KERNEL_TRANSFORM == EVOK_OBJ_KERNEL_EVAL_BATCHED + EVOK_OBJ_EVAL_BATCHED_KERNELS, "the transformed evaluation comes last");
 
 // the first table position and the number of kernels of each image
-constexpr int kImageFirst[kImages] = {0, EVOK_OBJ_KERNEL_BATCHED, EVOK_OBJ_KERNEL_EVAL_BATCHED};
-constexpr int kImageKernels[kImages] = {EVOK_OBJ_KERNELS, EVOK_OBJ_BATCHED_KERNELS, EVOK_OBJ_EVAL_BATCHED_KERNELS};
+constexpr int kImageFirst[kImages] = {0, EVOK_OBJ_KERNEL_BATCHED, EVOK_OBJ_KERNEL_EVAL_BATCHED, EVOK_OBJ_KERNEL_TRANSFORM};
+constexpr int kImageKernels[kImages] = {EVOK_OBJ_KERNELS, EVOK_OBJ_BATCHED_KERNELS, EVOK_OBJ_EVAL_BATCHED_KERNELS, EVOK_OBJ_TRANSFORM_KERNELS};
 
 static int kernel_threads(int k) {
   return (k >= EVOK_OBJ_KERNEL_EVAL && k < EVOK_OBJ_KERNEL_BATCHED) || k >= EVOK_OBJ_KERNEL_EVAL_BATCHED ? kEvalThreads : kSampleThreads;
 }
 
 // the image of a registered objective that holds kernel k: 0 = the one of evok_objective_register, 1 = the batched samplers,
-// 2 = the batched evaluation
-static int image_of(int k) { return k >= EVOK_OBJ_KERNEL_EVAL_BATCHED ? 2 : k >= EVOK_OBJ_KERNEL_BATCHED ? 1 : 0; }
+// 2 = the batched evaluation, 3 = the transformed evaluation
+static int image_of(int k) {
+  return k >= EVOK_OBJ_KERNEL_TRANSFORM ? 3 : k >= EVOK_OBJ_KERNEL_EVAL_BATCHED ? 2 : k >= EVOK_OBJ_KERNEL_BATCHED ? 1 : 0;
+}
 
 // The sampler of built-in objective OBJ with the variant bits V = sym | store << 1 | vec << 2 | push << 3 | sq << 4, if it
 // exists (the SQ sampler is plain and non-symmetric) and can be reached: EVOK_OBJ_NONE only stores samples, since
@@ -105,12 +108,14 @@ struct DeviceKernels {
   void* fn[kTableKernels] = {};
   int per_sm[kTableKernels] = {};  // resident CTAs per SM
   int sms = 0;
+  int smem_optin = 0;  // shared memory per CTA the fused transformed kernels may take (set with image 3)
 };
 
 struct Objective {
   // a registered objective's cubins and the lowered names of their kernels (in the EVOK_OBJ_KERNEL_* order): [0] from
   // evok_objective_register, [1] (the batched samplers, empty until attached) from evok_objective_register_batched, [2] (the
-  // batched evaluation, empty until attached) from evok_objective_register_eval_batched
+  // batched evaluation, empty until attached) from evok_objective_register_eval_batched; a transformed objective
+  // (evok_objective_register_transform) has [3] only
   std::vector<char> image[kImages];
   std::vector<std::string> names[kImages];
   // evok_objective_declare_data: the data names of its accumulator (0: none) and which of them are vectors of the row length
@@ -138,6 +143,7 @@ struct DriverApi {
   decltype(&cuModuleUnload) module_unload = nullptr;
   decltype(&cuOccupancyMaxActiveBlocksPerMultiprocessor) occupancy = nullptr;
   decltype(&cuLaunchKernel) launch = nullptr;
+  decltype(&cuFuncSetAttribute) func_attribute = nullptr;
 };
 static DriverApi g_driver;
 
@@ -156,7 +162,7 @@ static bool driver_api() {
   return driver_symbol("cuDeviceGet", d.device_get) && driver_symbol("cuDeviceGetAttribute", d.device_attribute) &&
          driver_symbol("cuModuleLoadData", d.module_load) && driver_symbol("cuModuleGetFunction", d.module_function) &&
          driver_symbol("cuModuleUnload", d.module_unload) && driver_symbol("cuOccupancyMaxActiveBlocksPerMultiprocessor", d.occupancy) &&
-         driver_symbol("cuLaunchKernel", d.launch);
+         driver_symbol("cuLaunchKernel", d.launch) && driver_symbol("cuFuncSetAttribute", d.func_attribute);
 }
 
 static std::mutex g_objective_mutex;
@@ -259,6 +265,11 @@ static int load_module(const Objective& obj, int part, int dev, DeviceKernels& d
     }
     d.fn[k] = fn;
     if (api.occupancy(&d.per_sm[k], fn, kernel_threads(k), 0) != CUDA_SUCCESS || d.per_sm[k] <= 0) d.per_sm[k] = 4;
+  }
+  if (part == 3) {  // the fused transformed kernels may take the device's opt-in shared memory per CTA
+    if (api.device_attribute(&d.smem_optin, CU_DEVICE_ATTRIBUTE_MAX_SHARED_MEMORY_PER_BLOCK_OPTIN, cu_dev) != CUDA_SUCCESS) d.smem_optin = 48 * 1024;
+    for (int v = 0; v < 2; ++v)
+      api.func_attribute(static_cast<CUfunction>(d.fn[EVOK_OBJ_KERNEL_TRANSFORM + v]), CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, d.smem_optin);
   }
   if (d.sms <= 0) d.sms = kNumSMs;
   d.state[part] = 1;
@@ -648,5 +659,172 @@ extern "C" EVOK_API int evok_eval_batched(int objective, const float* X, int64_t
     for (int i = 0; i < EVOK_MAX_DATA; ++i) dc.p[i] += b0 * dc.item_stride[i];
     void* args[] = {&Xc, &item_stride_x, &ldx, &n_rows, &D, &fc, &dc, &kc};
     return launch(data.base, c, args, (cudaStream_t)stream, nb);
+  });
+}
+
+// ------------------------------------------------------------------------------------------------
+// Transformed evaluation (evok_eval_transform_batched): the terms read y = M (x - o) per item.  Up to EVOK_TRANSFORM_FUSED_MAX_D
+// columns one fused launch per 65535 items computes y on the CUDA cores in shared memory (eval_transform_fused_kernel); above it
+// each item chunk is a fixed number of launches: x - o into the workspace (transform_center_kernel), the batched 3xTF32 GEMM
+// (evok_gemm_nt_batched) writes y next to it, and eval_transform_kernel folds the x and y rows.
+// ------------------------------------------------------------------------------------------------
+// The cutoff: both paths timed at the same D on the H100 (scripts/transformed_cutoff_sweep.py, DESIGN.md) cross between D = 96
+// and 112 at 1024 items.  Its upper end is the shared memory of one CTA (M and two rows), D = 236; the sweep builds 0 and 236.
+#ifndef EVOK_TRANSFORM_FUSED_MAX_D
+#define EVOK_TRANSFORM_FUSED_MAX_D 96
+#endif
+static_assert(EVOK_TRANSFORM_FUSED_MAX_D >= 0 && evok::transform_smem_floats(EVOK_TRANSFORM_FUSED_MAX_D, 2) * 4 <= 227 * 1024,
+              "the fused transformed kernel stages M in the 227 KB of shared memory a CTA can take on sm_90");
+
+namespace evok {
+
+constexpr int64_t kTransformTileRows = 32;                  // rows of one fused tile at most (even)
+constexpr size_t kTransformChunkBytes = size_t(256) << 20;  // x - o and y of one item chunk on the GEMM path, at most (>= one item)
+
+// out[b][r][k] = X[b][r][k] - o[b][k] for the n_rows x D rows of item b = blockIdx.y (out: item pitch n_rows * ld, row pitch ld)
+__global__ void transform_center_kernel(const float* __restrict__ X, int64_t item_stride_x, int64_t ldx, const float* __restrict__ o,
+                                        int64_t item_stride_o, int64_t n_rows, int64_t D, float* __restrict__ out, int64_t ld) {
+  const int64_t item = blockIdx.y;
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_rows * D) return;
+  const int64_t r = i / D, k = i - r * D;
+  out[(item * n_rows + r) * ld + k] = X[item * item_stride_x + r * ldx + k] - __ldg(o + item * item_stride_o + k);
+}
+
+static bool transform_fused(int64_t D) { return D <= EVOK_TRANSFORM_FUSED_MAX_D; }
+
+// the items of one chunk of the GEMM path: as many as keep x - o and y within kTransformChunkBytes, at least 1, at most kMaxGridY
+static int64_t transform_chunk(int64_t n_items, int64_t n_rows, int64_t D) {
+  const int64_t per_item = 2 * n_rows * round4(D) * (int64_t)sizeof(float);
+  int64_t c = (int64_t)kTransformChunkBytes / per_item;
+  if (c > n_items) c = n_items;
+  if (c > kMaxGridY) c = kMaxGridY;
+  return c < 1 ? 1 : c;
+}
+
+static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+// the workspace of a call: none on the fused path; x - o and y of one chunk, then the GEMM's own workspace, on the GEMM path
+static size_t transform_ws(const float* M, int64_t item_stride_m, int64_t n_items, int64_t n_rows, int64_t D) {
+  if (transform_fused(D) || n_items <= 0 || n_rows <= 0 || D <= 0) return 0;
+  const int64_t chunk = transform_chunk(n_items, n_rows, D), ld = round4(D);
+  const size_t half = align256((size_t)(chunk * n_rows * ld) * sizeof(float));
+  const float* xo = reinterpret_cast<const float*>(uintptr_t(256));  // where x - o goes: 256-byte aligned, row pitch ld
+  return 256 + 2 * half + evok_gemm_nt_batched_workspace_bytes(xo, ld, n_rows * ld, M, D, item_stride_m, chunk, n_rows, D, D);
+}
+
+}  // namespace evok
+
+extern "C" EVOK_API int evok_objective_register_transform(const void* cubin, size_t bytes, const char* const* kernel_names_host, int n_kernels,
+                                                          int* id_out_host) {
+  if (!cubin || !kernel_names_host || !id_out_host) return EVOK_E_NULLPTR;
+  if (bytes == 0 || n_kernels != EVOK_OBJ_TRANSFORM_KERNELS) return EVOK_E_BADSIZE;
+  for (int k = 0; k < n_kernels; ++k)
+    if (!kernel_names_host[k]) return EVOK_E_NULLPTR;
+  std::lock_guard<std::mutex> lock(g_objective_mutex);
+  const int n = g_user_count.load(std::memory_order_relaxed);
+  if (n >= EVOK_OBJ_USER_CAPACITY) return EVOK_E_BADSIZE;
+  Objective* obj = new Objective;
+  obj->image[3].assign(static_cast<const char*>(cubin), static_cast<const char*>(cubin) + bytes);
+  obj->names[3].assign(kernel_names_host, kernel_names_host + n_kernels);
+  g_user[n] = obj;
+  g_user_count.store(n + 1, std::memory_order_release);
+  *id_out_host = EVOK_OBJ_USER_BASE + n;
+  return 0;
+}
+
+extern "C" EVOK_API size_t evok_eval_transform_workspace_bytes(const float* M, int64_t item_stride_m, int64_t n_items, int64_t n_rows, int64_t D) {
+  return transform_ws(M, item_stride_m, n_items, n_rows, D);
+}
+
+extern "C" EVOK_API int evok_eval_transform_batched(int objective, const float* X, int64_t item_stride_x, int64_t ldx, const float* M,
+                                                    int64_t item_stride_m, const float* o, int64_t item_stride_o, int64_t n_items, int64_t n_rows,
+                                                    int64_t D, uint64_t seed, uint64_t stream_id0, void* ws, size_t ws_bytes, float* f,
+                                                    void* stream) {
+  if (!X || !M || !o || !f) return EVOK_E_NULLPTR;
+  const int base = base_of(objective);
+  if ((base <= EVOK_OBJ_NONE || base >= EVOK_OBJ_COUNT) && !is_user(base)) return EVOK_E_BADENUM;
+  if (n_items < 0 || n_rows < 0 || item_stride_x < 0 || item_stride_m < 0 || item_stride_o < 0 || D <= 0 || ldx < D ||
+      items_differ(objective, n_items))
+    return EVOK_E_BADSIZE;
+  if (!is_user(base) || lacks_image(base, 3)) return EVOK_E_NOKERNEL;
+  LaunchData data;
+  if (const int rc = bind_data(objective, D, n_items, &data)) return rc;
+  if (n_items == 0 || n_rows == 0) return 0;
+  const size_t need = transform_ws(M, item_stride_m, n_items, n_rows, D);
+  if (need > 0 && !ws) return EVOK_E_NULLPTR;
+  if (ws_bytes < need) return EVOK_E_BADSIZE;
+  const DeviceKernels* d = nullptr;
+  if (const int rc = device_kernels(data.base, 3, &d)) return rc;
+  const bool vec = D % 4 == 0 && aligned16(X) && ldx % 4 == 0 && item_stride_x % 4 == 0 && data.vec_ok;
+  // one key for all items: item b draws its noise on stream word (stream_id0 + b), chunk b0 from stream_lo + b0
+  const EvalKey noise{is_noisy(base) ? make_philox_key(seed, stream_id0) : PhiloxKey{}, nullptr, 0};
+  const cudaStream_t st = (cudaStream_t)stream;
+  auto chunk_args = [&](int64_t b0, EvalKey& kc, const float*& Xc, float*& fc, DataBinding& dc) {
+    kc = noise;
+    kc.key.stream_lo += (uint32_t)b0;
+    Xc = X + b0 * item_stride_x;
+    fc = f + b0 * n_rows;
+    dc = data.binding;
+    for (int i = 0; i < EVOK_MAX_DATA; ++i) dc.p[i] += b0 * dc.item_stride[i];
+  };
+  if (transform_fused(D)) {
+    const CUfunction fn = static_cast<CUfunction>(d->fn[EVOK_OBJ_KERNEL_TRANSFORM + (vec ? 1 : 0)]);
+    int64_t tile = n_rows + (n_rows & 1) < kTransformTileRows ? n_rows + (n_rows & 1) : kTransformTileRows;
+    while (tile > 2 && transform_smem_floats(D, tile) * (int64_t)sizeof(float) > d->smem_optin) tile -= 2;
+    const size_t smem = (size_t)transform_smem_floats(D, tile) * sizeof(float);
+    if (smem > (size_t)d->smem_optin) return EVOK_E_BADSIZE;
+    int per_sm = 0;
+    if (g_driver.occupancy(&per_sm, fn, kEvalThreads, smem) != CUDA_SUCCESS || per_sm <= 0) per_sm = 1;
+    const int64_t tiles = (n_rows + tile - 1) / tile;
+    return for_item_chunks(n_items, kMaxGridY, [&](int64_t b0, int64_t nb) {
+      EvalKey kc;
+      const float* Xc;
+      float* fc;
+      DataBinding dc;
+      chunk_args(b0, kc, Xc, fc, dc);
+      const float* Mc = M + b0 * item_stride_m;
+      const float* oc = o + b0 * item_stride_o;
+      int64_t g = (int64_t)per_sm * d->sms / nb;
+      if (g > tiles) g = tiles;
+      if (g < 1) g = 1;
+      void* args[] = {&Xc, &item_stride_x, &ldx, &Mc, &item_stride_m, &oc, &item_stride_o, &n_rows, &D, &tile, &fc, &dc, &kc};
+      const CUresult r = g_driver.launch(fn, (unsigned)g, (unsigned)nb, 1, kEvalThreads, 1, 1, (unsigned)smem, (CUstream)st, args, nullptr);
+      if (r != CUDA_SUCCESS) return (int)r;
+      count_launches(1);
+      return 0;
+    });
+  }
+  const int k = EVOK_OBJ_KERNEL_TRANSFORM + 2 + (vec ? 1 : 0);
+  const CUfunction fn = static_cast<CUfunction>(d->fn[k]);
+  int64_t ld = round4(D), item_stride_y = n_rows * ld;
+  const int64_t chunk = transform_chunk(n_items, n_rows, D);
+  char* w = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(ws) + 255) & ~(uintptr_t)255);
+  const size_t half = align256((size_t)(chunk * n_rows * ld) * sizeof(float));
+  float* xo = reinterpret_cast<float*>(w);
+  const float* Y = reinterpret_cast<const float*>(w + half);
+  void* gws = w + 2 * half;
+  const size_t gws_bytes = ws_bytes - (size_t)(static_cast<char*>(gws) - static_cast<char*>(ws));
+  const int64_t ctas_needed = (n_rows + kEvalThreads / 32 - 1) / (kEvalThreads / 32);
+  return for_item_chunks(n_items, chunk, [&](int64_t b0, int64_t nb) {
+    EvalKey kc;
+    const float* Xc;
+    float* fc;
+    DataBinding dc;
+    chunk_args(b0, kc, Xc, fc, dc);
+    transform_center_kernel<<<dim3((unsigned)((n_rows * D + 255) / 256), (unsigned)nb), 256, 0, st>>>(Xc, item_stride_x, ldx, o + b0 * item_stride_o,
+                                                                                                        item_stride_o, n_rows, D, xo, ld);
+    EVOK_CHECK_LAUNCH();
+    if (const int rc = evok_gemm_nt_batched(xo, ld, item_stride_y, M + b0 * item_stride_m, D, item_stride_m, nb, n_rows, D, D, const_cast<float*>(Y), ld,
+                                            item_stride_y, nullptr, 0, 0, nullptr, 0, nullptr, 0, gws, gws_bytes, st))
+      return rc;
+    int64_t g = (int64_t)d->per_sm[k] * d->sms / nb;
+    if (g > ctas_needed) g = ctas_needed;
+    if (g < 1) g = 1;
+    void* args[] = {&Xc, &item_stride_x, &ldx, &Y, &item_stride_y, &ld, &n_rows, &D, &fc, &dc, &kc};
+    const CUresult r = g_driver.launch(fn, (unsigned)g, (unsigned)nb, 1, kEvalThreads, 1, 1, 0, (CUstream)st, args, nullptr);
+    if (r != CUDA_SUCCESS) return (int)r;
+    count_launches(1);
+    return 0;
   });
 }

@@ -263,6 +263,9 @@ __device__ __forceinline__ void st_stream1(float* p, float a) {
 //   kNoise = true, kDraws <= 4, kNormalDraws (rand() / randn(): kDraws occurrences in the element terms, bit k of kNormalDraws
 //   set where occurrence k is randn(), and up to 4 in `value`):
 //     finish(D, key, stream_word, row) : row = the global row index; `value` draws with value_rand / value_randn.
+//   kTransform = true (terms of the transformed row y = M (x - o)): every fold takes the entry of y at the same column after
+//   that of x, add(x, y, j, ...), add_pair(x, xn, y, yn, j, ...), running(x, y, j, ...).  The kernels carry a column as XY (ColVal)
+//   and only the transformed evaluation kernels below instantiate such an accumulator.
 // An accumulator with data vectors or element draws takes the column entries of a fold after j (DataCols: d[i] = vec[i][j],
 // then d[kVectors + k] = element draw k at column j), in every fold, whether its terms use them or not:
 //   add(x, j, d[, r]),  running(x, j, d, h),  add_pair(x, xn, j, d, dn)  with dn the entries at column j + 1.
@@ -363,6 +366,8 @@ template <typename A> constexpr auto data_marker(int) -> decltype(Marker{A::kDat
 template <typename A> constexpr Marker data_marker(long) { return {}; }
 template <typename A> constexpr auto noise_marker(int) -> decltype(Marker{A::kNoise}) { return {A::kNoise, A::kDraws, A::kNormalDraws}; }
 template <typename A> constexpr Marker noise_marker(long) { return {}; }
+template <typename A> constexpr auto transform_marker(int) -> decltype(Marker{A::kTransform}) { return {A::kTransform}; }
+template <typename A> constexpr Marker transform_marker(long) { return {}; }
 // ObjAcc<EVOK_OBJ_NONE> samples without evaluating
 template <typename A> constexpr bool sample_only(const A*) { return false; }
 constexpr bool sample_only(const ObjAcc<EVOK_OBJ_NONE>*) { return true; }
@@ -375,6 +380,13 @@ template <typename T, typename F>
 struct Pick<true, T, F> {
   using type = T;
 };
+
+// one column of a row and of its transformed row y = M (x - o), for an accumulator with kTransform
+struct XY {
+  float x, y;
+};
+__device__ __forceinline__ float shfl_col(float v, int src) { return __shfl_sync(0xffffffffu, v, src); }
+__device__ __forceinline__ XY shfl_col(XY v, int src) { return {__shfl_sync(0xffffffffu, v.x, src), __shfl_sync(0xffffffffu, v.y, src)}; }
 
 // Every compile-time fact about an accumulator that the kernels use.  Each feature's code is under `if constexpr` on its
 // fact, so the kernels of an accumulator without it are those of one written without the feature.
@@ -391,6 +403,9 @@ struct AccTraits {
   static constexpr bool kNoise = kNoiseMark.on;
   static constexpr int kDraws = kNoise ? kNoiseMark.n : 0;  // element draws (those of `value` are the accumulator's own)
   static constexpr unsigned kNormal = kNoise ? kNoiseMark.mask : 0u;
+  static constexpr bool kTransform = transform_marker<Acc>(0).on;
+  // what a fold takes for one column: its x, or (x, y) with a transform
+  using ColVal = typename Pick<kTransform, XY, float>::type;
   // element draws: the + and - rows of a direction fold with their own column entries
   static constexpr bool kElementDraws = kDraws > 0;
   // the folds take column entries (data vectors, then element draws), kSlots of them per column
@@ -417,20 +432,32 @@ __device__ __forceinline__ Acc acc_make(int64_t D, const Arg& data) {
   if constexpr (AccTraits<Acc>::kData) return Acc(D, data);
   else return Acc(D);
 }
+// x: the column's ColVal, (x, y) with a transform.
 template <typename Acc, typename... Run>
-__device__ __forceinline__ void acc_add(Acc& acc, float x, int64_t j, const float (&d)[AccTraits<Acc>::kSlots], const Run&... r) {
-  if constexpr (AccTraits<Acc>::kCols) acc.add(x, j, d, r...);
+__device__ __forceinline__ void acc_add(Acc& acc, typename AccTraits<Acc>::ColVal x, int64_t j, const float (&d)[AccTraits<Acc>::kSlots],
+                                        const Run&... r) {
+  if constexpr (AccTraits<Acc>::kTransform) {
+    if constexpr (AccTraits<Acc>::kCols) acc.add(x.x, x.y, j, d, r...);
+    else acc.add(x.x, x.y, j, r...);
+  } else if constexpr (AccTraits<Acc>::kCols) acc.add(x, j, d, r...);
   else acc.add(x, j, r...);
 }
 template <typename Acc>
-__device__ __forceinline__ void acc_pair(Acc& acc, float x, float xn, int64_t j, const float (&d)[AccTraits<Acc>::kSlots],
-                                         const float (&dn)[AccTraits<Acc>::kSlots]) {
-  if constexpr (AccTraits<Acc>::kCols) acc.add_pair(x, xn, j, d, dn);
+__device__ __forceinline__ void acc_pair(Acc& acc, typename AccTraits<Acc>::ColVal x, typename AccTraits<Acc>::ColVal xn, int64_t j,
+                                         const float (&d)[AccTraits<Acc>::kSlots], const float (&dn)[AccTraits<Acc>::kSlots]) {
+  if constexpr (AccTraits<Acc>::kTransform) {
+    if constexpr (AccTraits<Acc>::kCols) acc.add_pair(x.x, xn.x, x.y, xn.y, j, d, dn);
+    else acc.add_pair(x.x, xn.x, x.y, xn.y, j);
+  } else if constexpr (AccTraits<Acc>::kCols) acc.add_pair(x, xn, j, d, dn);
   else acc.add_pair(x, xn, j);
 }
 template <typename Acc, int R>
-__device__ __forceinline__ void acc_running(Acc& acc, float x, int64_t j, const float (&d)[AccTraits<Acc>::kSlots], float (&h)[R]) {
-  if constexpr (AccTraits<Acc>::kCols) acc.running(x, j, d, h);
+__device__ __forceinline__ void acc_running(Acc& acc, typename AccTraits<Acc>::ColVal x, int64_t j, const float (&d)[AccTraits<Acc>::kSlots],
+                                            float (&h)[R]) {
+  if constexpr (AccTraits<Acc>::kTransform) {
+    if constexpr (AccTraits<Acc>::kCols) acc.running(x.x, x.y, j, d, h);
+    else acc.running(x.x, x.y, j, h);
+  } else if constexpr (AccTraits<Acc>::kCols) acc.running(x, j, d, h);
   else acc.running(x, j, h);
 }
 // key: null for an accumulator without noise (eval_kernel has no draw then)
@@ -444,7 +471,7 @@ __device__ __forceinline__ float acc_finish(Acc& acc, int64_t D, const PhiloxKey
 // all columns of the previous steps
 template <typename Acc>
 struct StepCarry {
-  float pair = 0.f;
+  typename AccTraits<Acc>::ColVal pair{};
   float run[AccTraits<Acc>::kRunningSums > 0 ? AccTraits<Acc>::kRunningSums : 1] = {};
 };
 
@@ -507,11 +534,11 @@ struct DataCols {
 // must call it on every step, in the same order (it shuffles); a column's left neighbour is always in the previous lane
 // or the previous step because each step covers 32 * N consecutive columns.
 // dc: the column entries of the same columns (with `left` loaded when j > 0).
-template <int N, typename Acc>
-__device__ __forceinline__ void fold_pairs(Acc& acc, const float (&v)[N], int64_t j, int n_valid, float& carry, const DataCols<Acc, N>& dc) {
+template <int N, typename Acc, typename V>
+__device__ __forceinline__ void fold_pairs(Acc& acc, const V (&v)[N], int64_t j, int n_valid, V& carry, const DataCols<Acc, N>& dc) {
   const int lane = threadIdx.x & 31;
-  const float rot = __shfl_sync(0xffffffffu, v[N - 1], (lane + 31) & 31);  // lane 0 receives lane 31's: next step's carry
-  const float left = lane == 0 ? carry : rot;
+  const V rot = shfl_col(v[N - 1], (lane + 31) & 31);  // lane 0 receives lane 31's: next step's carry
+  const V left = lane == 0 ? carry : rot;
   carry = rot;
   if (n_valid > 0 && j > 0) acc_pair(acc, left, v[0], j - 1, dc.left, dc.v[0]);
 #pragma unroll
@@ -525,8 +552,8 @@ __device__ __forceinline__ void fold_pairs(Acc& acc, const float (&v)[N], int64_
 // p_c, and takes the exclusive scan e of the lane totals p_{N-1} across the warp (a Kogge-Stone scan with __shfl_up_sync, five
 // rounds, then one shift); then c_{j+c} = p_c + (e + carry), where carry is the sum of all earlier steps of the row, and the
 // carry advances by the step total, the inclusive scan of lane 31.  Then each column's element terms are folded with its c.
-template <int N, typename Acc, int R>
-__device__ __forceinline__ void fold_running(Acc& acc, const float (&v)[N], int64_t j, int n_valid, float (&carry)[R], const DataCols<Acc, N>& dc) {
+template <int N, typename Acc, typename V, int R>
+__device__ __forceinline__ void fold_running(Acc& acc, const V (&v)[N], int64_t j, int n_valid, float (&carry)[R], const DataCols<Acc, N>& dc) {
   const int lane = threadIdx.x & 31;
   float p[N][R];
 #pragma unroll
@@ -560,8 +587,8 @@ __device__ __forceinline__ void fold_running(Acc& acc, const float (&v)[N], int6
 
 // the element folds and pair folds of one warp step (see fold_pairs and fold_running): the element folds of an accumulator
 // without running sums have been made by the caller already
-template <int N, typename Acc>
-__device__ __forceinline__ void fold_step(Acc& acc, const float (&v)[N], int64_t j, int n_valid, StepCarry<Acc>& carry, const DataCols<Acc, N>& dc) {
+template <int N, typename Acc, typename V>
+__device__ __forceinline__ void fold_step(Acc& acc, const V (&v)[N], int64_t j, int n_valid, StepCarry<Acc>& carry, const DataCols<Acc, N>& dc) {
   if constexpr (AccTraits<Acc>::kRunning) fold_running<N>(acc, v, j, n_valid, carry.run, dc);
   if constexpr (AccTraits<Acc>::kPairs) fold_pairs<N>(acc, v, j, n_valid, carry.pair, dc);
 }
@@ -789,6 +816,136 @@ __global__ void __launch_bounds__(kSampleThreads, AccTraits<Acc>::kSampleMinBloc
 
 constexpr int kEvalThreads = 256;
 
+// The columns of one row of an accumulator with kTransform as fold_row takes them: a row x of X (global memory, streaming loads)
+// and its transformed row y (shared memory or a workspace, 16-byte aligned where load4 reads it)
+struct RowColsXY {
+  const float* x;
+  const float* y;
+  __device__ __forceinline__ void load4(int64_t j, XY (&v)[4]) const {
+    const float4 a = ld_stream4(x + j);
+    const float4 b = *reinterpret_cast<const float4*>(y + j);
+    v[0] = {a.x, b.x}; v[1] = {a.y, b.y}; v[2] = {a.z, b.z}; v[3] = {a.w, b.w};
+  }
+  __device__ __forceinline__ XY load1(int64_t j) const { return {ld_stream1(x + j), y[j]}; }
+};
+
+// The fitness of row r (D columns, read through the loader make_row() returns; every lane gets it), with the data binding `data`
+// and, for an accumulator with noise, global row row0 + r of the draw (key, stream word sw); key is null for every other
+// accumulator.  eval_row below, with the columns of a loader, in its order on every path: the body of the transformed evaluation
+// kernels, which therefore give the bits eval_row gives the same (x, y) columns.  (eval_row keeps its own body: the built-in
+// kernels of libevok are compiled from it as they were.)  A change to the fold order of one must be made in the other; the GPU
+// test of permutation transforms (tests/test_transformed_objective_gpu.py) compares their bits.
+template <typename Acc, bool VEC, typename MakeRow>
+__device__ __forceinline__ float fold_row(int lane, const MakeRow& make_row, int64_t r, int64_t D, const typename AccTraits<Acc>::DataArg& data,
+                                          const PhiloxKey* key, uint32_t sw, int64_t row0) {
+  using T = AccTraits<Acc>;
+  using V = typename T::ColVal;
+  Acc acc = acc_make<Acc>(D, data);
+  const auto row = make_row();
+  if constexpr (T::kWarpSteps) {
+    // warp-uniform steps (fold_step shuffles); per lane the groups, element adds, running sums and pair folds of
+    // sample_eval_kernel's VEC path in the same order, so both kernels give the same fitness bit for bit on the same X
+    constexpr bool kFoldNow = !T::kRunning;
+    StepCarry<Acc> carry;
+    if (VEC) {
+      const int64_t nq = D >> 2;
+      int64_t b = 0;
+      for (; b + 128 <= nq; b += 128) {
+        const int64_t q = b + lane;
+        V g[4][4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) row.load4(4 * (q + 32 * k), g[k]);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const int64_t jk = 4 * (q + 32 * k);
+          const V (&v)[4] = g[k];
+          DataCols<Acc, 4> dc;
+          dc.load4(acc, jk);
+          if constexpr (T::kElementDraws) dc.draw4(*key, sw, row0 + r, (uint32_t)(q + 32 * k));
+          if constexpr (T::kPairs)
+            if (jk > 0) dc.load_left(acc, jk);
+          if constexpr (kFoldNow) {
+            acc_add(acc, v[0], jk, dc.v[0]); acc_add(acc, v[1], jk + 1, dc.v[1]); acc_add(acc, v[2], jk + 2, dc.v[2]); acc_add(acc, v[3], jk + 3, dc.v[3]);
+          }
+          fold_step<4>(acc, v, jk, 4, carry, dc);
+        }
+      }
+      for (; b < nq; b += 32) {
+        const int64_t q = b + lane;
+        const bool active = q < nq;
+        V v[4] = {};
+        if (active) row.load4(4 * q, v);
+        const int64_t ja = 4 * q;
+        DataCols<Acc, 4> dc;
+        if (active) {
+          dc.load4(acc, ja);
+          if constexpr (T::kElementDraws) dc.draw4(*key, sw, row0 + r, (uint32_t)q);
+          if constexpr (T::kPairs)
+            if (ja > 0) dc.load_left(acc, ja);
+          if constexpr (kFoldNow) {
+            acc_add(acc, v[0], ja, dc.v[0]); acc_add(acc, v[1], ja + 1, dc.v[1]); acc_add(acc, v[2], ja + 2, dc.v[2]); acc_add(acc, v[3], ja + 3, dc.v[3]);
+          }
+        }
+        fold_step<4>(acc, v, ja, active ? 4 : 0, carry, dc);
+      }
+    } else {
+      for (int64_t b = 0; b < D; b += 32) {
+        const int64_t j = b + lane;
+        const bool active = j < D;
+        V v[1] = {};
+        if (active) v[0] = row.load1(j);
+        DataCols<Acc, 1> dc;
+        if (active) {
+          dc.load1(acc, j, 0);
+          if constexpr (T::kElementDraws) dc.draw1(*key, sw, row0 + r, j, 0);
+          if constexpr (T::kPairs)
+            if (j > 0) dc.load_left(acc, j);
+          if constexpr (kFoldNow) acc_add(acc, v[0], j, dc.v[0]);
+        }
+        fold_step<1>(acc, v, j, active ? 1 : 0, carry, dc);
+      }
+    }
+  } else if (VEC) {
+    const int64_t nq = D >> 2;
+    int64_t q = lane;
+    // 4 independent 128-bit loads in flight per lane
+    for (; q + 96 < nq; q += 128) {
+      V a[4], b[4], c[4], d[4];
+      row.load4(4 * q, a); row.load4(4 * (q + 32), b); row.load4(4 * (q + 64), c); row.load4(4 * (q + 96), d);
+      const int64_t ja = 4 * q, jb = 4 * (q + 32), jc = 4 * (q + 64), jd = 4 * (q + 96);
+      DataCols<Acc, 4> da, db, dc, dd;
+      da.load4(acc, ja); db.load4(acc, jb); dc.load4(acc, jc); dd.load4(acc, jd);
+      if constexpr (T::kElementDraws) {
+        const uint64_t row = row0 + r;
+        da.draw4(*key, sw, row, (uint32_t)q); db.draw4(*key, sw, row, (uint32_t)(q + 32));
+        dc.draw4(*key, sw, row, (uint32_t)(q + 64)); dd.draw4(*key, sw, row, (uint32_t)(q + 96));
+      }
+      acc_add(acc, a[0], ja, da.v[0]); acc_add(acc, a[1], ja + 1, da.v[1]); acc_add(acc, a[2], ja + 2, da.v[2]); acc_add(acc, a[3], ja + 3, da.v[3]);
+      acc_add(acc, b[0], jb, db.v[0]); acc_add(acc, b[1], jb + 1, db.v[1]); acc_add(acc, b[2], jb + 2, db.v[2]); acc_add(acc, b[3], jb + 3, db.v[3]);
+      acc_add(acc, c[0], jc, dc.v[0]); acc_add(acc, c[1], jc + 1, dc.v[1]); acc_add(acc, c[2], jc + 2, dc.v[2]); acc_add(acc, c[3], jc + 3, dc.v[3]);
+      acc_add(acc, d[0], jd, dd.v[0]); acc_add(acc, d[1], jd + 1, dd.v[1]); acc_add(acc, d[2], jd + 2, dd.v[2]); acc_add(acc, d[3], jd + 3, dd.v[3]);
+    }
+    for (; q < nq; q += 32) {
+      V a[4];
+      row.load4(4 * q, a);
+      const int64_t ja = 4 * q;
+      DataCols<Acc, 4> da;
+      da.load4(acc, ja);
+      if constexpr (T::kElementDraws) da.draw4(*key, sw, row0 + r, (uint32_t)q);
+      acc_add(acc, a[0], ja, da.v[0]); acc_add(acc, a[1], ja + 1, da.v[1]); acc_add(acc, a[2], ja + 2, da.v[2]); acc_add(acc, a[3], ja + 3, da.v[3]);
+    }
+  } else {
+    for (int64_t j = lane; j < D; j += 32) {
+      DataCols<Acc, 1> dc;
+      dc.load1(acc, j, 0);
+      if constexpr (T::kElementDraws) dc.draw1(*key, sw, row0 + r, j, 0);
+      acc_add(acc, row.load1(j), j, dc.v[0]);
+    }
+  }
+  return acc_finish(acc, D, key, sw, (uint64_t)(row0 + r));
+}
+
+// eval_row's fold order is also that of fold_row above (the transformed kernels): change both together.
 // One row of the evaluation kernels: the fitness of row r of X (row pitch ldx, D columns; every lane gets it), with the data
 // binding `data` and, for an accumulator with noise, global row row0 + r of the draw (key, stream word sw); key is null for every
 // other accumulator.  The body of eval_kernel and of eval_batched_kernel, so both give the same bits for the same row, draw and
@@ -950,6 +1107,116 @@ __global__ void __launch_bounds__(kEvalThreads, AccTraits<Acc>::kEvalMinBlocks)
   const int64_t gw = (int64_t)blockIdx.x * (kEvalThreads / 32) + (threadIdx.x >> 5);
   for (int64_t r = gw; r < n_rows; r += warps_total) {
     const float v = eval_row<Acc, VEC>(lane, X, ldx, r, D, my_data, key, sw, 0);
+    if (lane == 0) f[r] = v;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Transformed evaluation (evok_eval_transform_batched): the terms of an accumulator with kTransform read y = M (x - o) of each row,
+// with M (D x D, row-major, row pitch D) and o (D) of the row's item at their item strides (0: shared by all items).  Each x_k - o_k
+// is rounded to float32 first, so a row equal to o has y = 0 exactly whatever M is.  Item b of a launch is blockIdx.y and draws
+// its noise as eval_batched_kernel's item b does (stream word key.stream_lo + b, global row = its row).
+// ------------------------------------------------------------------------------------------------
+// The shared-memory layout of the fused kernel: M with an odd row pitch (column reads of 32 rows hit 32 banks), o, then the tile's
+// x - o and y, rows at a pitch of round4(D) floats (16-byte aligned rows for fold_row's 16-byte loads).
+__host__ __device__ constexpr int64_t transform_pitch_m(int64_t D) { return D | 1; }
+__host__ __device__ constexpr int64_t round4(int64_t n) { return (n + 3) & ~int64_t(3); }
+__host__ __device__ constexpr int64_t transform_smem_floats(int64_t D, int64_t tile_rows) {
+  return round4(D * transform_pitch_m(D)) + round4(D) + 2 * tile_rows * round4(D);
+}
+
+// The small-D path, one launch: CTA (x, b) stages item b's M and o, then for each tile of `tile_rows` rows (tiles strided over
+// grid x) stages x - o, computes y_j = sum_{k=0}^{D-1} M[j][k] (x_k - o_k) as one FP32 FMA chain in increasing k from 0 (a thread
+// per column and pair of rows), and folds each row's (x, y) with one warp (fold_row: the order of eval_row).  With M a permutation
+// and o = 0 the y of a finite row are its permuted entries exactly, so the fitness is the bits of eval_batched_kernel on the
+// permuted rows, on the same path.  Dynamic shared memory: transform_smem_floats(D, tile_rows) floats, tile_rows even.
+template <typename Acc, bool VEC>
+__global__ void __launch_bounds__(kEvalThreads, 1)
+    eval_transform_fused_kernel(const float* __restrict__ X, int64_t item_stride_x, int64_t ldx, const float* __restrict__ M,
+                                int64_t item_stride_m, const float* __restrict__ o, int64_t item_stride_o, int64_t n_rows, int64_t D,
+                                int64_t tile_rows, float* __restrict__ f, const typename AccTraits<Acc>::DataArg data,
+                                const typename AccTraits<Acc>::EvalArg noise) {
+  extern __shared__ __align__(16) float smem[];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int64_t item = blockIdx.y;
+  X += item * item_stride_x;
+  M += item * item_stride_m;
+  o += item * item_stride_o;
+  f += item * n_rows;
+  const PhiloxKey* key = nullptr;
+  uint32_t sw = 0u;
+  if constexpr (AccTraits<Acc>::kNoise) {
+    key = &noise.key;
+    sw = noise.key.stream_lo + (uint32_t)item;
+  }
+  const typename AccTraits<Acc>::DataArg my_data = item_data(data, item);
+  const int64_t pm = transform_pitch_m(D), p4 = round4(D);
+  float* sM = smem;
+  float* so = smem + round4(D * pm);
+  float* sxo = so + p4;
+  float* sy = sxo + tile_rows * p4;
+  for (int64_t i = tid; i < D * D; i += kEvalThreads) {
+    const int64_t r = i / D;
+    sM[r * pm + (i - r * D)] = __ldg(M + i);
+  }
+  for (int64_t i = tid; i < D; i += kEvalThreads) so[i] = __ldg(o + i);
+  for (int64_t t0 = (int64_t)blockIdx.x * tile_rows; t0 < n_rows; t0 += (int64_t)gridDim.x * tile_rows) {
+    const int64_t rows = n_rows - t0 < tile_rows ? n_rows - t0 : tile_rows;
+    __syncthreads();  // M and o are staged, and the previous tile's folds have read their y
+    for (int64_t i = tid; i < rows * D; i += kEvalThreads) {
+      const int64_t r = i / D, k = i - r * D;
+      sxo[r * p4 + k] = X[(t0 + r) * ldx + k] - so[k];
+    }
+    __syncthreads();
+    const int64_t pairs = (rows + 1) >> 1;
+    for (int64_t i = tid; i < pairs * D; i += kEvalThreads) {
+      const int64_t r = 2 * (i / D), j = i - (r >> 1) * D;
+      const bool two = r + 1 < rows;
+      const float* m = sM + j * pm;
+      const float* a = sxo + r * p4;
+      const float* b = two ? a + p4 : a;
+      float ya = 0.f, yb = 0.f;
+#pragma unroll 4
+      for (int64_t k = 0; k < D; ++k) {
+        const float mk = m[k];
+        ya = fmaf(mk, a[k], ya);
+        yb = fmaf(mk, b[k], yb);
+      }
+      sy[r * p4 + j] = ya;
+      if (two) sy[(r + 1) * p4 + j] = yb;
+    }
+    __syncthreads();
+    for (int64_t r = warp; r < rows; r += kEvalThreads / 32) {
+      const float v = fold_row<Acc, VEC>(lane, [&] { return RowColsXY{X + (t0 + r) * ldx, sy + r * p4}; }, r, D, my_data, key, sw, t0);
+      if (lane == 0) f[t0 + r] = v;
+    }
+  }
+}
+
+// The large-D path's evaluation: the y of every row are in Y (written by the batched 3xTF32 GEMM of x - o and M), item b's row r
+// at Y + b * item_stride_y + r * ldy; one warp per row folds (x, y) as eval_batched_kernel folds x.
+// (at least one CTA per SM in the launch bounds: with none ptxas caps some accumulators at 64 registers and spills)
+template <typename Acc, bool VEC>
+__global__ void __launch_bounds__(kEvalThreads, AccTraits<Acc>::kNoise ? 2 : 1)
+    eval_transform_kernel(const float* __restrict__ X, int64_t item_stride_x, int64_t ldx, const float* __restrict__ Y, int64_t item_stride_y,
+                          int64_t ldy, int64_t n_rows, int64_t D, float* __restrict__ f, const typename AccTraits<Acc>::DataArg data,
+                          const typename AccTraits<Acc>::EvalArg noise) {
+  const int lane = threadIdx.x & 31;
+  const int64_t item = blockIdx.y;
+  X += item * item_stride_x;
+  Y += item * item_stride_y;
+  f += item * n_rows;
+  const PhiloxKey* key = nullptr;
+  uint32_t sw = 0u;
+  if constexpr (AccTraits<Acc>::kNoise) {
+    key = &noise.key;
+    sw = noise.key.stream_lo + (uint32_t)item;
+  }
+  const typename AccTraits<Acc>::DataArg my_data = item_data(data, item);
+  const int64_t warps_total = (int64_t)gridDim.x * (kEvalThreads / 32);
+  const int64_t gw = (int64_t)blockIdx.x * (kEvalThreads / 32) + (threadIdx.x >> 5);
+  for (int64_t r = gw; r < n_rows; r += warps_total) {
+    const float v = fold_row<Acc, VEC>(lane, [&] { return RowColsXY{X + r * ldx, Y + r * ldy}; }, r, D, my_data, key, sw, 0);
     if (lane == 0) f[r] = v;
   }
 }

@@ -38,7 +38,9 @@ The expression language (anything else raises ValueError):
     reductions, running sums and data;
   - constants  pi, e, numeric literals;
   - names      x (the element), xn (the next element x_{j+1}), j (the 0-based column of x) and D (the row length) in a
-    term, and the running names in an element term of a reduction; the reduction names and D in `value`.
+    term, and the running names in an element term of a reduction; the reduction names and D in `value`.  With a transform
+    (`transform=True` here, the matrix and offset bound by FusedObjective) also y, entry j of the transformed row
+    y = M (x - o), in element and running terms, and yn = y_{j+1} in pair terms (a term that uses xn or yn is a pair term).
   - data       up to 4 more names, each bound to a float32 tensor (`data={"t": t, "lam": lam}`).  Last dimension 1 makes a
     scalar, usable in the terms and in `value`; any other last dimension makes a vector, which must have the row length D and is
     usable in the terms only: `t` is its entry at column j and, in a pair term, `t_n` its entry at column j + 1 (as x and xn).
@@ -46,7 +48,8 @@ The expression language (anything else raises ValueError):
 The CUDA side evaluates in float32 with the precise libdevice functions (no fast math) and contracts a * b + c into fma.
 The source of an objective without pair terms is exactly that of the element-only language (no pair code in it), the source
 of one without data is exactly that of the language without data, and the source of one of sums without running sums is exactly
-that of the language before products, maxima, minima and running sums.  Which data name is a scalar and which a vector is part of
+that of the language before products, maxima, minima and running sums.  The source of an objective without a transform is
+exactly that of the language without transforms; one with a transform declares kTransform and its folds take y after x.  Which data name is a scalar and which a vector is part of
 the source; the tensors are not: they are bound to an instance of the compiled objective (`bind_instance`) and reach the
 kernels as a launch argument, so objectives with the same expressions and kinds share one compilation whatever their data.
 """
@@ -282,9 +285,13 @@ class ObjectiveSpec:
 
     def __init__(self, sums: Optional[Dict[str, str]], value: str, kinds: Optional[Dict[str, bool]] = None, *,
                  prods: Optional[Dict[str, str]] = None, maxs: Optional[Dict[str, str]] = None, mins: Optional[Dict[str, str]] = None,
-                 running: Optional[Dict[str, str]] = None):
-        """kinds: {data name: is a vector} in binding order (`data_kinds`), None or empty for an objective without data."""
+                 running: Optional[Dict[str, str]] = None, transform: bool = False):
+        """kinds: {data name: is a vector} in binding order (`data_kinds`), None or empty for an objective without data.
+        transform: the terms may read y and yn, the entries of the transformed row (and at least one of them must)."""
         self.kinds = dict(kinds or {})
+        self.transform = bool(transform)
+        # the names of the next column's entries: a term that reads one is a pair term
+        nexts = {"xn", "yn"} if self.transform else {"xn"}
         if value is None:
             raise ValueError("value: an objective needs a `value` expression of its reductions")
         groups = {"sums": sums, "prods": prods, "maxs": maxs, "mins": mins}
@@ -316,6 +323,12 @@ class ObjectiveSpec:
         self.sums, self.value = dict(sums or {}), value
         self.prods, self.maxs, self.mins, self.running = dict(prods or {}), dict(maxs or {}), dict(mins or {}), running
         term_names = {"x": "x", "xn": "xn", "j": "jf", "D": "Df"}
+        if self.transform:
+            taken = sorted({"y", "yn"} & (set(self.reductions) | set(running) | set(self.kinds)))
+            if taken:
+                raise ValueError(f"{taken[0]!r} names a reduction, running sum or data, but with a transform it is an entry of the "
+                                 "transformed row y = M (x - o)")
+            term_names.update(y="y", yn="yn")
         value_names = {s: f"S_{s}" for s in self.reductions}
         value_names["D"] = "Df"
         for name, vector in self.kinds.items():
@@ -345,7 +358,7 @@ class ObjectiveSpec:
         # row's draws in finish (evok_sampler.cuh: DataCols::draw4, value_rand / value_randn)
         self.element_draws = _Draws("the element terms", lambda k, name: f"d[{len(vectors) + k}]")
         self.value_draws = _Draws("`value`", lambda k, name: f"evok::value_{name}(key, sw, row, {MAX_DRAWS + k})")
-        self.running_terms = {c: _translate(tree, {k: v for k, v in term_names.items() if k != "xn"}, f"running[{c!r}]")
+        self.running_terms = {c: _translate(tree, {k: v for k, v in term_names.items() if k not in nexts}, f"running[{c!r}]")
                               for c, (tree, _) in running_trees.items()}
         for c, e in self.running_terms.items():
             n = next_entry(e)
@@ -355,17 +368,20 @@ class ObjectiveSpec:
         term_trees = {s: _parse(t, f"{GROUP_OF[self.reductions[s]]}[{s!r}]") for s, t in texts.items()}
         for s, (_, used) in term_trees.items():
             self._check_data_names(used, f"{GROUP_OF[self.reductions[s]]}[{s!r}]", term=True)
-            if used & set(running) and "xn" in used:
+            if used & set(running) and used & nexts:
                 raise ValueError(f"{GROUP_OF[self.reductions[s]]}[{s!r}]: {sorted(used & set(running))[0]!r} in a pair term; "
                                  f"{allowed_where}")
         value_tree, used = _parse(value, "value")
         self._check_data_names(used, "value", term=False)
         if used & set(running):
             raise ValueError(f"value: {sorted(used & set(running))[0]!r} is a running sum; {allowed_where}")
-        # a term that reads xn is a pair term, where rand() / randn() are refused
-        self.terms = {s: _translate(tree, run_names, f"{GROUP_OF[self.reductions[s]]}[{s!r}]", None if "xn" in used else self.element_draws)
+        # a term that reads xn (or yn) is a pair term, where rand() / randn() are refused
+        self.terms = {s: _translate(tree, run_names, f"{GROUP_OF[self.reductions[s]]}[{s!r}]", None if used & nexts else self.element_draws)
                       for s, (tree, used) in term_trees.items()}
-        self.pairs = frozenset(s for s, e in self.terms.items() if "xn" in e.names)
+        self.pairs = frozenset(s for s, e in self.terms.items() if e.names & nexts)
+        if self.transform and not any(e.names & {"y", "yn"} for e in list(self.terms.values()) + list(self.running_terms.values())):
+            raise ValueError("transform: no term reads y or yn, the entries of the transformed row; an objective of x alone needs no "
+                             "transform")
         for s, e in self.terms.items():
             n = next_entry(e)
             if n and s not in self.pairs:
@@ -402,6 +418,11 @@ class ObjectiveSpec:
                     "min": f"    s{i} = evok::min_nan(s{i}, {e});"}[ops[i]]
 
         lines = ['#include "evok_sampler.cuh"', "", "namespace evok_user {", "struct Acc {"]
+        if self.transform:
+            lines.append("  static constexpr bool kTransform = true;")
+        # the column values a fold takes: x, or x and its transformed entry y
+        col = "float x, float y, " if self.transform else "float x, "
+        cols = "float x, float xn, float y, float yn, " if self.transform else "float x, float xn, "
         if pair:
             lines.append("  static constexpr bool kPairs = true;")
         if nr:
@@ -430,17 +451,17 @@ class ObjectiveSpec:
             lines.append("  __device__ __forceinline__ explicit Acc(int64_t D) : Df((float)D) {}")
         if nr:
             run = [(i, e) for i, e in enumerate(self.running_terms.values())]
-            lines.append(f"  __device__ __forceinline__ void running(float x, int64_t j, {data_arg}float (&h)[{nr}]) {{")
+            lines.append(f"  __device__ __forceinline__ void running({col}int64_t j, {data_arg}float (&h)[{nr}]) {{")
             if uses_j(e for _, e in run):
                 lines.append("    const float jf = (float)j;")
             lines += entries(run, "v", "d")
             lines += [f"    h[{i}] = {e.cuda};" for i, e in run]
             lines.append("  }")
-            lines.append(f"  __device__ __forceinline__ void add(float x, int64_t j, {data_arg}const float (&r)[{nr}]) {{")
+            lines.append(f"  __device__ __forceinline__ void add({col}int64_t j, {data_arg}const float (&r)[{nr}]) {{")
         elif data_arg:
-            lines.append(f"  __device__ __forceinline__ void add(float x, int64_t j, const float (&d)[{nv}]) {{")
+            lines.append(f"  __device__ __forceinline__ void add({col}int64_t j, const float (&d)[{nv}]) {{")
         else:
-            lines.append("  __device__ __forceinline__ void add(float x, int64_t j) {")
+            lines.append(f"  __device__ __forceinline__ void add({col}int64_t j) {{")
         if uses_j(e for _, e in element):
             lines.append("    const float jf = (float)j;")
         lines += entries(element, "v", "d")
@@ -448,10 +469,10 @@ class ObjectiveSpec:
         lines.append("  }")
         if pair:
             if data_arg:
-                lines.append(f"  __device__ __forceinline__ void add_pair(float x, float xn, int64_t j, const float (&d)[{nv}], "
+                lines.append(f"  __device__ __forceinline__ void add_pair({cols}int64_t j, const float (&d)[{nv}], "
                              f"const float (&dn)[{nv}]) {{")
             else:
-                lines.append("  __device__ __forceinline__ void add_pair(float x, float xn, int64_t j) {")
+                lines.append(f"  __device__ __forceinline__ void add_pair({cols}int64_t j) {{")
             if uses_j(e for _, e in pair):
                 lines.append("    const float jf = (float)j;")
             lines += entries(pair, "v", "d") + entries(pair, "vn", "dn", "_n")
@@ -466,9 +487,11 @@ class ObjectiveSpec:
         lines += ["  }", "};", "}  // namespace evok_user", ""]
         return "\n".join(lines)
 
-    def torch_fn(self, X: torch.Tensor, data: Optional[Dict[str, torch.Tensor]] = None) -> torch.Tensor:
+    def torch_fn(self, X: torch.Tensor, data: Optional[Dict[str, torch.Tensor]] = None, transform: Optional[tuple] = None) -> torch.Tensor:
         """The fitnesses of the rows of X (..., N, D).  data: the tensors of the data names, cast to X's dtype and device; their
-        leading (batch) dimensions broadcast against the batch dimensions of X, and the result has the broadcast shape."""
+        leading (batch) dimensions broadcast against the batch dimensions of X, and the result has the broadcast shape.
+        transform: (M (..., D, D), o (..., D)) of an objective with a transform, cast likewise: y = (X - o) M^T with torch.matmul,
+        their batch dimensions broadcast as the data's do."""
         D = X.shape[-1]
         Dt = torch.tensor(float(D), dtype=X.dtype, device=X.device)
         env = {"x": X, "j": torch.arange(D, dtype=X.dtype, device=X.device), "D": Dt, "_dtype": X.dtype, "_device": X.device}
@@ -489,6 +512,13 @@ class ObjectiveSpec:
                     penv[f"{name}_n"] = t[..., 1:]
                 else:
                     venv[name] = t[..., 0]
+        if self.transform:
+            if transform is None:
+                raise ValueError("transform: this objective reads the transformed row y = M (x - o); expected (M, o)")
+            M, o = (t.to(dtype=X.dtype, device=X.device) for t in transform)
+            Y = torch.matmul(X - o.unsqueeze(-2), M.mT)
+            rows = torch.broadcast_shapes(rows, Y.shape[:-1])
+            env["y"], penv["y"], penv["yn"] = Y, Y[..., :-1], Y[..., 1:]
         env["_shape"] = rows + (D,)  # of an element draw (rand() / randn() in an element term): one per row and column
         for c, e in self.running_terms.items():  # c_j = sum_{k <= j} h(x_k, k, D)
             env[c] = torch.broadcast_to(_as_tensor(e.torch(env), env), rows + (D,)).cumsum(dim=-1)
@@ -556,9 +586,19 @@ def eval_batched_kernel_expressions() -> list:
     return [f"evok::eval_batched_kernel<evok_user::Acc, {'true' if vec else 'false'}>" for vec in (False, True)]
 
 
+def transform_kernel_expressions() -> list:
+    """The 4 kernels of an objective with a transform, in the order of EVOK_OBJ_KERNEL_TRANSFORM (+ vec, then + 2 + vec) of
+    include/evok.h: the fused small-D evaluation and the evaluation behind the GEMM.  They are its only kernels: no sampler can
+    produce the transformed row one column group at a time."""
+    b = lambda v: "true" if v else "false"  # noqa: E731
+    return ([f"evok::eval_transform_fused_kernel<evok_user::Acc, {b(vec)}>" for vec in (False, True)]
+            + [f"evok::eval_transform_kernel<evok_user::Acc, {b(vec)}>" for vec in (False, True)])
+
+
 N_KERNELS = 22
 N_BATCHED_KERNELS = 8
 N_EVAL_BATCHED_KERNELS = 2
+N_TRANSFORM_KERNELS = 4
 # -default-device: the declarations of the C ABI in include/evok.h (reached through evok_sampler.cuh) are unannotated
 NVRTC_OPTIONS = ("--gpu-architecture=sm_90a", "-std=c++17", "--fmad=true", "--ptxas-options=-v", "-default-device", f"-I{CSRC}",
                  f"-I{INCLUDE}")
@@ -726,7 +766,32 @@ def register_eval_batched(objective_id: int, cubin: bytes, names: list) -> None:
 _cache: Dict[str, CompiledObjective] = {}
 _batched_cache: Dict[str, CompiledObjective] = {}
 _eval_batched_cache: Dict[str, CompiledObjective] = {}
+_transform_cache: Dict[str, CompiledObjective] = {}
 _cache_lock = threading.Lock()
+
+
+def _declare(c: CompiledObjective, spec: ObjectiveSpec) -> None:
+    if spec.kinds:
+        declare_data(c.objective_id, spec.kinds)
+    if spec.noisy:
+        nat.check(nat.lib().evok_objective_declare_noise(c.objective_id), "evok_objective_declare_noise")
+
+
+def compile_transform(spec: ObjectiveSpec) -> CompiledObjective:
+    """Compile and register the objective of `spec` (one with a transform: `transform_kernel_expressions` are its kernels,
+    evok_objective_register_transform), once per process for one generated source."""
+    with _cache_lock:
+        c = _transform_cache.get(spec.source)
+        if c is None:
+            c = compile_source(spec.source, transform_kernel_expressions())
+            arr = (c_char_p * len(c.names))(*[n.encode() for n in c.names])
+            out = c_int()
+            nat.check(nat.lib().evok_objective_register_transform(c.cubin, len(c.cubin), arr, len(c.names), ctypes.byref(out)),
+                      "evok_objective_register_transform")
+            c.objective_id = out.value
+            _declare(c, spec)
+            _transform_cache[spec.source] = c
+        return c
 
 
 def compile_objective(spec: ObjectiveSpec) -> CompiledObjective:

@@ -283,6 +283,40 @@ def evaluate_batched(objective: int, X: torch.Tensor, *, seed: int, stream_id0: 
     return f
 
 
+def evaluate_transform_batched(objective: int, X: torch.Tensor, M: torch.Tensor, o: torch.Tensor, *, seed: int, stream_id0: int = 0,
+                               f: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """`evaluate_batched` of an objective with a transform (`jit.compile_transform`): its terms read y = M_b (x - o_b) of each row
+    of item b.  M: (1 or items, D, D), o: (1 or items, D), float32 CUDA, each item's entries contiguous (1: shared by every item).
+    Small D runs one fused launch; large D x - o, the batched 3xTF32 GEMM and the fold, with a workspace (`nat.workspace`)."""
+    if not (X.is_cuda and X.dtype == torch.float32 and X.ndim == 3 and (X.shape[2] <= 1 or X.stride(2) == 1)):
+        raise ValueError(f"X: expected a float32 CUDA tensor of shape (items, N, D) with unit column stride, got {tuple(X.shape)} "
+                         f"strides {X.stride()} {X.dtype} {X.device}")
+    B, n, D = X.shape
+    for name, t, tail in (("M", M, (D, D)), ("o", o, (D,))):
+        if not (t.dtype == torch.float32 and t.device == X.device and t.ndim == len(tail) + 1 and tuple(t.shape[1:]) == tail
+                and t.shape[0] in (1, B) and t[0].is_contiguous()):
+            raise ValueError(f"{name}: expected a float32 tensor of shape (1 or {B},) + {tail} on {X.device} with contiguous items, got "
+                             f"{tuple(t.shape)} {t.dtype} {t.device}")
+    sm = M.stride(0) if M.shape[0] > 1 else 0
+    so = o.stride(0) if o.shape[0] > 1 else 0
+    item_stride = X.stride(0) if B > 1 else 0
+    ldx = X.stride(1) if n > 1 else D
+    if f is None:
+        f = torch.empty(B, n, dtype=torch.float32, device=X.device)
+    f = _rows(f, "f", (B, n))
+    _check_data_device(objective, X)
+    if B == 0 or n == 0:
+        return f
+    lib = nat.lib()
+    nbytes = lib.evok_eval_transform_workspace_bytes(M.data_ptr(), sm, B, n, D)
+    ws = nat.workspace(X.device, nbytes, "transform") if nbytes else None
+    with _timed("eval"):
+        rc = lib.evok_eval_transform_batched(objective, X.data_ptr(), item_stride, ldx, M.data_ptr(), sm, o.data_ptr(), so, B, n, D, seed, stream_id0,
+                                             nat.ptr(ws), nbytes, f.data_ptr(), nat.stream_of(X))
+    nat.check(rc, "evok_eval_transform_batched")
+    return f
+
+
 # ------------------------------------------------------------------------------------------------ K3
 def _rank_ws(device: torch.device, n: int) -> torch.Tensor:
     return nat.workspace(device, nat.lib().evok_rank_workspace_bytes(n), "rank")

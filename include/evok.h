@@ -168,6 +168,20 @@ int evok_objective_register_batched(int objective, const void* cubin, size_t byt
 #define EVOK_OBJ_EVAL_BATCHED_KERNELS 2
 int evok_objective_register_eval_batched(int objective, const void* cubin, size_t bytes, const char* const* kernel_names_host, int n_kernels);
 
+/* Transformed objectives: an accumulator with kTransform (csrc/evok_sampler.cuh) whose terms read y = M (x - o) of each row as well
+ * as x.  Its sampler kernels cannot exist (a sampler produces a row one column group at a time, y needs the whole row), so it is
+ * registered with a fourth family only, evaluated by evok_eval_transform_batched:
+ *   EVOK_OBJ_KERNEL_TRANSFORM     + vec : eval_transform_fused_kernel<Acc, vec>  (small D: y on the CUDA cores in shared memory)
+ *   EVOK_OBJ_KERNEL_TRANSFORM + 2 + vec : eval_transform_kernel<Acc, vec>        (large D: y from the batched 3xTF32 GEMM)
+ * evok_objective_register_transform takes the sm_90a cubin of these EVOK_OBJ_TRANSFORM_KERNELS kernels (lowered names in this order)
+ * and writes a new id to *id_out_host, as evok_objective_register does; it needs no device.  evok_objective_declare_data and
+ * _declare_noise and evok_objective_instance apply to it as to any registered id; every other entry point that takes an objective
+ * yields EVOK_E_NOKERNEL for it, and evok_eval_transform_batched yields EVOK_E_NOKERNEL for every id without this family.
+ * Errors: EVOK_E_NULLPTR, EVOK_E_BADSIZE (bytes == 0, n_kernels != EVOK_OBJ_TRANSFORM_KERNELS, registry full). */
+#define EVOK_OBJ_KERNEL_TRANSFORM 32
+#define EVOK_OBJ_TRANSFORM_KERNELS 4
+int evok_objective_register_transform(const void* cubin, size_t bytes, const char* const* kernel_names_host, int n_kernels, int* id_out_host);
+
 /* Objectives with noise.  The accumulator of a registered objective may draw uniform and normal noise from the Philox key of
  * the population it evaluates (kNoise in csrc/evok_sampler.cuh); its eval_kernel<Acc, vec> then takes the draw of the rows as
  * its last argument.  evok_objective_declare_noise tells the library so, right after
@@ -450,6 +464,24 @@ int evok_sample_eval_batched(int objective, float* X, int64_t item_stride_x, int
  * (a data vector whose length is not D). */
 int evok_eval_batched(int objective, const float* X, int64_t item_stride_x, int64_t ldx, int64_t n_items, int64_t n_rows, int64_t D,
                       uint64_t seed, uint64_t stream_id0, float* f, void* stream);
+/* K2 of a transformed objective (evok_objective_register_transform) for a batch of populations: item b evaluates the n_rows rows of
+ * X + b * item_stride_x (row pitch ldx) with y = M_b (x - o_b), M_b the row-major D x D matrix at M + b * item_stride_m (row pitch
+ * D) and o_b the D-vector at o + b * item_stride_o (an item stride of 0 shares the operand), and writes f[b * n_rows ...].  Every
+ * x_k - o_k is rounded to float32 before any product, so a row equal to o_b has y = 0 exactly.  Noise and data as in
+ * evok_eval_batched: row r of item b draws on (seed, stream word stream_id0 + b) at global row r.  M and o are read in place.
+ * The library picks the path from D (no option): up to D = 96, the crossover of the two paths timed on the H100 (DESIGN.md), one
+ * fused launch per 65535
+ * items computes y as one FP32 FMA chain per entry in increasing k and needs no workspace; above it each chunk of items (x - o
+ * and y of a chunk within 256 MB) is three launches plus the GEMM's operand splits when M is not 16-byte aligned: x - o into
+ * `ws`, y = (x - o) M^T by evok_gemm_nt_batched (3xTF32), and the fold of the x and y rows.  ws: at least
+ * evok_eval_transform_workspace_bytes(M, item_stride_m, n_items, n_rows, D) bytes (0 on the fused path, where ws may be NULL).
+ * Errors in this order: EVOK_E_NULLPTR (X, M, o, f), EVOK_E_BADENUM, EVOK_E_BADSIZE (negative counts or item strides, D <= 0,
+ * ldx < D, an instance whose n_items is neither 1 nor the call's), EVOK_E_NOKERNEL (no transformed family), the data errors of
+ * evok_eval_batched, EVOK_E_NULLPTR (ws NULL where the path needs one), EVOK_E_BADSIZE (ws_bytes too small). */
+size_t evok_eval_transform_workspace_bytes(const float* M, int64_t item_stride_m, int64_t n_items, int64_t n_rows, int64_t D);
+int evok_eval_transform_batched(int objective, const float* X, int64_t item_stride_x, int64_t ldx, const float* M, int64_t item_stride_m,
+                                const float* o, int64_t item_stride_o, int64_t n_items, int64_t n_rows, int64_t D, uint64_t seed,
+                                uint64_t stream_id0, void* ws, size_t ws_bytes, float* f, void* stream);
 /* K3: f, w: [items][N].  ws: max(evok_rank_workspace_bytes(N), 8 * min(n_items, 65535) + 256) bytes */
 int evok_rank_batched(int method, const float* f, int64_t N, int64_t n_items, int higher_is_better, float* w, void* ws, size_t ws_bytes,
                       void* stream);
