@@ -126,6 +126,10 @@ _SIGNATURES = {
     "evok_cma_restart_batched_bipop": (c_int, [c_int, _P, _P, c_int64, c_int64, _P, _P, c_uint64, c_int64, c_int64, c_int64, c_int, _P, _P, _P, _P,
                                                _P, _P, _P, _P, _P, c_int64, _P, _P, _P, _P, _P, _P, _P, c_int64, _P, c_uint64, _P, _P, _P, c_int64,
                                                _P, _P, _P, _P, _P, _P, _P, c_int64, c_int64, _P]),
+    "evok_lmmaes_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int64, c_int64]),
+    "evok_lmmaes_ask_batched": (c_int, [_P, _P, _P, _P, _P, c_int64, c_int64, c_int64, c_int64, c_int64, _P, c_uint64, c_uint64, _P, c_size_t, _P]),
+    "evok_lmmaes_tell_batched": (c_int, [_P, _P, _P, _P, _P, _P, _P, c_int64, c_int64, c_int64, c_int64, c_int64, _P, _P, _P, _P, _P, _P, _P,
+                                         c_size_t, _P]),
     "evok_peer_alloc": (c_int, [c_size_t, _P, _P]),
     "evok_peer_open": (c_int, [_P, _P]),
     "evok_peer_close": (c_int, [_P]),

@@ -36,12 +36,21 @@ re-initialisation on the device, each item with its own generation counter:
 With `restarts(state, ..., popsize_multiplier=2, max_popsize=640)` every restart of an item doubles its population size (IPOP):
 the ask draws 640 rows per item and item b uses its first `rs.popsize[b]`.  With `bipop=True` as well, restarts alternate between
 that ladder and small runs of random population size and step size, each regime given a similar share of the evaluations (BIPOP).
+
+LM-MA-ES learns rotations at solution lengths where `cmaes` cannot hold its D x D matrices: each item keeps m ~ 4 + 3 ln D
+direction vectors, O(m D) state and work per sample, and a fixed number of launches per generation for all items:
+
+    state = lmmaes(center_init=torch.zeros(8, 100_000, device="cuda"), stdev_init=1.0, objective_sense="min")
+    for _ in range(generations):
+        population, evals = lmmaes_ask_and_evaluate(state, objective=rotated)   # (8, popsize, 100_000), (8, popsize)
+        state = lmmaes_tell(state, population, evals)
 """
 
 from .funcadam import AdamState, adam, adam_ask, adam_tell
 from .funccem import CEMState, cem, cem_ask, cem_ask_and_evaluate, cem_tell
 from .funcclipup import ClipUpState, clipup, clipup_ask, clipup_tell
 from .funccmaes import CMAESState, cmaes, cmaes_ask, cmaes_ask_and_evaluate, cmaes_tell
+from .funclmmaes import LMMAESState, lmmaes, lmmaes_ask, lmmaes_ask_and_evaluate, lmmaes_tell
 from .funcpgpe import PGPEState, pgpe, pgpe_ask, pgpe_ask_and_evaluate, pgpe_tell
 from .funcrestarts import IPOPLadder, RestartState, bipop_ladder, ipop_ladder, restarts, restarts_tell
 from .fused import LazyPopulation
@@ -50,7 +59,8 @@ from .funcsgd import SGDState, sgd, sgd_ask, sgd_tell
 from .misc import OptimizerFunctions, get_functional_optimizer
 
 __all__ = ["AdamState", "adam", "adam_ask", "adam_tell", "CEMState", "cem", "cem_ask", "cem_ask_and_evaluate", "cem_tell", "ClipUpState",
-           "clipup", "clipup_ask", "clipup_tell", "CMAESState", "cmaes", "cmaes_ask", "cmaes_ask_and_evaluate", "cmaes_tell", "LazyPopulation", "PGPEState", "pgpe", "pgpe_ask", "pgpe_ask_and_evaluate", "pgpe_tell",
+           "clipup", "clipup_ask", "clipup_tell", "CMAESState", "cmaes", "cmaes_ask", "cmaes_ask_and_evaluate", "cmaes_tell", "LazyPopulation",
+           "LMMAESState", "lmmaes", "lmmaes_ask", "lmmaes_ask_and_evaluate", "lmmaes_tell", "PGPEState", "pgpe", "pgpe_ask", "pgpe_ask_and_evaluate", "pgpe_tell",
            "IPOPLadder", "RestartState", "bipop_ladder", "ipop_ladder", "restarts", "restarts_tell",
            "SepCMAESState", "sepcmaes", "sepcmaes_ask", "sepcmaes_ask_and_evaluate", "sepcmaes_tell",
            "SGDState", "sgd", "sgd_ask", "sgd_tell", "OptimizerFunctions", "get_functional_optimizer"]

@@ -1203,6 +1203,70 @@ def cmaes_vector_update_batched(local_disp: torch.Tensor, shaped_disp: torch.Ten
         nat.check(lib.evok_cmaes_vector_update_batched_steps(*head, steps_dev.data_ptr(), *tail), "evok_cmaes_vector_update_batched_steps")
 
 
+LMMAES_MAX_VECTORS, LMMAES_MAX_POPSIZE = 64, 128  # EVOK_LMMAES_MAX_VECTORS, EVOK_LMMAES_MAX_POPSIZE
+
+
+def _lmmaes_operands(y: torch.Tensor, sigma: torch.Tensor, M: torch.Tensor, G: torch.Tensor, k: int, consts) -> tuple:
+    """Checks the state operands of the LM-MA-ES stages: y (items, D), sigma (items,), M (items, m, D), G (items, m, m), the
+    2 + 2m float64 constants (c_sigma, mu_eff, c_d[m], c_c[m]); returns (items, D, m, the constants as a C double array)."""
+    if not (y.is_cuda and y.dtype == torch.float32 and y.ndim == 2):
+        raise ValueError("y: expected a float32 CUDA tensor of shape (items, D)")
+    B, d = y.shape
+    if not (M.is_cuda and M.dtype == torch.float32 and M.ndim == 3 and M.shape[0] == B and M.shape[2] == d):
+        raise ValueError(f"M: expected a float32 CUDA tensor of shape ({B}, m, {d})")
+    m = M.shape[1]
+    _rows(y, "y", (B, d))
+    _rows(sigma, "sigma", (B,))
+    _rows(M, "M", (B, m, d))
+    _rows(G, "G", (B, m, m))
+    for t, name in ((sigma, "sigma"), (M, "M"), (G, "G")):
+        if t.device != y.device:
+            raise ValueError(f"{name}: expected on {y.device}, got {t.device}")
+    if len(consts) != 2 + 2 * m:
+        raise ValueError(f"consts: expected {2 + 2 * m} values (c_sigma, mu_eff, c_d[m], c_c[m]), got {len(consts)}")
+    return B, d, m, (ctypes.c_double * len(consts))(*[float(c) for c in consts])
+
+
+def _lmmaes_ws(device: torch.device, B: int, n: int, d: int, m: int) -> torch.Tensor:
+    return nat.workspace(device, nat.lib().evok_lmmaes_workspace_bytes(B, n, d, m), "lmmaes")
+
+
+def lmmaes_ask_batched(y: torch.Tensor, sigma: torch.Tensor, M: torch.Tensor, G: torch.Tensor, k: int, consts, popsize: int, *, seed: int,
+                       stream_id0: int = 0, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The LM-MA-ES ask of every item, (items, popsize, D): x_i = y + sigma d_i with d_i the step of z_i through the first k vectors
+    of M, z_i of item b the row of `sample_batched` with this seed on stream stream_id0 + b.  Three launches per item chunk (one
+    with k = 0, then x = fmaf(sigma, z, y))."""
+    B, d, m, c = _lmmaes_operands(y, sigma, M, G, k, consts)
+    out = torch.empty(B, popsize, d, dtype=torch.float32, device=y.device) if out is None else _rows(out, "out", (B, popsize, d))
+    ws = _lmmaes_ws(y.device, B, popsize, d, m)
+    with _timed("lmmaes_ask"):
+        rc = nat.lib().evok_lmmaes_ask_batched(out.data_ptr(), y.data_ptr(), sigma.data_ptr(), M.data_ptr(), G.data_ptr(), B, popsize, d, m, int(k),
+                                               c, seed, stream_id0, ws.data_ptr(), ws.numel(), nat.stream_of(y))
+    nat.check(rc, "evok_lmmaes_ask_batched")
+    return out
+
+
+def lmmaes_tell_batched(X: torch.Tensor, aw: torch.Tensor, y: torch.Tensor, sigma: torch.Tensor, p_sigma: torch.Tensor, M: torch.Tensor,
+                        G: torch.Tensor, k: int, consts) -> tuple:
+    """The LM-MA-ES tell of every item from its rows X (items, popsize, D) and their rank weights aw (items, popsize): the new
+    (y, sigma, p_sigma, M, G), all new tensors.  Four launches per item chunk."""
+    B, d, m, c = _lmmaes_operands(y, sigma, M, G, k, consts)
+    if not (aw.is_cuda and aw.dtype == torch.float32 and aw.ndim == 2 and aw.shape[0] == B):
+        raise ValueError(f"aw: expected a float32 CUDA tensor of shape ({B}, popsize)")
+    n = aw.shape[1]
+    _rows(aw, "aw", (B, n))
+    _rows(X, "X", (B, n, d))
+    _rows(p_sigma, "p_sigma", (B, d))
+    outs = (torch.empty_like(y), torch.empty_like(sigma), torch.empty_like(p_sigma), torch.empty_like(M), torch.empty_like(G))
+    ws = _lmmaes_ws(y.device, B, n, d, m)
+    with _timed("lmmaes_tell"):
+        rc = nat.lib().evok_lmmaes_tell_batched(X.data_ptr(), aw.data_ptr(), y.data_ptr(), sigma.data_ptr(), p_sigma.data_ptr(), M.data_ptr(),
+                                                G.data_ptr(), B, n, d, m, int(k), c, *(t.data_ptr() for t in outs), ws.data_ptr(), ws.numel(),
+                                                nat.stream_of(y))
+    nat.check(rc, "evok_lmmaes_tell_batched")
+    return outs
+
+
 RESTART_CRITERIA = ("tol_fun", "tol_x", "tol_x_up", "max_condition", "min_fitness_stdev", "max_generations")  # bits 0-5; bit 6: non-finite
 # bit 7 (BIPOP only): a small run has used half the evaluations of the item's latest large run; it has no threshold
 

@@ -769,6 +769,37 @@ int evok_grad_push(int form, const float* X, int64_t ldx, const float* w, const 
 int evok_peer_reduce(const float* slots_local, int world, int64_t n, const uint64_t* flags_local, uint64_t* epoch_dev,
                      uint32_t* done_dev, uint32_t* err_dev, uint64_t timeout_ns, float* out, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Limited-memory matrix adaptation (LM-MA-ES, Loshchilov, Glasmachers & Beyer, IEEE TEVC 23(2), 2019) for n_items independent
+ * searches (functional LM-MA-ES).  Item b holds y [D], sigma, p_sigma [D], m vectors M [m][D] and G = M M^T [m][m]; all operands
+ * are contiguous [items][...].  k = min(t, m) is the number of vectors in use at generation t.  consts_host: 2 + 2m doubles,
+ * (c_sigma, mu_eff, c_d,1 .. c_d,m, c_c,1 .. c_c,m).  Limits: 2 <= n_rows <= EVOK_LMMAES_MAX_POPSIZE, 1 <= m <=
+ * EVOK_LMMAES_MAX_VECTORS, 0 <= k <= m.  Column passes take tiles of 512 columns whatever n_items, so item b gives the bits of a
+ * one-item call on its own operands; sums are in fixed order, with no atomics.  Each entry launches per item chunk of at most
+ * 65535 items, one after another.  The workspace holds one chunk.
+ *   evok_lmmaes_ask_batched: X [items][n_rows][D], x_i = y + sigma d_i, d_i = z_i after k steps d <- (1 - c_d,j) d + c_d,j M_j (M_j^T d),
+ *       in the coefficient form: P = M_k Z^T (a Gram pass over z rebuilt from Philox), the recursion for beta (one CTA per item),
+ *       and the pass that writes x = y + sigma (alpha z + beta M_k).  z_i of item b is the row the batched sampler draws with
+ *       (seed, stream_id0 + b).  With k = 0 only the write pass runs, and x = fmaf(sigma, z, y): the bits of evok_sample_batched
+ *       with mean y and stdev sigma.  Launches per chunk: 3, or 1 with k = 0.
+ *   evok_lmmaes_tell_batched: aw [items][n_rows], the weights of the rows' ranks (0 for rows outside the best mu).  The rows with a
+ *       non-zero weight are read once: d = (x - y) / sigma, S_d = sum w_i d_i and Q = M_k D^T; the recovery of z (one CTA per
+ *       item) gives S_z = a S_d + sum_j c_j M_j; then M_j' = (1 - c_c,j) M_j + sqrt(mu_eff c_c,j (2 - c_c,j)) S_z for every j < m,
+ *       p_sigma' = (1 - c_sigma) p_sigma + sqrt(mu_eff c_sigma (2 - c_sigma)) S_z, y' = y + sigma S_d, G' = M' M'^T of the M' written,
+ *       sigma' = sigma exp((c_sigma / 2)(|p_sigma'|^2 / D - 1)).  The outputs must not overlap the inputs.  Launches per chunk: 4.
+ * Errors in this order: EVOK_E_NULLPTR, EVOK_E_BADSIZE (a count outside its limits), EVOK_E_WORKSPACE.
+ * --------------------------------------------------------------------------------------------- */
+#define EVOK_LMMAES_MAX_VECTORS 64
+#define EVOK_LMMAES_MAX_POPSIZE 128
+size_t evok_lmmaes_workspace_bytes(int64_t n_items, int64_t n_rows, int64_t D, int64_t m);
+int evok_lmmaes_ask_batched(float* X, const float* y, const float* sigma, const float* M, const float* G, int64_t n_items, int64_t n_rows,
+                            int64_t D, int64_t m, int64_t k, const double* consts_host, uint64_t seed, uint64_t stream_id0, void* ws,
+                            size_t ws_bytes, void* stream);
+int evok_lmmaes_tell_batched(const float* X, const float* aw, const float* y, const float* sigma, const float* p_sigma, const float* M,
+                             const float* G, int64_t n_items, int64_t n_rows, int64_t D, int64_t m, int64_t k, const double* consts_host,
+                             float* y_out, float* sigma_out, float* p_sigma_out, float* M_out, float* G_out, void* ws, size_t ws_bytes,
+                             void* stream);
+
 #ifdef __cplusplus
 }
 #endif
