@@ -130,6 +130,8 @@ _SIGNATURES = {
     "evok_lmmaes_ask_batched": (c_int, [_P, _P, _P, _P, _P, c_int64, c_int64, c_int64, c_int64, c_int64, _P, c_uint64, c_uint64, _P, c_size_t, _P]),
     "evok_lmmaes_tell_batched": (c_int, [_P, _P, _P, _P, _P, _P, _P, c_int64, c_int64, c_int64, c_int64, c_int64, _P, _P, _P, _P, _P, _P, _P,
                                          c_size_t, _P]),
+    "evok_sym_expm_pair_batched": (c_int, [_P, c_int64, c_int64, _P, _P, _P]),
+    "evok_xnes_tell_batched": (c_int, [_P, _P, _P, _P, _P, c_int64, c_int64, c_int64, c_float, c_float, _P, _P, _P, _P]),
     "evok_peer_alloc": (c_int, [c_size_t, _P, _P]),
     "evok_peer_open": (c_int, [_P, _P]),
     "evok_peer_close": (c_int, [_P]),

@@ -44,6 +44,18 @@ direction vectors, O(m D) state and work per sample, and a fixed number of launc
     for _ in range(generations):
         population, evals = lmmaes_ask_and_evaluate(state, objective=rotated)   # (8, popsize, 100_000), (8, popsize)
         state = lmmaes_tell(state, population, evals)
+
+XNES and SNES, the natural evolution strategies, run many searches at once too.  On CUDA float32 the XNES tell is one CTA per
+item for D <= 96 (its exponential map included), and SNES takes `lazy=True` like `pgpe`:
+
+    state = xnes(center_init=torch.randn(1024, 16, device="cuda"), stdev_init=1.0, objective_sense="min")
+    for _ in range(generations):
+        population, evals = xnes_ask_and_evaluate(state, objective=rastrigin)   # (1024, popsize, 16), (1024, popsize)
+        state = xnes_tell(state, population, evals)
+
+    state = snes(center_init=torch.zeros(64, 10_000, device="cuda"), stdev_init=1.0, objective_sense="min")
+    population, evals = snes_ask_and_evaluate(state, objective=rastrigin, lazy=True)
+    state = snes_tell(state, population, evals)
 """
 
 from .funcadam import AdamState, adam, adam_ask, adam_tell
@@ -56,6 +68,8 @@ from .funcrestarts import IPOPLadder, RestartState, bipop_ladder, ipop_ladder, r
 from .fused import LazyPopulation
 from .funcsepcmaes import SepCMAESState, sepcmaes, sepcmaes_ask, sepcmaes_ask_and_evaluate, sepcmaes_tell
 from .funcsgd import SGDState, sgd, sgd_ask, sgd_tell
+from .funcsnes import SNESState, snes, snes_ask, snes_ask_and_evaluate, snes_tell
+from .funcxnes import XNESState, xnes, xnes_ask, xnes_ask_and_evaluate, xnes_tell
 from .misc import OptimizerFunctions, get_functional_optimizer
 
 __all__ = ["AdamState", "adam", "adam_ask", "adam_tell", "CEMState", "cem", "cem_ask", "cem_ask_and_evaluate", "cem_tell", "ClipUpState",
@@ -63,4 +77,5 @@ __all__ = ["AdamState", "adam", "adam_ask", "adam_tell", "CEMState", "cem", "cem
            "LMMAESState", "lmmaes", "lmmaes_ask", "lmmaes_ask_and_evaluate", "lmmaes_tell", "PGPEState", "pgpe", "pgpe_ask", "pgpe_ask_and_evaluate", "pgpe_tell",
            "IPOPLadder", "RestartState", "bipop_ladder", "ipop_ladder", "restarts", "restarts_tell",
            "SepCMAESState", "sepcmaes", "sepcmaes_ask", "sepcmaes_ask_and_evaluate", "sepcmaes_tell",
-           "SGDState", "sgd", "sgd_ask", "sgd_tell", "OptimizerFunctions", "get_functional_optimizer"]
+           "SGDState", "sgd", "sgd_ask", "sgd_tell", "SNESState", "snes", "snes_ask", "snes_ask_and_evaluate", "snes_tell",
+           "XNESState", "xnes", "xnes_ask", "xnes_ask_and_evaluate", "xnes_tell", "OptimizerFunctions", "get_functional_optimizer"]

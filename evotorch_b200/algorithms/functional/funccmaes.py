@@ -28,9 +28,8 @@ from typing import Callable, NamedTuple, Optional
 import torch
 
 from ... import ops
-from ...objectives import is_transformed
 from ..cmaes import CMAESHyperparameters, cmaes_hyperparameters
-from .fused import LazyPopulation
+from .fused import LazyPopulation, ask_and_evaluate_keyed
 from .misc import draw_philox_seed, on_kernels
 
 
@@ -147,18 +146,7 @@ def cmaes_ask_and_evaluate(state: CMAESState, *, objective: Callable) -> tuple:
     per-item data gives item b its own data.  Otherwise this is `cmaes_ask` followed by `objective(values)`.  An objective whose
     data has a batch shape must have the state's batch shape.  There is no lazy form: `cmaes_tell` recovers its steps from the
     values."""
-    batch, _, _ = _items(state)
-    per_item = tuple(getattr(objective, "data_batch_shape", ()))
-    if per_item and per_item != batch:
-        raise ValueError(f"the data of {objective!r} has batch shape {per_item}, the CMA-ES state {batch}: each item of the data needs "
-                         "its own search (build the state with that batch shape)")
-    values, seed = _ask(state)
-    oid = getattr(objective, "evok_objective_id", None)
-    if seed is not None and oid is not None and oid != ops.OBJ_NONE and hasattr(objective, "evaluate_batched"):
-        return values, objective.evaluate_batched(values, seed=seed)
-    if seed is not None and is_transformed(objective):  # a FusedObjective of y = M (x - o): its own kernels
-        return values, objective.evaluate_batched(values, seed=seed)
-    return values, objective(values)
+    return ask_and_evaluate_keyed(lambda: _ask(state), _items(state)[0], objective, "CMA-ES")
 
 
 def _limit_stdev(C: torch.Tensor, sigma: torch.Tensor, lo: Optional[float], hi: Optional[float]) -> None:

@@ -26,8 +26,8 @@ from typing import Callable, NamedTuple, Optional
 import torch
 
 from ... import ops
-from ...objectives import is_transformed
 from .funccmaes import _assigned_weights
+from .fused import ask_and_evaluate_keyed
 from .misc import draw_philox_seed, on_kernels
 
 
@@ -183,17 +183,7 @@ def lmmaes_ask_and_evaluate(state: LMMAESState, *, objective: Callable) -> tuple
     every FusedObjective, transformed and noisy ones included) evaluates all items in one call, keyed with the ask's Philox seed,
     so a noisy objective gets the noise of the draw and per-item data gives item b its own data.  Otherwise this is `lmmaes_ask`
     followed by `objective(values)`.  An objective whose data has a batch shape must have the state's batch shape."""
-    batch, _, _ = _items(state)
-    per_item = tuple(getattr(objective, "data_batch_shape", ()))
-    if per_item and per_item != batch:
-        raise ValueError(f"the data of {objective!r} has batch shape {per_item}, the LM-MA-ES state {batch}: each item of the data needs "
-                         "its own search (build the state with that batch shape)")
-    values, seed = _ask(state)
-    oid = getattr(objective, "evok_objective_id", None)
-    fused = (oid is not None and oid != ops.OBJ_NONE) or is_transformed(objective)
-    if seed is not None and fused and hasattr(objective, "evaluate_batched"):
-        return values, objective.evaluate_batched(values, seed=seed)
-    return values, objective(values)
+    return ask_and_evaluate_keyed(lambda: _ask(state), _items(state)[0], objective, "LM-MA-ES")
 
 
 def _recovery_torch(state: LMMAESState, d_steps: torch.Tensor) -> tuple:

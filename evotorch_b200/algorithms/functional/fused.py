@@ -97,6 +97,24 @@ def data_batch(objective: Callable, batch: torch.Size) -> torch.Size:
     return per_item
 
 
+def ask_and_evaluate_keyed(ask: Callable, batch: tuple, objective: Callable, searcher: str) -> tuple:
+    """(values, evals) of a search whose ask is not the batched sampler's: `ask()` returns (values (*batch, popsize, D), the
+    Philox seed of its draw, or None off the kernels).  With a seed, an objective with `evaluate_batched` and a kernel (a
+    built-in objective or any FusedObjective, transformed and noisy ones included) evaluates every item in one call keyed with
+    that seed, so a noisy objective gets the noise of the draw and per-item data gives item b its own data; otherwise this is
+    `objective(values)`.  An objective whose data has a batch shape must have `batch` (ValueError naming `searcher` if not)."""
+    per_item = tuple(getattr(objective, "data_batch_shape", ()))
+    if per_item and per_item != tuple(batch):
+        raise ValueError(f"the data of {objective!r} has batch shape {per_item}, the {searcher} state {tuple(batch)}: each item of the data "
+                         "needs its own search (build the state with that batch shape)")
+    values, seed = ask()
+    oid = getattr(objective, "evok_objective_id", None)
+    fused = (oid is not None and oid != ops.OBJ_NONE) or is_transformed(objective)
+    if seed is not None and fused and hasattr(objective, "evaluate_batched"):
+        return values, objective.evaluate_batched(values, seed=seed)
+    return values, objective(values)
+
+
 def ask_and_evaluate(ask: Callable, center: torch.Tensor, stdev: torch.Tensor, popsize: int, symmetric: bool, objective: Callable,
                      lazy: bool) -> tuple:
     """(population, fitnesses) of one ask: fused when `fused_objective_id` applies, else `ask()` followed by `objective`."""

@@ -1267,6 +1267,43 @@ def lmmaes_tell_batched(X: torch.Tensor, aw: torch.Tensor, y: torch.Tensor, sigm
     return outs
 
 
+XNES_MAX_D = 96  # EVOK_XNES_MAX_D
+
+
+def sym_expm_pair_batched(S: torch.Tensor) -> tuple:
+    """(expm(S) - I, expm(-S) - I) of every symmetric matrix of S (items, D, D), 1 <= D <= XNES_MAX_D, one CTA per item: the
+    expm1 form, which keeps the relative precision of a tiny S.  Both are new tensors."""
+    if not (S.is_cuda and S.dtype == torch.float32 and S.ndim == 3 and S.shape[1] == S.shape[2]):
+        raise ValueError(f"S: expected a float32 CUDA tensor of shape (items, D, D), got {tuple(S.shape)} {S.dtype}")
+    B, d, _ = S.shape
+    S = _rows(S.contiguous(), "S", (B, d, d))
+    Fp, Fm = torch.empty_like(S), torch.empty_like(S)
+    with _timed("sym_expm_pair"):
+        rc = nat.lib().evok_sym_expm_pair_batched(S.data_ptr(), B, d, Fp.data_ptr(), Fm.data_ptr(), nat.stream_of(S))
+    nat.check(rc, "evok_sym_expm_pair_batched")
+    return Fp, Fm
+
+
+def xnes_tell_batched(X: torch.Tensor, w: torch.Tensor, mu: torch.Tensor, A: torch.Tensor, A_inv: torch.Tensor, lr_mu: float, lr_A: float) -> tuple:
+    """The XNES update of every item from its rows X (items, N, D) and their utilities w (items, N), centred where the ranking
+    needs it: z = A_inv (x - mu) for the rows with a non-zero weight, d = sum w z, S = (lr_A / 2)(sum w z z^T - (sum w) I), and
+    the new (mu + A (lr_mu d), A + A (e^S - I), A_inv + (e^-S - I) A_inv), all new tensors.  One launch per 65535 items."""
+    if not (mu.is_cuda and mu.dtype == torch.float32 and mu.ndim == 2):
+        raise ValueError("mu: expected a float32 CUDA tensor of shape (items, D)")
+    B, d = mu.shape
+    if not (w.is_cuda and w.dtype == torch.float32 and w.ndim == 2 and w.shape[0] == B):
+        raise ValueError(f"w: expected a float32 CUDA tensor of shape ({B}, N)")
+    n = w.shape[1]
+    w, mu = _rows(w, "w", (B, n)), _rows(mu, "mu", (B, d))
+    X, A, A_inv = _rows(X, "X", (B, n, d)), _rows(A, "A", (B, d, d)), _rows(A_inv, "A_inv", (B, d, d))
+    outs = (torch.empty_like(mu), torch.empty_like(A), torch.empty_like(A_inv))
+    with _timed("xnes_tell"):
+        rc = nat.lib().evok_xnes_tell_batched(X.data_ptr(), w.data_ptr(), mu.data_ptr(), A.data_ptr(), A_inv.data_ptr(), B, n, d, float(lr_mu),
+                                              float(lr_A), *(t.data_ptr() for t in outs), nat.stream_of(mu))
+    nat.check(rc, "evok_xnes_tell_batched")
+    return outs
+
+
 RESTART_CRITERIA = ("tol_fun", "tol_x", "tol_x_up", "max_condition", "min_fitness_stdev", "max_generations")  # bits 0-5; bit 6: non-finite
 # bit 7 (BIPOP only): a small run has used half the evaluations of the item's latest large run; it has no threshold
 

@@ -800,6 +800,24 @@ int evok_lmmaes_tell_batched(const float* X, const float* aw, const float* y, co
                              float* y_out, float* sigma_out, float* p_sigma_out, float* M_out, float* G_out, void* ws, size_t ws_bytes,
                              void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Functional XNES (csrc/evok_xnes.cu): one CTA per item, the working matrices in shared memory, 1 <= D <= EVOK_XNES_MAX_D.
+ * Items go in chunks of at most 65535, one launch each; sums are in fixed order, with no atomics, so item b gives the bits of a
+ * one-item call on its own operands.
+ *   evok_sym_expm_pair_batched: for every symmetric S [items][D][D], F_plus = expm(S) - I and F_minus = expm(-S) - I (the expm1
+ *       form keeps the relative precision of a tiny S).  Scaling and squaring with s = max(0, ceil(log2 |S|_1)) per item, a
+ *       degree-11 Taylor core in S^2 / 4^s shared by both signs, and F <- 2F + F^2 s times for each sign.
+ *   evok_xnes_tell_batched: X [items][n_rows][D], w [items][n_rows] the utilities (already centred where the ranking needs it),
+ *       mu [items][D], A and A_inv [items][D][D].  z_r = A_inv (x_r - mu) for the rows with w_r != 0, d = sum w_r z_r,
+ *       S = (lr_A / 2)(sum w_r z_r z_r^T - (sum w_r) I), then mu' = mu + A (lr_mu d), A' = A + A F+, A_inv' = A_inv + F- A_inv with
+ *       the exponential pair of S.  The outputs must not overlap the inputs.
+ * Errors in this order: EVOK_E_NULLPTR, EVOK_E_BADSIZE (n_items < 0, D < 1, D > EVOK_XNES_MAX_D, n_rows < 2).
+ * --------------------------------------------------------------------------------------------- */
+#define EVOK_XNES_MAX_D 96
+int evok_sym_expm_pair_batched(const float* S, int64_t n_items, int64_t D, float* F_plus, float* F_minus, void* stream);
+int evok_xnes_tell_batched(const float* X, const float* w, const float* mu, const float* A, const float* A_inv, int64_t n_items, int64_t n_rows,
+                           int64_t D, float lr_mu, float lr_A, float* mu_out, float* A_out, float* A_inv_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
